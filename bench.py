@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- CycleGAN-VC training-step throughput on B200 (BASELINE.json metric).
+"""bench.py -- CycleGAN-VC training-step throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16x3|bf16|fp32]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16x3|bf16|fp32] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one synthetic minibatch: G_A2B/G_B2A/D_A/D_B forward + cycle/identity/
@@ -12,6 +12,8 @@ Prints ONE JSON line (rank 0).  `value` is 256-sample steps per second summed ov
 on device-resident inputs; `e2e` is the same through CycleGAN.train() with host buffers (H2D of A and B and D2H of
 the losses inside the timed region).  `--impl reference` times the CPU oracle (a torch-CPU restatement of the
 reference graph; TensorFlow 1.x cannot be installed here -- see DESIGN.md) on a bounded sample of the same workload.
+`--dump-outputs DIR` writes what the last timed step computed (losses, a fixed sample of the updated parameters; converted
+batch for `--workload infer`) as DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -44,25 +46,30 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d["bf16_tflops_sustained"], "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback"}
+    # H100 SXM data sheet, dense, at 700 W (not a measured rate)
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
-def _ncu_traffic(kernel_class):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-    capture (profiles/*ncu_tc_kernels_summary.json; average over the captured launches), or None."""
-    import glob
-    import re
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "*ncu_tc_kernels_summary.json")),
-                   key=lambda f: [int(x) for x in re.findall(r"\d+", os.path.basename(f))])      # r01_v10 after r01_v7
-    if not files:
-        return None
-    try:
-        d = json.load(open(files[-1]))
-        ks = d["prof_tn" if kernel_class == 1 else "prof_nt"]
-        vals = [(k["dram_read_MB"] + k["dram_write_MB"]) * 1e6 for k in ks if k.get("dram_read_MB") is not None]
-        return sum(vals) / len(vals) if vals else None
-    except Exception:
-        return None
+DUMP_PARAM_SAMPLE = 4 << 20                                      # parameters written by --dump-outputs (fixed seeded sample, 16 MB)
+
+
+def dump_outputs(d, arrays):
+    """name -> array: DIR/<name>.npy in float32 (float64 arrays stay float64)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(d, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
+
+
+def param_sample(params):
+    """A fixed, seeded sample of the concatenated parameter tensors (the same elements for every build)."""
+    import numpy as np
+    flat = np.concatenate([np.asarray(v, dtype=np.float32).ravel() for v in params.values()])
+    if flat.size <= DUMP_PARAM_SAMPLE:
+        return flat
+    idx = np.sort(np.random.default_rng(0).choice(flat.size, DUMP_PARAM_SAMPLE, replace=False))
+    return flat[idx]
 
 
 class ClockSampler:
@@ -213,7 +220,7 @@ def pick_reference_batch(steps, warmup, budget_s, threads):
     return 16, per_sample
 
 
-def infer_measure(precision, local_rank, world, dist, steps, warmup):
+def infer_measure(precision, local_rank, world, dist, steps, warmup, dump_dir=None):
     """BASELINE.json configs[4] (convert.py path): generator-only A2B forward of 1024 x [24,128] per GPU.  Embarrassingly parallel
     over GPUs (no collective).  Returns a dict (rank 0) with frames/s device-resident and end to end (host numpy in / out)."""
     import numpy as np
@@ -222,7 +229,7 @@ def infer_measure(precision, local_rank, world, dist, steps, warmup):
     dev = torch.device("cuda", local_rank)
     nb = 1024
     m = cgvc.CycleGAN(num_features=FEATS, mode="test", max_batch=nb, max_frames=FRAMES, precision=precision, device=local_rank, seed=0)
-    x = torch.randn(nb, FEATS, FRAMES, device=dev)
+    x = torch.randn(nb, FEATS, FRAMES, device=dev, generator=torch.Generator(device=dev).manual_seed(2000))
     for _ in range(max(warmup, 3)):
         m.test(x, "A2B")
     if dist is not None:
@@ -231,9 +238,11 @@ def infer_measure(precision, local_rank, world, dist, steps, warmup):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
-        m.test(x, "A2B")
+        y = m.test(x, "A2B")
     e1.record(); torch.cuda.synchronize(dev)
     ms = e0.elapsed_time(e1)
+    if dump_dir and local_rank == 0:
+        dump_outputs(dump_dir, {"converted_A2B": y.cpu().numpy() if hasattr(y, "cpu") else y})
     # end to end: host float32 utterance crops in, converted host array out (pinned staging, H2D + D2H inside the timed region)
     xh = x.cpu().numpy()
     m.test(xh, "A2B")
@@ -271,7 +280,7 @@ def infer_bench(args, rank, local_rank, world):
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    r = infer_measure(args.precision, local_rank, world, dist, args.steps, args.warmup)
+    r = infer_measure(args.precision, local_rank, world, dist, max(args.steps, 1), args.warmup, args.dump_outputs)
     clocks = sampler.stop() if rank == 0 else None
     if rank == 0:
         r.update({"warmup": max(args.warmup, 3), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "data": "synthetic", "clocks": clocks,
@@ -304,9 +313,11 @@ def main():
     ap.add_argument("--replicas-only", action="store_true",
                     help="diagnostic for N > 1: every rank trains its own replica with no gradient exchange (what the step costs without the all-reduce, timed as the max over ranks like the real run); the line is marked and is not a data-parallel result")
     ap.add_argument("--set-option", action="append", default=[], metavar="NAME=VALUE",
-                    help="engine option (include/cgvc.h: side_wgrad, cta_pairs, post_onepass, fuse_in, ...) for A/B measurements; repeatable")
+                    help="engine option (include/cgvc.h: side_wgrad, post_onepass, fuse_in, ...) for A/B measurements; repeatable")
     ap.add_argument("--workload", default="train", choices=["train", "infer"],
                     help="train: the headline metric; infer: BASELINE config 5, generator-only forward of 1024 x [24,128] (frames/s)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -318,7 +329,7 @@ def main():
     workload = ("full CycleGAN-VC train step (4 generator + 2 discriminator applications fwd, losses, bwd, 2x Adam), "
                 "batch %d x [24 MCEP, 128 frames] per GPU, synthetic N(0,1) MCEP, glorot weights" % args.batch)
     config = {"workload": workload, "per_gpu_batch": args.batch, "frames": FRAMES, "parallelism": "dp%d" % max(world, 1), "precision": args.precision,
-              "l2": "per-step working set ~12 GB of activations >> 126 MB L2, no flush needed",
+              "l2": "per-step working set ~12 GB of activations >> 50 MB L2, no flush needed",
               "launch": "cuda_graph" if args.cuda_graph else "eager"}
 
     if args.impl == "reference":
@@ -401,6 +412,9 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     n1 = C.c_ulonglong(0); lib.cgvc_kernel_launches(C.byref(n1))
+    if args.dump_outputs and rank == 0:
+        # what the last timed step returned (its 8 losses) and the parameters it left behind
+        dump_outputs(args.dump_outputs, {"losses": m._losses.cpu().numpy(), "params_sample": param_sample(m.get_params())})
     clocks = sampler.stop() if rank == 0 else None
     if dist is not None:
         t = torch.tensor([ms], device=dev); dist.all_reduce(t, op=dist.ReduceOp.MAX); ms = float(t.item())
@@ -445,23 +459,21 @@ def main():
         ms_per_step_1stream = pe0.elapsed_time(pe1) / 2.0
         pk = _peaks()
         k = max(range(3), key=lambda i: ms2[i])            # the dominant kernel class of the step
-        knames = ["tc_pair_nt_kernel<BN,NPL,0> (conv forward + data-gradient gather-GEMM on CTA pairs, TMA im2col operand; the 15-tap 24-channel edge layers run as dense 1 x 1 layers on the same kernel)",
-                  "tc_pair_tn_kernel / tc_pair_tn_q_kernel (weight-gradient gather-GEMM on CTA pairs; tc_gg_tn_kernel where a layer has < 256 channels or columns)",
-                  "tc_pair_nt_kernel<256,NPL,1|2> (conv forward with the fused instance-norm + GLU / + residual epilogue)"]
+        knames = ["tc_gg_nt_kernel<BN,NPL,0> (conv forward + data-gradient gather-GEMM; the 15-tap 24-channel edge layers run as dense 1 x 1 layers on the same kernel)",
+                  "tc_gg_tn_kernel<NPL> (weight-gradient gather-GEMM)",
+                  "tc_gg_nt_kernel<256,NPL,1|2|5> (conv forward with the fused instance-norm + GLU / + residual epilogue)"]
         if ln2[k] > 0 and ms2[k] > 0:
             achieved = fl2[k] / (ms2[k] * 1e-3) / 1e12
             peak = pk["bf16_tflops_sustained"]
             roofline = {"bound": "tensor", "kernel": knames[k],
-                        "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": _ncu_traffic(k),
+                        "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                         "note": "achieved = algorithmic conv FLOPs (2*M*N*K, counted once) / summed CUDA-event time of %d launches over 2 steps (%.3f ms per launch avg); "
-                                "peak = %s sustained dense bf16 (cuBLAS); each product costs 3 bf16 MMAs in bf16x3 mode (frac bounded by 1/3) and 2 MMA units in f16f8 mode (one fp16 MMA + two e4m3 MMAs at twice the rate: bounded by 1/2; the weight-gradient kernel of that mode issues the fp16 MMA alone unless wgrad_f16=0); mma_rate_frac = issued MMA units / peak; "
-                                "timed with the two lanes of the step serialised on one stream; traffic = mean DRAM bytes (read + write) per launch over the launches of this kernel in the newest committed ncu --set full capture "
-                                "(profiles/*ncu_tc_kernels_summary.json, newest version; the file lists the launches it holds)"
+                                "peak = %s dense bf16; each product costs 3 bf16 MMAs in bf16x3 mode (frac bounded by 1/3) and 2 MMA units in f16f8 mode (one fp16 MMA + two e4m3 MMAs at twice the rate: bounded by 1/2; the weight-gradient kernel of that mode issues the fp16 MMA alone unless wgrad_f16=0); mma_rate_frac = issued MMA units / peak; "
+                                "timed with the two lanes of the step serialised on one stream"
                                 % (ln2[k], ms2[k] / ln2[k], pk["src"]),
                         "mma_rate_frac": achieved * {"bf16x3": 3.0, "f16f8": 2.0}.get(args.precision, 1.0) / peak,
                         # operand bytes the kernel pulls from L2 into shared memory: (128 + 256) rows x K x 4 B per 128 x 256 tile
-                        # (two 2-byte planes per operand) = 0.0234 B per algorithmic FLOP; the L2 slice throughput cap of this chip
-                        # (~6300 B/clk, B300_MICROARCH.md) is ~12 TB/s -- the ceiling the long-K layers sit at (DESIGN.md section 7)
+                        # (two 2-byte planes per operand) = 0.0234 B per algorithmic FLOP
                         "l2_operand_tbs": achieved * 0.0234375 if args.precision != "bf16" else achieved * 0.0234375 / 2,
                         "share_of_step": ms2[k] / 2.0 / ms_per_step_1stream, "ms_per_step_single_stream": ms_per_step_1stream,
                         "other_kernels": [{"kernel": knames[i], "ms_per_step": ms2[i] / 2.0,

@@ -1,5 +1,5 @@
 /*
- * cgvc.h -- C ABI of libcgvc.so, the B200-native CycleGAN-VC training/inference engine.
+ * cgvc.h -- C ABI of libcgvc.so, the H100-native CycleGAN-VC training/inference engine.
  *
  * The reference (leimao/Voice-Converter-CycleGAN) has no FFI of its own: its seam is the Python
  * class `CycleGAN` (model.py:7-169) driving a TensorFlow-1 session.  Each entry point below names
@@ -43,8 +43,8 @@ typedef struct cgvc_config {
 
 enum {
   CGVC_PREC_FP32_SIMT = 0,  /* every contraction in fp32 FFMA (reference arithmetic; slow, used as on-GPU cross-check) */
-  CGVC_PREC_BF16X3 = 1,     /* tcgen05 bf16 hi/lo split, 3 MMAs per product, fp32 accumulate (~2^-16 rel error; parity mode) */
-  CGVC_PREC_BF16 = 2,       /* tcgen05 single bf16 MMA (fast, NOT parity-grade) */
+  CGVC_PREC_BF16X3 = 1,     /* wgmma bf16 hi/lo split, 3 MMAs per product, fp32 accumulate (~2^-16 rel error; parity mode) */
+  CGVC_PREC_BF16 = 2,       /* wgmma single bf16 MMA (fast, NOT parity-grade) */
   CGVC_PREC_F16F8 = 3       /* fp16 hi*hi MMA + the two cross terms as e4m3 kind::f8f6f4 MMAs at twice the rate, their common power of
                              * two folded out by scale-input-d: 2 MMA units per product instead of 3, parity-grade (4.7e-5 on the
                              * generator output).  Forward and data gradient; the weight gradient -- a leaf of the graph, its rounding
@@ -155,10 +155,9 @@ int cgvc_kernel_launches(unsigned long long* count);
  * "fuse_in" (default 1): instance norm + GLU / + residual fused into the forward conv kernel's epilogue where the shape
  * allows (generator layers whose 128-row tiles hold whole samples); 0 always uses the separate streaming kernels.
  * "fuse_bwd" (default 0): GLU / instance-norm backward of the generator's residual stack fused into the epilogue of the
- * data-gradient kernel that produces its upstream gradient (one kernel per layer backward instead of three); correct and tested,
- * but measured ~1 % slower than the streaming kernels on B200 (DESIGN.md section 7), hence opt-in.
+ * data-gradient kernel that produces its upstream gradient (one kernel per layer backward instead of three); correct and tested, opt-in.
  * "side_wgrad" (default 0): the weight-gradient GEMMs of a train step run on a side stream per lane, off the critical path of the
- * data-gradient chain (needs two_streams; not combined with fuse_bwd).  Correct and tested; measured neutral on a power-capped B200.
+ * data-gradient chain (needs two_streams; not combined with fuse_bwd).  Correct and tested.
  * "pipelined_comm" (default 1): with a communicator attached, cgvc_train_step all-reduces the gradients network by network on a
  * communication stream and runs Adam + the weight-plane refresh of each network as soon as its all-reduce is done (0: one all-reduce
  * of the whole arena, then Adam).
@@ -180,11 +179,9 @@ int cgvc_kernel_launches(unsigned long long* count);
  * "post_stream" (default 1, process-wide): gated layers without pixel shuffle whose samples have 32, 48 or 64 positions take the streaming
  * form of the one-pass GLU / instance-norm backward: persistent CTAs walk (sample, channel block) items through a cp.async double buffer
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
- * "cta_pairs" (default 1, process-wide): tensor-core kernels on CTA pairs (tcgen05 cta_group::2, TMA im2col for the gathered
- * operand) where the shape allows; 0 = the one-CTA kernels everywhere.
  * "debug_taps" (default 0): see cgvc_debug_activation.
  * "tc_debug" (default 0): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
- * 1 = epilogue skips global stores, 2 = also skips TMEM loads, 4 = producers skip the activation gather. */
+ * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather. */
 int cgvc_set_option(cgvc_handle h, const char* name, int value);
 int cgvc_profile_enable(int on);
 int cgvc_profile_collect(double* ms3, double* flops3, long long* launches3);

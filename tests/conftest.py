@@ -11,7 +11,7 @@ for _p in (ROOT, HERE):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a)")
 
 
 @pytest.fixture(scope="session")

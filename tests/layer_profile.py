@@ -5,7 +5,7 @@
 
 Not a pytest file.  Prints one JSON object: rows = one entry per distinct (kernel class, M, N, K) with launch count,
 mean ms, algorithmic TFLOP/s and the fraction of the measured bf16 peak; with --debug-sweep the same table is taken with
-the forward/data-gradient kernel's diagnostic knobs (no epilogue stores / no TMEM loads / no activation gather) to see
+the forward/data-gradient kernel's diagnostic knobs (no epilogue stores / no accumulator reads / no activation gather) to see
 what bounds a tile.  Timings are serialised on one stream (two_streams = 0), like bench.py's roofline pass.
 """
 import argparse

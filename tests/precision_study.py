@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Offline numerical study (CPU, float64 emulation): which split-precision schemes for the tensor-core products stay
-inside the 1e-3 parity budget (BASELINE.json north_star), and what they cost in tcgen05 MMA issue slots.
+inside the 1e-3 parity budget (BASELINE.json north_star), and what they cost in tensor-core MMA issue slots.
 
 TEST INFRASTRUCTURE (imports oracle/): run by hand, results quoted in DESIGN.md section 10.  Nothing in the product
 imports this.

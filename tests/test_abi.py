@@ -26,14 +26,14 @@ def test_library_exports_every_declared_symbol():
     assert lib.cgvc_abi_version() == 1
 
 
-def test_library_is_sm100a_with_tcgen05():
+def test_library_is_sm90a_with_wgmma():
     import subprocess
     from cgvc import native
     out = subprocess.run(["cuobjdump", "-lelf", native.lib_path()], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     sass = subprocess.run(["cuobjdump", "-sass", native.lib_path()], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass and "LDTM" in sass, "tcgen05 kernels missing from the build"
-    assert "UTCQMMA" in sass, "the kind::f8f6f4 MMAs of the F16F8 forward precision are missing from the build"
+    assert "HGMMA.64x256x16.F32.BF16" in sass, "bf16 wgmma kernels missing from the build"
+    assert "QGMMA.64x256x32.F32.E4M3.E4M3" in sass, "the e4m3 wgmma of the F16F8 precision are missing from the build"
     assert "UTMALDG" in sass, "TMA tile loads missing from the build"
 
 

@@ -1,7 +1,7 @@
 """GPU parity of the per-kernel C-ABI entry points against the CPU oracle's primitives (float64).
 
 Tolerances: the fp32 SIMT path must agree to 2e-5 relative (it is the reference arithmetic, fp32);
-the tcgen05 bf16x3 path to 2e-4 relative per kernel (north_star: 1e-3 on activations end to end).
+the tensor-core bf16x3 path to 2e-4 relative per kernel (north_star: 1e-3 on activations end to end).
 """
 import ctypes as C
 

@@ -1,5 +1,5 @@
 """voice-converter-cyclegan_b200: the CycleGAN-VC training/inference hot path of leimao/Voice-Converter-CycleGAN
-re-built for B200 (sm_100a).  `CycleGAN` mirrors the reference class (model.py:7-169); `generator_gatedcnn` and
+re-built for H100 (sm_90a).  `CycleGAN` mirrors the reference class (model.py:7-169); `generator_gatedcnn` and
 `discriminator` mirror the network callables of module.py as native-engine descriptors.
 
 The directory name is not a Python identifier; import it through the root shim:  `import cgvc`.

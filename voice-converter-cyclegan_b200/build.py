@@ -1,4 +1,4 @@
-"""Build libcgvc.so (sm_100a only) in-tree with nvcc.  Used by __graft_entry__.build() and on first import."""
+"""Build libcgvc.so (sm_90a only) in-tree with nvcc.  Used by __graft_entry__.build() and on first import."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcgvc.so")
 SOURCES = ["engine.cu", "simt_kernels.cu", "tc_gemm.cu"]
-HEADERS = ["kernels.cuh", "tc_gemm.cuh", "geom.h", "im2col_map.h", os.path.join("..", "..", "include", "cgvc.h")]
+HEADERS = ["kernels.cuh", "tc_gemm.cuh", "wgmma.cuh", "geom.h", os.path.join("..", "..", "include", "cgvc.h")]
 
 
 def _nvcc():
@@ -39,7 +39,7 @@ def build(force=False, verbose=False):
             if not force and not is_stale():          # another rank built it while we waited
                 return LIB
             tmp = "%s.tmp.%d" % (LIB, os.getpid())
-            cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--threads", "3",
+            cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--threads", "3",
                    "-Xcompiler", "-fPIC", "-shared", "-o", tmp] + [os.path.join(CSRC, s) for s in SOURCES] + ["-lcudart", "-ldl"]
             if verbose:
                 cmd.insert(1, "-Xptxas"); cmd.insert(2, "-v")

@@ -5,7 +5,7 @@ utterance it does what convert.py:33-59 does around the generator call:
 
     f0' = pitch_conversion(f0)                      log-Gaussian pitch transformation with the stored logf0 statistics
     x   = (coded_sp.T - mean_src) / std_src         z-normalise the [24, T] MCEP matrix with the stored MCEP statistics
-    y   = model.test([x], direction)[0]             generator forward on the B200 engine (T % 4 == 0)
+    y   = model.test([x], direction)[0]             generator forward on the H100 engine (T % 4 == 0)
     coded_sp' = (y * std_tgt + mean_tgt).T
 
 What differs, and why:
@@ -180,7 +180,7 @@ def conversion(model_dir, model_name, data_dir, conversion_direction, output_dir
 
 
 def main():
-    p = argparse.ArgumentParser(description='Convert voices using a trained CycleGAN model (native B200 engine).')
+    p = argparse.ArgumentParser(description='Convert voices using a trained CycleGAN model (native H100 engine).')
     p.add_argument('--model_dir', type=str, default='./model/sf1_tm1')
     p.add_argument('--model_name', type=str, default='sf1_tm1.ckpt')
     p.add_argument('--data_dir', type=str, default='./data/evaluation_all/SF1')

@@ -117,9 +117,8 @@ struct cgvc_engine {
   int fuse_in = 1;              // fuse instance norm (+GLU / +residual) into the forward GEMM epilogue where the shape allows
   int debug_taps = 0;           // cgvc_generator_forward also writes the fp32 copy of every layer output (cgvc_debug_activation)
   int fuse_bwd = 0;             // fuse the instance-norm (+GLU) backward into the upstream data-gradient GEMM's epilogue likewise.
-                                // Off by default: measured 69.0 ms/step with it vs 68.2 without (profiles/r01_bench_v9_fusebwd*.json) --
-                                // the 4 epilogue warps need 3x the tile's MMA time for it, and unlike the streaming kernels that
-                                // work cannot overlap the other lane's tensor-core kernels
+                                // Off by default: unlike the streaming kernels, that epilogue work cannot overlap the other lane's
+                                // tensor-core kernels
   // data-parallel step: the gradient all-reduce runs per network on its own stream; Adam and the weight-plane refresh of a network
   // start as soon as its all-reduce has finished, while the next network's is still on the wire
   cudaStream_t comm_stream = nullptr; cudaEvent_t ev_grads = nullptr, ev_ar[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -127,9 +126,7 @@ struct cgvc_engine {
   int fuse_c1 = 1;              // discriminator input layer backward: GLU backward fused into its weight / data gradient kernels
   int edge_lower = 1;           // the generator's 15-tap, 24-channel edge layers as dense 1 x 1 GEMMs (taps moved into the channel / column dimension)
   int two_streams = 1;          // 0: both lanes are enqueued on the caller's stream (clean per-kernel timing for profiling)
-  int side_wgrad = 0;           // weight-gradient GEMMs on a side stream per lane (see SideQ); needs two_streams, excludes fuse_bwd.  Off by default:
-                                // measured neutral under the 1 kW power cap (60.6-60.8 vs 60.5 ms/step, profiles/r02_bench_ab_*.json) -- the step is
-                                // energy-bound there, so re-ordering work does not shorten it
+  int side_wgrad = 0;           // weight-gradient GEMMs on a side stream per lane (see SideQ); needs two_streams, excludes fuse_bwd.  Off by default
   SideQ sideq[2];
   // debug taps of the last forward
   std::map<std::string, std::pair<const float*, size_t>> taps;
@@ -238,7 +235,7 @@ static void build_discriminator(TableBuilder& tb, DiscNet& d) {
   d.end = tb.off;
 }
 
-// ---- conv building blocks (dispatch: tcgen05 where the layer is registered, else fp32 SIMT) ---------------------
+// ---- conv building blocks (dispatch: tensor cores where the layer is registered, else fp32 SIMT) ---------------------
 struct ConvIO {               // one convolution application
   const float* x; const __nv_bfloat16 *xhi, *xlo;   // input [n,H,W,Cin] fp32 (may be null on the tensor-core path) + bf16 planes
   int n, H, W;
@@ -992,7 +989,7 @@ int cgvc_create(const cgvc_config* cfg, cgvc_handle* out) {
   ce = dguard.set(cfg->device);
   if (ce != cudaSuccess) return fail(nullptr, CGVC_ERR_CUDA, "cudaSetDevice: %s", cudaGetErrorString(ce));
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, cfg->device);
-  if (prop.major != 10) return fail(nullptr, CGVC_ERR_CUDA, "libcgvc is built for sm_100a only; device is sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(nullptr, CGVC_ERR_CUDA, "libcgvc is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
   cgvc_engine* e = new cgvc_engine();
   e->cfg = *cfg;
   TableBuilder tb{e->tensors};
@@ -1521,7 +1518,7 @@ int cgvc_set_option(cgvc_handle e, const char* name, int value) {
   if (!strcmp(name, "debug_taps")) { e->debug_taps = value != 0; return 0; }
   if (!strcmp(name, "cuda_graph")) { e->use_graphs = value != 0; return 0; }
   if (!strcmp(name, "tc_debug")) { tc_set_debug(value); return 0; }
-  if (!strcmp(name, "post_onepass")) {                       // process-wide, like cta_pairs
+  if (!strcmp(name, "post_onepass")) {                       // process-wide, like prep_batched
     post_set_onepass(value);
     for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
     e->graphs.clear();
@@ -1541,12 +1538,6 @@ int cgvc_set_option(cgvc_handle e, const char* name, int value) {
   }
   if (!strcmp(name, "prep_batched")) {                       // process-wide; the captured Adam + refresh graphs hold the old kernels
     tc_set_prep_batched(value);
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-    e->graphs.clear();
-    return 0;
-  }
-  if (!strcmp(name, "cta_pairs")) {                          // process-wide switch; captured graphs hold the old kernels
-    tc_set_pair(value);
     for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
     e->graphs.clear();
     return 0;

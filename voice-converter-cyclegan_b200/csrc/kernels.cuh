@@ -1,4 +1,4 @@
-// Internal kernel-launcher declarations for libcgvc.so (sm_100a only).
+// Internal kernel-launcher declarations for libcgvc.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -35,6 +35,9 @@ __device__ __forceinline__ void cgvc_quant4(const float (&v)[4], float s_hi, flo
 #endif
 
 extern unsigned long long g_cgvc_launches;   // incremented by every kernel launch of the library
+
+// grid caps of the streaming kernels: multiples of the SM count of an H100 SXM
+#define CGVC_NUM_SMS 132
 
 #define CGVC_MAX_TAPS 18   // largest filter on the path: discriminator d3, 6x3 (module.py:208)
 

@@ -1,6 +1,6 @@
-// fp32 SIMT kernels of libcgvc.so (sm_100a).
+// fp32 SIMT kernels of libcgvc.so (sm_90a).
 //
-// These are (a) the reference-arithmetic path used as the on-GPU cross-check of the tcgen05 kernels and
+// These are (a) the reference-arithmetic path used as the on-GPU cross-check of the tensor-core kernels and
 // (b) the permanent path for everything that is not a dense contraction with K >= 64: the K=9 discriminator
 // input layer (HBM-bound), the 24-channel generator input/output convs, instance-norm / GLU / residual
 // elementwise passes, the discriminator head, the losses and Adam.
@@ -855,13 +855,13 @@ post_bwd_onepass_kernel(const __grid_constant__ PostBwdParams q) {
 }
 
 // Streaming form of the one-pass kernel (round 2): the register-resident kernel above issues its loads, waits, computes, stores -- with
-// 128 ... 189 registers per thread one or two CTAs fit on an SM and the memory pipe idles in the compute and store phases (measured
-// 2.0 ... 3.0 TB/s; the sums + apply pair of the longer samples moves 32 instead of 20 bytes per element at 2.4 ... 2.8 TB/s).  Here a
+// 128 ... 189 registers per thread one or two CTAs fit on an SM and the memory pipe idles in the compute and store phases (the sums +
+// apply pair of the longer samples moves 32 instead of 20 bytes per element).  Here a
 // persistent CTA walks (sample, channel block) items through a double buffer in shared memory: every thread copies its own rows of dY
 // and of the saved pre-norm outputs (+ the item's statistics / affine parameters) for item i + 1 with 16-byte cp.async while item i is
 // reduced and applied out of shared memory, so a CTA always has up to 48 KB (72 KB for 384 positions) of loads in flight and needs few
 // registers.  Item = all R positions of one sample x CB = 4 * NQL channels; R = (256 / NQL) * NRT covers every instance-normed layer of
-// the model at 128 frames: 32, 48, 64, 96, 128 and 384 positions, with or without the pixel-shuffle view.  4.7 TB/s measured.
+// the model at 128 frames: 32, 48, 64, 96, 128 and 384 positions, with or without the pixel-shuffle view.
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
@@ -1164,7 +1164,7 @@ static cudaError_t launch_post_fwd_stream(const PostParams& pp, cudaStream_t st)
   using Cfg = StreamFwdCfg<NQL, NRT>;
   const int cblocks = pp.C / Cfg::CB;
   const long long items = (long long)pp.B * cblocks;
-  const int grid = (int)(items < 2 * 148 ? items : 2 * 148);
+  const int grid = (int)(items < 2 * CGVC_NUM_SMS ? items : 2 * CGVC_NUM_SMS);
   ++g_cgvc_launches;
   post_fwd_stream_kernel<NQL, NRT><<<grid, 256, Cfg::SMEM, st>>>(pp, (int)items, cblocks);
   return cudaGetLastError();
@@ -1190,7 +1190,7 @@ static cudaError_t launch_post_bwd_stream(const PostBwdParams& pp, cudaStream_t 
   using Cfg = StreamCfg<NQL, NRT>;
   const int cblocks = pp.C / Cfg::CB;
   const long long items = (long long)pp.B * cblocks;
-  const int grid = (int)(items < Cfg::CTAS * 148 ? items : Cfg::CTAS * 148);
+  const int grid = (int)(items < Cfg::CTAS * CGVC_NUM_SMS ? items : Cfg::CTAS * CGVC_NUM_SMS);
   ++g_cgvc_launches;
   post_bwd_stream_kernel<NQL, NRT, GATE><<<grid, 256, Cfg::SMEM, st>>>(pp, (int)items, cblocks);
   return cudaGetLastError();
@@ -1452,7 +1452,7 @@ cudaError_t launch_adam(float* p, const float* g, float* m, float* v, long long 
   if (n == 0) return cudaSuccess;
   if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
        reinterpret_cast<uintptr_t>(v)) & 15) return cudaErrorMisalignedAddress;
-  long long nb = ((n >> 2) + 255) / 256; if (nb > 148 * 16) nb = 148 * 16; if (nb < 1) nb = 1;
+  long long nb = ((n >> 2) + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16; if (nb < 1) nb = 1;
   ++g_cgvc_launches; adam_kernel<<<(unsigned)nb, 256, 0, st>>>(p, g, m, v, n, hyper_dev, beta1, beta2, eps);
   return cudaGetLastError();
 }
@@ -1567,7 +1567,7 @@ cudaError_t launch_wgrad_c1(const GatherGeom& g, const float* src, const float* 
   if (M == 0) return cudaSuccess;
   int nq = N / 4;
   if (N % 4 != 0 || nq > 256 || 256 % nq != 0 || n_split % 4 != 0 || g_ld % 4 != 0) return cudaErrorInvalidValue;
-  int rpb = (int)((M + 148 * 8 - 1) / (148 * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
+  int rpb = (int)((M + CGVC_NUM_SMS * 8 - 1) / (CGVC_NUM_SMS * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
   ++g_cgvc_launches;
   if (g.ntaps <= 9) wgrad_c1_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb);
   else wgrad_c1_kernel<CGVC_MAX_TAPS><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb);
@@ -1653,7 +1653,7 @@ cudaError_t launch_glu_bwd_wgrad_c1(const GatherGeom& g, const float* src, const
   if (M == 0) return cudaSuccess;
   int nq = C / 4;
   if (C % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9) return cudaErrorInvalidValue;
-  int rpb = (int)((M + 148 * 8 - 1) / (148 * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
+  int rpb = (int)((M + CGVC_NUM_SMS * 8 - 1) / (CGVC_NUM_SMS * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
   ++g_cgvc_launches;
   glu_bwd_wgrad_c1_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, src, dy, P, C, dw_a, dw_g, db_a, db_g, rpb);
   return cudaGetLastError();
@@ -1725,10 +1725,10 @@ cudaError_t launch_glu_bwd_dgrad_c1(const float* dy, const float* P, int C, cons
   long long rows = (long long)B * Ho * Wo;
   if (rows == 0) return cudaSuccess;
   if (C != 128 || kh * kw > 9) return cudaErrorInvalidValue;
-  long long nb = (rows + 23) / 24; if (nb > 148 * 8) nb = 148 * 8;
+  long long nb = (rows + 23) / 24; if (nb > CGVC_NUM_SMS * 8) nb = CGVC_NUM_SMS * 8;
   g_cgvc_launches += 2;
   glu_bwd_proj_c1_kernel<<<(unsigned)nb, 256, 0, st>>>(dy, P, rows, wa, wg, kh * kw, Z);
-  long long n = (long long)B * H * W; long long nb2 = (n + 255) / 256; if (nb2 > 148 * 16) nb2 = 148 * 16;
+  long long n = (long long)B * H * W; long long nb2 = (n + 255) / 256; if (nb2 > CGVC_NUM_SMS * 16) nb2 = CGVC_NUM_SMS * 16;
   gather_taps_kernel<<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw);
   return cudaGetLastError();
 }
@@ -1801,10 +1801,10 @@ cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float*
   if (rows == 0) return cudaSuccess;
   if (C % 128 != 0 || kh * kw > CGVC_MAX_TAPS) return cudaErrorInvalidValue;
   size_t smem = (size_t)kh * kw * C * sizeof(float);
-  long long nb = (rows + 7) / 8; if (nb > 148 * 8) nb = 148 * 8;
+  long long nb = (rows + 7) / 8; if (nb > CGVC_NUM_SMS * 8) nb = CGVC_NUM_SMS * 8;
   g_cgvc_launches += 2;
   proj_taps_kernel<<<(unsigned)nb, 256, smem, st>>>(G, rows, C, wa, wg, c_split, kh * kw, Z);
-  long long n = (long long)B * H * W; long long nb2 = (n + 255) / 256; if (nb2 > 148 * 16) nb2 = 148 * 16;
+  long long n = (long long)B * H * W; long long nb2 = (n + 255) / 256; if (nb2 > CGVC_NUM_SMS * 16) nb2 = CGVC_NUM_SMS * 16;
   gather_taps_kernel<<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw);
   return cudaGetLastError();
 }
@@ -1840,7 +1840,7 @@ pad_split_q_kernel(const float* __restrict__ x, long long M, int C, int ld, int 
 cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st) {
   if (M == 0) return cudaSuccess;
   if (Cpad % 4) return cudaErrorInvalidValue;
-  long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > 148 * 16) nb = 148 * 16;
+  long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
   pad_split_q_kernel<<<(unsigned)nb, 256, 0, st>>>(x, M, C, ld, Cpad, (__half*)q16, (uint8_t*)q8);
   return cudaGetLastError();
@@ -1848,7 +1848,7 @@ cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int C
 
 cudaError_t launch_pad_split(const float* x, long long M, int C, int ld, int Cpad, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st) {
   if (M == 0) return cudaSuccess;
-  long long n = M * Cpad; long long nb = (n + 255) / 256; if (nb > 148 * 16) nb = 148 * 16;
+  long long n = M * Cpad; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
   pad_split_kernel<<<(unsigned)nb, 256, 0, st>>>(x, M, C, ld, Cpad, hi, lo);
   return cudaGetLastError();
@@ -1896,7 +1896,7 @@ cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw
   if (M == 0) return cudaSuccess;
   if (C % 4 || Cpad % 4 || Cpad < kw * C || T <= 0 || M % T) return cudaErrorInvalidValue;
   const int pl = (kw - 1) / 2;                      // TF SAME at stride 1: total pad kw - 1, the smaller half on the left
-  long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > 148 * 16) nb = 148 * 16;
+  long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
   if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo);
   else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo);
@@ -1927,7 +1927,7 @@ cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int 
   if (M == 0) return cudaSuccess;
   if (C % 4 || ldz % 4 || T <= 0 || M % T) return cudaErrorInvalidValue;
   const int pl = (kw - 1) / 2;
-  long long n = M * (C / 4); long long nb = (n + 255) / 256; if (nb > 148 * 16) nb = 148 * 16;
+  long long n = M * (C / 4); long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
   col2im_taps_kernel<<<(unsigned)nb, 256, 0, st>>>(z, ldz, M, T, C, kw, pl, dir, bias, y);
   return cudaGetLastError();
@@ -2145,7 +2145,7 @@ __global__ void __launch_bounds__(256) scale_kernel(float* __restrict__ x, long 
 }
 cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st) {
   if (n == 0) return cudaSuccess;
-  long long nb = (n + 255) / 256; if (nb > 148 * 8) nb = 148 * 8;
+  long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 8) nb = CGVC_NUM_SMS * 8;
   ++g_cgvc_launches; scale_kernel<<<(unsigned)nb, 256, 0, st>>>(x, n, a);
   return cudaGetLastError();
 }

@@ -1,25 +1,25 @@
-// tcgen05 gather-GEMM kernels of libcgvc.so (sm_100a): the dense contractions of the CycleGAN-VC hot path
-// (module.py:22-64 convolutions, forward / data-gradient / weight-gradient) on the 5th-generation tensor cores.
+// Tensor-core gather-GEMM kernels of libcgvc.so (sm_90a): the dense contractions of the CycleGAN-VC hot path
+// (module.py:22-64 convolutions, forward / data-gradient / weight-gradient) on the Hopper tensor cores (wgmma).
 //
 // Arithmetic: every fp32 operand x is kept in HBM as two bf16 planes (hi = bf16(x), lo = bf16(x - hi)); a product
-// is evaluated as hi*hi + hi*lo + lo*hi by three tcgen05.mma (kind::f16, bf16 inputs) accumulating in fp32 in
-// TMEM ("bf16x3", ~2^-16 relative error per product); CGVC_PREC_BF16 issues the first MMA only.  CGVC_PREC_F16F8 (forward
-// only) keeps fp16 + two scaled e4m3 planes instead and spends 2 MMA units per product: the two cross terms as kind::f8f6f4
-// MMAs first, then the fp16 hi*hi MMAs whose first one rescales the accumulator by 2^-15 (scale-input-d).
+// is evaluated as hi*hi + hi*lo + lo*hi by three wgmma (bf16 inputs) accumulating in fp32 registers ("bf16x3", ~2^-16
+// relative error per product); CGVC_PREC_BF16 issues the first MMA only.  CGVC_PREC_F16F8 keeps fp16 + two scaled e4m3 planes
+// instead and spends 2 MMA units per product: the two cross terms first (e4m3 wgmma), then the accumulator is rescaled by 2^-15
+// and the fp16 hi*hi wgmma follow.
 //
-// Kernel anatomy (both kernels are persistent, one CTA per SM, 288 threads, tiles / work items walked with stride gridDim.x):
-//   warps 0-3  producers: gather the activation rows (im2col rows, zero-filled at the TF-SAME borders) with 16-byte cp.async
-//              into SWIZZLE_128B shared memory; one thread TMA-loads the weight (NT) / gradient (TN) tile; both complete on
-//              the stage's "full" mbarrier.  They run ahead across tile boundaries.
-//   warp  4    allocates TMEM (2 accumulator stages), issues tcgen05.mma from one elected lane, frees stages with
-//              tcgen05.commit
-//   warps 5-8  epilogue: tcgen05.ld the finished accumulator stage while the next tile's MMAs run; bias / accumulate, the fused
-//              instance-norm (+GLU / +residual) forward epilogues, the opt-in fused backward epilogues; every global store is
-//              transposed through a per-warp shared-memory patch so that 8 lanes write one row (complete 128-byte lines)
+// Kernel anatomy (both kernels are persistent, one CTA per SM, 384 threads, tiles / work items walked with stride gridDim.x):
+//   warps 0-3   producers: gather the activation rows (im2col rows, zero-filled at the TF-SAME borders) with 16-byte cp.async
+//               into SWIZZLE_128B shared memory; one thread TMA-loads the weight (NT) / gradient (TN) tile; both complete on
+//               the stage's "full" mbarrier.
+//   warps 4-11  two consumer warpgroups, 64 accumulator rows each: wgmma from the shared-memory stages into registers, stages
+//               released through the "empty" mbarriers.  NT: the finished tile is passed through shared memory to the epilogue
+//               (bias / accumulate, the fused instance-norm (+GLU / +residual) forward epilogues, the opt-in fused backward
+//               epilogues), whose global stores are transposed through a per-warp patch so that 8 lanes write one row.
+//               TN: red.global.add of the accumulator fragments into the weight gradient.
 #include "tc_gemm.cuh"
 #include "geom.h"
 #include "kernels.cuh"
-#include "im2col_map.h"
+#include "wgmma.cuh"
 
 #include <cuda.h>      // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint, no libcuda link)
 #include <stdint.h>
@@ -100,157 +100,39 @@ __device__ __forceinline__ void tma_load3(uint32_t dst_smem, const CUtensorMap* 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "n"(COLS) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// kind::f8f6f4 (e4m3 x e4m3 here): 128 x N x 32 per instruction, same shared-memory tile layout (32 bytes per k-step)
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D = A * B + D * 2^-15  (scale-input-d): folds the common 2^15 of the fp8 cross products out of the accumulator
-__device__ __forceinline__ void umma_f16_rescale(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, 1, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p, 15;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc) : "memory");
-}
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------ CTA-pair (cta_group::2) PTX
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// A protocol error in a pair kernel must not hang the device: waits give up after ~4 s and trap (the launch then fails loudly).
-__device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
-  uint64_t t0 = 0;
-  for (uint32_t tries = 0;; ++tries) {
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    if (ok) return;
-    if ((tries & 0x3FFu) == 0x3FFu) {
-      uint64_t t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      if (t0 == 0) t0 = t; else if (t - t0 > 4000000000ull) __trap();
-    }
-  }
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc2(uint32_t* slot) {        // executed by the same warp of BOTH CTAs of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc2(uint32_t addr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "n"(COLS) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[both CTAs' smem, 128 rows each] * B[both CTAs' smem, N/2 rows each]; issued by the leader only
-__device__ __forceinline__ void umma2_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma2_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D = A * B + D * 2^-SHIFT (scale-input-d): folds the common scale of the fp8 cross products out of the accumulator
-template <int SHIFT>
-__device__ __forceinline__ void umma2_f16_rescale(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, 1, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p, %4;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "n"(SHIFT) : "memory");
-}
-// the barrier at this shared-memory offset receives one arrival in BOTH CTAs once all previously issued MMAs have completed
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// TMA loads of a pair: data lands in the issuing CTA's shared memory, the bytes are counted on the LEADER's barrier (peer bit cleared)
-__device__ __forceinline__ void tma2_load3(uint32_t dst_smem, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-               ::"r"(dst_smem), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar) & 0xFEFFFFFFu) : "memory");
-}
-__device__ __forceinline__ void tma2_im2col(uint32_t dst_smem, const CUtensorMap* map, int c, int w, int h, int n, unsigned short ow, unsigned short oh, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
-               ::"r"(dst_smem), "l"(map), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c), "r"(w), "r"(h), "r"(n), "h"(ow), "h"(oh) : "memory");
-}
-// one arrival on the barrier at this shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp): SWIZZLE_128B, version 1.
-//   K-major : 8-row groups of 128-byte rows, SBO = 1024 B between groups, LBO unused (1)
+// Shared-memory matrix descriptor of wgmma, SWIZZLE_128B (layout type 1 in bits 62-63):
+//   K-major : 8-row groups of 128-byte rows, SBO = 1024 B between groups, LBO unused
 //   MN-major: atoms of (64 MN-elements x 8 K-rows) = 1024 B; LBO = stride between atoms along MN, SBO = along K
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (2ull << 61);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 62);
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): bf16 x bf16 -> f32
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// keeps the compiler from moving accesses of the accumulator registers across the asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-// fp16 x fp16 -> f32 (kind::f16) and e4m3 x e4m3 -> f32 (kind::f8f6f4) share this encoding: formats 0 / 0, K-major
-__host__ __device__ constexpr uint32_t make_idesc_f0(int M, int N) { return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// the 256 consumer threads (two warpgroups) of a CTA; ids 1 and 2 are the epilogue groups' barriers
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
+__device__ __forceinline__ void st_shared16(uint32_t addr, uint4 v) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+// 8 e4m3 values -> 8 fp16 values (exact: every e4m3 number is an fp16 number)
+__device__ __forceinline__ uint4 e4m3x8_to_f16x8(uint2 v) {
+  uint32_t w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t src = (i < 2 ? v.x : v.y) >> (16 * (i & 1));
+    const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(src & 0xFFFFu), __NV_E4M3);
+    w[i] = (uint32_t)h.x | ((uint32_t)h.y << 16);
+  }
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
 
 // exact unsigned division by a runtime constant (n < 2^31): q = (umulhi(n, mul) + n) >> shr, Granlund-Montgomery round-up form
 struct FastDiv { uint32_t mul, shr, d; };
@@ -274,7 +156,7 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   int N;                                                 // real output columns (stores are guarded; tiles cover Nw)
   int n_tiles;                                           // column tiles to compute (host: covers the real columns only)
   int debug;                                             // diagnostic knobs (tc_set_debug): 1 = epilogue skips its global stores, 2 = also skips
-                                                         // the TMEM loads, 4 = producers skip the A gather.  Results are garbage; timing only.
+                                                         // the accumulator reads, 4 = producers skip the A gather.  Results are garbage; timing only.
   float* dst; int d_ld; const float* bias; int accumulate;
   int perm; int Cc;                                      // gated layers: weight rows / bias are stored tile-interleaved: tile j =
                                                          // [a-channels j*128..+127 | g-channels j*128..+127]; Cc = channels per branch
@@ -295,15 +177,6 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   const uint8_t *a8_hi, *a8_lo;                          // [rows, a_ld] bytes
   CUtensorMap tm_b8_hi, tm_b8_lo;                        // box [1][BN][128 bytes]
   uint8_t* y8;                                           // fused epilogues: q8hi plane of y [M, C_out] bytes, q8lo follows at + M * C_out (y_hi = q16)
-  // CTA-pair kernel (tc_pair_nt_kernel): the gathered operand comes through TMA im2col maps of the activation planes
-  // (128 pixels x 64 channels per load), each CTA of a pair loads half of the weight tile (box [1][BN/2][64])
-  Im2colGeom ig;
-  CUtensorMap tm_a_hi, tm_a_lo;
-  CUtensorMap tm_b2_hi, tm_b2_lo;
-  CUtensorMap tm_b64_hi, tm_b64_lo; int have_b64;        // the weight planes with 64-row boxes: 128-wide pair tiles chosen at launch time
-  // F16F8 on CTA pairs: tm_a_hi / tm_b2_hi are then the fp16 planes; the e4m3 planes (128 channels per 128-byte line):
-  CUtensorMap tm_a8_hi, tm_a8_lo;                        // im2col, 128 pixels x 128 bytes
-  CUtensorMap tm_b28_hi, tm_b28_lo;                      // box [1][BN/2][128 bytes]
 };
 
 struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[src(m,t), c] * G[m, n]
@@ -314,12 +187,9 @@ struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[
   int ksplit;
   FastDiv div_hw, div_w;                                 // m -> (b, y, x) without integer division
   CUtensorMap tm_g_hi, tm_g_lo;                          // TMA maps of the gradient planes [M][g_ld], box [64 rows][64 cols]
-  // CTA-pair kernel (tc_pair_tn_kernel): X through TMA im2col maps (64 pixels x 64 channels per load)
-  Im2colGeom ig;
-  CUtensorMap tm_x_hi, tm_x_lo;
-  // F16F8 weight gradient (tc_pair_tn_q_kernel), 128 K-rows per stage: fp16 planes (tm_xq: im2col 128 pixels x 64 channels, tm_gq: box
-  // [128 rows][64 columns]) and e4m3 planes (tm_x8_*: im2col 128 pixels x 128 channels, tm_g8_*: box [128 rows][128 columns])
-  CUtensorMap tm_xq, tm_gq, tm_x8_hi, tm_x8_lo, tm_g8_hi, tm_g8_lo;
+  // F16F8 (NPL 3): x_hi / tm_g_hi are the fp16 planes; the e4m3 planes of both operands (widened to fp16 by the producers)
+  const uint8_t *x8_hi, *x8_lo;                          // [rows_in, x_ld] bytes
+  const uint8_t *g8_hi, *g8_lo;                          // [M, g_ld] bytes
   int w16;                                               // 1: fp16 planes only (one MMA unit per product; weight gradients are leaves of the graph)
   int fold_n;                                            // != 0: tap-folded layer (TcLayer::fold): column = t * fold_n + n of a [taps][C][fold_n] TF kernel
 };
@@ -340,9 +210,24 @@ struct NTCfg {
   static constexpr int B_PLANE = BN * 128;
   static constexpr int PLANES = NPL == 1 ? 1 : 2;       // F16F8 (NPL = 3) stages hold two 128-byte-row tiles per operand as well
   static constexpr int STAGE = PLANES * (A_PLANE + B_PLANE);
-  static constexpr int STAGES = (200 * 1024) / STAGE;   // 2 (BN=256,x3), 3 (128,x3), 5 (32,x3), 4 (256,x1), 6 (128,x1), 10 (32,x1)
+  static constexpr int STAGES = (192 * 1024) / STAGE;   // 2 (BN=256,x3), 3 (128,x3), 4 (32,x3), 4 (256,x1), 6 (128,x1), 9 (32,x1)
   static constexpr int SMEM = STAGES * STAGE + 1024;
+  static_assert(STAGES * STAGE >= 128 * BN * 4, "the finished fp32 tile is staged over the pipeline stages");
 };
+
+// The finished 128 x BN fp32 tile in shared memory: row r, column n at r * BN + (n & ~31) + (((n >> 2) & 7) ^ (r & 7)) * 4 + (n & 3)
+// (16-byte chunks of every 32-column block XOR-swizzled by the row: the row-per-lane reads of acc_ld32 are conflict-free)
+template <int BN>
+__device__ __forceinline__ int acc_off(int r, int n) { return r * BN + (n & ~31) + ((((n >> 2) & 7) ^ (r & 7)) << 2) + (n & 3); }
+// columns [col, col + 32) of tile row r (col a multiple of 32)
+template <int BN>
+__device__ __forceinline__ void acc_ld32(const float* acc, int r, int col, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    const float4 x = *reinterpret_cast<const float4*>(acc + r * BN + col + ((c ^ (r & 7)) << 2));
+    v[4 * c] = __float_as_uint(x.x); v[4 * c + 1] = __float_as_uint(x.y); v[4 * c + 2] = __float_as_uint(x.z); v[4 * c + 3] = __float_as_uint(x.w);
+  }
+}
 
 // ---- fused instance-norm epilogue helpers -----------------------------------------------------------------------
 // Column sums over the 32 rows of a warp (row = lane): butterfly transpose-reduce, 31 shuffles for 32 columns.
@@ -437,23 +322,11 @@ __device__ __forceinline__ void pair_norm_coeffs(const float (&v0)[32], const fl
 }
 
 // ---- warp-cooperative coalesced row stores -----------------------------------------------------------------------
-// Every lane of an epilogue warp owns one tile row (TMEM lane == row).  If each lane stored its own 32 columns, one warp-wide
-// 16-byte store would touch 32 different rows: 32 half-used sectors and 32 address phases in the LSU, queued in front of the
-// producers' cp.async (measured: 8 % of the kernel, profiles/r01_layer_profile_v9.txt, tc_debug = 1).  Instead the warp
-// transposes each 32 x 32-word block through a 4 KB shared-memory patch (16-byte chunks XOR-swizzled by the row: conflict
-// free both ways) and writes it back with 8 lanes per row -- 4 complete 128-byte lines per instruction.
-__device__ __forceinline__ void stage_rows(float* stg, const float (&o)[32], int lane) {
-  __syncwarp();                                            // earlier readers of the patch are done
-#pragma unroll
-  for (int c = 0; c < 8; ++c)
-    *reinterpret_cast<float4*>(stg + lane * 32 + ((c ^ (lane & 7)) << 2)) = make_float4(o[4 * c], o[4 * c + 1], o[4 * c + 2], o[4 * c + 3]);
-  __syncwarp();
-}
-__device__ __forceinline__ float4 staged_chunk(const float* stg, int row, int chunk) {
-  return *reinterpret_cast<const float4*>(stg + row * 32 + ((chunk ^ (row & 7)) << 2));
-}
+// Every lane of an epilogue warp owns one tile row.  If each lane stored its own 32 columns, one warp-wide 16-byte store would
+// touch 32 different rows (32 half-used sectors); instead the warp transposes its rows through a shared-memory patch and writes
+// them back with several lanes per row.
 // ---- half-width transposition patch (NT epilogues) -------------------------------------------------------------------------
-// The forward / data-gradient epilogues run on up to 8 warps per CTA (CTA-pair kernel), and shared memory is full at 3 x 64 KB of
+// The forward / data-gradient epilogues run on 8 warps per CTA, and shared memory is full with the
 // pipeline stages, so their per-warp patch is 32 rows x 16 words = 2 KB: a 32-word row passes through it in two halves.  16-byte
 // chunk c (0..3) of row r lives at word r*16 + ((c ^ ((r >> 1) & 3)) << 2): conflict-free for the row-wise writes (lane = row) and
 // for the write-back role (chunk lane & 3 of rows (lane >> 2) + 8 i), which covers 8 rows x 64 bytes per warp instruction.
@@ -566,21 +439,20 @@ __device__ __forceinline__ void hwrite_yq(float* stg, const float (&y)[32], floa
   });
 }
 
-// ---- epilogue of one 128-row x BN-column accumulator tile (shared by the one-CTA and the CTA-pair kernels) ----------------
-// Called by the epilogue warps of a CTA: 4 warps (one per TMEM lane quarter q) form a group; with ngrp = 2 groups (CTA-pair kernel)
-// group grp takes the 32-column chunks grp, grp + 2, ... of the tile.  m0 = first row of this CTA's 128 rows, n0 = first column of
-// the tile, tacc = TMEM address of this warp's lanes of the accumulator stage; waits for `acc_full_bar` (parity aphase).
-// stg / rowp / bc: this warp's 2 KB transposition patch, destination-row table and coefficient broadcast area; epi_xch: the group's
-// cross-warp exchange area (statistics of samples that span several warps; barrier 1 + grp).
+// ---- epilogue of one 128-row x BN-column accumulator tile ------------------------------------------------------------------
+// Called by the 8 consumer warps of a CTA once the finished tile is in shared memory (acc, layout acc_off): 4 warps (one per 32-row
+// quarter q) form a group; group grp of ngrp takes the 32-column chunks grp, grp + ngrp, ... of the tile.  m0 = first row of the
+// tile, n0 = its first column.  stg / rowp / bc: this warp's 2 KB transposition patch, destination-row table and coefficient
+// broadcast area; epi_xch: the group's cross-warp exchange area (statistics of samples that span several warps; barrier 1 + grp).
 template <int BN, int NPL, int EPI>
 __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long long M, const int HW, const long long m0, const int n0,
                                                  const int q, const int lane, float* stg, float** rowp, float* bc, float (*epi_xch)[32],
-                                                 uint64_t* acc_full_bar, const uint32_t aphase, const uint32_t tacc,
-                                                 const int grp = 0, const int ngrp = 1) {
+                                                 const float* acc, const int grp = 0, const int ngrp = 1) {
   const GatherGeom& g = p.g;
   const int barid = 1 + grp;
+  const int arow = q * 32 + lane;                        // this lane's tile row
   const long long mq = m0 + q * 32;                      // first row of this warp
-  const long long m = mq + lane;                         // TMEM lane == tile row
+  const long long m = mq + lane;
   float* drow = nullptr;
   if (m < M && p.dst) {                                  // dst may be null for the fused forward epilogues (inference: nothing kept for backward)
     int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
@@ -591,8 +463,6 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
   __syncwarp();
   rowp[lane] = drow;                                     // destination row of every tile row, for the write-back lanes
   __syncwarp();
-  mbar_wait(acc_full_bar, aphase);
-  tc_fence_after();
   if (EPI == 0) {
 #pragma unroll 1
     for (int cb = grp; cb < BN / 32; cb += ngrp) {
@@ -605,7 +475,7 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
       if (n >= p.N) { if (p.perm) continue; else break; }  // warp-uniform
       if (p.debug & 2) continue;
       float o[32];
-      { uint32_t v[32]; tmem_ld32(tacc + (uint32_t)(cb * 32), v); tmem_ld_wait();
+      { uint32_t v[32]; acc_ld32<BN>(acc, arow, (cb * 32), v);
 #pragma unroll
         for (int k = 0; k < 32; ++k) o[k] = __uint_as_float(v[k]); }
       if (p.bias) {
@@ -615,12 +485,20 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
       if (!(p.debug & 1))
         rows_out(stg, o, lane, [&](int rr, int w0, float4 val) {
           float* rp = rowp[rr];
-          const int col = n + w0;                          // N is a multiple of 4; padded columns are never stored
+          const int col = n + w0;                          // padded columns are never stored
           if (rp != nullptr && col < p.N) {
-            if (p.accumulate)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(rp + col), "f"(val.x), "f"(val.y), "f"(val.z), "f"(val.w) : "memory");
-            else
-              *reinterpret_cast<float4*>(rp + col) = val;
+            if (col + 4 <= p.N && (p.d_ld & 3) == 0) {
+              if (p.accumulate)
+                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(rp + col), "f"(val.x), "f"(val.y), "f"(val.z), "f"(val.w) : "memory");
+              else
+                *reinterpret_cast<float4*>(rp + col) = val;
+            } else {                                       // a data gradient with cin % 4 != 0 (the discriminator's one-channel input)
+              const float v4[4] = {val.x, val.y, val.z, val.w};
+              for (int k = 0; k < 4 && col + k < p.N; ++k) {
+                if (p.accumulate) atomicAdd(rp + col + k, v4[k]);
+                else rp[col + k] = v4[k];
+              }
+            }
           }
         });
     }
@@ -636,11 +514,11 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
       for (int cb = grp; cb < 4; cb += ngrp) {
         const int ch = ch0 + cb * 32;
         float va[32], vg[32];
-        { uint32_t u[32]; tmem_ld32(tacc + (uint32_t)(cb * 32), u); tmem_ld_wait();
+        { uint32_t u[32]; acc_ld32<BN>(acc, arow, (cb * 32), u);
 #pragma unroll
           for (int k = 0; k < 32; k += 4) { float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + cb * 32 + k);
             va[k] = __uint_as_float(u[k]) + bb.x; va[k + 1] = __uint_as_float(u[k + 1]) + bb.y; va[k + 2] = __uint_as_float(u[k + 2]) + bb.z; va[k + 3] = __uint_as_float(u[k + 3]) + bb.w; } }
-        { uint32_t u[32]; tmem_ld32(tacc + (uint32_t)(128 + cb * 32), u); tmem_ld_wait();
+        { uint32_t u[32]; acc_ld32<BN>(acc, arow, (128 + cb * 32), u);
 #pragma unroll
           for (int k = 0; k < 32; k += 4) { float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + 128 + cb * 32 + k);
             vg[k] = __uint_as_float(u[k]) + bb.x; vg[k + 1] = __uint_as_float(u[k + 1]) + bb.y; vg[k + 2] = __uint_as_float(u[k + 2]) + bb.z; vg[k + 3] = __uint_as_float(u[k + 3]) + bb.w; } }
@@ -678,13 +556,13 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
       for (int cb = grp; cb < 2; cb += ngrp) {
         const int ch = ch0 + cb * 32;
         auto load = [&](float (&v)[32], int tcol) {
-          uint32_t u[32]; tmem_ld32(tacc + (uint32_t)tcol, u); tmem_ld_wait();
+          uint32_t u[32]; acc_ld32<BN>(acc, arow, tcol, u);
 #pragma unroll
           for (int k = 0; k < 32; k += 4) { float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + tcol + k);
             v[k] = __uint_as_float(u[k]) + bb.x; v[k + 1] = __uint_as_float(u[k + 1]) + bb.y; v[k + 2] = __uint_as_float(u[k + 2]) + bb.z; v[k + 3] = __uint_as_float(u[k + 3]) + bb.w; }
         };
         float mean_a, rstd_a, mean_g, rstd_g;
-        {                                                  // gate branch first: statistics only, the values are re-read from TMEM below
+        {                                                  // gate branch first: statistics only, the values are re-read from the tile below
           float g0[32], g1[32];
           load(g0, 128 + cb * 32); load(g1, 192 + cb * 32);
           if (p.dst) { hwrite_rows_f32(stg, g0, rowp, p.Cc + ch, lane); hwrite_rows_f32(stg, g1, rowp, p.Cc + Ch + ch, lane); }
@@ -727,7 +605,7 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
         float4 rpre[8];
         rows_fetch(rpre, p.resid, p.C_out, mq, M, ch, lane);
         float va[32];
-        { uint32_t u[32]; tmem_ld32(tacc + (uint32_t)(cb * 32), u); tmem_ld_wait();
+        { uint32_t u[32]; acc_ld32<BN>(acc, arow, (cb * 32), u);
 #pragma unroll
           for (int k = 0; k < 32; k += 4) { float4 bb = *reinterpret_cast<const float4*>(p.bias + ch + k);
             va[k] = __uint_as_float(u[k]) + bb.x; va[k + 1] = __uint_as_float(u[k + 1]) + bb.y; va[k + 2] = __uint_as_float(u[k + 2]) + bb.z; va[k + 3] = __uint_as_float(u[k + 3]) + bb.w; } }
@@ -763,7 +641,7 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
         const int ch = n0 + cb * 32;
         if (ch >= p.N) break;
         float dy[32], xa[32];
-        { uint32_t u[32]; tmem_ld32(tacc + (uint32_t)(cb * 32), u); tmem_ld_wait();
+        { uint32_t u[32]; acc_ld32<BN>(acc, arow, (cb * 32), u);
 #pragma unroll
           for (int k = 0; k < 32; ++k) dy[k] = __uint_as_float(u[k]); }
         if (p.accumulate) {
@@ -872,27 +750,106 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
   }
 }
 
+// ------------------------------------------------------------------------------------------------ consumer K loop
+// MMAs of one pipeline stage.  The kind is a template argument, so that no wgmma sits under a runtime branch (which makes ptxas
+// serialise the asynchronous MMAs): F16F8 walks its two passes as two calls.
+enum { MMA_BF16 = 0, MMA_BF16X3 = 1, MMA_E4M3_CROSS = 2, MMA_F16 = 3, MMA_F16_CROSS = 4 };
+
+// One consumer warpgroup walks nkb pipeline stages: wait for the stage, issue its MMAs, release the previous stage once those have
+// completed.  TN = 0: both operands K-major, 128-byte rows (forward / data gradient); TN = 1: both MN-major, 64-element atoms at
+// 8192 B (weight gradient).  The warpgroup's A rows (NT) / channels (TN) start at wg * 8192.
+template <int BN, int KIND, int TN, class Cfg>
+__device__ __forceinline__ void consume_stages(float (&d)[BN / 2], int nkb, int& stage, uint32_t& phase, int& prev,
+                                               uint64_t* full_bar, uint64_t* empty_bar, uint32_t smem_base, int wg, int lane) {
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    fence_proxy_async();                                     // producers' generic-proxy writes (cp.async, st.shared) -> wgmma reads
+    const uint32_t sA = smem_base + stage * Cfg::STAGE + wg * 8192;
+    const uint32_t sB = smem_base + stage * Cfg::STAGE + Cfg::PLANES * Cfg::A_PLANE;
+    fence_acc(d);
+    wgmma_fence();
+    if constexpr (TN == 0) {
+      if constexpr (KIND == MMA_E4M3_CROSS) {                // K = 32 e4m3 per instruction: a8_hi x b8_lo + a8_lo x b8_hi
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_e4m3<BN>(d, make_desc(sA + k * 32, 16, 1024), make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024), 1);
+          wgmma_e4m3<BN>(d, make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024), make_desc(sB + k * 32, 16, 1024), 1);
+        }
+      } else if constexpr (KIND == MMA_F16) {                // fp16 hi x hi, two 64-channel tiles of K = 16 steps
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma_f16<BN, 0, 0>(d, make_desc(sA + h * Cfg::A_PLANE + k * 32, 16, 1024), make_desc(sB + h * Cfg::B_PLANE + k * 32, 16, 1024), 1);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {                        // K = 16 bf16 = 32 bytes along the swizzled row
+          const uint64_t a_hi = make_desc(sA + k * 32, 16, 1024), b_hi = make_desc(sB + k * 32, 16, 1024);
+          wgmma_bf16<BN, 0, 0>(d, a_hi, b_hi, 1);
+          if constexpr (KIND == MMA_BF16X3) {
+            const uint64_t a_lo = make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024), b_lo = make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024);
+            wgmma_bf16<BN, 0, 0>(d, a_hi, b_lo, 1);
+            wgmma_bf16<BN, 0, 0>(d, a_lo, b_hi, 1);
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {                          // K = 16 K-rows = two 8-row groups = 2048 bytes
+        const uint64_t a0 = make_desc(sA + k * 2048, 8192, 1024), b0 = make_desc(sB + k * 2048, 8192, 1024);
+        const uint64_t a1 = make_desc(sA + Cfg::A_PLANE + k * 2048, 8192, 1024), b1 = make_desc(sB + Cfg::B_PLANE + k * 2048, 8192, 1024);
+        if constexpr (KIND == MMA_F16_CROSS) {               // the widened e4m3 planes: x8hi x g8lo + x8lo x g8hi
+          wgmma_f16<BN, 1, 1>(d, a0, b1, 1);
+          wgmma_f16<BN, 1, 1>(d, a1, b0, 1);
+        } else if constexpr (KIND == MMA_F16) {
+          wgmma_f16<BN, 1, 1>(d, a0, b0, 1);
+        } else {
+          wgmma_bf16<BN, 1, 1>(d, a0, b0, 1);
+          if constexpr (KIND == MMA_BF16X3) {
+            wgmma_bf16<BN, 1, 1>(d, a0, b1, 1);
+            wgmma_bf16<BN, 1, 1>(d, a1, b0, 1);
+          }
+        }
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                                         // the previous stage's MMAs have completed: release it
+    fence_acc(d);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+  }
+}
+// all MMAs issued so far complete, then D *= scale (folds the common power of two of the F16F8 cross products out of D)
+template <int N>
+__device__ __forceinline__ void rescale_acc(float (&d)[N], float scale) {
+  wgmma_wait<0>();
+  fence_acc(d);
+#pragma unroll
+  for (int i = 0; i < N; ++i) d[i] *= scale;
+}
+
 // ------------------------------------------------------------------------------------------------ NT kernel
 // Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... (m fastest, so CTAs that run
-// concurrently share the weight tile in L2).  288 threads:
-//   warps 0-3  producers (A rows by cp.async, weight tile by TMA), running ahead across tile boundaries
-//   warp  4    TMEM allocation + single-thread tcgen05.mma issue; accumulators are double-buffered in TMEM
-//              (2 x BN columns) so the MMAs of tile i+1 overlap the epilogue of tile i
-//   warps 5-8  epilogue: tcgen05.ld -> +bias / accumulate -> fp32 stores, then release the accumulator stage
-constexpr int kNTThreads = 288;
+// concurrently share the weight tile in L2).  384 threads:
+//   warps 0-3   producers (A rows by cp.async, weight tile by TMA), running ahead across K-blocks
+//   warps 4-11  two consumer warpgroups: wgmma of tile rows 64 wg .. + 63 into registers (BN / 2 per thread); then the whole tile
+//               is written to shared memory over the pipeline stages -- they hold nothing at that point, because the producers
+//               wait for the epilogue of a tile before they load the next one -- and the 8 warps run the epilogue in two groups
+//               of 4.  (The accumulator of a 256-wide tile does not fit next to the stages: 128 KB.)
+constexpr int kNTThreads = 384;
 
 template <int BN, int NPL, int EPI>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   using Cfg = NTCfg<BN, NPL>;
-  __shared__ float epi_xch[4][32];                           // cross-warp exchange of the fused epilogue
-  __shared__ __align__(16) float epi_bc[4][(EPI == 3 || EPI == 4) ? 384 : 128];   // per-warp broadcast of per-column coefficients (32 floats per quantity)
-  __shared__ __align__(16) float epi_stage[4][32 * 16];      // per-warp half-width transposition patch of the coalesced row stores
-  __shared__ float* epi_rowp[4][32];                         // destination row of every tile row
+  __shared__ float epi_xch[2][4][32];                        // cross-warp exchange of the fused epilogue, per group
+  __shared__ __align__(16) float epi_bc[8][(EPI == 3 || EPI == 4) ? 384 : 128];   // per-warp broadcast of per-column coefficients (32 floats per quantity)
+  __shared__ __align__(16) float epi_stage[8][32 * 16];      // per-warp half-width transposition patch of the coalesced row stores
+  __shared__ float* epi_rowp[8][32];                         // destination row of every tile row
   constexpr int S = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S], acc_free_bar;
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -900,7 +857,7 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   const long long M = (long long)g.B * g.Hy * g.Wx;
   const int HW = g.Hy * g.Wx;
   // K blocks ("stages"): 64 channels each; F16F8 walks the contraction twice with 128 channels per stage -- first the two
-  // fp8 cross products (planes a8_hi x b8_lo and a8_lo x b8_hi), then the fp16 hi x hi product whose first MMA rescales D
+  // fp8 cross products (planes a8_hi x b8_lo and a8_lo x b8_hi), then the fp16 hi x hi product after the rescale of D
   const int cchunks = NPL == 3 ? (p.C >> 7) : (p.C >> 6);
   const int kb_pass = g.ntaps * cchunks;
   const int num_kb = NPL == 3 ? 2 * kb_pass : kb_pass;     // > 0 (the host never launches an empty contraction)
@@ -909,28 +866,27 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   const int num_tiles = m_tiles * n_tiles;
 
   if (threadIdx.x == 0) {
-    // full: 128 cp.async arrivals (A rows) + 1 arrive.expect_tx whose bytes the weight-tile TMA completes
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], kProducerThreads + 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 4); }
+    // full: 128 cp.async arrivals (A rows) + 1 arrive.expect_tx whose bytes the weight-tile TMA completes; empty / acc_free: one
+    // arrival per consumer warp
+    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], kProducerThreads + 1); mbar_init(&empty_bar[s], 8); }
+    mbar_init(&acc_free_bar, 8);
     fence_barrier_init();
     tma_prefetch_desc(&p.tm_b_hi);
     if (NPL == 2) tma_prefetch_desc(&p.tm_b_lo);
     if (NPL == 3) { tma_prefetch_desc(&p.tm_b8_hi); tma_prefetch_desc(&p.tm_b8_lo); }
   }
-  if (warp == 4) tmem_alloc<2 * BN>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
   if (warp < 4) {
     // ===================== producers =====================
     const int t = threadIdx.x;
     const int chunk = t & 7, rsub = t >> 3;                 // 8 threads cover one 128-byte row; 16 rows per pass
     int stage = 0; uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const long long m0 = (long long)(tile % m_tiles) * 128;
       const int n0 = (tile / m_tiles) * BN;
+      if (it > 0) mbar_wait(&acc_free_bar, (uint32_t)(it - 1) & 1u);   // the previous tile's epilogue has left the stages
       int rb[8], ry[8], rx[8];                              // decoded output coordinates of this thread's 8 A rows
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -996,308 +952,70 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
         }
       }
     }
-  } else if (warp == 4) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc(128, BN, 0, 0);
-    int stage = 0; uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(&tmem_empty_bar[as], aphase ^ 1);            // epilogue has drained this accumulator stage
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        fence_proxy_async();
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sA = smem_base + stage * Cfg::STAGE;
-          const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
-          if (NPL == 3) {
-            constexpr uint32_t idq = make_idesc_f0(128, BN);
-            if (kb < kb_pass) {                              // fp8 cross products, K = 32 per instruction: a8_hi x b8_lo + a8_lo x b8_hi
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                umma_f8(tmem_d, make_desc(sA + k * 32, 16, 1024), make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024), idq, (kb | k) != 0);
-                umma_f8(tmem_d, make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024), make_desc(sB + k * 32, 16, 1024), idq, 1);
-              }
-            } else {                                         // fp16 hi x hi, two 64-channel tiles of K = 16 steps
-#pragma unroll
-              for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const uint64_t a = make_desc(sA + h * Cfg::A_PLANE + k * 32, 16, 1024), b = make_desc(sB + h * Cfg::B_PLANE + k * 32, 16, 1024);
-                  if (kb == kb_pass && h == 0 && k == 0) umma_f16_rescale(tmem_d, a, b, idq);     // D = A*B + D * 2^-15
-                  else umma_bf16(tmem_d, a, b, idq, 1);
-                }
-            }
-          } else {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {                      // UMMA_K = 16 bf16 = 32 bytes along the swizzled row
-            const uint64_t a_hi = make_desc(sA + k * 32, 16, 1024);
-            const uint64_t b_hi = make_desc(sB + k * 32, 16, 1024);
-            umma_bf16(tmem_d, a_hi, b_hi, idesc, (kb | k) != 0);
-            if (NPL == 2) {
-              const uint64_t a_lo = make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024);
-              const uint64_t b_lo = make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024);
-              umma_bf16(tmem_d, a_hi, b_lo, idesc, 1);
-              umma_bf16(tmem_d, a_lo, b_hi, idesc, 1);
-            }
-          }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit(&tmem_full_bar[as]);
-        }
-        __syncwarp();
-        if (++stage == S) { stage = 0; phase ^= 1; }
-      }
-    }
   } else {
-    // ===================== epilogue (warps 5..8) =====================
-    const int q = warp & 3;                                  // TMEM lane quarter this warp may access
-    float* stg = epi_stage[q];                               // this warp's 32 x 32-word transposition patch
-    float** rowp = epi_rowp[q];
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
+    // ===================== consumers: MMA, then epilogue =====================
+    const int cw = warp - 4;                                 // consumer warp 0..7
+    const int wg = cw >> 2;                                  // warpgroup: tile rows 64 wg .. + 63
+    const int tw = threadIdx.x - 128 * (wg + 1);             // thread within the warpgroup
+    float* acc_s = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const long long m0 = (long long)(tile % m_tiles) * 128;
       const int n0 = (tile / m_tiles) * BN;
-      nt_tile_epilogue<BN, NPL, EPI>(p, M, HW, m0, n0, q, lane, stg, rowp, epi_bc[q], epi_xch, &tmem_full_bar[as], aphase,
-                                     tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN));
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty_bar[as])) : "memory");
+      float d[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      int prev = -1;                                         // stage whose MMAs may still be in flight
+      if constexpr (NPL == 3) {                             // e4m3 cross products, then the fp16 hi x hi products after the rescale of D
+        consume_stages<BN, MMA_E4M3_CROSS, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+        rescale_acc(d, 1.f / (float)(1 << CGVC_Q_ACC_SHIFT));
+        consume_stages<BN, MMA_F16, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+      } else {
+        consume_stages<BN, NPL == 2 ? MMA_BF16X3 : MMA_BF16, 0, Cfg>(d, num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
       }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc<2 * BN>(tmem_base);
-}
-
-// ------------------------------------------------------------------------------------------------ CTA-pair NT kernel
-// The same contraction on CTA pairs (cluster of 2, tcgen05 cta_group::2): one 256 x BN tile per pair.  CTA r of a pair owns rows
-// m0 + 128 r .. + 127 -- its own gathered-operand tile and its own 128 accumulator lanes, so every epilogue is per CTA and identical
-// to the one-CTA kernel's -- and loads only rows n0 + r BN/2 .. of the weight tile; the leader issues M = 256 MMAs that read both
-// CTAs' shared memory.  Each SM therefore pulls (128 + BN/2) instead of (128 + BN) operand rows per K-block from L2: a third fewer
-// bytes at BN = 256, which is what bounds the one-CTA kernel (DESIGN.md section 7).  The gathered operand is no longer gathered by
-// threads: one TMA im2col load per (tap, 64-channel block, plane) delivers the 128 rows, zero-filled at the TF-SAME borders and
-// across sample boundaries (im2col_map.h), so a CTA is: producer warp (one lane), MMA issuer warp, and -- the thread budget the
-// gather used to take -- 8 epilogue warps in two groups of 4 (one warp per TMEM lane quarter and group; group g takes the 32-column
-// chunks g, g + 2, ... of a tile): with one warp per scheduler the long dependent chains of the fused instance-norm epilogues had
-// no other warp to hide their latency behind.  The fused-backward epilogues (EPI 3, 4) keep one group (their coefficient tables
-// would not fit twice into what 3 x 64 KB of pipeline stages leave of the shared memory).
-constexpr int kPairThreads = 192;       // weight-gradient pair kernels: producer, MMA issuer, 4 epilogue warps
-constexpr int kPairNTThreads = 320;     // forward / data-gradient pair kernel: producer, MMA issuer, 8 epilogue warps
-
-template <int BN, int NPL>
-struct PairCfg {
-  static constexpr int A_PLANE = 128 * 128;
-  static constexpr int B_PLANE = (BN / 2) * 128;
-  static constexpr int PLANES = NPL == 1 ? 1 : 2;          // F16F8 (NPL = 3) stages hold two 128-byte-row tiles per operand as well
-  static constexpr int STAGE = PLANES * (A_PLANE + B_PLANE);
-  static constexpr int STAGES_RAW = (196 * 1024) / STAGE;  // 3 (BN=256,x3), 4 (128,x3), 6 (256,x1), 8 (128,x1)
-  static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int SMEM = STAGES * STAGE + 1024;
-};
-
-template <int BN, int NPL, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kPairNTThreads, 1)
-tc_pair_nt_kernel(const __grid_constant__ TcNTParams p) {
-  using Cfg = PairCfg<BN, NPL>;
-  constexpr int S = Cfg::STAGES;
-  constexpr bool kBwdEpi = EPI == 3 || EPI == 4;             // the fused backward epilogues need 1.5 KB of coefficients per warp: one group
-  constexpr int NG = kBwdEpi ? 1 : 2;                        // epilogue warp groups
-  __shared__ float epi_xch[NG][4][32];
-  __shared__ __align__(16) float epi_bc[4 * NG][kBwdEpi ? 384 : 128];
-  __shared__ __align__(16) float epi_stage[4 * NG][32 * 16];
-  __shared__ float* epi_rowp[4 * NG][32];
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
-
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const GatherGeom& g = p.g;
-  const long long M = (long long)g.B * g.Hy * g.Wx;
-  const int HW = g.Hy * g.Wx;
-  // K blocks: 64 channels each; F16F8 (NPL = 3) walks the contraction twice with 128 channels per stage -- first the two e4m3 cross
-  // products, then the fp16 hi x hi product whose first MMA rescales the accumulator (same scheme as the one-CTA kernel)
-  const int cchunks = NPL == 3 ? (p.C >> 7) : (p.C >> 6);
-  const int kb_pass = g.ntaps * cchunks;
-  const int num_kb = NPL == 3 ? 2 * kb_pass : kb_pass;
-  const int m_tiles = (int)((M + 127) / 128);
-  const int m_pairs = (m_tiles + 1) >> 1;
-  const int num_tiles = m_pairs * p.n_tiles;
-
-  if (threadIdx.x == 0) {
-    // full (leader's is used): one arrive.expect_tx by the leader's producer, completed by the TMA bytes of BOTH CTAs;
-    // empty / tmem_full: one multicast commit; tmem_empty (leader's is used): the 4 * NG epilogue warps of both CTAs
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 8 * NG); }
-    fence_barrier_init();
-    tma_prefetch_desc(&p.tm_a_hi); tma_prefetch_desc(&p.tm_b2_hi);
-    if (NPL == 2) { tma_prefetch_desc(&p.tm_a_lo); tma_prefetch_desc(&p.tm_b2_lo); }
-    if (NPL == 3) { tma_prefetch_desc(&p.tm_a8_hi); tma_prefetch_desc(&p.tm_a8_lo); tma_prefetch_desc(&p.tm_b28_hi); tma_prefetch_desc(&p.tm_b28_lo); }
-  }
-  if (warp == 1) tmem_alloc2<2 * BN>(&tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                        // both CTAs' barriers exist before anyone signals the peer
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-
-  if (warp == 0) {
-    // ===================== producer (one lane) =====================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += npairs) {
-        const long long m0 = ((long long)(tile % m_pairs) * 2 + rank) * 128;
-        const int n0 = (tile / m_pairs) * BN + (int)rank * (BN / 2);
-        // base pixel of the tile's first row (rows beyond the tensor: sample index >= B, the unit fills zeros)
-        const int b = (int)(m0 / HW); const int rem = (int)(m0 - (long long)b * HW);
-        const int y = rem / g.Wx, x = rem - y * g.Wx;
-        const int cw = p.ig.lo_w + x * g.sx, ch = p.ig.lo_h + y * g.sy;
-        for (int pass = 0; pass < (NPL == 3 ? 2 : 1); ++pass)
-        for (int tap = 0; tap < g.ntaps; ++tap) {
-          const unsigned short ow = p.ig.off_w[tap], oh = p.ig.off_h[tap];
-          const int wslab = g.widx[tap];
-          for (int cc = 0; cc < cchunks; ++cc) {
-            const int c0 = NPL == 3 ? (cc << 7) : (cc << 6);
-            mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-            const uint32_t sA = smem_base + stage * Cfg::STAGE;
-            const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::STAGE);
-            if (NPL == 3) {
-              if (pass == 0) {                               // 128 e4m3 channels per line and plane
-                tma2_im2col(sA, &p.tm_a8_hi, c0, cw, ch, b, ow, oh, &full_bar[stage]);
-                tma2_im2col(sA + Cfg::A_PLANE, &p.tm_a8_lo, c0, cw, ch, b, ow, oh, &full_bar[stage]);
-                tma2_load3(sB, &p.tm_b28_hi, c0, n0, wslab, &full_bar[stage]);
-                tma2_load3(sB + Cfg::B_PLANE, &p.tm_b28_lo, c0, n0, wslab, &full_bar[stage]);
-              } else {                                       // fp16: two 64-channel tiles
-                tma2_im2col(sA, &p.tm_a_hi, c0, cw, ch, b, ow, oh, &full_bar[stage]);
-                tma2_im2col(sA + Cfg::A_PLANE, &p.tm_a_hi, c0 + 64, cw, ch, b, ow, oh, &full_bar[stage]);
-                tma2_load3(sB, &p.tm_b2_hi, c0, n0, wslab, &full_bar[stage]);
-                tma2_load3(sB + Cfg::B_PLANE, &p.tm_b2_hi, c0 + 64, n0, wslab, &full_bar[stage]);
-              }
-            } else {
-              tma2_im2col(sA, &p.tm_a_hi, c0, cw, ch, b, ow, oh, &full_bar[stage]);
-              if (NPL == 2) tma2_im2col(sA + Cfg::A_PLANE, &p.tm_a_lo, c0, cw, ch, b, ow, oh, &full_bar[stage]);
-              tma2_load3(sB, &p.tm_b2_hi, c0, n0, wslab, &full_bar[stage]);
-              if (NPL == 2) tma2_load3(sB + Cfg::B_PLANE, &p.tm_b2_lo, c0, n0, wslab, &full_bar[stage]);
-            }
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
+      wgmma_wait<0>();
+      fence_acc(d);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      // the tile into shared memory once both warpgroups are done reading the stages
+      consumer_bar();
+      if (!(p.debug & 2)) {
+        const int r0 = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2), c0 = 2 * (tw & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(acc_s + acc_off<BN>(r0, 8 * j + c0)) = make_float2(d[4 * j], d[4 * j + 1]);
+          *reinterpret_cast<float2*>(acc_s + acc_off<BN>(r0 + 8, 8 * j + c0)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
         }
       }
-      // tail: every stage this CTA filled has been released (the leader's multicast commits have all landed here) before it may exit
-      for (int s = 0; s < S; ++s) {
-        mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-        if (++stage == S) { stage = 0; phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA) =====================
-    if (rank == 0) {
-      constexpr uint32_t idesc = make_idesc(256, BN, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int tile = pair; tile < num_tiles; tile += npairs, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-        mbar_wait_bounded(&tmem_empty_bar[as], aphase ^ 1);  // both CTAs' epilogues have drained this accumulator stage
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait_bounded(&full_bar[stage], phase);
-          tc_fence_after();
-          if (lane == 0) {
-            const uint32_t sA = smem_base + stage * Cfg::STAGE;
-            const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
-            if (NPL == 3) {
-              constexpr uint32_t idq = make_idesc_f0(256, BN);
-              if (kb < kb_pass) {                            // e4m3 cross products, K = 32 per instruction: a8_hi x b8_lo + a8_lo x b8_hi
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  umma2_f8(tmem_d, make_desc(sA + k * 32, 16, 1024), make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024), idq, (kb | k) != 0);
-                  umma2_f8(tmem_d, make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024), make_desc(sB + k * 32, 16, 1024), idq, 1);
-                }
-              } else {                                       // fp16 hi x hi, two 64-channel tiles of K = 16 steps
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {
-                    const uint64_t a = make_desc(sA + h * Cfg::A_PLANE + k * 32, 16, 1024), b = make_desc(sB + h * Cfg::B_PLANE + k * 32, 16, 1024);
-                    if (kb == kb_pass && h == 0 && k == 0) umma2_f16_rescale<CGVC_Q_ACC_SHIFT>(tmem_d, a, b, idq);   // D = A*B + D * 2^-15
-                    else umma2_bf16(tmem_d, a, b, idq, 1);
-                  }
-              }
-            } else {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t a_hi = make_desc(sA + k * 32, 16, 1024);
-              const uint64_t b_hi = make_desc(sB + k * 32, 16, 1024);
-              umma2_bf16(tmem_d, a_hi, b_hi, idesc, (kb | k) != 0);
-              if (NPL == 2) {
-                const uint64_t a_lo = make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024);
-                const uint64_t b_lo = make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024);
-                umma2_bf16(tmem_d, a_hi, b_lo, idesc, 1);
-                umma2_bf16(tmem_d, a_lo, b_hi, idesc, 1);
-              }
-            }
-            }
-            umma2_commit_mc(&empty_bar[stage]);
-            if (kb == num_kb - 1) umma2_commit_mc(&tmem_full_bar[as]);
-          }
-          __syncwarp();
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if ((warp - 2) < 4 * NG) {
-    // ===================== epilogue (warps 2..9 in two groups; 2..5 for the fused-backward forms), this CTA's 128 rows ==========
-    const int q = warp & 3;                                  // TMEM lane quarter this warp may access
-    const int grp = (warp - 2) >> 2, ew = 4 * grp + q;       // warp group and slot of this warp's patch / tables
-    int it = 0;
-    for (int tile = pair; tile < num_tiles; tile += npairs, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-      const long long m0 = ((long long)(tile % m_pairs) * 2 + rank) * 128;
-      const int n0 = (tile / m_pairs) * BN;
-      nt_tile_epilogue<BN, NPL, EPI>(p, M, HW, m0, n0, q, lane, epi_stage[ew], epi_rowp[ew], epi_bc[ew], epi_xch[grp], &tmem_full_bar[as], aphase,
-                                     tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN), grp, NG);
-      tc_fence_before();
+      consumer_bar();
+      nt_tile_epilogue<BN, NPL, EPI>(p, M, HW, m0, n0, cw & 3, lane, epi_stage[cw], epi_rowp[cw], epi_bc[cw], epi_xch[wg], acc_s, wg, 2);
+      fence_proxy_async();                                   // generic accesses of the stages before the next tile's TMA writes
       __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tmem_empty_bar[as], 0);
+      if (lane == 0) mbar_arrive(&acc_free_bar);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                        // the peer may still be reading its accumulator half / shared memory
-  if (warp == 1) tmem_dealloc2<2 * BN>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------ TN kernel (wgrad)
 // Tile: 128 channels (GEMM M, operand A = X, MN-major) x 256 gradient columns (GEMM N, operand B = G, MN-major);
-// the contraction runs over rows m of the forward output grid, 64 rows per stage.
+// the contraction runs over rows m of the forward output grid, 64 rows per stage.  NPL 1 / 2: the bf16 planes (hi | hi + lo).
+// NPL 3 (CGVC_PREC_F16F8): X and G are kept as fp16 + two scaled e4m3 planes, both with the activation-role scales (1, 2^12), so
+// both cross products x8hi * g8lo and x8lo * g8hi carry 2^12.  Unless p.w16 is set, the row range of a work item is walked twice:
+// first the cross products -- e4m3 wgmma reads K-major operands only, and both operands are MN-major here, so the producers widen
+// the e4m3 tiles to fp16 (exactly) on their way into shared memory and the products run as fp16 MMAs --, then the accumulator is
+// rescaled by 2^-12 and the fp16 hi x hi products follow.
+#define CGVC_Q_WGRAD_SHIFT 12
 template <int NPL>
 struct TNCfg {
   static constexpr int A_PLANE = 64 * 256;              // 64 K-rows x 128 channels x 2 B  (2 MN-atoms side by side: LBO = 8192)
   static constexpr int B_PLANE = 64 * 512;              // 64 K-rows x 256 columns x 2 B  (4 MN-atoms: LBO = 8192)
-  static constexpr int STAGE = NPL * (A_PLANE + B_PLANE);
-  static constexpr int STAGES = (200 * 1024) / STAGE;   // 2 (x3), 4 (x1)
+  static constexpr int PLANES = NPL == 1 ? 1 : 2;
+  static constexpr int STAGE = PLANES * (A_PLANE + B_PLANE);
+  static constexpr int STAGES = (192 * 1024) / STAGE;   // 2 (x3, f16f8), 4 (x1)
   static constexpr int SMEM = STAGES * STAGE + 1024;
 };
 
 // Persistent like the NT kernel: work items (n-tile, c-tile, tap, K-split) are walked with stride gridDim.x (n fastest, so
-// concurrently running CTAs share the same rows of X and dP in L2); the accumulator is double-buffered in TMEM so the
-// red.global epilogue of item i overlaps the MMAs of item i+1.
+// concurrently running CTAs share the same rows of X and dP in L2).  Each consumer warpgroup owns 64 of the 128 channels.
 template <int NPL>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
@@ -1305,9 +1023,7 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   constexpr int S = Cfg::STAGES;
   constexpr int BN = 256;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(16) float epi_stage[4][32 * 32];      // per-warp transposition patch of the coalesced row stores
-  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S];
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1316,6 +1032,7 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   const int HW = g.Hy * g.Wx;
   const int n_tiles = (p.g_ld + BN - 1) / BN, c_tiles = (p.x_ld + 127) / 128;
   const int num_items = n_tiles * c_tiles * g.ntaps * p.ksplit;
+  const int pass0 = (NPL == 3 && !p.w16) ? 0 : 1;         // pass 0: the F16F8 cross products; pass 1: the main products
   long long chunk_rows = (M + p.ksplit - 1) / p.ksplit;
   chunk_rows = (chunk_rows + 63) / 64 * 64;
 
@@ -1333,17 +1050,12 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], kProducerThreads + 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 4); }
+    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], kProducerThreads + 1); mbar_init(&empty_bar[s], 8); }
     fence_barrier_init();
     tma_prefetch_desc(&p.tm_g_hi);
     if (NPL == 2) tma_prefetch_desc(&p.tm_g_lo);
   }
-  if (warp == 4) tmem_alloc<2 * BN>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
   if (warp < 4) {
     // ---- producers: every K-row (one output position m) is a contiguous run of channels / columns in global memory
@@ -1352,530 +1064,125 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
     int stage = 0; uint32_t phase = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       const Item w = decode(item);
+      for (int pass = pass0; pass < 2; ++pass)
       for (int kb = 0; kb < w.num_kb; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         const uint32_t sA = smem_base + stage * Cfg::STAGE;
-        const uint32_t sB = sA + NPL * Cfg::A_PLANE;
-        if (t == 0) {
-          // gradient tile: 64 K-rows x 256 columns = 4 MN-atoms of [64 rows][64 cols]; rows >= M are zero-filled by TMA
-          // (a stage never straddles two K-splits: split boundaries are multiples of 64 rows)
-          const int row0 = (int)(w.mbeg + (long long)kb * 64);
-          int natoms = 0;
-#pragma unroll
-          for (int a = 0; a < 4; ++a) natoms += (w.n0 + a * 64) < p.g_ld ? 1 : 0;
-          mbar_expect_tx(&full_bar[stage], NPL * natoms * 8192);
-#pragma unroll
-          for (int a = 0; a < 4; ++a) {
-            if ((w.n0 + a * 64) < p.g_ld) {
-              tma_load3(sB + a * 8192, &p.tm_g_hi, w.n0 + a * 64, row0, 0, &full_bar[stage]);
-              if (NPL == 2) tma_load3(sB + Cfg::B_PLANE + a * 8192, &p.tm_g_lo, w.n0 + a * 64, row0, 0, &full_bar[stage]);
-            }
-          }
-        }
+        const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
+        long long xoff[4];                                   // source row of each of this thread's 4 K-rows (-1: zero row)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const int kr = rsub + 16 * i;                       // K-row within the stage (0..63)
-          const long long m = w.mbeg + (long long)kb * 64 + kr;
-          long long xoff = -1;
+          const long long m = w.mbeg + (long long)kb * 64 + rsub + 16 * i;
+          xoff[i] = -1;
           if (m < w.mend) {
             const uint32_t mu = (uint32_t)m;
             int b = (int)fdiv(mu, p.div_hw); int rem = (int)(mu - (uint32_t)b * (uint32_t)HW);
             int y = (int)fdiv((uint32_t)rem, p.div_w); int x = rem - y * g.Wx;
             int yy = y * g.sy + g.oy[w.tap], xx = x * g.sx + g.ox[w.tap];
             if (yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws)
-              xoff = ((long long)(b * g.Hs + yy) * g.Ws + xx) * p.x_ld + w.c0 + chunk * 8;
-          }
-          const uint32_t so = sw128(kr, chunk);               // (kr/8)*1024 + (kr%8)*128 + swizzled chunk
-#pragma unroll
-          for (int a = 0; a < 2; ++a) {                       // 2 channel atoms of 64
-            const bool ok = xoff >= 0 && (w.c0 + a * 64) < p.x_ld;
-            const long long off = ok ? xoff + a * 64 : 0;
-            cp_async16(sA + a * 8192 + so, p.x_hi + off, ok ? 16u : 0u);
-            if (NPL == 2) cp_async16(sA + Cfg::A_PLANE + a * 8192 + so, p.x_lo + off, ok ? 16u : 0u);
+              xoff[i] = ((long long)(b * g.Hs + yy) * g.Ws + xx) * p.x_ld + w.c0 + chunk * 8;
           }
         }
-        cp_async_arrive_noinc(&full_bar[stage]);
+        if (NPL == 3 && pass == 0) {
+          // e4m3 planes, widened to fp16 here: plane 0 = hi, plane 1 = lo, for both operands
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int kr = rsub + 16 * i;
+            const uint32_t so = sw128(kr, chunk);
+#pragma unroll
+            for (int a = 0; a < 2; ++a) {                     // 2 channel atoms of 64
+              const bool ok = xoff[i] >= 0 && (w.c0 + a * 64) < p.x_ld;
+              uint2 vh = make_uint2(0u, 0u), vl = make_uint2(0u, 0u);
+              if (ok) { vh = __ldg(reinterpret_cast<const uint2*>(p.x8_hi + xoff[i] + a * 64)); vl = __ldg(reinterpret_cast<const uint2*>(p.x8_lo + xoff[i] + a * 64)); }
+              st_shared16(sA + a * 8192 + so, e4m3x8_to_f16x8(vh));
+              st_shared16(sA + Cfg::A_PLANE + a * 8192 + so, e4m3x8_to_f16x8(vl));
+            }
+            const long long m = w.mbeg + (long long)kb * 64 + kr;
+#pragma unroll
+            for (int a = 0; a < 4; ++a) {                     // 4 gradient-column atoms of 64
+              const int col = w.n0 + a * 64 + chunk * 8;
+              const bool ok = m < w.mend && col < p.g_ld;
+              uint2 vh = make_uint2(0u, 0u), vl = make_uint2(0u, 0u);
+              if (ok) { vh = __ldg(reinterpret_cast<const uint2*>(p.g8_hi + m * p.g_ld + col)); vl = __ldg(reinterpret_cast<const uint2*>(p.g8_lo + m * p.g_ld + col)); }
+              st_shared16(sB + a * 8192 + so, e4m3x8_to_f16x8(vh));
+              st_shared16(sB + Cfg::B_PLANE + a * 8192 + so, e4m3x8_to_f16x8(vl));
+            }
+          }
+          fence_proxy_async();                               // generic stores -> visible to the tensor cores' reads
+          if (t == 0) mbar_expect_tx(&full_bar[stage], 0);   // (the arrival the TMA thread makes in the other pass)
+          mbar_arrive(&full_bar[stage]);
+        } else {
+          if (t == 0) {
+            // gradient tile: 64 K-rows x 256 columns = 4 MN-atoms of [64 rows][64 cols]; rows >= M are zero-filled by TMA
+            // (a stage never straddles two K-splits: split boundaries are multiples of 64 rows)
+            const int row0 = (int)(w.mbeg + (long long)kb * 64);
+            int natoms = 0;
+#pragma unroll
+            for (int a = 0; a < 4; ++a) natoms += (w.n0 + a * 64) < p.g_ld ? 1 : 0;
+            mbar_expect_tx(&full_bar[stage], (NPL == 2 ? 2 : 1) * natoms * 8192);
+#pragma unroll
+            for (int a = 0; a < 4; ++a) {
+              if ((w.n0 + a * 64) < p.g_ld) {
+                tma_load3(sB + a * 8192, &p.tm_g_hi, w.n0 + a * 64, row0, 0, &full_bar[stage]);
+                if (NPL == 2) tma_load3(sB + Cfg::B_PLANE + a * 8192, &p.tm_g_lo, w.n0 + a * 64, row0, 0, &full_bar[stage]);
+              }
+            }
+          }
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const uint32_t so = sw128(rsub + 16 * i, chunk);   // (kr/8)*1024 + (kr%8)*128 + swizzled chunk
+#pragma unroll
+            for (int a = 0; a < 2; ++a) {                     // 2 channel atoms of 64
+              const bool ok = xoff[i] >= 0 && (w.c0 + a * 64) < p.x_ld;
+              const long long off = ok ? xoff[i] + a * 64 : 0;
+              cp_async16(sA + a * 8192 + so, p.x_hi + off, ok ? 16u : 0u);
+              if (NPL == 2) cp_async16(sA + Cfg::A_PLANE + a * 8192 + so, p.x_lo + off, ok ? 16u : 0u);
+            }
+          }
+          cp_async_arrive_noinc(&full_bar[stage]);
+        }
         if (++stage == S) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 4) {
-    constexpr uint32_t idesc = make_idesc(128, BN, 1, 1);
+  } else {
+    // ---- consumers: MMA, then red.global.add of the fragments into dW (TF layout [t][c][n]); split-K partials meet there
+    const int cw = warp - 4;
+    const int wg = cw >> 2;                                  // warpgroup: channels c0 + 64 wg .. + 63 (MN atom wg of the X tile)
+    const int tw = threadIdx.x - 128 * (wg + 1);
     int stage = 0; uint32_t phase = 0;
-    int it = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       const Item w = decode(item);
       if (w.num_kb == 0) continue;
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-      ++it;
-      mbar_wait(&tmem_empty_bar[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-      for (int kb = 0; kb < w.num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        fence_proxy_async();
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sA = smem_base + stage * Cfg::STAGE;
-          const uint32_t sB = sA + NPL * Cfg::A_PLANE;
+      float d[BN / 2];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {                      // UMMA_K = 16 K-rows = two 8-row groups = 2048 bytes
-            const uint64_t a_hi = make_desc(sA + k * 2048, 8192, 1024);
-            const uint64_t b_hi = make_desc(sB + k * 2048, 8192, 1024);
-            umma_bf16(tmem_d, a_hi, b_hi, idesc, (kb | k) != 0);
-            if (NPL == 2) {
-              const uint64_t a_lo = make_desc(sA + Cfg::A_PLANE + k * 2048, 8192, 1024);
-              const uint64_t b_lo = make_desc(sB + Cfg::B_PLANE + k * 2048, 8192, 1024);
-              umma_bf16(tmem_d, a_hi, b_lo, idesc, 1);
-              umma_bf16(tmem_d, a_lo, b_hi, idesc, 1);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == w.num_kb - 1) umma_commit(&tmem_full_bar[as]);
-        }
-        __syncwarp();
-        if (++stage == S) { stage = 0; phase ^= 1; }
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      int prev = -1;
+      if constexpr (NPL == 3) {                             // (with w16 the cross-product walk is empty and the rescale acts on zeros)
+        consume_stages<BN, MMA_F16_CROSS, 1, Cfg>(d, pass0 == 0 ? w.num_kb : 0, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+        rescale_acc(d, 1.f / (float)(1 << CGVC_Q_WGRAD_SHIFT));
+        consume_stages<BN, MMA_F16, 1, Cfg>(d, w.num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+      } else {
+        consume_stages<BN, NPL == 2 ? MMA_BF16X3 : MMA_BF16, 1, Cfg>(d, w.num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
       }
-    }
-  } else {
-    // ---- epilogue (warps 5..8): atomically accumulate the tile into dW (TF layout [t][c][n]); split-K partials meet there.
-    // Rows (= channels) are written back 8 lanes per row through the transposition patch, like the NT kernel's stores.
-    const int q = warp & 3;
-    float* stg = epi_stage[q];
-    const int sc = lane & 7, sr = lane >> 3;
-    int it = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      const Item w = decode(item);
-      if (w.num_kb == 0) continue;
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-      ++it;
-      mbar_wait(&tmem_full_bar[as], aphase);
-      tc_fence_after();
-      const int cq = w.c0 + q * 32;                           // first channel row of this warp (TMEM lane == channel row)
-#pragma unroll 1
-      for (int cb = 0; cb < BN / 32; ++cb) {
-        const int n = w.n0 + cb * 32;
-        if (n >= p.N) break;
-        float o[32];
-        { uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + cb * 32), v);
-          tmem_ld_wait();
+      wgmma_wait<0>();
+      fence_acc(d);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      const int c = w.c0 + wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2);   // fragment rows c and c + 8
 #pragma unroll
-          for (int k = 0; k < 32; ++k) o[k] = __uint_as_float(v[k]); }
-        stage_rows(stg, o, lane);
-        float* base; int nn; int ncols;
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = w.n0 + 8 * j + 2 * (tw & 3);
+        if (n >= p.N) continue;
+        float* base; int nn; int ncols;                      // (n even and n_split even: a column pair never straddles the split)
         if (n < p.n_split) { base = p.dw_a; nn = n; ncols = p.n_split; } else { base = p.dw_g; nn = n - p.n_split; ncols = p.N - p.n_split; }
-        if (n + 4 * sc < p.N) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = sr + 4 * i;
-            const int c = cq + rr;
-            if (c < p.C) {
-              const float4 val = staged_chunk(stg, rr, sc);
-              float* d = tn_dst(base, g.widx[w.tap], p.C, c, ncols, nn + 4 * sc, p.fold_n);
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(val.x), "f"(val.y), "f"(val.z), "f"(val.w) : "memory");
-            }
-          }
+        for (int h = 0; h < 2; ++h) {
+          if (c + 8 * h >= p.C) continue;
+          float* dst = tn_dst(base, g.widx[w.tap], p.C, c + 8 * h, ncols, nn, p.fold_n);
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[4 * j + 2 * h]), "f"(d[4 * j + 2 * h + 1]) : "memory");
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty_bar[as])) : "memory");
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc<2 * BN>(tmem_base);
-}
-
-// ------------------------------------------------------------------------------------------------ CTA-pair TN kernel
-// Weight gradient on CTA pairs: one 256-channel x 256-column tile per pair and work item.  CTA r owns channels c0 + 128 r .. (its X
-// tile, by two TMA im2col loads of 64 pixels x 64 channels per plane, and its 128 accumulator lanes) and loads gradient columns
-// n0 + 128 r .. (two [64 x 64] boxes per plane); 64 KB instead of 96 KB of operands per SM and K-block.
-template <int NPL>
-struct PairTNCfg {
-  static constexpr int A_PLANE = 64 * 256;              // 64 K-rows x 128 channels x 2 B (2 MN-atoms: LBO = 8192)
-  static constexpr int B_PLANE = 64 * 256;              // 64 K-rows x 128 columns x 2 B
-  static constexpr int STAGE = NPL * (A_PLANE + B_PLANE);
-  static constexpr int STAGES = (196 * 1024) / STAGE;   // 3 (x3), 6 (x1)
-  static constexpr int SMEM = STAGES * STAGE + 1024;
-};
-
-template <int NPL>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kPairThreads, 1)
-tc_pair_tn_kernel(const __grid_constant__ TcTNParams p) {
-  using Cfg = PairTNCfg<NPL>;
-  constexpr int S = Cfg::STAGES;
-  constexpr int BN = 256;
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(16) float epi_stage[4][32 * 32];
-  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
-
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const GatherGeom& g = p.g;
-  const long long M = (long long)g.B * g.Hy * g.Wx;
-  const int HW = g.Hy * g.Wx;
-  const int n_tiles = (p.g_ld + BN - 1) / BN, c_tiles = (p.x_ld + 255) / 256;
-  const int num_items = n_tiles * c_tiles * g.ntaps * p.ksplit;
-  long long chunk_rows = (M + p.ksplit - 1) / p.ksplit;
-  chunk_rows = (chunk_rows + 63) / 64 * 64;
-
-  struct Item { int n0, c0, tap; long long mbeg, mend; int num_kb; };
-  auto decode = [&](int item) -> Item {
-    Item w;
-    int n_t = item % n_tiles; int t1 = item / n_tiles;
-    int c_t = t1 % c_tiles; int t2 = t1 / c_tiles;
-    w.tap = t2 % g.ntaps; int ks = t2 / g.ntaps;
-    w.n0 = n_t * BN; w.c0 = c_t * 256;
-    w.mbeg = (long long)ks * chunk_rows;
-    w.mend = (w.mbeg + chunk_rows < M) ? w.mbeg + chunk_rows : M;
-    w.num_kb = w.mend > w.mbeg ? (int)((w.mend - w.mbeg + 63) / 64) : 0;
-    return w;
-  };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 8); }
-    fence_barrier_init();
-    tma_prefetch_desc(&p.tm_g_hi); tma_prefetch_desc(&p.tm_x_hi);
-    if (NPL == 2) { tma_prefetch_desc(&p.tm_g_lo); tma_prefetch_desc(&p.tm_x_lo); }
-  }
-  if (warp == 1) tmem_alloc2<2 * BN>(&tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int item = pair; item < num_items; item += npairs) {
-        const Item w = decode(item);
-        const int cA = w.c0 + (int)rank * 128, nB = w.n0 + (int)rank * 128;
-        const unsigned short ow = p.ig.off_w[w.tap], oh = p.ig.off_h[w.tap];
-        for (int kb = 0; kb < w.num_kb; ++kb) {
-          const long long mrow = w.mbeg + (long long)kb * 64;   // < M: a K-split never starts beyond the tensor
-          const uint32_t mu = (uint32_t)mrow;
-          const int b = (int)fdiv(mu, p.div_hw); const int rem = (int)(mu - (uint32_t)b * (uint32_t)HW);
-          const int y = (int)fdiv((uint32_t)rem, p.div_w); const int x = rem - y * g.Wx;
-          const int cw = p.ig.lo_w + x * g.sx, ch = p.ig.lo_h + y * g.sy;
-          mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-          const uint32_t sA = smem_base + stage * Cfg::STAGE;
-          const uint32_t sB = sA + NPL * Cfg::A_PLANE;
-          if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::STAGE);
-#pragma unroll
-          for (int a = 0; a < 2; ++a) {
-            // channels / columns beyond the tensors are zero-filled by the unit (the byte count stays the same)
-            tma2_im2col(sA + a * 8192, &p.tm_x_hi, cA + a * 64, cw, ch, b, ow, oh, &full_bar[stage]);
-            if (NPL == 2) tma2_im2col(sA + Cfg::A_PLANE + a * 8192, &p.tm_x_lo, cA + a * 64, cw, ch, b, ow, oh, &full_bar[stage]);
-            tma2_load3(sB + a * 8192, &p.tm_g_hi, nB + a * 64, (int)mrow, 0, &full_bar[stage]);
-            if (NPL == 2) tma2_load3(sB + Cfg::B_PLANE + a * 8192, &p.tm_g_lo, nB + a * 64, (int)mrow, 0, &full_bar[stage]);
-          }
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-      for (int s = 0; s < S; ++s) {
-        mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-        if (++stage == S) { stage = 0; phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (rank == 0) {
-      constexpr uint32_t idesc = make_idesc(256, BN, 1, 1);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int item = pair; item < num_items; item += npairs) {
-        const Item w = decode(item);
-        if (w.num_kb == 0) continue;
-        const int as = it & 1;
-        const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-        ++it;
-        mbar_wait_bounded(&tmem_empty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-        for (int kb = 0; kb < w.num_kb; ++kb) {
-          mbar_wait_bounded(&full_bar[stage], phase);
-          tc_fence_after();
-          if (lane == 0) {
-            const uint32_t sA = smem_base + stage * Cfg::STAGE;
-            const uint32_t sB = sA + NPL * Cfg::A_PLANE;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {                    // UMMA_K = 16 K-rows = two 8-row groups = 2048 bytes
-              const uint64_t a_hi = make_desc(sA + k * 2048, 8192, 1024);
-              const uint64_t b_hi = make_desc(sB + k * 2048, 8192, 1024);
-              umma2_bf16(tmem_d, a_hi, b_hi, idesc, (kb | k) != 0);
-              if (NPL == 2) {
-                const uint64_t a_lo = make_desc(sA + Cfg::A_PLANE + k * 2048, 8192, 1024);
-                const uint64_t b_lo = make_desc(sB + Cfg::B_PLANE + k * 2048, 8192, 1024);
-                umma2_bf16(tmem_d, a_hi, b_lo, idesc, 1);
-                umma2_bf16(tmem_d, a_lo, b_hi, idesc, 1);
-              }
-            }
-            umma2_commit_mc(&empty_bar[stage]);
-            if (kb == w.num_kb - 1) umma2_commit_mc(&tmem_full_bar[as]);
-          }
-          __syncwarp();
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ---- epilogue (warps 2..5): this CTA's 128 channel rows of the tile, atomically accumulated into dW (TF layout [t][c][n])
-    const int q = warp & 3;
-    float* stg = epi_stage[q];
-    const int sc = lane & 7, sr = lane >> 3;
-    int it = 0;
-    for (int item = pair; item < num_items; item += npairs) {
-      const Item w = decode(item);
-      if (w.num_kb == 0) continue;
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-      ++it;
-      mbar_wait_bounded(&tmem_full_bar[as], aphase);
-      tc_fence_after();
-      const int cq = w.c0 + (int)rank * 128 + q * 32;         // first channel row of this warp (TMEM lane == channel row)
-#pragma unroll 1
-      for (int cb = 0; cb < BN / 32; ++cb) {
-        const int n = w.n0 + cb * 32;
-        if (n >= p.N || cq >= p.C) break;
-        float o[32];
-        { uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + cb * 32), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int k = 0; k < 32; ++k) o[k] = __uint_as_float(v[k]); }
-        stage_rows(stg, o, lane);
-        float* base; int nn; int ncols;
-        if (n < p.n_split) { base = p.dw_a; nn = n; ncols = p.n_split; } else { base = p.dw_g; nn = n - p.n_split; ncols = p.N - p.n_split; }
-        if (n + 4 * sc < p.N) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = sr + 4 * i;
-            const int c = cq + rr;
-            if (c < p.C) {
-              const float4 val = staged_chunk(stg, rr, sc);
-              float* d = tn_dst(base, g.widx[w.tap], p.C, c, ncols, nn + 4 * sc, p.fold_n);
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(val.x), "f"(val.y), "f"(val.z), "f"(val.w) : "memory");
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tmem_empty_bar[as], 0);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) tmem_dealloc2<2 * BN>(tmem_base);
-}
-
-// ------------------------------------------------------------------------------------------------ CTA-pair TN kernel, F16F8
-// Weight gradient in the 2-MMA-unit precision (kernels.cuh): X and the gradient G are kept as fp16 + two scaled e4m3 planes, both
-// with the activation-role scales (1, 2^12), so both cross products x8hi * g8lo and x8lo * g8hi carry 2^12.  Per work item the row
-// range is walked twice, 128 K-rows per stage: first the e4m3 cross products (K = 32 per MMA, MN-major tiles: one 128-wide atom per
-// CTA and plane), then the fp16 product, whose first MMA rescales the accumulator by 2^-12 (scale-input-d).  Same tile, barriers
-// and epilogue as tc_pair_tn_kernel.
-#define CGVC_Q_WGRAD_SHIFT 12
-struct PairTNQCfg {
-  static constexpr int A_BYTES = 2 * 128 * 128;         // pass 0: x8hi | x8lo (128 K-rows x 128 B each); pass 1: two 64-channel fp16 atoms
-  static constexpr int B_BYTES = 2 * 128 * 128;         // pass 0: g8hi | g8lo; pass 1: two 64-column fp16 atoms
-  static constexpr int STAGE = A_BYTES + B_BYTES;       // 64 KB
-  static constexpr int STAGES = 3;
-  static constexpr int SMEM = STAGES * STAGE + 1024;
-};
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kPairThreads, 1)
-tc_pair_tn_q_kernel(const __grid_constant__ TcTNParams p) {
-  using Cfg = PairTNQCfg;
-  constexpr int S = Cfg::STAGES;
-  constexpr int BN = 256;
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(16) float epi_stage[4][32 * 32];
-  __shared__ __align__(8) uint64_t full_bar[S], empty_bar[S], tmem_full_bar[2], tmem_empty_bar[2];
-  __shared__ uint32_t tmem_slot;
-
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const GatherGeom& g = p.g;
-  const long long M = (long long)g.B * g.Hy * g.Wx;
-  const int HW = g.Hy * g.Wx;
-  const int n_tiles = (p.g_ld + BN - 1) / BN, c_tiles = (p.x_ld + 255) / 256;
-  const int num_items = n_tiles * c_tiles * g.ntaps * p.ksplit;
-  long long chunk_rows = (M + p.ksplit - 1) / p.ksplit;
-  chunk_rows = (chunk_rows + 127) / 128 * 128;
-
-  struct Item { int n0, c0, tap; long long mbeg, mend; int num_kb; };
-  auto decode = [&](int item) -> Item {
-    Item w;
-    int n_t = item % n_tiles; int t1 = item / n_tiles;
-    int c_t = t1 % c_tiles; int t2 = t1 / c_tiles;
-    w.tap = t2 % g.ntaps; int ks = t2 / g.ntaps;
-    w.n0 = n_t * BN; w.c0 = c_t * 256;
-    w.mbeg = (long long)ks * chunk_rows;
-    w.mend = (w.mbeg + chunk_rows < M) ? w.mbeg + chunk_rows : M;
-    w.num_kb = w.mend > w.mbeg ? (int)((w.mend - w.mbeg + 127) / 128) : 0;
-    return w;
-  };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 8); }
-    fence_barrier_init();
-    tma_prefetch_desc(&p.tm_xq); tma_prefetch_desc(&p.tm_gq); tma_prefetch_desc(&p.tm_x8_hi); tma_prefetch_desc(&p.tm_x8_lo);
-    tma_prefetch_desc(&p.tm_g8_hi); tma_prefetch_desc(&p.tm_g8_lo);
-  }
-  if (warp == 1) tmem_alloc2<2 * BN>(&tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int item = pair; item < num_items; item += npairs) {
-        const Item w = decode(item);
-        const int cA = w.c0 + (int)rank * 128, nB = w.n0 + (int)rank * 128;
-        const unsigned short ow = p.ig.off_w[w.tap], oh = p.ig.off_h[w.tap];
-        for (int pass = p.w16; pass < 2; ++pass)
-        for (int kb = 0; kb < w.num_kb; ++kb) {
-          const long long mrow = w.mbeg + (long long)kb * 128;
-          const uint32_t mu = (uint32_t)mrow;
-          const int b = (int)fdiv(mu, p.div_hw); const int rem = (int)(mu - (uint32_t)b * (uint32_t)HW);
-          const int y = (int)fdiv((uint32_t)rem, p.div_w); const int x = rem - y * g.Wx;
-          const int cw = p.ig.lo_w + x * g.sx, ch = p.ig.lo_h + y * g.sy;
-          mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-          const uint32_t sA = smem_base + stage * Cfg::STAGE;
-          const uint32_t sB = sA + Cfg::A_BYTES;
-          if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::STAGE);
-          if (pass == 0) {
-            tma2_im2col(sA, &p.tm_x8_hi, cA, cw, ch, b, ow, oh, &full_bar[stage]);
-            tma2_im2col(sA + 16384, &p.tm_x8_lo, cA, cw, ch, b, ow, oh, &full_bar[stage]);
-            tma2_load3(sB, &p.tm_g8_hi, nB, (int)mrow, 0, &full_bar[stage]);
-            tma2_load3(sB + 16384, &p.tm_g8_lo, nB, (int)mrow, 0, &full_bar[stage]);
-          } else {
-#pragma unroll
-            for (int a = 0; a < 2; ++a) {
-              tma2_im2col(sA + a * 16384, &p.tm_xq, cA + a * 64, cw, ch, b, ow, oh, &full_bar[stage]);
-              tma2_load3(sB + a * 16384, &p.tm_gq, nB + a * 64, (int)mrow, 0, &full_bar[stage]);
-            }
-          }
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-      for (int s = 0; s < S; ++s) {
-        mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-        if (++stage == S) { stage = 0; phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (rank == 0) {
-      // both operands MN-major; formats 0 / 0 = e4m3 (kind::f8f6f4) or fp16 (kind::f16)
-      constexpr uint32_t idq = make_idesc_f0(256, BN) | (1u << 15) | (1u << 16);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int item = pair; item < num_items; item += npairs) {
-        const Item w = decode(item);
-        if (w.num_kb == 0) continue;
-        const int as = it & 1;
-        const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-        ++it;
-        mbar_wait_bounded(&tmem_empty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-        for (int pass = p.w16; pass < 2; ++pass)
-        for (int kb = 0; kb < w.num_kb; ++kb) {
-          mbar_wait_bounded(&full_bar[stage], phase);
-          tc_fence_after();
-          if (lane == 0) {
-            const uint32_t sA = smem_base + stage * Cfg::STAGE;
-            const uint32_t sB = sA + Cfg::A_BYTES;
-            if (pass == 0) {
-              // e4m3, K = 32 K-rows = four 8-row groups = 4096 bytes per instruction; one 128-wide MN atom per CTA and plane
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                umma2_f8(tmem_d, make_desc(sA + k * 4096, 16384, 1024), make_desc(sB + 16384 + k * 4096, 16384, 1024), idq, (kb | k) != 0);
-                umma2_f8(tmem_d, make_desc(sA + 16384 + k * 4096, 16384, 1024), make_desc(sB + k * 4096, 16384, 1024), idq, 1);
-              }
-            } else {
-              // fp16, K = 16 K-rows = 2048 bytes per instruction; two 64-wide MN atoms per CTA (LBO = 16384)
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                const uint64_t a = make_desc(sA + k * 2048, 16384, 1024), b = make_desc(sB + k * 2048, 16384, 1024);
-                if (kb == 0 && k == 0 && !p.w16) umma2_f16_rescale<CGVC_Q_WGRAD_SHIFT>(tmem_d, a, b, idq);
-                else umma2_bf16(tmem_d, a, b, idq, (kb | k) != 0);
-              }
-            }
-            umma2_commit_mc(&empty_bar[stage]);
-            if (pass == 1 && kb == w.num_kb - 1) umma2_commit_mc(&tmem_full_bar[as]);
-          }
-          __syncwarp();
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    float* stg = epi_stage[q];
-    const int sc = lane & 7, sr = lane >> 3;
-    int it = 0;
-    for (int item = pair; item < num_items; item += npairs) {
-      const Item w = decode(item);
-      if (w.num_kb == 0) continue;
-      const int as = it & 1;
-      const uint32_t aphase = (uint32_t)(it >> 1) & 1u;
-      ++it;
-      mbar_wait_bounded(&tmem_full_bar[as], aphase);
-      tc_fence_after();
-      const int cq = w.c0 + (int)rank * 128 + q * 32;
-#pragma unroll 1
-      for (int cb = 0; cb < BN / 32; ++cb) {
-        const int n = w.n0 + cb * 32;
-        if (n >= p.N || cq >= p.C) break;
-        float o[32];
-        { uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + cb * 32), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int k = 0; k < 32; ++k) o[k] = __uint_as_float(v[k]); }
-        stage_rows(stg, o, lane);
-        float* base; int nn; int ncols;
-        if (n < p.n_split) { base = p.dw_a; nn = n; ncols = p.n_split; } else { base = p.dw_g; nn = n - p.n_split; ncols = p.N - p.n_split; }
-        if (n + 4 * sc < p.N) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = sr + 4 * i;
-            const int c = cq + rr;
-            if (c < p.C) {
-              const float4 val = staged_chunk(stg, rr, sc);
-              float* d = tn_dst(base, g.widx[w.tap], p.C, c, ncols, nn + 4 * sc, p.fold_n);
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(val.x), "f"(val.y), "f"(val.z), "f"(val.w) : "memory");
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tmem_empty_bar[as], 0);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) tmem_dealloc2<2 * BN>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------ weight planes
@@ -2068,7 +1375,6 @@ cudaError_t set_smem(K kernel, int bytes) {
 //      2 = NT with the fused instance-norm epilogue
 struct ProfRec { cudaEvent_t a, b; double flops; int cls; long long M; int N, K; };
 int g_tc_debug = 0;
-int g_tc_pair = 1;            // CTA-pair kernels (cta_group::2 + TMA im2col) where the shape allows; 0: one-CTA kernels only
 int g_tc_prep_batched = 1;    // F16F8 weight planes of all layers by prep_weights_q_all_kernel (one launch); 0: the per-layer kernels
 bool g_prof_on = false;
 std::vector<ProfRec> g_prof;
@@ -2085,62 +1391,25 @@ void prof_end(cudaStream_t st) { if (g_prof_on && !g_prof.empty()) cudaEventReco
 // gradient: a 128-wide tile would spend 5x the MMAs on zero padding), else 128
 inline int tile_rows(int n_real, int n_padded) { return (n_padded % 256 == 0) ? 256 : (n_real <= 32 ? 32 : 128); }
 
-cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi, bool pair_ok = false) {
+int num_sms() {
+  static int n = 0;
+  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); }
+  return n;
+}
+
+cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
   if (M == 0) return cudaSuccess;
   const bool x3 = precision == 1;
   if (p.g.ntaps == 0) return cudaErrorInvalidValue;      // empty contractions are the caller's business
   const int bn = tile_rows(p.N, p.Nw);
-  static int num_sms = 0;
-  if (!num_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev); }
   p.n_tiles = bn == 32 ? 1 : p.Nw / bn;                  // the 32-wide tile only ever covers the (<= 32) real columns
   const long long tiles = ((M + 127) / 128) * p.n_tiles;
-  dim3 grid((unsigned)(tiles < num_sms ? tiles : num_sms));
+  dim3 grid((unsigned)(tiles < num_sms() ? tiles : num_sms()));
   cudaError_t e;
   ++g_cgvc_launches;
   p.debug = g_tc_debug;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, (epi == 1 || epi == 2 || epi == 5) ? 2 : 0, M, p.N, p.g.ntaps * p.C);
-  if (pair_ok && g_tc_pair && bn != 32 && M < (1ll << 31)) {
-    // CTA pairs: 256 x bn tile per cluster of 2, persistent over min(#pair tiles, #SM pairs) clusters
-    const long long npairs = num_sms / 2;
-    const long long m_pairs = ((M + 127) / 128 + 1) / 2;
-    int pbn = bn;
-    if (epi == 0 && bn == 256 && p.have_b64 && !p.perm) {     // (gated forward layers keep their [128 a | 128 g] 256-wide tiles)
-      // wave quantisation: a launch whose 256-wide tiles fill the last round of the persistent grid badly runs 128-wide tiles
-      // instead (twice the tiles, 1.5x the operand bytes per FLOP: worth it only for a clearly better fill)
-      const long long t256 = m_pairs * (p.Nw / 256), t128 = m_pairs * (p.Nw / 128);
-      const double e256 = (double)t256 / (double)(((t256 + npairs - 1) / npairs) * npairs);
-      const double e128 = (double)t128 / (double)(((t128 + npairs - 1) / npairs) * npairs);
-      if (0.9 * e128 > e256) { pbn = 128; p.n_tiles = p.Nw / 128; p.tm_b2_hi = p.tm_b64_hi; p.tm_b2_lo = p.tm_b64_lo; }
-    }
-    const long long ptiles = m_pairs * p.n_tiles;
-    dim3 pgrid((unsigned)(2 * (ptiles < npairs ? ptiles : npairs)));
-#define LAUNCH_PAIR(BN_, NPL_, EPI_)                                                              \
-  do {                                                                                            \
-    e = set_smem(tc_pair_nt_kernel<BN_, NPL_, EPI_>, PairCfg<BN_, NPL_>::SMEM);                   \
-    if (e != cudaSuccess) return e;                                                               \
-    tc_pair_nt_kernel<BN_, NPL_, EPI_><<<pgrid, kPairNTThreads, PairCfg<BN_, NPL_>::SMEM, st>>>(p); \
-  } while (0)
-    if (epi != 0 && bn != 256) return cudaErrorInvalidValue;
-    if (precision == 3) {                                   // F16F8 (no fused backward epilogues in this precision)
-      if (epi == 1)        LAUNCH_PAIR(256, 3, 1);
-      else if (epi == 2)   LAUNCH_PAIR(256, 3, 2);
-      else if (epi == 5)   LAUNCH_PAIR(256, 3, 5);
-      else if (epi != 0)   return cudaErrorInvalidValue;
-      else if (pbn == 256) LAUNCH_PAIR(256, 3, 0);
-      else                 LAUNCH_PAIR(128, 3, 0);
-    }
-    else if (epi == 1)  { if (x3) LAUNCH_PAIR(256, 2, 1); else LAUNCH_PAIR(256, 1, 1); }
-    else if (epi == 2)  { if (x3) LAUNCH_PAIR(256, 2, 2); else LAUNCH_PAIR(256, 1, 2); }
-    else if (epi == 3)  { if (x3) LAUNCH_PAIR(256, 2, 3); else LAUNCH_PAIR(256, 1, 3); }
-    else if (epi == 4)  { if (x3) LAUNCH_PAIR(256, 2, 4); else LAUNCH_PAIR(256, 1, 4); }
-    else if (epi == 5)  { if (x3) LAUNCH_PAIR(256, 2, 5); else LAUNCH_PAIR(256, 1, 5); }
-    else if (pbn == 256) { if (x3) LAUNCH_PAIR(256, 2, 0); else LAUNCH_PAIR(256, 1, 0); }
-    else                 { if (x3) LAUNCH_PAIR(128, 2, 0); else LAUNCH_PAIR(128, 1, 0); }
-#undef LAUNCH_PAIR
-    prof_end(st);
-    return cudaGetLastError();
-  }
 #define LAUNCH_NT(BN_, NPL_, EPI_)                                                                \
   do {                                                                                            \
     e = set_smem(tc_gg_nt_kernel<BN_, NPL_, EPI_>, NTCfg<BN_, NPL_>::SMEM);                       \
@@ -2148,7 +1417,7 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi, boo
     tc_gg_nt_kernel<BN_, NPL_, EPI_><<<grid, kNTThreads, NTCfg<BN_, NPL_>::SMEM, st>>>(p);        \
   } while (0)
   if (epi != 0 && bn != 256) return cudaErrorInvalidValue;
-  if (precision == 3) {                                     // F16F8: forward form only
+  if (precision == 3) {                                     // F16F8 (no fused backward epilogues in this precision)
     if (epi == 1)       LAUNCH_NT(256, 3, 1);
     else if (epi == 2)  LAUNCH_NT(256, 3, 2);
     else if (epi == 5)  LAUNCH_NT(256, 3, 5);
@@ -2170,80 +1439,39 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi, boo
   return cudaGetLastError();
 }
 
-cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st, bool pair_ok = false) {
+cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st) {
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
   if (M == 0) return cudaSuccess;
-  const bool x3 = precision == 1;
   if (M >= (1ll << 31)) return cudaErrorInvalidValue;
-  // CTA pairs (256-channel x 256-column tiles) where both extents fill them
-  const bool pair = pair_ok && g_tc_pair && precision != 3 && p.x_ld % 256 == 0 && p.g_ld % 256 == 0;
-  int tiles = ((p.g_ld + 255) / 256) * ((p.x_ld + (pair ? 255 : 127)) / (pair ? 256 : 128)) * p.g.ntaps;
-  static int num_sms_dev = 0;
-  if (!num_sms_dev) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_sms_dev, cudaDevAttrMultiProcessorCount, dev); }
-  const int num_sms = pair ? num_sms_dev / 2 : num_sms_dev;   // persistent CTAs (or CTA pairs) the work items are spread over
+  const int tiles = ((p.g_ld + 255) / 256) * ((p.x_ld + 127) / 128) * p.g.ntaps;
+  const int nsm = num_sms();
   // split the row (contraction) range so that the work items fill whole rounds of the persistent grid; every item keeps
-  // >= 16 stages so that its red.global epilogue hides behind the next item's MMAs
+  // >= 16 stages so that the wait of its epilogue stays small next to its MMAs
   long long maxsplit = M / 1024; if (maxsplit < 1) maxsplit = 1; if (maxsplit > 32) maxsplit = 32;
   int ksplit = 1; double best = 0.0;
   for (int ks = 1; ks <= (int)maxsplit; ++ks) {
     long long items = (long long)tiles * ks;
-    double eff = (double)items / (double)(((items + num_sms - 1) / num_sms) * num_sms);
-    if (items < num_sms) eff *= 0.5;                       // a single partial round: prefer more, smaller items
+    double eff = (double)items / (double)(((items + nsm - 1) / nsm) * nsm);
+    if (items < nsm) eff *= 0.5;                           // a single partial round: prefer more, smaller items
     if (eff > best + 0.02) { best = eff; ksplit = ks; }
   }
   p.ksplit = ksplit;
   p.div_hw = make_fastdiv((uint32_t)(p.g.Hy * p.g.Wx)); p.div_w = make_fastdiv((uint32_t)p.g.Wx);
   const long long items = (long long)tiles * ksplit;
-  dim3 grid((unsigned)(items < num_sms ? items : num_sms));
+  dim3 grid((unsigned)(items < nsm ? items : nsm));
   cudaError_t e;
   ++g_cgvc_launches;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, 1, M, p.N, p.g.ntaps * p.C);
-  if (pair) {
-    dim3 pgrid((unsigned)(2 * (items < num_sms ? items : num_sms)));     // num_sms already counts pairs here
-    if (x3) {
-      e = set_smem(tc_pair_tn_kernel<2>, PairTNCfg<2>::SMEM); if (e != cudaSuccess) return e;
-      tc_pair_tn_kernel<2><<<pgrid, kPairThreads, PairTNCfg<2>::SMEM, st>>>(p);
-    } else {
-      e = set_smem(tc_pair_tn_kernel<1>, PairTNCfg<1>::SMEM); if (e != cudaSuccess) return e;
-      tc_pair_tn_kernel<1><<<pgrid, kPairThreads, PairTNCfg<1>::SMEM, st>>>(p);
-    }
-    prof_end(st);
-    return cudaGetLastError();
-  }
-  if (x3) {
+  if (precision == 3) {
+    e = set_smem(tc_gg_tn_kernel<3>, TNCfg<3>::SMEM); if (e != cudaSuccess) return e;
+    tc_gg_tn_kernel<3><<<grid, kNTThreads, TNCfg<3>::SMEM, st>>>(p);
+  } else if (precision == 1) {
     e = set_smem(tc_gg_tn_kernel<2>, TNCfg<2>::SMEM); if (e != cudaSuccess) return e;
     tc_gg_tn_kernel<2><<<grid, kNTThreads, TNCfg<2>::SMEM, st>>>(p);
   } else {
     e = set_smem(tc_gg_tn_kernel<1>, TNCfg<1>::SMEM); if (e != cudaSuccess) return e;
     tc_gg_tn_kernel<1><<<grid, kNTThreads, TNCfg<1>::SMEM, st>>>(p);
   }
-  prof_end(st);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_tn_q(TcTNParams p, cudaStream_t st) {
-  const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
-  if (M == 0) return cudaSuccess;
-  static int num_sms_dev = 0;
-  if (!num_sms_dev) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_sms_dev, cudaDevAttrMultiProcessorCount, dev); }
-  const int npairs = num_sms_dev / 2;
-  const int tiles = ((p.g_ld + 255) / 256) * ((p.x_ld + 255) / 256) * p.g.ntaps;
-  long long maxsplit = M / 2048; if (maxsplit < 1) maxsplit = 1; if (maxsplit > 32) maxsplit = 32;     // every item keeps >= 16 stages of 128 rows
-  int ksplit = 1; double best = 0.0;
-  for (int ks = 1; ks <= (int)maxsplit; ++ks) {
-    long long items = (long long)tiles * ks;
-    double eff = (double)items / (double)(((items + npairs - 1) / npairs) * npairs);
-    if (items < npairs) eff *= 0.5;
-    if (eff > best + 0.02) { best = eff; ksplit = ks; }
-  }
-  p.ksplit = ksplit;
-  p.div_hw = make_fastdiv((uint32_t)(p.g.Hy * p.g.Wx)); p.div_w = make_fastdiv((uint32_t)p.g.Wx);
-  const long long items = (long long)tiles * ksplit;
-  dim3 pgrid((unsigned)(2 * (items < npairs ? items : npairs)));
-  ++g_cgvc_launches;
-  prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, 1, M, p.N, p.g.ntaps * p.C);
-  cudaError_t e = set_smem(tc_pair_tn_q_kernel, PairTNQCfg::SMEM); if (e != cudaSuccess) return e;
-  tc_pair_tn_q_kernel<<<pgrid, kPairThreads, PairTNQCfg::SMEM, st>>>(p);
   prof_end(st);
   return cudaGetLastError();
 }
@@ -2268,62 +1496,36 @@ inline int layer_perm(const TcLayer& L) {
 }
 inline bool layer_ok(const TcLayer& L) {
   if (L.fold && (L.gated || L.kh * L.kw != 1 || L.cout % L.fold || (L.cout / L.fold) % 4)) return false;      // see TcLayer::fold
-  return L.kh * L.kw <= CGVC_MAX_TAPS && L.cin % 4 == 0 && Ntot(L) % 4 == 0;
+  return L.kh * L.kw <= CGVC_MAX_TAPS && Ntot(L) % 4 == 0;
 }
+// the F16F8 planes pack quads of input channels (cgvc_quant4)
+inline bool layer_ok_q(const TcLayer& L) { return layer_ok(L) && L.cin % 4 == 0; }
+
 
 // TMA descriptors of a layer's weight planes (call after wf_/wd_ pointers are set)
 bool make_layer_maps(TcLayer& L) {
   const int taps = L.kh * L.kw;
   const int bf = tile_rows(Ntot(L), nt_n(L)), bd = tile_rows(L.cin, cin_n(L));   // must match launch_nt's choice of BN
-  // pair kernels: each CTA of a pair loads half of the weight tile (tiles there are 256 or 128 rows wide, never 32)
-  const int bf2 = (bf == 256 ? 256 : 128) / 2, bd2 = (bd == 256 ? 256 : 128) / 2;
   return make_tmap3(&L.tm_f_hi, L.wf_hi, cin_k(L), nt_n(L), taps, bf) &&
          make_tmap3(&L.tm_f_lo, L.wf_lo, cin_k(L), nt_n(L), taps, bf) &&
          make_tmap3(&L.tm_d_hi, L.wd_hi, nt_k(L), cin_n(L), taps, bd) &&
-         make_tmap3(&L.tm_d_lo, L.wd_lo, nt_k(L), cin_n(L), taps, bd) &&
-         make_tmap3(&L.tm_f2_hi, L.wf_hi, cin_k(L), nt_n(L), taps, bf2) &&
-         make_tmap3(&L.tm_f2_lo, L.wf_lo, cin_k(L), nt_n(L), taps, bf2) &&
-         make_tmap3(&L.tm_d2_hi, L.wd_hi, nt_k(L), cin_n(L), taps, bd2) &&
-         make_tmap3(&L.tm_d2_lo, L.wd_lo, nt_k(L), cin_n(L), taps, bd2) &&
-         make_tmap3(&L.tm_f64_hi, L.wf_hi, cin_k(L), nt_n(L), taps, 64) &&
-         make_tmap3(&L.tm_f64_lo, L.wf_lo, cin_k(L), nt_n(L), taps, 64) &&
-         make_tmap3(&L.tm_d64_hi, L.wd_hi, nt_k(L), cin_n(L), taps, 64) &&
-         make_tmap3(&L.tm_d64_lo, L.wd_lo, nt_k(L), cin_n(L), taps, 64);
+         make_tmap3(&L.tm_d_lo, L.wd_lo, nt_k(L), cin_n(L), taps, bd);
 }
 
-// TMA im2col maps of the gathered operand planes (pair kernels); false if the geometry cannot be expressed
-bool make_gather_maps(TcNTParams& p, int precision = 1) {
-  p.ig = im2col_geom(p.g);
-  if (!p.ig.ok) return false;
-  if (precision == 3) {                                      // F16F8: fp16 plane + two e4m3 planes
-    return make_im2col_map(&p.tm_a_hi, p.a_hi, p.g, p.ig, p.C, p.a_ld, 128, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2) &&
-           make_im2col_map(&p.tm_a8_hi, p.a8_hi, p.g, p.ig, p.C, p.a_ld, 128, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1) &&
-           make_im2col_map(&p.tm_a8_lo, p.a8_lo, p.g, p.ig, p.C, p.a_ld, 128, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
-  }
-  if (!make_im2col_map(&p.tm_a_hi, p.a_hi, p.g, p.ig, p.C, p.a_ld, 128)) return false;
-  if (p.a_lo && !make_im2col_map(&p.tm_a_lo, p.a_lo, p.g, p.ig, p.C, p.a_ld, 128)) return false;
-  return true;
-}
 bool make_layer_maps_q(TcLayer& L) {
   const int taps = L.kh * L.kw;
   const int bf = tile_rows(Ntot(L), nt_n(L)), bd = tile_rows(L.cin, cin_n(L));
-  const int bf2 = (bf == 256 ? 256 : 128) / 2, bd2 = (bd == 256 ? 256 : 128) / 2;      // half tiles of the pair kernels
   const CUtensorMapDataType F16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16, U8 = CU_TENSOR_MAP_DATA_TYPE_UINT8;
   bool ok = make_tmap3_t(&L.tm_q16, L.wq16, F16, 2, cin_q(L), nt_n(L), taps, 64, bf) &&
             make_tmap3_t(&L.tm_q8hi, L.wq8hi, U8, 1, cin_q(L), nt_n(L), taps, 128, bf) &&
-            make_tmap3_t(&L.tm_q8lo, L.wq8lo, U8, 1, cin_q(L), nt_n(L), taps, 128, bf) &&
-            make_tmap3_t(&L.tm_q16h, L.wq16, F16, 2, cin_q(L), nt_n(L), taps, 64, bf2) &&
-            make_tmap3_t(&L.tm_q8hih, L.wq8hi, U8, 1, cin_q(L), nt_n(L), taps, 128, bf2) &&
-            make_tmap3_t(&L.tm_q8loh, L.wq8lo, U8, 1, cin_q(L), nt_n(L), taps, 128, bf2);
+            make_tmap3_t(&L.tm_q8lo, L.wq8lo, U8, 1, cin_q(L), nt_n(L), taps, 128, bf);
   if (ok && L.wdq16)
     ok = make_tmap3_t(&L.tm_dq16, L.wdq16, F16, 2, nt_q(L), cin_n(L), taps, 64, bd) &&
          make_tmap3_t(&L.tm_dq8hi, L.wdq8hi, U8, 1, nt_q(L), cin_n(L), taps, 128, bd) &&
-         make_tmap3_t(&L.tm_dq8lo, L.wdq8lo, U8, 1, nt_q(L), cin_n(L), taps, 128, bd) &&
-         make_tmap3_t(&L.tm_dq16h, L.wdq16, F16, 2, nt_q(L), cin_n(L), taps, 64, bd2) &&
-         make_tmap3_t(&L.tm_dq8hih, L.wdq8hi, U8, 1, nt_q(L), cin_n(L), taps, 128, bd2) &&
-         make_tmap3_t(&L.tm_dq8loh, L.wdq8lo, U8, 1, nt_q(L), cin_n(L), taps, 128, bd2);
+         make_tmap3_t(&L.tm_dq8lo, L.wdq8lo, U8, 1, nt_q(L), cin_n(L), taps, 128, bd);
   return ok;
 }
+
 
 int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba, const float* bg, cudaStream_t st) {
   const int taps = L.kh * L.kw;
@@ -2339,7 +1541,7 @@ int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba,
     copy_bias_kernel<<<(L.cout + 255) / 256, 256, 0, st>>>(bg, L.bias, L.cout, L.cout, perm);
   }
   if (L.wq16) {
-    long long tot = (long long)taps * L.cout * (L.cin / 4); long long nb = (tot + 255) / 256; if (nb > 148 * 32) nb = 148 * 32;
+    long long tot = (long long)taps * L.cout * (L.cin / 4); long long nb = (tot + 255) / 256; if (nb > num_sms() * 32) nb = num_sms() * 32;
     g_cgvc_launches += L.gated ? 2 : 1;
     prep_weights_q_kernel<<<(unsigned)nb, 256, 0, st>>>(ka, taps, L.cin, L.cout, nt_n(L), cin_q(L), 0, perm, fn, (__half*)L.wq16, L.wq8hi, L.wq8lo);
     if (L.gated) prep_weights_q_kernel<<<(unsigned)nb, 256, 0, st>>>(kg, taps, L.cin, L.cout, nt_n(L), cin_q(L), L.cout, perm, fn, (__half*)L.wq16, L.wq8hi, L.wq8lo);
@@ -2355,7 +1557,7 @@ int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba,
 // x planes: [n,H,W,cin_k] (channels beyond cin are zero)
 int layer_fwd(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
               float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused_out = nullptr) {
-  if (!layer_ok(L)) return TC_UNSUPPORTED;
+  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   TcNTParams p; memset(&p, 0, sizeof p);
   p.g = fwd_geom(n, H, W, L.kh, L.kw, sh, sw);
   p.a_hi = xhi; p.a_lo = xlo; p.a_ld = cin_k(L); p.C = cin_k(L);
@@ -2385,23 +1587,14 @@ int layer_fwd(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const _
   }
   if (fused_out) *fused_out = epi != 0;
   if (!epi && !P) return (int)cudaErrorInvalidValue;          // only the fused epilogues can do without the pre-norm output
-  bool pair_ok = false;
-  if (g_tc_pair && tile_rows(p.N, p.Nw) != 32) {
-    if (precision == 3) { p.tm_b2_hi = L.tm_q16h; p.tm_b28_hi = L.tm_q8hih; p.tm_b28_lo = L.tm_q8loh; }
-    else {
-      p.tm_b2_hi = L.tm_f2_hi; p.tm_b2_lo = L.tm_f2_lo;
-      p.tm_b64_hi = L.tm_f64_hi; p.tm_b64_lo = L.tm_f64_lo; p.have_b64 = 1;
-    }
-    pair_ok = make_gather_maps(p, precision);
-  }
-  return (int)launch_nt(p, precision, st, epi, pair_ok);
+  return (int)launch_nt(p, precision, st, epi);
 }
 
 // dP planes: [rows_out, nt_k]
 int layer_dgrad(const TcLayer& L, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                 float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused_out = nullptr) {
   if (fused_out) *fused_out = false;
-  if (!layer_ok(L) || (precision == 3 && !L.wdq16)) return TC_UNSUPPORTED;     // F16F8 needs the data-gradient planes (training engines)
+  if (!layer_ok(L) || (precision == 3 && (!layer_ok_q(L) || !L.wdq16))) return TC_UNSUPPORTED;     // F16F8 needs the data-gradient planes (training engines)
   std::vector<GatherGeom> gs = dgrad_geoms(n, H, W, L.kh, L.kw, sh, sw);
   for (const GatherGeom& g : gs) if (g.ntaps == 0) return TC_UNSUPPORTED;     // (never the case for this model's layers)
   // fused backward epilogue: stride-1 1-D layer (one geometry, dense rows), whole samples per 128-row tile, 256-wide tiles
@@ -2429,16 +1622,7 @@ int layer_dgrad(const TcLayer& L, int precision, const __nv_bfloat16* dPhi, cons
       p.bp = fuse->bp; p.bp_ld = fuse->bp_ld; p.dp_hi = fuse->dp_hi; p.dp_lo = fuse->dp_lo; p.dp_ld = fuse->dp_ld;
       p.dbeta_a = fuse->dbeta_a; p.dgamma_a = fuse->dgamma_a; p.dbeta_g = fuse->dbeta_g; p.dgamma_g = fuse->dgamma_g;
     }
-    bool pair_ok = false;
-    if (g_tc_pair && tile_rows(p.N, p.Nw) != 32) {
-      if (precision == 3) { p.tm_b2_hi = L.tm_dq16h; p.tm_b28_hi = L.tm_dq8hih; p.tm_b28_lo = L.tm_dq8loh; }
-      else {
-        p.tm_b2_hi = L.tm_d2_hi; p.tm_b2_lo = L.tm_d2_lo;
-        p.tm_b64_hi = L.tm_d64_hi; p.tm_b64_lo = L.tm_d64_lo; p.have_b64 = 1;
-      }
-      pair_ok = make_gather_maps(p, precision);
-    }
-    cudaError_t e = launch_nt(p, precision, st, epi, pair_ok);
+    cudaError_t e = launch_nt(p, precision, st, epi);
     if (e != cudaSuccess) return (int)e;
   }
   if (fused_out) *fused_out = epi != 0;
@@ -2448,42 +1632,27 @@ int layer_dgrad(const TcLayer& L, int precision, const __nv_bfloat16* dPhi, cons
 int layer_wgrad(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                 const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                 float* dwa, float* dwg, cudaStream_t st, int w16 = 0) {
-  if (!layer_ok(L)) return TC_UNSUPPORTED;
+  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   TcTNParams p; memset(&p, 0, sizeof p);
   p.w16 = (precision == 3 && w16) ? 1 : 0;
   p.fold_n = L.fold ? L.cout / L.fold : 0;
   p.g = fwd_geom(n, H, W, L.kh, L.kw, sh, sw);
-  if (precision == 3) {
-    // F16F8: x planes [rows_in, cin_q] and dP planes [M, nt_q], each q16 + (q8hi | q8lo); always the CTA-pair kernel
-    const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx, rows_in = (long long)n * H * W;
-    if (M >= (1ll << 31)) return (int)cudaErrorInvalidValue;
-    p.x_ld = cin_q(L); p.C = L.cin; p.g_ld = nt_q(L); p.N = Ntot(L);
-    p.dw_a = dwa; p.dw_g = dwg; p.n_split = L.cout;
-    const uint8_t* x8 = reinterpret_cast<const uint8_t*>(xlo); const uint8_t* g8 = reinterpret_cast<const uint8_t*>(dPlo);
-    p.ig = im2col_geom(p.g);
-    const CUtensorMapDataType F16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16, U8 = CU_TENSOR_MAP_DATA_TYPE_UINT8;
-    if (!p.ig.ok ||
-        !make_im2col_map(&p.tm_xq, xhi, p.g, p.ig, p.x_ld, p.x_ld, 128, F16, 2) ||
-        !make_im2col_map(&p.tm_x8_hi, x8, p.g, p.ig, p.x_ld, p.x_ld, 128, U8, 1) ||
-        !make_im2col_map(&p.tm_x8_lo, x8 + rows_in * p.x_ld, p.g, p.ig, p.x_ld, p.x_ld, 128, U8, 1) ||
-        !make_tmap3_t(&p.tm_gq, dPhi, F16, 2, (uint64_t)p.g_ld, (uint64_t)M, 1, 64, 128) ||
-        !make_tmap3_t(&p.tm_g8_hi, g8, U8, 1, (uint64_t)p.g_ld, (uint64_t)M, 1, 128, 128) ||
-        !make_tmap3_t(&p.tm_g8_lo, g8 + M * p.g_ld, U8, 1, (uint64_t)p.g_ld, (uint64_t)M, 1, 128, 128))
-      return TC_UNSUPPORTED;
-    return (int)launch_tn_q(p, st);
-  }
   p.x_hi = xhi; p.x_lo = xlo; p.x_ld = cin_k(L); p.C = L.cin;
   p.g_hi = dPhi; p.g_lo = dPlo; p.g_ld = nt_k(L); p.N = Ntot(L);
   p.dw_a = dwa; p.dw_g = dwg; p.n_split = L.cout;
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
-  if (!make_tmap3(&p.tm_g_hi, dPhi, (uint64_t)nt_k(L), (uint64_t)M, 1, 64) || !make_tmap3(&p.tm_g_lo, dPlo, (uint64_t)nt_k(L), (uint64_t)M, 1, 64))
+  if (precision == 3) {
+    // F16F8: x planes [rows_in, cin_q] and dP planes [M, nt_q], each q16 (xhi / dPhi) + q8hi followed by q8lo (xlo / dPlo)
+    const long long rows_in = (long long)n * H * W;
+    p.x_ld = cin_q(L); p.g_ld = nt_q(L); p.x_lo = p.g_lo = nullptr;
+    p.x8_hi = reinterpret_cast<const uint8_t*>(xlo); p.x8_lo = p.x8_hi + rows_in * p.x_ld;
+    p.g8_hi = reinterpret_cast<const uint8_t*>(dPlo); p.g8_lo = p.g8_hi + M * p.g_ld;
+    if (!make_tmap3_t(&p.tm_g_hi, dPhi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)p.g_ld, (uint64_t)M, 1, 64, 64))
+      return (int)cudaErrorInvalidValue;
+  } else if (!make_tmap3(&p.tm_g_hi, dPhi, (uint64_t)nt_k(L), (uint64_t)M, 1, 64) || !make_tmap3(&p.tm_g_lo, dPlo, (uint64_t)nt_k(L), (uint64_t)M, 1, 64)) {
     return (int)cudaErrorInvalidValue;
-  bool pair_ok = false;
-  if (g_tc_pair && p.x_ld % 256 == 0 && p.g_ld % 256 == 0) {
-    p.ig = im2col_geom(p.g);
-    pair_ok = p.ig.ok && make_im2col_map(&p.tm_x_hi, xhi, p.g, p.ig, p.x_ld, p.x_ld, 64) && make_im2col_map(&p.tm_x_lo, xlo, p.g, p.ig, p.x_ld, p.x_ld, 64);
   }
-  return (int)launch_tn(p, precision, st, pair_ok);
+  return (int)launch_tn(p, precision, st);
 }
 
 }  // namespace
@@ -2503,8 +1672,8 @@ int tc_alloc(TcWeights& w) {
   auto rnd = [](size_t b) { return (b + 255) & ~(size_t)255; };
   for (TcLayer& L : w.layers) {
     total += 2 * rnd(wf_elems(L) * sizeof(__nv_bfloat16)) + 2 * rnd(wd_elems(L) * sizeof(__nv_bfloat16)) + rnd((size_t)nt_n(L) * sizeof(float));
-    if (w.quant && layer_ok(L)) total += rnd(wq_elems(L) * 2) + 2 * rnd(wq_elems(L));
-    if (w.quant && w.quant_bwd && layer_ok(L)) total += rnd(wdq_elems(L) * 2) + 2 * rnd(wdq_elems(L));
+    if (w.quant && layer_ok_q(L)) total += rnd(wq_elems(L) * 2) + 2 * rnd(wq_elems(L));
+    if (w.quant && w.quant_bwd && layer_ok_q(L)) total += rnd(wdq_elems(L) * 2) + 2 * rnd(wdq_elems(L));
   }
   cudaError_t err = cudaMalloc(&w.pool, total);
   if (err != cudaSuccess) return (int)err;
@@ -2519,7 +1688,7 @@ int tc_alloc(TcWeights& w) {
     L.bias = (float*)p; p += rnd((size_t)nt_n(L) * sizeof(float));
     if (!make_layer_maps(L)) return (int)cudaErrorInvalidValue;
     L.wq16 = nullptr; L.wq8hi = L.wq8lo = nullptr; L.wdq16 = nullptr; L.wdq8hi = L.wdq8lo = nullptr;
-    if (w.quant && layer_ok(L)) {
+    if (w.quant && layer_ok_q(L)) {
       L.wq16 = p; p += rnd(wq_elems(L) * 2);
       L.wq8hi = (uint8_t*)p; p += rnd(wq_elems(L)); L.wq8lo = (uint8_t*)p; p += rnd(wq_elems(L));
       if (w.quant_bwd) {
@@ -2568,22 +1737,12 @@ static cudaError_t tc_init_kernels() {
 #define INIT_NT(BN_, NPL_, EPI_) if ((e = set_smem(tc_gg_nt_kernel<BN_, NPL_, EPI_>, NTCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
   INIT_NT(256, 2, 0) INIT_NT(256, 1, 0) INIT_NT(128, 2, 0) INIT_NT(128, 1, 0) INIT_NT(32, 2, 0) INIT_NT(32, 1, 0)
   INIT_NT(256, 2, 1) INIT_NT(256, 1, 1) INIT_NT(256, 2, 2) INIT_NT(256, 1, 2)
-  INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4)
-  INIT_NT(256, 3, 0) INIT_NT(128, 3, 0) INIT_NT(32, 3, 0) INIT_NT(256, 3, 1) INIT_NT(256, 3, 2)
+  INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4) INIT_NT(256, 2, 5) INIT_NT(256, 1, 5)
+  INIT_NT(256, 3, 0) INIT_NT(128, 3, 0) INIT_NT(32, 3, 0) INIT_NT(256, 3, 1) INIT_NT(256, 3, 2) INIT_NT(256, 3, 5)
 #undef INIT_NT
+  if ((e = set_smem(tc_gg_tn_kernel<3>, TNCfg<3>::SMEM)) != cudaSuccess) return e;
   if ((e = set_smem(tc_gg_tn_kernel<2>, TNCfg<2>::SMEM)) != cudaSuccess) return e;
   if ((e = set_smem(tc_gg_tn_kernel<1>, TNCfg<1>::SMEM)) != cudaSuccess) return e;
-#define INIT_PAIR(BN_, NPL_, EPI_) if ((e = set_smem(tc_pair_nt_kernel<BN_, NPL_, EPI_>, PairCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
-  INIT_PAIR(256, 2, 0) INIT_PAIR(256, 1, 0) INIT_PAIR(128, 2, 0) INIT_PAIR(128, 1, 0)
-  INIT_PAIR(256, 2, 1) INIT_PAIR(256, 1, 1) INIT_PAIR(256, 2, 2) INIT_PAIR(256, 1, 2)
-  INIT_PAIR(256, 2, 3) INIT_PAIR(256, 1, 3) INIT_PAIR(256, 2, 4) INIT_PAIR(256, 1, 4)
-#undef INIT_PAIR
-  if ((e = set_smem(tc_pair_tn_kernel<2>, PairTNCfg<2>::SMEM)) != cudaSuccess) return e;
-  if ((e = set_smem(tc_pair_tn_kernel<1>, PairTNCfg<1>::SMEM)) != cudaSuccess) return e;
-#define INIT_PAIR(BN_, NPL_, EPI_) if ((e = set_smem(tc_pair_nt_kernel<BN_, NPL_, EPI_>, PairCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
-  INIT_PAIR(256, 3, 0) INIT_PAIR(128, 3, 0) INIT_PAIR(256, 3, 1) INIT_PAIR(256, 3, 2)
-#undef INIT_PAIR
-  if ((e = set_smem(tc_pair_tn_q_kernel, PairTNQCfg::SMEM)) != cudaSuccess) return e;
   return cudaSuccess;
 }
 
@@ -2703,7 +1862,6 @@ int tc_profile_launches(double* ms, double* flops, long long* meta4, int capacit
   return 0;
 }
 void tc_set_debug(int v) { g_tc_debug = v; }
-void tc_set_pair(int v) { g_tc_pair = v != 0; }
 
 // ---- self-contained versions for the unit tests: fp32 in/out, temporary planes ----
 namespace {
@@ -2739,7 +1897,7 @@ static int adhoc_layer(Temp& T, TcLayer& L, cudaStream_t st) {
 int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float* bias, float* y,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st) {
   TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
-  if (!layer_ok(L)) return TC_UNSUPPORTED;
+  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   Temp T;
   int r = adhoc_layer(T, L, st); if (r) return r;
   size_t rows = (size_t)B * H * W;
@@ -2760,7 +1918,7 @@ int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float
 int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16) {
   TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
-  if (!layer_ok(L)) return TC_UNSUPPORTED;
+  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   Temp T;
   int r = adhoc_layer(T, L, st); if (r) return r;
   if (precision == 3) { r = adhoc_layer_q(T, L, st); if (r) return r; }

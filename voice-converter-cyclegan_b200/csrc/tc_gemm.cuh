@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) gather-GEMM path of libcgvc.so: bf16 hi/lo split operands, fp32 TMEM accumulators.
+// wgmma (Hopper tensor core) gather-GEMM path of libcgvc.so: bf16 hi/lo split operands, fp32 register accumulators.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -24,16 +24,13 @@ struct TcLayer {
   float* bias;                    // [Ntot_n]
   CUtensorMap tm_f_hi, tm_f_lo;   // TMA descriptors of wf (box [1][BN][64]) and wd, built once the planes are allocated
   CUtensorMap tm_d_hi, tm_d_lo;
-  CUtensorMap tm_f64_hi, tm_f64_lo, tm_d64_hi, tm_d64_lo;   // ... and with 64-row boxes (128-wide pair tiles)
-  CUtensorMap tm_f2_hi, tm_f2_lo, tm_d2_hi, tm_d2_lo;   // the same planes with half-tile boxes: each CTA of a pair loads half a weight tile
   // CGVC_PREC_F16F8 (allocated when TcWeights::quant): forward operand [taps][Ntot_n][cin_q], cin_q = cin rounded up
   // to 128, as fp16 + two e4m3 planes with the weight scales of kernels.cuh
   void* wq16; uint8_t *wq8hi, *wq8lo;
   CUtensorMap tm_q16, tm_q8hi, tm_q8lo;
-  CUtensorMap tm_q16h, tm_q8hih, tm_q8loh;          // the same planes with half-tile boxes (CTA-pair kernels)
   // F16F8 training (TcWeights::quant_bwd): data-gradient operand [taps][cin_n][nt_q], nt_q = Ntot rounded up to 128
   void* wdq16; uint8_t *wdq8hi, *wdq8lo;
-  CUtensorMap tm_dq16, tm_dq8hi, tm_dq8lo, tm_dq16h, tm_dq8hih, tm_dq8loh;
+  CUtensorMap tm_dq16, tm_dq8hi, tm_dq8lo;
 };
 
 struct TcWeights {
@@ -111,5 +108,4 @@ bool tc_profile_is_on();
 int tc_profile_collect(double ms[3], double flops[3], long long launches[3]);
 int tc_profile_launches(double* ms, double* flops, long long* meta4, int capacity, int* n_out);
 void tc_set_prep_batched(int v);   // 1 (default): F16F8 weight planes of all layers in one launch; 0: per-layer kernels
-void tc_set_pair(int v);      // 1 (default): CTA-pair kernels where the shape allows; 0: one-CTA kernels only
 void tc_set_debug(int v);     // diagnostic knobs of the NT kernel (timing experiments only; see TcNTParams::debug)

@@ -1,7 +1,7 @@
-"""`CycleGAN`: the reference's model class (model.py:7-169 of /root/reference) on the native B200 engine.
+"""`CycleGAN`: the reference's model class (model.py:7-169 of /root/reference) on the native H100 engine.
 
 Same constructor and method signatures as the reference; the TensorFlow-1 session is replaced by libcgvc.so
-(hand-written sm_100a CUDA behind the C ABI in include/cgvc.h).  PyTorch is used for device storage
+(hand-written sm_90a CUDA behind the C ABI in include/cgvc.h).  PyTorch is used for device storage
 (arenas, staging) only -- no torch op runs on the hot path.
 
 Differences a user of the reference should know:
@@ -41,7 +41,7 @@ class CycleGAN(object):
                 raise TypeError("CycleGAN(discriminator=..., generator=...) takes network descriptors (cgvc.module.generator_gatedcnn / "
                                 "cgvc.module.discriminator or equivalents), not %r: the native engine runs its own kernel graph" % (net,))
         if not torch.cuda.is_available():
-            raise RuntimeError("CycleGAN needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("CycleGAN needs a CUDA device (sm_90a); there is no CPU fallback")
         self.num_features = num_features
         self.input_shape = [None, num_features, None]
         self.discriminator = discriminator

@@ -25,7 +25,7 @@ def _pyworld():
         import pyworld
         return pyworld
     except ImportError as e:                                   # pragma: no cover - pyworld is absent in this image
-        raise ImportError("WORLD analysis/synthesis needs the `pyworld` package (CPU audio code, outside the B200 hot path); "
+        raise ImportError("WORLD analysis/synthesis needs the `pyworld` package (CPU audio code, outside the GPU hot path); "
                           "feed pre-extracted MCEP matrices instead (see cgvc.convert / cgvc.train)") from e
 
 

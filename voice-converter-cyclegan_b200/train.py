@@ -213,7 +213,7 @@ def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epoc
 
 
 def main():
-    p = argparse.ArgumentParser(description='Train CycleGAN model on pre-extracted MCEP features (native B200 engine).')
+    p = argparse.ArgumentParser(description='Train CycleGAN model on pre-extracted MCEP features (native H100 engine).')
     p.add_argument('--train_A_dir', type=str, default='./data/mcep/SF1')
     p.add_argument('--train_B_dir', type=str, default='./data/mcep/TM1')
     p.add_argument('--model_dir', type=str, default='./model/sf1_tm1')
