@@ -181,7 +181,8 @@ int cgvc_kernel_launches(unsigned long long* count);
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
  * "debug_taps" (default 0): see cgvc_debug_activation.
  * "tc_debug" (default 0): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
- * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather. */
+ * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather.  The plain
+ * epilogue stores straight from the accumulator registers, so for it 2 acts as 1. */
 int cgvc_set_option(cgvc_handle h, const char* name, int value);
 int cgvc_profile_enable(int on);
 int cgvc_profile_collect(double* ms3, double* flops3, long long* launches3);

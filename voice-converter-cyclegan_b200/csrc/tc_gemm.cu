@@ -12,9 +12,10 @@
 //               into SWIZZLE_128B shared memory; one thread TMA-loads the weight (NT) / gradient (TN) tile; both complete on
 //               the stage's "full" mbarrier.
 //   warps 4-11  two consumer warpgroups, 64 accumulator rows each: wgmma from the shared-memory stages into registers, stages
-//               released through the "empty" mbarriers.  NT: the finished tile is passed through shared memory to the epilogue
-//               (bias / accumulate, the fused instance-norm (+GLU / +residual) forward epilogues, the opt-in fused backward
-//               epilogues), whose global stores are transposed through a per-warp patch so that 8 lanes write one row.
+//               released through the "empty" mbarriers.  NT: the plain epilogue (bias / accumulate) stores the accumulator
+//               fragments from registers; for the fused instance-norm (+GLU / +residual) forward epilogues and the opt-in fused
+//               backward epilogues the finished tile is passed through shared memory, and their global stores are transposed
+//               through a per-warp patch so that 8 lanes write one row.
 //               TN: red.global.add of the accumulator fragments into the weight gradient.
 #include "tc_gemm.cuh"
 #include "geom.h"
@@ -52,7 +53,8 @@ bool make_tmap3(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d1, uint
              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// same for any element type: tensor [d2][d1][d0] (d0 contiguous, esize bytes), box [1][b1][b0], SWIZZLE_128B (b0 * esize == 128)
+// same for any element type: tensor [d2][d1][d0] (d0 contiguous, esize bytes), box [1][b1][b0], rows of b0 * esize bytes (128 or 64,
+// the swizzle span: SWIZZLE_128B or SWIZZLE_64B)
 bool make_tmap3_t(CUtensorMap* m, const void* base, CUtensorMapDataType dt, int esize, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1) {
   EncodeTiledFn enc = get_encoder();
   if (!enc) return false;
@@ -61,7 +63,8 @@ bool make_tmap3_t(CUtensorMap* m, const void* base, CUtensorMapDataType dt, int 
   cuuint32_t box[3] = {b0, b1, 1};
   cuuint32_t es[3] = {1, 1, 1};
   return enc(m, dt, 3, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+             b0 * esize == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------------ PTX wrappers
@@ -104,10 +107,12 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 // Shared-memory matrix descriptor of wgmma, SWIZZLE_128B (layout type 1 in bits 62-63):
 //   K-major : 8-row groups of 128-byte rows, SBO = 1024 B between groups, LBO unused
 //   MN-major: atoms of (64 MN-elements x 8 K-rows) = 1024 B; LBO = stride between atoms along MN, SBO = along K
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// make_desc64: SWIZZLE_64B (layout type 2), K-major: 8-row groups of 64-byte rows, SBO = 512 B
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout = 1) {
   return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 62);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (layout << 62);
 }
+__device__ __forceinline__ uint64_t make_desc64(uint32_t smem_addr) { return make_desc(smem_addr, 16, 512, 2); }
 // keeps the compiler from moving accesses of the accumulator registers across the asynchronous wgmma
 template <int N>
 __device__ __forceinline__ void fence_acc(float (&d)[N]) {
@@ -156,7 +161,8 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   int N;                                                 // real output columns (stores are guarded; tiles cover Nw)
   int n_tiles;                                           // column tiles to compute (host: covers the real columns only)
   int debug;                                             // diagnostic knobs (tc_set_debug): 1 = epilogue skips its global stores, 2 = also skips
-                                                         // the accumulator reads, 4 = producers skip the A gather.  Results are garbage; timing only.
+                                                         // the accumulator reads (the plain epilogue reads registers only: 2 acts as 1 there),
+                                                         // 4 = producers skip the A gather.  Results are garbage; timing only.
   float* dst; int d_ld; const float* bias; int accumulate;
   int perm; int Cc;                                      // gated layers: weight rows / bias are stored tile-interleaved: tile j =
                                                          // [a-channels j*128..+127 | g-channels j*128..+127]; Cc = channels per branch
@@ -175,7 +181,7 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   CUtensorMap tm_b_hi, tm_b_lo;                          // TMA maps of the weight planes, box [1][BN][64]
   // F16F8 mode (NPL == 3, forward only): a_hi / tm_b_hi are the fp16 planes; the e4m3 planes of both operands:
   const uint8_t *a8_hi, *a8_lo;                          // [rows, a_ld] bytes
-  CUtensorMap tm_b8_hi, tm_b8_lo;                        // box [1][BN][128 bytes]
+  CUtensorMap tm_b8_hi, tm_b8_lo;                        // box [1][BN][64 bytes], SWIZZLE_64B
   uint8_t* y8;                                           // fused epilogues: q8hi plane of y [M, C_out] bytes, q8lo follows at + M * C_out (y_hi = q16)
 };
 
@@ -204,13 +210,16 @@ __device__ __forceinline__ float* tn_dst(float* base, int slab, int C, int c, in
 constexpr int kProducerThreads = 128;
 
 
+// Stages of 64 contraction channels.  F16F8 (NPL = 3) stages hold one 128-byte-row tile per operand, like NPL 1: an fp16 stage the
+// fp16 tiles; a cross-term stage the A rows as [64 a8_hi bytes | 64 a8_lo bytes] (SWIZZLE_128B) and the weight tile as two
+// SWIZZLE_64B tiles of 64-byte rows, b8_hi then b8_lo (TMA boxes of 64 bytes).
 template <int BN, int NPL>
 struct NTCfg {
   static constexpr int A_PLANE = 128 * 128;            // bytes: 128 rows x 128 B
   static constexpr int B_PLANE = BN * 128;
-  static constexpr int PLANES = NPL == 1 ? 1 : 2;       // F16F8 (NPL = 3) stages hold two 128-byte-row tiles per operand as well
+  static constexpr int PLANES = NPL == 2 ? 2 : 1;
   static constexpr int STAGE = PLANES * (A_PLANE + B_PLANE);
-  static constexpr int STAGES = (192 * 1024) / STAGE;   // 2 (BN=256,x3), 3 (128,x3), 4 (32,x3), 4 (256,x1), 6 (128,x1), 9 (32,x1)
+  static constexpr int STAGES = (192 * 1024) / STAGE;   // BN = 256 / 128 / 32: 2 / 3 / 4 (x3), 4 / 6 / 9 (x1, f16f8)
   static constexpr int SMEM = STAGES * STAGE + 1024;
   static_assert(STAGES * STAGE >= 128 * BN * 4, "the finished fp32 tile is staged over the pipeline stages");
 };
@@ -463,46 +472,7 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
   __syncwarp();
   rowp[lane] = drow;                                     // destination row of every tile row, for the write-back lanes
   __syncwarp();
-  if (EPI == 0) {
-#pragma unroll 1
-    for (int cb = grp; cb < BN / 32; cb += ngrp) {
-      const int nb = n0 + cb * 32;                         // column in weight-row (bias) order
-      if (nb >= p.Nw) break;
-      // gated layers store their weight rows tile-interleaved ([128 a | 128 g] per 256-wide tile): map back
-      // (shuffled gated layers: [64 a s0 | 64 a s1 | 64 g s0 | 64 g s1] for 64 post-shuffle channels, see EPI 5)
-      const int n = p.perm == 2 ? ((cb >> 2) * p.Cc + ((cb >> 1) & 1) * (p.Cc >> 1) + (n0 >> 2) + (cb & 1) * 32)
-                  : p.perm      ? ((cb < 4) ? (n0 >> 1) + cb * 32 : p.Cc + (n0 >> 1) + (cb - 4) * 32) : nb;
-      if (n >= p.N) { if (p.perm) continue; else break; }  // warp-uniform
-      if (p.debug & 2) continue;
-      float o[32];
-      { uint32_t v[32]; acc_ld32<BN>(acc, arow, (cb * 32), v);
-#pragma unroll
-        for (int k = 0; k < 32; ++k) o[k] = __uint_as_float(v[k]); }
-      if (p.bias) {
-#pragma unroll
-        for (int k = 0; k < 32; k += 4) { float4 bb = *reinterpret_cast<const float4*>(p.bias + nb + k); o[k] += bb.x; o[k + 1] += bb.y; o[k + 2] += bb.z; o[k + 3] += bb.w; }
-      }
-      if (!(p.debug & 1))
-        rows_out(stg, o, lane, [&](int rr, int w0, float4 val) {
-          float* rp = rowp[rr];
-          const int col = n + w0;                          // padded columns are never stored
-          if (rp != nullptr && col < p.N) {
-            if (col + 4 <= p.N && (p.d_ld & 3) == 0) {
-              if (p.accumulate)
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(rp + col), "f"(val.x), "f"(val.y), "f"(val.z), "f"(val.w) : "memory");
-              else
-                *reinterpret_cast<float4*>(rp + col) = val;
-            } else {                                       // a data gradient with cin % 4 != 0 (the discriminator's one-channel input)
-              const float v4[4] = {val.x, val.y, val.z, val.w};
-              for (int k = 0; k < 4 && col + k < p.N; ++k) {
-                if (p.accumulate) atomicAdd(rp + col + k, v4[k]);
-                else rp[col + k] = v4[k];
-              }
-            }
-          }
-        });
-    }
-  } else {
+  {
     // ---- fused forward epilogue: the 128 rows of the tile are whole samples of R positions (R = 32, 64, 128) ----
     const int spw = p.R >> 5;                              // warps per sample
     const long long sample = mq / p.R;
@@ -771,16 +741,14 @@ __device__ __forceinline__ void consume_stages(float (&d)[BN / 2], int nkb, int&
     if constexpr (TN == 0) {
       if constexpr (KIND == MMA_E4M3_CROSS) {                // K = 32 e4m3 per instruction: a8_hi x b8_lo + a8_lo x b8_hi
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          wgmma_e4m3<BN>(d, make_desc(sA + k * 32, 16, 1024), make_desc(sB + Cfg::B_PLANE + k * 32, 16, 1024), 1);
-          wgmma_e4m3<BN>(d, make_desc(sA + Cfg::A_PLANE + k * 32, 16, 1024), make_desc(sB + k * 32, 16, 1024), 1);
+        for (int k = 0; k < 2; ++k) {
+          wgmma_e4m3<BN>(d, make_desc(sA + k * 32, 16, 1024), make_desc64(sB + Cfg::B_PLANE / 2 + k * 32), 1);
+          wgmma_e4m3<BN>(d, make_desc(sA + 64 + k * 32, 16, 1024), make_desc64(sB + k * 32), 1);
         }
-      } else if constexpr (KIND == MMA_F16) {                // fp16 hi x hi, two 64-channel tiles of K = 16 steps
+      } else if constexpr (KIND == MMA_F16) {                // fp16 hi x hi, one 64-channel tile of K = 16 steps
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            wgmma_f16<BN, 0, 0>(d, make_desc(sA + h * Cfg::A_PLANE + k * 32, 16, 1024), make_desc(sB + h * Cfg::B_PLANE + k * 32, 16, 1024), 1);
+        for (int k = 0; k < 4; ++k)
+          wgmma_f16<BN, 0, 0>(d, make_desc(sA + k * 32, 16, 1024), make_desc(sB + k * 32, 16, 1024), 1);
       } else {
 #pragma unroll
         for (int k = 0; k < 4; ++k) {                        // K = 16 bf16 = 32 bytes along the swizzled row
@@ -829,14 +797,64 @@ __device__ __forceinline__ void rescale_acc(float (&d)[N], float scale) {
   for (int i = 0; i < N; ++i) d[i] *= scale;
 }
 
+// ---- plain epilogue (EPI 0) straight from the accumulator fragments ----------------------------------------------------------
+// This thread's fragments are tile rows r and r + 8, columns 8 j + c + {0, 1} of every 8-column block j (c = 2 (t % 4)).  y = D (+ bias),
+// stored or (accumulate) added.  One float2 store of a warp covers 8 rows x 32 contiguous bytes: whole sectors.  Nothing passes through
+// the pipeline stages, so the producers fill them with the next tile's operands meanwhile.
+template <int BN>
+__device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const float (&d)[BN / 2], const long long M, const int HW,
+                                                   const long long m0, const int n0, const int r, const int c) {
+  const GatherGeom& g = p.g;
+  float* rowp[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const long long m = m0 + r + 8 * h;
+    rowp[h] = nullptr;
+    if (m < M && p.dst) {
+      int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
+      int y = rem / g.Wx; int x = rem - y * g.Wx;
+      rowp[h] = p.dst + ((long long)(b * g.Hd + y * g.dsy + g.doy) * g.Wd + x * g.dsx + g.dox) * p.d_ld;
+    }
+  }
+  const bool vec = (p.d_ld & 1) == 0;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int cb = j >> 2;                                   // 32-column block of the tile
+    // gated layers store their weight rows tile-interleaved ([128 a | 128 g] per 256-wide tile): map back
+    // (shuffled gated layers: [64 a s0 | 64 a s1 | 64 g s0 | 64 g s1] for 64 post-shuffle channels, see EPI 5)
+    const int n = (p.perm == 2 ? (cb >> 2) * p.Cc + ((cb >> 1) & 1) * (p.Cc >> 1) + (n0 >> 2) + (cb & 1) * 32
+                   : p.perm    ? ((cb < 4) ? (n0 >> 1) + cb * 32 : p.Cc + (n0 >> 1) + (cb - 4) * 32) : n0 + cb * 32) + ((8 * j) & 31) + c;
+    if (n >= p.N) continue;                                  // padded columns are never stored
+    float2 bb = make_float2(0.f, 0.f);
+    if (p.bias) bb = *reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + c);   // bias in weight-row order
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float* rp = rowp[h];
+      if (rp == nullptr) continue;
+      float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+      if (p.bias) { v0 += bb.x; v1 += bb.y; }
+      if (vec && n + 2 <= p.N) {
+        if (p.accumulate)
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(rp + n), "f"(v0), "f"(v1) : "memory");
+        else
+          *reinterpret_cast<float2*>(rp + n) = make_float2(v0, v1);
+      } else {                                               // a data gradient with an odd cin (the discriminator's one-channel input)
+        if (p.accumulate) atomicAdd(rp + n, v0); else rp[n] = v0;
+        if (n + 1 < p.N) { if (p.accumulate) atomicAdd(rp + n + 1, v1); else rp[n + 1] = v1; }
+      }
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ NT kernel
 // Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... (m fastest, so CTAs that run
 // concurrently share the weight tile in L2).  384 threads:
 //   warps 0-3   producers (A rows by cp.async, weight tile by TMA), running ahead across K-blocks
-//   warps 4-11  two consumer warpgroups: wgmma of tile rows 64 wg .. + 63 into registers (BN / 2 per thread); then the whole tile
-//               is written to shared memory over the pipeline stages -- they hold nothing at that point, because the producers
-//               wait for the epilogue of a tile before they load the next one -- and the 8 warps run the epilogue in two groups
-//               of 4.  (The accumulator of a 256-wide tile does not fit next to the stages: 128 KB.)
+//   warps 4-11  two consumer warpgroups: wgmma of tile rows 64 wg .. + 63 into registers (BN / 2 per thread).  The plain epilogue
+//               (EPI 0) stores the fragments from registers (nt_store_fragments) while the producers already load the next tile.
+//               The fused epilogues write the whole tile to shared memory over the pipeline stages -- they hold nothing at that
+//               point, because the producers wait for the epilogue of a tile before they load the next one -- and the 8 warps run
+//               the epilogue in two groups of 4.  (The accumulator of a 256-wide tile does not fit next to the stages: 128 KB.)
 constexpr int kNTThreads = 384;
 
 template <int BN, int NPL, int EPI>
@@ -856,9 +874,9 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   const GatherGeom& g = p.g;
   const long long M = (long long)g.B * g.Hy * g.Wx;
   const int HW = g.Hy * g.Wx;
-  // K blocks ("stages"): 64 channels each; F16F8 walks the contraction twice with 128 channels per stage -- first the two
-  // fp8 cross products (planes a8_hi x b8_lo and a8_lo x b8_hi), then the fp16 hi x hi product after the rescale of D
-  const int cchunks = NPL == 3 ? (p.C >> 7) : (p.C >> 6);
+  // K blocks ("stages"): 64 channels each; F16F8 walks the contraction twice -- first the two fp8 cross products (planes
+  // a8_hi x b8_lo and a8_lo x b8_hi), then the fp16 hi x hi product after the rescale of D
+  const int cchunks = p.C >> 6;
   const int kb_pass = g.ntaps * cchunks;
   const int num_kb = NPL == 3 ? 2 * kb_pass : kb_pass;     // > 0 (the host never launches an empty contraction)
   const int m_tiles = (int)((M + 127) / 128);
@@ -886,7 +904,7 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const long long m0 = (long long)(tile % m_tiles) * 128;
       const int n0 = (tile / m_tiles) * BN;
-      if (it > 0) mbar_wait(&acc_free_bar, (uint32_t)(it - 1) & 1u);   // the previous tile's epilogue has left the stages
+      if (EPI != 0 && it > 0) mbar_wait(&acc_free_bar, (uint32_t)(it - 1) & 1u);   // the previous tile's epilogue has left the stages
       int rb[8], ry[8], rx[8];                              // decoded output coordinates of this thread's 8 A rows
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -904,22 +922,21 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
         for (int i = 0; i < 8; ++i) {
           int yy = ry[i] + g.oy[tap], xx = rx[i] + g.ox[tap];
           bool ok = rb[i] >= 0 && yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws;
-          aoff[i] = ok ? ((long long)(rb[i] * g.Hs + yy) * g.Ws + xx) * p.a_ld + chunk * (NPL == 3 && pass == 0 ? 16 : 8) : -1;
+          aoff[i] = ok ? ((long long)(rb[i] * g.Hs + yy) * g.Ws + xx) * p.a_ld + (NPL == 3 && pass == 0 ? (chunk & 3) * 16 : chunk * 8) : -1;
         }
         for (int cc = 0; cc < cchunks; ++cc) {
-          const int c0 = NPL == 3 ? (cc << 7) : (cc << 6);
+          const int c0 = cc << 6;
           mbar_wait(&empty_bar[stage], phase ^ 1);
           const uint32_t sA = smem_base + stage * Cfg::STAGE;
           const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
-          if (t == 0) {                                      // weight tile [BN rows n][128 bytes of c] by TMA (hardware 128B swizzle)
+          if (t == 0) {                                      // weight tile [BN rows n][128 bytes of c] by TMA (hardware swizzle)
             mbar_expect_tx(&full_bar[stage], Cfg::PLANES * Cfg::B_PLANE);
             if (NPL == 3) {
-              if (pass == 0) {
+              if (pass == 0) {                               // e4m3: two tiles of 64-byte rows
                 tma_load3(sB, &p.tm_b8_hi, c0, n0, g.widx[tap], &full_bar[stage]);
-                tma_load3(sB + Cfg::B_PLANE, &p.tm_b8_lo, c0, n0, g.widx[tap], &full_bar[stage]);
-              } else {                                       // fp16: two 64-channel tiles
+                tma_load3(sB + Cfg::B_PLANE / 2, &p.tm_b8_lo, c0, n0, g.widx[tap], &full_bar[stage]);
+              } else {
                 tma_load3(sB, &p.tm_b_hi, c0, n0, g.widx[tap], &full_bar[stage]);
-                tma_load3(sB + Cfg::B_PLANE, &p.tm_b_hi, c0 + 64, n0, g.widx[tap], &full_bar[stage]);
               }
             } else {
               tma_load3(sB, &p.tm_b_hi, c0, n0, g.widx[tap], &full_bar[stage]);
@@ -934,13 +951,10 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
               const bool ok = aoff[i] >= 0;
               const long long off = ok ? aoff[i] + c0 : 0;
               if (NPL == 3) {
-                if (pass == 0) {                             // 128 e4m3 bytes per row and plane
-                  cp_async16(sA + so, p.a8_hi + off, ok ? 16u : 0u);
-                  cp_async16(sA + Cfg::A_PLANE + so, p.a8_lo + off, ok ? 16u : 0u);
-                } else {                                     // 2 x 64 fp16 per row
+                if (pass == 0)                               // row = [64 a8_hi bytes | 64 a8_lo bytes]
+                  cp_async16(sA + so, (chunk < 4 ? p.a8_hi : p.a8_lo) + off, ok ? 16u : 0u);
+                else                                         // 64 fp16
                   cp_async16(sA + so, p.a_hi + off, ok ? 16u : 0u);
-                  cp_async16(sA + Cfg::A_PLANE + so, p.a_hi + off + 64, ok ? 16u : 0u);
-                }
               } else {
                 cp_async16(sA + so, p.a_hi + off, ok ? 16u : 0u);
                 if (NPL == 2) cp_async16(sA + Cfg::A_PLANE + so, p.a_lo + off, ok ? 16u : 0u);
@@ -976,21 +990,25 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
       wgmma_wait<0>();
       fence_acc(d);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      // the tile into shared memory once both warpgroups are done reading the stages
-      consumer_bar();
-      if (!(p.debug & 2)) {
-        const int r0 = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2), c0 = 2 * (tw & 3);
+      const int r0 = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2), c0 = 2 * (tw & 3);   // this thread's fragment rows r0, r0 + 8
+      if constexpr (EPI == 0) {
+        if (!(p.debug & 3)) nt_store_fragments<BN>(p, d, M, HW, m0, n0, r0, c0);
+      } else {
+        // the tile into shared memory once both warpgroups are done reading the stages
+        consumer_bar();
+        if (!(p.debug & 2)) {
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(acc_s + acc_off<BN>(r0, 8 * j + c0)) = make_float2(d[4 * j], d[4 * j + 1]);
-          *reinterpret_cast<float2*>(acc_s + acc_off<BN>(r0 + 8, 8 * j + c0)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+          for (int j = 0; j < BN / 8; ++j) {
+            *reinterpret_cast<float2*>(acc_s + acc_off<BN>(r0, 8 * j + c0)) = make_float2(d[4 * j], d[4 * j + 1]);
+            *reinterpret_cast<float2*>(acc_s + acc_off<BN>(r0 + 8, 8 * j + c0)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+          }
         }
+        consumer_bar();
+        nt_tile_epilogue<BN, NPL, EPI>(p, M, HW, m0, n0, cw & 3, lane, epi_stage[cw], epi_rowp[cw], epi_bc[cw], epi_xch[wg], acc_s, wg, 2);
+        fence_proxy_async();                                 // generic accesses of the stages before the next tile's TMA writes
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&acc_free_bar);
       }
-      consumer_bar();
-      nt_tile_epilogue<BN, NPL, EPI>(p, M, HW, m0, n0, cw & 3, lane, epi_stage[cw], epi_rowp[cw], epi_bc[cw], epi_xch[wg], acc_s, wg, 2);
-      fence_proxy_async();                                   // generic accesses of the stages before the next tile's TMA writes
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_free_bar);
     }
   }
 }
@@ -1002,24 +1020,26 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
 // both cross products x8hi * g8lo and x8lo * g8hi carry 2^12.  Unless p.w16 is set, the row range of a work item is walked twice:
 // first the cross products -- e4m3 wgmma reads K-major operands only, and both operands are MN-major here, so the producers widen
 // the e4m3 tiles to fp16 (exactly) on their way into shared memory and the products run as fp16 MMAs --, then the accumulator is
-// rescaled by 2^-12 and the fp16 hi x hi products follow.
+// rescaled by 2^-12 and the fp16 hi x hi products follow.  W16 (selected by p.w16) is the fp16-only form: its stages hold one plane
+// per operand, so twice as many fit.
 #define CGVC_Q_WGRAD_SHIFT 12
-template <int NPL>
+template <int NPL, int W16>
 struct TNCfg {
   static constexpr int A_PLANE = 64 * 256;              // 64 K-rows x 128 channels x 2 B  (2 MN-atoms side by side: LBO = 8192)
   static constexpr int B_PLANE = 64 * 512;              // 64 K-rows x 256 columns x 2 B  (4 MN-atoms: LBO = 8192)
-  static constexpr int PLANES = NPL == 1 ? 1 : 2;
+  static constexpr int PLANES = (NPL == 1 || W16) ? 1 : 2;
   static constexpr int STAGE = PLANES * (A_PLANE + B_PLANE);
-  static constexpr int STAGES = (192 * 1024) / STAGE;   // 2 (x3, f16f8), 4 (x1)
+  static constexpr int STAGES = (192 * 1024) / STAGE;   // 2 (x3, f16f8), 4 (x1, f16f8 with W16)
   static constexpr int SMEM = STAGES * STAGE + 1024;
 };
 
 // Persistent like the NT kernel: work items (n-tile, c-tile, tap, K-split) are walked with stride gridDim.x (n fastest, so
 // concurrently running CTAs share the same rows of X and dP in L2).  Each consumer warpgroup owns 64 of the 128 channels.
-template <int NPL>
+template <int NPL, int W16>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
-  using Cfg = TNCfg<NPL>;
+  static_assert(W16 == 0 || NPL == 3, "the fp16-only weight gradient is a form of CGVC_PREC_F16F8");
+  using Cfg = TNCfg<NPL, W16>;
   constexpr int S = Cfg::STAGES;
   constexpr int BN = 256;
   extern __shared__ uint8_t smem_raw[];
@@ -1032,7 +1052,7 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   const int HW = g.Hy * g.Wx;
   const int n_tiles = (p.g_ld + BN - 1) / BN, c_tiles = (p.x_ld + 127) / 128;
   const int num_items = n_tiles * c_tiles * g.ntaps * p.ksplit;
-  const int pass0 = (NPL == 3 && !p.w16) ? 0 : 1;         // pass 0: the F16F8 cross products; pass 1: the main products
+  constexpr int pass0 = (NPL == 3 && !W16) ? 0 : 1;       // pass 0: the F16F8 cross products; pass 1: the main products
   long long chunk_rows = (M + p.ksplit - 1) / p.ksplit;
   chunk_rows = (chunk_rows + 63) / 64 * 64;
 
@@ -1157,9 +1177,11 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       int prev = -1;
-      if constexpr (NPL == 3) {                             // (with w16 the cross-product walk is empty and the rescale acts on zeros)
-        consume_stages<BN, MMA_F16_CROSS, 1, Cfg>(d, pass0 == 0 ? w.num_kb : 0, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+      if constexpr (NPL == 3 && !W16) {
+        consume_stages<BN, MMA_F16_CROSS, 1, Cfg>(d, w.num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
         rescale_acc(d, 1.f / (float)(1 << CGVC_Q_WGRAD_SHIFT));
+        consume_stages<BN, MMA_F16, 1, Cfg>(d, w.num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+      } else if constexpr (NPL == 3) {
         consume_stages<BN, MMA_F16, 1, Cfg>(d, w.num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
       } else {
         consume_stages<BN, NPL == 2 ? MMA_BF16X3 : MMA_BF16, 1, Cfg>(d, w.num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
@@ -1462,16 +1484,16 @@ cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st) {
   cudaError_t e;
   ++g_cgvc_launches;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, 1, M, p.N, p.g.ntaps * p.C);
-  if (precision == 3) {
-    e = set_smem(tc_gg_tn_kernel<3>, TNCfg<3>::SMEM); if (e != cudaSuccess) return e;
-    tc_gg_tn_kernel<3><<<grid, kNTThreads, TNCfg<3>::SMEM, st>>>(p);
-  } else if (precision == 1) {
-    e = set_smem(tc_gg_tn_kernel<2>, TNCfg<2>::SMEM); if (e != cudaSuccess) return e;
-    tc_gg_tn_kernel<2><<<grid, kNTThreads, TNCfg<2>::SMEM, st>>>(p);
-  } else {
-    e = set_smem(tc_gg_tn_kernel<1>, TNCfg<1>::SMEM); if (e != cudaSuccess) return e;
-    tc_gg_tn_kernel<1><<<grid, kNTThreads, TNCfg<1>::SMEM, st>>>(p);
-  }
+#define LAUNCH_TN(NPL_, W16_)                                                                     \
+  do {                                                                                            \
+    e = set_smem(tc_gg_tn_kernel<NPL_, W16_>, TNCfg<NPL_, W16_>::SMEM);                           \
+    if (e != cudaSuccess) return e;                                                               \
+    tc_gg_tn_kernel<NPL_, W16_><<<grid, kNTThreads, TNCfg<NPL_, W16_>::SMEM, st>>>(p);            \
+  } while (0)
+  if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1); else LAUNCH_TN(3, 0); }
+  else if (precision == 1) LAUNCH_TN(2, 0);
+  else                     LAUNCH_TN(1, 0);
+#undef LAUNCH_TN
   prof_end(st);
   return cudaGetLastError();
 }
@@ -1517,12 +1539,12 @@ bool make_layer_maps_q(TcLayer& L) {
   const int bf = tile_rows(Ntot(L), nt_n(L)), bd = tile_rows(L.cin, cin_n(L));
   const CUtensorMapDataType F16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16, U8 = CU_TENSOR_MAP_DATA_TYPE_UINT8;
   bool ok = make_tmap3_t(&L.tm_q16, L.wq16, F16, 2, cin_q(L), nt_n(L), taps, 64, bf) &&
-            make_tmap3_t(&L.tm_q8hi, L.wq8hi, U8, 1, cin_q(L), nt_n(L), taps, 128, bf) &&
-            make_tmap3_t(&L.tm_q8lo, L.wq8lo, U8, 1, cin_q(L), nt_n(L), taps, 128, bf);
+            make_tmap3_t(&L.tm_q8hi, L.wq8hi, U8, 1, cin_q(L), nt_n(L), taps, 64, bf) &&
+            make_tmap3_t(&L.tm_q8lo, L.wq8lo, U8, 1, cin_q(L), nt_n(L), taps, 64, bf);
   if (ok && L.wdq16)
     ok = make_tmap3_t(&L.tm_dq16, L.wdq16, F16, 2, nt_q(L), cin_n(L), taps, 64, bd) &&
-         make_tmap3_t(&L.tm_dq8hi, L.wdq8hi, U8, 1, nt_q(L), cin_n(L), taps, 128, bd) &&
-         make_tmap3_t(&L.tm_dq8lo, L.wdq8lo, U8, 1, nt_q(L), cin_n(L), taps, 128, bd);
+         make_tmap3_t(&L.tm_dq8hi, L.wdq8hi, U8, 1, nt_q(L), cin_n(L), taps, 64, bd) &&
+         make_tmap3_t(&L.tm_dq8lo, L.wdq8lo, U8, 1, nt_q(L), cin_n(L), taps, 64, bd);
   return ok;
 }
 
@@ -1740,9 +1762,9 @@ static cudaError_t tc_init_kernels() {
   INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4) INIT_NT(256, 2, 5) INIT_NT(256, 1, 5)
   INIT_NT(256, 3, 0) INIT_NT(128, 3, 0) INIT_NT(32, 3, 0) INIT_NT(256, 3, 1) INIT_NT(256, 3, 2) INIT_NT(256, 3, 5)
 #undef INIT_NT
-  if ((e = set_smem(tc_gg_tn_kernel<3>, TNCfg<3>::SMEM)) != cudaSuccess) return e;
-  if ((e = set_smem(tc_gg_tn_kernel<2>, TNCfg<2>::SMEM)) != cudaSuccess) return e;
-  if ((e = set_smem(tc_gg_tn_kernel<1>, TNCfg<1>::SMEM)) != cudaSuccess) return e;
+#define INIT_TN(NPL_, W16_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
+  INIT_TN(3, 1) INIT_TN(3, 0) INIT_TN(2, 0) INIT_TN(1, 0)
+#undef INIT_TN
   return cudaSuccess;
 }
 
