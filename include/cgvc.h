@@ -109,6 +109,16 @@ int cgvc_adam_step(cgvc_handle h, float lr_generator, float lr_discriminator, fl
  * anything else returns CGVC_ERR_DIRECTION ("Conversion direction must be specified.", model.py:135). */
 int cgvc_generator_forward(cgvc_handle h, int direction, const float* in_dev, float* out_dev,
                            int batch, int frames, void* stream);
+/* generator forward of n utterances of different lengths in one call (conversion): utterance u is the row-major
+ * [num_features][len_u] block at element num_features * offsets_host[u] of in_dev, and its converted block lands at the same place
+ * in out_dev -- the corpus layout of cgvc_sample_plan.  offsets_host: n + 1 int64 frame prefix sums, offsets_host[0] = 0, every
+ * len_u = offsets_host[u+1] - offsets_host[u] a positive multiple of 4.  Needs n <= max_batch and offsets_host[n] <= max_batch *
+ * max_frames.  Every utterance's result is what cgvc_generator_forward gives for it alone, up to the summation order of its
+ * instance-norm statistics.  Bad offsets, n or capacity return CGVC_ERR_ARG naming the offending utterance; the offsets are copied
+ * to the device on the stream before the call returns.  With "debug_taps" a tap holds the concatenated rows of all utterances at
+ * that layer's resolution (d2: offsets_host[n] / 4 x 512 elements). */
+int cgvc_generator_forward_packed(cgvc_handle h, int direction, const float* in_dev, float* out_dev,
+                                  const long long* offsets_host, int n, void* stream);
 /* discriminator forward, which 0 = discriminator_A, 1 = discriminator_B: out [batch, 6, frames/16] (module.py:188-213) */
 int cgvc_discriminator_forward(cgvc_handle h, int which, const float* in_dev, float* out_dev,
                                int batch, int frames, void* stream);

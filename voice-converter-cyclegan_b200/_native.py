@@ -52,6 +52,7 @@ def _declare(lib):
         "cgvc_compute_gradients": (ci, [vp, vp, vp, ci, ci, cf, cf, vp, vp, vp, vp]),
         "cgvc_adam_step": (ci, [vp, cf, cf, cf, vp]),
         "cgvc_generator_forward": (ci, [vp, ci, vp, vp, ci, ci, vp]),
+        "cgvc_generator_forward_packed": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp]),
         "cgvc_discriminator_forward": (ci, [vp, ci, vp, vp, ci, ci, vp]),
         "cgvc_debug_activation": (ci, [vp, C.c_char_p, vp, sz, P(sz), vp]),
         "cgvc_comm_unique_id": (ci, [vp, vp]),

@@ -14,8 +14,9 @@ What differs, and why:
     one `.npz` per utterance holding `f0` [T], `coded_sp` [T, 24] and optionally `ap`, as `world_decompose` +
     `world_encode_spectral_envelop` produce them.  The output is an `.npz` with `f0`, `coded_sp` (converted) and `ap`.
   * utterances are BATCHED: all utterances are padded to T % 4 == 0 (edge frames replicated, cropped off again after the
-    generator), grouped by padded length, and each group goes through `model.test` in batches bounded by a frame budget
-    (instance norm is per sample, so batching does not change any result); the engine is sized once for the whole job.
+    generator) and go through `model.test_packed` in chunks of any lengths bounded by an utterance count and a frame budget
+    (convolutions and instance norm stay within each utterance, so batching does not change any result); models without
+    `test_packed` get groups of equal padded length through `model.test`.  The engine is sized once for the whole job.
 
     python -m cgvc.convert --model_dir ./model/sf1_tm1 --model_name sf1_tm1.ckpt --data_dir ./features/SF1 --conversion_direction A2B
 """
@@ -79,6 +80,29 @@ def plan_groups(lengths, max_group=256, frame_budget=65536):
     return plan
 
 
+def plan_chunks(lengths, max_group=256, frame_budget=65536):
+    """Consecutive runs of utterance indices for packed generator calls (`model.test_packed`): a chunk holds at most `max_group`
+    utterances and `frame_budget` frames; an utterance longer than the budget gets a chunk of its own."""
+    plan, cur, frames = [], [], 0
+    for i, n in enumerate(lengths):
+        if cur and (len(cur) == max_group or frames + n > frame_budget):
+            plan.append(cur)
+            cur, frames = [], 0
+        cur.append(i)
+        frames += n
+    if cur:
+        plan.append(cur)
+    return plan
+
+
+def _special_norm_length(T):
+    """Whether the engine's forward of one T-frame utterance runs an instance norm through a kernel specialised for its positions per
+    sample: the fused GEMM epilogues (32, 64 or 128) or the streaming one-pass kernels (32, 48, 64, 96, 128 or 384), at the T, T/2 or
+    T/4 level.  `model.test` then sums the statistics in another order than `model.test_packed`, which moves results by about 1e-5,
+    so conversion keeps such utterances on the length-grouped path; for every other length the two paths agree bit for bit."""
+    return any(T % d == 0 and T // d in (32, 48, 64, 96, 128, 384) for d in (1, 2, 4))
+
+
 def convert_features(model, coded_sps, direction, mcep_stats, max_group=256, frame_budget=65536):
     """Convert a list of MCEP matrices (each [T_i, 24], time-major like pyworld returns them).
 
@@ -93,18 +117,40 @@ def convert_features(model, coded_sps, direction, mcep_stats, max_group=256, fra
     for c in coded_sps:
         x, left = _pad_frames(np.asarray(c, dtype=np.float64).T, 4)          # [24, T']
         padded.append(x); lefts.append(left)
-    plan = plan_groups([c.shape[1] for c in padded], max_group, frame_budget)
+    out = [None] * len(padded)
+
+    def crop(i, y):
+        T = np.asarray(coded_sps[i]).shape[0]
+        conv = (y.astype(np.float64) * std_t + mean_t).T                     # [T', 24]
+        out[i] = np.ascontiguousarray(conv[lefts[i]:lefts[i] + T])
+
+    grouped = list(range(len(padded)))
+    if hasattr(model, "test_packed"):
+        # utterances of any lengths share one generator call: a few large GEMMs instead of one small call per length
+        packed = [i for i in grouped if not (hasattr(model, "test") and _special_norm_length(padded[i].shape[1]))]
+        grouped = sorted(set(grouped) - set(packed))
+        lengths = [padded[i].shape[1] for i in packed]
+        chunks = [[packed[j] for j in ch] for ch in plan_chunks(lengths, max_group, frame_budget)]
+        if chunks and hasattr(model, "_ensure_capacity"):
+            # one size for the whole job: the engine takes a chunk when n <= max_batch and its frames <= max_batch * max_frames
+            batch = max(len(ch) for ch in chunks)
+            frames = max(sum(padded[i].shape[1] for i in ch) for ch in chunks)
+            model._ensure_capacity(batch, max(16, -(-frames // (4 * batch)) * 4))
+        for part in chunks:
+            ys = model.test_packed([(padded[i] - mean_s) / std_s for i in part], direction)
+            for i, y in zip(part, ys):
+                crop(i, y)
+        if not grouped:
+            return out
+    plan = [(f, [grouped[j] for j in part]) for f, part in plan_groups([padded[i].shape[1] for i in grouped], max_group, frame_budget)]
     if plan and hasattr(model, "_ensure_capacity"):
         # size the engine once for the whole job (its workspace is re-planned, never re-allocated, per call)
         model._ensure_capacity(max(len(part) for _, part in plan), max(frames for frames, _ in plan))
-    out = [None] * len(padded)
     for frames, part in plan:
         x = np.stack([(padded[i] - mean_s) / std_s for i in part])           # [n, 24, T']
         y = model.test(inputs=x, direction=direction)
         for j, i in enumerate(part):
-            T = np.asarray(coded_sps[i]).shape[0]
-            conv = (y[j].astype(np.float64) * std_t + mean_t).T              # [T', 24]
-            out[i] = np.ascontiguousarray(conv[lefts[i]:lefts[i] + T])
+            crop(i, y[j])
     return out
 
 

@@ -39,6 +39,9 @@ struct DiscNet { Gated h1; Gated d[3]; size_t dense_k, dense_b; size_t begin, en
 struct GLAct { float* P; float* stats; float* Y; __nv_bfloat16 *Yhi, *Ylo; };
 struct GenActs {
   int n, T;
+  const long long* off;         // packed utterances (cgvc_generator_forward_packed): n + 1 device frame prefix sums, else null
+  long long rows;               // rows at full resolution: n * T, or off[n]
+  int max_len;                  // packed: the longest utterance
   const float* x_cl; __nv_bfloat16 *xhi, *xlo;
   __nv_bfloat16 *xchi, *xclo;   // im2col of the input over h1's taps: operand planes [n*T, ru128(kw*F)] (edge_lower)
   float* z;                     // o1's per-tap products [n*T, kw*F] before the tap-shifted sum (edge_lower)
@@ -239,6 +242,7 @@ static void build_discriminator(TableBuilder& tb, DiscNet& d) {
 struct ConvIO {               // one convolution application
   const float* x; const __nv_bfloat16 *xhi, *xlo;   // input [n,H,W,Cin] fp32 (may be null on the tensor-core path) + bf16 planes
   int n, H, W;
+  PackGeom pk{};              // packed utterances (pk.off != null): n = H = 1, W = rows at the level of divisor pk.div
 };
 
 static int conv_out_dims(const ConvW& c, int sh, int sw, int H, int W, int& Ho, int& Wo) {
@@ -254,8 +258,15 @@ static int conv_fwd_simt(cgvc_engine* e, const float* Pm, const ConvW& c, int sh
   op.src = io.x; op.s_ld = c.cin; op.s_coff = 0; op.C = c.cin;
   op.w = Pm + c.k; op.w_ts = (long long)c.cin * c.cout; op.w_cs = c.cout; op.w_ns = 1; op.N = c.cout;
   op.dst = dst; op.d_ld = ld; op.d_coff = coff; op.bias = Pm + c.b; op.accumulate = 0;
-  CK(launch_gg_simt(g, op, st));
+  if (io.pk.off) CK(launch_gg_simt_packed(g, op, io.pk, st));
+  else CK(launch_gg_simt(g, op, st));
   return 0;
+}
+
+// one tensor-core forward convolution of a layer over io (packed or dense geometry), plain epilogue
+static int tc_fwd_io(cgvc_engine* e, int slot, const ConvIO& io, int sh, int sw, float* P, cudaStream_t st) {
+  if (io.pk.off) return tc_conv_fwd_packed(e->tcw, slot, e->cfg.precision, io.xhi, io.xlo, io.W, sw, io.pk, P, st);
+  return tc_conv_fwd(e->tcw, slot, e->cfg.precision, io.xhi, io.xlo, io.n, io.H, io.W, sh, sw, P, st);
 }
 
 // dx (+)= dgrad(dy[., coff:coff+cout], w)
@@ -297,11 +308,11 @@ static bool use_tc(const cgvc_engine* e, int slot) { return slot >= 0 && tc_enab
 // gated layer: conv_a || conv_g -> P [rows, 2*cout]
 static int gated_conv_fwd(cgvc_engine* e, const Gated& L, const ConvIO& io, float* P, cudaStream_t st) {
   if (use_tc(e, L.tc_slot) && io.xhi) {
-    int r = tc_conv_fwd(e->tcw, L.tc_slot, e->cfg.precision, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, P, st);
+    int r = tc_fwd_io(e, L.tc_slot, io, L.sh, L.sw, P, st);
     if (r == 0) return 0;
     if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc_conv_fwd failed: %s", cudaGetErrorString((cudaError_t)r));
   }
-  if (L.a.cin == 1 && io.x && L.a.cout % 4 == 0 && 256 % (L.a.cout / 2) == 0) {   // discriminator h1: HBM-bound special
+  if (L.a.cin == 1 && io.x && !io.pk.off && L.a.cout % 4 == 0 && 256 % (L.a.cout / 2) == 0) {   // discriminator h1: HBM-bound special
     GatherGeom g = fwd_geom(io.n, io.H, io.W, L.a.kh, L.a.kw, L.sh, L.sw);
     const float* Pm = e->P();
     CK(launch_conv_c1_fwd(g, io.x, Pm + L.a.k, Pm + L.g.k, Pm + L.a.b, Pm + L.g.b, L.a.cout, P, st));
@@ -351,12 +362,23 @@ static PostParams post_params(const cgvc_engine* e, const Gated& L, const GLAct&
   return q;
 }
 
+// Packed utterances (G.off): q was built for one sample holding all q.R view rows.  Instance norm then runs per utterance over its
+// own view rows; the GLU-only layer is row-local and keeps that view.
+static void pack_post(PostParams& q, const GenActs& G) {
+  if (!G.off || !q.has_in) return;
+  const long long view_rows = q.R;
+  const int div = (int)(G.rows / view_rows);
+  q.seg = PackGeom{G.off, G.n, div, G.max_len}; q.seg_rows = view_rows;
+  q.B = G.n; q.R = G.max_len / div;
+}
+
 // gated layer forward with instance norm + GLU fused into the GEMM epilogue when the tensor-core path can (1-D layer whose
-// 128-row tiles hold whole samples); otherwise conv kernel + the two streaming instance-norm kernels
+// 128-row tiles hold whole samples); otherwise conv kernel + the two streaming instance-norm kernels.  G: the generator's
+// activations when io is a packed geometry (never fused)
 static int gated_layer_forward(cgvc_engine* e, const Gated& L, const ConvIO& io, const GLAct& A, int n, int rows_per_sample_out,
-                               bool keep_y, float* post_scratch, cudaStream_t st, bool save_pre = true) {
+                               bool keep_y, float* post_scratch, cudaStream_t st, bool save_pre = true, const GenActs* G = nullptr) {
   const float* Pm = e->P();
-  if (use_tc(e, L.tc_slot) && io.xhi && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && e->fuse_in) {
+  if (use_tc(e, L.tc_slot) && io.xhi && !io.pk.off && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && e->fuse_in) {
     TcFuse f; memset(&f, 0, sizeof f);
     f.R = rows_per_sample_out;
     f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta; f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta;
@@ -375,6 +397,7 @@ static int gated_layer_forward(cgvc_engine* e, const Gated& L, const ConvIO& io,
   }
   RET(gated_conv_fwd(e, L, io, A.P, st));
   PostParams q = post_params(e, L, A, n, rows_per_sample_out, keep_y, post_scratch);
+  if (G) pack_post(q, *G);
   CK(launch_post_fwd(q, st));
   return 0;
 }
@@ -395,10 +418,11 @@ static void plan_gated(Bump& ws, GLAct& a, long long rows_out, int cout2, int n,
   if (planes) { a.Yhi = ws.take<__nv_bfloat16>((size_t)y_elems); a.Ylo = ws.take<__nv_bfloat16>((size_t)y_elems); }
 }
 
-static void plan_generator(cgvc_engine* e, Bump& ws, GenActs& A, int n, int T) {
+// activations of n samples of r1 rows in all (n x T, or n packed utterances)
+static void plan_generator_rows(cgvc_engine* e, Bump& ws, GenActs& A, int n, long long r1) {
   const bool pl = e->cfg.precision != CGVC_PREC_FP32_SIMT;
-  A.n = n; A.T = T; A.xhi = A.xlo = nullptr; A.post = nullptr;
-  long long r1 = (long long)n * T, r2 = r1 / 2, r4 = r1 / 4;
+  A.n = n; A.T = 0; A.off = nullptr; A.rows = r1; A.max_len = 0; A.xhi = A.xlo = nullptr; A.post = nullptr;
+  long long r2 = r1 / 2, r4 = r1 / 4;
   if (pl) { A.xhi = ws.take<__nv_bfloat16>((size_t)r1 * 128); A.xlo = ws.take<__nv_bfloat16>((size_t)r1 * 128); }   // input planes, channels padded to 64 (128: F16F8)
   A.xchi = A.xclo = nullptr; A.z = nullptr;
   if (pl) {                                                    // tap-lowered edge layers (edge_on)
@@ -422,19 +446,29 @@ static void plan_generator(cgvc_engine* e, Bump& ws, GenActs& A, int n, int T) {
   A.out_cl = ws.take<float>((size_t)r1 * e->cfg.num_features);
 }
 
+static void plan_generator(cgvc_engine* e, Bump& ws, GenActs& A, int n, int T) {
+  plan_generator_rows(e, ws, A, n, (long long)n * T);
+  A.T = T;
+}
+
 // keep_y: also write the fp32 copy of every activation (debug taps / SIMT path); the tensor-core training path only
 // needs fp32 where a residual add or the discriminator head reads it.
 // save_pre = false (inference): the fused layers do not write their pre-norm outputs / statistics (nothing runs backward)
 static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const float* x_cl, cudaStream_t st, bool keep_y, bool save_pre = true) {
-  const int n = A.n, T = A.T, nf = e->cfg.num_features;
+  // packed utterances (A.off): the geometry is one sequence of all rows, n = 1 and T = the row count; every layer's taps, instance
+  // norms and edge-layer tap lowering then follow the utterance boundaries of A.off instead
+  const bool packed = A.off != nullptr;
+  const int n = packed ? 1 : A.n, T = packed ? (int)A.rows : A.T, nf = e->cfg.num_features;
+  const GenActs* G = packed ? &A : nullptr;
+  auto at = [&](ConvIO& c, int W) { c.W = W; if (packed) c.pk = PackGeom{A.off, A.n, (int)(A.rows / W), A.max_len}; };
   const float* Pm = e->P();
   A.x_cl = x_cl;
   const bool edge = edge_on(e, N) && A.xchi && A.z;
   const int qm = e->cfg.precision == CGVC_PREC_F16F8;
-  ConvIO io; io.x = x_cl; io.xhi = A.xhi; io.xlo = A.xlo; io.n = n; io.H = 1; io.W = T;
+  ConvIO io; io.x = x_cl; io.xhi = A.xhi; io.xlo = A.xlo; io.n = n; io.H = 1; at(io, T);
   if (edge) {
     // h1 = dense [n*T, kw*F] x [kw*F, 2*128] GEMM on the im2col of the input
-    CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), qm, A.xchi, A.xclo, st));
+    CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), qm, A.xchi, A.xclo, st, A.off, A.n));
     int r = tc_conv_fwd(e->tcw, N.h1c_slot, e->cfg.precision, A.xchi, A.xclo, n, 1, T, 1, 1, A.h1.P, st);
     if (r != 0) return fail(e, r == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc h1 fwd (tap-lowered): %d", r);
   } else {
@@ -448,20 +482,23 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
   const GLAct* cur = &A.h1;
   int W = T;
   for (int i = 0; i < 2; ++i) {
-    io.x = cur->Y; io.xhi = cur->Yhi; io.xlo = cur->Ylo; io.W = W;
+    io.x = cur->Y; io.xhi = cur->Yhi; io.xlo = cur->Ylo; at(io, W);
     if (!keep_y && cur->Yhi) io.x = nullptr;
     W /= 2;
-    RET(gated_layer_forward(e, N.d[i], io, A.d[i], n, W, keep_y || i == 1, A.post, st, save_pre));   // d2's fp32 output is the first residual input
+    RET(gated_layer_forward(e, N.d[i], io, A.d[i], n, W, keep_y || i == 1, A.post, st, save_pre, G));   // d2's fp32 output is the first residual input
     cur = &A.d[i];
   }
   const float* res = A.d[1].Y; const __nv_bfloat16 *rhi = A.d[1].Yhi, *rlo = A.d[1].Ylo;
   for (int i = 0; i < 6; ++i) {
     const ResBlock& R = N.r[i];
-    io.x = res; io.xhi = rhi; io.xlo = rlo; io.W = W;
-    RET(gated_layer_forward(e, R.h1, io, A.r[i].a, n, W, keep_y, A.post, st, save_pre));
-    ConvIO io2; io2.x = (keep_y || !A.r[i].a.Yhi) ? A.r[i].a.Y : nullptr; io2.xhi = A.r[i].a.Yhi; io2.xlo = A.r[i].a.Ylo; io2.n = n; io2.H = 1; io2.W = W;
+    io.x = res; io.xhi = rhi; io.xlo = rlo; at(io, W);
+    RET(gated_layer_forward(e, R.h1, io, A.r[i].a, n, W, keep_y, A.post, st, save_pre, G));
+    ConvIO io2; io2.x = (keep_y || !A.r[i].a.Yhi) ? A.r[i].a.Y : nullptr; io2.xhi = A.r[i].a.Yhi; io2.xlo = A.r[i].a.Ylo; io2.n = n; io2.H = 1; at(io2, W);
     bool done = false, fused = false;
-    if (use_tc(e, R.tc_slot2) && io2.xhi) {
+    if (use_tc(e, R.tc_slot2) && io2.xhi && packed) {
+      int r = tc_fwd_io(e, R.tc_slot2, io2, 1, 1, A.r[i].Pb, st);
+      if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc h2 fwd (packed): %s", cudaGetErrorString((cudaError_t)r));
+    } else if (use_tc(e, R.tc_slot2) && io2.xhi) {
       TcFuse f; memset(&f, 0, sizeof f);
       f.R = e->fuse_in && A.r[i].Yrhi ? W : 0;                // R = 0: plain conv epilogue
       f.gamma_a = Pm + R.in2.gamma; f.beta_a = Pm + R.in2.beta; f.stats = save_pre ? A.r[i].sb : nullptr; f.resid = res;
@@ -477,28 +514,29 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
     q.beta_a = Pm + R.in2.beta; q.gamma_a = Pm + R.in2.gamma; q.has_in = 1; q.has_gate = 0;
     q.resid = res; q.y = A.r[i].Yr; q.stats = A.r[i].sb; q.y_hi = A.r[i].Yrhi; q.y_lo = A.r[i].Yrlo; q.scratch = A.post;
     q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+    if (G) pack_post(q, *G);
     CK(launch_post_fwd(q, st));
     res = A.r[i].Yr; rhi = A.r[i].Yrhi; rlo = A.r[i].Yrlo;
   }
   io.x = res; io.xhi = rhi; io.xlo = rlo;
   for (int i = 0; i < 2; ++i) {
-    io.W = W;
-    RET(gated_layer_forward(e, N.u[i], io, A.u[i], n, W, keep_y, A.post, st, save_pre));      // W = conv rows per sample; the shuffle doubles them
+    at(io, W);
+    RET(gated_layer_forward(e, N.u[i], io, A.u[i], n, W, keep_y, A.post, st, save_pre, G));      // W = conv rows per sample; the shuffle doubles them
     W *= 2;
     io.x = (keep_y || !A.u[i].Yhi) ? A.u[i].Y : nullptr; io.xhi = A.u[i].Yhi; io.xlo = A.u[i].Ylo;
   }
-  io.W = W;
+  at(io, W);
   {
     bool done = false;
     if (edge && io.xhi) {
       // o1: Z[m, (t, c)] = U[m, :] . W[t][:, c] as one dense GEMM, then out[m, c] = b[c] + sum_t Z[m + t - 7, (t, c)]
       int r = tc_conv_fwd(e->tcw, N.o1f_slot, e->cfg.precision, io.xhi, io.xlo, n, 1, W, 1, 1, A.z, st);
       if (r != 0) return fail(e, r == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc o1 fwd (tap-lowered): %d", r);
-      CK(launch_col2im_taps(A.z, N.o1.kw * nf, (long long)n * W, W, nf, N.o1.kw, +1, Pm + N.o1.b, A.out_cl, st));
+      CK(launch_col2im_taps(A.z, N.o1.kw * nf, (long long)n * W, W, nf, N.o1.kw, +1, Pm + N.o1.b, A.out_cl, st, A.off, A.n));
       done = true;
     }
     if (!done && use_tc(e, N.o1_slot) && io.xhi) {
-      int r = tc_conv_fwd(e->tcw, N.o1_slot, e->cfg.precision, io.xhi, io.xlo, n, 1, W, 1, 1, A.out_cl, st);
+      int r = tc_fwd_io(e, N.o1_slot, io, 1, 1, A.out_cl, st);
       if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc o1 fwd: %s", cudaGetErrorString((cudaError_t)r));
     }
     if (!done) RET(conv_fwd_simt(e, Pm, N.o1, 1, 1, io, A.out_cl, nf, 0, st));
@@ -1154,6 +1192,41 @@ int cgvc_generator_forward(cgvc_handle e, int direction, const float* in_dev, fl
   if (!e->debug_taps) e->taps.clear();
   RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->debug_taps != 0, false));
   CK(launch_transpose_ft(F.g.out_cl, out_dev, batch, frames, e->cfg.num_features, st));
+  return 0;
+}
+
+int cgvc_generator_forward_packed(cgvc_handle e, int direction, const float* in_dev, float* out_dev,
+                                  const long long* offsets_host, int n, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
+  if (!in_dev || !out_dev || !offsets_host) return fail(e, CGVC_ERR_ARG, "null buffer");
+  if (n < 1 || n > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", n, e->cfg.max_batch);
+  if (offsets_host[0] != 0) return fail(e, CGVC_ERR_ARG, "offsets[0] is %lld, must be 0", offsets_host[0]);
+  long long max_len = 0;
+  for (int u = 0; u < n; ++u) {
+    const long long len = offsets_host[u + 1] - offsets_host[u];
+    if (len <= 0 || len % 4 != 0)
+      return fail(e, CGVC_ERR_ARG, "utterance %d: length %lld (offsets %lld .. %lld) must be a positive multiple of 4", u, len,
+                  offsets_host[u], offsets_host[u + 1]);
+    if (len > max_len) max_len = len;
+  }
+  const long long rows = offsets_host[n], cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
+  if (rows > cap) return fail(e, CGVC_ERR_ARG, "%lld frames in all exceed the engine's capacity of max_batch x max_frames = %lld", rows, cap);
+  RET(need_arenas(e, false));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nf = e->cfg.num_features;
+  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
+  FwdPlan F; F.in_cl = ws.take<float>((size_t)rows * nf);
+  plan_generator_rows(e, ws, F.g, n, rows);                  // within work_bytes_needed: n <= max_batch, rows <= max_batch x max_frames
+  long long* off_dev = ws.take<long long>((size_t)n + 1);    // (inside the discriminator's share of the plan)
+  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
+  F.g.off = off_dev; F.g.max_len = (int)max_len;
+  CK(cudaMemcpyAsync(off_dev, offsets_host, ((size_t)n + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CK(launch_transpose_packed(in_dev, F.in_cl, off_dev, n, rows, nf, 1, st));
+  if (!e->debug_taps) e->taps.clear();
+  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->debug_taps != 0, false));
+  CK(launch_transpose_packed(F.g.out_cl, out_dev, off_dev, n, rows, nf, 0, st));
   return 0;
 }
 

@@ -59,6 +59,20 @@ struct GatherGeom {
   short oy[CGVC_MAX_TAPS], ox[CGVC_MAX_TAPS], widx[CGVC_MAX_TAPS];
 };
 
+// Packed variable-length 1-D geometry (cgvc_generator_forward_packed): n utterances concatenated along time.  off = n + 1 device
+// frame prefix sums at full resolution, every length a multiple of 4, so at a level of divisor div (1, 2 or 4: the T, T/2, T/4
+// resolutions of the generator) utterance u owns the rows [off[u] / div, off[u+1] / div) exactly.  max_len: the longest utterance at
+// full resolution (launch sizing on the host).
+struct PackGeom { const long long* off; int n; int div; int max_len; };
+#ifdef __CUDACC__
+// the utterance holding full-resolution frame f: off[u] <= f < off[u+1] (binary search; off is small and stays in L1 / L2)
+__device__ __forceinline__ int pack_find(const long long* __restrict__ off, int n, long long f) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (__ldg(off + mid) <= f) lo = mid; else hi = mid; }
+  return lo;
+}
+#endif
+
 struct GemmOperands {
   const float* src; int s_ld; int s_coff; int C;      // gathered operand: row stride, column offset, #channels contracted
   const float* w; long long w_ts; int w_cs; int w_ns; // weight element (tap slab, c, n) = w[widx*w_ts + c*w_cs + n*w_ns]
@@ -70,6 +84,9 @@ struct GemmOperands {
 
 // ---- fp32 SIMT path (reference arithmetic on the GPU; also the permanent path for the tiny-K layers)
 cudaError_t launch_gg_simt(const GatherGeom& g, const GemmOperands& op, cudaStream_t st);
+// the same over a packed geometry: g = fwd_geom(1, 1, rows at the source level, 1, kw, 1, sw) of a 1-D layer, pk.div = the source
+// level's divisor; taps read only their own utterance's rows (TF-SAME zero padding at every utterance edge)
+cudaError_t launch_gg_simt_packed(const GatherGeom& g, const GemmOperands& op, const PackGeom& pk, cudaStream_t st);
 // weight gradient in forward geometry: dW[widx[t]][c][n] += sum_m S[src(m,t), c] * G[m, n]   (atomic accumulate)
 cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, int s_coff, int C,
                               const float* grad, int g_ld, int g_coff, int N,
@@ -89,6 +106,9 @@ struct PostParams {
   __nv_bfloat16 *y_hi, *y_lo;           // optional bf16 split planes of y for the tensor-core path
   float* scratch;                       // [B,4,C] fp32 workspace for the instance-norm sums (null: internal buffer, single-stream use only)
   int qmode;                            // 1: the planes are F16F8 planes instead: y_hi = q16 [B*R*C halves], y_lo = q8hi [B*R*C bytes] followed by q8lo
+  // packed variable-length samples (seg.off != null): sample b = view rows [seg.off[b] / seg.div, seg.off[b+1] / seg.div) of seg_rows
+  // rows in all (the planes' extent is seg_rows * C); R = the longest sample (grid size).  launch_post_fwd only
+  PackGeom seg; long long seg_rows;
 };
 cudaError_t launch_post_fwd(const PostParams& pp, cudaStream_t st);
 
@@ -126,6 +146,8 @@ cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, 
 cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st);
 // [B,F,T] <-> [B,T,F]
 cudaError_t launch_transpose_ft(const float* in, float* out, int B, int F, int T, cudaStream_t st);
+// packed [F][len_u] blocks (block u at element F * off[u]) <-> channels-last rows [off[n], F]; to_rows = 1: blocks -> rows
+cudaError_t launch_transpose_packed(const float* in, float* out, const long long* off, int n, long long rows, int F, int to_rows, cudaStream_t st);
 // y = a + b
 cudaError_t launch_add(const float* a, const float* b, float* y, long long n, cudaStream_t st);
 
@@ -154,8 +176,11 @@ cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int C
 // stride-1 1-D TF-SAME convolution into operand planes [M, Cpad] (qmode 1: F16F8 planes q16 / q8hi|q8lo, else bf16 hi / lo), dir = +1:
 // out[m, t*C + c] = x[m + t - pl, c], dir = -1: x[m - t + pl, c] (zero outside the sample, pl = (kw - 1) / 2), and the matching sum
 // y[m, c] = bias[c] + sum_t z[m + dir*(t - pl), t*C + c]
-cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st);
-cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st);
+// With off (n + 1 device frame prefix sums, packed utterances) the samples are [off[u], off[u+1]) instead of T-row blocks (T ignored).
+cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st,
+                               const long long* off = nullptr, int n_off = 0);
+cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st,
+                               const long long* off = nullptr, int n_off = 0);
 // P[m, 0:2*cout] = [bias_a | bias_g] + sum_t x[src(m,t)] * [wa | wg][t]   (single input channel, TF kernels [taps][1][cout])
 cudaError_t launch_conv_c1_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                                int cout, float* P, cudaStream_t st);

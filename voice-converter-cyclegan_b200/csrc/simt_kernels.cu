@@ -17,9 +17,15 @@ unsigned long long g_cgvc_launches = 0;   // kernels launched by this library (b
 // ------------------------------------------------------------------------------------------------
 // gather-GEMM, forward / data-gradient form
 // ------------------------------------------------------------------------------------------------
-template <int BM, int BK, bool VEC>
+// Packed variable-length utterances (launch_gg_simt_packed; VEC only): the instantiations with one trailing PackGeom argument.  Their
+// A-row slots keep (first source row of the utterance, its length at the source level, local position * stride) where the dense form
+// keeps (b, y, x).  The dense instantiations take no such argument.
+__device__ __forceinline__ const PackGeom& pack_arg(const PackGeom& p) { return p; }
+template <int BM, int BK, bool VEC, class... PKs>
 __global__ void __launch_bounds__(256)
-gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ GemmOperands op) {
+gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ GemmOperands op, const PKs... pks) {
+  constexpr bool PK = sizeof...(PKs) > 0;
+  static_assert(VEC || !PK, "the packed form gathers 4-channel quads");
   constexpr int BN = 64;
   constexpr int TM = BM / 16;
   __shared__ __align__(16) float As[BK][BM + 4];
@@ -52,17 +58,30 @@ gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ Gem
       long long m = m0 + row;
       rvalid[s] = (idx < BM * QPR) && (m < M);
       long long mm = rvalid[s] ? m : 0;
-      int b = (int)(mm / HW); int rem = (int)(mm - (long long)b * HW);
-      int y = rem / g.Wx; int x = rem - y * g.Wx;
-      rb[s] = b; ry[s] = y * g.sy; rx[s] = x * g.sx;
+      if constexpr (PK) {
+        const PackGeom& pk = pack_arg(pks...);
+        const int dout = pk.div * g.sx;
+        const int u = pack_find(pk.off, pk.n, mm * dout);
+        const long long o0 = __ldg(pk.off + u), o1 = __ldg(pk.off + u + 1);
+        rb[s] = (int)(o0 / pk.div); ry[s] = (int)((o1 - o0) / pk.div); rx[s] = (int)(mm - o0 / dout) * g.sx;
+      } else {
+        int b = (int)(mm / HW); int rem = (int)(mm - (long long)b * HW);
+        int y = rem / g.Wx; int x = rem - y * g.Wx;
+        rb[s] = b; ry[s] = y * g.sy; rx[s] = x * g.sx;
+      }
     }
     for (int t = 0; t < g.ntaps; ++t) {
       const float* aptr[SLOTS];
 #pragma unroll
       for (int s = 0; s < SLOTS; ++s) {
-        int yy = ry[s] + g.oy[t], xx = rx[s] + g.ox[t];
-        bool ok = rvalid[s] && yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws;
-        aptr[s] = ok ? op.src + ((long long)(rb[s] * g.Hs + yy) * g.Ws + xx) * op.s_ld + op.s_coff + rkq[s] : nullptr;
+        if constexpr (PK) {
+          const int xx = rx[s] + g.ox[t];
+          aptr[s] = rvalid[s] && xx >= 0 && xx < ry[s] ? op.src + (long long)(rb[s] + xx) * op.s_ld + op.s_coff + rkq[s] : nullptr;
+        } else {
+          int yy = ry[s] + g.oy[t], xx = rx[s] + g.ox[t];
+          bool ok = rvalid[s] && yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws;
+          aptr[s] = ok ? op.src + ((long long)(rb[s] * g.Hs + yy) * g.Ws + xx) * op.s_ld + op.s_coff + rkq[s] : nullptr;
+        }
       }
       const float* wt = op.w + (long long)g.widx[t] * op.w_ts;
       for (int c0 = 0; c0 < op.C; c0 += BK) {
@@ -172,6 +191,23 @@ gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ Gem
       }
     }
   }
+}
+
+cudaError_t launch_gg_simt_packed(const GatherGeom& g, const GemmOperands& op, const PackGeom& pk, cudaStream_t st) {
+  const long long M = (long long)g.B * g.Hy * g.Wx;
+  if (M == 0 || op.N == 0) return cudaSuccess;
+  const bool aligned = (op.s_ld % 4 == 0) && (op.s_coff % 4 == 0) && ((reinterpret_cast<uintptr_t>(op.src) & 15) == 0);
+  if (!pk.off || g.B != 1 || g.Hy != 1 || g.Hs != 1 || g.Hd != 1 || !aligned || op.C % 8) return cudaErrorInvalidValue;
+  ++g_cgvc_launches;
+  const dim3 block(256);
+  if (op.C % 16 == 0) {
+    if (M >= 4096) gg_simt_kernel<128, 16, true, PackGeom><<<dim3((unsigned)((M + 127) / 128), (op.N + 63) / 64), block, 0, st>>>(g, op, pk);
+    else           gg_simt_kernel<64, 16, true, PackGeom><<<dim3((unsigned)((M + 63) / 64), (op.N + 63) / 64), block, 0, st>>>(g, op, pk);
+  } else {
+    if (M >= 4096) gg_simt_kernel<128, 8, true, PackGeom><<<dim3((unsigned)((M + 127) / 128), (op.N + 63) / 64), block, 0, st>>>(g, op, pk);
+    else           gg_simt_kernel<64, 8, true, PackGeom><<<dim3((unsigned)((M + 63) / 64), (op.N + 63) / 64), block, 0, st>>>(g, op, pk);
+  }
+  return cudaGetLastError();
 }
 
 cudaError_t launch_gg_simt(const GatherGeom& g, const GemmOperands& op, cudaStream_t st) {
@@ -411,21 +447,33 @@ __device__ __forceinline__ void sum_over_rows(F4 (&x)[NQ], float4 (*red)[32], in
   }
 }
 
+// sample b's first view row and its positions (PK: packed variable-length samples, PostParams::seg)
+template <bool PK>
+__device__ __forceinline__ void post_sample(const PostParams& q, int b, long long& s0, int& R) {
+  if constexpr (PK) {
+    const long long o0 = q.seg.off[b], o1 = q.seg.off[b + 1];
+    s0 = o0 / q.seg.div; R = (int)((o1 - o0) / q.seg.div);
+  } else {
+    s0 = (long long)b * q.R; R = q.R;
+  }
+}
+
 // scratch[b][q][c], q = 0..3: sum(a-ka), sum((a-ka)^2), sum(g-kg), sum((g-kg)^2)
-template <bool HAS_GATE>
+template <bool HAS_GATE, bool PK = false>
 __global__ void __launch_bounds__(256)
 post_stats_kernel(const __grid_constant__ PostParams q, float* __restrict__ scratch) {
   __shared__ float4 red[8][32];
   const PostIdx ix(q.C);
   const int lane = threadIdx.x & 31;
-  const int Rw = q.R / q.sh;
-  const float* pb = q.p + (long long)ix.b * Rw * q.ldp;
+  long long s0; int R;
+  post_sample<PK>(q, ix.b, s0, R);
+  const float* pb = q.p + s0 / q.sh * q.ldp;                  // s0 is a multiple of sh (whole conv rows)
   F4 acc[4] = {zero4(), zero4(), zero4(), zero4()};
   if (ix.cvalid) {
     const F4 ka = ld4(pb + ix.c), kg = HAS_GATE ? ld4(pb + q.Cc + ix.c) : zero4();       // shift = value at position 0
     // the whole position range is reduced inside one CTA (grid.y == 1): deterministic, no atomics
 #pragma unroll 4
-    for (int r = ix.rl; r < q.R; r += 8) {
+    for (int r = ix.rl; r < R; r += 8) {
       {
         int w = r >> (q.sh - 1); int s = r & (q.sh - 1);
         long long a = (long long)w * q.ldp + s * q.C + ix.c;
@@ -448,18 +496,20 @@ post_stats_kernel(const __grid_constant__ PostParams q, float* __restrict__ scra
   }
 }
 
-template <bool HAS_IN, bool HAS_GATE>
+template <bool HAS_IN, bool HAS_GATE, bool PK = false>
 __global__ void __launch_bounds__(256)
 post_apply_fwd_kernel(const __grid_constant__ PostParams q, const float* __restrict__ scratch) {
   const PostIdx ix(q.C);
   if (!ix.cvalid) return;
-  const int Rw = q.R / q.sh;
-  const float* pb = q.p + (long long)ix.b * Rw * q.ldp;
+  long long s0; int R;
+  post_sample<PK>(q, ix.b, s0, R);
+  if (PK && (int)blockIdx.y * kPostRows >= R) return;        // past the end of a shorter sample (R >= 1: block y = 0 stays and writes the stats)
+  const float* pb = q.p + s0 / q.sh * q.ldp;
   // per channel: norm(x) = x * sc + of  (sc = rstd*gamma, of = beta - mean*sc)
   F4 sca = one4(), ofa = zero4(), scg = one4(), ofg = zero4();
   if (HAS_IN) {
     const float* sc = scratch + (long long)ix.b * 4 * q.C + ix.c;
-    const float invR = 1.f / (float)q.R;
+    const float invR = 1.f / (float)R;
     F4 mean_a, rstd_a, mean_g = zero4(), rstd_g = one4();
     {
       F4 ka = ld4(pb + ix.c), s1 = ld4(sc), s2 = ld4(sc + q.C), ga = ld4(q.gamma_a + ix.c), ba = ld4(q.beta_a + ix.c);
@@ -488,7 +538,7 @@ post_apply_fwd_kernel(const __grid_constant__ PostParams q, const float* __restr
 #pragma unroll
   for (int i = 0; i < kPostRows / 8; ++i) {
     const int r = ix.r0 + 8 * i;
-    if (r < q.R) {
+    if (r < R) {
       const int w = r >> shs, s = r & shs;
       const long long a = (long long)w * q.ldp + s * q.C + ix.c;
       F4 xa = ld4(pb + a), xg = HAS_GATE ? ld4(pb + a + q.Cc) : zero4(), y;
@@ -501,13 +551,13 @@ post_apply_fwd_kernel(const __grid_constant__ PostParams q, const float* __restr
         }
         y.v[k] = na;
       }
-      const long long o = ((long long)ix.b * q.R + r) * q.C + ix.c;
+      const long long o = (s0 + r) * q.C + ix.c;
       if (q.resid) { F4 rr = ld4(q.resid + o);
 #pragma unroll
         for (int k = 0; k < 4; ++k) y.v[k] += rr.v[k]; }
       if (q.y) st4(q.y + o, y);
       if (q.y_hi) {
-        if (q.qmode) st4_quant(q.y_hi, q.y_lo, o, (long long)q.B * q.R * q.C, y);
+        if (q.qmode) st4_quant(q.y_hi, q.y_lo, o, PK ? q.seg_rows * q.C : (long long)q.B * q.R * q.C, y);
         else st4_split(q.y_hi + o, q.y_lo + o, y);
       }
     }
@@ -535,9 +585,28 @@ static bool post_aligned(const void* a, const void* b, const void* c, int ldp, i
 
 static bool post_fwd_stream_dispatch(const PostParams& pp, cudaStream_t st, cudaError_t* err);      // streaming one-pass form, further down
 
+// packed variable-length samples (PostParams::seg): one CTA column per sample, grid.y sized by the longest
+static cudaError_t launch_post_fwd_packed(const PostParams& pp, cudaStream_t st) {
+  if (pp.seg.div < 1 || 4 % (pp.seg.div * pp.sh)) return cudaErrorInvalidValue;     // samples start on whole conv rows: off[u] / div % sh == 0
+  dim3 grid((pp.C + kPostChan - 1) / kPostChan, (pp.R + kPostRows - 1) / kPostRows, pp.B);
+  float* scratch = pp.scratch;
+  if (pp.has_in) {
+    cudaError_t e = cudaSuccess;
+    if (!scratch) { e = post_scratch((size_t)pp.B * 4 * pp.C, &scratch); if (e != cudaSuccess) return e; }
+    ++g_cgvc_launches;
+    if (pp.has_gate) post_stats_kernel<true, true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
+    else post_stats_kernel<false, true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
+  }
+  ++g_cgvc_launches;
+  if (pp.has_in) { if (pp.has_gate) post_apply_fwd_kernel<true, true, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_fwd_kernel<true, false, true><<<grid, 256, 0, st>>>(pp, scratch); }
+  else           { if (pp.has_gate) post_apply_fwd_kernel<false, true, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_fwd_kernel<false, false, true><<<grid, 256, 0, st>>>(pp, scratch); }
+  return cudaGetLastError();
+}
+
 cudaError_t launch_post_fwd(const PostParams& pp, cudaStream_t st) {
   if (pp.B == 0) return cudaSuccess;
   if (!post_aligned(pp.p, pp.y, pp.resid, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535) return cudaErrorInvalidValue;
+  if (pp.seg.off) return launch_post_fwd_packed(pp, st);
   { cudaError_t se = cudaSuccess; if (post_fwd_stream_dispatch(pp, st, &se)) return se; }
   dim3 grid((pp.C + kPostChan - 1) / kPostChan, (pp.R + kPostRows - 1) / kPostRows, pp.B);
   float* scratch = pp.scratch;
@@ -1399,6 +1468,32 @@ cudaError_t launch_transpose_ft(const float* in, float* out, int B, int F, int T
   return cudaGetLastError();
 }
 
+// packed utterances: element (frame m, feature f) is row-major m * F + f, and f * len_u + (m - off[u]) of utterance u's [F][len_u]
+// block at F * off[u].  TO_ROWS: blocks -> rows (reads gather, writes coalesce), else rows -> blocks.
+template <bool TO_ROWS>
+__global__ void __launch_bounds__(256)
+transpose_packed_kernel(const float* __restrict__ in, float* __restrict__ out, const long long* __restrict__ off, int n, long long rows, int F) {
+  const long long total = rows * F;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const long long m = i / F; const int f = (int)(i - m * F);
+    const int u = pack_find(off, n, m);
+    const long long o0 = __ldg(off + u), len = __ldg(off + u + 1) - o0;
+    const long long b = F * o0 + f * len + (m - o0);
+    if (TO_ROWS) out[i] = in[b]; else out[b] = in[i];
+  }
+}
+
+cudaError_t launch_transpose_packed(const float* in, float* out, const long long* off, int n, long long rows, int F, int to_rows, cudaStream_t st) {
+  const long long total = rows * F;
+  if (total == 0) return cudaSuccess;
+  if (!off || n < 1) return cudaErrorInvalidValue;
+  long long nb = (total + 255) / 256; if (nb > 2368) nb = 2368;
+  ++g_cgvc_launches;
+  if (to_rows) transpose_packed_kernel<true><<<(unsigned)nb, 256, 0, st>>>(in, out, off, n, rows, F);
+  else transpose_packed_kernel<false><<<(unsigned)nb, 256, 0, st>>>(in, out, off, n, rows, F);
+  return cudaGetLastError();
+}
+
 __global__ void __launch_bounds__(256)
 add_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y, long long n) {
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) y[i] = a[i] + b[i];
@@ -1863,16 +1958,29 @@ cudaError_t launch_pad_split(const float* x, long long M, int C, int ld, int Cpa
 // im2col over the taps of a stride-1 1-D TF-SAME convolution of a NARROW channels-last tensor x [B*T, C] (C % 4 == 0):
 //   out[m, t*C + c] = x[m + dir*(t - pl), c]  if that row lies in the same sample, else 0;   columns [kw*C, Cpad) = 0
 // Q = 1: F16F8 planes (q16; q8hi followed by q8lo, activation-role scales); Q = 0: bf16 hi / lo planes.
+// row m's position in its sample and the sample's length: T-row blocks, or (off != null) the packed utterances [off[u], off[u+1])
+__device__ __forceinline__ int tap_sample(long long m, int T, const long long* __restrict__ off, int n_off, int& len) {
+  if (off) {
+    const int u = pack_find(off, n_off, m);
+    const long long o0 = __ldg(off + u);
+    len = (int)(__ldg(off + u + 1) - o0);
+    return (int)(m - o0);
+  }
+  len = T;
+  return (int)(m % T);
+}
+
 template <int Q>
 __global__ void __launch_bounds__(256)
-im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int kw, int pl, int dir, int Cpad, void* __restrict__ hi, void* __restrict__ lo) {
+im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int kw, int pl, int dir, int Cpad, void* __restrict__ hi, void* __restrict__ lo,
+                   const long long* __restrict__ off, int n_off) {
   const long long n = M * Cpad, nq = n / 4;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nq; i += (long long)gridDim.x * 256) {
     const long long e = i * 4; const int col = (int)(e % Cpad); const long long m = e / Cpad;
     const int t = col / C, c = col - t * C;
-    const int w = (int)(m % T), ws = w + dir * (t - pl);
+    int len; const int w = tap_sample(m, T, off, n_off, len), ws = w + dir * (t - pl);
     float v[4] = {0.f, 0.f, 0.f, 0.f};
-    if (t < kw && ws >= 0 && ws < T) {
+    if (t < kw && ws >= 0 && ws < len) {
       const float4 q = *reinterpret_cast<const float4*>(x + (m + (long long)(ws - w)) * C + c);
       v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
     }
@@ -1892,30 +2000,32 @@ im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int k
   }
 }
 
-cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st) {
+cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st,
+                               const long long* off, int n_off) {
   if (M == 0) return cudaSuccess;
-  if (C % 4 || Cpad % 4 || Cpad < kw * C || T <= 0 || M % T) return cudaErrorInvalidValue;
+  if (C % 4 || Cpad % 4 || Cpad < kw * C || (!off && (T <= 0 || M % T)) || (off && n_off < 1)) return cudaErrorInvalidValue;
   const int pl = (kw - 1) / 2;                      // TF SAME at stride 1: total pad kw - 1, the smaller half on the left
   long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
-  if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo);
-  else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo);
+  if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off);
+  else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off);
   return cudaGetLastError();
 }
 
 // the inverse gather: y[m, c] = (bias ? bias[c] : 0) + sum_t z[m + dir*(t - pl), t*C + c] over the rows of the same sample; z row stride ldz.
 // One thread per 4 output channels; the 15 partial sums are added in tap order (deterministic).
 __global__ void __launch_bounds__(256)
-col2im_taps_kernel(const float* __restrict__ z, int ldz, long long M, int T, int C, int kw, int pl, int dir, const float* __restrict__ bias, float* __restrict__ y) {
+col2im_taps_kernel(const float* __restrict__ z, int ldz, long long M, int T, int C, int kw, int pl, int dir, const float* __restrict__ bias, float* __restrict__ y,
+                   const long long* __restrict__ off, int n_off) {
   const int cq = C / 4;
   const long long n = M * cq;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
     const int c = (int)(i % cq) * 4; const long long m = i / cq;
-    const int w = (int)(m % T);
+    int len; const int w = tap_sample(m, T, off, n_off, len);
     float4 acc = bias ? *reinterpret_cast<const float4*>(bias + c) : make_float4(0.f, 0.f, 0.f, 0.f);
     for (int t = 0; t < kw; ++t) {
       const int ws = w + dir * (t - pl);
-      if (ws < 0 || ws >= T) continue;
+      if (ws < 0 || ws >= len) continue;
       const float4 q = *reinterpret_cast<const float4*>(z + (m + (long long)(ws - w)) * ldz + t * C + c);
       acc.x += q.x; acc.y += q.y; acc.z += q.z; acc.w += q.w;
     }
@@ -1923,13 +2033,14 @@ col2im_taps_kernel(const float* __restrict__ z, int ldz, long long M, int T, int
   }
 }
 
-cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st) {
+cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st,
+                               const long long* off, int n_off) {
   if (M == 0) return cudaSuccess;
-  if (C % 4 || ldz % 4 || T <= 0 || M % T) return cudaErrorInvalidValue;
+  if (C % 4 || ldz % 4 || (!off && (T <= 0 || M % T)) || (off && n_off < 1)) return cudaErrorInvalidValue;
   const int pl = (kw - 1) / 2;
   long long n = M * (C / 4); long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
-  col2im_taps_kernel<<<(unsigned)nb, 256, 0, st>>>(z, ldz, M, T, C, kw, pl, dir, bias, y);
+  col2im_taps_kernel<<<(unsigned)nb, 256, 0, st>>>(z, ldz, M, T, C, kw, pl, dir, bias, y, off, n_off);
   return cudaGetLastError();
 }
 

@@ -183,6 +183,9 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   const uint8_t *a8_hi, *a8_lo;                          // [rows, a_ld] bytes
   CUtensorMap tm_b8_hi, tm_b8_lo;                        // box [1][BN][64 bytes], SWIZZLE_64B
   uint8_t* y8;                                           // fused epilogues: q8hi plane of y [M, C_out] bytes, q8lo follows at + M * C_out (y_hi = q16)
+  // packed variable-length utterances (the PK kernels, plain epilogue only): g is the 1-D geometry of all rows, pk.div the source
+  // level's divisor; the output level's is pk.div * g.sx
+  PackGeom pk;
 };
 
 struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[src(m,t), c] * G[m, n]
@@ -857,9 +860,12 @@ __device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const fl
 //               the epilogue in two groups of 4.  (The accumulator of a 256-wide tile does not fit next to the stages: 128 KB.)
 constexpr int kNTThreads = 384;
 
-template <int BN, int NPL, int EPI>
+// PK: the packed form (cgvc_generator_forward_packed).  Row m's source rows are those of its own utterance: the producers keep
+// (first source row of the utterance, its length at the source level, local position * stride) where the dense form keeps (b, y, x).
+template <int BN, int NPL, int EPI, bool PK = false>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
+  static_assert(!PK || EPI == 0, "packed rows never take the fused epilogues (they need whole equal-length samples per tile)");
   using Cfg = NTCfg<BN, NPL>;
   __shared__ float epi_xch[2][4][32];                        // cross-warp exchange of the fused epilogue, per group
   __shared__ __align__(16) float epi_bc[8][(EPI == 3 || EPI == 4) ? 384 : 128];   // per-warp broadcast of per-column coefficients (32 floats per quantity)
@@ -910,9 +916,16 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
       for (int i = 0; i < 8; ++i) {
         long long m = m0 + rsub + 16 * i;
         if (m < M) {
-          int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
-          int y = rem / g.Wx; int x = rem - y * g.Wx;
-          rb[i] = b; ry[i] = y * g.sy; rx[i] = x * g.sx;
+          if constexpr (PK) {                                // rb = first source row, ry = source length, rx = local position * stride
+            const int dout = p.pk.div * g.sx;
+            const int u = pack_find(p.pk.off, p.pk.n, m * dout);
+            const long long o0 = __ldg(p.pk.off + u), o1 = __ldg(p.pk.off + u + 1);
+            rb[i] = (int)(o0 / p.pk.div); ry[i] = (int)((o1 - o0) / p.pk.div); rx[i] = (int)(m - o0 / dout) * g.sx;
+          } else {
+            int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
+            int y = rem / g.Wx; int x = rem - y * g.Wx;
+            rb[i] = b; ry[i] = y * g.sy; rx[i] = x * g.sx;
+          }
         } else { rb[i] = -1; ry[i] = 0; rx[i] = 0; }
       }
       for (int pass = 0; pass < (NPL == 3 ? 2 : 1); ++pass)
@@ -920,9 +933,15 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
         long long aoff[8];                                   // element offset of the source row, or -1
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          int yy = ry[i] + g.oy[tap], xx = rx[i] + g.ox[tap];
-          bool ok = rb[i] >= 0 && yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws;
-          aoff[i] = ok ? ((long long)(rb[i] * g.Hs + yy) * g.Ws + xx) * p.a_ld + (NPL == 3 && pass == 0 ? (chunk & 3) * 16 : chunk * 8) : -1;
+          const int cofs = NPL == 3 && pass == 0 ? (chunk & 3) * 16 : chunk * 8;
+          if constexpr (PK) {
+            const int xx = rx[i] + g.ox[tap];
+            aoff[i] = rb[i] >= 0 && xx >= 0 && xx < ry[i] ? (long long)(rb[i] + xx) * p.a_ld + cofs : -1;
+          } else {
+            int yy = ry[i] + g.oy[tap], xx = rx[i] + g.ox[tap];
+            bool ok = rb[i] >= 0 && yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws;
+            aoff[i] = ok ? ((long long)(rb[i] * g.Hs + yy) * g.Ws + xx) * p.a_ld + cofs : -1;
+          }
         }
         for (int cc = 0; cc < cchunks; ++cc) {
           const int c0 = cc << 6;
@@ -1432,14 +1451,21 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   ++g_cgvc_launches;
   p.debug = g_tc_debug;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, (epi == 1 || epi == 2 || epi == 5) ? 2 : 0, M, p.N, p.g.ntaps * p.C);
-#define LAUNCH_NT(BN_, NPL_, EPI_)                                                                \
-  do {                                                                                            \
-    e = set_smem(tc_gg_nt_kernel<BN_, NPL_, EPI_>, NTCfg<BN_, NPL_>::SMEM);                       \
-    if (e != cudaSuccess) return e;                                                               \
-    tc_gg_nt_kernel<BN_, NPL_, EPI_><<<grid, kNTThreads, NTCfg<BN_, NPL_>::SMEM, st>>>(p);        \
+#define LAUNCH_NT(BN_, NPL_, EPI_, ...)                                                                        \
+  do {                                                                                                         \
+    e = set_smem(tc_gg_nt_kernel<BN_, NPL_, EPI_, ##__VA_ARGS__>, NTCfg<BN_, NPL_>::SMEM);                     \
+    if (e != cudaSuccess) return e;                                                                            \
+    tc_gg_nt_kernel<BN_, NPL_, EPI_, ##__VA_ARGS__><<<grid, kNTThreads, NTCfg<BN_, NPL_>::SMEM, st>>>(p);      \
   } while (0)
   if (epi != 0 && bn != 256) return cudaErrorInvalidValue;
-  if (precision == 3) {                                     // F16F8 (no fused backward epilogues in this precision)
+  if (p.pk.off) {                                           // packed utterances: plain epilogue only
+    if (epi != 0 || p.g.B != 1 || p.g.Hy != 1) return cudaErrorInvalidValue;
+    const int npl = precision == 3 ? 3 : x3 ? 2 : 1;
+    if (bn == 256)      { if (npl == 3) LAUNCH_NT(256, 3, 0, true); else if (npl == 2) LAUNCH_NT(256, 2, 0, true); else LAUNCH_NT(256, 1, 0, true); }
+    else if (bn == 128) { if (npl == 3) LAUNCH_NT(128, 3, 0, true); else if (npl == 2) LAUNCH_NT(128, 2, 0, true); else LAUNCH_NT(128, 1, 0, true); }
+    else                { if (npl == 3) LAUNCH_NT(32, 3, 0, true);  else if (npl == 2) LAUNCH_NT(32, 2, 0, true);  else LAUNCH_NT(32, 1, 0, true); }
+  }
+  else if (precision == 3) {                                // F16F8 (no fused backward epilogues in this precision)
     if (epi == 1)       LAUNCH_NT(256, 3, 1);
     else if (epi == 2)  LAUNCH_NT(256, 3, 2);
     else if (epi == 5)  LAUNCH_NT(256, 3, 5);
@@ -1578,10 +1604,12 @@ int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba,
 
 // x planes: [n,H,W,cin_k] (channels beyond cin are zero)
 int layer_fwd(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
-              float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused_out = nullptr) {
+              float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused_out = nullptr, const PackGeom* pk = nullptr) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
+  if (pk && (n != 1 || H != 1 || L.kh != 1 || fuse)) return (int)cudaErrorInvalidValue;
   TcNTParams p; memset(&p, 0, sizeof p);
   p.g = fwd_geom(n, H, W, L.kh, L.kw, sh, sw);
+  if (pk) p.pk = *pk;
   p.a_hi = xhi; p.a_lo = xlo; p.a_ld = cin_k(L); p.C = cin_k(L);
   p.b_hi = L.wf_hi; p.b_lo = L.wf_lo; p.Nw = nt_n(L); p.N = Ntot(L);
   p.dst = P; p.d_ld = Ntot(L); p.bias = L.bias; p.accumulate = 0;
@@ -1762,6 +1790,10 @@ static cudaError_t tc_init_kernels() {
   INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4) INIT_NT(256, 2, 5) INIT_NT(256, 1, 5)
   INIT_NT(256, 3, 0) INIT_NT(128, 3, 0) INIT_NT(32, 3, 0) INIT_NT(256, 3, 1) INIT_NT(256, 3, 2) INIT_NT(256, 3, 5)
 #undef INIT_NT
+#define INIT_NT_PK(BN_, NPL_) if ((e = set_smem(tc_gg_nt_kernel<BN_, NPL_, 0, true>, NTCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
+  INIT_NT_PK(256, 1) INIT_NT_PK(256, 2) INIT_NT_PK(256, 3) INIT_NT_PK(128, 1) INIT_NT_PK(128, 2) INIT_NT_PK(128, 3)
+  INIT_NT_PK(32, 1) INIT_NT_PK(32, 2) INIT_NT_PK(32, 3)
+#undef INIT_NT_PK
 #define INIT_TN(NPL_, W16_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
   INIT_TN(3, 1) INIT_TN(3, 0) INIT_TN(2, 0) INIT_TN(1, 0)
 #undef INIT_TN
@@ -1829,6 +1861,11 @@ int tc_conv_fwd(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi,
 int tc_conv_fwd_fused(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                       int n, int H, int W, int sh, int sw, float* P, const TcFuse& fuse, bool* fused, cudaStream_t st) {
   return layer_fwd(w.layers[slot], precision, xhi, xlo, n, H, W, sh, sw, P, st, &fuse, fused);
+}
+
+int tc_conv_fwd_packed(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+                       int rows, int sw, const PackGeom& pk, float* P, cudaStream_t st) {
+  return layer_fwd(w.layers[slot], precision, xhi, xlo, 1, 1, rows, 1, sw, P, st, nullptr, nullptr, &pk);
 }
 
 int tc_conv_dgrad(TcWeights& w, int slot, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo,

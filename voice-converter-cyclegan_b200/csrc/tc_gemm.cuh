@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <stddef.h>
 #include <vector>
+#include "kernels.cuh"
 
 #define TC_UNSUPPORTED (-12345)
 
@@ -83,6 +84,10 @@ int tc_conv_fwd(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi,
 // the separate instance-norm kernels).
 int tc_conv_fwd_fused(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                       int n, int H, int W, int sh, int sw, float* P, const TcFuse& fuse, bool* fused, cudaStream_t st);
+// P = conv(x) + bias of a 1-D layer over packed variable-length utterances (kernels.cuh PackGeom): x planes [rows, .] at the source
+// level of divisor pk.div, stride sw; every tap reads only its own utterance's rows.  Plain epilogue only.
+int tc_conv_fwd_packed(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+                       int rows, int sw, const PackGeom& pk, float* P, cudaStream_t st);
 // dx[n,H,W,cin] (+)= dgrad(dP)            (dP planes [rows_out, Ntot]; H, W are the INPUT dims)
 int tc_conv_dgrad(TcWeights& w, int slot, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo,
                   int n, int H, int W, int sh, int sw, float* dx, int accumulate, cudaStream_t st);

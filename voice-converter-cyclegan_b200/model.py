@@ -313,6 +313,52 @@ class CycleGAN(object):
         torch.cuda.current_stream(self.device).synchronize()
         return out.numpy().copy()
 
+    def test_packed(self, inputs, direction):
+        """Generator forward of utterances of different lengths in one engine call.  inputs: a list of [24, T_i] arrays, every
+        T_i a positive multiple of 4: host arrays of any float dtype (returns a list of float32 numpy arrays) or CUDA tensors
+        (returns a list of CUDA tensors).  Each result is what test() gives for that utterance alone, up to the summation order
+        of its instance-norm statistics."""
+        if direction == 'A2B':
+            d = 0
+        elif direction == 'B2A':
+            d = 1
+        else:
+            raise Exception('Conversion direction must be specified.')
+        if len(inputs) == 0:
+            return []
+        on_device = all(isinstance(x, torch.Tensor) and x.is_cuda for x in inputs)
+        lengths = []
+        for x in inputs:
+            if len(x.shape) != 2 or x.shape[0] != self.num_features:
+                raise ValueError("expected [%d, frames] utterances, got %r" % (self.num_features, tuple(x.shape)))
+            lengths.append(int(x.shape[1]))
+        offsets = np.zeros(len(lengths) + 1, dtype=np.int64)
+        np.cumsum(lengths, out=offsets[1:])
+        n, total = len(lengths), int(offsets[-1])
+        if n > self._max_batch or total > self._max_batch * self._max_frames:
+            batch = max(n, self._max_batch)
+            self._ensure_capacity(batch, max(self._max_frames, -(-total // (4 * batch)) * 4))
+        F = self.num_features
+        if on_device:
+            x = torch.cat([t.to(dtype=torch.float32).reshape(-1) for t in inputs])
+        else:
+            host = torch.empty(total * F, dtype=torch.float32).pin_memory()
+            hv = host.numpy()
+            for u, a in enumerate(inputs):       # cast to fp32 at the boundary, like test()
+                hv[F * offsets[u]:F * offsets[u + 1]].reshape(F, lengths[u])[...] = np.asarray(a)
+            x = torch.empty(total * F, dtype=torch.float32, device=self.device)
+            x.copy_(host, non_blocking=True)
+        y = torch.empty_like(x)
+        off = offsets.ctypes.data_as(C.POINTER(C.c_longlong))
+        self._chk(self._lib.cgvc_generator_forward_packed(self._handle, d, _ptr(x), _ptr(y), off, n, self._stream()))
+        if on_device:
+            return [y[F * offsets[u]:F * offsets[u + 1]].view(F, lengths[u]) for u in range(n)]
+        out = torch.empty(y.shape, dtype=torch.float32).pin_memory()
+        out.copy_(y, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        ov = out.numpy()
+        return [ov[F * offsets[u]:F * offsets[u + 1]].reshape(F, lengths[u]).copy() for u in range(n)]
+
     def discriminate(self, inputs, which):
         """Discriminator forward (module.py:188-213): which in {'A','B'}; returns [B, 6, T/16, 1]."""
         x = self._to_device(inputs, "disc")
