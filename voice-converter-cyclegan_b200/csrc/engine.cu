@@ -15,6 +15,7 @@
 
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 static thread_local std::string g_create_error;
@@ -29,13 +30,20 @@ static thread_local std::string g_create_error;
 struct TensorInfo { std::string name; size_t off; int ndim; int shape[4]; size_t numel; };
 struct ConvW { size_t k, b; int kh, kw, cin, cout; };
 struct InW { size_t beta, gamma; int c; };
-struct Gated { ConvW a, g; InW ina, ing; int has_in; int sh, sw; int shuffle; int tc_slot; };
-struct ResBlock { Gated h1; ConvW h2; InW in2; int tc_slot2; };
-struct GenNet { Gated h1; Gated d[2]; ResBlock r[6]; Gated u[2]; ConvW o1; int o1_slot; size_t begin, end;
-                int h1c_slot, o1f_slot; };      // the tap-lowered forms of the two 15-tap edge layers (`edge_lower`, see edge_on)
-struct DiscNet { Gated h1; Gated d[3]; size_t dense_k, dense_b; size_t begin, end; };
+// One layer: convolution a, in the gated layers beside convolution g over the same input (P = [a | g]), then optionally instance
+// norm (of each branch), the GLU of the two branches and the pixel shuffle.  The residual blocks' h2 is a layer without gate whose
+// normalised output is added to the block input.
+struct Layer {
+  ConvW a, g; InW ina, ing; int has_in; int sh, sw; int shuffle; int tc_slot = -1;
+  bool gated() const { return g.cout != 0; }
+  int width() const { return gated() ? 2 * a.cout : a.cout; }       // columns of P
+};
+struct ResBlock { Layer h1, h2; };
+struct GenNet { Layer h1; Layer d[2]; ResBlock r[6]; Layer u[2]; Layer o1; size_t begin, end;
+                int h1c_slot = -1, o1f_slot = -1; };      // the tap-lowered forms of the two 15-tap edge layers (`edge_lower`, see edge_on)
+struct DiscNet { Layer h1; Layer d[3]; size_t dense_k, dense_b; size_t begin, end; };
 
-// per-layer activations kept for backward
+// per-layer activations kept for backward: pre-norm conv output, instance-norm statistics, output (fp32 and operand planes)
 struct GLAct { float* P; float* stats; float* Y; __nv_bfloat16 *Yhi, *Ylo; };
 struct GenActs {
   int n, T;
@@ -46,7 +54,7 @@ struct GenActs {
   __nv_bfloat16 *xchi, *xclo;   // im2col of the input over h1's taps: operand planes [n*T, ru128(kw*F)] (edge_lower)
   float* z;                     // o1's per-tap products [n*T, kw*F] before the tap-shifted sum (edge_lower)
   GLAct h1, d[2];
-  struct { GLAct a; float *Pb, *sb, *Yr; __nv_bfloat16 *Yrhi, *Yrlo; } r[6];
+  struct { GLAct h1, h2; } r[6];
   GLAct u[2];
   float* out_cl;
   float* post;                  // scratch for the instance-norm sums [n,4,1024] (null: the kernels' own lazily grown buffer)
@@ -189,13 +197,13 @@ struct TableBuilder {
 
 static void build_generator(TableBuilder& tb, GenNet& g, int nf) {
   g.begin = tb.off;
-  g.h1 = Gated{}; g.h1.a = tb.conv1d("h1_conv", 15, nf, 128); g.h1.g = tb.conv1d("h1_conv_gates", 15, nf, 128);
+  g.h1 = Layer{}; g.h1.a = tb.conv1d("h1_conv", 15, nf, 128); g.h1.g = tb.conv1d("h1_conv_gates", 15, nf, 128);
   g.h1.has_in = 0; g.h1.sh = 1; g.h1.sw = 1; g.h1.shuffle = 1;
   int idx = 0, cin = 128;
   const int dco[2] = {256, 512};
   for (int i = 0; i < 2; ++i) {
     std::string p = "downsample1d_block" + std::to_string(i + 1) + "_";
-    Gated& L = g.d[i]; L = Gated{};
+    Layer& L = g.d[i]; L = Layer{};
     L.a = tb.conv1d(p + "h1_conv", 5, cin, dco[i]); L.ina = tb.inorm(idx++, dco[i]);
     L.g = tb.conv1d(p + "h1_gates", 5, cin, dco[i]); L.ing = tb.inorm(idx++, dco[i]);
     L.has_in = 1; L.sh = 1; L.sw = 2; L.shuffle = 1; cin = dco[i];
@@ -206,30 +214,32 @@ static void build_generator(TableBuilder& tb, GenNet& g, int nf) {
     R.h1.a = tb.conv1d(p + "h1_conv", 3, 512, 1024); R.h1.ina = tb.inorm(idx++, 1024);
     R.h1.g = tb.conv1d(p + "h1_gates", 3, 512, 1024); R.h1.ing = tb.inorm(idx++, 1024);
     R.h1.has_in = 1; R.h1.sh = 1; R.h1.sw = 1; R.h1.shuffle = 1;
-    R.h2 = tb.conv1d(p + "h2_conv", 3, 1024, 512); R.in2 = tb.inorm(idx++, 512);
+    R.h2.a = tb.conv1d(p + "h2_conv", 3, 1024, 512); R.h2.ina = tb.inorm(idx++, 512);
+    R.h2.has_in = 1; R.h2.sh = 1; R.h2.sw = 1; R.h2.shuffle = 1;
   }
   cin = 512;
   const int uco[2] = {1024, 512};
   for (int i = 0; i < 2; ++i) {
     std::string p = "upsample1d_block" + std::to_string(i + 1) + "_";
-    Gated& L = g.u[i]; L = Gated{};
+    Layer& L = g.u[i]; L = Layer{};
     L.a = tb.conv1d(p + "h1_conv", 5, cin, uco[i]); L.ina = tb.inorm(idx++, uco[i] / 2);
     L.g = tb.conv1d(p + "h1_gates", 5, cin, uco[i]); L.ing = tb.inorm(idx++, uco[i] / 2);
     L.has_in = 1; L.sh = 1; L.sw = 1; L.shuffle = 2; cin = uco[i] / 2;
   }
-  g.o1 = tb.conv1d("o1_conv", 15, 256, nf);
+  g.o1 = Layer{}; g.o1.a = tb.conv1d("o1_conv", 15, 256, nf);
+  g.o1.has_in = 0; g.o1.sh = 1; g.o1.sw = 1; g.o1.shuffle = 1;
   g.end = tb.off;
 }
 
 static void build_discriminator(TableBuilder& tb, DiscNet& d) {
   d.begin = tb.off;
-  d.h1 = Gated{}; d.h1.a = tb.conv2d("h1_conv", 3, 3, 1, 128); d.h1.g = tb.conv2d("h1_conv_gates", 3, 3, 1, 128);
+  d.h1 = Layer{}; d.h1.a = tb.conv2d("h1_conv", 3, 3, 1, 128); d.h1.g = tb.conv2d("h1_conv_gates", 3, 3, 1, 128);
   d.h1.has_in = 0; d.h1.sh = 1; d.h1.sw = 2; d.h1.shuffle = 1;
   int idx = 0, cin = 128;
   const int kh[3] = {3, 3, 6}, co[3] = {256, 512, 1024}, sh[3] = {2, 2, 1};
   for (int i = 0; i < 3; ++i) {
     std::string p = "downsample2d_block" + std::to_string(i + 1) + "_";
-    Gated& L = d.d[i]; L = Gated{};
+    Layer& L = d.d[i]; L = Layer{};
     L.a = tb.conv2d(p + "h1_conv", kh[i], 3, cin, co[i]); L.ina = tb.inorm(idx++, co[i]);
     L.g = tb.conv2d(p + "h1_gates", kh[i], 3, cin, co[i]); L.ing = tb.inorm(idx++, co[i]);
     L.has_in = 1; L.sh = sh[i]; L.sw = 2; L.shuffle = 1; cin = co[i];
@@ -244,6 +254,9 @@ struct ConvIO {               // one convolution application
   int n, H, W;
   PackGeom pk{};              // packed utterances (pk.off != null): n = H = 1, W = rows at the level of divisor pk.div
 };
+static const PackGeom* packed(const ConvIO& io) { return io.pk.off ? &io.pk : nullptr; }
+
+struct PlanePair { __nv_bfloat16 *hi, *lo; };
 
 static int conv_out_dims(const ConvW& c, int sh, int sw, int H, int W, int& Ho, int& Wo) {
   int p; same_pad(H, c.kh, sh, p, Ho); same_pad(W, c.kw, sw, p, Wo); return 0;
@@ -261,12 +274,6 @@ static int conv_fwd_simt(cgvc_engine* e, const float* Pm, const ConvW& c, int sh
   if (io.pk.off) CK(launch_gg_simt_packed(g, op, io.pk, st));
   else CK(launch_gg_simt(g, op, st));
   return 0;
-}
-
-// one tensor-core forward convolution of a layer over io (packed or dense geometry), plain epilogue
-static int tc_fwd_io(cgvc_engine* e, int slot, const ConvIO& io, int sh, int sw, float* P, cudaStream_t st) {
-  if (io.pk.off) return tc_conv_fwd_packed(e->tcw, slot, e->cfg.precision, io.xhi, io.xlo, io.W, sw, io.pk, P, st);
-  return tc_conv_fwd(e->tcw, slot, e->cfg.precision, io.xhi, io.xlo, io.n, io.H, io.W, sh, sw, P, st);
 }
 
 // dx (+)= dgrad(dy[., coff:coff+cout], w)
@@ -305,99 +312,109 @@ static float loss_scale(const cgvc_engine* e, int batch) {
 static bool tc_enabled(const cgvc_engine* e) { return e->cfg.precision != CGVC_PREC_FP32_SIMT && e->tcw.ready; }
 static bool use_tc(const cgvc_engine* e, int slot) { return slot >= 0 && tc_enabled(e); }
 
-// gated layer: conv_a || conv_g -> P [rows, 2*cout]
-static int gated_conv_fwd(cgvc_engine* e, const Gated& L, const ConvIO& io, float* P, cudaStream_t st) {
-  if (use_tc(e, L.tc_slot) && io.xhi) {
-    int r = tc_fwd_io(e, L.tc_slot, io, L.sh, L.sw, P, st);
-    if (r == 0) return 0;
-    if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc_conv_fwd failed: %s", cudaGetErrorString((cudaError_t)r));
-  }
-  if (L.a.cin == 1 && io.x && !io.pk.off && L.a.cout % 4 == 0 && 256 % (L.a.cout / 2) == 0) {   // discriminator h1: HBM-bound special
+// How a tensor-core call on layer c (null: an ad-hoc convolution) ended: done (*done = true); unsupported (TC_UNSUPPORTED, nothing
+// launched): the caller falls back to SIMT where it passes `done`, else CGVC_ERR_UNSUPPORTED; or failed: CGVC_ERR_CUDA
+static int tc_result(cgvc_engine* e, int r, const ConvW* c, const char* what, bool* done = nullptr) {
+  if (r == 0) { if (done) *done = true; return 0; }
+  if (r == TC_UNSUPPORTED && done) return 0;
+  std::string where = what;
+  if (c) for (const TensorInfo& t : e->tensors) if (t.off == c->k) where = t.name + " " + what;
+  if (r == TC_UNSUPPORTED) return fail(e, CGVC_ERR_UNSUPPORTED, "%s: shape not supported by the tensor-core path", where.c_str());
+  return fail(e, CGVC_ERR_CUDA, "%s on the tensor cores: %s", where.c_str(), cudaGetErrorString((cudaError_t)r));
+}
+
+// P = conv(x) + bias, plain epilogue (gated: conv_a || conv_g -> P [rows, 2*cout])
+static int conv_fwd(cgvc_engine* e, const Layer& L, const ConvIO& io, float* P, cudaStream_t st) {
+  bool done = false;
+  if (use_tc(e, L.tc_slot) && io.xhi)
+    RET(tc_result(e, tc_conv_fwd(e->tcw, L.tc_slot, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, P, st, nullptr, nullptr, packed(io)),
+                  &L.a, "forward", &done));
+  if (done) return 0;
+  const float* Pm = e->P();
+  if (L.gated() && L.a.cin == 1 && io.x && !io.pk.off && L.a.cout % 4 == 0 && 256 % (L.a.cout / 2) == 0) {   // discriminator h1: HBM-bound special
     GatherGeom g = fwd_geom(io.n, io.H, io.W, L.a.kh, L.a.kw, L.sh, L.sw);
-    const float* Pm = e->P();
     CK(launch_conv_c1_fwd(g, io.x, Pm + L.a.k, Pm + L.g.k, Pm + L.a.b, Pm + L.g.b, L.a.cout, P, st));
     return 0;
   }
-  RET(conv_fwd_simt(e, e->P(), L.a, L.sh, L.sw, io, P, 2 * L.a.cout, 0, st));
-  RET(conv_fwd_simt(e, e->P(), L.g, L.sh, L.sw, io, P, 2 * L.a.cout, L.a.cout, st));
+  RET(conv_fwd_simt(e, Pm, L.a, L.sh, L.sw, io, P, L.width(), 0, st));
+  if (L.gated()) RET(conv_fwd_simt(e, Pm, L.g, L.sh, L.sw, io, P, L.width(), L.a.cout, st));
   return 0;
 }
 
-static int gated_conv_dgrad(cgvc_engine* e, const Gated& L, int n, int H, int W, const float* dP,
-                            const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, float* dx, int accumulate, cudaStream_t st) {
-  if (use_tc(e, L.tc_slot) && dPhi) {
-    int r = tc_conv_dgrad(e->tcw, L.tc_slot, e->cfg.precision, dPhi, dPlo, n, H, W, L.sh, L.sw, dx, accumulate, st);
-    if (r == 0) return 0;
-    if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc_conv_dgrad failed: %s", cudaGetErrorString((cudaError_t)r));
-  }
-  RET(conv_dgrad_simt(e, e->P(), L.a, L.sh, L.sw, n, H, W, dP, 2 * L.a.cout, 0, dx, accumulate, st));
-  RET(conv_dgrad_simt(e, e->P(), L.g, L.sh, L.sw, n, H, W, dP, 2 * L.a.cout, L.a.cout, dx, 1, st));
+// dx[io's n,H,W] (+)= dgrad(dP); fuse: see tc_conv_dgrad
+static int conv_dgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const float* dP, PlanePair dp, float* dx, int accumulate,
+                      cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr) {
+  bool done = false;
+  if (use_tc(e, L.tc_slot) && dp.hi)
+    RET(tc_result(e, tc_conv_dgrad(e->tcw, L.tc_slot, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, dx, accumulate, st, fuse, fused),
+                  &L.a, "data gradient", &done));
+  if (done) return 0;
+  RET(conv_dgrad_simt(e, e->P(), L.a, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), 0, dx, accumulate, st));
+  if (L.gated()) RET(conv_dgrad_simt(e, e->P(), L.g, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), L.a.cout, dx, 1, st));
   return 0;
 }
 
-static int gated_conv_wgrad(cgvc_engine* e, const Gated& L, const ConvIO& io, const float* dP,
-                            const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, cudaStream_t st) {
-  if (use_tc(e, L.tc_slot) && dPhi && io.xhi) {
-    int r = tc_conv_wgrad(e->tcw, L.tc_slot, e->cfg.precision, io.xhi, io.xlo, dPhi, dPlo, io.n, io.H, io.W, L.sh, L.sw,
-                          e->G() + L.a.k, e->G() + L.g.k, nullptr, nullptr, st);
-    if (r == 0) return 0;
-    if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc_conv_wgrad failed: %s", cudaGetErrorString((cudaError_t)r));
-  }
-  RET(conv_wgrad_simt(e, e->G(), L.a, L.sh, L.sw, io, dP, 2 * L.a.cout, 0, st));
-  RET(conv_wgrad_simt(e, e->G(), L.g, L.sh, L.sw, io, dP, 2 * L.a.cout, L.a.cout, st));
+static int conv_wgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const float* dP, PlanePair dp, cudaStream_t st) {
+  float* Gm = e->G();
+  bool done = false;
+  if (use_tc(e, L.tc_slot) && dp.hi && io.xhi)
+    RET(tc_result(e, tc_conv_wgrad(e->tcw, L.tc_slot, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw,
+                                   Gm + L.a.k, L.gated() ? Gm + L.g.k : nullptr, st), &L.a, "weight gradient", &done));
+  if (done) return 0;
+  RET(conv_wgrad_simt(e, Gm, L.a, L.sh, L.sw, io, dP, L.width(), 0, st));
+  if (L.gated()) RET(conv_wgrad_simt(e, Gm, L.g, L.sh, L.sw, io, dP, L.width(), L.a.cout, st));
   return 0;
 }
 
-static PostParams post_params(const cgvc_engine* e, const Gated& L, const GLAct& A, int n, int rows_per_sample_out, bool keep_y, float* scratch) {
+// instance norm (+ GLU | + resid) and pixel shuffle of A.P, the output of L's convolution over io (rows_per_sample_out rows per sample)
+static PostParams post_params(const cgvc_engine* e, const Layer& L, const ConvIO& io, const GLAct& A, int rows_per_sample_out, bool keep_y,
+                              float* scratch, const float* resid = nullptr) {
   PostParams q; memset(&q, 0, sizeof q);
   q.scratch = scratch;
   const float* Pm = e->P();
-  q.p = A.P; q.ldp = 2 * L.a.cout; q.Cc = L.a.cout; q.B = n; q.sh = L.shuffle;
+  q.p = A.P; q.ldp = L.width(); q.Cc = L.a.cout; q.B = io.n; q.sh = L.shuffle;
   q.R = rows_per_sample_out * L.shuffle; q.C = L.a.cout / L.shuffle;
-  q.has_in = L.has_in; q.has_gate = 1;
-  if (L.has_in) { q.beta_a = Pm + L.ina.beta; q.gamma_a = Pm + L.ina.gamma; q.beta_g = Pm + L.ing.beta; q.gamma_g = Pm + L.ing.gamma; }
+  q.has_in = L.has_in; q.has_gate = L.gated();
+  if (L.has_in) { q.beta_a = Pm + L.ina.beta; q.gamma_a = Pm + L.ina.gamma; }
+  if (L.has_in && L.gated()) { q.beta_g = Pm + L.ing.beta; q.gamma_g = Pm + L.ing.gamma; }
+  q.resid = resid;
   q.y = (keep_y || !A.Yhi) ? A.Y : nullptr;      // without planes the fp32 activation is the only copy
   q.stats = L.has_in ? A.stats : nullptr; q.y_hi = A.Yhi; q.y_lo = A.Ylo;
   q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+  if (io.pk.off && L.has_in) {
+    // packed utterances: q describes one sample holding all q.R view rows; instance norm runs per utterance over its own view rows
+    // (the GLU-only layer is row-local and keeps that view)
+    const long long view_rows = q.R;
+    const int div = (int)((long long)io.pk.div * io.W / view_rows);
+    q.seg = PackGeom{io.pk.off, io.pk.n, div, io.pk.max_len}; q.seg_rows = view_rows;
+    q.B = io.pk.n; q.R = io.pk.max_len / div;
+  }
   return q;
 }
 
-// Packed utterances (G.off): q was built for one sample holding all q.R view rows.  Instance norm then runs per utterance over its
-// own view rows; the GLU-only layer is row-local and keeps that view.
-static void pack_post(PostParams& q, const GenActs& G) {
-  if (!G.off || !q.has_in) return;
-  const long long view_rows = q.R;
-  const int div = (int)(G.rows / view_rows);
-  q.seg = PackGeom{G.off, G.n, div, G.max_len}; q.seg_rows = view_rows;
-  q.B = G.n; q.R = G.max_len / div;
-}
-
-// gated layer forward with instance norm + GLU fused into the GEMM epilogue when the tensor-core path can (1-D layer whose
-// 128-row tiles hold whole samples); otherwise conv kernel + the two streaming instance-norm kernels.  G: the generator's
-// activations when io is a packed geometry (never fused)
-static int gated_layer_forward(cgvc_engine* e, const Gated& L, const ConvIO& io, const GLAct& A, int n, int rows_per_sample_out,
-                               bool keep_y, float* post_scratch, cudaStream_t st, bool save_pre = true, const GenActs* G = nullptr) {
-  const float* Pm = e->P();
+// One layer's forward: convolution, then instance norm (+ GLU | + resid) and pixel shuffle into A.  The paths, in order: tensor
+// cores with the norm fused into the GEMM epilogue (1-D layer, not packed, whole samples per 128-row tile); else tensor cores with
+// the plain epilogue, or SIMT, then the instance-norm kernels.  keep_y: also write the fp32 output.  save_pre = false (inference):
+// the fused epilogue need not write the pre-norm output and statistics, as nothing runs backward
+static int layer_forward(cgvc_engine* e, const Layer& L, const ConvIO& io, const GLAct& A, int rows_per_sample_out, bool keep_y,
+                         bool save_pre, float* post_scratch, cudaStream_t st, const float* resid = nullptr) {
+  bool done = false;
   if (use_tc(e, L.tc_slot) && io.xhi && !io.pk.off && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && e->fuse_in) {
+    const float* Pm = e->P();
     TcFuse f; memset(&f, 0, sizeof f);
     f.R = rows_per_sample_out;
-    f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta; f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta;
-    f.stats = save_pre ? A.stats : nullptr; f.y = keep_y ? A.Y : nullptr; f.y_hi = A.Yhi; f.y_lo = A.Ylo;
+    f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta;
+    if (L.gated()) { f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta; }
+    f.stats = save_pre ? A.stats : nullptr; f.resid = resid; f.y = keep_y ? A.Y : nullptr; f.y_hi = A.Yhi; f.y_lo = A.Ylo;
     bool fused = false;
-    int r = tc_conv_fwd_fused(e->tcw, L.tc_slot, e->cfg.precision, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, save_pre ? A.P : nullptr, f, &fused, st);
+    int r = tc_conv_fwd(e->tcw, L.tc_slot, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, save_pre ? A.P : nullptr, st, &f, &fused);
     if (r != 0 && !save_pre)                                  // shape not fusable: the two-kernel path needs P as its intermediate
-      r = tc_conv_fwd_fused(e->tcw, L.tc_slot, e->cfg.precision, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, A.P, f, &fused, st);
-    if (r != 0 && r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc_conv_fwd_fused failed: %s", cudaGetErrorString((cudaError_t)r));
-    if (r == 0 && fused) return 0;
-    if (r == 0) {                                             // conv done, epilogue not fusable for this shape
-      PostParams q = post_params(e, L, A, n, rows_per_sample_out, keep_y, post_scratch);
-      CK(launch_post_fwd(q, st));
-      return 0;
-    }
+      r = tc_conv_fwd(e->tcw, L.tc_slot, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, A.P, st, &f, &fused);
+    RET(tc_result(e, r, &L.a, "forward", &done));
+    if (fused) return 0;
   }
-  RET(gated_conv_fwd(e, L, io, A.P, st));
-  PostParams q = post_params(e, L, A, n, rows_per_sample_out, keep_y, post_scratch);
-  if (G) pack_post(q, *G);
+  if (!done) RET(conv_fwd(e, L, io, A.P, st));
+  PostParams q = post_params(e, L, io, A, rows_per_sample_out, keep_y, post_scratch, resid);
   CK(launch_post_fwd(q, st));
   return 0;
 }
@@ -428,18 +445,14 @@ static void plan_generator_rows(cgvc_engine* e, Bump& ws, GenActs& A, int n, lon
   if (pl) {                                                    // tap-lowered edge layers (edge_on)
     const size_t cp = (size_t)edge_cpad(e->gen[0].h1.a.kw * e->cfg.num_features);
     A.xchi = ws.take<__nv_bfloat16>((size_t)r1 * cp); A.xclo = ws.take<__nv_bfloat16>((size_t)r1 * cp);
-    A.z = ws.take<float>((size_t)r1 * e->gen[0].o1.kw * e->cfg.num_features);
+    A.z = ws.take<float>((size_t)r1 * e->gen[0].o1.a.kw * e->cfg.num_features);
   }
   plan_gated(ws, A.h1, r1, 256, n, 128, pl, r1 * 128);
   plan_gated(ws, A.d[0], r2, 512, n, 256, pl, r2 * 256);
   plan_gated(ws, A.d[1], r4, 1024, n, 512, pl, r4 * 512);
   for (int i = 0; i < 6; ++i) {
-    plan_gated(ws, A.r[i].a, r4, 2048, n, 1024, pl, r4 * 1024);
-    A.r[i].Pb = ws.take<float>((size_t)r4 * 512);
-    A.r[i].sb = ws.take<float>((size_t)n * 4 * 512);
-    A.r[i].Yr = ws.take<float>((size_t)r4 * 512);
-    A.r[i].Yrhi = A.r[i].Yrlo = nullptr;
-    if (pl) { A.r[i].Yrhi = ws.take<__nv_bfloat16>((size_t)r4 * 512); A.r[i].Yrlo = ws.take<__nv_bfloat16>((size_t)r4 * 512); }
+    plan_gated(ws, A.r[i].h1, r4, 2048, n, 1024, pl, r4 * 1024);
+    plan_gated(ws, A.r[i].h2, r4, 512, n, 512, pl, r4 * 512);
   }
   plan_gated(ws, A.u[0], r4, 2048, n, 512, pl, r2 * 512);
   plan_gated(ws, A.u[1], r2, 1024, n, 256, pl, r1 * 256);
@@ -459,151 +472,109 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
   // norms and edge-layer tap lowering then follow the utterance boundaries of A.off instead
   const bool packed = A.off != nullptr;
   const int n = packed ? 1 : A.n, T = packed ? (int)A.rows : A.T, nf = e->cfg.num_features;
-  const GenActs* G = packed ? &A : nullptr;
-  auto at = [&](ConvIO& c, int W) { c.W = W; if (packed) c.pk = PackGeom{A.off, A.n, (int)(A.rows / W), A.max_len}; };
-  const float* Pm = e->P();
+  auto at = [&](const float* x, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int W) {
+    ConvIO io; io.x = x; io.xhi = hi; io.xlo = lo; io.n = n; io.H = 1; io.W = W;
+    if (packed) io.pk = PackGeom{A.off, A.n, (int)(A.rows / W), A.max_len};
+    return io;
+  };
+  auto of = [&](const GLAct& a, int W) { return at((keep_y || !a.Yhi) ? a.Y : nullptr, a.Yhi, a.Ylo, W); };   // a layer output as input
   A.x_cl = x_cl;
   const bool edge = edge_on(e, N) && A.xchi && A.z;
-  const int qm = e->cfg.precision == CGVC_PREC_F16F8;
-  ConvIO io; io.x = x_cl; io.xhi = A.xhi; io.xlo = A.xlo; io.n = n; io.H = 1; at(io, T);
+  ConvIO io = at(x_cl, A.xhi, A.xlo, T);
   if (edge) {
     // h1 = dense [n*T, kw*F] x [kw*F, 2*128] GEMM on the im2col of the input
-    CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), qm, A.xchi, A.xclo, st, A.off, A.n));
-    int r = tc_conv_fwd(e->tcw, N.h1c_slot, e->cfg.precision, A.xchi, A.xclo, n, 1, T, 1, 1, A.h1.P, st);
-    if (r != 0) return fail(e, r == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc h1 fwd (tap-lowered): %d", r);
+    CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
+                          A.xchi, A.xclo, st, A.off, A.n));
+    RET(tc_result(e, tc_conv_fwd(e->tcw, N.h1c_slot, A.xchi, A.xclo, n, 1, T, 1, 1, A.h1.P, st), &N.h1.a, "forward (tap-lowered)"));
+    PostParams q = post_params(e, N.h1, io, A.h1, T, keep_y, A.post); CK(launch_post_fwd(q, st));
   } else {
-    if (A.xhi && tc_enabled(e)) {
-      if (qm) CK(launch_pad_split_q(x_cl, (long long)n * T, nf, nf, 128, A.xhi, A.xlo, st));
-      else CK(launch_pad_split(x_cl, (long long)n * T, nf, nf, 64, A.xhi, A.xlo, st));
-    }
-    RET(gated_conv_fwd(e, N.h1, io, A.h1.P, st));
+    if (A.xhi && tc_enabled(e)) CK(tc_split_planes(e->cfg.precision, x_cl, (long long)n * T, nf, A.xhi, A.xlo, st));
+    RET(layer_forward(e, N.h1, io, A.h1, T, keep_y, save_pre, A.post, st));
   }
-  { PostParams q = post_params(e, N.h1, A.h1, n, T, keep_y, A.post); CK(launch_post_fwd(q, st)); }
   const GLAct* cur = &A.h1;
   int W = T;
   for (int i = 0; i < 2; ++i) {
-    io.x = cur->Y; io.xhi = cur->Yhi; io.xlo = cur->Ylo; at(io, W);
-    if (!keep_y && cur->Yhi) io.x = nullptr;
+    io = of(*cur, W);
     W /= 2;
-    RET(gated_layer_forward(e, N.d[i], io, A.d[i], n, W, keep_y || i == 1, A.post, st, save_pre, G));   // d2's fp32 output is the first residual input
+    RET(layer_forward(e, N.d[i], io, A.d[i], W, keep_y || i == 1, save_pre, A.post, st));   // d2's fp32 output is the first residual input
     cur = &A.d[i];
   }
-  const float* res = A.d[1].Y; const __nv_bfloat16 *rhi = A.d[1].Yhi, *rlo = A.d[1].Ylo;
-  for (int i = 0; i < 6; ++i) {
-    const ResBlock& R = N.r[i];
-    io.x = res; io.xhi = rhi; io.xlo = rlo; at(io, W);
-    RET(gated_layer_forward(e, R.h1, io, A.r[i].a, n, W, keep_y, A.post, st, save_pre, G));
-    ConvIO io2; io2.x = (keep_y || !A.r[i].a.Yhi) ? A.r[i].a.Y : nullptr; io2.xhi = A.r[i].a.Yhi; io2.xlo = A.r[i].a.Ylo; io2.n = n; io2.H = 1; at(io2, W);
-    bool done = false, fused = false;
-    if (use_tc(e, R.tc_slot2) && io2.xhi && packed) {
-      int r = tc_fwd_io(e, R.tc_slot2, io2, 1, 1, A.r[i].Pb, st);
-      if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc h2 fwd (packed): %s", cudaGetErrorString((cudaError_t)r));
-    } else if (use_tc(e, R.tc_slot2) && io2.xhi) {
-      TcFuse f; memset(&f, 0, sizeof f);
-      f.R = e->fuse_in && A.r[i].Yrhi ? W : 0;                // R = 0: plain conv epilogue
-      f.gamma_a = Pm + R.in2.gamma; f.beta_a = Pm + R.in2.beta; f.stats = save_pre ? A.r[i].sb : nullptr; f.resid = res;
-      f.y = A.r[i].Yr; f.y_hi = A.r[i].Yrhi; f.y_lo = A.r[i].Yrlo;
-      int r = tc_conv_fwd_fused(e->tcw, R.tc_slot2, e->cfg.precision, io2.xhi, io2.xlo, n, 1, W, 1, 1, (save_pre || !f.R) ? A.r[i].Pb : nullptr, f, &fused, st);
-      if (r != 0 && !save_pre && f.R) { f.stats = A.r[i].sb; r = tc_conv_fwd_fused(e->tcw, R.tc_slot2, e->cfg.precision, io2.xhi, io2.xlo, n, 1, W, 1, 1, A.r[i].Pb, f, &fused, st); }
-      if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc h2 fwd: %s", cudaGetErrorString((cudaError_t)r));
-    }
-    if (!done) RET(conv_fwd_simt(e, Pm, R.h2, 1, 1, io2, A.r[i].Pb, 512, 0, st));
-    if (fused) { res = A.r[i].Yr; rhi = A.r[i].Yrhi; rlo = A.r[i].Yrlo; continue; }
-    PostParams q; memset(&q, 0, sizeof q);
-    q.p = A.r[i].Pb; q.ldp = 512; q.Cc = 512; q.B = n; q.R = W; q.C = 512; q.sh = 1;
-    q.beta_a = Pm + R.in2.beta; q.gamma_a = Pm + R.in2.gamma; q.has_in = 1; q.has_gate = 0;
-    q.resid = res; q.y = A.r[i].Yr; q.stats = A.r[i].sb; q.y_hi = A.r[i].Yrhi; q.y_lo = A.r[i].Yrlo; q.scratch = A.post;
-    q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
-    if (G) pack_post(q, *G);
-    CK(launch_post_fwd(q, st));
-    res = A.r[i].Yr; rhi = A.r[i].Yrhi; rlo = A.r[i].Yrlo;
+  for (int i = 0; i < 6; ++i) {       // cur: the block input, whose fp32 copy is always written
+    RET(layer_forward(e, N.r[i].h1, at(cur->Y, cur->Yhi, cur->Ylo, W), A.r[i].h1, W, keep_y, save_pre, A.post, st));
+    RET(layer_forward(e, N.r[i].h2, of(A.r[i].h1, W), A.r[i].h2, W, true, save_pre, A.post, st, cur->Y));
+    cur = &A.r[i].h2;
   }
-  io.x = res; io.xhi = rhi; io.xlo = rlo;
+  io = at(cur->Y, cur->Yhi, cur->Ylo, W);
   for (int i = 0; i < 2; ++i) {
-    at(io, W);
-    RET(gated_layer_forward(e, N.u[i], io, A.u[i], n, W, keep_y, A.post, st, save_pre, G));      // W = conv rows per sample; the shuffle doubles them
+    RET(layer_forward(e, N.u[i], io, A.u[i], W, keep_y, save_pre, A.post, st));      // W = conv rows per sample; the shuffle doubles them
     W *= 2;
-    io.x = (keep_y || !A.u[i].Yhi) ? A.u[i].Y : nullptr; io.xhi = A.u[i].Yhi; io.xlo = A.u[i].Ylo;
+    io = of(A.u[i], W);
   }
-  at(io, W);
-  {
-    bool done = false;
-    if (edge && io.xhi) {
-      // o1: Z[m, (t, c)] = U[m, :] . W[t][:, c] as one dense GEMM, then out[m, c] = b[c] + sum_t Z[m + t - 7, (t, c)]
-      int r = tc_conv_fwd(e->tcw, N.o1f_slot, e->cfg.precision, io.xhi, io.xlo, n, 1, W, 1, 1, A.z, st);
-      if (r != 0) return fail(e, r == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc o1 fwd (tap-lowered): %d", r);
-      CK(launch_col2im_taps(A.z, N.o1.kw * nf, (long long)n * W, W, nf, N.o1.kw, +1, Pm + N.o1.b, A.out_cl, st, A.off, A.n));
-      done = true;
-    }
-    if (!done && use_tc(e, N.o1_slot) && io.xhi) {
-      int r = tc_fwd_io(e, N.o1_slot, io, 1, 1, A.out_cl, st);
-      if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc o1 fwd: %s", cudaGetErrorString((cudaError_t)r));
-    }
-    if (!done) RET(conv_fwd_simt(e, Pm, N.o1, 1, 1, io, A.out_cl, nf, 0, st));
+  if (edge && io.xhi) {
+    // o1: Z[m, (t, c)] = U[m, :] . W[t][:, c] as one dense GEMM, then out[m, c] = b[c] + sum_t Z[m + t - 7, (t, c)]
+    RET(tc_result(e, tc_conv_fwd(e->tcw, N.o1f_slot, io.xhi, io.xlo, n, 1, W, 1, 1, A.z, st), &N.o1.a, "forward (tap-lowered)"));
+    CK(launch_col2im_taps(A.z, N.o1.a.kw * nf, (long long)n * W, W, nf, N.o1.a.kw, +1, e->P() + N.o1.a.b, A.out_cl, st, A.off, A.n));
+  } else {
+    RET(conv_fwd(e, N.o1, io, A.out_cl, st));
   }
   if (keep_y) {
     e->taps.clear();
     size_t r1 = (size_t)n * T;
     e->taps["h1_glu"] = {A.h1.Y, r1 * 128}; e->taps["d1"] = {A.d[0].Y, r1 / 2 * 256}; e->taps["d2"] = {A.d[1].Y, r1 / 4 * 512};
-    for (int i = 0; i < 6; ++i) e->taps["r" + std::to_string(i + 1)] = {A.r[i].Yr, r1 / 4 * 512};
+    for (int i = 0; i < 6; ++i) e->taps["r" + std::to_string(i + 1)] = {A.r[i].h2.Y, r1 / 4 * 512};
     e->taps["u1"] = {A.u[0].Y, r1 / 2 * 512}; e->taps["u2"] = {A.u[1].Y, r1 * 256};
     e->taps["out_cl"] = {A.out_cl, r1 * (size_t)nf};
   }
   return 0;
 }
 
+// ---- backward -----------------------------------------------------------------------------------------------
 struct BwdScratch { float *bufA, *bufB, *dP; __nv_bfloat16 *dPhi, *dPlo; float* post;
                     __nv_bfloat16 *dP2hi, *dP2lo;      // second plane pair: a fused dgrad epilogue writes the next layer's dP while reading this one's
                     __nv_bfloat16 *dPbhi, *dPblo;      // ping-pong partner of dPhi / dPlo (same size) for the side-stream weight gradients
                     SideQ* sq; };
 
-struct PlanePair { __nv_bfloat16 *hi, *lo; };
+static bool side_on(const BwdScratch& S) { return S.sq && S.sq->on && S.dPbhi; }
 
-// fp32 dP is only materialised when a SIMT kernel will read it
-static PostBwdParams post_bwd_params(const cgvc_engine* e, const Gated& L, const float* dy, const GLAct& A,
-                                     int n, int rows_per_sample_out, const BwdScratch& S, bool wgrad, bool need_fp32,
-                                     const PlanePair* out = nullptr) {
-  PostBwdParams q; memset(&q, 0, sizeof q);
-  const float* Pm = e->P(); float* Gm = e->G();
-  q.dy1 = dy; q.p = A.P; q.ldp = 2 * L.a.cout; q.Cc = L.a.cout; q.B = n; q.sh = L.shuffle;
-  q.R = rows_per_sample_out * L.shuffle; q.C = L.a.cout / L.shuffle;
-  q.has_in = L.has_in; q.has_gate = 1; q.stats = A.stats;
-  if (L.has_in) {
-    q.beta_a = Pm + L.ina.beta; q.gamma_a = Pm + L.ina.gamma; q.beta_g = Pm + L.ing.beta; q.gamma_g = Pm + L.ing.gamma;
-    if (wgrad) { q.dbeta_a = Gm + L.ina.beta; q.dgamma_a = Gm + L.ina.gamma; q.dbeta_g = Gm + L.ing.beta; q.dgamma_g = Gm + L.ing.gamma; }
-  }
-  if (wgrad) { q.dbias_a = Gm + L.a.b; q.dbias_g = Gm + L.g.b; }
-  q.scratch = S.post;
-  const bool tc = use_tc(e, L.tc_slot) && S.dPhi;
-  q.dp = (!tc || need_fp32) ? S.dP : nullptr;
-  if (tc) { q.dp_hi = out ? out->hi : S.dPhi; q.dp_lo = out ? out->lo : S.dPlo; }
-  q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
-  return q;
-}
+// The dP planes of one backward walk.  Fused backward (tensor-core path, fuse_bwd): a stride-1 data-gradient launch whose result is
+// d loss / d (output of an instance-normed layer) runs that layer's instance-norm (+GLU) backward in its epilogue and writes the
+// layer's dP planes directly, reading one plane pair while writing the other.
+struct BwdWalk {
+  const BwdScratch& S;
+  bool fuse;                  // fuse_bwd in effect
+  PlanePair pb[2];            // [0]: the planes a GLU / instance-norm backward writes (side_wgrad off), [1]: its fused-epilogue partner
+  int have = -1;              // pb[have] already holds the dP planes of the layer differentiated next, or -1
+  int cur = 0;                // the pb index of the planes handed out last
+  BwdWalk(const BwdScratch& s, bool f) : S(s), fuse(f), pb{{s.dPhi, s.dPlo}, {s.dP2hi, s.dP2lo}} {}
+};
 
-// the plane pair the next GLU / instance-norm backward may write (waits, on st, for the weight gradient that last read it)
-static PlanePair dp_acquire(const BwdScratch& S, cudaStream_t st) {
-  SideQ* q = S.sq;
-  if (!q || !q->on || !S.dPbhi) return PlanePair{S.dPhi, S.dPlo};
+// The dP plane pair of the next layer: the one the previous data-gradient launch's fused epilogue wrote (*written), else the pair for
+// its GLU / instance-norm backward to write: with side_wgrad the ping-pong buffer, once the weight gradient that last read it (on the
+// side stream) has finished
+static PlanePair dp_planes(BwdWalk& w, cudaStream_t st, bool* written = nullptr) {
+  if (written) *written = w.have >= 0;
+  if (w.have >= 0) { w.cur = w.have; w.have = -1; return w.pb[w.cur]; }
+  w.cur = 0;
+  if (!side_on(w.S)) return w.pb[0];
+  SideQ* q = w.S.sq;
   q->cur ^= 1;
   if (q->used[q->cur]) cudaStreamWaitEvent(st, q->done[q->cur], 0);
-  return q->cur ? PlanePair{S.dPbhi, S.dPblo} : PlanePair{S.dPhi, S.dPlo};
+  return q->cur ? PlanePair{w.S.dPbhi, w.S.dPblo} : PlanePair{w.S.dPhi, w.S.dPlo};
 }
-// stream for the weight gradient of the planes acquired last (their producer has been enqueued on st) ...
-static cudaStream_t wgrad_begin(const BwdScratch& S, cudaStream_t st) {
+
+// Runs wgrad(stream), a weight gradient of the planes handed out last.  With side_wgrad and planes, on the side stream behind an
+// event on them, recording when it is done with them; else on st
+template <class F> static int run_wgrad(const BwdScratch& S, bool planes, cudaStream_t st, F&& wgrad) {
+  if (!planes || !side_on(S)) return wgrad(st);
   SideQ* q = S.sq;
-  if (!q || !q->on || !S.dPbhi) return st;
   cudaEventRecord(q->ready[q->cur], st);
   cudaStreamWaitEvent(q->side, q->ready[q->cur], 0);
-  return q->side;
-}
-// ... and the end of that weight gradient
-static void wgrad_end(const BwdScratch& S) {
-  SideQ* q = S.sq;
-  if (!q || !q->on || !S.dPbhi) return;
+  const int r = wgrad(q->side);
   cudaEventRecord(q->done[q->cur], q->side);
   q->used[q->cur] = true;
+  return r;
 }
+
 // every side-stream weight gradient of this lane has finished before st continues
 static void side_join(const BwdScratch& S, cudaStream_t st) {
   SideQ* q = S.sq;
@@ -611,26 +582,73 @@ static void side_join(const BwdScratch& S, cudaStream_t st) {
   for (int b = 0; b < 2; ++b) if (q->used[b]) { cudaStreamWaitEvent(st, q->done[b], 0); q->used[b] = false; }
 }
 
-// fused-backward descriptors (see tc_conv_dgrad_fused): instance-norm backward of a residual block's h2 convolution ...
-static TcBwdFuse in2_bwd_fuse(const cgvc_engine* e, const ResBlock& R, const float* Pb, const float* sb, int rows_per_sample, PlanePair out) {
-  TcBwdFuse f; memset(&f, 0, sizeof f);
+// GLU / instance-norm backward of a layer into dP planes `out`; fp32 dP is only materialised when a SIMT kernel will read it
+static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const float* dy, const GLAct& A, int n, int rows_per_sample_out,
+                                     const BwdScratch& S, bool wgrad, bool need_fp32, PlanePair out) {
+  PostBwdParams q; memset(&q, 0, sizeof q);
   const float* Pm = e->P(); float* Gm = e->G();
-  f.R = rows_per_sample; f.gated = 0; f.bp = Pb; f.bp_ld = 512; f.stats = sb;
-  f.gamma_a = Pm + R.in2.gamma; f.beta_a = Pm + R.in2.beta;
-  f.dp_hi = out.hi; f.dp_lo = out.lo; f.dp_ld = 512;
-  f.dgamma_a = Gm + R.in2.gamma; f.dbeta_a = Gm + R.in2.beta;
-  return f;
+  q.dy1 = dy; q.p = A.P; q.ldp = L.width(); q.Cc = L.a.cout; q.B = n; q.sh = L.shuffle;
+  q.R = rows_per_sample_out * L.shuffle; q.C = L.a.cout / L.shuffle;
+  q.has_in = L.has_in; q.has_gate = L.gated(); q.stats = A.stats;
+  if (L.has_in) {
+    q.beta_a = Pm + L.ina.beta; q.gamma_a = Pm + L.ina.gamma;
+    if (wgrad) { q.dbeta_a = Gm + L.ina.beta; q.dgamma_a = Gm + L.ina.gamma; }
+  }
+  if (L.has_in && L.gated()) {
+    q.beta_g = Pm + L.ing.beta; q.gamma_g = Pm + L.ing.gamma;
+    if (wgrad) { q.dbeta_g = Gm + L.ing.beta; q.dgamma_g = Gm + L.ing.gamma; }
+  }
+  if (wgrad) { q.dbias_a = Gm + L.a.b; if (L.gated()) q.dbias_g = Gm + L.g.b; }
+  q.scratch = S.post;
+  const bool tc = use_tc(e, L.tc_slot) && S.dPhi;
+  q.dp = (!tc || need_fp32) ? S.dP : nullptr;
+  if (tc) { q.dp_hi = out.hi; q.dp_lo = out.lo; }
+  q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+  return q;
 }
-// ... and GLU + instance-norm backward of a gated layer (no pixel shuffle)
-static TcBwdFuse gated_bwd_fuse(const cgvc_engine* e, const Gated& L, const GLAct& A, int rows_per_sample, PlanePair out) {
+
+// the fused backward epilogue (tc_conv_dgrad) of L's instance norm (+ GLU; no pixel shuffle), writing its dP planes into `out`
+static TcBwdFuse bwd_fuse(const cgvc_engine* e, const Layer& L, const GLAct& A, int rows_per_sample, PlanePair out) {
   TcBwdFuse f; memset(&f, 0, sizeof f);
   const float* Pm = e->P(); float* Gm = e->G();
   f.R = (L.has_in && L.shuffle == 1) ? rows_per_sample : 0;      // R = 0: not fusable
-  f.gated = 1; f.bp = A.P; f.bp_ld = 2 * L.a.cout; f.stats = A.stats;
-  f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta; f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta;
-  f.dp_hi = out.hi; f.dp_lo = out.lo; f.dp_ld = 2 * L.a.cout;
-  f.dgamma_a = Gm + L.ina.gamma; f.dbeta_a = Gm + L.ina.beta; f.dgamma_g = Gm + L.ing.gamma; f.dbeta_g = Gm + L.ing.beta;
+  f.gated = L.gated(); f.bp = A.P; f.bp_ld = L.width(); f.stats = A.stats;
+  f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta;
+  f.dp_hi = out.hi; f.dp_lo = out.lo; f.dp_ld = L.width();
+  f.dgamma_a = Gm + L.ina.gamma; f.dbeta_a = Gm + L.ina.beta;
+  if (L.gated()) { f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta; f.dgamma_g = Gm + L.ing.gamma; f.dbeta_g = Gm + L.ing.beta; }
   return f;
+}
+
+// dP of a layer: the GLU / instance-norm backward kernel, unless the previous data-gradient launch's fused epilogue wrote it
+static int layer_dp(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAct& A, const float* dy, int n, int rows_per_sample_out,
+                    bool wgrad, cudaStream_t st, PostBwdParams& q) {
+  bool written = false;
+  const PlanePair out = dp_planes(w, st, &written);
+  q = post_bwd_params(e, L, dy, A, n, rows_per_sample_out, w.S, wgrad, false, out);
+  if (!written) CK(launch_post_bwd(q, st));
+  return 0;
+}
+
+// Backward through one layer, whose input was `in` and upstream gradient is dy: (1) dP (layer_dp); (2) with wgrad, the weight
+// gradient (run_wgrad); (3) dx (+)= the data gradient (dx null: none), with the instance-norm backward of `up` -- the layer whose
+// output is `in`, activations upA -- fused into its epilogue under fuse_bwd where the shape allows
+static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAct& A, const ConvIO& in, const float* dy,
+                          int rows_per_sample_out, bool wgrad, float* dx, int accumulate, cudaStream_t st,
+                          const Layer* up = nullptr, const GLAct* upA = nullptr) {
+  PostBwdParams q;
+  RET(layer_dp(e, w, L, A, dy, in.n, rows_per_sample_out, wgrad, st, q));
+  const PlanePair dp{q.dp_hi, q.dp_lo};
+  if (wgrad) RET(run_wgrad(w.S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, L, in, q.dp, dp, ws); }));
+  if (!dx) return 0;
+  const int other = 1 - w.cur;
+  TcBwdFuse f;
+  const bool fuse = up && w.fuse && dp.hi;
+  if (fuse) f = bwd_fuse(e, *up, *upA, in.W, w.pb[other]);
+  bool fused = false;
+  RET(conv_dgrad(e, L, in, q.dp, dp, dx, accumulate, st, fuse ? &f : nullptr, &fused));
+  if (fused) w.have = other;
+  return 0;
 }
 
 // Backward through one generator application.  d_out_cl: [n*T, 24] gradient w.r.t. the channels-last output.
@@ -638,191 +656,68 @@ static TcBwdFuse gated_bwd_fuse(const cgvc_engine* e, const Gated& L, const GLAc
 static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A, const float* d_out_cl, float* d_in_cl,
                               const BwdScratch& S, cudaStream_t st) {
   const int n = A.n, T = A.T, nf = e->cfg.num_features;
-  const float* Pm = e->P(); float* Gm = e->G();
-  ConvIO io; io.n = n; io.H = 1;
+  float* Gm = e->G();
+  auto at = [&](const float* x, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int W) {
+    ConvIO io; io.x = x; io.xhi = hi; io.xlo = lo; io.n = n; io.H = 1; io.W = W; return io;
+  };
+  auto of = [&](const GLAct& a, int W) { return at(a.Y, a.Yhi, a.Ylo, W); };
+  BwdWalk w(S, e->fuse_bwd && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi && A.r[0].h2.Yhi);
+  const bool edge = edge_on(e, N) && A.xchi && A.z;
   // o1 (no norm, no gate): bias gradient = column sums of d_out
-  io.x = A.u[1].Y; io.xhi = A.u[1].Yhi; io.xlo = A.u[1].Ylo; io.W = T;
-  CK(launch_colsum(d_out_cl, (long long)n * T, nf, 0, nf, Gm + N.o1.b, st));
-  {
-    bool done = false;
-    const bool edge = edge_on(e, N) && A.xchi && A.z;
-    if (edge && io.xhi && S.dPhi) {
-      // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
-      const PlanePair pp = dp_acquire(S, st);
-      CK(launch_im2col_taps(d_out_cl, (long long)n * T, T, nf, N.o1.kw, -1, edge_cpad(N.o1.kw * nf), e->cfg.precision == CGVC_PREC_F16F8, pp.hi, pp.lo, st));
-      cudaStream_t ws = wgrad_begin(S, st);
-      int r = tc_conv_wgrad(e->tcw, N.o1f_slot, e->cfg.precision, io.xhi, io.xlo, pp.hi, pp.lo, n, 1, T, 1, 1, Gm + N.o1.k, nullptr, nullptr, nullptr, ws);
-      wgrad_end(S);
-      if (r == 0) r = tc_conv_dgrad(e->tcw, N.o1f_slot, e->cfg.precision, pp.hi, pp.lo, n, 1, T, 1, 1, S.bufA, 0, st);
-      if (r != 0) return fail(e, r == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc o1 bwd (tap-lowered): %d", r);
-      done = true;
+  CK(launch_colsum(d_out_cl, (long long)n * T, nf, 0, nf, Gm + N.o1.a.b, st));
+  const ConvIO u2 = of(A.u[1], T);
+  if (edge && u2.xhi && S.dPhi) {
+    // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
+    const PlanePair dp = dp_planes(w, st);
+    CK(launch_im2col_taps(d_out_cl, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
+                          dp.hi, dp.lo, st));
+    RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
+      return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, u2.xhi, u2.xlo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws),
+                       &N.o1.a, "weight gradient (tap-lowered)"); }));
+    RET(tc_result(e, tc_conv_dgrad(e->tcw, N.o1f_slot, dp.hi, dp.lo, n, 1, T, 1, 1, S.bufA, 0, st), &N.o1.a, "data gradient (tap-lowered)"));
+  } else {
+    PlanePair dp{nullptr, nullptr};
+    if (use_tc(e, N.o1.tc_slot) && u2.xhi && S.dPhi) {
+      dp = dp_planes(w, st);
+      CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st));
     }
-    if (!done && use_tc(e, N.o1_slot) && io.xhi && S.dPhi) {
-      const PlanePair pp = dp_acquire(S, st);
-      if (e->cfg.precision == CGVC_PREC_F16F8) CK(launch_pad_split_q(d_out_cl, (long long)n * T, nf, nf, 128, pp.hi, pp.lo, st));
-      else CK(launch_pad_split(d_out_cl, (long long)n * T, nf, nf, 64, pp.hi, pp.lo, st));
-      cudaStream_t ws = wgrad_begin(S, st);
-      int r = tc_conv_wgrad(e->tcw, N.o1_slot, e->cfg.precision, io.xhi, io.xlo, pp.hi, pp.lo, n, 1, T, 1, 1, Gm + N.o1.k, nullptr, nullptr, nullptr, ws);
-      wgrad_end(S);
-      if (r == 0) r = tc_conv_dgrad(e->tcw, N.o1_slot, e->cfg.precision, pp.hi, pp.lo, n, 1, T, 1, 1, S.bufA, 0, st);
-      if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc o1 bwd: %s", cudaGetErrorString((cudaError_t)r));
-    }
-    if (!done) {
-      RET(conv_wgrad_simt(e, Gm, N.o1, 1, 1, io, d_out_cl, nf, 0, st));
-      RET(conv_dgrad_simt(e, Pm, N.o1, 1, 1, n, 1, T, d_out_cl, nf, 0, S.bufA, 0, st));
-    }
+    RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, u2, d_out_cl, dp, ws); }));
+    RET(conv_dgrad(e, N.o1, u2, d_out_cl, dp, S.bufA, 0, st));
   }
   float* cur = S.bufA; float* oth = S.bufB;
-  int W = T;      // W tracks the output width of the layer being differentiated
-  // Fused backward (tensor-core path): a stride-1 data-gradient launch whose result is d loss / d (output of an instance-normed
-  // layer) runs that layer's instance-norm (+GLU) backward in its epilogue and writes the layer's dP planes directly.  It reads
-  // one plane pair while writing the other: pb[0] / pb[1]; `have` = which pair holds the dP planes of the layer differentiated next.
-  const bool side_on = S.sq && S.sq->on && S.dPbhi;
-  const bool fuse_ok = e->fuse_bwd && !side_on && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].a.Yhi && A.r[0].Yrhi;
-  PlanePair pb[2] = {{S.dPhi, S.dPlo}, {S.dP2hi, S.dP2lo}};
-  int have = -1;
-  for (int i = 1; i >= 0; --i) {
-    // upsample block i: conv at width W/2 -> shuffle -> width W
-    int Wc = W / 2;
-    const float* Xin; const __nv_bfloat16 *Xhi, *Xlo;
-    if (i == 1) { Xin = A.u[0].Y; Xhi = A.u[0].Yhi; Xlo = A.u[0].Ylo; } else { Xin = A.r[5].Yr; Xhi = A.r[5].Yrhi; Xlo = A.r[5].Yrlo; }
-    const PlanePair ppu = dp_acquire(S, st);
-    PostBwdParams q = post_bwd_params(e, N.u[i], cur, A.u[i], n, Wc, S, true, false, &ppu);
-    CK(launch_post_bwd(q, st));
-    io.x = Xin; io.xhi = Xhi; io.xlo = Xlo; io.W = Wc;
-    { cudaStream_t ws = q.dp_hi ? wgrad_begin(S, st) : st;
-      int rw = gated_conv_wgrad(e, N.u[i], io, q.dp, q.dp_hi, q.dp_lo, ws);
-      if (q.dp_hi) wgrad_end(S);
-      RET(rw); }
-    bool fusedu = false;
-    if (i == 0 && fuse_ok) {
-      // u1's data gradient is d loss / d (residual block 6 output): run that block's h2 instance-norm backward in the epilogue
-      TcBwdFuse f = in2_bwd_fuse(e, N.r[5], A.r[5].Pb, A.r[5].sb, Wc, pb[1]);
-      int r = tc_conv_dgrad_fused(e->tcw, N.u[0].tc_slot, e->cfg.precision, q.dp_hi, q.dp_lo, n, 1, Wc, 1, 1, oth, 0, f, &fusedu, st);
-      if (r != 0 && r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc u1 dgrad (fused): %s", cudaGetErrorString((cudaError_t)r));
-      if (r != 0) fusedu = false;
-      if (r == 0 && fusedu) have = 1;
-      if (r != 0) RET(gated_conv_dgrad(e, N.u[i], n, 1, Wc, q.dp, q.dp_hi, q.dp_lo, oth, 0, st));
-    } else {
-      RET(gated_conv_dgrad(e, N.u[i], n, 1, Wc, q.dp, q.dp_hi, q.dp_lo, oth, 0, st));
-    }
-    float* t = cur; cur = oth; oth = t;
-    W = Wc;
-  }
-  // residual blocks (width W = T/4); cur holds d(block output)
+  // up-sampling blocks, convolutions at T/2 and T/4 (the shuffle doubles the rows).  u1's data gradient is d loss / d (residual block
+  // 6 output), so its launch can run that block's h2 instance-norm backward
+  RET(layer_backward(e, w, N.u[1], A.u[1], of(A.u[0], T / 2), cur, T / 2, true, oth, 0, st));
+  std::swap(cur, oth);
+  RET(layer_backward(e, w, N.u[0], A.u[0], of(A.r[5].h2, T / 4), cur, T / 4, true, oth, 0, st, &N.r[5].h2, &A.r[5].h2));
+  std::swap(cur, oth);
+  // residual blocks (width T/4); cur holds d(block output).  h2's data gradient is d loss / d (h1's GLU output); h1's is added to cur
+  // in place (the skip), making it d loss / d (previous block's output) -- or, for the first block, of the second down-sampling
+  // layer's output
   for (int i = 5; i >= 0; --i) {
-    const ResBlock& R = N.r[i];
-    const float* Xin; const __nv_bfloat16 *Xhi, *Xlo;
-    if (i == 0) { Xin = A.d[1].Y; Xhi = A.d[1].Yhi; Xlo = A.d[1].Ylo; } else { Xin = A.r[i - 1].Yr; Xhi = A.r[i - 1].Yrhi; Xlo = A.r[i - 1].Yrlo; }
-    const bool tc2 = use_tc(e, R.tc_slot2) && S.dPhi && A.r[i].a.Yhi;
-    // (1) dP of the h2 convolution: already in pb[have] when the previous data-gradient launch fused it, else the streaming kernels
-    int b2 = have;
-    if (b2 < 0) {
-      if (side_on) pb[0] = dp_acquire(S, st);
-      PostBwdParams q; memset(&q, 0, sizeof q);
-      q.dy1 = cur; q.p = A.r[i].Pb; q.ldp = 512; q.Cc = 512; q.B = n; q.R = W; q.C = 512; q.sh = 1;
-      q.beta_a = Pm + R.in2.beta; q.gamma_a = Pm + R.in2.gamma; q.has_in = 1; q.has_gate = 0; q.stats = A.r[i].sb;
-      q.dp = tc2 ? nullptr : S.dP; if (tc2) { q.dp_hi = pb[0].hi; q.dp_lo = pb[0].lo; }
-      q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
-      q.scratch = S.post;
-      q.dbeta_a = Gm + R.in2.beta; q.dgamma_a = Gm + R.in2.gamma; q.dbias_a = Gm + R.h2.b;
-      CK(launch_post_bwd(q, st));
-      b2 = 0;
-    }
-    have = -1;
-    ConvIO io2; io2.x = A.r[i].a.Y; io2.xhi = A.r[i].a.Yhi; io2.xlo = A.r[i].a.Ylo; io2.n = n; io2.H = 1; io2.W = W;
-    // (2) h2: weight gradient, then data gradient = d loss / d (h1's GLU output), with h1's GLU + instance-norm backward fused
-    bool done = false, fused1 = false;
-    int b1 = 0;
-    if (tc2) {
-      cudaStream_t ws = side_on ? wgrad_begin(S, st) : st;
-      int r = tc_conv_wgrad(e->tcw, R.tc_slot2, e->cfg.precision, io2.xhi, io2.xlo, pb[b2].hi, pb[b2].lo, n, 1, W, 1, 1,
-                            Gm + R.h2.k, nullptr, nullptr, nullptr, ws);
-      if (side_on) wgrad_end(S);
-      if (r == 0) {
-        if (fuse_ok && use_tc(e, R.h1.tc_slot)) {
-          TcBwdFuse f = gated_bwd_fuse(e, R.h1, A.r[i].a, W, pb[1 - b2]);
-          r = tc_conv_dgrad_fused(e->tcw, R.tc_slot2, e->cfg.precision, pb[b2].hi, pb[b2].lo, n, 1, W, 1, 1, oth, 0, f, &fused1, st);
-          if (r == 0 && fused1) b1 = 1 - b2;
-        } else {
-          r = tc_conv_dgrad(e->tcw, R.tc_slot2, e->cfg.precision, pb[b2].hi, pb[b2].lo, n, 1, W, 1, 1, oth, 0, st);
-        }
-      }
-      if (r == 0) done = true; else if (r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc h2 bwd: %s", cudaGetErrorString((cudaError_t)r));
-    }
-    if (!done) {
-      RET(conv_wgrad_simt(e, Gm, R.h2, 1, 1, io2, S.dP, 512, 0, st));
-      RET(conv_dgrad_simt(e, Pm, R.h2, 1, 1, n, 1, W, S.dP, 512, 0, oth, 0, st));
-    }
-    const float* dp1 = nullptr; const __nv_bfloat16 *dp1hi = pb[b1].hi, *dp1lo = pb[b1].lo;
-    if (!fused1) {
-      // writes pb[0] (free again: h2's launches are done), or the other buffer of the ping-pong when the weight gradients run aside
-      const PlanePair pp1 = side_on ? dp_acquire(S, st) : pb[0];
-      PostBwdParams q2 = post_bwd_params(e, R.h1, oth, A.r[i].a, n, W, S, true, false, &pp1);
-      CK(launch_post_bwd(q2, st));
-      dp1 = q2.dp; dp1hi = q2.dp_hi; dp1lo = q2.dp_lo; b1 = 0;
-    }
-    // (3) h1: weight gradient, then d_in = d_out (skip) + data gradient, in place in `cur`; that is d loss / d (previous block's
-    //     output) -- or, for the first block, of the second down-sampling layer's output: fuse that layer's backward as well
-    io.x = Xin; io.xhi = Xhi; io.xlo = Xlo; io.W = W;
-    { cudaStream_t ws = (side_on && dp1hi) ? wgrad_begin(S, st) : st;
-      int rw = gated_conv_wgrad(e, R.h1, io, dp1, dp1hi, dp1lo, ws);
-      if (side_on && dp1hi) wgrad_end(S);
-      RET(rw); }
-    bool fused0 = false;
-    if (fuse_ok && use_tc(e, R.h1.tc_slot) && dp1hi) {
-      TcBwdFuse f = (i > 0) ? in2_bwd_fuse(e, N.r[i - 1], A.r[i - 1].Pb, A.r[i - 1].sb, W, pb[1 - b1])
-                            : gated_bwd_fuse(e, N.d[1], A.d[1], W, pb[1 - b1]);
-      int r = tc_conv_dgrad_fused(e->tcw, R.h1.tc_slot, e->cfg.precision, dp1hi, dp1lo, n, 1, W, 1, 1, cur, 1, f, &fused0, st);
-      if (r != 0 && r != TC_UNSUPPORTED) return fail(e, CGVC_ERR_CUDA, "tc h1 dgrad (fused): %s", cudaGetErrorString((cudaError_t)r));
-      if (r != 0) { fused0 = false; RET(gated_conv_dgrad(e, R.h1, n, 1, W, dp1, dp1hi, dp1lo, cur, 1, st)); }
-      if (fused0) have = 1 - b1;
-    } else {
-      RET(gated_conv_dgrad(e, R.h1, n, 1, W, dp1, dp1hi, dp1lo, cur, 1, st));
-    }
+    const Layer& Lin = i > 0 ? N.r[i - 1].h2 : N.d[1];
+    const GLAct& Ain = i > 0 ? A.r[i - 1].h2 : A.d[1];
+    RET(layer_backward(e, w, N.r[i].h2, A.r[i].h2, of(A.r[i].h1, T / 4), cur, T / 4, true, oth, 0, st, &N.r[i].h1, &A.r[i].h1));
+    RET(layer_backward(e, w, N.r[i].h1, A.r[i].h1, of(Ain, T / 4), oth, T / 4, true, cur, 1, st, &Lin, &Ain));
   }
-  // downsample blocks
-  for (int i = 1; i >= 0; --i) {
-    const GLAct& in = (i == 1) ? A.d[0] : A.h1;
-    const PlanePair ppd = (i == 1 && have >= 0) ? pb[have] : dp_acquire(S, st);
-    PostBwdParams q = post_bwd_params(e, N.d[i], cur, A.d[i], n, W, S, true, false, &ppd);
-    if (i == 1 && have >= 0) { q.dp = nullptr; q.dp_hi = pb[have].hi; q.dp_lo = pb[have].lo; have = -1; }   // produced by the fused epilogue of r1.h1's dgrad
-    else CK(launch_post_bwd(q, st));
-    io.x = in.Y; io.xhi = in.Yhi; io.xlo = in.Ylo; io.W = W * 2;
-    { cudaStream_t ws = (side_on && q.dp_hi) ? wgrad_begin(S, st) : st;
-      int rw = gated_conv_wgrad(e, N.d[i], io, q.dp, q.dp_hi, q.dp_lo, ws);
-      if (side_on && q.dp_hi) wgrad_end(S);
-      RET(rw); }
-    RET(gated_conv_dgrad(e, N.d[i], n, 1, W * 2, q.dp, q.dp_hi, q.dp_lo, oth, 0, st));
-    float* t = cur; cur = oth; oth = t;
-    W *= 2;
-  }
+  // down-sampling blocks (stride 2)
+  RET(layer_backward(e, w, N.d[1], A.d[1], of(A.d[0], T / 2), cur, T / 4, true, oth, 0, st));
+  std::swap(cur, oth);
+  RET(layer_backward(e, w, N.d[0], A.d[0], of(A.h1, T), cur, T / 2, true, oth, 0, st));
+  std::swap(cur, oth);
   // h1 (no IN)
-  {
-    const PlanePair pph = dp_acquire(S, st);
-    PostBwdParams q = post_bwd_params(e, N.h1, cur, A.h1, n, T, S, true, false, &pph);
-    CK(launch_post_bwd(q, st));
-    io.x = A.x_cl; io.xhi = A.xhi; io.xlo = A.xlo; io.W = T;
-    if (edge_on(e, N) && A.xchi && A.z && q.dp_hi) {
-      // tap-lowered h1: the weight gradient is im2col(x)^T dP straight into the [15,24,128] kernels' GRAD ranges; the data gradient
-      // (cycle passes only) is the dense dP . W^T [n*T, kw*F] followed by the tap-shifted sum
-      { cudaStream_t ws = side_on ? wgrad_begin(S, st) : st;
-        int rw = tc_conv_wgrad(e->tcw, N.h1c_slot, e->cfg.precision, A.xchi, A.xclo, q.dp_hi, q.dp_lo, n, 1, T, 1, 1,
-                               Gm + N.h1.a.k, Gm + N.h1.g.k, nullptr, nullptr, ws);
-        if (side_on) wgrad_end(S);
-        if (rw != 0) return fail(e, rw == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc h1 wgrad (tap-lowered): %d", rw); }
-      if (d_in_cl) {
-        int r = tc_conv_dgrad(e->tcw, N.h1c_slot, e->cfg.precision, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, oth, 0, st);
-        if (r != 0) return fail(e, r == TC_UNSUPPORTED ? CGVC_ERR_UNSUPPORTED : CGVC_ERR_CUDA, "tc h1 dgrad (tap-lowered): %d", r);
-        CK(launch_col2im_taps(oth, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, d_in_cl, st));
-      }
-      return 0;
-    }
-    { cudaStream_t ws = (side_on && q.dp_hi) ? wgrad_begin(S, st) : st;
-      int rw = gated_conv_wgrad(e, N.h1, io, q.dp, q.dp_hi, q.dp_lo, ws);
-      if (side_on && q.dp_hi) wgrad_end(S);
-      RET(rw); }
-    if (d_in_cl) RET(gated_conv_dgrad(e, N.h1, n, 1, T, q.dp, q.dp_hi, q.dp_lo, d_in_cl, 0, st));
+  const ConvIO x = at(A.x_cl, A.xhi, A.xlo, T);
+  if (!edge) return layer_backward(e, w, N.h1, A.h1, x, cur, T, true, d_in_cl, 0, st);
+  // tap-lowered h1: the weight gradient is im2col(x)^T dP straight into the [15,24,128] kernels' GRAD ranges; the data gradient
+  // (cycle passes only) is the dense dP . W^T [n*T, kw*F] followed by the tap-shifted sum
+  PostBwdParams q;
+  RET(layer_dp(e, w, N.h1, A.h1, cur, n, T, true, st, q));
+  RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
+    return tc_result(e, tc_conv_wgrad(e->tcw, N.h1c_slot, A.xchi, A.xclo, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, Gm + N.h1.a.k, Gm + N.h1.g.k, ws),
+                     &N.h1.a, "weight gradient (tap-lowered)"); }));
+  if (d_in_cl) {
+    RET(tc_result(e, tc_conv_dgrad(e->tcw, N.h1c_slot, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, oth, 0, st), &N.h1.a, "data gradient (tap-lowered)"));
+    CK(launch_col2im_taps(oth, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, d_in_cl, st));
   }
   return 0;
 }
@@ -850,19 +745,16 @@ static int discriminator_forward(cgvc_engine* e, const DiscNet& N, DiscActs& A, 
       256 % (N.h1.a.cout / 4) == 0) {
     // input layer (one input channel, K = 9, gate without norm): convolution + GLU in one HBM-bound pass; P is kept for the backward pass
     const GatherGeom g = fwd_geom(n, H0, T, N.h1.a.kh, N.h1.a.kw, N.h1.sh, N.h1.sw);
-    const PostParams q = post_params(e, N.h1, A.h1, n, H * W, keep_y, A.post);
+    const PostParams q = post_params(e, N.h1, io, A.h1, H * W, keep_y, A.post);
     CK(launch_conv_c1_glu_fwd(g, x, Pm + N.h1.a.k, Pm + N.h1.g.k, Pm + N.h1.a.b, Pm + N.h1.g.b, N.h1.a.cout, A.h1.P, q.y, q.y_hi, q.y_lo, q.qmode, st));
   } else {
-    RET(gated_conv_fwd(e, N.h1, io, A.h1.P, st));
-    PostParams q = post_params(e, N.h1, A.h1, n, H * W, keep_y, A.post); CK(launch_post_fwd(q, st));
+    RET(layer_forward(e, N.h1, io, A.h1, H * W, keep_y, true, A.post, st));
   }
   const GLAct* cur = &A.h1;
   for (int i = 0; i < 3; ++i) {
     io.x = (keep_y || !cur->Yhi) ? cur->Y : nullptr; io.xhi = cur->Yhi; io.xlo = cur->Ylo; io.H = H; io.W = W;
-    RET(gated_conv_fwd(e, N.d[i], io, A.d[i].P, st));
     int Ho, Wo; conv_out_dims(N.d[i].a, N.d[i].sh, N.d[i].sw, H, W, Ho, Wo); H = Ho; W = Wo;
-    PostParams q = post_params(e, N.d[i], A.d[i], n, H * W, keep_y, A.post);     // d3 has no planes: its fp32 output feeds the head
-    CK(launch_post_fwd(q, st));
+    RET(layer_forward(e, N.d[i], io, A.d[i], H * W, keep_y, true, A.post, st));     // d3 has no planes: its fp32 output feeds the head
     cur = &A.d[i];
   }
   CK(launch_head_fwd(cur->Y, (long long)n * H * W, 1024, Pm + N.dense_k, Pm + N.dense_b, A.prob, st));
@@ -904,21 +796,11 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   const float* dy = dY3;
   float* bufs[2] = {S.bufA, S.bufB};
   int flip = 0;
-  ConvIO io; io.n = n;
+  BwdWalk w(S, false);
   for (int i = 2; i >= 0; --i) {
     const GLAct& in = (i == 0) ? A.h1 : A.d[i - 1];
-    const PlanePair ppd = dp_acquire(S, st);
-    PostBwdParams q = post_bwd_params(e, N.d[i], dy, A.d[i], n, Hs[i + 1] * Ws[i + 1], S, wgrad, false, &ppd);
-    CK(launch_post_bwd(q, st));
-    io.x = in.Y; io.xhi = in.Yhi; io.xlo = in.Ylo; io.H = Hs[i]; io.W = Ws[i];
-    if (wgrad) {
-      const bool aside = S.sq && S.sq->on && S.dPbhi && q.dp_hi;
-      cudaStream_t ws = aside ? wgrad_begin(S, st) : st;
-      int rw = gated_conv_wgrad(e, N.d[i], io, q.dp, q.dp_hi, q.dp_lo, ws);
-      if (aside) wgrad_end(S);
-      RET(rw);
-    }
-    RET(gated_conv_dgrad(e, N.d[i], n, Hs[i], Ws[i], q.dp, q.dp_hi, q.dp_lo, bufs[flip], 0, st));
+    ConvIO io; io.x = in.Y; io.xhi = in.Yhi; io.xlo = in.Ylo; io.n = n; io.H = Hs[i]; io.W = Ws[i];
+    RET(layer_backward(e, w, N.d[i], A.d[i], io, dy, Hs[i + 1] * Ws[i + 1], wgrad, bufs[flip], 0, st));
     dy = bufs[flip]; flip ^= 1;
   }
   // h1: one input channel (K = 9), gate without instance norm.  Fused form: the GLU backward is recomputed inside the weight-gradient /
@@ -931,7 +813,7 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
     if (d_in) CK(launch_glu_bwd_dgrad_c1(dy, A.h1.P, 128, e->P() + N.h1.a.k, e->P() + N.h1.g.k, bufs[flip], d_in, n, H0, T, 3, 3, N.h1.sh, N.h1.sw, st));
     return 0;
   }
-  PostBwdParams q = post_bwd_params(e, N.h1, dy, A.h1, n, Hs[0] * Ws[0], S, wgrad, true);
+  PostBwdParams q = post_bwd_params(e, N.h1, dy, A.h1, n, Hs[0] * Ws[0], S, wgrad, true, PlanePair{S.dPhi, S.dPlo});
   CK(launch_post_bwd(q, st));
   if (wgrad) {
     GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
@@ -1036,12 +918,6 @@ int cgvc_create(const cgvc_config* cfg, cgvc_handle* out) {
   for (int i = 0; i < 2; ++i) { tb.scope = dn[i]; build_discriminator(tb, e->disc[i]); }
   e->n_params = (tb.off + 3) & ~(size_t)3;
   e->n_real_params = tb.real;
-  for (int i = 0; i < 2; ++i) {
-    GenNet& g = e->gen[i];
-    g.h1.tc_slot = -1; g.o1_slot = -1; g.h1c_slot = -1; g.o1f_slot = -1; for (int k = 0; k < 2; ++k) { g.d[k].tc_slot = -1; g.u[k].tc_slot = -1; }
-    for (int k = 0; k < 6; ++k) { g.r[k].h1.tc_slot = -1; g.r[k].tc_slot2 = -1; }
-    DiscNet& d = e->disc[i]; d.h1.tc_slot = -1; for (int k = 0; k < 3; ++k) d.d[k].tc_slot = -1;
-  }
   ce = post_init_kernels();
   if (ce != cudaSuccess) { delete e; return fail(nullptr, CGVC_ERR_CUDA, "post_init_kernels: %s", cudaGetErrorString(ce)); }
   ce = cudaMalloc(&e->d_scalars, 64 * sizeof(float));
@@ -1059,30 +935,26 @@ int cgvc_create(const cgvc_config* cfg, cgvc_handle* out) {
   cudaStreamCreateWithFlags(&e->graph_stream, cudaStreamNonBlocking);
   cudaEventCreateWithFlags(&e->ev_bridge, cudaEventDisableTiming); cudaEventCreateWithFlags(&e->ev_bridge2, cudaEventDisableTiming);
   if (cfg->precision != CGVC_PREC_FP32_SIMT) {
-    // register every dense gated layer with the tensor-core weight store
+    // register every dense layer with the tensor-core weight store (in this order: the F16F8 plane jobs of a network are contiguous)
+    auto reg = [&](Layer& L) {
+      L.tc_slot = tc_register(e->tcw, L.a.k, L.g.k, L.a.b, L.g.b, L.a.kh, L.a.kw, L.a.cin, L.a.cout, L.gated(), L.shuffle);
+    };
     for (int i = 0; i < 2; ++i) {
       GenNet& g = e->gen[i];
       // the 24-channel edge layers run on the tensor cores too (channel dims zero-padded to 64 / 128 inside the planes)
-      g.h1.tc_slot = tc_register(e->tcw, g.h1.a.k, g.h1.g.k, g.h1.a.b, g.h1.g.b, 1, 15, g.h1.a.cin, g.h1.a.cout, 1);
-      g.o1_slot = tc_register(e->tcw, g.o1.k, 0, g.o1.b, 0, 1, 15, g.o1.cin, g.o1.cout, 0);
+      reg(g.h1); reg(g.o1);
       // ... and, preferred (edge_lower), as dense 1 x 1 layers with the taps in the channel (h1) / column (o1) dimension: see edge_on
-      if ((g.h1.a.kw * g.h1.a.cin) % 4 == 0 && g.o1.cout % 4 == 0) {
-        g.h1c_slot = tc_register(e->tcw, g.h1.a.k, g.h1.g.k, g.h1.a.b, g.h1.g.b, 1, 1, g.h1.a.kw * g.h1.a.cin, g.h1.a.cout, 1);
-        g.o1f_slot = tc_register(e->tcw, g.o1.k, 0, g.o1.b, 0, 1, 1, g.o1.cin, g.o1.kw * g.o1.cout, 0, 1, g.o1.kw);
+      const ConvW &h1 = g.h1.a, &o1 = g.o1.a;
+      if ((h1.kw * h1.cin) % 4 == 0 && o1.cout % 4 == 0) {
+        g.h1c_slot = tc_register(e->tcw, h1.k, g.h1.g.k, h1.b, g.h1.g.b, 1, 1, h1.kw * h1.cin, h1.cout, 1);
+        g.o1f_slot = tc_register(e->tcw, o1.k, 0, o1.b, 0, 1, 1, o1.cin, o1.kw * o1.cout, 0, 1, o1.kw);
       }
-      for (int k = 0; k < 2; ++k) g.d[k].tc_slot = tc_register(e->tcw, g.d[k].a.k, g.d[k].g.k, g.d[k].a.b, g.d[k].g.b, 1, 5, g.d[k].a.cin, g.d[k].a.cout, 1);
-      for (int k = 0; k < 6; ++k) {
-        g.r[k].h1.tc_slot = tc_register(e->tcw, g.r[k].h1.a.k, g.r[k].h1.g.k, g.r[k].h1.a.b, g.r[k].h1.g.b, 1, 3, 512, 1024, 1);
-        g.r[k].tc_slot2 = tc_register(e->tcw, g.r[k].h2.k, 0, g.r[k].h2.b, 0, 1, 3, 1024, 512, 0);
-      }
-      for (int k = 0; k < 2; ++k) g.u[k].tc_slot = tc_register(e->tcw, g.u[k].a.k, g.u[k].g.k, g.u[k].a.b, g.u[k].g.b, 1, 5, g.u[k].a.cin, g.u[k].a.cout, 1, 2);
-      DiscNet& d = e->disc[i];
-      for (int k = 0; k < 3; ++k) d.d[k].tc_slot = tc_register(e->tcw, d.d[k].a.k, d.d[k].g.k, d.d[k].a.b, d.d[k].g.b, d.d[k].a.kh, 3, d.d[k].a.cin, d.d[k].a.cout, 1);
+      for (Layer& L : g.d) reg(L);
+      for (ResBlock& R : g.r) { reg(R.h1); reg(R.h2); }
+      for (Layer& L : g.u) reg(L);
+      for (Layer& L : e->disc[i].d) reg(L);
     }
-    e->tcw.quant = cfg->precision == CGVC_PREC_F16F8;
-    e->tcw.quant_bwd = e->tcw.quant && cfg->train;           // training in that precision also needs the data-gradient planes
-    e->tcw.wgrad16 = e->tcw.quant;                           // weight gradients (leaves of the graph) from the fp16 planes alone; option "wgrad_f16"
-    int r = tc_alloc(e->tcw);
+    int r = tc_alloc(e->tcw, cfg->precision, cfg->train);
     if (r != 0) { std::string m = cudaGetErrorString((cudaError_t)r); cudaFree(e->d_scalars); delete e; return fail(nullptr, CGVC_ERR_CUDA, "tc_alloc: %s", m.c_str()); }
   }
   *out = e;
@@ -1659,12 +1531,8 @@ int cgvc_conv_forward(cgvc_handle e, int precision, const float* x, const float*
   if (kh * kw > CGVC_MAX_TAPS) return fail(e, CGVC_ERR_UNSUPPORTED, "at most %d filter taps", CGVC_MAX_TAPS);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision != CGVC_PREC_FP32_SIMT) {
-    int r = tc_conv_fwd_adhoc(precision, x, w, bias, y, B, H, W, Cin, kh, kw, Cout, sh, sw, st);
-    if (r == TC_UNSUPPORTED) return fail(e, CGVC_ERR_UNSUPPORTED, "shape not supported by the tensor-core path");
-    if (r != 0) return fail(e, CGVC_ERR_CUDA, "tc conv fwd: %s", cudaGetErrorString((cudaError_t)r));
-    return 0;
-  }
+  if (precision != CGVC_PREC_FP32_SIMT)
+    return tc_result(e, tc_conv_fwd_adhoc(precision, x, w, bias, y, B, H, W, Cin, kh, kw, Cout, sh, sw, st), nullptr, "conv forward");
   GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
   GemmOperands op; memset(&op, 0, sizeof op);
   op.src = x; op.s_ld = Cin; op.C = Cin; op.w = w; op.w_ts = (long long)Cin * Cout; op.w_cs = Cout; op.w_ns = 1; op.N = Cout;
@@ -1679,12 +1547,9 @@ int cgvc_conv_backward(cgvc_handle e, int precision, const float* x, const float
   if (kh * kw > CGVC_MAX_TAPS) return fail(e, CGVC_ERR_UNSUPPORTED, "at most %d filter taps", CGVC_MAX_TAPS);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision != CGVC_PREC_FP32_SIMT) {
-    int r = tc_conv_bwd_adhoc(precision, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16 ? 1 : 0);
-    if (r == TC_UNSUPPORTED) return fail(e, CGVC_ERR_UNSUPPORTED, "shape not supported by the tensor-core path");
-    if (r != 0) return fail(e, CGVC_ERR_CUDA, "tc conv bwd: %s", cudaGetErrorString((cudaError_t)r));
-    return 0;
-  }
+  if (precision != CGVC_PREC_FP32_SIMT)
+    return tc_result(e, tc_conv_bwd_adhoc(precision, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16 ? 1 : 0),
+                     nullptr, "conv backward");
   ConvW c; c.k = 0; c.b = 0; c.kh = kh; c.kw = kw; c.cin = Cin; c.cout = Cout;
   if (dx) RET(conv_dgrad_simt(e, w, c, sh, sw, B, H, W, dy, Cout, 0, dx, 0, st));
   if (dw) {

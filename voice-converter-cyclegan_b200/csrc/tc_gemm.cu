@@ -1716,8 +1716,12 @@ int tc_register(TcWeights& w, size_t ka, size_t kg, size_t ba, size_t bg, int kh
 
 static cudaError_t tc_init_kernels();
 
-int tc_alloc(TcWeights& w) {
+int tc_alloc(TcWeights& w, int precision, bool train) {
   { cudaError_t ie = tc_init_kernels(); if (ie != cudaSuccess) return (int)ie; }
+  w.precision = precision;
+  w.quant = precision == 3;
+  w.quant_bwd = w.quant && train;
+  w.wgrad16 = w.quant;                              // option "wgrad_f16"
   size_t total = 0;
   auto rnd = [](size_t b) { return (b + 255) & ~(size_t)255; };
   for (TcLayer& L : w.layers) {
@@ -1853,36 +1857,24 @@ int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, si
 
 void tc_set_prep_batched(int v) { g_tc_prep_batched = v != 0; }
 
-int tc_conv_fwd(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                int n, int H, int W, int sh, int sw, float* P, cudaStream_t st) {
-  return layer_fwd(w.layers[slot], precision, xhi, xlo, n, H, W, sh, sw, P, st);
+cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st) {
+  return precision == 3 ? launch_pad_split_q(x, rows, C, C, ru(C, 128), hi, lo, st) : launch_pad_split(x, rows, C, C, ru(C, 64), hi, lo, st);
 }
 
-int tc_conv_fwd_fused(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                      int n, int H, int W, int sh, int sw, float* P, const TcFuse& fuse, bool* fused, cudaStream_t st) {
-  return layer_fwd(w.layers[slot], precision, xhi, xlo, n, H, W, sh, sw, P, st, &fuse, fused);
+int tc_conv_fwd(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
+                float* P, cudaStream_t st, const TcFuse* fuse, bool* fused, const PackGeom* pk) {
+  return layer_fwd(w.layers[slot], w.precision, xhi, xlo, n, H, W, sh, sw, P, st, fuse, fused, pk);
 }
 
-int tc_conv_fwd_packed(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                       int rows, int sw, const PackGeom& pk, float* P, cudaStream_t st) {
-  return layer_fwd(w.layers[slot], precision, xhi, xlo, 1, 1, rows, 1, sw, P, st, nullptr, nullptr, &pk);
+int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
+                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused) {
+  return layer_dgrad(w.layers[slot], w.precision, dPhi, dPlo, n, H, W, sh, sw, dx, accumulate, st, fuse, fused);
 }
 
-int tc_conv_dgrad(TcWeights& w, int slot, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo,
-                  int n, int H, int W, int sh, int sw, float* dx, int accumulate, cudaStream_t st) {
-  return layer_dgrad(w.layers[slot], precision, dPhi, dPlo, n, H, W, sh, sw, dx, accumulate, st);
-}
-
-int tc_conv_dgrad_fused(TcWeights& w, int slot, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo,
-                        int n, int H, int W, int sh, int sw, float* dx, int accumulate, const TcBwdFuse& fuse, bool* fused, cudaStream_t st) {
-  return layer_dgrad(w.layers[slot], precision, dPhi, dPlo, n, H, W, sh, sw, dx, accumulate, st, &fuse, fused);
-}
-
-int tc_conv_wgrad(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, float* dba, float* dbg, cudaStream_t st) {
-  (void)dba; (void)dbg;   // bias gradients are column sums of the fp32 dP: done by the caller (launch_colsum)
-  return layer_wgrad(w.layers[slot], precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16 ? 1 : 0);
+                  float* dwa, float* dwg, cudaStream_t st) {
+  return layer_wgrad(w.layers[slot], w.precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16 ? 1 : 0);
 }
 
 bool tc_profile_is_on() { return g_prof_on; }
@@ -1967,8 +1959,7 @@ int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float
   if (!xhi || !xlo || !zero) return (int)cudaErrorMemoryAllocation;
   cudaMemsetAsync(zero, 0, Cout * sizeof(float), st);
   r = refresh_layer(L, w, nullptr, bias ? bias : zero, nullptr, st); if (r) return r;
-  cudaError_t e = precision == 3 ? launch_pad_split_q(x, (long long)rows, Cin, Cin, cpad, xhi, xlo, st)
-                                 : launch_pad_split(x, (long long)rows, Cin, Cin, cpad, xhi, xlo, st);
+  cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
   if (e != cudaSuccess) return (int)e;
   r = layer_fwd(L, precision, xhi, xlo, B, H, W, sh, sw, y, st); if (r) return r;
   return (int)cudaStreamSynchronize(st);
@@ -1990,11 +1981,9 @@ int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float
   if (!xhi || !xlo || !ghi || !glo || !zero) return (int)cudaErrorMemoryAllocation;
   cudaMemsetAsync(zero, 0, Cout * sizeof(float), st);
   r = refresh_layer(L, w, nullptr, zero, nullptr, st); if (r) return r;
-  cudaError_t e = precision == 3 ? launch_pad_split_q(x, (long long)rows, Cin, Cin, xpad, xhi, xlo, st)
-                                 : launch_pad_split(x, (long long)rows, Cin, Cin, xpad, xhi, xlo, st);
+  cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
   if (e != cudaSuccess) return (int)e;
-  e = precision == 3 ? launch_pad_split_q(dy, (long long)orows, Cout, Cout, gpad, ghi, glo, st)
-                     : launch_pad_split(dy, (long long)orows, Cout, Cout, gpad, ghi, glo, st);
+  e = tc_split_planes(precision, dy, (long long)orows, Cout, ghi, glo, st);
   if (e != cudaSuccess) return (int)e;
   if (dx) { r = layer_dgrad(L, precision, ghi, glo, B, H, W, sh, sw, dx, 0, st); if (r) return r; }
   if (dw) {

@@ -39,7 +39,8 @@ struct TcWeights {
   void* pool = nullptr;
   size_t pool_bytes = 0;
   bool ready = false;
-  bool quant = false;             // also keep the F16F8 forward planes (set before tc_alloc)
+  int precision = 0;              // the engine's CGVC_PREC_* (set by tc_alloc): the operand planes every slot-based call reads and writes
+  bool quant = false;             // also keep the F16F8 forward planes (precision F16F8)
   bool wgrad16 = false;           // F16F8 only: weight gradients from the fp16 planes alone (one MMA unit per product instead of two)
   bool quant_bwd = false;         // ... and the F16F8 data-gradient planes (training in that precision)
   void* prep_jobs = nullptr;      // device job table of the batched F16F8 plane kernel (tc_gemm.cu PrepJob), one job per layer branch
@@ -47,7 +48,7 @@ struct TcWeights {
   std::vector<size_t> job_ka;     // PARAM offset of the job's layer (range filter of tc_refresh_weights_range)
 };
 
-// what the fused forward epilogue needs besides the convolution itself (see tc_conv_fwd_fused)
+// what the fused forward epilogue needs besides the convolution itself (see tc_conv_fwd)
 struct TcFuse {
   int R;                                            // positions per sample of the layer output
   const float *gamma_a, *beta_a, *gamma_g, *beta_g; // instance-norm affine parameters (g: gate branch, null when not gated)
@@ -56,7 +57,7 @@ struct TcFuse {
   float* y; __nv_bfloat16 *y_hi, *y_lo;             // outputs [rows, C] (fp32 optional)
 };
 
-// what the fused backward epilogue of a data-gradient launch needs (see tc_conv_dgrad_fused): the gradient this launch computes
+// what the fused backward epilogue of a data-gradient launch needs (see tc_conv_dgrad): the gradient this launch computes
 // is d loss / d (output of an upstream layer); that layer's instance-norm (+ GLU) backward runs in the epilogue
 struct TcBwdFuse {
   int R;                                            // positions per sample
@@ -69,37 +70,37 @@ struct TcBwdFuse {
 };
 
 int tc_register(TcWeights& w, size_t ka, size_t kg, size_t ba, size_t bg, int kh, int kw, int cin, int cout, int gated, int shuffle = 1, int fold = 0);
-int tc_alloc(TcWeights& w);                                     // cudaError_t as int
+// precision: CGVC_PREC_*; train: an F16F8 engine also keeps the data-gradient planes.  cudaError_t as int
+int tc_alloc(TcWeights& w, int precision, bool train);
 void tc_free(TcWeights& w);
 int tc_refresh_weights(TcWeights& w, const float* params, cudaStream_t st);
 int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, size_t end, cudaStream_t st);
 
-// activation / gradient planes handed to these functions have their channel count rounded up to a multiple of 64
-// (zero-filled): x [n,H,W,ru64(cin)], dP [rows, ru64(Ntot)]
-// P[rows, Ntot] = conv(x) + bias
-int tc_conv_fwd(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                int n, int H, int W, int sh, int sw, float* P, cudaStream_t st);
-// Same, with instance norm (+ GLU | + residual) fused into the epilogue when the shape allows (1-D layer, whole samples per
-// 128-row tile: R in {32,64,128}); *fused tells the caller whether it happened (if not, P is written and the caller runs
-// the separate instance-norm kernels).
-int tc_conv_fwd_fused(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                      int n, int H, int W, int sh, int sw, float* P, const TcFuse& fuse, bool* fused, cudaStream_t st);
-// P = conv(x) + bias of a 1-D layer over packed variable-length utterances (kernels.cuh PackGeom): x planes [rows, .] at the source
-// level of divisor pk.div, stride sw; every tap reads only its own utterance's rows.  Plain epilogue only.
-int tc_conv_fwd_packed(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                       int rows, int sw, const PackGeom& pk, float* P, cudaStream_t st);
+// x [rows, C] fp32 -> the operand planes of `precision` with C zero-padded to the contraction width: bf16 hi / lo [rows, ru64(C)],
+// F16F8: q16 (hi) and q8hi followed by q8lo (lo) [rows, ru128(C)].  cudaError_t
+cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st);
+
+// The slot-based calls below read and write the planes of w.precision (tc_split_planes), with their channel count rounded up
+// (zero-filled): x [n,H,W,cin], dP [rows, Ntot].  They return 0, TC_UNSUPPORTED (no launch: the shape has no tensor-core form)
+// or a cudaError_t.
+// P[rows, Ntot] = conv(x) + bias.
+//   fuse: instance norm (+ GLU | + residual) fused into the epilogue when the shape allows (1-D layer, whole samples per 128-row
+//         tile: R in {32,64,128}); *fused tells the caller whether it happened (if not, P is written and the caller runs the
+//         separate instance-norm kernels).
+//   pk:   a 1-D layer over packed variable-length utterances (kernels.cuh PackGeom): n = H = 1, x planes [W, .] at the source level
+//         of divisor pk->div; every tap reads only its own utterance's rows.  Plain epilogue only.
+int tc_conv_fwd(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
+                float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused = nullptr, const PackGeom* pk = nullptr);
 // dx[n,H,W,cin] (+)= dgrad(dP)            (dP planes [rows_out, Ntot]; H, W are the INPUT dims)
-int tc_conv_dgrad(TcWeights& w, int slot, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo,
-                  int n, int H, int W, int sh, int sw, float* dx, int accumulate, cudaStream_t st);
-// Same, with the upstream layer's instance-norm (+ GLU) backward fused into the epilogue when the shape allows (stride-1 1-D
-// layer, whole samples per 128-row tile): the launch then writes that layer's dP planes (and, for gated = 0, dx = dY) instead
-// of / besides dx; *fused tells whether it happened (if not, dx holds the plain data gradient as with tc_conv_dgrad).
-int tc_conv_dgrad_fused(TcWeights& w, int slot, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo,
-                        int n, int H, int W, int sh, int sw, float* dx, int accumulate, const TcBwdFuse& fuse, bool* fused, cudaStream_t st);
-// dW_a/dW_g (TF layout) += x^T dP ; db += colsum(dP)
-int tc_conv_wgrad(TcWeights& w, int slot, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+//   fuse: the upstream layer's instance-norm (+ GLU) backward fused into the epilogue when the shape allows (stride-1 1-D layer,
+//         whole samples per 128-row tile): the launch then writes that layer's dP planes (and, for gated = 0, dx = dY) instead
+//         of / besides dx; *fused tells whether it happened (if not, dx holds the plain data gradient).
+int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
+                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr);
+// dW_a/dW_g (TF layout) += x^T dP  (the bias gradients are column sums of dP: the instance-norm backward kernels or launch_colsum)
+int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, float* dba, float* dbg, cudaStream_t st);
+                  float* dwa, float* dwg, cudaStream_t st);
 // self-contained versions for unit tests (fp32 in/out, temporary planes allocated internally)
 int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float* bias, float* y,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st);
