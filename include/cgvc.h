@@ -80,9 +80,43 @@ int cgvc_param_info(cgvc_handle h, int index, const char** name, size_t* offset,
 /* Must be called after the caller (re)writes the PARAM arena (init, checkpoint load): refreshes the engine's
  * derived bf16 operand copies.  Replaces sess.run(global_variables_initializer) / Saver.restore side effects. */
 int cgvc_params_updated(cgvc_handle h, void* stream);
-/* Reset Adam step count t (beta-power accumulators of both optimizers, model.py:107-108) */
+/* Reset Adam step count t (beta-power accumulators of both optimizers, model.py:107-108).  With option "loss_scale" = 2 the count
+ * lives on the device (a skipped step does not advance it): both calls then synchronise the device. */
 int cgvc_set_adam_step(cgvc_handle h, long long t);
 int cgvc_get_adam_step(cgvc_handle h, long long* t);
+
+/* -- loss scaling of the F16F8 gradient planes (option "loss_scale", DESIGN.md section 10) ---------------------------------------
+ * The planes of a gradient tensor x are fp16(x) and two e4m3 cross terms (S_hi = 1, S_lo = 2^12).  They are exact only in a window:
+ * the hi plane clamps once |fp16(x)| > 448, the lo plane from |x| >= 256, fp16(x) overflows to inf at 65504 -- and a clamped cross term
+ * is a wrong product, not a NaN.  Training multiplies every loss gradient by a power-of-two scale and Adam divides it out again.
+ *   "loss_scale" = 0 (default): static, 2^(9 + floor(log2 batch)) in F16F8, 1 otherwise.  No extra work per step.
+ *                = 1: monitor.  The static scale and the kernels of 0 (same arithmetic), but every train step counts its saturated plane
+ *                     groups and checks GRAD for non-finite values (read with cgvc_loss_scale_state).
+ *                = 2: dynamic.  A step whose gradient planes saturated (summed over ranks) or whose all-reduced GRAD holds a
+ *                     non-finite value is skipped -- PARAM, ADAM_M, ADAM_V and the Adam step count stay as they were -- and the
+ *                     scale halves (floor 1); after "loss_scale_growth_interval" (default 2000) good steps in a row it doubles
+ *                     (cap 2^24).  It starts from the static scale of the first step's batch unless set with
+ *                     cgvc_set_loss_scale_state.  In bf16x3, bf16 and fp32 the scale stays 1 and only non-finite steps are skipped.
+ * Counted: the planes the instance-norm / GLU kernels (forward and backward), the input and output-gradient splits of the generator
+ * and the discriminator's input layer write in a train step.  Not counted: the fused instance-norm epilogues of the forward GEMMs
+ * (activation planes: with "fuse_in" = 1, the default, the generator layers whose instance norm is fused into the GEMM) and the weight
+ * planes; with loss_scale != 0 the opt-in fused backward epilogues ("fuse_bwd") are not used, so with "fuse_bwd" = 1 modes 1 and 2 run
+ * the unfused backward kernels and are not bit-identical to mode 0 (the unfused path is the default one).
+ * Changing either option invalidates the captured step graphs.  With a communicator and "pipelined_comm", mode 2 makes every
+ * network's Adam wait for the whole all-reduce and the scaler. */
+typedef struct cgvc_loss_scale_info {
+  float scale;                    /* the scale the next step's gradients are formed with (static: that of the last step's batch) */
+  int good_steps;                 /* consecutive steps not skipped (dynamic) */
+  long long skipped;              /* steps skipped so far (dynamic) */
+  int last_skipped;               /* the last step was skipped (dynamic) */
+  unsigned nonfinite;             /* the last step's GRAD held a non-finite value: bit 0 generators, bit 1 discriminators */
+  unsigned long long sat_grad;    /* the last step's saturated 4-value groups in gradient planes (dynamic: summed over ranks) */
+  unsigned long long sat_act;     /* ... in activation planes: a diagnostic, the loss scale cannot fix a forward activation */
+} cgvc_loss_scale_info;
+/* asynchronous: copies the state into out_dev (device memory) on the stream */
+int cgvc_loss_scale_state(cgvc_handle h, cgvc_loss_scale_info* out_dev, void* stream);
+/* resume a dynamic scale: scale in [1, 2^24]; last_skipped, nonfinite, sat_grad and sat_act are cleared.  Synchronises the stream. */
+int cgvc_set_loss_scale_state(cgvc_handle h, float scale, int good_steps, long long skipped, void* stream);
 
 /* -- the hot path: replaces CycleGAN.train (model.py:110-125) ------------------------------------------
  * One G step + one D step from the same pre-update weights, then both Adam updates.
@@ -102,7 +136,8 @@ int cgvc_compute_gradients(cgvc_handle h, const float* A_dev, const float* B_dev
                            float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream);
 
 /* TF-style Adam on the bound arenas (model.py:107-108; tf.train.AdamOptimizer beta1=0.5): advances t by one.
- * grad_scale multiplies every gradient first (1/nranks after a sum-all-reduce). */
+ * grad_scale multiplies every gradient first (1/nranks after a sum-all-reduce).  The same in every "loss_scale" mode (no skip: the
+ * GRAD arena is the caller's); with "loss_scale" = 2, where t lives on the device, the call synchronises the device twice. */
 int cgvc_adam_step(cgvc_handle h, float lr_generator, float lr_discriminator, float grad_scale, void* stream);
 
 /* -- replaces CycleGAN.test (model.py:128-137): one generator forward.  direction 0 = 'A2B', 1 = 'B2A';
@@ -189,6 +224,7 @@ int cgvc_kernel_launches(unsigned long long* count);
  * "post_stream" (default 1, process-wide): gated layers without pixel shuffle whose samples have 32, 48 or 64 positions take the streaming
  * form of the one-pass GLU / instance-norm backward: persistent CTAs walk (sample, channel block) items through a cp.async double buffer
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
+ * "loss_scale" (default 0) and "loss_scale_growth_interval" (default 2000): see cgvc_loss_scale_state.
  * "debug_taps" (default 0): see cgvc_debug_activation.
  * "tc_debug" (default 0): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
  * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather.  The plain

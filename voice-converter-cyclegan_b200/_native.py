@@ -27,6 +27,15 @@ class Config(C.Structure):
                 ("precision", C.c_int), ("device", C.c_int), ("train", C.c_int)]
 
 
+LOSS_SCALE_MODES = {"static": 0, "monitor": 1, "dynamic": 2}
+
+
+class LossScaleInfo(C.Structure):
+    """cgvc_loss_scale_info of include/cgvc.h"""
+    _fields_ = [("scale", C.c_float), ("good_steps", C.c_int), ("skipped", C.c_longlong), ("last_skipped", C.c_int),
+                ("nonfinite", C.c_uint), ("sat_grad", C.c_ulonglong), ("sat_act", C.c_ulonglong)]
+
+
 class CgvcError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("libcgvc error %d: %s" % (code, msg))
@@ -48,6 +57,8 @@ def _declare(lib):
         "cgvc_params_updated": (ci, [vp, vp]),
         "cgvc_set_adam_step": (ci, [vp, C.c_longlong]),
         "cgvc_get_adam_step": (ci, [vp, P(C.c_longlong)]),
+        "cgvc_loss_scale_state": (ci, [vp, vp, vp]),
+        "cgvc_set_loss_scale_state": (ci, [vp, cf, ci, C.c_longlong, vp]),
         "cgvc_train_step": (ci, [vp, vp, vp, ci, ci, cf, cf, cf, cf, vp, vp, vp, vp]),
         "cgvc_compute_gradients": (ci, [vp, vp, vp, ci, ci, cf, cf, vp, vp, vp, vp]),
         "cgvc_adam_step": (ci, [vp, cf, cf, cf, vp]),

@@ -8,6 +8,7 @@
 #include "geom.h"
 
 #include <dlfcn.h>
+#include <stddef.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -139,6 +140,15 @@ struct cgvc_engine {
   int two_streams = 1;          // 0: both lanes are enqueued on the caller's stream (clean per-kernel timing for profiling)
   int side_wgrad = 0;           // weight-gradient GEMMs on a side stream per lane (see SideQ); needs two_streams, excludes fuse_bwd.  Off by default
   SideQ sideq[2];
+  // loss scaling (option "loss_scale"): 0 static, 1 monitor (static scale, counters collected), 2 dynamic.  ls: the device state;
+  // d_scalars[16 + l] holds the static scale of batches [2^l, 2^(l+1)) (loss_scale), so that the loss kernels always read a pointer
+  int ls_mode = 0;
+  int ls_growth = 2000;         // option "loss_scale_growth_interval"
+  LossScaler* ls = nullptr;
+  bool ls_ready = false;        // dynamic mode: ls->scale holds a scale (set on the first step from the static one, or by the caller)
+  int ls_batch = 0;             // monitor mode: the batch whose static scale ls->scale reports
+  bool counting = false;        // a train step is being enqueued: the plane writers count saturation (ls_mode != 0, F16F8)
+  cudaEvent_t ev_ls = nullptr;  // data parallel: the saturation all-reduce and the GRAD check are done (comm stream)
   // debug taps of the last forward
   std::map<std::string, std::pair<const float*, size_t>> taps;
 
@@ -308,6 +318,20 @@ static float loss_scale(const cgvc_engine* e, int batch) {
   int l = 0; while ((2 << l) <= batch && l < 9) ++l;       // floor(log2(batch)), capped
   return ldexpf(1.f, 9 + l);
 }
+// the device copy of loss_scale(e, batch) (d_scalars[16 + floor(log2 batch)], written at creation), or in dynamic mode the scaler's
+// current scale: what the loss-gradient kernels multiply by
+static const float* loss_scale_dev(const cgvc_engine* e, int batch) {
+  if (e->ls_mode == 2) return &e->ls->scale;
+  int l = 0; while ((2 << l) <= batch && l < 9) ++l;
+  return e->d_scalars + 16 + l;
+}
+// saturation counters of the plane writers (null: not counted): only F16F8 has reduced-range planes, only train steps are counted
+static unsigned long long* sat_grad(const cgvc_engine* e) {
+  return e->counting && e->ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_grad : nullptr;
+}
+static unsigned long long* sat_act(const cgvc_engine* e) {
+  return e->counting && e->ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_act : nullptr;
+}
 
 static bool tc_enabled(const cgvc_engine* e) { return e->cfg.precision != CGVC_PREC_FP32_SIMT && e->tcw.ready; }
 static bool use_tc(const cgvc_engine* e, int slot) { return slot >= 0 && tc_enabled(e); }
@@ -381,6 +405,7 @@ static PostParams post_params(const cgvc_engine* e, const Layer& L, const ConvIO
   q.y = (keep_y || !A.Yhi) ? A.Y : nullptr;      // without planes the fp32 activation is the only copy
   q.stats = L.has_in ? A.stats : nullptr; q.y_hi = A.Yhi; q.y_lo = A.Ylo;
   q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+  q.sat = sat_act(e);
   if (io.pk.off && L.has_in) {
     // packed utterances: q describes one sample holding all q.R view rows; instance norm runs per utterance over its own view rows
     // (the GLU-only layer is row-local and keeps that view)
@@ -484,11 +509,11 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
   if (edge) {
     // h1 = dense [n*T, kw*F] x [kw*F, 2*128] GEMM on the im2col of the input
     CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
-                          A.xchi, A.xclo, st, A.off, A.n));
+                          A.xchi, A.xclo, st, A.off, A.n, sat_act(e)));
     RET(tc_result(e, tc_conv_fwd(e->tcw, N.h1c_slot, A.xchi, A.xclo, n, 1, T, 1, 1, A.h1.P, st), &N.h1.a, "forward (tap-lowered)"));
     PostParams q = post_params(e, N.h1, io, A.h1, T, keep_y, A.post); CK(launch_post_fwd(q, st));
   } else {
-    if (A.xhi && tc_enabled(e)) CK(tc_split_planes(e->cfg.precision, x_cl, (long long)n * T, nf, A.xhi, A.xlo, st));
+    if (A.xhi && tc_enabled(e)) CK(tc_split_planes(e->cfg.precision, x_cl, (long long)n * T, nf, A.xhi, A.xlo, st, sat_act(e)));
     RET(layer_forward(e, N.h1, io, A.h1, T, keep_y, save_pre, A.post, st));
   }
   const GLAct* cur = &A.h1;
@@ -604,6 +629,7 @@ static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const
   q.dp = (!tc || need_fp32) ? S.dP : nullptr;
   if (tc) { q.dp_hi = out.hi; q.dp_lo = out.lo; }
   q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+  q.sat = sat_grad(e);
   return q;
 }
 
@@ -661,7 +687,8 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
     ConvIO io; io.x = x; io.xhi = hi; io.xlo = lo; io.n = n; io.H = 1; io.W = W; return io;
   };
   auto of = [&](const GLAct& a, int W) { return at(a.Y, a.Yhi, a.Ylo, W); };
-  BwdWalk w(S, e->fuse_bwd && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi && A.r[0].h2.Yhi);
+  // the fused backward epilogues do not count saturation: a step whose planes are counted takes the separate kernels
+  BwdWalk w(S, e->fuse_bwd && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi && A.r[0].h2.Yhi);
   const bool edge = edge_on(e, N) && A.xchi && A.z;
   // o1 (no norm, no gate): bias gradient = column sums of d_out
   CK(launch_colsum(d_out_cl, (long long)n * T, nf, 0, nf, Gm + N.o1.a.b, st));
@@ -670,7 +697,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
     // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
     const PlanePair dp = dp_planes(w, st);
     CK(launch_im2col_taps(d_out_cl, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
-                          dp.hi, dp.lo, st));
+                          dp.hi, dp.lo, st, nullptr, 0, sat_grad(e)));
     RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
       return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, u2.xhi, u2.xlo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws),
                        &N.o1.a, "weight gradient (tap-lowered)"); }));
@@ -679,7 +706,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
     PlanePair dp{nullptr, nullptr};
     if (use_tc(e, N.o1.tc_slot) && u2.xhi && S.dPhi) {
       dp = dp_planes(w, st);
-      CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st));
+      CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st, sat_grad(e)));
     }
     RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, u2, d_out_cl, dp, ws); }));
     RET(conv_dgrad(e, N.o1, u2, d_out_cl, dp, S.bufA, 0, st));
@@ -746,7 +773,7 @@ static int discriminator_forward(cgvc_engine* e, const DiscNet& N, DiscActs& A, 
     // input layer (one input channel, K = 9, gate without norm): convolution + GLU in one HBM-bound pass; P is kept for the backward pass
     const GatherGeom g = fwd_geom(n, H0, T, N.h1.a.kh, N.h1.a.kw, N.h1.sh, N.h1.sw);
     const PostParams q = post_params(e, N.h1, io, A.h1, H * W, keep_y, A.post);
-    CK(launch_conv_c1_glu_fwd(g, x, Pm + N.h1.a.k, Pm + N.h1.g.k, Pm + N.h1.a.b, Pm + N.h1.g.b, N.h1.a.cout, A.h1.P, q.y, q.y_hi, q.y_lo, q.qmode, st));
+    CK(launch_conv_c1_glu_fwd(g, x, Pm + N.h1.a.k, Pm + N.h1.g.k, Pm + N.h1.a.b, Pm + N.h1.g.b, N.h1.a.cout, A.h1.P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat));
   } else {
     RET(layer_forward(e, N.h1, io, A.h1, H * W, keep_y, true, A.post, st));
   }
@@ -923,6 +950,15 @@ int cgvc_create(const cgvc_config* cfg, cgvc_handle* out) {
   ce = cudaMalloc(&e->d_scalars, 64 * sizeof(float));
   if (ce != cudaSuccess) { delete e; return fail(nullptr, CGVC_ERR_CUDA, "cudaMalloc scalars: %s", cudaGetErrorString(ce)); }
   cudaMemset(e->d_scalars, 0, 64 * sizeof(float));
+  {
+    float st[10];
+    for (int l = 0; l < 10; ++l) st[l] = loss_scale(e, 1 << l);
+    cudaMemcpy(e->d_scalars + 16, st, sizeof st, cudaMemcpyHostToDevice);
+  }
+  ce = cudaMalloc(&e->ls, sizeof(LossScaler));
+  if (ce != cudaSuccess) { cudaFree(e->d_scalars); delete e; return fail(nullptr, CGVC_ERR_CUDA, "cudaMalloc loss scaler: %s", cudaGetErrorString(ce)); }
+  cudaMemset(e->ls, 0, sizeof(LossScaler));
+  cudaEventCreateWithFlags(&e->ev_ls, cudaEventDisableTiming);
   for (int l = 0; l < 2; ++l) { cudaStreamCreateWithFlags(&e->lane_stream[l], cudaStreamNonBlocking); cudaEventCreateWithFlags(&e->ev_join[l], cudaEventDisableTiming); }
   cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming);
   { int lo = 0, hi = 0; cudaDeviceGetStreamPriorityRange(&lo, &hi); cudaStreamCreateWithPriority(&e->comm_stream, cudaStreamNonBlocking, hi); }
@@ -955,7 +991,7 @@ int cgvc_create(const cgvc_config* cfg, cgvc_handle* out) {
       for (Layer& L : e->disc[i].d) reg(L);
     }
     int r = tc_alloc(e->tcw, cfg->precision, cfg->train);
-    if (r != 0) { std::string m = cudaGetErrorString((cudaError_t)r); cudaFree(e->d_scalars); delete e; return fail(nullptr, CGVC_ERR_CUDA, "tc_alloc: %s", m.c_str()); }
+    if (r != 0) { std::string m = cudaGetErrorString((cudaError_t)r); cudaFree(e->d_scalars); cudaFree(e->ls); delete e; return fail(nullptr, CGVC_ERR_CUDA, "tc_alloc: %s", m.c_str()); }
   }
   *out = e;
   return 0;
@@ -982,6 +1018,8 @@ int cgvc_destroy(cgvc_handle e) {
   if (e->ev_bridge) cudaEventDestroy(e->ev_bridge);
   if (e->ev_bridge2) cudaEventDestroy(e->ev_bridge2);
   cudaFree(e->d_scalars);
+  cudaFree(e->ls);
+  if (e->ev_ls) cudaEventDestroy(e->ev_ls);
   delete e;
   return 0;
 }
@@ -1038,8 +1076,48 @@ int cgvc_params_updated(cgvc_handle e, void* stream) {
   return 0;
 }
 
-int cgvc_set_adam_step(cgvc_handle e, long long t) { if (!e || t < 0) return CGVC_ERR_ARG; e->adam_t = t; return 0; }
-int cgvc_get_adam_step(cgvc_handle e, long long* t) { if (!e || !t) return CGVC_ERR_ARG; *t = e->adam_t; return 0; }
+// in dynamic loss-scale mode the step count lives on the device (the scaler advances it): these two synchronise the device
+int cgvc_set_adam_step(cgvc_handle e, long long t) {
+  if (!e || t < 0) return CGVC_ERR_ARG;
+  e->adam_t = t;
+  if (e->ls_mode == 2) {
+    DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(&e->ls->t, &t, sizeof t, cudaMemcpyHostToDevice));
+  }
+  return 0;
+}
+int cgvc_get_adam_step(cgvc_handle e, long long* t) {
+  if (!e || !t) return CGVC_ERR_ARG;
+  if (e->ls_mode == 2) {
+    DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(&e->adam_t, &e->ls->t, sizeof e->adam_t, cudaMemcpyDeviceToHost));
+  }
+  *t = e->adam_t;
+  return 0;
+}
+
+static_assert(sizeof(cgvc_loss_scale_info) == offsetof(LossScaler, t) && offsetof(cgvc_loss_scale_info, sat_act) == offsetof(LossScaler, sat_act) &&
+              offsetof(cgvc_loss_scale_info, nonfinite) == offsetof(LossScaler, nonfinite) && offsetof(cgvc_loss_scale_info, skipped) == offsetof(LossScaler, skipped),
+              "cgvc_loss_scale_info is the head of LossScaler");
+int cgvc_loss_scale_state(cgvc_handle e, cgvc_loss_scale_info* out_dev, void* stream) {
+  if (!e || !out_dev) return fail(e, CGVC_ERR_ARG, "null argument");
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(cudaMemcpyAsync(out_dev, e->ls, sizeof(cgvc_loss_scale_info), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+int cgvc_set_loss_scale_state(cgvc_handle e, float scale, int good_steps, long long skipped, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if (!(scale >= 1.f && scale <= 16777216.f) || good_steps < 0 || skipped < 0)
+    return fail(e, CGVC_ERR_ARG, "cgvc_set_loss_scale_state: scale %g outside [1, 2^24] or negative counts", (double)scale);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  const cgvc_loss_scale_info v{scale, good_steps, skipped, 0, 0, 0, 0};     // the last step's flag and counters cleared
+  CK(cudaMemcpyAsync(e->ls, &v, sizeof v, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  CK(cudaStreamSynchronize((cudaStream_t)stream));           // v lives on this stack frame
+  e->ls_ready = true;
+  return 0;
+}
 
 static int check_bt(cgvc_engine* e, int batch, int frames, int mult) {
   if (batch < 1 || batch > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "batch %d outside [1, %d]", batch, e->cfg.max_batch);
@@ -1153,7 +1231,7 @@ static int run_lane(cgvc_engine* e, LanePlan& L, int lane, const float* Yreal_de
   if (gen_out_dev) CK(cudaMemcpyAsync(gen_out_dev, L.din + img, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
   RET(discriminator_forward(e, DN, L.d, L.din, st, false));
   // ---- losses and their gradients (model.py:57-90) ----
-  const float ls = loss_scale(e, B);                            // scales every gradient of the step (not the loss values); Adam divides it out
+  const float* ls = loss_scale_dev(e, B);                       // scales every gradient of the step (not the loss values); Adam divides it out
   CK(launch_l1_loss_grad(L.gcyc.out_cl, X_cl, (long long)img, Ls + 0, sc + 0, L.d_cyc, 0, st, ls));          // cycle term
   CK(launch_l1_loss_grad(idY_cl, Y_cl, (long long)img, Ls + 1, sc + 1, L.d_out + img, 0, st, ls));           // identity term
   const long long hrows = (long long)B * (nf / 4) * (T / 16);   // head rows per half
@@ -1201,6 +1279,9 @@ static int forward_backward(cgvc_engine* e, const float* A_dev, const float* B_d
   float* sc = e->d_scalars; float* L = sc + 8;
   (void)lc;                                                  // lambdas are already in d_scalars[0..1] (set_step_scalars)
   CK(cudaMemsetAsync(L, 0, 8 * sizeof(float), st));
+  if (e->ls_mode) CK(cudaMemsetAsync(&e->ls->nonfinite, 0, (char*)(&e->ls->sat_act + 1) - (char*)&e->ls->nonfinite, st));   // this step's counters
+  struct Counting { cgvc_engine* e; ~Counting() { e->counting = false; } } counting{e};
+  e->counting = true;
   CK(cudaMemsetAsync(e->G(), 0, e->n_params * sizeof(float), st));
   // channels-last copies of the real samples: lane 0 reads [A;B], lane 1 [B;A]
   CK(launch_transpose_ft(A_dev, P.lane[0].in, B, nf, T, st));
@@ -1237,8 +1318,16 @@ static int set_lambdas(cgvc_engine* e, float lc, float li, cudaStream_t st) {
   CK(launch_set_scalars(e->d_scalars, 0, 2, v, st));
   return 0;
 }
-static int set_adam_scalars(cgvc_engine* e, float lr_g, float lr_d, float grad_scale, cudaStream_t st) {
+// deferred (a train step in dynamic loss-scale mode): see below
+static int set_adam_scalars(cgvc_engine* e, float lr_g, float lr_d, float grad_scale, cudaStream_t st, bool deferred = false) {
   e->adam_t += 1;                                            // both optimizers advance once per train() (Appendix A.6)
+  if (deferred) {
+    // dynamic loss scale: t lives on the device and only the scaler knows whether this step goes through; it turns these raw values
+    // into lr_t and the grad_scale (loss_scale_update_kernel)
+    float v[6] = {lr_g, grad_scale, lr_d, grad_scale, 0, 0};
+    CK(launch_set_scalars(e->d_scalars, 2, 4, v, st));
+    return 0;
+  }
   double t = (double)e->adam_t;
   double corr = sqrt(1.0 - pow((double)ADAM_B2, t)) / (1.0 - pow((double)ADAM_B1, t));
   float v[6] = {(float)(lr_g * corr), grad_scale, (float)(lr_d * corr), grad_scale, 0, 0};
@@ -1246,12 +1335,35 @@ static int set_adam_scalars(cgvc_engine* e, float lr_g, float lr_d, float grad_s
   return 0;
 }
 // the capturable part of the optimizer step: two Adam ranges + refresh of the tensor-core weight planes
-static int adam_body(cgvc_engine* e, cudaStream_t st) {
+static int adam_body(cgvc_engine* e, cudaStream_t st, const int* skip = nullptr) {
   float* p = e->P(); float* g = e->G(); float* m = (float*)e->arena[CGVC_ARENA_ADAM_M]; float* v = (float*)e->arena[CGVC_ARENA_ADAM_V];
   size_t gend = e->gen[1].end;   // generators occupy [0, gend), discriminators [gend, n_params)  (model.py:94-95)
-  CK(launch_adam(p, g, m, v, (long long)gend, e->d_scalars + 2, ADAM_B1, ADAM_B2, ADAM_EPS, st));
-  CK(launch_adam(p + gend, g + gend, m + gend, v + gend, (long long)(e->n_params - gend), e->d_scalars + 4, ADAM_B1, ADAM_B2, ADAM_EPS, st));
+  CK(launch_adam(p, g, m, v, (long long)gend, e->d_scalars + 2, ADAM_B1, ADAM_B2, ADAM_EPS, st, skip));
+  CK(launch_adam(p + gend, g + gend, m + gend, v + gend, (long long)(e->n_params - gend), e->d_scalars + 4, ADAM_B1, ADAM_B2, ADAM_EPS, st, skip));
   return cgvc_params_updated(e, (void*)st);
+}
+
+// Loss scaling after the gradients are complete (and summed over ranks): the non-finite check of GRAD per optimizer range, then in
+// dynamic mode the scaler update, whose skip word the Adam kernels read
+static int ls_check_grads(cgvc_engine* e, cudaStream_t st) {
+  CK(launch_check_finite(e->G(), (long long)e->n_params, (long long)e->gen[1].end, &e->ls->nonfinite, st));
+  return 0;
+}
+static int ls_update(cgvc_engine* e, cudaStream_t st) {
+  CK(launch_loss_scale_update(e->ls, e->d_scalars + 2, e->cfg.precision == CGVC_PREC_F16F8, e->ls_growth, ADAM_B1, ADAM_B2, st));
+  return 0;
+}
+static const int* ls_skip(const cgvc_engine* e) { return e->ls_mode == 2 ? &e->ls->last_skipped : nullptr; }
+
+// Before a step is enqueued: dynamic mode starts from the static scale of the step's batch unless the caller set one
+// (cgvc_set_loss_scale_state); monitor mode reports the static scale in use
+static int ls_prepare(cgvc_engine* e, int batch, cudaStream_t st) {
+  const bool dyn = e->ls_mode == 2 && !e->ls_ready, mon = e->ls_mode == 1 && e->ls_batch != batch;
+  if (!dyn && !mon) return 0;
+  const float v[6] = {loss_scale(e, batch), 0, 0, 0, 0, 0};
+  CK(launch_set_scalars(&e->ls->scale, 0, 1, v, st));
+  e->ls_ready = e->ls_mode == 2; e->ls_batch = e->ls_mode == 1 ? batch : 0;
+  return 0;
 }
 
 // ---- CUDA graphs: the ~650 launches of a step are captured once per (buffers, batch, frames, identity-on/off) and replayed.
@@ -1302,9 +1414,11 @@ int cgvc_compute_gradients(cgvc_handle e, const float* A_dev, const float* B_dev
   if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   RET(set_lambdas(e, lambda_cycle, lambda_identity, (cudaStream_t)stream));
+  RET(ls_prepare(e, batch, (cudaStream_t)stream));
   RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, (cudaStream_t)stream));
-  const float ls = loss_scale(e, batch);                     // the gradients are handed out, not fed to Adam: remove the loss scale here
-  if (ls != 1.f) CK(launch_scale(e->G(), (long long)e->n_params, 1.f / ls, (cudaStream_t)stream));
+  // the gradients are handed out, not fed to Adam: remove the loss scale here (in dynamic mode the device scale they were formed with)
+  if (e->ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
+  else if (loss_scale(e, batch) != 1.f) CK(launch_scale(e->G(), (long long)e->n_params, 1.f / loss_scale(e, batch), (cudaStream_t)stream));
   return 0;
 }
 
@@ -1312,11 +1426,15 @@ int cgvc_adam_step(cgvc_handle e, float lr_g, float lr_d, float grad_scale, void
   if (!e) return CGVC_ERR_ARG;
   for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  // dynamic loss-scale mode keeps t on the device: bring it to the host (synchronises), step with the host's lr_t like the other
+  // modes, and write the advanced t back (synchronises again).  No skip: the caller decides on this step
+  if (e->ls_mode == 2) { long long t; RET(cgvc_get_adam_step(e, &t)); }
   const long long t_before = e->adam_t;
   RET(set_adam_scalars(e, lr_g, lr_d, grad_scale, (cudaStream_t)stream));
   int r = adam_body(e, (cudaStream_t)stream);
-  if (r != 0) e->adam_t = t_before;
-  return r;
+  if (r != 0) { e->adam_t = t_before; return r; }
+  if (e->ls_mode == 2) RET(cgvc_set_adam_step(e, e->adam_t));
+  return 0;
 }
 
 int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int batch, int frames,
@@ -1333,7 +1451,8 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
   // capture failure, NCCL error) must not change the bias correction of the next one
   const long long adam_t_before = e->adam_t;
   struct Rollback { cgvc_engine* e; long long t; bool armed; ~Rollback() { if (armed) e->adam_t = t; } } rollback{e, adam_t_before, true};
-  RET(set_adam_scalars(e, lr_g, lr_d, gscale, st));
+  RET(set_adam_scalars(e, lr_g, lr_d, e->ls_mode == 2 ? (e->comm ? 1.f / (float)e->nranks : 1.f) : gscale, st, e->ls_mode == 2));
+  RET(ls_prepare(e, batch, st));
   if (e->use_graphs && !tc_profile_is_on()) {
     // the graphs read the inputs from fixed staging buffers and leave the results in the WORK arena / d_scalars, so one
     // captured graph serves any caller pointers; the copies either side are eager
@@ -1374,13 +1493,24 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
       if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
       CK(cudaEventRecord(e->ev_ar[k], e->comm_stream));
     }
+    if (e->ls_mode) {
+      // every rank takes the same decision: the saturation counts are summed like the gradients (the GRAD check after the sum is
+      // consistent by construction), and in dynamic mode each network's Adam waits for the scaler
+      if (e->ls_mode == 2) {
+        int r = e->nccl.AllReduce(&e->ls->sat_grad, &e->ls->sat_grad, 1, 5, 0, e->comm, e->comm_stream);     // ncclUint64, ncclSum
+        if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
+      }
+      RET(ls_check_grads(e, e->comm_stream));
+      CK(cudaEventRecord(e->ev_ls, e->comm_stream));
+      if (e->ls_mode == 2) { CK(cudaStreamWaitEvent(st, e->ev_ls, 0)); RET(ls_update(e, st)); }
+    }
     float* pp = e->P(); float* gg = e->G(); float* mm = (float*)e->arena[CGVC_ARENA_ADAM_M]; float* vv = (float*)e->arena[CGVC_ARENA_ADAM_V];
     for (int k = 0; k < 4; ++k) {
       CK(cudaStreamWaitEvent(st, e->ev_ar[k], 0));
       GraphKey kk; memset(&kk, 0, sizeof kk); kk.kind = 2 + k;
       const Range R = rg[k];
       RET(run_captured(e, kk, st, [&](cudaStream_t s) {
-        CK(launch_adam(pp + R.b, gg + R.b, mm + R.b, vv + R.b, (long long)R.n, R.hyper, ADAM_B1, ADAM_B2, ADAM_EPS, s));
+        CK(launch_adam(pp + R.b, gg + R.b, mm + R.b, vv + R.b, (long long)R.n, R.hyper, ADAM_B1, ADAM_B2, ADAM_EPS, s, ls_skip(e)));
         if (e->cfg.precision != CGVC_PREC_FP32_SIMT) {
           int r = tc_refresh_weights_range(e->tcw, pp, R.b, R.b + R.n, s);
           if (r != 0) return fail(e, CGVC_ERR_CUDA, "tc_refresh_weights: %s", cudaGetErrorString((cudaError_t)r));
@@ -1388,12 +1518,23 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
         return 0;
       }));
     }
+    if (e->ls_mode == 1) CK(cudaStreamWaitEvent(st, e->ev_ls, 0));
     rollback.armed = false;
     return 0;
   }
-  if (e->comm) RET(cgvc_allreduce_grads(e, stream));
+  if (e->comm) {
+    RET(cgvc_allreduce_grads(e, stream));
+    if (e->ls_mode == 2) {
+      int r = e->nccl.AllReduce(&e->ls->sat_grad, &e->ls->sat_grad, 1, 5, 0, e->comm, st);                      // ncclUint64, ncclSum
+      if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
+    }
+  }
   GraphKey k2; memset(&k2, 0, sizeof k2); k2.kind = 1;
-  RET(run_captured(e, k2, st, [&](cudaStream_t s) { return adam_body(e, s); }));
+  RET(run_captured(e, k2, st, [&](cudaStream_t s) {
+    if (e->ls_mode) RET(ls_check_grads(e, s));
+    if (e->ls_mode == 2) RET(ls_update(e, s));
+    return adam_body(e, s, ls_skip(e));
+  }));
   rollback.armed = false;
   return 0;
 }
@@ -1472,6 +1613,22 @@ int cgvc_set_option(cgvc_handle e, const char* name, int value) {
   if (!strcmp(name, "wgrad_f16")) {                          // F16F8 only: weight gradients from the fp16 planes alone
     e->tcw.wgrad16 = value != 0;
     for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
+    e->graphs.clear();
+    return 0;
+  }
+  if (!strcmp(name, "loss_scale") || !strcmp(name, "loss_scale_growth_interval")) {
+    const bool mode = !strcmp(name, "loss_scale");
+    if (mode ? (value < 0 || value > 2) : value < 1) return fail(e, CGVC_ERR_ARG, "option %s: bad value %d", name, value);
+    if (mode && value != e->ls_mode) {
+      DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+      long long t = 0;
+      RET(cgvc_get_adam_step(e, &t));                        // the step count moves between host and device with the mode
+      e->ls_mode = value;
+      RET(cgvc_set_adam_step(e, t));
+      e->ls_ready = false; e->ls_batch = 0;
+    }
+    if (!mode) e->ls_growth = value;
+    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);   // the captured steps hold the mode's pointers and the interval
     e->graphs.clear();
     return 0;
   }

@@ -5,6 +5,10 @@
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 #include <stdint.h>
+#ifdef __CUDACC__
+#include <cooperative_groups.h>
+#include <cooperative_groups/reduce.h>
+#endif
 
 // ---- "F16F8" operand planes (CGVC_PREC_F16F8; forward, data gradient and weight gradient since round 2): an fp32 tensor x is kept as
 //        q16  = fp16(x)                                   2 bytes / element   (hi * hi product: one kind::f16 MMA)
@@ -32,7 +36,50 @@ __device__ __forceinline__ void cgvc_quant4(const float (&v)[4], float s_hi, flo
   q8hi = cgvc_e4m3x4(f01.x * s_hi, f01.y * s_hi, f23.x * s_hi, f23.y * s_hi);
   q8lo = cgvc_e4m3x4((v[0] - f01.x) * s_lo, (v[1] - f01.y) * s_lo, (v[2] - f23.x) * s_lo, (v[3] - f23.y) * s_lo);
 }
+// Whether cgvc_quant4's planes of 4 values are wrong: true if an e4m3 conversion clamped (|scaled value| > 448, the largest e4m3 number, in
+// the hi or the lo plane) or fp16(x) is not finite.  With the activation-role scales the hi plane clamps once |fp16(x)| > 448 and the lo
+// plane, whose rounding residual reaches |x| * 2^-11, from |x| >= 256; fp16(x) itself overflows at 65504.
+#define CGVC_E4M3_MAX 448.f
+__device__ __forceinline__ bool cgvc_sat4(const float (&v)[4], float s_hi, float s_lo) {
+  bool bad = false;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float f = __half2float(__float2half_rn(v[k]));
+    bad |= !(fabsf(f * s_hi) <= CGVC_E4M3_MAX) || !(fabsf((v[k] - f) * s_lo) <= CGVC_E4M3_MAX);     // NaN / inf compare false
+  }
+  return bad;
+}
+// *ctr += hits, aggregated over the lanes of the warp that reach this call together: one reduction and, only if the sum is non-zero,
+// one atomic per such group.  The writers call this inside divergent loops, so the group is discovered (coalesced_threads), not
+// assumed to be the full warp
+__device__ __forceinline__ void cgvc_count_hits(unsigned long long* ctr, unsigned hits) {
+  namespace cg = cooperative_groups;
+  const cg::coalesced_group g = cg::coalesced_threads();
+  const unsigned n = cg::reduce(g, hits, cg::plus<unsigned>());
+  if (n && g.thread_rank() == 0) atomicAdd(ctr, (unsigned long long)n);
+}
 #endif
+
+// ---- dynamic loss scaling (engine option "loss_scale"; DESIGN.md section 10).  One per engine, in device memory.  The first fields
+// are cgvc_loss_scale_info of include/cgvc.h, in its layout (cgvc_loss_scale_state copies them out); the counters and the non-finite
+// flag are zeroed at the start of every train step and filled by the plane writers and the GRAD check
+struct LossScaler {
+  float scale;                    // loss scale the next step's gradients are formed with
+  int good_steps;                 // consecutive steps that were not skipped
+  long long skipped;              // steps skipped so far
+  int last_skipped;               // the last step was skipped
+  unsigned nonfinite;             // the last step's GRAD held a non-finite value: bit 0 generators, bit 1 discriminators
+  unsigned long long sat_grad;    // the last step's saturated 4-value groups in gradient planes
+  unsigned long long sat_act;     // ... in activation planes (diagnostic)
+  // engine-internal
+  long long t;                    // Adam step count (dynamic mode)
+  float scale_used;               // the scale the last step's gradients were formed with
+};
+// the Adam hyper-parameters of both optimizers after a step: hyper = d_scalars + 2 = [lr_G, 1/nranks, lr_D, 1/nranks] as the host wrote
+// them on entry, overwritten with [lr_t G, grad_scale, lr_t D, grad_scale] unless the step is skipped (see simt_kernels.cu)
+cudaError_t launch_loss_scale_update(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, cudaStream_t st);
+// nonfinite |= (bit 0 if a non-finite value lies in g[0, cut), bit 1 if in g[cut, n))
+cudaError_t launch_check_finite(const float* g, long long n, long long cut, unsigned* nonfinite, cudaStream_t st);
 
 extern unsigned long long g_cgvc_launches;   // incremented by every kernel launch of the library
 
@@ -109,6 +156,7 @@ struct PostParams {
   // packed variable-length samples (seg.off != null): sample b = view rows [seg.off[b] / seg.div, seg.off[b+1] / seg.div) of seg_rows
   // rows in all (the planes' extent is seg_rows * C); R = the longest sample (grid size).  launch_post_fwd only
   PackGeom seg; long long seg_rows;
+  unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
 };
 cudaError_t launch_post_fwd(const PostParams& pp, cudaStream_t st);
 
@@ -125,6 +173,7 @@ struct PostBwdParams {
   float *dbias_a, *dbias_g;             // conv-bias gradients [Cc] = column sums of dp (accumulated atomically; may be null)
   int qmode;                            // 1: dp_hi / dp_lo are F16F8 planes (q16; q8hi followed by q8lo) with the activation-role scales
   float* scratch;                       // [B,4,C] fp32 workspace (null: internal buffer, single-stream use only)
+  unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
 };
 cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st);
 void post_set_stream(int on);      // 1 (default): gated layers without shuffle and 32 / 48 / 64 positions per sample take the streaming (cp.async double-buffered) form of it
@@ -137,13 +186,15 @@ cudaError_t launch_head_fwd(const float* y, long long rows, int C, const float* 
 // dy[row,:] = dz * w (if dy);  dw += sum dz*y[row,:], db += sum dz (if dw)
 cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long rows, int C, const float* w,
                                  float target, float coef, float* loss_slot,
-                                 float* dy, float* dw, float* db, cudaStream_t st, float grad_mult = 1.f);
+                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev = nullptr);
 
 // ---- L1 loss + gradient (utils.py:6-8): loss_slot += mean|yhat - y|; d[i] = gscale * sign(yhat - y)/n  (accumulate optional)
 cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, float* loss_slot,
-                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, float grad_mult = 1.f);
-// grad_mult (both loss kernels): the gradients -- not the loss values -- are multiplied by it: the loss scale of the F16F8 gradient planes
-cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st);
+                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, const float* grad_mult_dev = nullptr);
+// grad_mult_dev (both loss kernels, null: 1): the gradients -- not the loss values -- are multiplied by *grad_mult_dev, the loss scale of the
+// F16F8 gradient planes; a device pointer, so that a captured step follows the dynamic scale
+// x *= a, or with div_dev x *= a / *div_dev
+cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st, const float* div_dev = nullptr);
 // [B,F,T] <-> [B,T,F]
 cudaError_t launch_transpose_ft(const float* in, float* out, int B, int F, int T, cudaStream_t st);
 // packed [F][len_u] blocks (block u at element F * off[u]) <-> channels-last rows [off[n], F]; to_rows = 1: blocks -> rows
@@ -152,9 +203,9 @@ cudaError_t launch_transpose_packed(const float* in, float* out, const long long
 cudaError_t launch_add(const float* a, const float* b, float* y, long long n, cudaStream_t st);
 
 // ---- TF-style Adam over a flat range (tf.train.AdamOptimizer; SURVEY.md Appendix A.6)
-// hyper_dev: [0] = lr_t (already bias-corrected step size), [1] = grad_scale
+// hyper_dev: [0] = lr_t (already bias-corrected step size), [1] = grad_scale.  skip_dev (may be null): when *skip_dev != 0, p, m, v stay untouched
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, long long n,
-                        const float* hyper_dev, float beta1, float beta2, float eps, cudaStream_t st);
+                        const float* hyper_dev, float beta1, float beta2, float eps, cudaStream_t st, const int* skip_dev = nullptr);
 // final loss algebra (model.py:72,83,88,90) on the 8-slot buffer
 cudaError_t launch_finalize_losses(float* losses8, const float* lambdas_dev, cudaStream_t st);
 
@@ -171,14 +222,17 @@ cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float*
 // fp32 [M, C] (row stride ld) -> zero-padded bf16 hi/lo planes [M, Cpad]
 cudaError_t launch_pad_split(const float* x, long long M, int C, int ld, int Cpad, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st);
 // same into F16F8 planes: q16 [M, Cpad] halves, q8 = [M*Cpad bytes of q8hi | M*Cpad bytes of q8lo] (activation scales)
-cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st);
+// sat (may be null): count of saturated 4-value groups (cgvc_quant4_sat)
+cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st,
+                               unsigned long long* sat = nullptr);
 // tap lowering of the generator's 15-tap edge layers (simt_kernels.cu): im2col of a narrow channels-last tensor over the taps of a
 // stride-1 1-D TF-SAME convolution into operand planes [M, Cpad] (qmode 1: F16F8 planes q16 / q8hi|q8lo, else bf16 hi / lo), dir = +1:
 // out[m, t*C + c] = x[m + t - pl, c], dir = -1: x[m - t + pl, c] (zero outside the sample, pl = (kw - 1) / 2), and the matching sum
 // y[m, c] = bias[c] + sum_t z[m + dir*(t - pl), t*C + c]
 // With off (n + 1 device frame prefix sums, packed utterances) the samples are [off[u], off[u+1]) instead of T-row blocks (T ignored).
+// sat (qmode, may be null): count of saturated 4-value groups (cgvc_quant4_sat)
 cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st,
-                               const long long* off = nullptr, int n_off = 0);
+                               const long long* off = nullptr, int n_off = 0, unsigned long long* sat = nullptr);
 cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st,
                                const long long* off = nullptr, int n_off = 0);
 // P[m, 0:2*cout] = [bias_a | bias_g] + sum_t x[src(m,t)] * [wa | wg][t]   (single input channel, TF kernels [taps][1][cout])
@@ -188,7 +242,8 @@ cudaError_t launch_conv_c1_fwd(const GatherGeom& g, const float* x, const float*
 // ... and with the layer's GLU in the same pass (gate without instance norm): also y = a * sigmoid(g) as fp32 [M, cout] (optional) and as
 // operand planes (bf16 hi / lo, or with qmode the F16F8 planes q16; q8hi followed by q8lo); <= 9 taps
 cudaError_t launch_conv_c1_glu_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
-                                   int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st);
+                                   int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st,
+                                   unsigned long long* sat = nullptr);
 
 // s[off .. off+n) = v6_host[0..n)  (n <= 6), passed by value in the kernel arguments (no host-memory copy node)
 cudaError_t launch_set_scalars(float* s, int off, int n, const float* v6_host, cudaStream_t st);

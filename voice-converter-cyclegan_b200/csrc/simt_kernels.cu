@@ -402,19 +402,27 @@ __device__ __forceinline__ void st4_split(__nv_bfloat16* hi, __nv_bfloat16* lo, 
   *reinterpret_cast<uint2*>(hi) = hv;
   *reinterpret_cast<uint2*>(lo) = lv;
 }
-// F16F8 planes of 4 consecutive activation values (o = element offset, n = elements per plane)
-__device__ __forceinline__ void st4_quant(__nv_bfloat16* q16, __nv_bfloat16* q8, long long o, long long n, const F4& a) {
+// F16F8 planes of 4 consecutive activation values (o = element offset, n = elements per plane); sat: see cgvc_count_hits (null: no count)
+__device__ __forceinline__ void st4_quant(__nv_bfloat16* q16, __nv_bfloat16* q8, long long o, long long n, const F4& a,
+                                          unsigned long long* sat = nullptr) {
   uint2 h; uint32_t b_hi, b_lo;
   cgvc_quant4(a.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO, h, b_hi, b_lo);
   *reinterpret_cast<uint2*>(q16 + o) = h;
   uint8_t* base = reinterpret_cast<uint8_t*>(q8);
   *reinterpret_cast<uint32_t*>(base + o) = b_hi;
   *reinterpret_cast<uint32_t*>(base + n + o) = b_lo;
+  if (sat) cgvc_count_hits(sat, cgvc_sat4(a.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
 }
 __device__ __forceinline__ F4 zero4() { return F4{{0.f, 0.f, 0.f, 0.f}}; }
 __device__ __forceinline__ F4 one4() { return F4{{1.f, 1.f, 1.f, 1.f}}; }
 __device__ __forceinline__ void atomic_add4(float* p, const F4& a) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a.v[0]), "f"(a.v[1]), "f"(a.v[2]), "f"(a.v[3]) : "memory");
+}
+
+// saturated groups among the gradient planes of da (and dg): out of line, so that the counting leaves the register allocation of the
+// kernel's uncounted path alone
+__device__ __noinline__ unsigned sat_groups(const F4 da, const F4 dg, bool gate) {
+  return cgvc_sat4(da.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO) + (gate && cgvc_sat4(dg.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
 }
 
 constexpr int kPostRows = 32;      // positions per CTA
@@ -557,7 +565,7 @@ post_apply_fwd_kernel(const __grid_constant__ PostParams q, const float* __restr
         for (int k = 0; k < 4; ++k) y.v[k] += rr.v[k]; }
       if (q.y) st4(q.y + o, y);
       if (q.y_hi) {
-        if (q.qmode) st4_quant(q.y_hi, q.y_lo, o, PK ? q.seg_rows * q.C : (long long)q.B * q.R * q.C, y);
+        if (q.qmode) st4_quant(q.y_hi, q.y_lo, o, PK ? q.seg_rows * q.C : (long long)q.B * q.R * q.C, y, q.sat);
         else st4_split(q.y_hi + o, q.y_lo + o, y);
       }
     }
@@ -697,6 +705,7 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
   const float* pb = q.p + (long long)ix.b * Rw * q.ldp;
   const long long dpoff = (long long)ix.b * Rw * q.ldp;
   F4 bsum[2] = {zero4(), zero4()};                      // this thread's share of the conv-bias gradients (a, g)
+  unsigned nsat = 0;                                     // saturated plane groups (q.sat), added to the counter after the loop
   if (ix.cvalid) {
     // per channel (Appendix A.7):  xhat = x*r + h ; norm = x*sc + of ; dx = c1*dn - c2 - xhat*c3
     F4 ra = one4(), ha = zero4(), sca = one4(), ofa = zero4(), c1a = one4(), c2a = zero4(), c3a = zero4();
@@ -760,6 +769,7 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
             const long long nq = (long long)q.B * Rw * q.ldp;
             st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da);
             if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg);
+            if (q.sat) nsat += sat_groups(da, dg, HAS_GATE);
           } else {
             st4_split(q.dp_hi + dpoff + a, q.dp_lo + dpoff + a, da);
             if (HAS_GATE) st4_split(q.dp_hi + dpoff + a + q.Cc, q.dp_lo + dpoff + a + q.Cc, dg);
@@ -768,6 +778,7 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
       }
     }
   }
+  if (q.sat) cgvc_count_hits(q.sat, nsat);
   if (q.dbias_a) {
     // positions of lane rl have shuffle phase rl % sh (chunk size and lane stride are even): reduce per phase
     red[0][ix.rl][lane] = make_float4(bsum[0].v[0], bsum[0].v[1], bsum[0].v[2], bsum[0].v[3]);
@@ -895,8 +906,8 @@ post_bwd_onepass_kernel(const __grid_constant__ PostBwdParams q) {
         if (q.dp_hi) {
           if (q.qmode) {                                     // F16F8 gradient planes (activation-role scales): q16, then q8hi | q8lo
             const long long nq = (long long)q.B * Rw * q.ldp;
-            st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da);
-            if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg);
+            st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da, q.sat);
+            if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg, q.sat);
           } else {
             st4_split(q.dp_hi + dpoff + a, q.dp_lo + dpoff + a, da);
             if (HAS_GATE) st4_split(q.dp_hi + dpoff + a + q.Cc, q.dp_lo + dpoff + a + q.Cc, dg);
@@ -1080,7 +1091,7 @@ post_bwd_stream_kernel(const __grid_constant__ PostBwdParams q, int items, int c
       const long long a = dpoff + (long long)(r >> shs) * q.ldp + (r & shs) * q.C;
       if (q.dp) { st4(q.dp + a, da); if (GATE) st4(q.dp + a + q.Cc, dg); }
       if (q.dp_hi) {
-        if (q.qmode) { st4_quant(q.dp_hi, q.dp_lo, a, nplane, da); if (GATE) st4_quant(q.dp_hi, q.dp_lo, a + q.Cc, nplane, dg); }
+        if (q.qmode) { st4_quant(q.dp_hi, q.dp_lo, a, nplane, da, q.sat); if (GATE) st4_quant(q.dp_hi, q.dp_lo, a + q.Cc, nplane, dg, q.sat); }
         else { st4_split(q.dp_hi + a, q.dp_lo + a, da); if (GATE) st4_split(q.dp_hi + a + q.Cc, q.dp_lo + a + q.Cc, dg); }
       }
     }
@@ -1219,7 +1230,7 @@ post_fwd_stream_kernel(const __grid_constant__ PostParams q, int items, int cblo
       const long long e = ((long long)b * R + r) * q.C + c;
       if (q.y) st4(q.y + e, y);
       if (q.y_hi) {
-        if (q.qmode) st4_quant(q.y_hi, q.y_lo, e, nplane, y);
+        if (q.qmode) st4_quant(q.y_hi, q.y_lo, e, nplane, y, q.sat);
         else st4_split(q.y_hi + e, q.y_lo + e, y);
       }
     }
@@ -1357,9 +1368,10 @@ cudaError_t launch_head_fwd(const float* y, long long rows, int C, const float* 
 __global__ void __launch_bounds__(256)
 head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y, long long rows, int C,
                      const float* __restrict__ w, float target, float coef, float* __restrict__ loss_slot,
-                     float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ db, float grad_mult) {
+                     float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ db, const float* __restrict__ grad_mult_dev) {
   __shared__ float red[8][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float grad_mult = grad_mult_dev ? *grad_mult_dev : 1.f;
   float4 accw[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) accw[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1408,12 +1420,12 @@ head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y
 
 cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long rows, int C, const float* w,
                                  float target, float coef, float* loss_slot,
-                                 float* dy, float* dw, float* db, cudaStream_t st, float grad_mult) {
+                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev) {
   if (rows == 0) return cudaSuccess;
   if (C != 1024) return cudaErrorInvalidValue;
   long long nb = (rows + 7) / 8;
   if (nb > 296) nb = 296;
-  ++g_cgvc_launches; head_loss_bwd_kernel<<<(unsigned)nb, 256, 0, st>>>(prob, y, rows, C, w, target, coef, loss_slot, dy, dw, db, grad_mult);
+  ++g_cgvc_launches; head_loss_bwd_kernel<<<(unsigned)nb, 256, 0, st>>>(prob, y, rows, C, w, target, coef, loss_slot, dy, dw, db, grad_mult_dev);
   return cudaGetLastError();
 }
 
@@ -1422,10 +1434,10 @@ cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long ro
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 l1_loss_grad_kernel(const float* __restrict__ yhat, const float* __restrict__ y, long long n, float* __restrict__ loss_slot,
-                    const float* __restrict__ gscale_dev, float* __restrict__ d, int accumulate, float grad_mult) {
+                    const float* __restrict__ gscale_dev, float* __restrict__ d, int accumulate, const float* __restrict__ grad_mult_dev) {
   __shared__ float red[8][32];
   const float inv = 1.f / (float)n;
-  const float gs = (gscale_dev ? gscale_dev[0] * inv : inv) * grad_mult;
+  const float gs = (gscale_dev ? gscale_dev[0] * inv : inv) * (grad_mult_dev ? *grad_mult_dev : 1.f);
   float s = 0.f;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
     float e = yhat[i] - y[i];
@@ -1443,10 +1455,10 @@ l1_loss_grad_kernel(const float* __restrict__ yhat, const float* __restrict__ y,
 }
 
 cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, float* loss_slot,
-                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, float grad_mult) {
+                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, const float* grad_mult_dev) {
   if (n == 0) return cudaSuccess;
   long long nb = (n + 255) / 256; if (nb > 592) nb = 592;
-  ++g_cgvc_launches; l1_loss_grad_kernel<<<(unsigned)nb, 256, 0, st>>>(yhat, y, n, loss_slot, gscale_dev, d, accumulate, grad_mult);
+  ++g_cgvc_launches; l1_loss_grad_kernel<<<(unsigned)nb, 256, 0, st>>>(yhat, y, n, loss_slot, gscale_dev, d, accumulate, grad_mult_dev);
   return cudaGetLastError();
 }
 
@@ -1511,7 +1523,8 @@ cudaError_t launch_add(const float* a, const float* b, float* y, long long n, cu
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n,
-            const float* __restrict__ hyper, float beta1, float beta2, float eps) {
+            const float* __restrict__ hyper, float beta1, float beta2, float eps, const int* __restrict__ skip) {
+  if (skip && *skip) return;                         // a step the loss scaler skipped: p, m and v keep their values
   const float lr_t = hyper[0], gscale = hyper[1];
   const long long n4 = n >> 2;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
@@ -1543,12 +1556,71 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
 }
 
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, long long n,
-                        const float* hyper_dev, float beta1, float beta2, float eps, cudaStream_t st) {
+                        const float* hyper_dev, float beta1, float beta2, float eps, cudaStream_t st, const int* skip_dev) {
   if (n == 0) return cudaSuccess;
   if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
        reinterpret_cast<uintptr_t>(v)) & 15) return cudaErrorMisalignedAddress;
   long long nb = ((n >> 2) + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16; if (nb < 1) nb = 1;
-  ++g_cgvc_launches; adam_kernel<<<(unsigned)nb, 256, 0, st>>>(p, g, m, v, n, hyper_dev, beta1, beta2, eps);
+  ++g_cgvc_launches; adam_kernel<<<(unsigned)nb, 256, 0, st>>>(p, g, m, v, n, hyper_dev, beta1, beta2, eps, skip_dev);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Dynamic loss scaling (DESIGN.md section 10): the GRAD check and the once-per-step scaler update
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+check_finite_kernel(const float* __restrict__ g, long long n, long long cut, unsigned* __restrict__ nonfinite) {
+  unsigned bits = 0;
+  const long long n4 = n >> 2;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
+    const float4 v = reinterpret_cast<const float4*>(g)[i];
+    const float a[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) if (!isfinite(a[k])) bits |= (4 * i + k) < cut ? 1u : 2u;
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const long long i = (n4 << 2) + threadIdx.x;
+    if (!isfinite(g[i])) bits |= i < cut ? 1u : 2u;
+  }
+  bits = __reduce_or_sync(0xffffffffu, bits);
+  if ((threadIdx.x & 31) == 0 && bits) atomicOr(nonfinite, bits);
+}
+
+cudaError_t launch_check_finite(const float* g, long long n, long long cut, unsigned* nonfinite, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  if (reinterpret_cast<uintptr_t>(g) & 15) return cudaErrorMisalignedAddress;
+  long long nb = ((n >> 2) + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16; if (nb < 1) nb = 1;
+  ++g_cgvc_launches; check_finite_kernel<<<(unsigned)nb, 256, 0, st>>>(g, n, cut, nonfinite);
+  return cudaGetLastError();
+}
+
+// One thread.  Overflow (a saturated gradient plane or a non-finite gradient): skip the step, halve the scale (floor 1), reset the
+// good-step count.  Otherwise advance Adam's t and, after growth_interval good steps in a row, double the scale (cap 2^24).  adapt = 0
+// (the precisions without reduced-range gradient planes): the scale stays where it is and only the skip applies.  lr_t uses the same
+// double-precision formula as the host's set_adam_scalars (engine.cu); CUDA's pow is within 2 ulp, not correctly rounded, so the fp32
+// result can differ from the host's in the last bit when the double lies at an fp32 rounding boundary.
+__global__ void loss_scale_update_kernel(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2) {
+  const float used = s->scale;
+  s->scale_used = used;
+  if (s->sat_grad > 0 || s->nonfinite) {
+    s->last_skipped = 1; s->good_steps = 0; s->skipped += 1;
+    if (adapt) s->scale = fmaxf(1.f, used * 0.5f);
+    return;
+  }
+  s->last_skipped = 0;
+  s->t += 1;
+  if (++s->good_steps >= growth_interval) {
+    s->good_steps = 0;
+    if (adapt) s->scale = fminf(16777216.f, used * 2.f);
+  }
+  const double t = (double)s->t;
+  const double corr = sqrt(1.0 - pow((double)beta2, t)) / (1.0 - pow((double)beta1, t));
+  hyper[0] = (float)(hyper[0] * corr); hyper[1] = hyper[1] / used;      // generator optimizer: lr -> lr_t, 1/nranks -> grad_scale
+  hyper[2] = (float)(hyper[2] * corr); hyper[3] = hyper[3] / used;      // discriminator optimizer
+}
+
+cudaError_t launch_loss_scale_update(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, cudaStream_t st) {
+  ++g_cgvc_launches; loss_scale_update_kernel<<<1, 1, 0, st>>>(s, hyper, adapt, growth_interval, beta1, beta2);
   return cudaGetLastError();
 }
 
@@ -1917,7 +1989,8 @@ pad_split_kernel(const float* __restrict__ x, long long M, int C, int ld, int Cp
 
 // fp32 rows [M, C] -> F16F8 planes [M, Cpad] (Cpad a multiple of 4), zero channels [C, Cpad)
 __global__ void __launch_bounds__(256)
-pad_split_q_kernel(const float* __restrict__ x, long long M, int C, int ld, int Cpad, __half* __restrict__ q16, uint8_t* __restrict__ q8) {
+pad_split_q_kernel(const float* __restrict__ x, long long M, int C, int ld, int Cpad, __half* __restrict__ q16, uint8_t* __restrict__ q8,
+                   unsigned long long* __restrict__ sat) {
   const long long n = M * Cpad, nq = n / 4;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nq; i += (long long)gridDim.x * 256) {
     const long long e = i * 4; const int c = (int)(e % Cpad); const long long m = e / Cpad;
@@ -1929,15 +2002,16 @@ pad_split_q_kernel(const float* __restrict__ x, long long M, int C, int ld, int 
     *reinterpret_cast<uint2*>(q16 + e) = h;
     *reinterpret_cast<uint32_t*>(q8 + e) = b_hi;
     *reinterpret_cast<uint32_t*>(q8 + n + e) = b_lo;
+    if (sat) cgvc_count_hits(sat, cgvc_sat4(v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
   }
 }
 
-cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st) {
+cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st, unsigned long long* sat) {
   if (M == 0) return cudaSuccess;
   if (Cpad % 4) return cudaErrorInvalidValue;
   long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
-  pad_split_q_kernel<<<(unsigned)nb, 256, 0, st>>>(x, M, C, ld, Cpad, (__half*)q16, (uint8_t*)q8);
+  pad_split_q_kernel<<<(unsigned)nb, 256, 0, st>>>(x, M, C, ld, Cpad, (__half*)q16, (uint8_t*)q8, sat);
   return cudaGetLastError();
 }
 
@@ -1973,7 +2047,7 @@ __device__ __forceinline__ int tap_sample(long long m, int T, const long long* _
 template <int Q>
 __global__ void __launch_bounds__(256)
 im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int kw, int pl, int dir, int Cpad, void* __restrict__ hi, void* __restrict__ lo,
-                   const long long* __restrict__ off, int n_off) {
+                   const long long* __restrict__ off, int n_off, unsigned long long* __restrict__ sat) {
   const long long n = M * Cpad, nq = n / 4;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nq; i += (long long)gridDim.x * 256) {
     const long long e = i * 4; const int col = (int)(e % Cpad); const long long m = e / Cpad;
@@ -1990,6 +2064,7 @@ im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int k
       *reinterpret_cast<uint2*>((__half*)hi + e) = h;
       *reinterpret_cast<uint32_t*>((uint8_t*)lo + e) = b_hi;
       *reinterpret_cast<uint32_t*>((uint8_t*)lo + n + e) = b_lo;
+      if (sat) cgvc_count_hits(sat, cgvc_sat4(v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
     } else {
       __align__(8) __nv_bfloat16 h[4]; __align__(8) __nv_bfloat16 l[4];
 #pragma unroll
@@ -2001,14 +2076,14 @@ im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int k
 }
 
 cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st,
-                               const long long* off, int n_off) {
+                               const long long* off, int n_off, unsigned long long* sat) {
   if (M == 0) return cudaSuccess;
   if (C % 4 || Cpad % 4 || Cpad < kw * C || (!off && (T <= 0 || M % T)) || (off && n_off < 1)) return cudaErrorInvalidValue;
   const int pl = (kw - 1) / 2;                      // TF SAME at stride 1: total pad kw - 1, the smaller half on the left
   long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
-  if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off);
-  else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off);
+  if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off, sat);
+  else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off, nullptr);
   return cudaGetLastError();
 }
 
@@ -2102,7 +2177,7 @@ __global__ void __launch_bounds__(256)
 conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ x, const float* __restrict__ wa, const float* __restrict__ wg,
                        const float* __restrict__ ba, const float* __restrict__ bg, int cout, float* __restrict__ P,
                        float* __restrict__ y, __nv_bfloat16* __restrict__ y_hi, __nv_bfloat16* __restrict__ y_lo, int qmode, long long plane_elems,
-                       int rows_per_block) {
+                       int rows_per_block, unsigned long long* __restrict__ sat) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   const int nq = cout / 4;                             // channel quads (host guarantees nq divides 256)
   const int cq = threadIdx.x % nq, rl = threadIdx.x / nq, rstep = 256 / nq;
@@ -2140,7 +2215,7 @@ conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __rest
       const long long e = m * cout + n;
       if (y) st4(y + e, o);
       if (y_hi) {
-        if (qmode) st4_quant(y_hi, y_lo, e, plane_elems, o);
+        if (qmode) st4_quant(y_hi, y_lo, e, plane_elems, o, sat);
         else st4_split(y_hi + e, y_lo + e, o);
       }
     }
@@ -2148,14 +2223,15 @@ conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __rest
 }
 
 cudaError_t launch_conv_c1_glu_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
-                                   int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st) {
+                                   int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st,
+                                   unsigned long long* sat) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = cout / 4;
   if (cout % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9) return cudaErrorInvalidValue;
   int rpb = 4 * kC1Rows;
   ++g_cgvc_launches;
-  conv_c1_glu_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode, M * cout, rpb);
+  conv_c1_glu_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode, M * cout, rpb, sat);
   return cudaGetLastError();
 }
 
@@ -2251,12 +2327,13 @@ cudaError_t launch_gather_minibatch(const float* cA, const long long* off_A, con
 
 
 // x *= a  (un-scaling the gradient arena after a loss-scaled backward pass whose result is handed out instead of going into Adam)
-__global__ void __launch_bounds__(256) scale_kernel(float* __restrict__ x, long long n, float a) {
+__global__ void __launch_bounds__(256) scale_kernel(float* __restrict__ x, long long n, float a, const float* __restrict__ div) {
+  if (div) a = a / *div;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) x[i] *= a;
 }
-cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st) {
+cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st, const float* div_dev) {
   if (n == 0) return cudaSuccess;
   long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 8) nb = CGVC_NUM_SMS * 8;
-  ++g_cgvc_launches; scale_kernel<<<(unsigned)nb, 256, 0, st>>>(x, n, a);
+  ++g_cgvc_launches; scale_kernel<<<(unsigned)nb, 256, 0, st>>>(x, n, a, div_dev);
   return cudaGetLastError();
 }

@@ -11,6 +11,8 @@ Differences a user of the reference should know:
   * checkpoints are .npz files keyed by the TF variable names (plus `<var>/Adam`, `<var>/Adam_1`, `adam_step`)
   * with `torch.distributed` initialised and `data_parallel=True`, one process per GPU trains data-parallel:
     a single NCCL all-reduce of the flat gradient arena per step
+  * `loss_scale='monitor'` counts saturated F16F8 gradient / activation planes and non-finite gradients every step;
+    `loss_scale='dynamic'` also skips such steps and adapts the loss scale (include/cgvc.h, DESIGN.md section 10)
 """
 from __future__ import annotations
 
@@ -35,7 +37,7 @@ class CycleGAN(object):
 
     def __init__(self, num_features, discriminator=_discriminator, generator=_generator_gatedcnn, mode='train',
                  log_dir='./log', *, max_batch=1, max_frames=None, precision='bf16x3', device=None, seed=0,
-                 data_parallel=False, summary_interval=0):
+                 data_parallel=False, summary_interval=0, loss_scale='static'):
         for net in (discriminator, generator):
             if not hasattr(net, "check_engine_table"):
                 raise TypeError("CycleGAN(discriminator=..., generator=...) takes network descriptors (cgvc.module.generator_gatedcnn / "
@@ -57,6 +59,12 @@ class CycleGAN(object):
         self._max_frames = int(max_frames) if max_frames else 128
         self._arenas = {}
         self._options = {}
+        if loss_scale not in N.LOSS_SCALE_MODES:
+            raise ValueError("loss_scale must be one of %s, got %r" % (sorted(N.LOSS_SCALE_MODES), loss_scale))
+        if loss_scale != 'static':
+            self._options["loss_scale"] = N.LOSS_SCALE_MODES[loss_scale]     # applied by _create_engine, like any remembered option
+        self.last_step_skipped = False
+        self.last_loss_scale = None
         self._create_engine()
         # the descriptors state the architecture the caller expects (model.py:14-15); the engine must implement exactly that
         for scope in ("generator_A2B", "generator_B2A"):
@@ -115,21 +123,50 @@ class CycleGAN(object):
             self._chk(self._lib.cgvc_bind_arena(h, kind, _ptr(t), t.numel() * 4))
         self._losses = torch.zeros(8, dtype=torch.float32, device=self.device)
         self._losses_host = torch.zeros(8, dtype=torch.float32).pin_memory()
+        self._ls_dev = torch.zeros(C.sizeof(N.LossScaleInfo), dtype=torch.uint8, device=self.device)
+        self._ls_host = torch.zeros(C.sizeof(N.LossScaleInfo), dtype=torch.uint8).pin_memory()
         self._staging = {}
         for name, value in self._options.items():            # the engine is re-created when batch / frames outgrow it
             self._chk(self._lib.cgvc_set_option(self._handle, name.encode(), int(value)))
 
     def set_option(self, name, value):
-        """Engine options of include/cgvc.h (`two_streams`, `cuda_graph`, `fuse_in`, `fuse_bwd`, `debug_taps`); remembered across
-        engine re-creations."""
+        """Engine options of include/cgvc.h (`two_streams`, `cuda_graph`, `fuse_in`, `fuse_bwd`, `debug_taps`, `loss_scale`, ...);
+        remembered across engine re-creations."""
         self._chk(self._lib.cgvc_set_option(self._handle, name.encode(), int(value)))
         self._options[name] = int(value)
+
+    @property
+    def loss_scale(self):
+        """'static', 'monitor' or 'dynamic' (engine option "loss_scale")."""
+        mode = self._options.get("loss_scale", 0)
+        return next(k for k, v in N.LOSS_SCALE_MODES.items() if v == mode)
+
+    def _enqueue_loss_scale_state(self):
+        self._chk(self._lib.cgvc_loss_scale_state(self._handle, _ptr(self._ls_dev), self._stream()))
+        self._ls_host.copy_(self._ls_dev, non_blocking=True)
+
+    def _read_loss_scale_state(self):
+        """after the stream synchronisation that follows _enqueue_loss_scale_state"""
+        info = N.LossScaleInfo.from_buffer_copy(self._ls_host.numpy().tobytes())
+        self.last_loss_scale = {f: getattr(info, f) for f, _ in N.LossScaleInfo._fields_}
+        self.last_loss_scale["last_skipped"] = bool(info.last_skipped)
+        self.last_step_skipped = self.last_loss_scale["last_skipped"]
+        return dict(self.last_loss_scale)
+
+    def loss_scale_state(self):
+        """The loss scaler's state after the most recent step (synchronises): scale, good_steps, skipped, last_skipped and the last
+        step's sat_grad / sat_act (saturated 4-value groups of the F16F8 gradient / activation planes) and nonfinite (bit 0: a
+        generator gradient, bit 1: a discriminator gradient).  The counters are collected in 'monitor' and 'dynamic' mode only."""
+        self._enqueue_loss_scale_state()
+        torch.cuda.current_stream(self.device).synchronize()
+        return self._read_loss_scale_state()
 
     def _ensure_capacity(self, batch, frames):
         if batch <= self._max_batch and frames <= self._max_frames:
             return
         step = C.c_longlong(0)
         self._lib.cgvc_get_adam_step(self._handle, C.byref(step))
+        ls = self.loss_scale_state() if self.loss_scale == 'dynamic' else None
         self._lib.cgvc_destroy(self._handle)
         self._max_batch = max(batch, self._max_batch)
         self._max_frames = max(frames, self._max_frames)
@@ -137,6 +174,8 @@ class CycleGAN(object):
         torch.cuda.empty_cache()
         self._create_engine()
         self._lib.cgvc_set_adam_step(self._handle, step)
+        if ls is not None and ls["scale"] >= 1:
+            self._chk(self._lib.cgvc_set_loss_scale_state(self._handle, ls["scale"], ls["good_steps"], ls["skipped"], self._stream()))
         if self._data_parallel:
             # cgvc_destroy freed the NCCL communicator with the old engine: a data-parallel model must get a new one, or it would
             # silently train without the all-reduce.  Collective: every rank has to grow in the same call (same batch / frames).
@@ -252,7 +291,12 @@ class CycleGAN(object):
                                             float(generator_learning_rate), float(discriminator_learning_rate),
                                             None, None, _ptr(self._losses), self._stream()))
         self._losses_host.copy_(self._losses, non_blocking=True)
+        monitored = self.loss_scale != 'static'
+        if monitored:
+            self._enqueue_loss_scale_state()
         torch.cuda.current_stream(self.device).synchronize()
+        if monitored:
+            self._read_loss_scale_state()
         l = self._losses_host.numpy()
         self.last_losses = {k: float(v) for k, v in zip(N.LOSS_NAMES, l)}
         if self.writer is not None and self.summary_interval and self.train_step % self.summary_interval == 0:
@@ -273,7 +317,12 @@ class CycleGAN(object):
         """(generator_loss, discriminator_loss) of the most recent train_async step: the one device -> host read (32 bytes) and stream
         synchronisation a device-resident training loop needs, at the steps it logs."""
         self._losses_host.copy_(self._losses, non_blocking=True)
+        monitored = self.loss_scale != 'static'
+        if monitored:
+            self._enqueue_loss_scale_state()
         torch.cuda.current_stream(self.device).synchronize()
+        if monitored:
+            self._read_loss_scale_state()
         l = self._losses_host.numpy()
         self.last_losses = {k: float(v) for k, v in zip(N.LOSS_NAMES, l)}
         if self.writer is not None and self.summary_interval:
@@ -397,6 +446,11 @@ class CycleGAN(object):
         step = C.c_longlong(0)
         self._lib.cgvc_get_adam_step(self._handle, C.byref(step))
         blob["adam_step"] = np.int64(step.value)
+        if self.loss_scale != 'static':
+            ls = self.loss_scale_state()
+            blob["loss_scale"] = np.float32(ls["scale"])
+            blob["loss_scale_good_steps"] = np.int64(ls["good_steps"])
+            blob["loss_scale_skipped"] = np.int64(ls["skipped"])
         blob["train_step"] = np.int64(self.train_step)
         with open(path + ".npz" if not path.endswith(".npz") else path, "wb") as f:
             np.savez(f, **blob)
@@ -420,6 +474,9 @@ class CycleGAN(object):
             self._lib.cgvc_set_adam_step(self._handle, int(z["adam_step"]))
         if "train_step" in z:
             self.train_step = int(z["train_step"])
+        if self.loss_scale == 'dynamic' and "loss_scale" in z and float(z["loss_scale"]) >= 1:
+            self._chk(self._lib.cgvc_set_loss_scale_state(self._handle, float(z["loss_scale"]), int(z["loss_scale_good_steps"]),
+                                                          int(z["loss_scale_skipped"]), self._stream()))
         self._params_updated()
 
     def _load_tf_bundle(self, prefix):

@@ -146,13 +146,23 @@ def validation_conversions(model, epoch, validation_A_dir, validation_B_dir, out
     return written
 
 
+def loss_scale_log(model, loss_scale):
+    """The loss-scaler part of the periodic log line (empty in static mode): the state train() / fetch_losses() read last."""
+    ls = model.last_loss_scale if loss_scale != 'static' else None
+    if not ls:
+        return ''
+    return ', Loss Scale: {:g}, Skipped Steps: {:d}, Saturated Groups (gradient / activation): {:d} / {:d}{}'.format(
+        ls['scale'], ls['skipped'], ls['sat_grad'], ls['sat_act'], ', Non-finite Gradients' if ls['nonfinite'] else '')
+
+
 def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epochs, mini_batch_size, synthetic=0,
           precision="bf16x3", log_every=50, device_data=True, validation_A_dir=None, validation_B_dir=None, output_dir='./validation_output',
-          tensorboard_log_dir='./log'):
+          tensorboard_log_dir='./log', loss_scale='static'):
     """The reference's training loop (train.py:78-118).  device_data=True (default): the normalised corpus is uploaded once and the
     epoch sampler runs on the device (DeviceDataset), so no step copies anything host -> device and the losses are read back only
     when they are printed; device_data=False feeds host minibatches from the numpy sampler through CycleGAN.train(), like the
-    reference's feed_dict."""
+    reference's feed_dict.  loss_scale: 'static', 'monitor' or 'dynamic' (CycleGAN); when not static the log line also reports the
+    loss scale, the skipped steps and the last step's saturated F16F8 plane groups."""
     from .model import CycleGAN
     np.random.seed(random_seed)                                   # train.py:13
     f0_A = f0_B = None
@@ -173,7 +183,7 @@ def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epoc
         logf0_stats = {'mean_A': mA, 'std_A': sA, 'mean_B': mB, 'std_B': sB}
     mcep_stats = {'mean_A': A_mean, 'std_A': A_std, 'mean_B': B_mean, 'std_B': B_std}
     model = CycleGAN(num_features=NUM_MCEP, max_batch=mini_batch_size, max_frames=N_FRAMES, precision=precision, seed=random_seed,
-                     log_dir=tensorboard_log_dir)
+                     log_dir=tensorboard_log_dir, loss_scale=loss_scale)
     test_model = None
     data = DeviceDataset(model, A_norm, B_norm, mini_batch_size, N_FRAMES, seed=random_seed) if device_data else None
     g_loss = d_loss = float("nan")
@@ -201,7 +211,7 @@ def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epoc
                                              generator_learning_rate=lr_g, discriminator_learning_rate=lr_d)
             if log:
                 print('Iteration: {:07d}, Generator Learning Rate: {:.7f}, Discriminator Learning Rate: {:.7f}, Generator Loss : {:.3f}, '
-                      'Discriminator Loss : {:.3f}'.format(num_iterations, lr_g, lr_d, g_loss, d_loss))
+                      'Discriminator Loss : {:.3f}'.format(num_iterations, lr_g, lr_d, g_loss, d_loss) + loss_scale_log(model, loss_scale))
         model.save(directory=model_dir, filename=model_name)      # train.py:113
         if (validation_A_dir is not None or validation_B_dir is not None) and epoch % VALIDATION_INTERVAL == 0:      # train.py:119-155
             if test_model is None:
@@ -227,13 +237,16 @@ def main():
     p.add_argument('--tensorboard_log_dir', type=str, default='./log')                # train.py:172
     p.add_argument('--synthetic', type=int, default=0, help='use N random utterances per speaker instead of the data directories')
     p.add_argument('--precision', type=str, default='bf16x3')
+    p.add_argument('--loss_scale', type=str, default='static', choices=['static', 'monitor', 'dynamic'],
+                   help='F16F8 gradient-plane loss scale: static (fixed), monitor (fixed, saturation counted and logged) or dynamic '
+                        '(saturated or non-finite steps skipped, scale adapted)')
     p.add_argument('--host_data', action='store_true', help='feed host minibatches from the numpy sampler every step (the reference\'s feed) '
                                                              'instead of the device-resident corpus + device sampler')
     a = p.parse_args()
     none = lambda v: None if v in ('None', 'none') else v                                # train.py:191-192
     train(a.train_A_dir, a.train_B_dir, a.model_dir, a.model_name, a.random_seed, a.epochs, a.batch_size, a.synthetic, a.precision,
           device_data=not a.host_data, validation_A_dir=none(a.validation_A_dir), validation_B_dir=none(a.validation_B_dir),
-          output_dir=a.output_dir, tensorboard_log_dir=a.tensorboard_log_dir)
+          output_dir=a.output_dir, tensorboard_log_dir=a.tensorboard_log_dir, loss_scale=a.loss_scale)
 
 
 if __name__ == '__main__':
