@@ -103,7 +103,13 @@ int cgvc_get_adam_step(cgvc_handle h, long long* t);
  * planes; with loss_scale != 0 the opt-in fused backward epilogues ("fuse_bwd") are not used, so with "fuse_bwd" = 1 modes 1 and 2 run
  * the unfused backward kernels and are not bit-identical to mode 0 (the unfused path is the default one).
  * Changing either option invalidates the captured step graphs.  With a communicator and "pipelined_comm", mode 2 makes every
- * network's Adam wait for the whole all-reduce and the scaler. */
+ * network's Adam wait for the whole all-reduce and the scaler.
+ * The window, measured on one H100 80GB HBM3 (700 W power limit; DESIGN.md section 10, tests/test_gpu_planes.py): an F16F8 GEMM stays
+ * within 4e-4 of float64 while an activation / gradient operand's RMS lies in 2^-14 .. 2^12 (full precision for 2^-6 .. 2^6 with no
+ * element above 256), a weight operand's from about 2^-13 up.  The batch-2 train step's gradients are within 1e-3 of float64 at every
+ * scale from 2^4 up whose planes did not saturate (2^2: 1.2e-3, 2^0: 1.9e-3; the first saturation at 2^14), so the static scale
+ * (2^10 at batch 2) lies 2^6 above the lower edge.  The scaler has no underflow signal: at batch 1 with lambda_cycle = 1e4 it settles
+ * on 2, where the worst gradient is 1.2e-3 from float64 -- not parity-grade. */
 typedef struct cgvc_loss_scale_info {
   float scale;                    /* the scale the next step's gradients are formed with (static: that of the last step's batch) */
   int good_steps;                 /* consecutive steps not skipped (dynamic) */
@@ -256,6 +262,32 @@ int cgvc_in_glu_backward(cgvc_handle h, const float* dy, const float* p, const f
                          const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
                          float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
                          int B, int R, int C, int shuffle, void* stream);
+/* The operand-plane writers of a train step, one call each, so that their planes and saturation counts can be checked against a
+ * host reference (tests/f16f8_ref.py).  precision CGVC_PREC_BF16X3 or CGVC_PREC_BF16: bf16 planes hi = bf16(x), lo = bf16(x - hi);
+ * CGVC_PREC_F16F8: hi = q16 = fp16(x), lo = q8hi followed by q8lo (e4m3 bytes, activation-role scales; kernels.cuh cgvc_quant4).
+ * sat: a device counter the call ADDS the saturated 4-value groups of F16F8 planes to (kernels.cuh cgvc_sat4), or NULL.
+ * cgvc_split_planes: x [rows, C] -> planes [rows, Cpad], Cpad = C rounded up to 64 (bf16) / 128 (F16F8), zero columns [C, Cpad):
+ *   the input and output-gradient splits of the generator. */
+int cgvc_split_planes(cgvc_handle h, int precision, const float* x, long long rows, int C, void* hi, void* lo,
+                      unsigned long long* sat, void* stream);
+/* cgvc_im2col_planes: the tap lowering of a stride-1 1-D TF-'SAME' convolution (option "edge_lower"): x [rows, C] holds rows / T
+ *   samples of T positions; planes [rows, Cpad], Cpad = kw * C rounded up to 128, column t * C + c of row m = x[m + dir * (t - (kw-1)/2), c]
+ *   when that row lies in the same sample, else 0.  dir = +1: the h1 input, -1: the o1 output gradient. */
+int cgvc_im2col_planes(cgvc_handle h, int precision, const float* x, long long rows, int T, int C, int kw, int dir, void* hi, void* lo,
+                       unsigned long long* sat, void* stream);
+/* cgvc_in_glu_forward / _backward with the planes of y [B, R, C] / of dp (layout of p) written by the same kernels:
+ *   precision CGVC_PREC_FP32_SIMT writes no planes (hi, lo, sat ignored: the two calls above);
+ *   gate 1: the gated form above; gate 0: the residual block's h2 form, p [B, R/shuffle, C*shuffle], y = IN(a) (+ resid [B, R, C] if
+ *   not NULL), beta_g / gamma_g / dbeta_g / dgamma_g unused. */
+int cgvc_in_glu_forward_planes(cgvc_handle h, const float* p, const float* beta_a, const float* gamma_a,
+                               const float* beta_g, const float* gamma_g, float* y, float* stats,
+                               int B, int R, int C, int shuffle, int precision, int gate, const float* resid,
+                               void* hi, void* lo, unsigned long long* sat, void* stream);
+int cgvc_in_glu_backward_planes(cgvc_handle h, const float* dy, const float* p, const float* stats,
+                                const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                                float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
+                                int B, int R, int C, int shuffle, int precision, int gate,
+                                void* hi, void* lo, unsigned long long* sat, void* stream);
 
 /* error codes */
 enum {

@@ -81,6 +81,10 @@ def _declare(lib):
         "cgvc_conv_backward": (ci, [vp, ci, vp, vp, vp, vp, vp, vp] + [ci] * 9 + [vp]),
         "cgvc_in_glu_forward": (ci, [vp] * 8 + [ci] * 4 + [vp]),
         "cgvc_in_glu_backward": (ci, [vp] * 13 + [ci] * 4 + [vp]),
+        "cgvc_split_planes": (ci, [vp, ci, vp, C.c_longlong, ci, vp, vp, vp, vp]),
+        "cgvc_im2col_planes": (ci, [vp, ci, vp, C.c_longlong, ci, ci, ci, ci, vp, vp, vp, vp]),
+        "cgvc_in_glu_forward_planes": (ci, [vp] * 8 + [ci] * 6 + [vp] * 5),
+        "cgvc_in_glu_backward_planes": (ci, [vp] * 13 + [ci] * 6 + [vp] * 4),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the library does not export a declared symbol

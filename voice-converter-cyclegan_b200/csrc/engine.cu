@@ -1717,31 +1717,86 @@ int cgvc_conv_backward(cgvc_handle e, int precision, const float* x, const float
   return 0;
 }
 
-int cgvc_in_glu_forward(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
-                        float* y, float* stats, int B, int R, int C, int shuffle, void* stream) {
+// ---- operand-plane writers (test entry points: exact planes and saturation counts against a host reference) --------------
+static int plane_precision(cgvc_engine* e, int precision, const void* hi, const void* lo) {
+  if (precision != CGVC_PREC_BF16X3 && precision != CGVC_PREC_BF16 && precision != CGVC_PREC_F16F8)
+    return fail(e, CGVC_ERR_ARG, "operand planes: precision %d has none", precision);
+  if (!hi || !lo) return fail(e, CGVC_ERR_ARG, "null argument");
+  return 0;
+}
+
+int cgvc_split_planes(cgvc_handle e, int precision, const float* x, long long rows, int C, void* hi, void* lo,
+                      unsigned long long* sat, void* stream) {
+  if (!e || !x) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(plane_precision(e, precision, hi, lo));
+  if (rows < 0 || C < 1) return fail(e, CGVC_ERR_ARG, "cgvc_split_planes: bad shape [%lld, %d]", rows, C);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(tc_split_planes(precision, x, rows, C, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, (cudaStream_t)stream, sat));
+  return 0;
+}
+
+int cgvc_im2col_planes(cgvc_handle e, int precision, const float* x, long long rows, int T, int C, int kw, int dir, void* hi, void* lo,
+                       unsigned long long* sat, void* stream) {
+  if (!e || !x) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(plane_precision(e, precision, hi, lo));
+  if (T < 1 || rows < 0 || rows % T || C < 4 || C % 4 || kw < 1 || kw > CGVC_MAX_TAPS || (dir != 1 && dir != -1))
+    return fail(e, CGVC_ERR_ARG, "cgvc_im2col_planes: bad shape (rows %lld, T %d, C %d, kw %d, dir %d)", rows, T, C, kw, dir);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_im2col_taps(x, rows, T, C, kw, dir, edge_cpad(kw * C), precision == CGVC_PREC_F16F8, hi, lo, (cudaStream_t)stream,
+                        nullptr, 0, sat));
+  return 0;
+}
+
+int cgvc_in_glu_forward_planes(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g,
+                               const float* gamma_g, float* y, float* stats, int B, int R, int C, int shuffle, int precision, int gate,
+                               const float* resid, void* hi, void* lo, unsigned long long* sat, void* stream) {
   if (!e || !p || !y || !stats) return fail(e, CGVC_ERR_ARG, "null argument");
   if (C % 32 != 0 || shuffle < 1 || R % shuffle != 0) return fail(e, CGVC_ERR_UNSUPPORTED, "C must be a multiple of 32 and R of shuffle");
+  if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   PostParams q; memset(&q, 0, sizeof q);
-  q.p = p; q.ldp = 2 * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
-  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = 1; q.y = y; q.stats = stats;
+  q.p = p; q.ldp = (gate ? 2 : 1) * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
+  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = gate != 0; q.resid = resid;
+  q.y = y; q.stats = stats;
+  if (precision != CGVC_PREC_FP32_SIMT) {
+    q.y_hi = (__nv_bfloat16*)hi; q.y_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
+  }
   CK(launch_post_fwd(q, (cudaStream_t)stream));
   return 0;
+}
+
+int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, const float* stats,
+                                const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                                float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
+                                int B, int R, int C, int shuffle, int precision, int gate, void* hi, void* lo, unsigned long long* sat,
+                                void* stream) {
+  if (!e || !dy || !p || !stats || !dp) return fail(e, CGVC_ERR_ARG, "null argument");
+  if (C % 32 != 0 || shuffle < 1 || R % shuffle != 0) return fail(e, CGVC_ERR_UNSUPPORTED, "C must be a multiple of 32 and R of shuffle");
+  if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  PostBwdParams q; memset(&q, 0, sizeof q);
+  q.dy1 = dy; q.p = p; q.ldp = (gate ? 2 : 1) * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
+  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = gate != 0; q.stats = stats;
+  q.dp = dp; q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = dbeta_g; q.dgamma_g = dgamma_g;
+  if (precision != CGVC_PREC_FP32_SIMT) {
+    q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
+  }
+  CK(launch_post_bwd(q, (cudaStream_t)stream));
+  return 0;
+}
+
+int cgvc_in_glu_forward(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                        float* y, float* stats, int B, int R, int C, int shuffle, void* stream) {
+  return cgvc_in_glu_forward_planes(e, p, beta_a, gamma_a, beta_g, gamma_g, y, stats, B, R, C, shuffle, CGVC_PREC_FP32_SIMT, 1, nullptr,
+                                    nullptr, nullptr, nullptr, stream);
 }
 
 int cgvc_in_glu_backward(cgvc_handle e, const float* dy, const float* p, const float* stats,
                          const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
                          float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
                          int B, int R, int C, int shuffle, void* stream) {
-  if (!e || !dy || !p || !stats || !dp) return fail(e, CGVC_ERR_ARG, "null argument");
-  if (C % 32 != 0 || shuffle < 1 || R % shuffle != 0) return fail(e, CGVC_ERR_UNSUPPORTED, "C must be a multiple of 32 and R of shuffle");
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  PostBwdParams q; memset(&q, 0, sizeof q);
-  q.dy1 = dy; q.p = p; q.ldp = 2 * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
-  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = 1; q.stats = stats;
-  q.dp = dp; q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = dbeta_g; q.dgamma_g = dgamma_g;
-  CK(launch_post_bwd(q, (cudaStream_t)stream));
-  return 0;
+  return cgvc_in_glu_backward_planes(e, dy, p, stats, beta_a, gamma_a, beta_g, gamma_g, dp, dbeta_a, dgamma_a, dbeta_g, dgamma_g,
+                                     B, R, C, shuffle, CGVC_PREC_FP32_SIMT, 1, nullptr, nullptr, nullptr, stream);
 }
 
 }  // extern "C"
