@@ -231,6 +231,14 @@ int cgvc_kernel_launches(unsigned long long* count);
  * form of the one-pass GLU / instance-norm backward: persistent CTAs walk (sample, channel block) items through a cp.async double buffer
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
  * "loss_scale" (default 0) and "loss_scale_growth_interval" (default 2000): see cgvc_loss_scale_state.
+ * "deterministic" (default 0): 1 makes cgvc_train_step and cgvc_compute_gradients bitwise reproducible on one GPU.  The same inputs,
+ * PARAM, ADAM_M / ADAM_V, Adam step, loss-scaler state, batch, frames, precision and options give the same bits of PARAM, GRAD, ADAM_M,
+ * ADAM_V, the 8 losses, gen_A / gen_B and the scaler state, in every precision and loss_scale mode, on repeated calls and fresh
+ * engines, and whatever "two_streams" and "cuda_graph" are.  Every kernel that adds into GRAD or a loss slot from many CTAs then stores
+ * per-CTA partials to a slab in WORK and a second kernel adds them in a fixed order, one add per element (DESIGN.md section 11).
+ * "fuse_bwd" and "side_wgrad" are ignored while it is on.  It enlarges WORK (cgvc_arena_bytes): bind the larger arena after setting
+ * it, or the calls return CGVC_ERR_UNBOUND; cgvc_conv_backward and cgvc_in_glu_backward(_planes) honour it too and then need WORK
+ * bound.  With a communicator attached each rank's gradients are deterministic; the NCCL all-reduce that sums them is not covered.
  * "debug_taps" (default 0): see cgvc_debug_activation.
  * "tc_debug" (default 0): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
  * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather.  The plain

@@ -139,6 +139,8 @@ struct cgvc_engine {
   int edge_lower = 1;           // the generator's 15-tap, 24-channel edge layers as dense 1 x 1 GEMMs (taps moved into the channel / column dimension)
   int two_streams = 1;          // 0: both lanes are enqueued on the caller's stream (clean per-kernel timing for profiling)
   int side_wgrad = 0;           // weight-gradient GEMMs on a side stream per lane (see SideQ); needs two_streams, excludes fuse_bwd.  Off by default
+  int deterministic = 0;        // bit-reproducible steps: fixed-order reductions into GRAD and the loss slots (DESIGN.md section 11);
+                                // ignores fuse_bwd and side_wgrad
   SideQ sideq[2];
   // loss scaling (option "loss_scale"): 0 static, 1 monitor (static scale, counters collected), 2 dynamic.  ls: the device state;
   // d_scalars[16 + l] holds the static scale of batches [2^l, 2^(l+1)) (loss_scale), so that the loss kernels always read a pointer
@@ -303,10 +305,10 @@ static int conv_dgrad_simt(cgvc_engine* e, const float* Pm, const ConvW& c, int 
 
 // dW += x^T * dy (forward geometry); the bias gradient comes from the IN/GLU backward kernel (or launch_colsum for o1)
 static int conv_wgrad_simt(cgvc_engine* e, float* Gm, const ConvW& c, int sh, int sw, const ConvIO& io,
-                           const float* dy, int ld, int coff, cudaStream_t st) {
+                           const float* dy, int ld, int coff, cudaStream_t st, const DetSlab* det) {
   if (!io.x || !dy) return fail(e, CGVC_ERR_UNSUPPORTED, "fp32 tensors were not kept for a layer that fell back to the SIMT path");
   GatherGeom g = fwd_geom(io.n, io.H, io.W, c.kh, c.kw, sh, sw);
-  CK(launch_wgrad_simt(g, io.x, c.cin, 0, c.cin, dy, ld, coff, c.cout, Gm + c.k, (long long)c.cin * c.cout, c.cout, 1, st));
+  CK(launch_wgrad_simt(g, io.x, c.cin, 0, c.cin, dy, ld, coff, c.cout, Gm + c.k, (long long)c.cin * c.cout, c.cout, 1, st, det != nullptr));
   return 0;
 }
 
@@ -378,15 +380,16 @@ static int conv_dgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const fl
   return 0;
 }
 
-static int conv_wgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const float* dP, PlanePair dp, cudaStream_t st) {
+// det: deterministic mode (the lane's partials slab), else null
+static int conv_wgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const float* dP, PlanePair dp, cudaStream_t st, const DetSlab* det) {
   float* Gm = e->G();
   bool done = false;
   if (use_tc(e, L.tc_slot) && dp.hi && io.xhi)
     RET(tc_result(e, tc_conv_wgrad(e->tcw, L.tc_slot, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw,
-                                   Gm + L.a.k, L.gated() ? Gm + L.g.k : nullptr, st), &L.a, "weight gradient", &done));
+                                   Gm + L.a.k, L.gated() ? Gm + L.g.k : nullptr, st, det), &L.a, "weight gradient", &done));
   if (done) return 0;
-  RET(conv_wgrad_simt(e, Gm, L.a, L.sh, L.sw, io, dP, L.width(), 0, st));
-  if (L.gated()) RET(conv_wgrad_simt(e, Gm, L.g, L.sh, L.sw, io, dP, L.width(), L.a.cout, st));
+  RET(conv_wgrad_simt(e, Gm, L.a, L.sh, L.sw, io, dP, L.width(), 0, st, det));
+  if (L.gated()) RET(conv_wgrad_simt(e, Gm, L.g, L.sh, L.sw, io, dP, L.width(), L.a.cout, st, det));
   return 0;
 }
 
@@ -557,9 +560,11 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
 struct BwdScratch { float *bufA, *bufB, *dP; __nv_bfloat16 *dPhi, *dPlo; float* post;
                     __nv_bfloat16 *dP2hi, *dP2lo;      // second plane pair: a fused dgrad epilogue writes the next layer's dP while reading this one's
                     __nv_bfloat16 *dPbhi, *dPblo;      // ping-pong partner of dPhi / dPlo (same size) for the side-stream weight gradients
-                    SideQ* sq; };
+                    SideQ* sq;
+                    DetSlab det; };                    // deterministic mode: the lane's partials slab (det.p null otherwise)
 
 static bool side_on(const BwdScratch& S) { return S.sq && S.sq->on && S.dPbhi; }
+static const DetSlab* det_of(const BwdScratch& S) { return S.det.p ? &S.det : nullptr; }
 
 // The dP planes of one backward walk.  Fused backward (tensor-core path, fuse_bwd): a stride-1 data-gradient launch whose result is
 // d loss / d (output of an instance-normed layer) runs that layer's instance-norm (+GLU) backward in its epilogue and writes the
@@ -630,6 +635,7 @@ static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const
   if (tc) { q.dp_hi = out.hi; q.dp_lo = out.lo; }
   q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
   q.sat = sat_grad(e);
+  if (wgrad) q.det = S.det;                 // passes without parameter gradients keep the faster (equally deterministic) forms
   return q;
 }
 
@@ -665,7 +671,7 @@ static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAc
   PostBwdParams q;
   RET(layer_dp(e, w, L, A, dy, in.n, rows_per_sample_out, wgrad, st, q));
   const PlanePair dp{q.dp_hi, q.dp_lo};
-  if (wgrad) RET(run_wgrad(w.S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, L, in, q.dp, dp, ws); }));
+  if (wgrad) RET(run_wgrad(w.S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, L, in, q.dp, dp, ws, det_of(w.S)); }));
   if (!dx) return 0;
   const int other = 1 - w.cur;
   TcBwdFuse f;
@@ -688,10 +694,11 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   };
   auto of = [&](const GLAct& a, int W) { return at(a.Y, a.Yhi, a.Ylo, W); };
   // the fused backward epilogues do not count saturation: a step whose planes are counted takes the separate kernels
-  BwdWalk w(S, e->fuse_bwd && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi && A.r[0].h2.Yhi);
+  BwdWalk w(S, e->fuse_bwd && !e->deterministic && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi &&
+               A.r[0].h2.Yhi);
   const bool edge = edge_on(e, N) && A.xchi && A.z;
   // o1 (no norm, no gate): bias gradient = column sums of d_out
-  CK(launch_colsum(d_out_cl, (long long)n * T, nf, 0, nf, Gm + N.o1.a.b, st));
+  CK(launch_colsum(d_out_cl, (long long)n * T, nf, 0, nf, Gm + N.o1.a.b, st, det_of(S)));
   const ConvIO u2 = of(A.u[1], T);
   if (edge && u2.xhi && S.dPhi) {
     // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
@@ -699,7 +706,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
     CK(launch_im2col_taps(d_out_cl, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
                           dp.hi, dp.lo, st, nullptr, 0, sat_grad(e)));
     RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-      return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, u2.xhi, u2.xlo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws),
+      return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, u2.xhi, u2.xlo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws, det_of(S)),
                        &N.o1.a, "weight gradient (tap-lowered)"); }));
     RET(tc_result(e, tc_conv_dgrad(e->tcw, N.o1f_slot, dp.hi, dp.lo, n, 1, T, 1, 1, S.bufA, 0, st), &N.o1.a, "data gradient (tap-lowered)"));
   } else {
@@ -708,7 +715,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
       dp = dp_planes(w, st);
       CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st, sat_grad(e)));
     }
-    RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, u2, d_out_cl, dp, ws); }));
+    RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, u2, d_out_cl, dp, ws, det_of(S)); }));
     RET(conv_dgrad(e, N.o1, u2, d_out_cl, dp, S.bufA, 0, st));
   }
   float* cur = S.bufA; float* oth = S.bufB;
@@ -740,7 +747,8 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   PostBwdParams q;
   RET(layer_dp(e, w, N.h1, A.h1, cur, n, T, true, st, q));
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-    return tc_result(e, tc_conv_wgrad(e->tcw, N.h1c_slot, A.xchi, A.xclo, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, Gm + N.h1.a.k, Gm + N.h1.g.k, ws),
+    return tc_result(e, tc_conv_wgrad(e->tcw, N.h1c_slot, A.xchi, A.xclo, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, Gm + N.h1.a.k, Gm + N.h1.g.k, ws,
+                                      det_of(S)),
                      &N.h1.a, "weight gradient (tap-lowered)"); }));
   if (d_in_cl) {
     RET(tc_result(e, tc_conv_dgrad(e->tcw, N.h1c_slot, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, oth, 0, st), &N.h1.a, "data gradient (tap-lowered)"));
@@ -835,7 +843,8 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   if (e->fuse_c1 && N.h1.a.cout == 128 && N.h1.a.kh * N.h1.a.kw <= 9 && !N.h1.has_in) {
     if (wgrad) {
       GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
-      CK(launch_glu_bwd_wgrad_c1(g, A.x, dy, A.h1.P, 128, e->G() + N.h1.a.k, e->G() + N.h1.g.k, e->G() + N.h1.a.b, e->G() + N.h1.g.b, st));
+      CK(launch_glu_bwd_wgrad_c1(g, A.x, dy, A.h1.P, 128, e->G() + N.h1.a.k, e->G() + N.h1.g.k, e->G() + N.h1.a.b, e->G() + N.h1.g.b, st,
+                                 det_of(S)));
     }
     if (d_in) CK(launch_glu_bwd_dgrad_c1(dy, A.h1.P, 128, e->P() + N.h1.a.k, e->P() + N.h1.g.k, bufs[flip], d_in, n, H0, T, 3, 3, N.h1.sh, N.h1.sw, st));
     return 0;
@@ -844,7 +853,7 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   CK(launch_post_bwd(q, st));
   if (wgrad) {
     GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
-    CK(launch_wgrad_c1(g, A.x, S.dP, 256, 256, e->G() + N.h1.a.k, e->G() + N.h1.g.k, 128, nullptr, nullptr, st));
+    CK(launch_wgrad_c1(g, A.x, S.dP, 256, 256, e->G() + N.h1.a.k, e->G() + N.h1.g.k, 128, nullptr, nullptr, st, det_of(S)));
   }
   if (d_in) CK(launch_dgrad_c1(S.dP, 256, e->P() + N.h1.a.k, e->P() + N.h1.g.k, 128, bufs[flip], d_in, n, H0, T, 3, 3, N.h1.sh, N.h1.sw, st));
   return 0;
@@ -891,6 +900,13 @@ static void plan_train(cgvc_engine* e, Bump& ws, TrainPlan& P, int B, int T) {
     L.S.dPbhi = L.S.dPblo = nullptr;
     if (pl) { L.S.dPbhi = ws.take<__nv_bfloat16>(dp); L.S.dPblo = ws.take<__nv_bfloat16>(dp); }
     L.S.sq = &e->sideq[l];
+    L.S.det = DetSlab{nullptr, 0};
+    if (e->deterministic) {
+      // the weight-gradient partials are capped by CGVC_DET_SLAB_FLOATS (launch_tn lowers the split); the GLU / instance-norm bias partials,
+      // one row of 2 x (conv columns) per 32 positions of a sample, grow with the batch and stay below dp / 8
+      const long long slab = CGVC_DET_SLAB_FLOATS > (long long)(dp / 8) ? CGVC_DET_SLAB_FLOATS : (long long)(dp / 8);
+      L.S.det = DetSlab{ws.take<float>((size_t)slab), slab};
+    }
     L.S.post = ws.take<float>(n2 * 4 * 1024);
     plan_generator(e, ws, L.gfirst, 2 * B, T); plan_generator(e, ws, L.gcyc, B, T);
     plan_discriminator(e, ws, L.d, 2 * B, T);
@@ -909,7 +925,24 @@ static size_t work_bytes_needed(cgvc_engine* e) {
   plan_generator(e, ws, F.g, e->cfg.max_batch, e->cfg.max_frames);
   plan_discriminator(e, ws, F.d, e->cfg.max_batch, e->cfg.max_frames);
   if (ws.off > need) need = ws.off;
+  if (e->deterministic) {                     // the per-kernel entry points' slab (plan_entry_det)
+    ws.reset(nullptr, 0); ws.take<float>((size_t)CGVC_DET_SLAB_FLOATS);
+    if (ws.off > need) need = ws.off;
+  }
   return need + 4096;
+}
+
+// Deterministic mode in a per-kernel entry point: the partials slab at the start of WORK, which work_bytes_needed reserves.  *det stays
+// null outside deterministic mode; CGVC_ERR_UNBOUND when WORK is missing or too small
+static int plan_entry_det(cgvc_engine* e, DetSlab* slab, const DetSlab** det) {
+  *det = nullptr;
+  if (!e->deterministic) return 0;
+  if (!e->arena[CGVC_ARENA_WORK]) return fail(e, CGVC_ERR_UNBOUND, "deterministic mode needs the WORK arena bound");
+  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
+  *slab = DetSlab{ws.take<float>((size_t)CGVC_DET_SLAB_FLOATS), CGVC_DET_SLAB_FLOATS};
+  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small for the deterministic partials slab");
+  *det = slab;
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1232,20 +1265,21 @@ static int run_lane(cgvc_engine* e, LanePlan& L, int lane, const float* Yreal_de
   RET(discriminator_forward(e, DN, L.d, L.din, st, false));
   // ---- losses and their gradients (model.py:57-90) ----
   const float* ls = loss_scale_dev(e, B);                       // scales every gradient of the step (not the loss values); Adam divides it out
-  CK(launch_l1_loss_grad(L.gcyc.out_cl, X_cl, (long long)img, Ls + 0, sc + 0, L.d_cyc, 0, st, ls));          // cycle term
-  CK(launch_l1_loss_grad(idY_cl, Y_cl, (long long)img, Ls + 1, sc + 1, L.d_out + img, 0, st, ls));           // identity term
+  const DetSlab* det = det_of(L.S);
+  CK(launch_l1_loss_grad(L.gcyc.out_cl, X_cl, (long long)img, Ls + 0, sc + 0, L.d_cyc, 0, st, ls, det));     // cycle term
+  CK(launch_l1_loss_grad(idY_cl, Y_cl, (long long)img, Ls + 1, sc + 1, L.d_out + img, 0, st, ls, det));      // identity term
   const long long hrows = (long long)B * (nf / 4) * (T / 16);   // head rows per half
   const float* Y3 = L.d.d[2].Y;
   float* Dslot = Ls + (lane == 0 ? 6 : 5);                      // discriminator_loss_B / _A
   float* Gslot = Ls + (lane == 0 ? 2 : 3);                      // generator_loss_A2B / _B2A
   // discriminator loss: real half -> target 1, fake half -> target 0, each weighted 1/2 (model.py:81-88)
-  CK(launch_head_loss_bwd(L.d.prob, Y3, hrows, 1024, Pm + DN.dense_k, 1.f, 0.5f, Dslot, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, ls));
+  CK(launch_head_loss_bwd(L.d.prob, Y3, hrows, 1024, Pm + DN.dense_k, 1.f, 0.5f, Dslot, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, ls, det));
   CK(launch_head_loss_bwd(L.d.prob + hrows, Y3 + hrows * 1024, hrows, 1024, Pm + DN.dense_k, 0.f, 0.5f, Dslot,
-                          L.dY3 + hrows * 1024, Gm + DN.dense_k, Gm + DN.dense_b, st, ls));
+                          L.dY3 + hrows * 1024, Gm + DN.dense_k, Gm + DN.dense_b, st, ls, det));
   RET(discriminator_backward(e, DN, L.d, L.dY3, true, nullptr, L.S, st));
   // generator adversarial loss on the fake half: target 1 (model.py:68-69); the gradient flows to the fake only
   DiscActs V = disc_view(e, L.d, B, B);
-  CK(launch_head_loss_bwd(V.prob, V.d[2].Y, hrows, 1024, Pm + DN.dense_k, 1.f, 1.f, Gslot, L.dY3, nullptr, nullptr, st, ls));
+  CK(launch_head_loss_bwd(V.prob, V.d[2].Y, hrows, 1024, Pm + DN.dense_k, 1.f, 1.f, Gslot, L.dY3, nullptr, nullptr, st, ls, det));
   RET(discriminator_backward(e, DN, V, L.dY3, false, L.d_adv, L.S, st));
   // ---- generator backward ----
   // cycle pass: G_{Y->X}(gen_Y) <- d cycle_X ; its input gradient is the first half of the first pass's upstream
@@ -1290,7 +1324,7 @@ static int forward_backward(cgvc_engine* e, const float* A_dev, const float* B_d
   CK(cudaMemcpyAsync(P.lane[1].in + img, P.lane[0].in, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
   for (int l = 0; l < 2; ++l) {
     SideQ& q = e->sideq[l];
-    q.on = e->side_wgrad && e->two_streams && !e->fuse_bwd && !tc_profile_is_on() && q.side != nullptr;
+    q.on = e->side_wgrad && e->two_streams && !e->fuse_bwd && !e->deterministic && !tc_profile_is_on() && q.side != nullptr;
     q.used[0] = q.used[1] = false; q.cur = 0;
   }
   if (e->two_streams) {
@@ -1407,11 +1441,24 @@ static int run_captured(cgvc_engine* e, const GraphKey& key, cudaStream_t user, 
   return 0;
 }
 
+// The step's WORK plan fits the bound arena (checked before anything is enqueued: a call refused for a short WORK -- e.g. after
+// "deterministic" was switched on without re-binding -- launches nothing)
+static int check_work_train(cgvc_engine* e, int batch, int frames) {
+  RET(check_bt(e, batch, frames, 16));
+  if (!e->cfg.train) return fail(e, CGVC_ERR_ARG, "engine was created with train = 0");
+  RET(need_arenas(e, true));
+  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
+  TrainPlan P; plan_train(e, ws, P, batch, frames);
+  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small for batch %d x %d frames", batch, frames);
+  return 0;
+}
+
 extern "C" {
 
 int cgvc_compute_gradients(cgvc_handle e, const float* A_dev, const float* B_dev, int batch, int frames,
                            float lambda_cycle, float lambda_identity, float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream) {
   if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(check_work_train(e, batch, frames));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   RET(set_lambdas(e, lambda_cycle, lambda_identity, (cudaStream_t)stream));
   RET(ls_prepare(e, batch, (cudaStream_t)stream));
@@ -1442,7 +1489,7 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
                     float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream) {
   if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
   for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
-  RET(check_bt(e, batch, frames, 16));
+  RET(check_work_train(e, batch, frames));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const float gscale = (e->comm ? 1.f / (float)e->nranks : 1.f) / loss_scale(e, batch);
@@ -1463,7 +1510,8 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
     CK(cudaMemcpyAsync(sA, A_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CK(cudaMemcpyAsync(sB, B_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
     GraphKey key; memset(&key, 0, sizeof key);
-    key.batch = batch; key.frames = frames; key.id_off = lambda_identity == 0.f; key.lanes = e->two_streams; key.fuse = e->fuse_in | (e->fuse_bwd << 1) | (e->side_wgrad << 2) | (e->fuse_c1 << 3) | (e->edge_lower << 4); key.kind = 0;
+    key.batch = batch; key.frames = frames; key.id_off = lambda_identity == 0.f; key.lanes = e->two_streams; key.fuse = e->fuse_in | (e->fuse_bwd << 1) | (e->side_wgrad << 2) | (e->fuse_c1 << 3) | (e->edge_lower << 4) |
+               (e->deterministic << 5); key.kind = 0;
     RET(run_captured(e, key, st, [&](cudaStream_t s) {
       return forward_backward(e, sA, sB, batch, frames, lambda_cycle, lambda_identity, nullptr, nullptr, nullptr, s);
     }));
@@ -1599,6 +1647,14 @@ int cgvc_set_option(cgvc_handle e, const char* name, int value) {
   if (!strcmp(name, "fuse_bwd")) { e->fuse_bwd = value != 0; return 0; }
   if (!strcmp(name, "edge_lower")) { e->edge_lower = value != 0; return 0; }
   if (!strcmp(name, "side_wgrad")) { e->side_wgrad = value != 0; return 0; }
+  if (!strcmp(name, "deterministic")) {
+    // changes the WORK plan (cgvc_arena_bytes): the caller re-binds a larger arena after switching it on.  The captured steps hold
+    // the slab addresses of the old plan (GraphKey carries the mode as well)
+    e->deterministic = value != 0;
+    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
+    e->graphs.clear();
+    return 0;
+  }
   if (!strcmp(name, "pipelined_comm")) { e->pipelined_comm = value != 0; return 0; }
   if (!strcmp(name, "fuse_c1")) { e->fuse_c1 = value != 0; return 0; }
   if (!strcmp(name, "debug_taps")) { e->debug_taps = value != 0; return 0; }
@@ -1702,17 +1758,19 @@ int cgvc_conv_backward(cgvc_handle e, int precision, const float* x, const float
                        float* dx, float* dw, float* dbias, int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, void* stream) {
   if (!e || !x || !w || !dy) return fail(e, CGVC_ERR_ARG, "null argument");
   if (kh * kw > CGVC_MAX_TAPS) return fail(e, CGVC_ERR_UNSUPPORTED, "at most %d filter taps", CGVC_MAX_TAPS);
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   if (precision != CGVC_PREC_FP32_SIMT)
-    return tc_result(e, tc_conv_bwd_adhoc(precision, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16 ? 1 : 0),
+    return tc_result(e, tc_conv_bwd_adhoc(precision, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16 ? 1 : 0, det),
                      nullptr, "conv backward");
   ConvW c; c.k = 0; c.b = 0; c.kh = kh; c.kw = kw; c.cin = Cin; c.cout = Cout;
   if (dx) RET(conv_dgrad_simt(e, w, c, sh, sw, B, H, W, dy, Cout, 0, dx, 0, st));
   if (dw) {
     GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
-    CK(launch_wgrad_simt(g, x, Cin, 0, Cin, dy, Cout, 0, Cout, dw, (long long)Cin * Cout, Cout, 1, st));
-    if (dbias) CK(launch_colsum(dy, (long long)g.B * g.Hy * g.Wx, Cout, 0, Cout, dbias, st));
+    CK(launch_wgrad_simt(g, x, Cin, 0, Cin, dy, Cout, 0, Cout, dw, (long long)Cin * Cout, Cout, 1, st, det != nullptr));
+    if (dbias) CK(launch_colsum(dy, (long long)g.B * g.Hy * g.Wx, Cout, 0, Cout, dbias, st, det));
   }
   return 0;
 }
@@ -1773,8 +1831,11 @@ int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, 
   if (!e || !dy || !p || !stats || !dp) return fail(e, CGVC_ERR_ARG, "null argument");
   if (C % 32 != 0 || shuffle < 1 || R % shuffle != 0) return fail(e, CGVC_ERR_UNSUPPORTED, "C must be a multiple of 32 and R of shuffle");
   if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   PostBwdParams q; memset(&q, 0, sizeof q);
+  if (det) q.det = *det;
   q.dy1 = dy; q.p = p; q.ldp = (gate ? 2 : 1) * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
   q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = gate != 0; q.stats = stats;
   q.dp = dp; q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = dbeta_g; q.dgamma_g = dgamma_g;

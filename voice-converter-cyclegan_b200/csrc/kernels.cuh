@@ -88,6 +88,16 @@ extern unsigned long long g_cgvc_launches;   // incremented by every kernel laun
 
 #define CGVC_MAX_TAPS 18   // largest filter on the path: discriminator d3, 6x3 (module.py:208)
 
+// ---- deterministic mode (engine option "deterministic"; DESIGN.md section 11).  A writer that would add into GRAD or a loss slot from
+// many CTAs at once instead stores each CTA's contribution as one row of a partials slab with plain stores; launch_reduce_parts then
+// sums the rows in index order and makes one add per element.  The slab is carved from the WORK arena, CGVC_DET_SLAB_FLOATS floats
+// per lane; every launcher checks on the host that its rows fit and returns an error, never launches, when they do not.
+#define CGVC_DET_SLAB_FLOATS (8ll << 20)
+struct DetSlab { float* p; long long cap; };          // cap: floats; p == null: the default atomic accumulation
+// up to four destinations of one partial row: dst[i][j] += sum_k part[k * row + off[i] + j], j < len[i] (null dst: skipped)
+struct DetSegs { float* dst[4]; long long off[4]; long long len[4]; };
+cudaError_t launch_reduce_parts(const float* part, long long nparts, long long row, const DetSegs& s, cudaStream_t st);
+
 // Geometry of a "gather-GEMM":  D[m, n] = sum_t sum_c  S[src(m,t), c] * Wt[t][c][n]
 //   m enumerates a logical output grid (b, y, x); src(m,t) = (b, y*sy + oy[t], x*sx + ox[t]) in the source
 //   tensor [B,Hs,Ws,*] (zero outside), and row m is written to (b, y*dsy + doy, x*dsx + dox) of the
@@ -137,9 +147,10 @@ cudaError_t launch_gg_simt_packed(const GatherGeom& g, const GemmOperands& op, c
 // weight gradient in forward geometry: dW[widx[t]][c][n] += sum_m S[src(m,t), c] * G[m, n]   (atomic accumulate)
 cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, int s_coff, int C,
                               const float* grad, int g_ld, int g_coff, int N,
-                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st);
+                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det = 0);
 // db[n] += sum_m G[m, g_coff + n]
-cudaError_t launch_colsum(const float* grad, long long rows, int g_ld, int g_coff, int N, float* db, cudaStream_t st);
+cudaError_t launch_colsum(const float* grad, long long rows, int g_ld, int g_coff, int N, float* db, cudaStream_t st,
+                          const DetSlab* det = nullptr);
 
 // ---- instance-norm / GLU / residual "post" kernels (module.py:3-20, 66-146)
 struct PostParams {
@@ -174,6 +185,7 @@ struct PostBwdParams {
   int qmode;                            // 1: dp_hi / dp_lo are F16F8 planes (q16; q8hi followed by q8lo) with the activation-role scales
   float* scratch;                       // [B,4,C] fp32 workspace (null: internal buffer, single-stream use only)
   unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
+  DetSlab det;                          // deterministic mode (det.p != null): the sums + apply form, parameter and bias gradients reduced in order
 };
 cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st);
 void post_set_stream(int on);      // 1 (default): gated layers without shuffle and 32 / 48 / 64 positions per sample take the streaming (cp.async double-buffered) form of it
@@ -186,11 +198,13 @@ cudaError_t launch_head_fwd(const float* y, long long rows, int C, const float* 
 // dy[row,:] = dz * w (if dy);  dw += sum dz*y[row,:], db += sum dz (if dw)
 cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long rows, int C, const float* w,
                                  float target, float coef, float* loss_slot,
-                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev = nullptr);
+                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev = nullptr,
+                                 const DetSlab* det = nullptr);
 
 // ---- L1 loss + gradient (utils.py:6-8): loss_slot += mean|yhat - y|; d[i] = gscale * sign(yhat - y)/n  (accumulate optional)
 cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, float* loss_slot,
-                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, const float* grad_mult_dev = nullptr);
+                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, const float* grad_mult_dev = nullptr,
+                                const DetSlab* det = nullptr);
 // grad_mult_dev (both loss kernels, null: 1): the gradients -- not the loss values -- are multiplied by *grad_mult_dev, the loss scale of the
 // F16F8 gradient planes; a device pointer, so that a captured step follows the dynamic scale
 // x *= a, or with div_dev x *= a / *div_dev
@@ -215,7 +229,7 @@ cudaError_t launch_split_bf16(const float* x, __nv_bfloat16* hi, __nv_bfloat16* 
 // ---- single-input-channel specials (discriminator h1, K = 9, HBM-bound)
 // dW[t][0][n] += sum_m x[src(m,t)] * G[m,n]; columns [0,n_split) -> dw_a, the rest -> dw_g; db = column sums (optional)
 cudaError_t launch_wgrad_c1(const GatherGeom& g, const float* src, const float* grad, int g_ld, int N,
-                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st);
+                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det = nullptr);
 // dx[B,H,W] = conv-transpose of G [rows, C] with w = [wa | wg] ([taps][c_split], [taps][C - c_split]); Z is scratch [rows, taps]
 cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float* wg, int c_split, float* Z, float* dx,
                             int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st);
@@ -260,6 +274,6 @@ cudaError_t launch_gather_minibatch(const float* cA, const long long* off_A, con
 // formed in registers and consumed in place -- weight + bias gradients, or the data gradient (Z scratch [rows, taps]) -- instead of
 // being written to HBM and read back.  C = channels per branch (128).
 cudaError_t launch_glu_bwd_wgrad_c1(const GatherGeom& g, const float* src, const float* dy, const float* P, int C,
-                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st);
+                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det = nullptr);
 cudaError_t launch_glu_bwd_dgrad_c1(const float* dy, const float* P, int C, const float* wa, const float* wg, float* Z, float* dx,
                                     int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st);

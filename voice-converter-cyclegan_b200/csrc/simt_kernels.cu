@@ -313,12 +313,12 @@ wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict_
 
 cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, int s_coff, int C,
                               const float* grad, int g_ld, int g_coff, int N,
-                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st) {
+                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   ++g_cgvc_launches;
   int tiles = ((N + 63) / 64) * ((C + 63) / 64) * g.ntaps;
-  int ksplit = (592 + tiles - 1) / tiles;
+  int ksplit = det ? 1 : (592 + tiles - 1) / tiles;       // det: one CTA, one thread and one add per element
   long long maxsplit = (M + 63) / 64;
   if (ksplit > maxsplit) ksplit = (int)maxsplit;
   if (ksplit < 1) ksplit = 1;
@@ -333,7 +333,8 @@ cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, i
 
 // db[n] += sum over rows
 __global__ void __launch_bounds__(256)
-colsum_kernel(const float* __restrict__ grad, long long rows, int g_ld, int g_coff, int N, float* __restrict__ db, int rows_per_block) {
+colsum_kernel(const float* __restrict__ grad, long long rows, int g_ld, int g_coff, int N, float* __restrict__ db, int rows_per_block,
+              float* __restrict__ part) {
   __shared__ float red[8][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x * 32 + lane;
@@ -348,15 +349,45 @@ colsum_kernel(const float* __restrict__ grad, long long rows, int g_ld, int g_co
     float tsum = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) tsum += red[w][lane];
-    atomicAdd(db + n, tsum);
+    if (part) part[(long long)blockIdx.y * N + n] = tsum;
+    else atomicAdd(db + n, tsum);
   }
 }
 
-cudaError_t launch_colsum(const float* grad, long long rows, int g_ld, int g_coff, int N, float* db, cudaStream_t st) {
+cudaError_t launch_colsum(const float* grad, long long rows, int g_ld, int g_coff, int N, float* db, cudaStream_t st, const DetSlab* det) {
   if (rows == 0) return cudaSuccess;
   int rpb = 2048;
   dim3 grid((N + 31) / 32, (unsigned)((rows + rpb - 1) / rpb));
-  ++g_cgvc_launches; colsum_kernel<<<grid, 256, 0, st>>>(grad, rows, g_ld, g_coff, N, db, rpb);
+  float* part = det ? det->p : nullptr;
+  if (part && (long long)grid.y * N > det->cap) return cudaErrorInvalidValue;
+  ++g_cgvc_launches; colsum_kernel<<<grid, 256, 0, st>>>(grad, rows, g_ld, g_coff, N, db, rpb, part);
+  if (!part) return cudaGetLastError();
+  return launch_reduce_parts(part, grid.y, N, DetSegs{{db}, {0}, {N}}, st);
+}
+
+// deterministic mode: dst[i][j] += the rows' values summed in row order, one atomic add per element (the other lane may add into the
+// same GRAD element concurrently; with one add per lane the result does not depend on which comes first)
+__global__ void __launch_bounds__(256)
+reduce_parts_kernel(const float* __restrict__ part, long long nparts, long long row, const DetSegs s, long long total) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= total) return;
+  int k = 0; long long j = i;
+  while (j >= s.len[k]) { j -= s.len[k]; ++k; }
+  if (!s.dst[k]) return;
+  const float* p = part + s.off[k] + j;
+  float acc = p[0];
+  for (long long r = 1; r < nparts; ++r) acc += p[r * row];
+  atomicAdd(s.dst[k] + j, acc);
+}
+
+cudaError_t launch_reduce_parts(const float* part, long long nparts, long long row, const DetSegs& s, cudaStream_t st) {
+  long long total = 0;
+  for (int k = 0; k < 4; ++k) {
+    if (s.len[k] < 0 || (s.len[k] && s.off[k] + s.len[k] > row)) return cudaErrorInvalidValue;
+    total += s.len[k];
+  }
+  if (total == 0 || nparts < 1) return cudaSuccess;
+  ++g_cgvc_launches; reduce_parts_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(part, nparts, row, s, total);
   return cudaGetLastError();
 }
 
@@ -688,7 +719,7 @@ post_bwd_sums_kernel(const __grid_constant__ PostBwdParams q, float* __restrict_
     float* sc = scratch + (long long)ix.b * 4 * q.C + ix.c;
     st4(sc, acc[0]); st4(sc + q.C, acc[1]);
     if (HAS_GATE) { st4(sc + 2 * q.C, acc[2]); st4(sc + 3 * q.C, acc[3]); }
-    if (q.dgamma_a) {                                    // null when only the data gradient is wanted (G-step through D)
+    if (q.dgamma_a && !q.det.p) {                        // null when only the data gradient is wanted (G-step through D); det: see launch_post_bwd
       atomic_add4(q.dbeta_a + ix.c, acc[0]); atomic_add4(q.dgamma_a + ix.c, acc[1]);
       if (HAS_GATE) { atomic_add4(q.dbeta_g + ix.c, acc[2]); atomic_add4(q.dgamma_g + ix.c, acc[3]); }
     }
@@ -791,7 +822,8 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
         if (!db || (br == 1 && !HAS_GATE)) continue;
         F4 t = zero4();
         for (int w = ix.rl; w < 8; w += q.sh) { float4 v = red[br][w][lane]; t.v[0] += v.x; t.v[1] += v.y; t.v[2] += v.z; t.v[3] += v.w; }
-        atomic_add4(db + ix.rl * q.C + ix.c, t);
+        if (q.det.p) st4(q.det.p + ((long long)blockIdx.z * gridDim.y + blockIdx.y) * 2 * q.Cc + br * q.Cc + ix.rl * q.C + ix.c, t);
+        else atomic_add4(db + ix.rl * q.C + ix.c, t);
       }
     }
   }
@@ -1312,8 +1344,13 @@ cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st) {
   if (pp.B == 0) return cudaSuccess;
   if (!post_aligned(pp.p, pp.dy1, pp.dy2, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535) return cudaErrorInvalidValue;
   dim3 grid((pp.C + kPostChan - 1) / kPostChan, (pp.R + kPostRows - 1) / kPostRows, pp.B);
-  { cudaError_t se = cudaSuccess; if (post_bwd_stream_dispatch(pp, st, &se)) return se; }
-  if (pp.has_in && pp.R <= 64 && g_post_onepass) {
+  // deterministic mode takes the sums + apply form: its per-sample sums are the parameter-gradient contributions, and its bias partials
+  // go to one slab row per (sample, position block)
+  const bool det = pp.det.p != nullptr;
+  const bool det_bias = det && pp.dbias_a;
+  if (det_bias && (long long)pp.B * grid.y * 2 * pp.Cc > pp.det.cap) return cudaErrorInvalidValue;
+  if (!det) { cudaError_t se = cudaSuccess; if (post_bwd_stream_dispatch(pp, st, &se)) return se; }
+  if (!det && pp.has_in && pp.R <= 64 && g_post_onepass) {
     ++g_cgvc_launches;
     const dim3 g1(grid.x, 1, grid.z);
 #define ONEPASS(NR_) do { if (pp.has_gate) post_bwd_onepass_kernel<true, NR_><<<g1, 256, 0, st>>>(pp); else post_bwd_onepass_kernel<false, NR_><<<g1, 256, 0, st>>>(pp); } while (0)
@@ -1329,11 +1366,18 @@ cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st) {
     ++g_cgvc_launches;
     if (pp.has_gate) post_bwd_sums_kernel<true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
     else post_bwd_sums_kernel<false><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
+    if (det && pp.dgamma_a) {                            // scratch[b] = [S1a | S2a | S1g | S2g] = sample b's dbeta_a, dgamma_a, dbeta_g, dgamma_g
+      const long long C = pp.C, g = pp.has_gate ? C : 0;
+      cudaError_t e = launch_reduce_parts(scratch, pp.B, 4 * C, DetSegs{{pp.dbeta_a, pp.dgamma_a, pp.dbeta_g, pp.dgamma_g}, {0, C, 2 * C, 3 * C}, {C, C, g, g}}, st);
+      if (e != cudaSuccess) return e;
+    }
   }
   ++g_cgvc_launches;
   if (pp.has_in) { if (pp.has_gate) post_apply_bwd_kernel<true, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_bwd_kernel<true, false><<<grid, 256, 0, st>>>(pp, scratch); }
   else           { if (pp.has_gate) post_apply_bwd_kernel<false, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_bwd_kernel<false, false><<<grid, 256, 0, st>>>(pp, scratch); }
-  return cudaGetLastError();
+  if (!det_bias) return cudaGetLastError();
+  const long long Cc = pp.Cc;
+  return launch_reduce_parts(pp.det.p, (long long)pp.B * grid.y, 2 * Cc, DetSegs{{pp.dbias_a, pp.has_gate ? pp.dbias_g : nullptr}, {0, Cc}, {Cc, pp.has_gate ? Cc : 0}}, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1368,8 +1412,10 @@ cudaError_t launch_head_fwd(const float* y, long long rows, int C, const float* 
 __global__ void __launch_bounds__(256)
 head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y, long long rows, int C,
                      const float* __restrict__ w, float target, float coef, float* __restrict__ loss_slot,
-                     float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ db, const float* __restrict__ grad_mult_dev) {
+                     float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ db, const float* __restrict__ grad_mult_dev,
+                     float* __restrict__ part) {
   __shared__ float red[8][32];
+  float* prow = part ? part + (long long)blockIdx.x * (C + 2) : nullptr;     // det: [dw (C) | db | loss] of this CTA
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const float grad_mult = grad_mult_dev ? *grad_mult_dev : 1.f;
   float4 accw[8];
@@ -1400,8 +1446,11 @@ head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y
   float l = block_sum8(lane == 0 ? lsum : 0.f, red, warp, lane);
   float dbs = block_sum8(lane == 0 ? dbsum : 0.f, red, warp, lane);
   if (threadIdx.x == 0) {
-    if (loss_slot) atomicAdd(loss_slot, coef * l * inv);
-    if (db) atomicAdd(db, dbs);
+    if (prow) { prow[C] = dbs; prow[C + 1] = coef * l * inv; }
+    else {
+      if (loss_slot) atomicAdd(loss_slot, coef * l * inv);
+      if (db) atomicAdd(db, dbs);
+    }
   }
   if (dw) {
 #pragma unroll
@@ -1412,7 +1461,8 @@ head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y
       float vw = block_sum8(accw[i].w, red, warp, lane);
       if (warp == 0) {
         int c = lane * 4 + i * 128;
-        atomicAdd(dw + c, vx); atomicAdd(dw + c + 1, vy); atomicAdd(dw + c + 2, vz); atomicAdd(dw + c + 3, vw);
+        if (prow) { prow[c] = vx; prow[c + 1] = vy; prow[c + 2] = vz; prow[c + 3] = vw; }
+        else { atomicAdd(dw + c, vx); atomicAdd(dw + c + 1, vy); atomicAdd(dw + c + 2, vz); atomicAdd(dw + c + 3, vw); }
       }
     }
   }
@@ -1420,13 +1470,16 @@ head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y
 
 cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long rows, int C, const float* w,
                                  float target, float coef, float* loss_slot,
-                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev) {
+                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev, const DetSlab* det) {
   if (rows == 0) return cudaSuccess;
   if (C != 1024) return cudaErrorInvalidValue;
   long long nb = (rows + 7) / 8;
   if (nb > 296) nb = 296;
-  ++g_cgvc_launches; head_loss_bwd_kernel<<<(unsigned)nb, 256, 0, st>>>(prob, y, rows, C, w, target, coef, loss_slot, dy, dw, db, grad_mult_dev);
-  return cudaGetLastError();
+  float* part = det ? det->p : nullptr;
+  if (part && nb * (C + 2) > det->cap) return cudaErrorInvalidValue;
+  ++g_cgvc_launches; head_loss_bwd_kernel<<<(unsigned)nb, 256, 0, st>>>(prob, y, rows, C, w, target, coef, loss_slot, dy, dw, db, grad_mult_dev, part);
+  if (!part) return cudaGetLastError();
+  return launch_reduce_parts(part, nb, C + 2, DetSegs{{dw, db, loss_slot}, {0, C, C + 1}, {dw ? C : 0, db ? 1 : 0, loss_slot ? 1 : 0}}, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1434,7 +1487,8 @@ cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long ro
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 l1_loss_grad_kernel(const float* __restrict__ yhat, const float* __restrict__ y, long long n, float* __restrict__ loss_slot,
-                    const float* __restrict__ gscale_dev, float* __restrict__ d, int accumulate, const float* __restrict__ grad_mult_dev) {
+                    const float* __restrict__ gscale_dev, float* __restrict__ d, int accumulate, const float* __restrict__ grad_mult_dev,
+                    float* __restrict__ part) {
   __shared__ float red[8][32];
   const float inv = 1.f / (float)n;
   const float gs = (gscale_dev ? gscale_dev[0] * inv : inv) * (grad_mult_dev ? *grad_mult_dev : 1.f);
@@ -1451,15 +1505,19 @@ l1_loss_grad_kernel(const float* __restrict__ yhat, const float* __restrict__ y,
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   float t = block_sum8(lane == 0 ? s : 0.f, red, warp, lane);
-  if (threadIdx.x == 0 && loss_slot) atomicAdd(loss_slot, t * inv);
+  if (threadIdx.x == 0 && part) part[blockIdx.x] = t * inv;
+  else if (threadIdx.x == 0 && loss_slot) atomicAdd(loss_slot, t * inv);
 }
 
 cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, float* loss_slot,
-                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, const float* grad_mult_dev) {
+                                const float* gscale_dev, float* d, int accumulate, cudaStream_t st, const float* grad_mult_dev, const DetSlab* det) {
   if (n == 0) return cudaSuccess;
   long long nb = (n + 255) / 256; if (nb > 592) nb = 592;
-  ++g_cgvc_launches; l1_loss_grad_kernel<<<(unsigned)nb, 256, 0, st>>>(yhat, y, n, loss_slot, gscale_dev, d, accumulate, grad_mult_dev);
-  return cudaGetLastError();
+  float* part = det && loss_slot ? det->p : nullptr;
+  if (part && nb > det->cap) return cudaErrorInvalidValue;
+  ++g_cgvc_launches; l1_loss_grad_kernel<<<(unsigned)nb, 256, 0, st>>>(yhat, y, n, loss_slot, gscale_dev, d, accumulate, grad_mult_dev, part);
+  if (!part) return cudaGetLastError();
+  return launch_reduce_parts(part, nb, 1, DetSegs{{loss_slot}, {0}, {1}}, st);
 }
 
 // [B,F,T] -> [B,T,F] (F = 24 features; T frames).  Call with (F,T) swapped for the inverse.
@@ -1681,7 +1739,7 @@ template <int NT>
 __global__ void __launch_bounds__(256)
 wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ src, const float* __restrict__ grad, int g_ld, int N,
                 float* __restrict__ dw_a, float* __restrict__ dw_g, int n_split, float* __restrict__ db_a, float* __restrict__ db_g,
-                int rows_per_block) {
+                int rows_per_block, float* __restrict__ part) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   __shared__ float4 red[256];
   const int nq = N / 4;                                 // host guarantees nq divides 256
@@ -1723,22 +1781,34 @@ wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ 
       float4 sacc = make_float4(0.f, 0.f, 0.f, 0.f);
       for (int l = 0; l < rstep; ++l) { float4 v = red[l * nq + cq]; sacc.x += v.x; sacc.y += v.y; sacc.z += v.z; sacc.w += v.w; }
       float* dst = t < NT ? dw + (long long)g.widx[t] * ncols + nn : (db ? db + nn : nullptr);
-      if (dst) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(sacc.x), "f"(sacc.y), "f"(sacc.z), "f"(sacc.w) : "memory");
+      if (part) {                                          // det: row [dw_a | dw_g | db_a | db_g] of this CTA
+        float* pr = part + (long long)blockIdx.x * (g.ntaps + 1) * N;
+        const long long o = n < n_split ? 0 : (long long)g.ntaps * n_split;
+        const long long ob = (long long)g.ntaps * N + (n < n_split ? 0 : n_split);
+        float* pd = t < NT ? pr + o + (long long)g.widx[t] * ncols + nn : pr + ob + nn;
+        *reinterpret_cast<float4*>(pd) = sacc;
+      } else if (dst) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(sacc.x), "f"(sacc.y), "f"(sacc.z), "f"(sacc.w) : "memory");
     }
   }
 }
 
 cudaError_t launch_wgrad_c1(const GatherGeom& g, const float* src, const float* grad, int g_ld, int N,
-                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st) {
+                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = N / 4;
   if (N % 4 != 0 || nq > 256 || 256 % nq != 0 || n_split % 4 != 0 || g_ld % 4 != 0) return cudaErrorInvalidValue;
   int rpb = (int)((M + CGVC_NUM_SMS * 8 - 1) / (CGVC_NUM_SMS * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
+  const long long nb = (M + rpb - 1) / rpb, row = (long long)(g.ntaps + 1) * N, nt = g.ntaps;
+  float* part = det ? det->p : nullptr;
+  if (part && nb * row > det->cap) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
-  if (g.ntaps <= 9) wgrad_c1_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb);
-  else wgrad_c1_kernel<CGVC_MAX_TAPS><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb);
-  return cudaGetLastError();
+  if (g.ntaps <= 9) wgrad_c1_kernel<9><<<(unsigned)nb, 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb, part);
+  else wgrad_c1_kernel<CGVC_MAX_TAPS><<<(unsigned)nb, 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb, part);
+  if (!part) return cudaGetLastError();
+  const long long na = n_split, ng = N - n_split;
+  return launch_reduce_parts(part, nb, row, DetSegs{{dw_a, dw_g, db_a, db_g}, {0, nt * na, nt * N, nt * N + na},
+                                                    {nt * na, nt * ng, db_a ? na : 0, db_g ? ng : 0}}, st);
 }
 
 __global__ void gather_taps_kernel(const float* __restrict__ Z, float* __restrict__ dx, int B, int H, int W, int Ho, int Wo, int kh, int kw,
@@ -1755,7 +1825,7 @@ template <int NT>
 __global__ void __launch_bounds__(256)
 glu_bwd_wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ src, const float* __restrict__ dy,
                         const float* __restrict__ P, int C, float* __restrict__ dw_a, float* __restrict__ dw_g,
-                        float* __restrict__ db_a, float* __restrict__ db_g, int rows_per_block) {
+                        float* __restrict__ db_a, float* __restrict__ db_g, int rows_per_block, float* __restrict__ part) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   __shared__ float4 red[256];
   const int nq = C / 4;                                 // column quads per branch; host guarantees nq divides 256
@@ -1808,22 +1878,31 @@ glu_bwd_wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __res
         float4 sacc = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int l = 0; l < rstep; ++l) { float4 v = red[l * nq + cq]; sacc.x += v.x; sacc.y += v.y; sacc.z += v.z; sacc.w += v.w; }
         float* dst = t < NT ? dw + (long long)g.widx[t] * C + n : (db ? db + n : nullptr);
-        if (dst) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(sacc.x), "f"(sacc.y), "f"(sacc.z), "f"(sacc.w) : "memory");
+        if (part) {                                        // det: row [dw_a | dw_g | db_a | db_g] of this CTA
+          float* pr = part + (long long)blockIdx.x * 2 * (g.ntaps + 1) * C;
+          float* pd = t < NT ? pr + ((long long)br * g.ntaps + g.widx[t]) * C + n : pr + (2ll * g.ntaps + br) * C + n;
+          *reinterpret_cast<float4*>(pd) = sacc;
+        } else if (dst) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(sacc.x), "f"(sacc.y), "f"(sacc.z), "f"(sacc.w) : "memory");
       }
     }
   }
 }
 
 cudaError_t launch_glu_bwd_wgrad_c1(const GatherGeom& g, const float* src, const float* dy, const float* P, int C,
-                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st) {
+                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = C / 4;
   if (C % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9) return cudaErrorInvalidValue;
   int rpb = (int)((M + CGVC_NUM_SMS * 8 - 1) / (CGVC_NUM_SMS * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
+  const long long nb = (M + rpb - 1) / rpb, nt = g.ntaps, Cl = C, row = 2 * (nt + 1) * Cl;
+  float* part = det ? det->p : nullptr;
+  if (part && nb * row > det->cap) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
-  glu_bwd_wgrad_c1_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, src, dy, P, C, dw_a, dw_g, db_a, db_g, rpb);
-  return cudaGetLastError();
+  glu_bwd_wgrad_c1_kernel<9><<<(unsigned)nb, 256, 0, st>>>(g, src, dy, P, C, dw_a, dw_g, db_a, db_g, rpb, part);
+  if (!part) return cudaGetLastError();
+  return launch_reduce_parts(part, nb, row, DetSegs{{dw_a, dw_g, db_a, db_g}, {0, nt * Cl, 2 * nt * Cl, (2 * nt + 1) * Cl},
+                                                    {nt * Cl, nt * Cl, db_a ? Cl : 0, db_g ? Cl : 0}}, st);
 }
 
 // column sums over the 32 rows of a warp (row = lane): butterfly transpose-reduce, 31 shuffles for 32 columns; lane j ends with column j

@@ -201,6 +201,8 @@ struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[
   const uint8_t *g8_hi, *g8_lo;                          // [M, g_ld] bytes
   int w16;                                               // 1: fp16 planes only (one MMA unit per product; weight gradients are leaves of the graph)
   int fold_n;                                            // != 0: tap-folded layer (TcLayer::fold): column = t * fold_n + n of a [taps][C][fold_n] TF kernel
+  // deterministic form (DET): split k stores its partial tile to part + k * part_k, laid out like [dw_a | dw_g] (dw_g at numel_a)
+  float* part; long long part_k, numel_a;
 };
 
 // address of weight-gradient element (tap slab, channel c, column col) in the TF-layout kernel [taps][C][ncols]; with fold_n the layer's
@@ -1054,7 +1056,9 @@ struct TNCfg {
 
 // Persistent like the NT kernel: work items (n-tile, c-tile, tap, K-split) are walked with stride gridDim.x (n fastest, so
 // concurrently running CTAs share the same rows of X and dP in L2).  Each consumer warpgroup owns 64 of the 128 channels.
-template <int NPL, int W16>
+// DET (deterministic mode, ksplit > 1): the fragments are stored to the K-split's partial slab instead of added into dW; launch_tn then
+// adds the partials in K-split order (launch_reduce_parts)
+template <int NPL, int W16, int DET>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   static_assert(W16 == 0 || NPL == 3, "the fp16-only weight gradient is a form of CGVC_PREC_F16F8");
@@ -1075,12 +1079,12 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   long long chunk_rows = (M + p.ksplit - 1) / p.ksplit;
   chunk_rows = (chunk_rows + 63) / 64 * 64;
 
-  struct Item { int n0, c0, tap; long long mbeg, mend; int num_kb; };
+  struct Item { int n0, c0, tap, ks; long long mbeg, mend; int num_kb; };
   auto decode = [&](int item) -> Item {
     Item w;
     int n_t = item % n_tiles; int t1 = item / n_tiles;
     int c_t = t1 % c_tiles; int t2 = t1 / c_tiles;
-    w.tap = t2 % g.ntaps; int ks = t2 / g.ntaps;
+    w.tap = t2 % g.ntaps; const int ks = t2 / g.ntaps; w.ks = ks;
     w.n0 = n_t * BN; w.c0 = c_t * 128;
     w.mbeg = (long long)ks * chunk_rows;
     w.mend = (w.mbeg + chunk_rows < M) ? w.mbeg + chunk_rows : M;
@@ -1214,12 +1218,14 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
         const int n = w.n0 + 8 * j + 2 * (tw & 3);
         if (n >= p.N) continue;
         float* base; int nn; int ncols;                      // (n even and n_split even: a column pair never straddles the split)
-        if (n < p.n_split) { base = p.dw_a; nn = n; ncols = p.n_split; } else { base = p.dw_g; nn = n - p.n_split; ncols = p.N - p.n_split; }
+        if (n < p.n_split) { base = DET ? p.part + w.ks * p.part_k : p.dw_a; nn = n; ncols = p.n_split; }
+        else { base = DET ? p.part + w.ks * p.part_k + p.numel_a : p.dw_g; nn = n - p.n_split; ncols = p.N - p.n_split; }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (c + 8 * h >= p.C) continue;
           float* dst = tn_dst(base, g.widx[w.tap], p.C, c + 8 * h, ncols, nn, p.fold_n);
-          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[4 * j + 2 * h]), "f"(d[4 * j + 2 * h + 1]) : "memory");
+          if constexpr (DET) asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[4 * j + 2 * h]), "f"(d[4 * j + 2 * h + 1]) : "memory");
+          else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[4 * j + 2 * h]), "f"(d[4 * j + 2 * h + 1]) : "memory");
         }
       }
     }
@@ -1487,7 +1493,7 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st) {
+cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st, const DetSlab* det) {
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
   if (M == 0) return cudaSuccess;
   if (M >= (1ll << 31)) return cudaErrorInvalidValue;
@@ -1503,6 +1509,14 @@ cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st) {
     if (items < nsm) eff *= 0.5;                           // a single partial round: prefer more, smaller items
     if (eff > best + 0.02) { best = eff; ksplit = ks; }
   }
+  // deterministic mode: every element of every split's partial tile is stored (so no split may have an empty row range), and the
+  // ksplit partial copies of dW must fit the slab; a layer too large for two copies runs unsplit, whose adds are one per element
+  const long long numel = (long long)p.g.ntaps * p.C * p.N;
+  auto chunk_of = [&](int ks) { return ((M + ks - 1) / ks + 63) / 64 * 64; };
+  if (det && det->p)
+    while (ksplit > 1 && ((long long)ksplit * numel > det->cap || (long long)(ksplit - 1) * chunk_of(ksplit) >= M)) --ksplit;
+  const bool det_split = det && det->p && ksplit > 1;
+  if (det_split) { p.part = det->p; p.part_k = numel; p.numel_a = (long long)p.g.ntaps * p.C * p.n_split; }
   p.ksplit = ksplit;
   p.div_hw = make_fastdiv((uint32_t)(p.g.Hy * p.g.Wx)); p.div_w = make_fastdiv((uint32_t)p.g.Wx);
   const long long items = (long long)tiles * ksplit;
@@ -1510,18 +1524,27 @@ cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st) {
   cudaError_t e;
   ++g_cgvc_launches;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, 1, M, p.N, p.g.ntaps * p.C);
-#define LAUNCH_TN(NPL_, W16_)                                                                     \
+#define LAUNCH_TN(NPL_, W16_, DET_)                                                               \
   do {                                                                                            \
-    e = set_smem(tc_gg_tn_kernel<NPL_, W16_>, TNCfg<NPL_, W16_>::SMEM);                           \
+    e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_>, TNCfg<NPL_, W16_>::SMEM);                     \
     if (e != cudaSuccess) return e;                                                               \
-    tc_gg_tn_kernel<NPL_, W16_><<<grid, kNTThreads, TNCfg<NPL_, W16_>::SMEM, st>>>(p);            \
+    tc_gg_tn_kernel<NPL_, W16_, DET_><<<grid, kNTThreads, TNCfg<NPL_, W16_>::SMEM, st>>>(p);      \
   } while (0)
-  if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1); else LAUNCH_TN(3, 0); }
-  else if (precision == 1) LAUNCH_TN(2, 0);
-  else                     LAUNCH_TN(1, 0);
+  if (det_split) {
+    if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1); else LAUNCH_TN(3, 0, 1); }
+    else if (precision == 1) LAUNCH_TN(2, 0, 1);
+    else                     LAUNCH_TN(1, 0, 1);
+  } else {
+    if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 0); else LAUNCH_TN(3, 0, 0); }
+    else if (precision == 1) LAUNCH_TN(2, 0, 0);
+    else                     LAUNCH_TN(1, 0, 0);
+  }
 #undef LAUNCH_TN
   prof_end(st);
-  return cudaGetLastError();
+  if (!det_split) return cudaGetLastError();
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return launch_reduce_parts(p.part, ksplit, numel, DetSegs{{p.dw_a, p.dw_g}, {0, p.numel_a}, {p.numel_a, p.dw_g ? numel - p.numel_a : 0}}, st);
 }
 
 inline int ru(int v, int m) { return (v + m - 1) / m * m; }
@@ -1681,7 +1704,7 @@ int layer_dgrad(const TcLayer& L, int precision, const __nv_bfloat16* dPhi, cons
 
 int layer_wgrad(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                 const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                float* dwa, float* dwg, cudaStream_t st, int w16 = 0) {
+                float* dwa, float* dwg, cudaStream_t st, int w16 = 0, const DetSlab* det = nullptr) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   TcTNParams p; memset(&p, 0, sizeof p);
   p.w16 = (precision == 3 && w16) ? 1 : 0;
@@ -1702,7 +1725,7 @@ int layer_wgrad(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const
   } else if (!make_tmap3(&p.tm_g_hi, dPhi, (uint64_t)nt_k(L), (uint64_t)M, 1, 64) || !make_tmap3(&p.tm_g_lo, dPlo, (uint64_t)nt_k(L), (uint64_t)M, 1, 64)) {
     return (int)cudaErrorInvalidValue;
   }
-  return (int)launch_tn(p, precision, st);
+  return (int)launch_tn(p, precision, st, det);
 }
 
 }  // namespace
@@ -1798,8 +1821,9 @@ static cudaError_t tc_init_kernels() {
   INIT_NT_PK(256, 1) INIT_NT_PK(256, 2) INIT_NT_PK(256, 3) INIT_NT_PK(128, 1) INIT_NT_PK(128, 2) INIT_NT_PK(128, 3)
   INIT_NT_PK(32, 1) INIT_NT_PK(32, 2) INIT_NT_PK(32, 3)
 #undef INIT_NT_PK
-#define INIT_TN(NPL_, W16_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
-  INIT_TN(3, 1) INIT_TN(3, 0) INIT_TN(2, 0) INIT_TN(1, 0)
+#define INIT_TN(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
+  INIT_TN(3, 1, 0) INIT_TN(3, 0, 0) INIT_TN(2, 0, 0) INIT_TN(1, 0, 0)
+  INIT_TN(3, 1, 1) INIT_TN(3, 0, 1) INIT_TN(2, 0, 1) INIT_TN(1, 0, 1)
 #undef INIT_TN
   return cudaSuccess;
 }
@@ -1874,8 +1898,8 @@ int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_
 
 int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, cudaStream_t st) {
-  return layer_wgrad(w.layers[slot], w.precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16 ? 1 : 0);
+                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det) {
+  return layer_wgrad(w.layers[slot], w.precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16 ? 1 : 0, det);
 }
 
 bool tc_profile_is_on() { return g_prof_on; }
@@ -1967,7 +1991,7 @@ int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float
 }
 
 int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16) {
+                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16, const DetSlab* det) {
   TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   Temp T;
@@ -1988,8 +2012,8 @@ int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float
   if (e != cudaSuccess) return (int)e;
   if (dx) { r = layer_dgrad(L, precision, ghi, glo, B, H, W, sh, sw, dx, 0, st); if (r) return r; }
   if (dw) {
-    r = layer_wgrad(L, precision, xhi, xlo, ghi, glo, B, H, W, sh, sw, dw, nullptr, st, w16); if (r) return r;
-    if (dbias) { e = launch_colsum(dy, (long long)orows, Cout, 0, Cout, dbias, st); if (e != cudaSuccess) return (int)e; }
+    r = layer_wgrad(L, precision, xhi, xlo, ghi, glo, B, H, W, sh, sw, dw, nullptr, st, w16, det); if (r) return r;
+    if (dbias) { e = launch_colsum(dy, (long long)orows, Cout, 0, Cout, dbias, st, det); if (e != cudaSuccess) return (int)e; }
   }
   return (int)cudaStreamSynchronize(st);
 }

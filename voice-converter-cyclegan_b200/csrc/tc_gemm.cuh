@@ -102,12 +102,13 @@ int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_
 // dW_a/dW_g (TF layout) += x^T dP  (the bias gradients are column sums of dP: the instance-norm backward kernels or launch_colsum)
 int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, cudaStream_t st);
+                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det = nullptr);   // det: deterministic mode (kernels.cuh DetSlab)
 // self-contained versions for unit tests (fp32 in/out, temporary planes allocated internally)
 int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float* bias, float* y,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st);
 int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16 = 0);   // w16: F16F8 weight gradient from the fp16 planes alone
+                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16 = 0,   // w16: F16F8 weight gradient from the fp16 planes alone
+                      const DetSlab* det = nullptr);
 
 // per-launch CUDA-event timing of the tensor-core kernels (class 0 = forward/dgrad kernel with the plain epilogue,
 // 1 = wgrad kernel, 2 = forward kernel with the fused instance-norm epilogue)

@@ -13,6 +13,9 @@ Differences a user of the reference should know:
     a single NCCL all-reduce of the flat gradient arena per step
   * `loss_scale='monitor'` counts saturated F16F8 gradient / activation planes and non-finite gradients every step;
     `loss_scale='dynamic'` also skips such steps and adapts the loss scale (include/cgvc.h, DESIGN.md section 10)
+  * `deterministic=True` makes every train step bit-reproducible on one GPU: the same weights, Adam and loss-scale state and inputs give
+    the same bits whatever the stream schedule or CUDA-graph replay, so a rerun of a seed or a resumed checkpoint follows the
+    same trajectory (include/cgvc.h option "deterministic", DESIGN.md section 11; the NCCL sum of a data-parallel step is not covered)
 """
 from __future__ import annotations
 
@@ -37,7 +40,7 @@ class CycleGAN(object):
 
     def __init__(self, num_features, discriminator=_discriminator, generator=_generator_gatedcnn, mode='train',
                  log_dir='./log', *, max_batch=1, max_frames=None, precision='bf16x3', device=None, seed=0,
-                 data_parallel=False, summary_interval=0, loss_scale='static'):
+                 data_parallel=False, summary_interval=0, loss_scale='static', deterministic=False):
         for net in (discriminator, generator):
             if not hasattr(net, "check_engine_table"):
                 raise TypeError("CycleGAN(discriminator=..., generator=...) takes network descriptors (cgvc.module.generator_gatedcnn / "
@@ -63,6 +66,8 @@ class CycleGAN(object):
             raise ValueError("loss_scale must be one of %s, got %r" % (sorted(N.LOSS_SCALE_MODES), loss_scale))
         if loss_scale != 'static':
             self._options["loss_scale"] = N.LOSS_SCALE_MODES[loss_scale]     # applied by _create_engine, like any remembered option
+        if deterministic:
+            self._options["deterministic"] = 1
         self.last_step_skipped = False
         self.last_loss_scale = None
         self._create_engine()
@@ -107,6 +112,8 @@ class CycleGAN(object):
             self._chk(self._lib.cgvc_param_info(h, i, C.byref(name), C.byref(off), C.byref(nd), C.byref(shp)))
             self._table[name.value.decode()] = (off.value, tuple(shp[k] for k in range(nd.value)))
         self._generator_end = max(o + int(np.prod(s)) for n, (o, s) in self._table.items() if 'generator' in n)
+        if "deterministic" in self._options:                  # sizes WORK (its partials slab): set before the arenas are bound
+            self._chk(self._lib.cgvc_set_option(h, b"deterministic", self._options["deterministic"]))
         kinds = [N.ARENA_PARAM, N.ARENA_WORK]
         if self.mode == 'train':
             kinds += [N.ARENA_GRAD, N.ARENA_ADAM_M, N.ARENA_ADAM_V]
@@ -134,6 +141,18 @@ class CycleGAN(object):
         remembered across engine re-creations."""
         self._chk(self._lib.cgvc_set_option(self._handle, name.encode(), int(value)))
         self._options[name] = int(value)
+        if name == "deterministic":
+            # the option changes the WORK plan: a larger arena is allocated and bound before the next call needs it
+            nbytes = C.c_size_t(0)
+            self._chk(self._lib.cgvc_arena_bytes(self._handle, N.ARENA_WORK, C.byref(nbytes)))
+            work = self._arenas[N.ARENA_WORK]
+            if nbytes.value > work.numel() * 4:
+                torch.cuda.synchronize(self.device)                      # the old arena may still be read by enqueued work
+                del work
+                self._arenas.pop(N.ARENA_WORK)
+                work = torch.empty((nbytes.value + 3) // 4, dtype=torch.float32, device=self.device)
+                self._arenas[N.ARENA_WORK] = work
+                self._chk(self._lib.cgvc_bind_arena(self._handle, N.ARENA_WORK, _ptr(work), work.numel() * 4))
 
     @property
     def loss_scale(self):

@@ -157,12 +157,13 @@ def loss_scale_log(model, loss_scale):
 
 def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epochs, mini_batch_size, synthetic=0,
           precision="bf16x3", log_every=50, device_data=True, validation_A_dir=None, validation_B_dir=None, output_dir='./validation_output',
-          tensorboard_log_dir='./log', loss_scale='static'):
+          tensorboard_log_dir='./log', loss_scale='static', deterministic=False):
     """The reference's training loop (train.py:78-118).  device_data=True (default): the normalised corpus is uploaded once and the
     epoch sampler runs on the device (DeviceDataset), so no step copies anything host -> device and the losses are read back only
     when they are printed; device_data=False feeds host minibatches from the numpy sampler through CycleGAN.train(), like the
     reference's feed_dict.  loss_scale: 'static', 'monitor' or 'dynamic' (CycleGAN); when not static the log line also reports the
-    loss scale, the skipped steps and the last step's saturated F16F8 plane groups."""
+    loss scale, the skipped steps and the last step's saturated F16F8 plane groups.  deterministic: bit-reproducible steps
+    (CycleGAN), so that a rerun of the same seed writes the same checkpoints."""
     from .model import CycleGAN
     np.random.seed(random_seed)                                   # train.py:13
     f0_A = f0_B = None
@@ -183,7 +184,7 @@ def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epoc
         logf0_stats = {'mean_A': mA, 'std_A': sA, 'mean_B': mB, 'std_B': sB}
     mcep_stats = {'mean_A': A_mean, 'std_A': A_std, 'mean_B': B_mean, 'std_B': B_std}
     model = CycleGAN(num_features=NUM_MCEP, max_batch=mini_batch_size, max_frames=N_FRAMES, precision=precision, seed=random_seed,
-                     log_dir=tensorboard_log_dir, loss_scale=loss_scale)
+                     log_dir=tensorboard_log_dir, loss_scale=loss_scale, deterministic=deterministic)
     test_model = None
     data = DeviceDataset(model, A_norm, B_norm, mini_batch_size, N_FRAMES, seed=random_seed) if device_data else None
     g_loss = d_loss = float("nan")
@@ -215,7 +216,8 @@ def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epoc
         model.save(directory=model_dir, filename=model_name)      # train.py:113
         if (validation_A_dir is not None or validation_B_dir is not None) and epoch % VALIDATION_INTERVAL == 0:      # train.py:119-155
             if test_model is None:
-                test_model = CycleGAN(num_features=NUM_MCEP, mode='test', precision=precision, log_dir=tensorboard_log_dir)
+                test_model = CycleGAN(num_features=NUM_MCEP, mode='test', precision=precision, log_dir=tensorboard_log_dir,
+                                      deterministic=deterministic)
             validation_conversions(model, epoch, validation_A_dir, validation_B_dir, output_dir, mcep_stats, logf0_stats, test_model=test_model)
         dt = time.time() - t0
         print('Epoch %d: %d iterations, time elapsed %02d:%02d:%02d' % (epoch, n_iter, dt // 3600, dt % 3600 // 60, dt % 60))
@@ -242,11 +244,12 @@ def main():
                         '(saturated or non-finite steps skipped, scale adapted)')
     p.add_argument('--host_data', action='store_true', help='feed host minibatches from the numpy sampler every step (the reference\'s feed) '
                                                              'instead of the device-resident corpus + device sampler')
+    p.add_argument('--deterministic', action='store_true', help='bit-reproducible train steps (fixed-order gradient and loss reductions)')
     a = p.parse_args()
     none = lambda v: None if v in ('None', 'none') else v                                # train.py:191-192
     train(a.train_A_dir, a.train_B_dir, a.model_dir, a.model_name, a.random_seed, a.epochs, a.batch_size, a.synthetic, a.precision,
           device_data=not a.host_data, validation_A_dir=none(a.validation_A_dir), validation_B_dir=none(a.validation_B_dir),
-          output_dir=a.output_dir, tensorboard_log_dir=a.tensorboard_log_dir, loss_scale=a.loss_scale)
+          output_dir=a.output_dir, tensorboard_log_dir=a.tensorboard_log_dir, loss_scale=a.loss_scale, deterministic=a.deterministic)
 
 
 if __name__ == '__main__':
