@@ -115,6 +115,20 @@ struct GatherGeom {
   int Hd, Wd, dsy, dsx, doy, dox;
   short oy[CGVC_MAX_TAPS], ox[CGVC_MAX_TAPS], widx[CGVC_MAX_TAPS];
 };
+#ifdef __CUDACC__
+// The taps that rows of output rows y_lo .. y_hi can read (bit t): those with some y in the range and 0 <= y*sy + oy[t] < Hs.  Every
+// other tap reads only the zero padding for all of these rows.  Along x nothing is dropped.
+__host__ __device__ __forceinline__ uint32_t gather_tap_mask(const GatherGeom& g, int y_lo, int y_hi) {
+  uint32_t mask = 0;
+  for (int t = 0; t < g.ntaps; ++t) {
+    const int oy = g.oy[t];
+    int y = y_lo;                                            // the first y >= y_lo whose source row is not above the tensor
+    if (oy < 0 && (-oy + g.sy - 1) / g.sy > y) y = (-oy + g.sy - 1) / g.sy;
+    if (y <= y_hi && y * g.sy + oy < g.Hs) mask |= 1u << t;
+  }
+  return mask;
+}
+#endif
 
 // Packed variable-length 1-D geometry (cgvc_generator_forward_packed): n utterances concatenated along time.  off = n + 1 device
 // frame prefix sums at full resolution, every length a multiple of 4, so at a level of divisor div (1, 2 or 4: the T, T/2, T/4

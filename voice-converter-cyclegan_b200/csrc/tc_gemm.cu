@@ -186,7 +186,25 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   // packed variable-length utterances (the PK kernels, plain epilogue only): g is the 1-D geometry of all rows, pk.div the source
   // level's divisor; the output level's is pk.div * g.sx
   PackGeom pk;
+  FastDiv div_bw, div_w;                                 // B * Wx and Wx: row m -> (y, b, x), see nt_row
 };
+
+// Rows of the NT kernel are walked output row y outermost: m = (y * B + b) * Wx + x, so that a 128-row tile spans few output rows and
+// skips the taps that read only the padding for all of them (gather_tap_mask).  With Hy == 1 this is the sample order m = b * Wx + x.
+struct RowPos { int b, y, x; };
+__device__ __forceinline__ RowPos nt_row(const TcNTParams& p, long long m) {
+  RowPos r;
+  r.y = (int)fdiv((uint32_t)m, p.div_bw);
+  const uint32_t rem = (uint32_t)m - (uint32_t)r.y * p.div_bw.d;
+  r.b = (int)fdiv(rem, p.div_w);
+  r.x = (int)(rem - (uint32_t)r.b * p.div_w.d);
+  return r;
+}
+// the taps the tile of rows m0 .. m0 + 127 contracts over: the same list for its producers and its consumers
+__device__ __forceinline__ uint32_t nt_tile_taps(const TcNTParams& p, long long m0, long long M) {
+  const long long m1 = m0 + 127 < M ? m0 + 127 : M - 1;
+  return gather_tap_mask(p.g, nt_row(p, m0).y, nt_row(p, m1).y);
+}
 
 struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[src(m,t), c] * G[m, n]
   GatherGeom g;
@@ -459,7 +477,7 @@ __device__ __forceinline__ void hwrite_yq(float* stg, const float (&y)[32], floa
 // tile, n0 = its first column.  stg / rowp / bc: this warp's 2 KB transposition patch, destination-row table and coefficient
 // broadcast area; epi_xch: the group's cross-warp exchange area (statistics of samples that span several warps; barrier 1 + grp).
 template <int BN, int NPL, int EPI>
-__device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long long M, const int HW, const long long m0, const int n0,
+__device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long long M, const long long m0, const int n0,
                                                  const int q, const int lane, float* stg, float** rowp, float* bc, float (*epi_xch)[32],
                                                  const float* acc, const int grp = 0, const int ngrp = 1) {
   const GatherGeom& g = p.g;
@@ -469,9 +487,8 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
   const long long m = mq + lane;
   float* drow = nullptr;
   if (m < M && p.dst) {                                  // dst may be null for the fused forward epilogues (inference: nothing kept for backward)
-    int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
-    int y = rem / g.Wx; int x = rem - y * g.Wx;
-    long long dr = ((long long)(b * g.Hd + y * g.dsy + g.doy) * g.Wd + x * g.dsx + g.dox);
+    const RowPos o = nt_row(p, m);
+    long long dr = ((long long)(o.b * g.Hd + o.y * g.dsy + g.doy) * g.Wd + o.x * g.dsx + g.dox);
     drow = p.dst + dr * p.d_ld;
   }
   __syncwarp();
@@ -807,7 +824,7 @@ __device__ __forceinline__ void rescale_acc(float (&d)[N], float scale) {
 // stored or (accumulate) added.  One float2 store of a warp covers 8 rows x 32 contiguous bytes: whole sectors.  Nothing passes through
 // the pipeline stages, so the producers fill them with the next tile's operands meanwhile.
 template <int BN>
-__device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const float (&d)[BN / 2], const long long M, const int HW,
+__device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const float (&d)[BN / 2], const long long M,
                                                    const long long m0, const int n0, const int r, const int c) {
   const GatherGeom& g = p.g;
   float* rowp[2];
@@ -816,9 +833,8 @@ __device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const fl
     const long long m = m0 + r + 8 * h;
     rowp[h] = nullptr;
     if (m < M && p.dst) {
-      int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
-      int y = rem / g.Wx; int x = rem - y * g.Wx;
-      rowp[h] = p.dst + ((long long)(b * g.Hd + y * g.dsy + g.doy) * g.Wd + x * g.dsx + g.dox) * p.d_ld;
+      const RowPos o = nt_row(p, m);
+      rowp[h] = p.dst + ((long long)(o.b * g.Hd + o.y * g.dsy + g.doy) * g.Wd + o.x * g.dsx + g.dox) * p.d_ld;
     }
   }
   const bool vec = (p.d_ld & 1) == 0;
@@ -852,8 +868,8 @@ __device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const fl
 }
 
 // ------------------------------------------------------------------------------------------------ NT kernel
-// Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... (m fastest, so CTAs that run
-// concurrently share the weight tile in L2).  384 threads:
+// Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... (m or n fastest, see n_fast).
+// 384 threads:
 //   warps 0-3   producers (A rows by cp.async, weight tile by TMA), running ahead across K-blocks
 //   warps 4-11  two consumer warpgroups: wgmma of tile rows 64 wg .. + 63 into registers (BN / 2 per thread).  The plain epilogue
 //               (EPI 0) stores the fragments from registers (nt_store_fragments) while the producers already load the next tile.
@@ -881,15 +897,17 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const GatherGeom& g = p.g;
   const long long M = (long long)g.B * g.Hy * g.Wx;
-  const int HW = g.Hy * g.Wx;
   // K blocks ("stages"): 64 channels each; F16F8 walks the contraction twice -- first the two fp8 cross products (planes
-  // a8_hi x b8_lo and a8_lo x b8_hi), then the fp16 hi x hi product after the rescale of D
+  // a8_hi x b8_lo and a8_lo x b8_hi), then the fp16 hi x hi product after the rescale of D.  A tile walks only its taps
+  // (nt_tile_taps): cchunks stages per tap and pass
   const int cchunks = p.C >> 6;
-  const int kb_pass = g.ntaps * cchunks;
-  const int num_kb = NPL == 3 ? 2 * kb_pass : kb_pass;     // > 0 (the host never launches an empty contraction)
   const int m_tiles = (int)((M + 127) / 128);
   const int n_tiles = p.n_tiles;
   const int num_tiles = m_tiles * n_tiles;
+  // Tile order.  1-D layers walk m fastest: the CTAs that run at once share the weight tile in L2.  2-D layers (rows output row y
+  // outermost, see nt_row) walk n fastest: the CTAs that run at once share the activation rows of a few m tiles, which all kernel
+  // rows re-read, while the m tiles of different output rows read overlapping source rows at different times
+  const bool n_fast = g.Hy > 1;
 
   if (threadIdx.x == 0) {
     // full: 128 cp.async arrivals (A rows) + 1 arrive.expect_tx whose bytes the weight-tile TMA completes; empty / acc_free: one
@@ -910,9 +928,10 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
     int stage = 0; uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const long long m0 = (long long)(tile % m_tiles) * 128;
-      const int n0 = (tile / m_tiles) * BN;
+      const long long m0 = (long long)(n_fast ? tile / n_tiles : tile % m_tiles) * 128;
+      const int n0 = (n_fast ? tile % n_tiles : tile / m_tiles) * BN;
       if (EPI != 0 && it > 0) mbar_wait(&acc_free_bar, (uint32_t)(it - 1) & 1u);   // the previous tile's epilogue has left the stages
+      const uint32_t taps = nt_tile_taps(p, m0, M);
       int rb[8], ry[8], rx[8];                              // decoded output coordinates of this thread's 8 A rows
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -924,14 +943,14 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
             const long long o0 = __ldg(p.pk.off + u), o1 = __ldg(p.pk.off + u + 1);
             rb[i] = (int)(o0 / p.pk.div); ry[i] = (int)((o1 - o0) / p.pk.div); rx[i] = (int)(m - o0 / dout) * g.sx;
           } else {
-            int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
-            int y = rem / g.Wx; int x = rem - y * g.Wx;
-            rb[i] = b; ry[i] = y * g.sy; rx[i] = x * g.sx;
+            const RowPos o = nt_row(p, m);
+            rb[i] = o.b; ry[i] = o.y * g.sy; rx[i] = o.x * g.sx;
           }
         } else { rb[i] = -1; ry[i] = 0; rx[i] = 0; }
       }
       for (int pass = 0; pass < (NPL == 3 ? 2 : 1); ++pass)
       for (int tap = 0; tap < g.ntaps; ++tap) {
+        if (!((taps >> tap) & 1u)) continue;                 // its A tile would be all zeros
         long long aoff[8];                                   // element offset of the source row, or -1
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -995,25 +1014,26 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
     float* acc_s = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
     int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const long long m0 = (long long)(tile % m_tiles) * 128;
-      const int n0 = (tile / m_tiles) * BN;
+      const long long m0 = (long long)(n_fast ? tile / n_tiles : tile % m_tiles) * 128;
+      const int n0 = (n_fast ? tile % n_tiles : tile / m_tiles) * BN;
       float d[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       int prev = -1;                                         // stage whose MMAs may still be in flight
+      const int kb_pass = __popc(nt_tile_taps(p, m0, M)) * cchunks;   // (> 0 for TF-SAME geometries; 0 is safe)
       if constexpr (NPL == 3) {                             // e4m3 cross products, then the fp16 hi x hi products after the rescale of D
         consume_stages<BN, MMA_E4M3_CROSS, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
         rescale_acc(d, 1.f / (float)(1 << CGVC_Q_ACC_SHIFT));
         consume_stages<BN, MMA_F16, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
       } else {
-        consume_stages<BN, NPL == 2 ? MMA_BF16X3 : MMA_BF16, 0, Cfg>(d, num_kb, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+        consume_stages<BN, NPL == 2 ? MMA_BF16X3 : MMA_BF16, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
       }
       wgmma_wait<0>();
       fence_acc(d);
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       const int r0 = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2), c0 = 2 * (tw & 3);   // this thread's fragment rows r0, r0 + 8
       if constexpr (EPI == 0) {
-        if (!(p.debug & 3)) nt_store_fragments<BN>(p, d, M, HW, m0, n0, r0, c0);
+        if (!(p.debug & 3)) nt_store_fragments<BN>(p, d, M, m0, n0, r0, c0);
       } else {
         // the tile into shared memory once both warpgroups are done reading the stages
         consumer_bar();
@@ -1025,7 +1045,7 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
           }
         }
         consumer_bar();
-        nt_tile_epilogue<BN, NPL, EPI>(p, M, HW, m0, n0, cw & 3, lane, epi_stage[cw], epi_rowp[cw], epi_bc[cw], epi_xch[wg], acc_s, wg, 2);
+        nt_tile_epilogue<BN, NPL, EPI>(p, M, m0, n0, cw & 3, lane, epi_stage[cw], epi_rowp[cw], epi_bc[cw], epi_xch[wg], acc_s, wg, 2);
         fence_proxy_async();                                 // generic accesses of the stages before the next tile's TMA writes
         __syncwarp();
         if (lane == 0) mbar_arrive(&acc_free_bar);
@@ -1447,8 +1467,10 @@ int num_sms() {
 cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
   if (M == 0) return cudaSuccess;
+  if (M >= (1ll << 31)) return cudaErrorInvalidValue;    // (nt_row divides 32-bit row indices)
   const bool x3 = precision == 1;
   if (p.g.ntaps == 0) return cudaErrorInvalidValue;      // empty contractions are the caller's business
+  p.div_bw = make_fastdiv((uint32_t)(p.g.B * p.g.Wx)); p.div_w = make_fastdiv((uint32_t)p.g.Wx);
   const int bn = tile_rows(p.N, p.Nw);
   p.n_tiles = bn == 32 ? 1 : p.Nw / bn;                  // the 32-wide tile only ever covers the (<= 32) real columns
   const long long tiles = ((M + 127) / 128) * p.n_tiles;
