@@ -296,6 +296,34 @@ int cgvc_in_glu_backward_planes(cgvc_handle h, const float* dy, const float* p, 
                                 float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
                                 int B, int R, int C, int shuffle, int precision, int gate,
                                 void* hi, void* lo, unsigned long long* sat, void* stream);
+/* One generator layer with its instance norm, as a train step or a conversion runs it, so that the fused gather-GEMM epilogues can be
+ * checked against float64 and against the separate kernels.  precision CGVC_PREC_BF16X3, _BF16 or _F16F8 (planes as above).
+ * fuse = 1: the instance norm runs in the GEMM epilogue where the shape allows (1-D layer, R = 32, 64 or 128 positions per sample);
+ * fuse = 0, or a shape it refuses: the plain epilogue writes P and the instance-norm kernels follow.  *fused (may be NULL) tells which
+ * ran.  Both paths take the same arguments and write the same outputs.
+ * cgvc_conv_in_forward: the 1-D TF-'SAME' convolution of x [B, W, Cin] with stride sw, R = ceil(W / sw) positions per sample, then
+ *   gated (w_g given): y = IN(a; beta_a, gamma_a) * sigmoid(IN(g; beta_g, gamma_g)), shuffle 1 or 2 (the pixel shuffle of the upsample
+ *   blocks: IN over the shuffled view, module.py:115-146);
+ *   residual (w_g NULL, shuffle 1): y = resid [B, R, Cout] + IN(a; beta_a, gamma_a).
+ *   w_a / w_g [kw, Cin, Cout] and b_a / b_g [Cout] (TF layout).  Outputs, each NULL to skip: p [B, R, Ntot] the pre-norm convolution
+ *   (a in columns [0, Cout), g after; Ntot = Cout or 2 Cout), stats [B, 4, C] (mean_a, rstd_a, mean_g, rstd_g; C = Cout / shuffle),
+ *   y [B, R * shuffle, C] fp32; hi / lo, the planes of y, are required.  p = stats = NULL is the inference form.
+ * cgvc_conv_in_backward: dY = dgrad(dp) (+ dx when accumulate) of a stride-1 1-D layer L (w_a / w_g [kw, Cin, Cout] as above, no bias),
+ *   dp [B, R, Ntot] fp32; then the instance-norm backward of the upstream layer U whose output L read: bp [B, R, Cin or 2 Cin] its
+ *   pre-norm output, stats [B, 4, Cin] its statistics.
+ *   gate 1: U is gated (y = IN(a) * sigmoid(IN(g))); dx is only read (dY's accumulate term, or NULL).
+ *   gate 0: U is the residual h2 form (y = resid + IN(a)); dx (+)= dgrad(dp), so that dx = dY, the skip gradient.
+ *   hi / lo receive U's dP planes (layout of bp).  dbeta_a, dgamma_a (and dbeta_g, dgamma_g for gate 1): all NULL or all given, then
+ *   accumulated.  Never fused in CGVC_PREC_F16F8 or with the option "deterministic" on (which also needs WORK bound, as
+ *   cgvc_in_glu_backward). */
+int cgvc_conv_in_forward(cgvc_handle h, int precision, const float* x, const float* w_a, const float* w_g, const float* b_a,
+                         const float* b_g, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                         const float* resid, float* p, float* stats, float* y, void* hi, void* lo,
+                         int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused, void* stream);
+int cgvc_conv_in_backward(cgvc_handle h, int precision, const float* dp, const float* w_a, const float* w_g, const float* bp,
+                          const float* stats, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                          float* dx, void* hi, void* lo, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
+                          int B, int R, int Cin, int kw, int Cout, int gate, int accumulate, int fuse, int* fused, void* stream);
 
 /* error codes */
 enum {

@@ -1846,6 +1846,53 @@ int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, 
   return 0;
 }
 
+// ---- one generator layer with its instance norm, fused into the gather-GEMM epilogue or not (test entry points) ----------------
+int cgvc_conv_in_forward(cgvc_handle e, int precision, const float* x, const float* w_a, const float* w_g, const float* b_a, const float* b_g,
+                         const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g, const float* resid,
+                         float* p, float* stats, float* y, void* hi, void* lo,
+                         int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused, void* stream) {
+  if (fused) *fused = 0;
+  if (!e || !x || !w_a || !b_a || !beta_a || !gamma_a) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(plane_precision(e, precision, hi, lo));
+  const bool gated = w_g != nullptr;
+  if (gated ? (!b_g || !beta_g || !gamma_g) : (!resid || shuffle != 1))
+    return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_forward: a gated layer needs b_g, beta_g and gamma_g; a residual one resid and shuffle 1");
+  if (B < 1 || W < 1 || Cin < 1 || kw < 1 || kw > CGVC_MAX_TAPS || sw < 1 || (shuffle != 1 && shuffle != 2) || Cout % (32 * shuffle))
+    return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_forward: bad shape (B %d, W %d, Cin %d, kw %d, Cout %d, sw %d, shuffle %d)", B, W, Cin, kw, Cout, sw, shuffle);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  TcFuse f; memset(&f, 0, sizeof f);
+  f.gamma_a = gamma_a; f.beta_a = beta_a; f.gamma_g = gamma_g; f.beta_g = beta_g;
+  f.stats = stats; f.resid = resid; f.y = y; f.y_hi = (__nv_bfloat16*)hi; f.y_lo = (__nv_bfloat16*)lo;
+  return tc_result(e, tc_conv_in_fwd_adhoc(precision, x, w_a, w_g, b_a, b_g, f, p, B, W, Cin, kw, Cout, sw, shuffle, fuse, fused, (cudaStream_t)stream),
+                   nullptr, "conv + instance norm forward");
+}
+
+int cgvc_conv_in_backward(cgvc_handle e, int precision, const float* dp, const float* w_a, const float* w_g, const float* bp, const float* stats,
+                          const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g, float* dx, void* hi, void* lo,
+                          float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
+                          int B, int R, int Cin, int kw, int Cout, int gate, int accumulate, int fuse, int* fused, void* stream) {
+  if (fused) *fused = 0;
+  if (!e || !dp || !w_a || !bp || !stats || !beta_a || !gamma_a) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(plane_precision(e, precision, hi, lo));
+  if (gate ? (!beta_g || !gamma_g) : !dx)
+    return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_backward: the gated form needs beta_g and gamma_g; the residual form dx");
+  if (accumulate && !dx) return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_backward: accumulate needs dx");
+  const bool some = dbeta_a || dgamma_a || dbeta_g || dgamma_g, all = dbeta_a && dgamma_a && (!gate || (dbeta_g && dgamma_g));
+  if (some && !all) return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_backward: the affine gradients are all given or none");
+  if (B < 1 || R < 1 || Cin < 1 || Cin % 32 || kw < 1 || kw > CGVC_MAX_TAPS || Cout < 1)
+    return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_backward: bad shape (B %d, R %d, Cin %d, kw %d, Cout %d)", B, R, Cin, kw, Cout);
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  TcBwdFuse f; memset(&f, 0, sizeof f);
+  f.gated = gate != 0; f.bp = bp; f.stats = stats;
+  f.gamma_a = gamma_a; f.beta_a = beta_a; f.gamma_g = gamma_g; f.beta_g = beta_g;
+  f.dp_hi = (__nv_bfloat16*)hi; f.dp_lo = (__nv_bfloat16*)lo;
+  f.dbeta_a = dbeta_a; f.dgamma_a = dgamma_a; f.dbeta_g = dbeta_g; f.dgamma_g = dgamma_g;
+  return tc_result(e, tc_conv_in_bwd_adhoc(precision, dp, w_a, w_g, f, dx, accumulate, B, R, Cin, kw, Cout, fuse, fused, det, (cudaStream_t)stream),
+                   nullptr, "conv data gradient + instance norm backward");
+}
+
 int cgvc_in_glu_forward(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
                         float* y, float* stats, int B, int R, int C, int shuffle, void* stream) {
   return cgvc_in_glu_forward_planes(e, p, beta_a, gamma_a, beta_g, gamma_g, y, stats, B, R, C, shuffle, CGVC_PREC_FP32_SIMT, 1, nullptr,

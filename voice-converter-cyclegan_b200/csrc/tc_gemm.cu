@@ -2039,3 +2039,89 @@ int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float
   }
   return (int)cudaStreamSynchronize(st);
 }
+
+// an ad-hoc 1-D layer (kh = 1) with its weight planes and bias, gated when wg is given
+static int adhoc_layer_1d(Temp& T, TcLayer& L, int precision, const float* wa, const float* wg, const float* ba, const float* bg,
+                          int Cin, int kw, int Cout, int shuffle, cudaStream_t st) {
+  L.kh = 1; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = wg != nullptr; L.shuffle = shuffle;
+  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
+  int r = adhoc_layer(T, L, st); if (r) return r;
+  if (precision == 3) { r = adhoc_layer_q(T, L, st); if (r) return r; }
+  float* zero = T.get<float>(Cout);
+  if (!zero) return (int)cudaErrorMemoryAllocation;
+  cudaMemsetAsync(zero, 0, Cout * sizeof(float), st);
+  return refresh_layer(L, wa, wg, ba ? ba : zero, bg ? bg : zero, st);
+}
+
+int tc_conv_in_fwd_adhoc(int precision, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
+                         const TcFuse& fz, float* P, int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused,
+                         cudaStream_t st) {
+  if (fused) *fused = 0;
+  TcLayer L{};
+  Temp T;
+  int r = adhoc_layer_1d(T, L, precision, wa, wg, ba, bg, Cin, kw, Cout, shuffle, st); if (r) return r;
+  const size_t rows = (size_t)B * W;
+  const int Wo = (W + sw - 1) / sw, cpad = precision == 3 ? cin_q(L) : cin_k(L);
+  __nv_bfloat16* xhi = T.get<__nv_bfloat16>(rows * cpad); __nv_bfloat16* xlo = T.get<__nv_bfloat16>(rows * cpad);
+  if (!xhi || !xlo) return (int)cudaErrorMemoryAllocation;
+  cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
+  if (e != cudaSuccess) return (int)e;
+  TcFuse f = fz; f.R = Wo;
+  bool have_p = false;
+  if (fuse) {
+    bool done = false;
+    r = layer_fwd(L, precision, xhi, xlo, B, 1, W, 1, sw, P, st, &f, &done);
+    if (r != 0 && (done || P)) return r;                 // a failed launch (not the missing P of a shape the epilogue refuses)
+    if (done) { if (fused) *fused = 1; return (int)cudaStreamSynchronize(st); }
+    have_p = P != nullptr;                                 // refused: P already holds the plain-epilogue output
+  }
+  // the engine's fallback: the plain epilogue, then the instance-norm kernels
+  float* Pw = P ? P : T.get<float>((size_t)B * Wo * Ntot(L));
+  float* stats = fz.stats ? fz.stats : T.get<float>((size_t)B * 4 * (Cout / shuffle));
+  if (!Pw || !stats) return (int)cudaErrorMemoryAllocation;
+  if (!have_p) { r = layer_fwd(L, precision, xhi, xlo, B, 1, W, 1, sw, Pw, st); if (r) return r; }
+  PostParams q; memset(&q, 0, sizeof q);
+  q.p = Pw; q.ldp = Ntot(L); q.Cc = Cout; q.B = B; q.sh = shuffle; q.R = Wo * shuffle; q.C = Cout / shuffle;
+  q.has_in = 1; q.has_gate = L.gated;
+  q.beta_a = fz.beta_a; q.gamma_a = fz.gamma_a; q.beta_g = fz.beta_g; q.gamma_g = fz.gamma_g; q.resid = fz.resid;
+  q.y = fz.y; q.stats = stats; q.y_hi = fz.y_hi; q.y_lo = fz.y_lo; q.qmode = precision == 3;
+  e = launch_post_fwd(q, st);
+  if (e != cudaSuccess) return (int)e;
+  return (int)cudaStreamSynchronize(st);
+}
+
+int tc_conv_in_bwd_adhoc(int precision, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
+                         int B, int R, int Cin, int kw, int Cout, int fuse, int* fused, const DetSlab* det, cudaStream_t st) {
+  if (fused) *fused = 0;
+  TcLayer L{};
+  Temp T;
+  int r = adhoc_layer_1d(T, L, precision, wa, wg, nullptr, nullptr, Cin, kw, Cout, 1, st); if (r) return r;
+  const size_t rows = (size_t)B * R;
+  const int gpad = precision == 3 ? nt_q(L) : nt_k(L);
+  __nv_bfloat16* ghi = T.get<__nv_bfloat16>(rows * gpad); __nv_bfloat16* glo = T.get<__nv_bfloat16>(rows * gpad);
+  if (!ghi || !glo) return (int)cudaErrorMemoryAllocation;
+  cudaError_t e = tc_split_planes(precision, dP, (long long)rows, Ntot(L), ghi, glo, st);
+  if (e != cudaSuccess) return (int)e;
+  // dY = dgrad(dP) (+ dx): the residual form keeps it in dx; the gated form works on a copy, so that dx is only read
+  float* dY = dx;
+  if (uf.gated) {
+    dY = T.get<float>(rows * Cin);
+    if (!dY) return (int)cudaErrorMemoryAllocation;
+    if (accumulate) { e = cudaMemcpyAsync(dY, dx, rows * Cin * sizeof(float), cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) return (int)e; }
+  }
+  TcBwdFuse f = uf; f.R = R; f.bp_ld = f.dp_ld = (uf.gated ? 2 : 1) * Cin;
+  bool done = false;
+  r = layer_dgrad(L, precision, ghi, glo, B, 1, R, 1, 1, dY, accumulate, st, fuse && !det ? &f : nullptr, &done);
+  if (r) return r;
+  if (done) { if (fused) *fused = 1; return (int)cudaStreamSynchronize(st); }
+  // the engine's fallback: the plain data gradient above, then the instance-norm (+ GLU) backward kernels
+  PostBwdParams q; memset(&q, 0, sizeof q);
+  if (det) q.det = *det;
+  q.dy1 = dY; q.p = uf.bp; q.ldp = f.bp_ld; q.Cc = Cin; q.B = B; q.R = R; q.C = Cin; q.sh = 1;
+  q.beta_a = uf.beta_a; q.gamma_a = uf.gamma_a; q.beta_g = uf.beta_g; q.gamma_g = uf.gamma_g; q.has_in = 1; q.has_gate = uf.gated;
+  q.stats = uf.stats; q.dp_hi = uf.dp_hi; q.dp_lo = uf.dp_lo; q.qmode = precision == 3;
+  q.dbeta_a = uf.dbeta_a; q.dgamma_a = uf.dgamma_a; q.dbeta_g = uf.dbeta_g; q.dgamma_g = uf.dgamma_g;
+  e = launch_post_bwd(q, st);
+  if (e != cudaSuccess) return (int)e;
+  return (int)cudaStreamSynchronize(st);
+}

@@ -109,6 +109,17 @@ int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float
 int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16 = 0,   // w16: F16F8 weight gradient from the fp16 planes alone
                       const DetSlab* det = nullptr);
+// one generator layer as the engine runs it (include/cgvc.h cgvc_conv_in_forward): the 1-D convolution of x [B, W, Cin] (gated when wg
+// is given) and the instance norm of fz (fz.R is set here).  fuse: the fused epilogue where the shape allows (*fused = 1), else the
+// plain epilogue and launch_post_fwd; P may be null (inference: a temporary when the shape needs the fallback)
+int tc_conv_in_fwd_adhoc(int precision, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
+                         const TcFuse& fz, float* P, int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused,
+                         cudaStream_t st);
+// the data gradient of a stride-1 1-D layer from fp32 dP [B*R, Ntot] with the upstream layer's instance-norm (+ GLU) backward uf
+// (uf.R, bp_ld and dp_ld are set here; include/cgvc.h cgvc_conv_in_backward): fused where the shape allows, else the plain data
+// gradient and launch_post_bwd.  det: deterministic mode (never fused)
+int tc_conv_in_bwd_adhoc(int precision, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
+                         int B, int R, int Cin, int kw, int Cout, int fuse, int* fused, const DetSlab* det, cudaStream_t st);
 
 // per-launch CUDA-event timing of the tensor-core kernels (class 0 = forward/dgrad kernel with the plain epilogue,
 // 1 = wgrad kernel, 2 = forward kernel with the fused instance-norm epilogue)
