@@ -201,7 +201,10 @@ int cgvc_allreduce_grads(cgvc_handle h, void* stream);
  * epilogue), the summed device time [ms], algorithmic FLOPs (2*M*N*K, counted once, whatever the bf16 split multiplies it by)
  * and launch count since the enable call. */
 int cgvc_kernel_launches(unsigned long long* count);
-/* options: "two_streams" (default 1): run the two symmetric halves of a train step on two internal streams; 0 enqueues
+/* options.  Every option belongs to its handle: it changes what that engine launches and no other engine's, and a call that changes
+ * an option's value drops that handle's captured step graphs (the next step captures anew).  The options below that are flags take
+ * any value, non-zero meaning 1; a value outside an option's range is refused with CGVC_ERR_ARG.
+ * "two_streams" (default 1): run the two symmetric halves of a train step on two internal streams; 0 enqueues
  * everything on the caller's stream (used while per-kernel timings are taken).
  * "fuse_in" (default 1): instance norm + GLU / + residual fused into the forward conv kernel's epilogue where the shape
  * allows (generator layers whose 128-row tiles hold whole samples); 0 always uses the separate streaming kernels.
@@ -222,15 +225,15 @@ int cgvc_kernel_launches(unsigned long long* count);
  * 24-channel side padded to a 64 / 128-channel line per tap (forward / data gradient on a 32-wide tile).
  * "wgrad_f16" (CGVC_PREC_F16F8 only, default 1): weight-gradient GEMMs from the fp16 planes alone, one MMA unit per product; every
  * gradient tensor stays within 3.6e-4 of the float64 oracle (tolerance 1e-3; 1.8e-4 with 0 = fp16 + two e4m3 cross terms, 2 units).
- * "prep_batched" (CGVC_PREC_F16F8 only, default 1, process-wide): the fp16 + e4m3 weight planes of all layers (forward and data-gradient
+ * "prep_batched" (CGVC_PREC_F16F8 only, default 1): the fp16 + e4m3 weight planes of all layers (forward and data-gradient
  * layouts, biases) are rebuilt after Adam by ONE kernel that walks a job table in 32 x 64 tiles (one per network range in the pipelined
  * data-parallel schedule); 0 = three small kernels per layer branch (~210 launches per step).  Bit-identical planes.
- * "post_onepass" (default 1, process-wide): GLU / instance-norm backward of samples with <= 64 positions in one kernel that keeps the
+ * "post_onepass" (default 1): GLU / instance-norm backward of samples with <= 64 positions in one kernel that keeps the
  * sample's rows in registers (reads dY and the pre-norm outputs once); 0 = always the sums + apply kernel pair.
- * "post_stream" (default 1, process-wide): gated layers without pixel shuffle whose samples have 32, 48 or 64 positions take the streaming
+ * "post_stream" (default 1): gated layers without pixel shuffle whose samples have 32, 48 or 64 positions take the streaming
  * form of the one-pass GLU / instance-norm backward: persistent CTAs walk (sample, channel block) items through a cp.async double buffer
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
- * "loss_scale" (default 0) and "loss_scale_growth_interval" (default 2000): see cgvc_loss_scale_state.
+ * "loss_scale" (default 0; 0, 1 or 2) and "loss_scale_growth_interval" (default 2000; >= 1): see cgvc_loss_scale_state.
  * "deterministic" (default 0): 1 makes cgvc_train_step and cgvc_compute_gradients bitwise reproducible on one GPU.  The same inputs,
  * PARAM, ADAM_M / ADAM_V, Adam step, loss-scaler state, batch, frames, precision and options give the same bits of PARAM, GRAD, ADAM_M,
  * ADAM_V, the 8 losses, gen_A / gen_B and the scaler state, in every precision and loss_scale mode, on repeated calls and fresh
@@ -240,7 +243,7 @@ int cgvc_kernel_launches(unsigned long long* count);
  * it, or the calls return CGVC_ERR_UNBOUND; cgvc_conv_backward and cgvc_in_glu_backward(_planes) honour it too and then need WORK
  * bound.  With a communicator attached each rank's gradients are deterministic; the NCCL all-reduce that sums them is not covered.
  * "debug_taps" (default 0): see cgvc_debug_activation.
- * "tc_debug" (default 0): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
+ * "tc_debug" (default 0; 0 to 7): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
  * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather.  The plain
  * epilogue stores straight from the accumulator registers, so for it 2 acts as 1. */
 int cgvc_set_option(cgvc_handle h, const char* name, int value);

@@ -8,6 +8,7 @@
 #include "geom.h"
 
 #include <dlfcn.h>
+#include <limits.h>
 #include <stddef.h>
 #include <math.h>
 #include <stdarg.h>
@@ -58,12 +59,12 @@ struct GenActs {
   struct { GLAct h1, h2; } r[6];
   GLAct u[2];
   float* out_cl;
-  float* post;                  // scratch for the instance-norm sums [n,4,1024] (null: the kernels' own lazily grown buffer)
+  float* post;                  // scratch for the instance-norm sums [n,4,1024]
 };
 struct DiscActs { int n, T; const float* x; GLAct h1, d[3]; float* prob; float* post; };
 
 struct GraphKey {
-  int batch, frames, id_off, kind, lanes, fuse;
+  int batch, frames, id_off, kind;
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 struct GraphEntry { cudaGraphExec_t exec; unsigned long long launches; };
@@ -102,8 +103,30 @@ struct SideQ {
   bool on = false;
 };
 
+// The engine's options (cgvc_set_option, include/cgvc.h) with their defaults.  Those that only the tensor-core module reads
+// (wgrad_f16, prep_batched, tc_debug) live in TcWeights.
+struct Options {
+  int fuse_in = 1;              // fuse instance norm (+GLU / +residual) into the forward GEMM epilogue where the shape allows
+  int fuse_bwd = 0;             // fuse the instance-norm (+GLU) backward into the upstream data-gradient GEMM's epilogue likewise.
+                                // Off by default: unlike the streaming kernels, that epilogue work cannot overlap the other lane's
+                                // tensor-core kernels
+  int edge_lower = 1;           // the generator's 15-tap, 24-channel edge layers as dense 1 x 1 GEMMs (taps moved into the channel / column dimension)
+  int side_wgrad = 0;           // weight-gradient GEMMs on a side stream per lane (see SideQ); needs two_streams, excludes fuse_bwd.  Off by default
+  int fuse_c1 = 1;              // discriminator input layer backward: GLU backward fused into its weight / data gradient kernels
+  int two_streams = 1;          // 0: both lanes are enqueued on the caller's stream (clean per-kernel timing for profiling)
+  int pipelined_comm = 1;       // data parallel: all-reduce, Adam and plane refresh network by network (see comm_stream)
+  int deterministic = 0;        // bit-reproducible steps: fixed-order reductions into GRAD and the loss slots (DESIGN.md section 11);
+                                // ignores fuse_bwd and side_wgrad
+  int debug_taps = 0;           // cgvc_generator_forward also writes the fp32 copy of every layer output (cgvc_debug_activation)
+  int use_graphs = 1;           // "cuda_graph": replay the step as a CUDA graph (turned off when a capture fails)
+  int ls_mode = 0;              // "loss_scale": 0 static, 1 monitor (static scale, counters collected), 2 dynamic
+  int ls_growth = 2000;         // "loss_scale_growth_interval"
+  PostForms post = {1, 1};      // "post_onepass", "post_stream": the forms the instance-norm kernels may take (kernels.cuh)
+};
+
 struct cgvc_engine {
   cgvc_config cfg;
+  Options opt;
   std::string err;
   std::vector<TensorInfo> tensors;
   size_t n_params = 0;        // arena length in elements (tensors padded to 16-byte boundaries)
@@ -122,30 +145,15 @@ struct cgvc_engine {
   // the two lanes of a training step run on their own streams (forked from / joined into the caller's stream)
   cudaStream_t lane_stream[2] = {nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
-  int use_graphs = 1;           // replay the step as a CUDA graph (disabled automatically if capture is not possible)
   std::map<GraphKey, GraphEntry> graphs;
   float* stage = nullptr;       // [2][max_batch,num_features,max_frames]: fixed-address copies of the step's inputs for the graphs
   cudaStream_t graph_stream = nullptr; cudaEvent_t ev_bridge = nullptr, ev_bridge2 = nullptr;
-  int fuse_in = 1;              // fuse instance norm (+GLU / +residual) into the forward GEMM epilogue where the shape allows
-  int debug_taps = 0;           // cgvc_generator_forward also writes the fp32 copy of every layer output (cgvc_debug_activation)
-  int fuse_bwd = 0;             // fuse the instance-norm (+GLU) backward into the upstream data-gradient GEMM's epilogue likewise.
-                                // Off by default: unlike the streaming kernels, that epilogue work cannot overlap the other lane's
-                                // tensor-core kernels
   // data-parallel step: the gradient all-reduce runs per network on its own stream; Adam and the weight-plane refresh of a network
   // start as soon as its all-reduce has finished, while the next network's is still on the wire
   cudaStream_t comm_stream = nullptr; cudaEvent_t ev_grads = nullptr, ev_ar[4] = {nullptr, nullptr, nullptr, nullptr};
-  int pipelined_comm = 1;
-  int fuse_c1 = 1;              // discriminator input layer backward: GLU backward fused into its weight / data gradient kernels
-  int edge_lower = 1;           // the generator's 15-tap, 24-channel edge layers as dense 1 x 1 GEMMs (taps moved into the channel / column dimension)
-  int two_streams = 1;          // 0: both lanes are enqueued on the caller's stream (clean per-kernel timing for profiling)
-  int side_wgrad = 0;           // weight-gradient GEMMs on a side stream per lane (see SideQ); needs two_streams, excludes fuse_bwd.  Off by default
-  int deterministic = 0;        // bit-reproducible steps: fixed-order reductions into GRAD and the loss slots (DESIGN.md section 11);
-                                // ignores fuse_bwd and side_wgrad
   SideQ sideq[2];
-  // loss scaling (option "loss_scale"): 0 static, 1 monitor (static scale, counters collected), 2 dynamic.  ls: the device state;
-  // d_scalars[16 + l] holds the static scale of batches [2^l, 2^(l+1)) (loss_scale), so that the loss kernels always read a pointer
-  int ls_mode = 0;
-  int ls_growth = 2000;         // option "loss_scale_growth_interval"
+  // loss scaling (opt.ls_mode).  ls: the device state; d_scalars[16 + l] holds the static scale of batches [2^l, 2^(l+1)) (loss_scale),
+  // so that the loss kernels always read a pointer
   LossScaler* ls = nullptr;
   bool ls_ready = false;        // dynamic mode: ls->scale holds a scale (set on the first step from the static one, or by the caller)
   int ls_batch = 0;             // monitor mode: the batch whose static scale ls->scale reports
@@ -153,6 +161,8 @@ struct cgvc_engine {
   cudaEvent_t ev_ls = nullptr;  // data parallel: the saturation all-reduce and the GRAD check are done (comm stream)
   // debug taps of the last forward
   std::map<std::string, std::pair<const float*, size_t>> taps;
+  // the instance-norm sums scratch of the calls outside a train step (which has its WORK slices): conversions, cgvc_in_glu_*
+  float* post_buf = nullptr; size_t post_elems = 0;
 
   float* P() const { return (float*)arena[CGVC_ARENA_PARAM]; }
   float* G() const { return (float*)arena[CGVC_ARENA_GRAD]; }
@@ -169,6 +179,25 @@ static int fail(cgvc_engine* e, int code, const char* fmt, ...) {
   do { cudaError_t _e = (call);                                                                    \
        if (_e != cudaSuccess) return fail(e, CGVC_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(_e)); } while (0)
 #define RET(call) do { int _r = (call); if (_r != 0) return _r; } while (0)
+
+// Captured step graphs hold the kernels, options and addresses of the moment they were captured: dropped whenever one of those changes
+static void drop_graphs(cgvc_engine* e) {
+  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
+  e->graphs.clear();
+}
+
+// e->post_buf with room for `elems` floats (on the engine's device: called under its DeviceGuard)
+static cudaError_t grow_post_buf(cgvc_engine* e, size_t elems, float** out) {
+  if (elems > e->post_elems) {
+    cudaFree(e->post_buf);
+    const size_t want = elems < (size_t)(1 << 22) ? (size_t)(1 << 22) : elems * 2;
+    cudaError_t ce = cudaMalloc(&e->post_buf, want * sizeof(float));
+    if (ce != cudaSuccess) { e->post_buf = nullptr; e->post_elems = 0; return ce; }
+    e->post_elems = want;
+  }
+  *out = e->post_buf;
+  return cudaSuccess;
+}
 
 // Every entry point runs on the engine's device and leaves the caller's current device as it found it (a single process may
 // drive several GPUs through torch, whose current device must not change behind its back).
@@ -323,16 +352,16 @@ static float loss_scale(const cgvc_engine* e, int batch) {
 // the device copy of loss_scale(e, batch) (d_scalars[16 + floor(log2 batch)], written at creation), or in dynamic mode the scaler's
 // current scale: what the loss-gradient kernels multiply by
 static const float* loss_scale_dev(const cgvc_engine* e, int batch) {
-  if (e->ls_mode == 2) return &e->ls->scale;
+  if (e->opt.ls_mode == 2) return &e->ls->scale;
   int l = 0; while ((2 << l) <= batch && l < 9) ++l;
   return e->d_scalars + 16 + l;
 }
 // saturation counters of the plane writers (null: not counted): only F16F8 has reduced-range planes, only train steps are counted
 static unsigned long long* sat_grad(const cgvc_engine* e) {
-  return e->counting && e->ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_grad : nullptr;
+  return e->counting && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_grad : nullptr;
 }
 static unsigned long long* sat_act(const cgvc_engine* e) {
-  return e->counting && e->ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_act : nullptr;
+  return e->counting && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_act : nullptr;
 }
 
 static bool tc_enabled(const cgvc_engine* e) { return e->cfg.precision != CGVC_PREC_FP32_SIMT && e->tcw.ready; }
@@ -427,7 +456,7 @@ static PostParams post_params(const cgvc_engine* e, const Layer& L, const ConvIO
 static int layer_forward(cgvc_engine* e, const Layer& L, const ConvIO& io, const GLAct& A, int rows_per_sample_out, bool keep_y,
                          bool save_pre, float* post_scratch, cudaStream_t st, const float* resid = nullptr) {
   bool done = false;
-  if (use_tc(e, L.tc_slot) && io.xhi && !io.pk.off && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && e->fuse_in) {
+  if (use_tc(e, L.tc_slot) && io.xhi && !io.pk.off && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && e->opt.fuse_in) {
     const float* Pm = e->P();
     TcFuse f; memset(&f, 0, sizeof f);
     f.R = rows_per_sample_out;
@@ -443,7 +472,7 @@ static int layer_forward(cgvc_engine* e, const Layer& L, const ConvIO& io, const
   }
   if (!done) RET(conv_fwd(e, L, io, A.P, st));
   PostParams q = post_params(e, L, io, A, rows_per_sample_out, keep_y, post_scratch, resid);
-  CK(launch_post_fwd(q, st));
+  CK(launch_post_fwd(q, e->opt.post, st));
   return 0;
 }
 
@@ -453,7 +482,7 @@ static int layer_forward(cgvc_engine* e, const Layer& L, const ConvIO& io, const
 // [360,128] matrix as it lies in memory, so forward, data and weight gradient address the same PARAM / GRAD ranges), o1 a 1 x 1 layer
 // with the taps folded into its output columns (TcLayer::fold) followed by the tap-shifted sum.
 static inline int edge_cpad(int c) { return (c + 127) / 128 * 128; }      // operand-plane width of kw * F channels (a multiple of 128 serves both precisions)
-static bool edge_on(const cgvc_engine* e, const GenNet& N) { return e->edge_lower && use_tc(e, N.h1c_slot) && use_tc(e, N.o1f_slot); }
+static bool edge_on(const cgvc_engine* e, const GenNet& N) { return e->opt.edge_lower && use_tc(e, N.h1c_slot) && use_tc(e, N.o1f_slot); }
 
 static void plan_gated(Bump& ws, GLAct& a, long long rows_out, int cout2, int n, int Cstat, bool planes, long long y_elems) {
   a.P = ws.take<float>((size_t)rows_out * cout2);
@@ -514,7 +543,7 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
     CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
                           A.xchi, A.xclo, st, A.off, A.n, sat_act(e)));
     RET(tc_result(e, tc_conv_fwd(e->tcw, N.h1c_slot, A.xchi, A.xclo, n, 1, T, 1, 1, A.h1.P, st), &N.h1.a, "forward (tap-lowered)"));
-    PostParams q = post_params(e, N.h1, io, A.h1, T, keep_y, A.post); CK(launch_post_fwd(q, st));
+    PostParams q = post_params(e, N.h1, io, A.h1, T, keep_y, A.post); CK(launch_post_fwd(q, e->opt.post, st));
   } else {
     if (A.xhi && tc_enabled(e)) CK(tc_split_planes(e->cfg.precision, x_cl, (long long)n * T, nf, A.xhi, A.xlo, st, sat_act(e)));
     RET(layer_forward(e, N.h1, io, A.h1, T, keep_y, save_pre, A.post, st));
@@ -658,7 +687,7 @@ static int layer_dp(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAct& A, 
   bool written = false;
   const PlanePair out = dp_planes(w, st, &written);
   q = post_bwd_params(e, L, dy, A, n, rows_per_sample_out, w.S, wgrad, false, out);
-  if (!written) CK(launch_post_bwd(q, st));
+  if (!written) CK(launch_post_bwd(q, e->opt.post, st));
   return 0;
 }
 
@@ -694,7 +723,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   };
   auto of = [&](const GLAct& a, int W) { return at(a.Y, a.Yhi, a.Ylo, W); };
   // the fused backward epilogues do not count saturation: a step whose planes are counted takes the separate kernels
-  BwdWalk w(S, e->fuse_bwd && !e->deterministic && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi &&
+  BwdWalk w(S, e->opt.fuse_bwd && !e->opt.deterministic && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi &&
                A.r[0].h2.Yhi);
   const bool edge = edge_on(e, N) && A.xchi && A.z;
   // o1 (no norm, no gate): bias gradient = column sums of d_out
@@ -776,7 +805,7 @@ static int discriminator_forward(cgvc_engine* e, const DiscNet& N, DiscActs& A, 
   A.x = x;
   ConvIO io; io.x = x; io.xhi = nullptr; io.xlo = nullptr; io.n = n; io.H = H0; io.W = T;
   int H = H0, W = T / 2;
-  if (e->fuse_c1 && !use_tc(e, N.h1.tc_slot) && N.h1.a.cin == 1 && !N.h1.has_in && N.h1.a.kh * N.h1.a.kw <= 9 && N.h1.a.cout % 4 == 0 &&
+  if (e->opt.fuse_c1 && !use_tc(e, N.h1.tc_slot) && N.h1.a.cin == 1 && !N.h1.has_in && N.h1.a.kh * N.h1.a.kw <= 9 && N.h1.a.cout % 4 == 0 &&
       256 % (N.h1.a.cout / 4) == 0) {
     // input layer (one input channel, K = 9, gate without norm): convolution + GLU in one HBM-bound pass; P is kept for the backward pass
     const GatherGeom g = fwd_geom(n, H0, T, N.h1.a.kh, N.h1.a.kw, N.h1.sh, N.h1.sw);
@@ -840,7 +869,7 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   }
   // h1: one input channel (K = 9), gate without instance norm.  Fused form: the GLU backward is recomputed inside the weight-gradient /
   // data-gradient kernels, dP never goes to HBM
-  if (e->fuse_c1 && N.h1.a.cout == 128 && N.h1.a.kh * N.h1.a.kw <= 9 && !N.h1.has_in) {
+  if (e->opt.fuse_c1 && N.h1.a.cout == 128 && N.h1.a.kh * N.h1.a.kw <= 9 && !N.h1.has_in) {
     if (wgrad) {
       GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
       CK(launch_glu_bwd_wgrad_c1(g, A.x, dy, A.h1.P, 128, e->G() + N.h1.a.k, e->G() + N.h1.g.k, e->G() + N.h1.a.b, e->G() + N.h1.g.b, st,
@@ -850,7 +879,7 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
     return 0;
   }
   PostBwdParams q = post_bwd_params(e, N.h1, dy, A.h1, n, Hs[0] * Ws[0], S, wgrad, true, PlanePair{S.dPhi, S.dPlo});
-  CK(launch_post_bwd(q, st));
+  CK(launch_post_bwd(q, e->opt.post, st));
   if (wgrad) {
     GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
     CK(launch_wgrad_c1(g, A.x, S.dP, 256, 256, e->G() + N.h1.a.k, e->G() + N.h1.g.k, 128, nullptr, nullptr, st, det_of(S)));
@@ -901,7 +930,7 @@ static void plan_train(cgvc_engine* e, Bump& ws, TrainPlan& P, int B, int T) {
     if (pl) { L.S.dPbhi = ws.take<__nv_bfloat16>(dp); L.S.dPblo = ws.take<__nv_bfloat16>(dp); }
     L.S.sq = &e->sideq[l];
     L.S.det = DetSlab{nullptr, 0};
-    if (e->deterministic) {
+    if (e->opt.deterministic) {
       // the weight-gradient partials are capped by CGVC_DET_SLAB_FLOATS (launch_tn lowers the split); the GLU / instance-norm bias partials,
       // one row of 2 x (conv columns) per 32 positions of a sample, grow with the batch and stay below dp / 8
       const long long slab = CGVC_DET_SLAB_FLOATS > (long long)(dp / 8) ? CGVC_DET_SLAB_FLOATS : (long long)(dp / 8);
@@ -925,7 +954,7 @@ static size_t work_bytes_needed(cgvc_engine* e) {
   plan_generator(e, ws, F.g, e->cfg.max_batch, e->cfg.max_frames);
   plan_discriminator(e, ws, F.d, e->cfg.max_batch, e->cfg.max_frames);
   if (ws.off > need) need = ws.off;
-  if (e->deterministic) {                     // the per-kernel entry points' slab (plan_entry_det)
+  if (e->opt.deterministic) {                 // the per-kernel entry points' slab (plan_entry_det)
     ws.reset(nullptr, 0); ws.take<float>((size_t)CGVC_DET_SLAB_FLOATS);
     if (ws.off > need) need = ws.off;
   }
@@ -936,7 +965,7 @@ static size_t work_bytes_needed(cgvc_engine* e) {
 // null outside deterministic mode; CGVC_ERR_UNBOUND when WORK is missing or too small
 static int plan_entry_det(cgvc_engine* e, DetSlab* slab, const DetSlab** det) {
   *det = nullptr;
-  if (!e->deterministic) return 0;
+  if (!e->opt.deterministic) return 0;
   if (!e->arena[CGVC_ARENA_WORK]) return fail(e, CGVC_ERR_UNBOUND, "deterministic mode needs the WORK arena bound");
   Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
   *slab = DetSlab{ws.take<float>((size_t)CGVC_DET_SLAB_FLOATS), CGVC_DET_SLAB_FLOATS};
@@ -1044,9 +1073,9 @@ int cgvc_destroy(cgvc_handle e) {
     if (e->sideq[l].side) cudaStreamDestroy(e->sideq[l].side);
     for (int b = 0; b < 2; ++b) { if (e->sideq[l].ready[b]) cudaEventDestroy(e->sideq[l].ready[b]); if (e->sideq[l].done[b]) cudaEventDestroy(e->sideq[l].done[b]); }
   }
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-  e->graphs.clear();
+  drop_graphs(e);
   if (e->stage) cudaFree(e->stage);
+  cudaFree(e->post_buf);
   if (e->graph_stream) cudaStreamDestroy(e->graph_stream);
   if (e->ev_bridge) cudaEventDestroy(e->ev_bridge);
   if (e->ev_bridge2) cudaEventDestroy(e->ev_bridge2);
@@ -1070,8 +1099,7 @@ int cgvc_bind_arena(cgvc_handle e, int arena, void* p, size_t bytes) {
   if (!p || bytes < need) return fail(e, CGVC_ERR_UNBOUND, "arena %d needs %zu bytes, got %zu", arena, need, bytes);
   if ((uintptr_t)p & 255) return fail(e, CGVC_ERR_ARG, "arena %d must be 256-byte aligned", arena);
   e->arena[arena] = p; e->arena_bytes[arena] = bytes;
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);   // captured graphs hold the old addresses
-  e->graphs.clear();
+  drop_graphs(e);
   return 0;
 }
 
@@ -1113,7 +1141,7 @@ int cgvc_params_updated(cgvc_handle e, void* stream) {
 int cgvc_set_adam_step(cgvc_handle e, long long t) {
   if (!e || t < 0) return CGVC_ERR_ARG;
   e->adam_t = t;
-  if (e->ls_mode == 2) {
+  if (e->opt.ls_mode == 2) {
     DeviceGuard dguard; CK(dguard.set(e->cfg.device));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(&e->ls->t, &t, sizeof t, cudaMemcpyHostToDevice));
@@ -1122,7 +1150,7 @@ int cgvc_set_adam_step(cgvc_handle e, long long t) {
 }
 int cgvc_get_adam_step(cgvc_handle e, long long* t) {
   if (!e || !t) return CGVC_ERR_ARG;
-  if (e->ls_mode == 2) {
+  if (e->opt.ls_mode == 2) {
     DeviceGuard dguard; CK(dguard.set(e->cfg.device));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(&e->adam_t, &e->ls->t, sizeof e->adam_t, cudaMemcpyDeviceToHost));
@@ -1171,9 +1199,10 @@ int cgvc_generator_forward(cgvc_handle e, int direction, const float* in_dev, fl
   FwdPlan F; F.in_cl = ws.take<float>((size_t)batch * e->cfg.num_features * frames);
   plan_generator(e, ws, F.g, batch, frames);
   if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
+  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &F.g.post));
   CK(launch_transpose_ft(in_dev, F.in_cl, batch, e->cfg.num_features, frames, st));
-  if (!e->debug_taps) e->taps.clear();
-  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->debug_taps != 0, false));
+  if (!e->opt.debug_taps) e->taps.clear();
+  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->opt.debug_taps != 0, false));
   CK(launch_transpose_ft(F.g.out_cl, out_dev, batch, frames, e->cfg.num_features, st));
   return 0;
 }
@@ -1205,10 +1234,11 @@ int cgvc_generator_forward_packed(cgvc_handle e, int direction, const float* in_
   long long* off_dev = ws.take<long long>((size_t)n + 1);    // (inside the discriminator's share of the plan)
   if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
   F.g.off = off_dev; F.g.max_len = (int)max_len;
+  CK(grow_post_buf(e, (size_t)n * 4 * 1024, &F.g.post));
   CK(cudaMemcpyAsync(off_dev, offsets_host, ((size_t)n + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
   CK(launch_transpose_packed(in_dev, F.in_cl, off_dev, n, rows, nf, 1, st));
-  if (!e->debug_taps) e->taps.clear();
-  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->debug_taps != 0, false));
+  if (!e->opt.debug_taps) e->taps.clear();
+  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->opt.debug_taps != 0, false));
   CK(launch_transpose_packed(F.g.out_cl, out_dev, off_dev, n, rows, nf, 0, st));
   return 0;
 }
@@ -1226,6 +1256,7 @@ int cgvc_discriminator_forward(cgvc_handle e, int which, const float* in_dev, fl
   plan_generator(e, ws, F.g, batch, frames);   // keep layout identical to work_bytes_needed
   plan_discriminator(e, ws, F.d, batch, frames);
   if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
+  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &F.d.post));
   RET(discriminator_forward(e, e->disc[which], F.d, in_dev, st, true));
   CK(cudaMemcpyAsync(out_dev, F.d.prob, (size_t)batch * (e->cfg.num_features / 4) * (frames / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
@@ -1313,7 +1344,7 @@ static int forward_backward(cgvc_engine* e, const float* A_dev, const float* B_d
   float* sc = e->d_scalars; float* L = sc + 8;
   (void)lc;                                                  // lambdas are already in d_scalars[0..1] (set_step_scalars)
   CK(cudaMemsetAsync(L, 0, 8 * sizeof(float), st));
-  if (e->ls_mode) CK(cudaMemsetAsync(&e->ls->nonfinite, 0, (char*)(&e->ls->sat_act + 1) - (char*)&e->ls->nonfinite, st));   // this step's counters
+  if (e->opt.ls_mode) CK(cudaMemsetAsync(&e->ls->nonfinite, 0, (char*)(&e->ls->sat_act + 1) - (char*)&e->ls->nonfinite, st));   // this step's counters
   struct Counting { cgvc_engine* e; ~Counting() { e->counting = false; } } counting{e};
   e->counting = true;
   CK(cudaMemsetAsync(e->G(), 0, e->n_params * sizeof(float), st));
@@ -1324,10 +1355,10 @@ static int forward_backward(cgvc_engine* e, const float* A_dev, const float* B_d
   CK(cudaMemcpyAsync(P.lane[1].in + img, P.lane[0].in, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
   for (int l = 0; l < 2; ++l) {
     SideQ& q = e->sideq[l];
-    q.on = e->side_wgrad && e->two_streams && !e->fuse_bwd && !e->deterministic && !tc_profile_is_on() && q.side != nullptr;
+    q.on = e->opt.side_wgrad && e->opt.two_streams && !e->opt.fuse_bwd && !e->opt.deterministic && !tc_profile_is_on() && q.side != nullptr;
     q.used[0] = q.used[1] = false; q.cur = 0;
   }
-  if (e->two_streams) {
+  if (e->opt.two_streams) {
     // fork
     CK(cudaEventRecord(e->ev_fork, st));
     for (int l = 0; l < 2; ++l) CK(cudaStreamWaitEvent(e->lane_stream[l], e->ev_fork, 0));
@@ -1384,19 +1415,19 @@ static int ls_check_grads(cgvc_engine* e, cudaStream_t st) {
   return 0;
 }
 static int ls_update(cgvc_engine* e, cudaStream_t st) {
-  CK(launch_loss_scale_update(e->ls, e->d_scalars + 2, e->cfg.precision == CGVC_PREC_F16F8, e->ls_growth, ADAM_B1, ADAM_B2, st));
+  CK(launch_loss_scale_update(e->ls, e->d_scalars + 2, e->cfg.precision == CGVC_PREC_F16F8, e->opt.ls_growth, ADAM_B1, ADAM_B2, st));
   return 0;
 }
-static const int* ls_skip(const cgvc_engine* e) { return e->ls_mode == 2 ? &e->ls->last_skipped : nullptr; }
+static const int* ls_skip(const cgvc_engine* e) { return e->opt.ls_mode == 2 ? &e->ls->last_skipped : nullptr; }
 
 // Before a step is enqueued: dynamic mode starts from the static scale of the step's batch unless the caller set one
 // (cgvc_set_loss_scale_state); monitor mode reports the static scale in use
 static int ls_prepare(cgvc_engine* e, int batch, cudaStream_t st) {
-  const bool dyn = e->ls_mode == 2 && !e->ls_ready, mon = e->ls_mode == 1 && e->ls_batch != batch;
+  const bool dyn = e->opt.ls_mode == 2 && !e->ls_ready, mon = e->opt.ls_mode == 1 && e->ls_batch != batch;
   if (!dyn && !mon) return 0;
   const float v[6] = {loss_scale(e, batch), 0, 0, 0, 0, 0};
   CK(launch_set_scalars(&e->ls->scale, 0, 1, v, st));
-  e->ls_ready = e->ls_mode == 2; e->ls_batch = e->ls_mode == 1 ? batch : 0;
+  e->ls_ready = e->opt.ls_mode == 2; e->ls_batch = e->opt.ls_mode == 1 ? batch : 0;
   return 0;
 }
 
@@ -1405,7 +1436,7 @@ static int ls_prepare(cgvc_engine* e, int batch, cudaStream_t st) {
 // so a replay is exact.  Capture needs a non-legacy stream: work arriving on the legacy default stream is bridged with events.
 template <class Body>
 static int run_captured(cgvc_engine* e, const GraphKey& key, cudaStream_t user, Body body) {
-  if (!e->use_graphs || tc_profile_is_on()) return body(user);
+  if (!e->opt.use_graphs || tc_profile_is_on()) return body(user);
   cudaStream_t st = user;
   const bool bridge = (user == nullptr || user == cudaStreamLegacy || user == cudaStreamPerThread);
   if (bridge) { st = e->graph_stream; CK(cudaEventRecord(e->ev_bridge, user)); CK(cudaStreamWaitEvent(st, e->ev_bridge, 0)); }
@@ -1413,11 +1444,11 @@ static int run_captured(cgvc_engine* e, const GraphKey& key, cudaStream_t user, 
   GraphEntry ent{nullptr, 0};
   if (it != e->graphs.end()) ent = it->second;
   else {
-    if (e->graphs.size() >= 16) { for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec); e->graphs.clear(); }
+    if (e->graphs.size() >= 16) drop_graphs(e);
     cudaGraph_t graph = nullptr;
     const unsigned long long before = g_cgvc_launches;
     cudaError_t ce = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-    if (ce != cudaSuccess) { cudaGetLastError(); e->use_graphs = 0; return body(user); }
+    if (ce != cudaSuccess) { cudaGetLastError(); e->opt.use_graphs = 0; return body(user); }
     int rc = body(st);
     ce = cudaStreamEndCapture(st, &graph);
     ent.launches = g_cgvc_launches - before;                 // kernels recorded, not run: counted per replay below
@@ -1426,12 +1457,12 @@ static int run_captured(cgvc_engine* e, const GraphKey& key, cudaStream_t user, 
       if (graph) cudaGraphDestroy(graph);
       cudaGetLastError();
       if (rc != 0 && ce == cudaSuccess) return rc;           // the body itself refused (bad argument, arena too small): not a capture problem
-      e->use_graphs = 0;                                     // fall back to eager launches for the rest of this engine's life
+      e->opt.use_graphs = 0;                                     // fall back to eager launches for the rest of this engine's life
       return body(user);
     }
     ce = cudaGraphInstantiate(&ent.exec, graph, 0);
     cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) { cudaGetLastError(); e->use_graphs = 0; return body(user); }
+    if (ce != cudaSuccess) { cudaGetLastError(); e->opt.use_graphs = 0; return body(user); }
     e->graphs[key] = ent;
   }
   cudaGraphExec_t exec = ent.exec;
@@ -1464,7 +1495,7 @@ int cgvc_compute_gradients(cgvc_handle e, const float* A_dev, const float* B_dev
   RET(ls_prepare(e, batch, (cudaStream_t)stream));
   RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, (cudaStream_t)stream));
   // the gradients are handed out, not fed to Adam: remove the loss scale here (in dynamic mode the device scale they were formed with)
-  if (e->ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
+  if (e->opt.ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
   else if (loss_scale(e, batch) != 1.f) CK(launch_scale(e->G(), (long long)e->n_params, 1.f / loss_scale(e, batch), (cudaStream_t)stream));
   return 0;
 }
@@ -1475,12 +1506,12 @@ int cgvc_adam_step(cgvc_handle e, float lr_g, float lr_d, float grad_scale, void
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   // dynamic loss-scale mode keeps t on the device: bring it to the host (synchronises), step with the host's lr_t like the other
   // modes, and write the advanced t back (synchronises again).  No skip: the caller decides on this step
-  if (e->ls_mode == 2) { long long t; RET(cgvc_get_adam_step(e, &t)); }
+  if (e->opt.ls_mode == 2) { long long t; RET(cgvc_get_adam_step(e, &t)); }
   const long long t_before = e->adam_t;
   RET(set_adam_scalars(e, lr_g, lr_d, grad_scale, (cudaStream_t)stream));
   int r = adam_body(e, (cudaStream_t)stream);
   if (r != 0) { e->adam_t = t_before; return r; }
-  if (e->ls_mode == 2) RET(cgvc_set_adam_step(e, e->adam_t));
+  if (e->opt.ls_mode == 2) RET(cgvc_set_adam_step(e, e->adam_t));
   return 0;
 }
 
@@ -1498,9 +1529,9 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
   // capture failure, NCCL error) must not change the bias correction of the next one
   const long long adam_t_before = e->adam_t;
   struct Rollback { cgvc_engine* e; long long t; bool armed; ~Rollback() { if (armed) e->adam_t = t; } } rollback{e, adam_t_before, true};
-  RET(set_adam_scalars(e, lr_g, lr_d, e->ls_mode == 2 ? (e->comm ? 1.f / (float)e->nranks : 1.f) : gscale, st, e->ls_mode == 2));
+  RET(set_adam_scalars(e, lr_g, lr_d, e->opt.ls_mode == 2 ? (e->comm ? 1.f / (float)e->nranks : 1.f) : gscale, st, e->opt.ls_mode == 2));
   RET(ls_prepare(e, batch, st));
-  if (e->use_graphs && !tc_profile_is_on()) {
+  if (e->opt.use_graphs && !tc_profile_is_on()) {
     // the graphs read the inputs from fixed staging buffers and leave the results in the WORK arena / d_scalars, so one
     // captured graph serves any caller pointers; the copies either side are eager
     const size_t img = (size_t)batch * e->cfg.num_features * frames;
@@ -1510,8 +1541,7 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
     CK(cudaMemcpyAsync(sA, A_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CK(cudaMemcpyAsync(sB, B_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
     GraphKey key; memset(&key, 0, sizeof key);
-    key.batch = batch; key.frames = frames; key.id_off = lambda_identity == 0.f; key.lanes = e->two_streams; key.fuse = e->fuse_in | (e->fuse_bwd << 1) | (e->side_wgrad << 2) | (e->fuse_c1 << 3) | (e->edge_lower << 4) |
-               (e->deterministic << 5); key.kind = 0;
+    key.batch = batch; key.frames = frames; key.id_off = lambda_identity == 0.f; key.kind = 0;
     RET(run_captured(e, key, st, [&](cudaStream_t s) {
       return forward_backward(e, sA, sB, batch, frames, lambda_cycle, lambda_identity, nullptr, nullptr, nullptr, s);
     }));
@@ -1525,7 +1555,7 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
   } else {
     RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, st));
   }
-  if (e->comm && e->pipelined_comm && e->comm_stream) {
+  if (e->comm && e->opt.pipelined_comm && e->comm_stream) {
     // one all-reduce per network (arena order), all enqueued on the communication stream behind the step's gradients; the caller's
     // stream then takes the networks one by one: wait for its all-reduce, Adam over its range, refresh of its tensor-core planes
     // the four networks in arena order; every tensor starts on a 16-byte boundary, so the ranges are cut at the aligned start of each
@@ -1541,16 +1571,16 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
       if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
       CK(cudaEventRecord(e->ev_ar[k], e->comm_stream));
     }
-    if (e->ls_mode) {
+    if (e->opt.ls_mode) {
       // every rank takes the same decision: the saturation counts are summed like the gradients (the GRAD check after the sum is
       // consistent by construction), and in dynamic mode each network's Adam waits for the scaler
-      if (e->ls_mode == 2) {
+      if (e->opt.ls_mode == 2) {
         int r = e->nccl.AllReduce(&e->ls->sat_grad, &e->ls->sat_grad, 1, 5, 0, e->comm, e->comm_stream);     // ncclUint64, ncclSum
         if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
       }
       RET(ls_check_grads(e, e->comm_stream));
       CK(cudaEventRecord(e->ev_ls, e->comm_stream));
-      if (e->ls_mode == 2) { CK(cudaStreamWaitEvent(st, e->ev_ls, 0)); RET(ls_update(e, st)); }
+      if (e->opt.ls_mode == 2) { CK(cudaStreamWaitEvent(st, e->ev_ls, 0)); RET(ls_update(e, st)); }
     }
     float* pp = e->P(); float* gg = e->G(); float* mm = (float*)e->arena[CGVC_ARENA_ADAM_M]; float* vv = (float*)e->arena[CGVC_ARENA_ADAM_V];
     for (int k = 0; k < 4; ++k) {
@@ -1566,21 +1596,21 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
         return 0;
       }));
     }
-    if (e->ls_mode == 1) CK(cudaStreamWaitEvent(st, e->ev_ls, 0));
+    if (e->opt.ls_mode == 1) CK(cudaStreamWaitEvent(st, e->ev_ls, 0));
     rollback.armed = false;
     return 0;
   }
   if (e->comm) {
     RET(cgvc_allreduce_grads(e, stream));
-    if (e->ls_mode == 2) {
+    if (e->opt.ls_mode == 2) {
       int r = e->nccl.AllReduce(&e->ls->sat_grad, &e->ls->sat_grad, 1, 5, 0, e->comm, st);                      // ncclUint64, ncclSum
       if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
     }
   }
   GraphKey k2; memset(&k2, 0, sizeof k2); k2.kind = 1;
   RET(run_captured(e, k2, st, [&](cudaStream_t s) {
-    if (e->ls_mode) RET(ls_check_grads(e, s));
-    if (e->ls_mode == 2) RET(ls_update(e, s));
+    if (e->opt.ls_mode) RET(ls_check_grads(e, s));
+    if (e->opt.ls_mode == 2) RET(ls_update(e, s));
     return adam_body(e, s, ls_skip(e));
   }));
   rollback.armed = false;
@@ -1640,67 +1670,42 @@ int cgvc_allreduce_grads(cgvc_handle e, void* stream) {
   return 0;
 }
 
+// Every option: its name, valid range and home.  A flag (range [0, 1]) takes any value, non-zero meaning 1
+struct OptionDef { const char* name; int lo, hi; int* (*field)(cgvc_engine*); };
+#define OPT(name, lo, hi, member) {name, lo, hi, [](cgvc_engine* e) { return &e->member; }}
+static const OptionDef kOptions[] = {
+  OPT("two_streams", 0, 1, opt.two_streams),        OPT("fuse_in", 0, 1, opt.fuse_in),
+  OPT("fuse_bwd", 0, 1, opt.fuse_bwd),              OPT("edge_lower", 0, 1, opt.edge_lower),
+  OPT("side_wgrad", 0, 1, opt.side_wgrad),          OPT("deterministic", 0, 1, opt.deterministic),
+  OPT("pipelined_comm", 0, 1, opt.pipelined_comm),  OPT("fuse_c1", 0, 1, opt.fuse_c1),
+  OPT("debug_taps", 0, 1, opt.debug_taps),          OPT("cuda_graph", 0, 1, opt.use_graphs),
+  OPT("post_onepass", 0, 1, opt.post.onepass),      OPT("post_stream", 0, 1, opt.post.stream),
+  OPT("loss_scale", 0, 2, opt.ls_mode),             OPT("loss_scale_growth_interval", 1, INT_MAX, opt.ls_growth),
+  OPT("wgrad_f16", 0, 1, tcw.wgrad16),              OPT("prep_batched", 0, 1, tcw.prep_batched),
+  OPT("tc_debug", 0, 7, tcw.debug),
+};
+#undef OPT
+
 int cgvc_set_option(cgvc_handle e, const char* name, int value) {
   if (!e || !name) return CGVC_ERR_ARG;
-  if (!strcmp(name, "two_streams")) { e->two_streams = value != 0; return 0; }
-  if (!strcmp(name, "fuse_in")) { e->fuse_in = value != 0; return 0; }
-  if (!strcmp(name, "fuse_bwd")) { e->fuse_bwd = value != 0; return 0; }
-  if (!strcmp(name, "edge_lower")) { e->edge_lower = value != 0; return 0; }
-  if (!strcmp(name, "side_wgrad")) { e->side_wgrad = value != 0; return 0; }
-  if (!strcmp(name, "deterministic")) {
-    // changes the WORK plan (cgvc_arena_bytes): the caller re-binds a larger arena after switching it on.  The captured steps hold
-    // the slab addresses of the old plan (GraphKey carries the mode as well)
-    e->deterministic = value != 0;
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-    e->graphs.clear();
-    return 0;
+  const OptionDef* d = nullptr;
+  for (const OptionDef& o : kOptions) if (!strcmp(o.name, name)) d = &o;
+  if (!d) return fail(e, CGVC_ERR_ARG, "unknown option '%s'", name);
+  if (d->lo == 0 && d->hi == 1) value = value != 0;
+  if (value < d->lo || value > d->hi) return fail(e, CGVC_ERR_ARG, "option %s: bad value %d", name, value);
+  int* field = d->field(e);
+  if (*field == value) return 0;
+  if (field == &e->opt.ls_mode) {
+    DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+    long long t = 0;
+    RET(cgvc_get_adam_step(e, &t));                          // the step count moves between host and device with the mode
+    e->opt.ls_mode = value;
+    RET(cgvc_set_adam_step(e, t));
+    e->ls_ready = false; e->ls_batch = 0;
   }
-  if (!strcmp(name, "pipelined_comm")) { e->pipelined_comm = value != 0; return 0; }
-  if (!strcmp(name, "fuse_c1")) { e->fuse_c1 = value != 0; return 0; }
-  if (!strcmp(name, "debug_taps")) { e->debug_taps = value != 0; return 0; }
-  if (!strcmp(name, "cuda_graph")) { e->use_graphs = value != 0; return 0; }
-  if (!strcmp(name, "tc_debug")) { tc_set_debug(value); return 0; }
-  if (!strcmp(name, "post_onepass")) {                       // process-wide, like prep_batched
-    post_set_onepass(value);
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-    e->graphs.clear();
-    return 0;
-  }
-  if (!strcmp(name, "wgrad_f16")) {                          // F16F8 only: weight gradients from the fp16 planes alone
-    e->tcw.wgrad16 = value != 0;
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-    e->graphs.clear();
-    return 0;
-  }
-  if (!strcmp(name, "loss_scale") || !strcmp(name, "loss_scale_growth_interval")) {
-    const bool mode = !strcmp(name, "loss_scale");
-    if (mode ? (value < 0 || value > 2) : value < 1) return fail(e, CGVC_ERR_ARG, "option %s: bad value %d", name, value);
-    if (mode && value != e->ls_mode) {
-      DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-      long long t = 0;
-      RET(cgvc_get_adam_step(e, &t));                        // the step count moves between host and device with the mode
-      e->ls_mode = value;
-      RET(cgvc_set_adam_step(e, t));
-      e->ls_ready = false; e->ls_batch = 0;
-    }
-    if (!mode) e->ls_growth = value;
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);   // the captured steps hold the mode's pointers and the interval
-    e->graphs.clear();
-    return 0;
-  }
-  if (!strcmp(name, "post_stream")) {                        // process-wide, like post_onepass
-    post_set_stream(value);
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-    e->graphs.clear();
-    return 0;
-  }
-  if (!strcmp(name, "prep_batched")) {                       // process-wide; the captured Adam + refresh graphs hold the old kernels
-    tc_set_prep_batched(value);
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-    e->graphs.clear();
-    return 0;
-  }
-  return fail(e, CGVC_ERR_ARG, "unknown option '%s'", name);
+  *field = value;
+  drop_graphs(e);
+  return 0;
 }
 int cgvc_kernel_launches(unsigned long long* count) { if (!count) return CGVC_ERR_ARG; *count = g_cgvc_launches; return 0; }
 int cgvc_profile_enable(int on) { tc_profile_enable(on); return 0; }
@@ -1745,7 +1750,7 @@ int cgvc_conv_forward(cgvc_handle e, int precision, const float* x, const float*
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   if (precision != CGVC_PREC_FP32_SIMT)
-    return tc_result(e, tc_conv_fwd_adhoc(precision, x, w, bias, y, B, H, W, Cin, kh, kw, Cout, sh, sw, st), nullptr, "conv forward");
+    return tc_result(e, tc_conv_fwd_adhoc(precision, e->tcw.debug, x, w, bias, y, B, H, W, Cin, kh, kw, Cout, sh, sw, st), nullptr, "conv forward");
   GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
   GemmOperands op; memset(&op, 0, sizeof op);
   op.src = x; op.s_ld = Cin; op.C = Cin; op.w = w; op.w_ts = (long long)Cin * Cout; op.w_cs = Cout; op.w_ns = 1; op.N = Cout;
@@ -1763,7 +1768,7 @@ int cgvc_conv_backward(cgvc_handle e, int precision, const float* x, const float
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   if (precision != CGVC_PREC_FP32_SIMT)
-    return tc_result(e, tc_conv_bwd_adhoc(precision, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16 ? 1 : 0, det),
+    return tc_result(e, tc_conv_bwd_adhoc(precision, e->tcw.debug, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16, det),
                      nullptr, "conv backward");
   ConvW c; c.k = 0; c.b = 0; c.kh = kh; c.kw = kw; c.cin = Cin; c.cout = Cout;
   if (dx) RET(conv_dgrad_simt(e, w, c, sh, sw, B, H, W, dy, Cout, 0, dx, 0, st));
@@ -1819,7 +1824,8 @@ int cgvc_in_glu_forward_planes(cgvc_handle e, const float* p, const float* beta_
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.y_hi = (__nv_bfloat16*)hi; q.y_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
   }
-  CK(launch_post_fwd(q, (cudaStream_t)stream));
+  CK(grow_post_buf(e, (size_t)B * 4 * C, &q.scratch));
+  CK(launch_post_fwd(q, e->opt.post, (cudaStream_t)stream));
   return 0;
 }
 
@@ -1842,7 +1848,8 @@ int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, 
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
   }
-  CK(launch_post_bwd(q, (cudaStream_t)stream));
+  CK(grow_post_buf(e, (size_t)B * 4 * C, &q.scratch));
+  CK(launch_post_bwd(q, e->opt.post, (cudaStream_t)stream));
   return 0;
 }
 
@@ -1863,7 +1870,7 @@ int cgvc_conv_in_forward(cgvc_handle e, int precision, const float* x, const flo
   TcFuse f; memset(&f, 0, sizeof f);
   f.gamma_a = gamma_a; f.beta_a = beta_a; f.gamma_g = gamma_g; f.beta_g = beta_g;
   f.stats = stats; f.resid = resid; f.y = y; f.y_hi = (__nv_bfloat16*)hi; f.y_lo = (__nv_bfloat16*)lo;
-  return tc_result(e, tc_conv_in_fwd_adhoc(precision, x, w_a, w_g, b_a, b_g, f, p, B, W, Cin, kw, Cout, sw, shuffle, fuse, fused, (cudaStream_t)stream),
+  return tc_result(e, tc_conv_in_fwd_adhoc(precision, e->tcw.debug, e->opt.post, x, w_a, w_g, b_a, b_g, f, p, B, W, Cin, kw, Cout, sw, shuffle, fuse, fused, (cudaStream_t)stream),
                    nullptr, "conv + instance norm forward");
 }
 
@@ -1889,7 +1896,7 @@ int cgvc_conv_in_backward(cgvc_handle e, int precision, const float* dp, const f
   f.gamma_a = gamma_a; f.beta_a = beta_a; f.gamma_g = gamma_g; f.beta_g = beta_g;
   f.dp_hi = (__nv_bfloat16*)hi; f.dp_lo = (__nv_bfloat16*)lo;
   f.dbeta_a = dbeta_a; f.dgamma_a = dgamma_a; f.dbeta_g = dbeta_g; f.dgamma_g = dgamma_g;
-  return tc_result(e, tc_conv_in_bwd_adhoc(precision, dp, w_a, w_g, f, dx, accumulate, B, R, Cin, kw, Cout, fuse, fused, det, (cudaStream_t)stream),
+  return tc_result(e, tc_conv_in_bwd_adhoc(precision, e->tcw.debug, e->opt.post, dp, w_a, w_g, f, dx, accumulate, B, R, Cin, kw, Cout, fuse, fused, det, (cudaStream_t)stream),
                    nullptr, "conv data gradient + instance norm backward");
 }
 

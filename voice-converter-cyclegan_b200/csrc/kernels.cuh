@@ -176,14 +176,18 @@ struct PostParams {
   float* y;                             // [B,R,C] (may be null when only the planes are wanted)
   float* stats;                         // [B,4,C]: mean_a, rstd_a, mean_g, rstd_g (written if has_in)
   __nv_bfloat16 *y_hi, *y_lo;           // optional bf16 split planes of y for the tensor-core path
-  float* scratch;                       // [B,4,C] fp32 workspace for the instance-norm sums (null: internal buffer, single-stream use only)
+  float* scratch;                       // [B,4,C] fp32 workspace for the instance-norm sums (required when has_in)
   int qmode;                            // 1: the planes are F16F8 planes instead: y_hi = q16 [B*R*C halves], y_lo = q8hi [B*R*C bytes] followed by q8lo
   // packed variable-length samples (seg.off != null): sample b = view rows [seg.off[b] / seg.div, seg.off[b+1] / seg.div) of seg_rows
   // rows in all (the planes' extent is seg_rows * C); R = the longest sample (grid size).  launch_post_fwd only
   PackGeom seg; long long seg_rows;
   unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
 };
-cudaError_t launch_post_fwd(const PostParams& pp, cudaStream_t st);
+// Which forms of the kernels a launch may take (the engine's options "post_onepass" and "post_stream", include/cgvc.h).
+// onepass: samples of <= 64 positions take the one-pass backward kernel, else always sums + apply.  stream: the layer shapes that
+// have one take the streaming (cp.async double-buffered) form, the backward's only with onepass
+struct PostForms { int onepass, stream; };
+cudaError_t launch_post_fwd(const PostParams& pp, PostForms forms, cudaStream_t st);
 
 struct PostBwdParams {
   const float* dy1; const float* dy2;   // upstream gradient(s) [B,R,C]; dy2 may be null (summed if present)
@@ -197,14 +201,12 @@ struct PostBwdParams {
   float *dbeta_a, *dgamma_a, *dbeta_g, *dgamma_g;   // accumulated atomically (may be null when has_in == 0)
   float *dbias_a, *dbias_g;             // conv-bias gradients [Cc] = column sums of dp (accumulated atomically; may be null)
   int qmode;                            // 1: dp_hi / dp_lo are F16F8 planes (q16; q8hi followed by q8lo) with the activation-role scales
-  float* scratch;                       // [B,4,C] fp32 workspace (null: internal buffer, single-stream use only)
+  float* scratch;                       // [B,4,C] fp32 workspace (required when has_in)
   unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
   DetSlab det;                          // deterministic mode (det.p != null): the sums + apply form, parameter and bias gradients reduced in order
 };
-cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st);
-void post_set_stream(int on);      // 1 (default): gated layers without shuffle and 32 / 48 / 64 positions per sample take the streaming (cp.async double-buffered) form of it
+cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st);
 cudaError_t post_init_kernels();   // shared-memory opt-in of the streaming kernels (call once, outside any stream capture)
-void post_set_onepass(int on);     // 1 (default): samples of <= 64 positions take the one-pass backward kernel; 0: always sums + apply
 
 // ---- discriminator head: dense(1024->1) + sigmoid (module.py:211) and LSGAN loss (model.py:68-69,81-86)
 cudaError_t launch_head_fwd(const float* y, long long rows, int C, const float* w, const float* b, float* prob, cudaStream_t st);

@@ -603,26 +603,11 @@ post_apply_fwd_kernel(const __grid_constant__ PostParams q, const float* __restr
   }
 }
 
-// lazily grown device scratch for the per-(sample, channel) sums (single stream use)
-static float* g_post_scratch = nullptr;
-static size_t g_post_scratch_elems = 0;
-static cudaError_t post_scratch(size_t elems, float** out) {
-  if (elems > g_post_scratch_elems) {
-    if (g_post_scratch) cudaFree(g_post_scratch);
-    size_t want = elems < (size_t)(1 << 22) ? (size_t)(1 << 22) : elems * 2;
-    cudaError_t e = cudaMalloc(&g_post_scratch, want * sizeof(float));
-    if (e != cudaSuccess) { g_post_scratch = nullptr; g_post_scratch_elems = 0; return e; }
-    g_post_scratch_elems = want;
-  }
-  *out = g_post_scratch;
-  return cudaSuccess;
-}
-
 static bool post_aligned(const void* a, const void* b, const void* c, int ldp, int C, int Cc) {
   return ldp % 4 == 0 && C % 4 == 0 && Cc % 4 == 0 && ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
 }
 
-static bool post_fwd_stream_dispatch(const PostParams& pp, cudaStream_t st, cudaError_t* err);      // streaming one-pass form, further down
+static bool post_fwd_stream_dispatch(const PostParams& pp, bool stream, cudaStream_t st, cudaError_t* err);   // streaming one-pass form, further down
 
 // packed variable-length samples (PostParams::seg): one CTA column per sample, grid.y sized by the longest
 static cudaError_t launch_post_fwd_packed(const PostParams& pp, cudaStream_t st) {
@@ -630,8 +615,6 @@ static cudaError_t launch_post_fwd_packed(const PostParams& pp, cudaStream_t st)
   dim3 grid((pp.C + kPostChan - 1) / kPostChan, (pp.R + kPostRows - 1) / kPostRows, pp.B);
   float* scratch = pp.scratch;
   if (pp.has_in) {
-    cudaError_t e = cudaSuccess;
-    if (!scratch) { e = post_scratch((size_t)pp.B * 4 * pp.C, &scratch); if (e != cudaSuccess) return e; }
     ++g_cgvc_launches;
     if (pp.has_gate) post_stats_kernel<true, true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
     else post_stats_kernel<false, true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
@@ -642,17 +625,15 @@ static cudaError_t launch_post_fwd_packed(const PostParams& pp, cudaStream_t st)
   return cudaGetLastError();
 }
 
-cudaError_t launch_post_fwd(const PostParams& pp, cudaStream_t st) {
+cudaError_t launch_post_fwd(const PostParams& pp, PostForms forms, cudaStream_t st) {
   if (pp.B == 0) return cudaSuccess;
-  if (!post_aligned(pp.p, pp.y, pp.resid, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535) return cudaErrorInvalidValue;
+  if (!post_aligned(pp.p, pp.y, pp.resid, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535 || (pp.has_in && !pp.scratch))
+    return cudaErrorInvalidValue;
   if (pp.seg.off) return launch_post_fwd_packed(pp, st);
-  { cudaError_t se = cudaSuccess; if (post_fwd_stream_dispatch(pp, st, &se)) return se; }
+  { cudaError_t se = cudaSuccess; if (post_fwd_stream_dispatch(pp, forms.stream, st, &se)) return se; }
   dim3 grid((pp.C + kPostChan - 1) / kPostChan, (pp.R + kPostRows - 1) / kPostRows, pp.B);
   float* scratch = pp.scratch;
   if (pp.has_in) {
-    size_t n = (size_t)pp.B * 4 * pp.C;
-    cudaError_t e = cudaSuccess;
-    if (!scratch) { e = post_scratch(n, &scratch); if (e != cudaSuccess) return e; }
     ++g_cgvc_launches;
     if (pp.has_gate) post_stats_kernel<true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
     else post_stats_kernel<false><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
@@ -1282,10 +1263,6 @@ static cudaError_t launch_post_fwd_stream(const PostParams& pp, cudaStream_t st)
   return cudaGetLastError();
 }
 
-static int g_post_onepass = 1;
-void post_set_onepass(int on) { g_post_onepass = on != 0; }
-static int g_post_stream = 1;
-void post_set_stream(int on) { g_post_stream = on != 0; }
 #define STREAM_CONFIGS(X) X(32, 4, true) X(32, 4, false) X(16, 3, true) X(16, 4, true) X(8, 3, true) X(8, 4, true) X(4, 6, true)
 cudaError_t post_init_kernels() {
   cudaError_t e;
@@ -1307,8 +1284,8 @@ static cudaError_t launch_post_bwd_stream(const PostBwdParams& pp, cudaStream_t 
   post_bwd_stream_kernel<NQL, NRT, GATE><<<grid, 256, Cfg::SMEM, st>>>(pp, (int)items, cblocks);
   return cudaGetLastError();
 }
-static bool post_fwd_stream_dispatch(const PostParams& pp, cudaStream_t st, cudaError_t* err) {
-  if (!(pp.has_in && pp.has_gate && !pp.resid && g_post_stream && (pp.sh == 1 || pp.sh == 2) && pp.Cc == pp.C * pp.sh &&
+static bool post_fwd_stream_dispatch(const PostParams& pp, bool stream, cudaStream_t st, cudaError_t* err) {
+  if (!(pp.has_in && pp.has_gate && !pp.resid && stream && (pp.sh == 1 || pp.sh == 2) && pp.Cc == pp.C * pp.sh &&
         (long long)pp.B * (pp.C / 16) < (1ll << 30)))
     return false;
   const int R = pp.R, C = pp.C;
@@ -1321,8 +1298,8 @@ static bool post_fwd_stream_dispatch(const PostParams& pp, cudaStream_t st, cuda
   return false;
 }
 // the streaming kernel's configuration for a layer shape, if it has one
-static bool post_bwd_stream_dispatch(const PostBwdParams& pp, cudaStream_t st, cudaError_t* err) {
-  if (!(pp.has_in && g_post_onepass && g_post_stream && !pp.dy2 && pp.stats && (pp.sh == 1 || pp.sh == 2) && pp.Cc == pp.C * pp.sh &&
+static bool post_bwd_stream_dispatch(const PostBwdParams& pp, PostForms forms, cudaStream_t st, cudaError_t* err) {
+  if (!(pp.has_in && forms.onepass && forms.stream && !pp.dy2 && pp.stats && (pp.sh == 1 || pp.sh == 2) && pp.Cc == pp.C * pp.sh &&
         (long long)pp.B * (pp.C / 16) < (1ll << 30)))
     return false;
   const int R = pp.R, C = pp.C;
@@ -1340,17 +1317,18 @@ static bool post_bwd_stream_dispatch(const PostBwdParams& pp, cudaStream_t st, c
 }
 
 
-cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st) {
+cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st) {
   if (pp.B == 0) return cudaSuccess;
-  if (!post_aligned(pp.p, pp.dy1, pp.dy2, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535) return cudaErrorInvalidValue;
+  if (!post_aligned(pp.p, pp.dy1, pp.dy2, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535 || (pp.has_in && !pp.scratch))
+    return cudaErrorInvalidValue;
   dim3 grid((pp.C + kPostChan - 1) / kPostChan, (pp.R + kPostRows - 1) / kPostRows, pp.B);
   // deterministic mode takes the sums + apply form: its per-sample sums are the parameter-gradient contributions, and its bias partials
   // go to one slab row per (sample, position block)
   const bool det = pp.det.p != nullptr;
   const bool det_bias = det && pp.dbias_a;
   if (det_bias && (long long)pp.B * grid.y * 2 * pp.Cc > pp.det.cap) return cudaErrorInvalidValue;
-  if (!det) { cudaError_t se = cudaSuccess; if (post_bwd_stream_dispatch(pp, st, &se)) return se; }
-  if (!det && pp.has_in && pp.R <= 64 && g_post_onepass) {
+  if (!det) { cudaError_t se = cudaSuccess; if (post_bwd_stream_dispatch(pp, forms, st, &se)) return se; }
+  if (!det && pp.has_in && pp.R <= 64 && forms.onepass) {
     ++g_cgvc_launches;
     const dim3 g1(grid.x, 1, grid.z);
 #define ONEPASS(NR_) do { if (pp.has_gate) post_bwd_onepass_kernel<true, NR_><<<g1, 256, 0, st>>>(pp); else post_bwd_onepass_kernel<false, NR_><<<g1, 256, 0, st>>>(pp); } while (0)
@@ -1360,9 +1338,6 @@ cudaError_t launch_post_bwd(const PostBwdParams& pp, cudaStream_t st) {
   }
   float* scratch = pp.scratch;
   if (pp.has_in) {
-    size_t n = (size_t)pp.B * 4 * pp.C;
-    cudaError_t e = cudaSuccess;
-    if (!scratch) { e = post_scratch(n, &scratch); if (e != cudaSuccess) return e; }
     ++g_cgvc_launches;
     if (pp.has_gate) post_bwd_sums_kernel<true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
     else post_bwd_sums_kernel<false><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);

@@ -160,7 +160,7 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   const __nv_bfloat16 *b_hi, *b_lo; int Nw;              // weights [slab][Nw][C]
   int N;                                                 // real output columns (stores are guarded; tiles cover Nw)
   int n_tiles;                                           // column tiles to compute (host: covers the real columns only)
-  int debug;                                             // diagnostic knobs (tc_set_debug): 1 = epilogue skips its global stores, 2 = also skips
+  int debug;                                             // diagnostic knobs (option "tc_debug", TcWeights::debug): 1 = epilogue skips its global stores, 2 = also skips
                                                          // the accumulator reads (the plain epilogue reads registers only: 2 acts as 1 there),
                                                          // 4 = producers skip the A gather.  Results are garbage; timing only.
   float* dst; int d_ld; const float* bias; int accumulate;
@@ -1441,8 +1441,6 @@ cudaError_t set_smem(K kernel, int bytes) {
 // ---- optional per-launch event timing (bench.py roofline): class 0 = NT (fwd/dgrad, plain epilogue), 1 = TN (wgrad),
 //      2 = NT with the fused instance-norm epilogue
 struct ProfRec { cudaEvent_t a, b; double flops; int cls; long long M; int N, K; };
-int g_tc_debug = 0;
-int g_tc_prep_batched = 1;    // F16F8 weight planes of all layers by prep_weights_q_all_kernel (one launch); 0: the per-layer kernels
 bool g_prof_on = false;
 std::vector<ProfRec> g_prof;
 void prof_begin(cudaStream_t st, double flops, int cls, long long M = 0, int N = 0, int K = 0) {
@@ -1477,7 +1475,6 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   dim3 grid((unsigned)(tiles < num_sms() ? tiles : num_sms()));
   cudaError_t e;
   ++g_cgvc_launches;
-  p.debug = g_tc_debug;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, (epi == 1 || epi == 2 || epi == 5) ? 2 : 0, M, p.N, p.g.ntaps * p.C);
 #define LAUNCH_NT(BN_, NPL_, EPI_, ...)                                                                        \
   do {                                                                                                         \
@@ -1648,7 +1645,7 @@ int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba,
 }
 
 // x planes: [n,H,W,cin_k] (channels beyond cin are zero)
-int layer_fwd(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
+int layer_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
               float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused_out = nullptr, const PackGeom* pk = nullptr) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   if (pk && (n != 1 || H != 1 || L.kh != 1 || fuse)) return (int)cudaErrorInvalidValue;
@@ -1659,7 +1656,7 @@ int layer_fwd(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const _
   p.b_hi = L.wf_hi; p.b_lo = L.wf_lo; p.Nw = nt_n(L); p.N = Ntot(L);
   p.dst = P; p.d_ld = Ntot(L); p.bias = L.bias; p.accumulate = 0;
   p.perm = layer_perm(L); p.Cc = L.cout;
-  p.tm_b_hi = L.tm_f_hi; p.tm_b_lo = L.tm_f_lo;
+  p.tm_b_hi = L.tm_f_hi; p.tm_b_lo = L.tm_f_lo; p.debug = debug;
   if (precision == 3) {
     // F16F8: x planes are [rows, cin_q] -- xhi = q16, xlo = q8hi followed by q8lo (kernels.cuh)
     if (!L.wq16) return TC_UNSUPPORTED;
@@ -1686,7 +1683,7 @@ int layer_fwd(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const _
 }
 
 // dP planes: [rows_out, nt_k]
-int layer_dgrad(const TcLayer& L, int precision, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
+int layer_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                 float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused_out = nullptr) {
   if (fused_out) *fused_out = false;
   if (!layer_ok(L) || (precision == 3 && (!layer_ok_q(L) || !L.wdq16))) return TC_UNSUPPORTED;     // F16F8 needs the data-gradient planes (training engines)
@@ -1704,7 +1701,7 @@ int layer_dgrad(const TcLayer& L, int precision, const __nv_bfloat16* dPhi, cons
     p.a_hi = dPhi; p.a_lo = dPlo; p.a_ld = nt_k(L); p.C = nt_k(L);
     p.b_hi = L.wd_hi; p.b_lo = L.wd_lo; p.Nw = cin_n(L); p.N = L.cin;
     p.dst = dx; p.d_ld = L.cin; p.bias = nullptr; p.accumulate = accumulate;
-    p.tm_b_hi = L.tm_d_hi; p.tm_b_lo = L.tm_d_lo;
+    p.tm_b_hi = L.tm_d_hi; p.tm_b_lo = L.tm_d_lo; p.debug = debug;
     if (precision == 3) {
       // F16F8: dP planes are [rows, nt_q] -- dPhi = q16, dPlo = q8hi followed by q8lo (activation-role scales); weights from the wdq planes
       p.a_ld = nt_q(L); p.C = nt_q(L); p.a_lo = nullptr;
@@ -1867,7 +1864,7 @@ static int refresh_jobs(TcWeights& w, const float* params, int j0, int j1, cudaS
 
 int tc_refresh_weights(TcWeights& w, const float* params, cudaStream_t st) {
   if (!w.pool) return 0;
-  const bool batched = g_tc_prep_batched && w.prep_jobs;
+  const bool batched = w.prep_batched && w.prep_jobs;
   for (TcLayer& L : w.layers) {
     if (batched && L.wq16) continue;
     int r = refresh_layer(L, params + L.ka, params + L.kg, params + L.ba, params + L.bg, st);
@@ -1881,7 +1878,7 @@ int tc_refresh_weights(TcWeights& w, const float* params, cudaStream_t st) {
 // the layers whose kernels live in [begin, end) of the parameter arena (one network)
 int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, size_t end, cudaStream_t st) {
   if (!w.pool) return 0;
-  const bool batched = g_tc_prep_batched && w.prep_jobs;
+  const bool batched = w.prep_batched && w.prep_jobs;
   for (TcLayer& L : w.layers) {
     if (L.ka < begin || L.ka >= end) continue;
     if (batched && L.wq16) continue;
@@ -1901,8 +1898,6 @@ int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, si
   return 0;
 }
 
-void tc_set_prep_batched(int v) { g_tc_prep_batched = v != 0; }
-
 cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st,
                             unsigned long long* sat) {
   return precision == 3 ? launch_pad_split_q(x, rows, C, C, ru(C, 128), hi, lo, st, sat) : launch_pad_split(x, rows, C, C, ru(C, 64), hi, lo, st);
@@ -1910,18 +1905,18 @@ cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C
 
 int tc_conv_fwd(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
                 float* P, cudaStream_t st, const TcFuse* fuse, bool* fused, const PackGeom* pk) {
-  return layer_fwd(w.layers[slot], w.precision, xhi, xlo, n, H, W, sh, sw, P, st, fuse, fused, pk);
+  return layer_fwd(w.layers[slot], w.precision, w.debug, xhi, xlo, n, H, W, sh, sw, P, st, fuse, fused, pk);
 }
 
 int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused) {
-  return layer_dgrad(w.layers[slot], w.precision, dPhi, dPlo, n, H, W, sh, sw, dx, accumulate, st, fuse, fused);
+  return layer_dgrad(w.layers[slot], w.precision, w.debug, dPhi, dPlo, n, H, W, sh, sw, dx, accumulate, st, fuse, fused);
 }
 
 int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dwa, float* dwg, cudaStream_t st, const DetSlab* det) {
-  return layer_wgrad(w.layers[slot], w.precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16 ? 1 : 0, det);
+  return layer_wgrad(w.layers[slot], w.precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16, det);
 }
 
 bool tc_profile_is_on() { return g_prof_on; }
@@ -1959,7 +1954,6 @@ int tc_profile_launches(double* ms, double* flops, long long* meta4, int capacit
   if (n_out) *n_out = n;
   return 0;
 }
-void tc_set_debug(int v) { g_tc_debug = v; }
 
 // ---- self-contained versions for the unit tests: fp32 in/out, temporary planes ----
 namespace {
@@ -1992,7 +1986,7 @@ static int adhoc_layer(Temp& T, TcLayer& L, cudaStream_t st) {
   return 0;
 }
 
-int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float* bias, float* y,
+int tc_conv_fwd_adhoc(int precision, int debug, const float* x, const float* w, const float* bias, float* y,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st) {
   TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
@@ -2008,11 +2002,11 @@ int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float
   r = refresh_layer(L, w, nullptr, bias ? bias : zero, nullptr, st); if (r) return r;
   cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
   if (e != cudaSuccess) return (int)e;
-  r = layer_fwd(L, precision, xhi, xlo, B, H, W, sh, sw, y, st); if (r) return r;
+  r = layer_fwd(L, precision, debug, xhi, xlo, B, H, W, sh, sw, y, st); if (r) return r;
   return (int)cudaStreamSynchronize(st);
 }
 
-int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
+int tc_conv_bwd_adhoc(int precision, int debug, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16, const DetSlab* det) {
   TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
@@ -2032,7 +2026,7 @@ int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float
   if (e != cudaSuccess) return (int)e;
   e = tc_split_planes(precision, dy, (long long)orows, Cout, ghi, glo, st);
   if (e != cudaSuccess) return (int)e;
-  if (dx) { r = layer_dgrad(L, precision, ghi, glo, B, H, W, sh, sw, dx, 0, st); if (r) return r; }
+  if (dx) { r = layer_dgrad(L, precision, debug, ghi, glo, B, H, W, sh, sw, dx, 0, st); if (r) return r; }
   if (dw) {
     r = layer_wgrad(L, precision, xhi, xlo, ghi, glo, B, H, W, sh, sw, dw, nullptr, st, w16, det); if (r) return r;
     if (dbias) { e = launch_colsum(dy, (long long)orows, Cout, 0, Cout, dbias, st, det); if (e != cudaSuccess) return (int)e; }
@@ -2053,7 +2047,7 @@ static int adhoc_layer_1d(Temp& T, TcLayer& L, int precision, const float* wa, c
   return refresh_layer(L, wa, wg, ba ? ba : zero, bg ? bg : zero, st);
 }
 
-int tc_conv_in_fwd_adhoc(int precision, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
+int tc_conv_in_fwd_adhoc(int precision, int debug, PostForms forms, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                          const TcFuse& fz, float* P, int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused,
                          cudaStream_t st) {
   if (fused) *fused = 0;
@@ -2070,7 +2064,7 @@ int tc_conv_in_fwd_adhoc(int precision, const float* x, const float* wa, const f
   bool have_p = false;
   if (fuse) {
     bool done = false;
-    r = layer_fwd(L, precision, xhi, xlo, B, 1, W, 1, sw, P, st, &f, &done);
+    r = layer_fwd(L, precision, debug, xhi, xlo, B, 1, W, 1, sw, P, st, &f, &done);
     if (r != 0 && (done || P)) return r;                 // a failed launch (not the missing P of a shape the epilogue refuses)
     if (done) { if (fused) *fused = 1; return (int)cudaStreamSynchronize(st); }
     have_p = P != nullptr;                                 // refused: P already holds the plain-epilogue output
@@ -2078,19 +2072,20 @@ int tc_conv_in_fwd_adhoc(int precision, const float* x, const float* wa, const f
   // the engine's fallback: the plain epilogue, then the instance-norm kernels
   float* Pw = P ? P : T.get<float>((size_t)B * Wo * Ntot(L));
   float* stats = fz.stats ? fz.stats : T.get<float>((size_t)B * 4 * (Cout / shuffle));
-  if (!Pw || !stats) return (int)cudaErrorMemoryAllocation;
-  if (!have_p) { r = layer_fwd(L, precision, xhi, xlo, B, 1, W, 1, sw, Pw, st); if (r) return r; }
+  float* scratch = T.get<float>((size_t)B * 4 * (Cout / shuffle));
+  if (!Pw || !stats || !scratch) return (int)cudaErrorMemoryAllocation;
+  if (!have_p) { r = layer_fwd(L, precision, debug, xhi, xlo, B, 1, W, 1, sw, Pw, st); if (r) return r; }
   PostParams q; memset(&q, 0, sizeof q);
   q.p = Pw; q.ldp = Ntot(L); q.Cc = Cout; q.B = B; q.sh = shuffle; q.R = Wo * shuffle; q.C = Cout / shuffle;
   q.has_in = 1; q.has_gate = L.gated;
   q.beta_a = fz.beta_a; q.gamma_a = fz.gamma_a; q.beta_g = fz.beta_g; q.gamma_g = fz.gamma_g; q.resid = fz.resid;
-  q.y = fz.y; q.stats = stats; q.y_hi = fz.y_hi; q.y_lo = fz.y_lo; q.qmode = precision == 3;
-  e = launch_post_fwd(q, st);
+  q.y = fz.y; q.stats = stats; q.y_hi = fz.y_hi; q.y_lo = fz.y_lo; q.qmode = precision == 3; q.scratch = scratch;
+  e = launch_post_fwd(q, forms, st);
   if (e != cudaSuccess) return (int)e;
   return (int)cudaStreamSynchronize(st);
 }
 
-int tc_conv_in_bwd_adhoc(int precision, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
+int tc_conv_in_bwd_adhoc(int precision, int debug, PostForms forms, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
                          int B, int R, int Cin, int kw, int Cout, int fuse, int* fused, const DetSlab* det, cudaStream_t st) {
   if (fused) *fused = 0;
   TcLayer L{};
@@ -2111,17 +2106,19 @@ int tc_conv_in_bwd_adhoc(int precision, const float* dP, const float* wa, const 
   }
   TcBwdFuse f = uf; f.R = R; f.bp_ld = f.dp_ld = (uf.gated ? 2 : 1) * Cin;
   bool done = false;
-  r = layer_dgrad(L, precision, ghi, glo, B, 1, R, 1, 1, dY, accumulate, st, fuse && !det ? &f : nullptr, &done);
+  r = layer_dgrad(L, precision, debug, ghi, glo, B, 1, R, 1, 1, dY, accumulate, st, fuse && !det ? &f : nullptr, &done);
   if (r) return r;
   if (done) { if (fused) *fused = 1; return (int)cudaStreamSynchronize(st); }
   // the engine's fallback: the plain data gradient above, then the instance-norm (+ GLU) backward kernels
+  float* scratch = T.get<float>((size_t)B * 4 * Cin);
+  if (!scratch) return (int)cudaErrorMemoryAllocation;
   PostBwdParams q; memset(&q, 0, sizeof q);
   if (det) q.det = *det;
   q.dy1 = dY; q.p = uf.bp; q.ldp = f.bp_ld; q.Cc = Cin; q.B = B; q.R = R; q.C = Cin; q.sh = 1;
   q.beta_a = uf.beta_a; q.gamma_a = uf.gamma_a; q.beta_g = uf.beta_g; q.gamma_g = uf.gamma_g; q.has_in = 1; q.has_gate = uf.gated;
   q.stats = uf.stats; q.dp_hi = uf.dp_hi; q.dp_lo = uf.dp_lo; q.qmode = precision == 3;
-  q.dbeta_a = uf.dbeta_a; q.dgamma_a = uf.dgamma_a; q.dbeta_g = uf.dbeta_g; q.dgamma_g = uf.dgamma_g;
-  e = launch_post_bwd(q, st);
+  q.dbeta_a = uf.dbeta_a; q.dgamma_a = uf.dgamma_a; q.dbeta_g = uf.dbeta_g; q.dgamma_g = uf.dgamma_g; q.scratch = scratch;
+  e = launch_post_bwd(q, forms, st);
   if (e != cudaSuccess) return (int)e;
   return (int)cudaStreamSynchronize(st);
 }

@@ -41,11 +41,15 @@ struct TcWeights {
   bool ready = false;
   int precision = 0;              // the engine's CGVC_PREC_* (set by tc_alloc): the operand planes every slot-based call reads and writes
   bool quant = false;             // also keep the F16F8 forward planes (precision F16F8)
-  bool wgrad16 = false;           // F16F8 only: weight gradients from the fp16 planes alone (one MMA unit per product instead of two)
   bool quant_bwd = false;         // ... and the F16F8 data-gradient planes (training in that precision)
   void* prep_jobs = nullptr;      // device job table of the batched F16F8 plane kernel (tc_gemm.cu PrepJob), one job per layer branch
   std::vector<int> job_first;     // first block of every job + total (size jobs + 1)
   std::vector<size_t> job_ka;     // PARAM offset of the job's layer (range filter of tc_refresh_weights_range)
+  // options of the engine that only this module reads (include/cgvc.h cgvc_set_option)
+  int wgrad16 = 0;                // "wgrad_f16" (F16F8 only; tc_alloc sets it there): weight gradients from the fp16 planes alone
+                                  // (one MMA unit per product instead of two)
+  int prep_batched = 1;           // "prep_batched": F16F8 weight planes of all layers in one launch; 0: per-layer kernels
+  int debug = 0;                  // "tc_debug": diagnostic knobs of the NT kernel (timing experiments only; see TcNTParams::debug)
 };
 
 // what the fused forward epilogue needs besides the convolution itself (see tc_conv_fwd)
@@ -103,22 +107,23 @@ int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_
 int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dwa, float* dwg, cudaStream_t st, const DetSlab* det = nullptr);   // det: deterministic mode (kernels.cuh DetSlab)
-// self-contained versions for unit tests (fp32 in/out, temporary planes allocated internally)
-int tc_conv_fwd_adhoc(int precision, const float* x, const float* w, const float* bias, float* y,
+// self-contained versions for unit tests (fp32 in/out, temporary planes allocated internally); debug, w16 and forms: the calling
+// engine's TcWeights::debug, TcWeights::wgrad16 and instance-norm kernel forms
+int tc_conv_fwd_adhoc(int precision, int debug, const float* x, const float* w, const float* bias, float* y,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st);
-int tc_conv_bwd_adhoc(int precision, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16 = 0,   // w16: F16F8 weight gradient from the fp16 planes alone
-                      const DetSlab* det = nullptr);
+int tc_conv_bwd_adhoc(int precision, int debug, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
+                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16,
+                      const DetSlab* det);
 // one generator layer as the engine runs it (include/cgvc.h cgvc_conv_in_forward): the 1-D convolution of x [B, W, Cin] (gated when wg
 // is given) and the instance norm of fz (fz.R is set here).  fuse: the fused epilogue where the shape allows (*fused = 1), else the
 // plain epilogue and launch_post_fwd; P may be null (inference: a temporary when the shape needs the fallback)
-int tc_conv_in_fwd_adhoc(int precision, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
+int tc_conv_in_fwd_adhoc(int precision, int debug, PostForms forms, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                          const TcFuse& fz, float* P, int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused,
                          cudaStream_t st);
 // the data gradient of a stride-1 1-D layer from fp32 dP [B*R, Ntot] with the upstream layer's instance-norm (+ GLU) backward uf
 // (uf.R, bp_ld and dp_ld are set here; include/cgvc.h cgvc_conv_in_backward): fused where the shape allows, else the plain data
 // gradient and launch_post_bwd.  det: deterministic mode (never fused)
-int tc_conv_in_bwd_adhoc(int precision, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
+int tc_conv_in_bwd_adhoc(int precision, int debug, PostForms forms, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
                          int B, int R, int Cin, int kw, int Cout, int fuse, int* fused, const DetSlab* det, cudaStream_t st);
 
 // per-launch CUDA-event timing of the tensor-core kernels (class 0 = forward/dgrad kernel with the plain epilogue,
@@ -127,5 +132,3 @@ void tc_profile_enable(int on);
 bool tc_profile_is_on();
 int tc_profile_collect(double ms[3], double flops[3], long long launches[3]);
 int tc_profile_launches(double* ms, double* flops, long long* meta4, int capacity, int* n_out);
-void tc_set_prep_batched(int v);   // 1 (default): F16F8 weight planes of all layers in one launch; 0: per-layer kernels
-void tc_set_debug(int v);     // diagnostic knobs of the NT kernel (timing experiments only; see TcNTParams::debug)
