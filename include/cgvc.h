@@ -327,6 +327,43 @@ int cgvc_conv_in_backward(cgvc_handle h, int precision, const float* dp, const f
                           const float* stats, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
                           float* dx, void* hi, void* lo, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
                           int B, int R, int Cin, int kw, int Cout, int gate, int accumulate, int fuse, int* fused, void* stream);
+/* The layers without an instance norm and the loss heads, as a train step runs them, so that they can be checked against float64
+ * (tests/test_gpu_glu_layers.py).  Planes and sat as cgvc_split_planes; precision CGVC_PREC_FP32_SIMT writes no planes (hi, lo, sat
+ * ignored).  The calls that add into their outputs from many CTAs honour the option "deterministic" (then WORK must be bound, as for
+ * cgvc_in_glu_backward).
+ * cgvc_glu_forward_planes: the gated form without instance norm (generator h1, discriminator h1): p [B, R, 2C] = [a | g],
+ *   y [B, R, C] = a * sigmoid(g) (y may be NULL when hi / lo are given).  C a multiple of 4, B <= 65535.
+ * cgvc_glu_backward_planes: dy [B, R, C], p as above -> dp [B, R, 2C] (= dy s(g), dy a s(g) (1 - s(g)); may be NULL when hi / lo are
+ *   given) and its planes; dbias_a, dbias_g [C] (both NULL or both given) += the column sums of dp. */
+int cgvc_glu_forward_planes(cgvc_handle h, const float* p, float* y, int B, int R, int C, int precision, void* hi, void* lo,
+                            unsigned long long* sat, void* stream);
+int cgvc_glu_backward_planes(cgvc_handle h, const float* dy, const float* p, float* dp, float* dbias_a, float* dbias_g, int B, int R, int C,
+                             int precision, void* hi, void* lo, unsigned long long* sat, void* stream);
+/* cgvc_disc_input_forward: the discriminator's input layer (one input channel, kh * kw <= 9 taps, Cout = 128, gate without instance norm;
+ *   module.py:196-203): x [B, H, W], w_a / w_g [kh, kw, 1, Cout], b_a / b_g [Cout], strides sh, sw, M = B * ceil(H / sh) * ceil(W / sw)
+ *   output rows.  p [M, 2 Cout] = [a | g] = conv(x) + bias (required: the backward pass reads it), y [M, Cout] = a * sigmoid(g) and
+ *   its planes (y may be NULL when hi / lo are given).  fuse = 1: one pass (option "fuse_c1", the default); 0: the convolution, then
+ *   the GLU kernels of cgvc_glu_forward_planes.  *fused (may be NULL) tells which ran.
+ * cgvc_disc_input_backward: dy [M, Cout], the saved p, x and the weights -> dw_a, dw_g [kh, kw, 1, Cout], db_a, db_g [Cout] (all four
+ *   NULL or all given, then accumulated) and dx [B, H, W] (NULL: no data gradient).  fuse = 1: dP is formed inside the weight-gradient
+ *   and data-gradient kernels; 0: the GLU backward writes an fp32 dP that they read. */
+int cgvc_disc_input_forward(cgvc_handle h, int precision, const float* x, const float* w_a, const float* w_g, const float* b_a, const float* b_g,
+                            float* p, float* y, void* hi, void* lo, unsigned long long* sat,
+                            int B, int H, int W, int kh, int kw, int Cout, int sh, int sw, int fuse, int* fused, void* stream);
+int cgvc_disc_input_backward(cgvc_handle h, const float* dy, const float* p, const float* x, const float* w_a, const float* w_g,
+                             float* dw_a, float* dw_g, float* db_a, float* db_g, float* dx,
+                             int B, int H, int W, int kh, int kw, int Cout, int sh, int sw, int fuse, int* fused, void* stream);
+/* cgvc_head_forward: the discriminator's dense head (module.py:211): prob[r] = sigmoid(y[r, :] . w + b[0]), y [rows, 1024].
+ * cgvc_head_loss_backward: the LSGAN loss of those probabilities (model.py:68-69,81-86): *loss += coef * mean((prob - target)^2) (loss
+ *   may be NULL); with dz = g coef 2 (prob - target) / rows * prob (1 - prob), g = *grad_mult (NULL: 1): dy [rows, 1024] = dz w (NULL:
+ *   not written), dw [1024] += sum dz y, db [1] += sum dz (both NULL or both given; then y is required).
+ * cgvc_l1_loss_grad: the L1 loss (utils.py:6-8): *loss += mean |yhat - y| over n elements (loss may be NULL); d[i] (+)= s sign(yhat[i] -
+ *   y[i]) with s = (*gscale / n) * *grad_mult (a NULL pointer stands for 1), added to d when accumulate (d NULL: not written). */
+int cgvc_head_forward(cgvc_handle h, const float* y, long long rows, const float* w, const float* b, float* prob, void* stream);
+int cgvc_head_loss_backward(cgvc_handle h, const float* prob, const float* y, long long rows, const float* w, float target, float coef,
+                            const float* grad_mult, float* loss, float* dy, float* dw, float* db, void* stream);
+int cgvc_l1_loss_grad(cgvc_handle h, const float* yhat, const float* y, long long n, const float* gscale, const float* grad_mult, float* loss,
+                      float* d, int accumulate, void* stream);
 
 /* error codes */
 enum {

@@ -559,7 +559,8 @@ def test_side_stream_weight_gradients_and_kernel_variants_match_default_path(big
         for k in opts:
             assert lib.cgvc_set_option(h, k, defaults[k]) == 0
     for name, _ in cases[1:]:
-        # the unfused discriminator input layer rounds dP into fp16 + e4m3 planes before the per-tap projection, the fused one keeps fp32;
+        # the unfused discriminator input layer writes its dP in fp32 (D.h1 has no tensor-core slot, so no planes) and sums its weight,
+        # bias and projection terms in another order than the fused kernels -- the only difference (test_gpu_glu_layers.py);
         # the three instance-norm backward forms add their per-sample sums in different orders, and in f16f8 a last-bit difference of a
         # dP element can land on the other side of a rounding boundary of its fp16 + e4m3 planes: the difference then travels down
         # the backward chain at the plane resolution (8e-5 measured at the generator's first layer; each form is within 3.6e-4 of the oracle)

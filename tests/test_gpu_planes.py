@@ -3,6 +3,8 @@
 a. Every counted plane writer (the pad-split, the tap im2col, the instance-norm / GLU kernels forward and backward in every dispatch
    form): each plane value equals the reference, and the saturation counter equals the reference count of cgvc_sat4 groups exactly --
    the count dynamic loss scaling trusts when it accepts a step.  A second call doubles the count; a NULL counter gives the same planes.
+   The two writers of the layers without an instance norm -- the GLU-only form's y and dP planes (generator h1) and the discriminator
+   input layer's y planes (conv_c1_glu_fwd) -- are checked by the same protocol in test_gpu_glu_layers.py.
 b. The F16F8 GEMMs against float64 with each operand scaled by powers of two: the window in which the planes are parity-grade.
 c. The train step's gradients at every loss scale the dynamic scaler can reach, against the float64 oracle.
 """

@@ -87,6 +87,13 @@ def _declare(lib):
         "cgvc_in_glu_backward_planes": (ci, [vp] * 13 + [ci] * 6 + [vp] * 4),
         "cgvc_conv_in_forward": (ci, [vp, ci] + [vp] * 15 + [ci] * 8 + [P(ci), vp]),
         "cgvc_conv_in_backward": (ci, [vp, ci] + [vp] * 16 + [ci] * 8 + [P(ci), vp]),
+        "cgvc_glu_forward_planes": (ci, [vp] * 3 + [ci] * 4 + [vp] * 4),
+        "cgvc_glu_backward_planes": (ci, [vp] * 6 + [ci] * 4 + [vp] * 4),
+        "cgvc_disc_input_forward": (ci, [vp, ci] + [vp] * 10 + [ci] * 9 + [P(ci), vp]),
+        "cgvc_disc_input_backward": (ci, [vp] * 11 + [ci] * 9 + [P(ci), vp]),
+        "cgvc_head_forward": (ci, [vp, vp, C.c_longlong, vp, vp, vp, vp]),
+        "cgvc_head_loss_backward": (ci, [vp, vp, vp, C.c_longlong, vp, cf, cf] + [vp] * 6),
+        "cgvc_l1_loss_grad": (ci, [vp, vp, vp, C.c_longlong] + [vp] * 4 + [ci, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the library does not export a declared symbol

@@ -799,21 +799,61 @@ static void plan_discriminator(cgvc_engine* e, Bump& ws, DiscActs& A, int n, int
   A.prob = ws.take<float>((size_t)r3);
 }
 
+// The discriminator's input layer (one input channel, <= 9 taps, gate without instance norm: module.py:196-203), its weights and
+// gradients by pointer, so that the walk and the test entry points (cgvc_disc_input_forward / _backward) run the same launches.
+struct C1Layer { const float *wa, *wg, *ba, *bg; int kh, kw, cout, sh, sw; };
+struct C1Grads { float *dwa, *dwg, *dba, *dbg; };      // all null: no weight gradient
+static C1Layer c1_layer(const cgvc_engine* e, const Layer& L) {
+  const float* Pm = e->P();
+  return C1Layer{Pm + L.a.k, Pm + L.g.k, Pm + L.a.b, Pm + L.g.b, L.a.kh, L.a.kw, L.a.cout, L.sh, L.sw};
+}
+
+// P [n * Ho * Wo, 2 cout] = [a | g] = conv(x [n, H, W]) + bias, and the GLU that q describes (q.p = P: y, its planes and their count).
+// fuse: convolution + GLU in one HBM-bound pass (P is written for the backward pass but not read back); else the convolution, then the
+// GLU-only post kernels
+static int disc_input_forward(cgvc_engine* e, const C1Layer& c, const float* x, int n, int H, int W, float* P, const PostParams& q, bool fuse,
+                              cudaStream_t st) {
+  const GatherGeom g = fwd_geom(n, H, W, c.kh, c.kw, c.sh, c.sw);
+  if (fuse) {
+    CK(launch_conv_c1_glu_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat));
+    return 0;
+  }
+  CK(launch_conv_c1_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, st));
+  CK(launch_post_fwd(q, e->opt.post, st));
+  return 0;
+}
+
+// Backward of the same layer from dy [n * Ho * Wo, cout] and the saved P: d's weight and bias gradients += (d.dwa null: none), dx [n, H, W]
+// = the data gradient (null: none), Z scratch [n * Ho * Wo, taps].  fuse: dP = (dy s(g), dy a s(g) (1 - s(g))) formed in registers inside
+// the weight-gradient and data-gradient kernels; else the GLU-only backward q (bias gradients included) writes the fp32 dP q.dp, which
+// wgrad_c1 and dgrad_c1 read.  det: deterministic mode's partials slab, else null
+static int disc_input_backward(cgvc_engine* e, const C1Layer& c, const C1Grads& d, const float* x, const float* dy, const float* P, int n, int H,
+                               int W, float* dx, float* Z, bool fuse, const PostBwdParams& q, const DetSlab* det, cudaStream_t st) {
+  const GatherGeom g = fwd_geom(n, H, W, c.kh, c.kw, c.sh, c.sw);
+  if (fuse) {
+    if (d.dwa) CK(launch_glu_bwd_wgrad_c1(g, x, dy, P, c.cout, d.dwa, d.dwg, d.dba, d.dbg, st, det));
+    if (dx) CK(launch_glu_bwd_dgrad_c1(dy, P, c.cout, c.wa, c.wg, Z, dx, n, H, W, c.kh, c.kw, c.sh, c.sw, st));
+    return 0;
+  }
+  CK(launch_post_bwd(q, e->opt.post, st));
+  if (d.dwa) CK(launch_wgrad_c1(g, x, q.dp, 2 * c.cout, 2 * c.cout, d.dwa, d.dwg, c.cout, nullptr, nullptr, st, det));
+  if (dx) CK(launch_dgrad_c1(q.dp, 2 * c.cout, c.wa, c.wg, c.cout, Z, dx, n, H, W, c.kh, c.kw, c.sh, c.sw, st));
+  return 0;
+}
+
+// the input layer takes the fused kernels (option fuse_c1)
+static bool c1_fused(const cgvc_engine* e, const Layer& L) {
+  return e->opt.fuse_c1 && !use_tc(e, L.tc_slot) && L.a.cin == 1 && !L.has_in && L.a.kh * L.a.kw <= 9 && L.a.cout == 128;
+}
+
 static int discriminator_forward(cgvc_engine* e, const DiscNet& N, DiscActs& A, const float* x, cudaStream_t st, bool keep_y) {
   const int n = A.n, T = A.T, H0 = e->cfg.num_features;
   const float* Pm = e->P();
   A.x = x;
   ConvIO io; io.x = x; io.xhi = nullptr; io.xlo = nullptr; io.n = n; io.H = H0; io.W = T;
   int H = H0, W = T / 2;
-  if (e->opt.fuse_c1 && !use_tc(e, N.h1.tc_slot) && N.h1.a.cin == 1 && !N.h1.has_in && N.h1.a.kh * N.h1.a.kw <= 9 && N.h1.a.cout % 4 == 0 &&
-      256 % (N.h1.a.cout / 4) == 0) {
-    // input layer (one input channel, K = 9, gate without norm): convolution + GLU in one HBM-bound pass; P is kept for the backward pass
-    const GatherGeom g = fwd_geom(n, H0, T, N.h1.a.kh, N.h1.a.kw, N.h1.sh, N.h1.sw);
-    const PostParams q = post_params(e, N.h1, io, A.h1, H * W, keep_y, A.post);
-    CK(launch_conv_c1_glu_fwd(g, x, Pm + N.h1.a.k, Pm + N.h1.g.k, Pm + N.h1.a.b, Pm + N.h1.g.b, N.h1.a.cout, A.h1.P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat));
-  } else {
-    RET(layer_forward(e, N.h1, io, A.h1, H * W, keep_y, true, A.post, st));
-  }
+  // input layer: one input channel, K = 9, gate without norm; P is kept for the backward pass
+  RET(disc_input_forward(e, c1_layer(e, N.h1), x, n, H0, T, A.h1.P, post_params(e, N.h1, io, A.h1, H * W, keep_y, A.post), c1_fused(e, N.h1), st));
   const GLAct* cur = &A.h1;
   for (int i = 0; i < 3; ++i) {
     io.x = (keep_y || !cur->Yhi) ? cur->Y : nullptr; io.xhi = cur->Yhi; io.xlo = cur->Ylo; io.H = H; io.W = W;
@@ -868,24 +908,11 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
     dy = bufs[flip]; flip ^= 1;
   }
   // h1: one input channel (K = 9), gate without instance norm.  Fused form: the GLU backward is recomputed inside the weight-gradient /
-  // data-gradient kernels, dP never goes to HBM
-  if (e->opt.fuse_c1 && N.h1.a.cout == 128 && N.h1.a.kh * N.h1.a.kw <= 9 && !N.h1.has_in) {
-    if (wgrad) {
-      GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
-      CK(launch_glu_bwd_wgrad_c1(g, A.x, dy, A.h1.P, 128, e->G() + N.h1.a.k, e->G() + N.h1.g.k, e->G() + N.h1.a.b, e->G() + N.h1.g.b, st,
-                                 det_of(S)));
-    }
-    if (d_in) CK(launch_glu_bwd_dgrad_c1(dy, A.h1.P, 128, e->P() + N.h1.a.k, e->P() + N.h1.g.k, bufs[flip], d_in, n, H0, T, 3, 3, N.h1.sh, N.h1.sw, st));
-    return 0;
-  }
-  PostBwdParams q = post_bwd_params(e, N.h1, dy, A.h1, n, Hs[0] * Ws[0], S, wgrad, true, PlanePair{S.dPhi, S.dPlo});
-  CK(launch_post_bwd(q, e->opt.post, st));
-  if (wgrad) {
-    GatherGeom g = fwd_geom(n, H0, T, 3, 3, N.h1.sh, N.h1.sw);
-    CK(launch_wgrad_c1(g, A.x, S.dP, 256, 256, e->G() + N.h1.a.k, e->G() + N.h1.g.k, 128, nullptr, nullptr, st, det_of(S)));
-  }
-  if (d_in) CK(launch_dgrad_c1(S.dP, 256, e->P() + N.h1.a.k, e->P() + N.h1.g.k, 128, bufs[flip], d_in, n, H0, T, 3, 3, N.h1.sh, N.h1.sw, st));
-  return 0;
+  // data-gradient kernels, dP never goes to HBM.  D.h1 has no tensor-core slot, so the unfused form's dP is fp32 (no planes)
+  float* Gm = e->G();
+  const C1Grads d = wgrad ? C1Grads{Gm + N.h1.a.k, Gm + N.h1.g.k, Gm + N.h1.a.b, Gm + N.h1.g.b} : C1Grads{nullptr, nullptr, nullptr, nullptr};
+  const PostBwdParams q = post_bwd_params(e, N.h1, dy, A.h1, n, Hs[0] * Ws[0], S, wgrad, true, PlanePair{S.dPhi, S.dPlo});
+  return disc_input_backward(e, c1_layer(e, N.h1), d, A.x, dy, A.h1.P, n, H0, T, d_in, bufs[flip], c1_fused(e, N.h1), q, det_of(S), st);
 }
 
 // ---- workspace sizing ---------------------------------------------------------------------------------------
@@ -1912,6 +1939,144 @@ int cgvc_in_glu_backward(cgvc_handle e, const float* dy, const float* p, const f
                          int B, int R, int C, int shuffle, void* stream) {
   return cgvc_in_glu_backward_planes(e, dy, p, stats, beta_a, gamma_a, beta_g, gamma_g, dp, dbeta_a, dgamma_a, dbeta_g, dgamma_g,
                                      B, R, C, shuffle, CGVC_PREC_FP32_SIMT, 1, nullptr, nullptr, nullptr, stream);
+}
+
+// ---- the layers without an instance norm and the loss heads (test entry points) --------------------------------------------------
+// A gated layer without instance norm or shuffle (generator h1, discriminator h1) over P [B * R, 2C], in the engine's own description
+static Layer glu_layer(int C) {
+  Layer L{}; L.a.cout = C; L.g.cout = C; L.a.cin = L.g.cin = 1; L.has_in = 0; L.sh = L.sw = 1; L.shuffle = 1;
+  return L;
+}
+static ConvIO rows_io(int B) { ConvIO io{}; io.n = B; return io; }
+
+// post_params / post_bwd_params of that layer; the fields they take from the engine's precision and train-step state (plane format,
+// saturation counter, arena gradients, partials slab) come from the caller's arguments instead
+static PostParams glu_fwd_params(cgvc_engine* e, const float* p, float* y, int B, int R, int C, int precision, void* hi, void* lo,
+                                 unsigned long long* sat) {
+  const GLAct A{const_cast<float*>(p), nullptr, y, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo};
+  PostParams q = post_params(e, glu_layer(C), rows_io(B), A, R, true, nullptr);
+  q.qmode = precision == CGVC_PREC_F16F8;
+  q.sat = q.qmode && hi ? sat : nullptr;
+  return q;
+}
+static PostBwdParams glu_bwd_params(cgvc_engine* e, const float* dy, const float* p, float* dp, float* dbias_a, float* dbias_g, int B, int R,
+                                    int C, int precision, void* hi, void* lo, unsigned long long* sat, const DetSlab* det) {
+  const GLAct A{const_cast<float*>(p), nullptr, nullptr, nullptr, nullptr};
+  BwdScratch S; memset(&S, 0, sizeof S); S.dP = dp;
+  PostBwdParams q = post_bwd_params(e, glu_layer(C), dy, A, B, R, S, false, true, PlanePair{nullptr, nullptr});
+  q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo;
+  q.qmode = precision == CGVC_PREC_F16F8;
+  q.sat = q.qmode && hi ? sat : nullptr;
+  q.dbias_a = dbias_a; q.dbias_g = dbias_g;
+  if (dbias_a && det) q.det = *det;
+  return q;
+}
+
+static int glu_shape(cgvc_engine* e, const char* what, long long B, long long R, int C) {
+  if (B < 1 || B > 65535 || R < 1 || C < 4 || C % 4) return fail(e, CGVC_ERR_ARG, "%s: bad shape (B %lld, R %lld, C %d)", what, B, R, C);
+  return 0;
+}
+
+int cgvc_glu_forward_planes(cgvc_handle e, const float* p, float* y, int B, int R, int C, int precision, void* hi, void* lo,
+                            unsigned long long* sat, void* stream) {
+  if (!e || !p || (!y && !hi)) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(glu_shape(e, "cgvc_glu_forward_planes", B, R, C));
+  if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
+  else hi = lo = nullptr;
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_post_fwd(glu_fwd_params(e, p, y, B, R, C, precision, hi, lo, sat), e->opt.post, (cudaStream_t)stream));
+  return 0;
+}
+
+int cgvc_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, float* dp, float* dbias_a, float* dbias_g, int B, int R, int C,
+                             int precision, void* hi, void* lo, unsigned long long* sat, void* stream) {
+  if (!e || !dy || !p || (!dp && !hi) || (!dbias_a != !dbias_g)) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(glu_shape(e, "cgvc_glu_backward_planes", B, R, C));
+  if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
+  else hi = lo = nullptr;
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_post_bwd(glu_bwd_params(e, dy, p, dp, dbias_a, dbias_g, B, R, C, precision, hi, lo, sat, det), e->opt.post, (cudaStream_t)stream));
+  return 0;
+}
+
+static int c1_shape(cgvc_engine* e, const char* what, int B, int H, int W, int kh, int kw, int Cout, int sh, int sw) {
+  if (B < 1 || H < 1 || W < 1 || kh < 1 || kw < 1 || kh * kw > 9 || Cout != 128 || sh < 1 || sw < 1)
+    return fail(e, CGVC_ERR_ARG, "%s: bad shape (B %d, H %d, W %d, kh %d, kw %d, Cout %d, sh %d, sw %d)", what, B, H, W, kh, kw, Cout, sh, sw);
+  const long long rows = (long long)((H + sh - 1) / sh) * ((W + sw - 1) / sw);
+  return glu_shape(e, what, B, rows, Cout);
+}
+
+int cgvc_disc_input_forward(cgvc_handle e, int precision, const float* x, const float* w_a, const float* w_g, const float* b_a, const float* b_g,
+                            float* p, float* y, void* hi, void* lo, unsigned long long* sat,
+                            int B, int H, int W, int kh, int kw, int Cout, int sh, int sw, int fuse, int* fused, void* stream) {
+  if (fused) *fused = 0;
+  if (!e || !x || !w_a || !w_g || !b_a || !b_g || !p || (!y && !hi)) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(c1_shape(e, "cgvc_disc_input_forward", B, H, W, kh, kw, Cout, sh, sw));
+  if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
+  else hi = lo = nullptr;
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  const int R = ((H + sh - 1) / sh) * ((W + sw - 1) / sw);
+  const C1Layer c{w_a, w_g, b_a, b_g, kh, kw, Cout, sh, sw};
+  RET(disc_input_forward(e, c, x, B, H, W, p, glu_fwd_params(e, p, y, B, R, Cout, precision, hi, lo, sat), fuse != 0, (cudaStream_t)stream));
+  if (fused) *fused = fuse != 0;
+  return 0;
+}
+
+int cgvc_disc_input_backward(cgvc_handle e, const float* dy, const float* p, const float* x, const float* w_a, const float* w_g,
+                             float* dw_a, float* dw_g, float* db_a, float* db_g, float* dx,
+                             int B, int H, int W, int kh, int kw, int Cout, int sh, int sw, int fuse, int* fused, void* stream) {
+  if (fused) *fused = 0;
+  if (!e || !dy || !p || !x || !w_a || !w_g) return fail(e, CGVC_ERR_ARG, "null argument");
+  const bool some = dw_a || dw_g || db_a || db_g;
+  if (some && !(dw_a && dw_g && db_a && db_g))
+    return fail(e, CGVC_ERR_ARG, "cgvc_disc_input_backward: the weight and bias gradients are all given or none");
+  RET(c1_shape(e, "cgvc_disc_input_backward", B, H, W, kh, kw, Cout, sh, sw));
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  const long long rows = (long long)B * ((H + sh - 1) / sh) * ((W + sw - 1) / sw);
+  // scratch: the fp32 dP of the unfused form [rows, 2 Cout], then Z [rows, taps]
+  const long long ndp = fuse ? 0 : rows * 2 * Cout;
+  float* buf;
+  CK(grow_post_buf(e, (size_t)(ndp + rows * kh * kw), &buf));
+  const C1Layer c{w_a, w_g, nullptr, nullptr, kh, kw, Cout, sh, sw};
+  const PostBwdParams q = glu_bwd_params(e, dy, p, fuse ? nullptr : buf, db_a, db_g, B, (int)(rows / B), Cout, CGVC_PREC_FP32_SIMT, nullptr,
+                                         nullptr, nullptr, det);
+  RET(disc_input_backward(e, c, C1Grads{dw_a, dw_g, db_a, db_g}, x, dy, p, B, H, W, dx, buf + ndp, fuse != 0, q, det, (cudaStream_t)stream));
+  if (fused) *fused = fuse != 0;
+  return 0;
+}
+
+int cgvc_head_forward(cgvc_handle e, const float* y, long long rows, const float* w, const float* b, float* prob, void* stream) {
+  if (!e || !y || !w || !b || !prob) return fail(e, CGVC_ERR_ARG, "null argument");
+  if (rows < 0) return fail(e, CGVC_ERR_ARG, "cgvc_head_forward: rows %lld", rows);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_head_fwd(y, rows, 1024, w, b, prob, (cudaStream_t)stream));
+  return 0;
+}
+
+int cgvc_head_loss_backward(cgvc_handle e, const float* prob, const float* y, long long rows, const float* w, float target, float coef,
+                            const float* grad_mult, float* loss, float* dy, float* dw, float* db, void* stream) {
+  if (!e || !prob || !w || ((dw || db) && !y) || (!dw != !db)) return fail(e, CGVC_ERR_ARG, "null argument");
+  if (rows < 0) return fail(e, CGVC_ERR_ARG, "cgvc_head_loss_backward: rows %lld", rows);
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_head_loss_bwd(prob, y, rows, 1024, w, target, coef, loss, dy, dw, db, (cudaStream_t)stream, grad_mult, det));
+  return 0;
+}
+
+int cgvc_l1_loss_grad(cgvc_handle e, const float* yhat, const float* y, long long n, const float* gscale, const float* grad_mult, float* loss,
+                      float* d, int accumulate, void* stream) {
+  if (!e || !yhat || !y) return fail(e, CGVC_ERR_ARG, "null argument");
+  if (n < 0) return fail(e, CGVC_ERR_ARG, "cgvc_l1_loss_grad: n %lld", n);
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_l1_loss_grad(yhat, y, n, loss, gscale, d, accumulate, (cudaStream_t)stream, grad_mult, det));
+  return 0;
 }
 
 }  // extern "C"
