@@ -364,6 +364,32 @@ int cgvc_head_loss_backward(cgvc_handle h, const float* prob, const float* y, lo
                             const float* grad_mult, float* loss, float* dy, float* dw, float* db, void* stream);
 int cgvc_l1_loss_grad(cgvc_handle h, const float* yhat, const float* y, long long n, const float* gscale, const float* grad_mult, float* loss,
                       float* d, int accumulate, void* stream);
+/* The generator's two 15-tap edge layers as the step runs them with option "edge_lower" (module.py:85-86 h1, module.py:148 o1): dense
+ * 1 x 1 GEMMs over an im2col of the 24-channel side.  They act on the handle's generator `direction` (0 = A2B, 1 = B2A): weights
+ * from PARAM through the planes cgvc_params_updated prepares, kernel and bias gradients accumulated into that generator's GRAD
+ * ranges.  Rows are B samples of T positions, or for the forwards (offsets, host, not NULL) B packed utterances with the offsets
+ * contract of cgvc_generator_forward_packed (T ignored).  F = 24 features, K = 15 taps; plane buffers hold [rows, 384] values in the
+ * engine's precision (bf16 hi / lo; F16F8 fp16 hi, then lo = the two e4m3 planes one after the other).  CGVC_ERR_UNSUPPORTED when
+ * the layers are not lowered (edge_lower 0, CGVC_PREC_FP32_SIMT, or before cgvc_params_updated).  The backward calls honour
+ * "deterministic" (WORK bound).
+ * cgvc_edge_h1_forward: x [rows, F] -> p [rows, 256] = [a | g] (the GEMM over im2col(x) [rows, K F], bias included), y [rows, 128]
+ *   = a * sigmoid(g) and, when hi / lo are given, y's planes.
+ * cgvc_edge_o1_forward: u [rows, 256] (its planes are written here) -> z [rows, K F] = u . W' with column t F + c the tap t product
+ *   for output channel c (may be NULL), out [rows, F] = bias + sum_t z[r + t - 7, t F + c] over the rows of r's sample.
+ * cgvc_edge_o1_backward: u, d_out [rows, F] -> GRAD o1 kernel += u^T dZ, bias += column sums of d_out; du [rows, 256] = dZ . W'^T;
+ *   dZ [rows, K F] = d_out shifted by tap (dZ[r, t F + c] = d_out[r - t + 7, c] within the sample) as planes into dz_hi / dz_lo
+ *   (both NULL: scratch).
+ * cgvc_edge_h1_backward: x, p and dy [rows, 128] (d loss / d y) -> GRAD h1 a and g kernels += im2col(x)^T dP and biases += column
+ *   sums of dP, dP [rows, 256] the GLU backward; dp = that dP (may be NULL), dz [rows, K F] = dP . W^T (may be NULL), dx [rows, F] =
+ *   sum_t dz[r - t + 7, t F + c] within the sample (may be NULL). */
+int cgvc_edge_h1_forward(cgvc_handle h, int direction, const float* x, int B, int T, const long long* offsets, float* p, float* y,
+                         void* hi, void* lo, void* stream);
+int cgvc_edge_o1_forward(cgvc_handle h, int direction, const float* u, int B, int T, const long long* offsets, float* z, float* out,
+                         void* stream);
+int cgvc_edge_o1_backward(cgvc_handle h, int direction, const float* u, const float* d_out, int B, int T, float* du, void* dz_hi,
+                          void* dz_lo, void* stream);
+int cgvc_edge_h1_backward(cgvc_handle h, int direction, const float* x, const float* p, const float* dy, int B, int T, float* dp, float* dz,
+                          float* dx, void* stream);
 
 /* error codes */
 enum {

@@ -307,8 +307,10 @@ def certificate(case, prec, x, w, b, dy, w16=1, device="cpu", P=None, forms=("fw
             tot = tot + _t(np.abs(bias), device)
         res.append((form, "total", float(tot.max()), 2.0 ** ACC_BITS * g))
         if prec == F16F8 and form != "wgrad":
-            gc = 2.0 ** min(lsb(Pa, ka) + lsb(Pb, kb) for _, ka, kb in prs[1:])
-            res.append((form, "e4m3", float(sum(prods[1:]).max()), 2.0 ** E4M3_ACC_BITS * gc))
+            # (an operand whose fp16 plane holds it exactly has all-zero e4m3 lo planes: those cross products have no terms)
+            ec = [lsb(Pa, ka) + lsb(Pb, kb) for _, ka, kb in prs[1:] if lsb(Pa, ka) is not None and lsb(Pb, kb) is not None]
+            if ec:
+                res.append((form, "e4m3", float(sum(prods[1:]).max()), 2.0 ** E4M3_ACC_BITS * 2.0 ** min(ec)))
     if "db" in forms:
         dyc = np.abs(np.asarray(dy, np.float64)).reshape(-1, Cout).sum(0)
         res.append(("db", "total", float(dyc.max()), 2.0 ** ACC_BITS * 2.0 ** lsb_exp(dy)))

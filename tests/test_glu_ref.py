@@ -120,7 +120,7 @@ REACHED = {
     "wgrad_c1_kernel": "test_gpu_glu_layers.py", "gather_taps_kernel": "test_gpu_glu_layers.py", "glu_bwd_wgrad_c1_kernel": "test_gpu_glu_layers.py",
     "glu_bwd_proj_c1_kernel": "test_gpu_glu_layers.py", "proj_taps_kernel": "test_gpu_glu_layers.py", "conv_c1_fwd_kernel": "test_gpu_glu_layers.py",
     "conv_c1_glu_fwd_kernel": "test_gpu_glu_layers.py", "pad_split_q_kernel": "test_gpu_planes.py", "pad_split_kernel": "test_gpu_planes.py",
-    "im2col_taps_kernel": "test_gpu_planes.py", "col2im_taps_kernel": "test_tap_lowering.py (CPU algebra) / test_gpu_model.py",
+    "im2col_taps_kernel": "test_gpu_planes.py", "col2im_taps_kernel": "test_gpu_edge_layers.py",
     "check_finite_kernel": "test_gpu_loss_scale.py", "loss_scale_update_kernel": "test_gpu_loss_scale.py",
 }
 # kernels checked only through whole-model tests against the oracle, with the reason no unit tier is needed

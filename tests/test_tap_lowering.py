@@ -4,40 +4,14 @@ are computed on the GPU as dense 1 x 1 GEMMs over an im2col of the 24-channel te
 (dir = +1 / -1, pad_left = 7, zero outside the sample, TF kernel [15,24,128] read as a [360,128] matrix, o1's taps folded into
 output columns t * 24 + n) are restated here in numpy and held against the oracle's TF-'SAME' convolution and its autograd
 gradients, so a sign or offset error in the lowering would show without a GPU.  (The CUDA kernels themselves are compared with the
-oracle and with the 15-tap gather-GEMMs in tests/test_gpu_model.py.)"""
+oracle and with the 15-tap gather-GEMMs in tests/test_gpu_model.py, and layer by layer against the float64 emulation of
+their operand planes in tests/test_gpu_edge_layers.py; the restatements live in tests/edge_ref.py.)"""
 import numpy as np
 import torch
 
 from oracle import cyclegan_oracle as O
 
-KW, F_, PL = 15, 24, 7          # taps, narrow channel count, TF SAME pad_left at stride 1 = (kw - 1) // 2
-
-
-def im2col_taps(x, direction):
-    """x [n, T, C] -> [n, T, KW * C]: out[m, t*C + c] = x[m + direction * (t - PL), c], zero outside the sample (im2col_taps_kernel)."""
-    n, T, C = x.shape
-    out = np.zeros((n, T, KW * C), dtype=x.dtype)
-    for t in range(KW):
-        s = direction * (t - PL)
-        lo, hi = max(0, -s), min(T, T - s)
-        out[:, lo:hi, t * C:(t + 1) * C] = x[:, lo + s:hi + s, :]
-    return out
-
-
-def col2im_taps(z, C, direction, bias=None):
-    """z [n, T, KW * C] -> [n, T, C]: y[m, c] = bias[c] + sum_t z[m + direction * (t - PL), t*C + c] over rows of the sample (col2im_taps_kernel)."""
-    n, T, _ = z.shape
-    y = np.zeros((n, T, C), dtype=z.dtype)
-    for t in range(KW):
-        s = direction * (t - PL)
-        lo, hi = max(0, -s), min(T, T - s)
-        y[:, lo:hi, :] += z[:, lo + s:hi + s, t * C:(t + 1) * C]
-    return y if bias is None else y + bias
-
-
-def fold_columns(w):
-    """TF kernel [KW, Cin, Cout] -> [Cin, KW * Cout] with column t * Cout + n (TcLayer::fold / w_src)."""
-    return np.concatenate([w[t] for t in range(KW)], axis=1)
+from edge_ref import F_, KW, PL, col2im_replay, col2im_taps, fold_columns, im2col_taps, o1_z_weights
 
 
 def test_pad_left_matches_tf_same():
@@ -92,3 +66,47 @@ def test_fold_index_functions():
         for ci in (0, 3, Cin - 1):
             t = co // fold_n
             assert flat[(t * Cin + ci) * fold_n + (co - t * fold_n)] == w[t, ci, co % fold_n]
+
+
+def test_fold_of_a_tf_kernel():
+    """edge_ref.o1_z_weights: column t * 24 + n of the folded [256, 360] matrix is element [t][c][n] of o1's TF kernel, and the 1 x 1
+    layer over it followed by the tap-shifted sum is the 15-tap convolution"""
+    rs = np.random.RandomState(2)
+    w = rs.randn(KW, 256, F_)
+    wf = o1_z_weights(w)
+    assert wf.shape == (1, 1, 256, KW * F_)
+    for t, c, n in ((0, 0, 0), (7, 100, 5), (14, 255, 23), (3, 17, 12)):
+        assert wf[0, 0, c, t * F_ + n] == w[t, c, n]
+    u = rs.randn(2, 20, 256); b = rs.randn(F_)
+    y_ref = O.conv1d_same(torch.tensor(u), torch.tensor(w), torch.tensor(b)).numpy()
+    assert np.allclose(col2im_taps(u @ wf[0, 0], F_, +1, b), y_ref, atol=1e-10)
+
+
+def test_col2im_replay_is_the_kernels_fp32_order():
+    """edge_ref.col2im_replay: bias first, then taps 0..14 in order in float32, skipping rows outside the sample, per sample or per
+    packed utterance; it agrees with the float64 col2im to fp32 rounding, and an element whose partial sums all round shows the order"""
+    rs = np.random.RandomState(3)
+    for direction in (+1, -1):
+        for T, offsets in ((4, None), (36, None), (None, np.array([0, 4, 40, 48, 176]))):
+            rows = 3 * T if T else int(offsets[-1])
+            z = rs.randn(rows, KW * F_).astype(np.float32)
+            b = rs.randn(F_).astype(np.float32) if direction == +1 else None
+            got = col2im_replay(z, F_, direction, T=T, offsets=offsets, bias=b)
+            bounds = [(s, T) for s in range(0, rows, T)] if T else list(zip(offsets[:-1], np.diff(offsets)))
+            ref = np.concatenate([col2im_taps(z[s:s + L].astype(np.float64)[None], F_, direction, b)[0] for s, L in bounds])
+            assert np.allclose(got, ref, rtol=0, atol=1e-5)
+            # the same in a plain float32 loop, element by element
+            s0, L = bounds[-1]
+            for m in (0, L - 1, L // 2):
+                for c in (0, 23):
+                    acc = np.float32(b[c]) if b is not None else np.float32(0)
+                    for t in range(KW):
+                        ws = m + direction * (t - PL)
+                        if 0 <= ws < L:
+                            acc = np.float32(acc + z[s0 + ws, t * F_ + c])
+                    assert acc == got[s0 + m, c], (direction, T, m, c)
+    # order matters: 1 + 2^-24 + ... rounds differently from the reverse order; the replay takes the kernel's
+    z = np.zeros((1, KW * F_), np.float32)
+    z[0, PL * F_] = 2.0 ** -24
+    got = col2im_replay(z, F_, +1, T=1, bias=np.ones(F_, np.float32))
+    assert got[0, 0] == np.float32(1.0)

@@ -94,6 +94,10 @@ def _declare(lib):
         "cgvc_head_forward": (ci, [vp, vp, C.c_longlong, vp, vp, vp, vp]),
         "cgvc_head_loss_backward": (ci, [vp, vp, vp, C.c_longlong, vp, cf, cf] + [vp] * 6),
         "cgvc_l1_loss_grad": (ci, [vp, vp, vp, C.c_longlong] + [vp] * 4 + [ci, vp]),
+        "cgvc_edge_h1_forward": (ci, [vp, ci, vp, ci, ci] + [vp] * 6),
+        "cgvc_edge_o1_forward": (ci, [vp, ci, vp, ci, ci] + [vp] * 4),
+        "cgvc_edge_o1_backward": (ci, [vp, ci, vp, vp, ci, ci] + [vp] * 4),
+        "cgvc_edge_h1_backward": (ci, [vp, ci, vp, vp, vp, ci, ci] + [vp] * 4),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the library does not export a declared symbol

@@ -521,6 +521,28 @@ static void plan_generator(cgvc_engine* e, Bump& ws, GenActs& A, int n, int T) {
   A.T = T;
 }
 
+// The tap-lowered edge layers (edge_on) by pointer, so that the walks and the test entry points (cgvc_edge_*) run the same launches.
+// Rows: n samples of T, or (off) one sequence of T rows holding n_off packed utterances (n = 1).
+// h1: the im2col planes xc of x [n*T, F], P [n*T, 256] = [a | g] = xc . W + bias, then the GLU that q describes (q.p = P)
+static int h1_edge_forward(cgvc_engine* e, const GenNet& N, const float* x, int n, int T, const long long* off, int n_off,
+                           __nv_bfloat16* xchi, __nv_bfloat16* xclo, float* P, const PostParams& q, cudaStream_t st) {
+  const int nf = e->cfg.num_features;
+  CK(launch_im2col_taps(x, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
+                        xchi, xclo, st, off, n_off, sat_act(e)));
+  RET(tc_result(e, tc_conv_fwd(e->tcw, N.h1c_slot, xchi, xclo, n, 1, T, 1, 1, P, st), &N.h1.a, "forward (tap-lowered)"));
+  CK(launch_post_fwd(q, e->opt.post, st));
+  return 0;
+}
+
+// o1: Z [n*W, kw*F] = U . W' (the taps folded into the columns) from U's planes, then out [n*W, F] = bias + the tap-shifted sum of Z
+static int o1_edge_forward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16* uhi, const __nv_bfloat16* ulo, int n, int W,
+                           const long long* off, int n_off, float* z, float* out, cudaStream_t st) {
+  const int nf = e->cfg.num_features;
+  RET(tc_result(e, tc_conv_fwd(e->tcw, N.o1f_slot, uhi, ulo, n, 1, W, 1, 1, z, st), &N.o1.a, "forward (tap-lowered)"));
+  CK(launch_col2im_taps(z, N.o1.a.kw * nf, (long long)n * W, W, nf, N.o1.a.kw, +1, e->P() + N.o1.a.b, out, st, off, n_off));
+  return 0;
+}
+
 // keep_y: also write the fp32 copy of every activation (debug taps / SIMT path); the tensor-core training path only
 // needs fp32 where a residual add or the discriminator head reads it.
 // save_pre = false (inference): the fused layers do not write their pre-norm outputs / statistics (nothing runs backward)
@@ -540,10 +562,7 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
   ConvIO io = at(x_cl, A.xhi, A.xlo, T);
   if (edge) {
     // h1 = dense [n*T, kw*F] x [kw*F, 2*128] GEMM on the im2col of the input
-    CK(launch_im2col_taps(x_cl, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
-                          A.xchi, A.xclo, st, A.off, A.n, sat_act(e)));
-    RET(tc_result(e, tc_conv_fwd(e->tcw, N.h1c_slot, A.xchi, A.xclo, n, 1, T, 1, 1, A.h1.P, st), &N.h1.a, "forward (tap-lowered)"));
-    PostParams q = post_params(e, N.h1, io, A.h1, T, keep_y, A.post); CK(launch_post_fwd(q, e->opt.post, st));
+    RET(h1_edge_forward(e, N, x_cl, n, T, A.off, A.n, A.xchi, A.xclo, A.h1.P, post_params(e, N.h1, io, A.h1, T, keep_y, A.post), st));
   } else {
     if (A.xhi && tc_enabled(e)) CK(tc_split_planes(e->cfg.precision, x_cl, (long long)n * T, nf, A.xhi, A.xlo, st, sat_act(e)));
     RET(layer_forward(e, N.h1, io, A.h1, T, keep_y, save_pre, A.post, st));
@@ -569,8 +588,7 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
   }
   if (edge && io.xhi) {
     // o1: Z[m, (t, c)] = U[m, :] . W[t][:, c] as one dense GEMM, then out[m, c] = b[c] + sum_t Z[m + t - 7, (t, c)]
-    RET(tc_result(e, tc_conv_fwd(e->tcw, N.o1f_slot, io.xhi, io.xlo, n, 1, W, 1, 1, A.z, st), &N.o1.a, "forward (tap-lowered)"));
-    CK(launch_col2im_taps(A.z, N.o1.a.kw * nf, (long long)n * W, W, nf, N.o1.a.kw, +1, e->P() + N.o1.a.b, A.out_cl, st, A.off, A.n));
+    RET(o1_edge_forward(e, N, io.xhi, io.xlo, n, W, A.off, A.n, A.z, A.out_cl, st));
   } else {
     RET(conv_fwd(e, N.o1, io, A.out_cl, st));
   }
@@ -712,6 +730,38 @@ static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAc
   return 0;
 }
 
+// The tap-lowered edge layers' backward (see h1_edge_forward), n samples of T rows.
+// o1 from d_out [n*T, F]: its dZ planes (the im2col of d_out, dir -1), the kernel gradient U^T dZ into GRAD (run_wgrad, folded columns
+// scattered by tn_dst) and du [n*T, 256] = dZ . W'^T.  The bias gradient, the column sums of d_out, is the caller's
+static int o1_edge_backward(cgvc_engine* e, const GenNet& N, const float* d_out, const __nv_bfloat16* uhi, const __nv_bfloat16* ulo, int n,
+                            int T, PlanePair dz, float* du, const BwdScratch& S, cudaStream_t st) {
+  const int nf = e->cfg.num_features;
+  float* Gm = e->G();
+  CK(launch_im2col_taps(d_out, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
+                        dz.hi, dz.lo, st, nullptr, 0, sat_grad(e)));
+  RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
+    return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws, det_of(S)),
+                     &N.o1.a, "weight gradient (tap-lowered)"); }));
+  RET(tc_result(e, tc_conv_dgrad(e->tcw, N.o1f_slot, dz.hi, dz.lo, n, 1, T, 1, 1, du, 0, st), &N.o1.a, "data gradient (tap-lowered)"));
+  return 0;
+}
+
+// h1 from its dP planes (written by the GLU backward, which also takes the bias gradients): the kernel gradients xc^T dP straight into
+// the [15,24,128] a and g ranges of GRAD (run_wgrad); with dz, dz [n*T, kw*F] = dP . W^T, and with dx too, dx [n*T, F] = the
+// tap-shifted sum of dz (dir -1)
+static int h1_edge_backward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16* xchi, const __nv_bfloat16* xclo, PlanePair dp, int n,
+                            int T, float* dz, float* dx, const BwdScratch& S, cudaStream_t st) {
+  const int nf = e->cfg.num_features;
+  float* Gm = e->G();
+  RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
+    return tc_result(e, tc_conv_wgrad(e->tcw, N.h1c_slot, xchi, xclo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.h1.a.k, Gm + N.h1.g.k, ws,
+                                      det_of(S)),
+                     &N.h1.a, "weight gradient (tap-lowered)"); }));
+  if (dz) RET(tc_result(e, tc_conv_dgrad(e->tcw, N.h1c_slot, dp.hi, dp.lo, n, 1, T, 1, 1, dz, 0, st), &N.h1.a, "data gradient (tap-lowered)"));
+  if (dz && dx) CK(launch_col2im_taps(dz, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, dx, st));
+  return 0;
+}
+
 // Backward through one generator application.  d_out_cl: [n*T, 24] gradient w.r.t. the channels-last output.
 // Weight gradients are accumulated into the GRAD arena; d_in_cl (optional) receives d loss / d input (channels-last).
 static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A, const float* d_out_cl, float* d_in_cl,
@@ -731,13 +781,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   const ConvIO u2 = of(A.u[1], T);
   if (edge && u2.xhi && S.dPhi) {
     // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
-    const PlanePair dp = dp_planes(w, st);
-    CK(launch_im2col_taps(d_out_cl, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
-                          dp.hi, dp.lo, st, nullptr, 0, sat_grad(e)));
-    RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-      return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, u2.xhi, u2.xlo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws, det_of(S)),
-                       &N.o1.a, "weight gradient (tap-lowered)"); }));
-    RET(tc_result(e, tc_conv_dgrad(e->tcw, N.o1f_slot, dp.hi, dp.lo, n, 1, T, 1, 1, S.bufA, 0, st), &N.o1.a, "data gradient (tap-lowered)"));
+    RET(o1_edge_backward(e, N, d_out_cl, u2.xhi, u2.xlo, n, T, dp_planes(w, st), S.bufA, S, st));
   } else {
     PlanePair dp{nullptr, nullptr};
     if (use_tc(e, N.o1.tc_slot) && u2.xhi && S.dPhi) {
@@ -775,15 +819,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   // (cycle passes only) is the dense dP . W^T [n*T, kw*F] followed by the tap-shifted sum
   PostBwdParams q;
   RET(layer_dp(e, w, N.h1, A.h1, cur, n, T, true, st, q));
-  RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-    return tc_result(e, tc_conv_wgrad(e->tcw, N.h1c_slot, A.xchi, A.xclo, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, Gm + N.h1.a.k, Gm + N.h1.g.k, ws,
-                                      det_of(S)),
-                     &N.h1.a, "weight gradient (tap-lowered)"); }));
-  if (d_in_cl) {
-    RET(tc_result(e, tc_conv_dgrad(e->tcw, N.h1c_slot, q.dp_hi, q.dp_lo, n, 1, T, 1, 1, oth, 0, st), &N.h1.a, "data gradient (tap-lowered)"));
-    CK(launch_col2im_taps(oth, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, d_in_cl, st));
-  }
-  return 0;
+  return h1_edge_backward(e, N, A.xchi, A.xclo, PlanePair{q.dp_hi, q.dp_lo}, n, T, d_in_cl ? oth : nullptr, d_in_cl, S, st);
 }
 
 // ---- discriminator ---------------------------------------------------------------------------------------
@@ -2077,6 +2113,146 @@ int cgvc_l1_loss_grad(cgvc_handle e, const float* yhat, const float* y, long lon
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   CK(launch_l1_loss_grad(yhat, y, n, loss, gscale, d, accumulate, (cudaStream_t)stream, grad_mult, det));
   return 0;
+}
+
+}  // extern "C"
+
+// ---- the generator's tap-lowered edge layers (test entry points) -----------------------------------------------------------------
+// What every cgvc_edge_* call checks: the handle's generator `direction` runs its edge layers tap-lowered (edge_on: option edge_lower,
+// a tensor-core precision, weights prepared by cgvc_params_updated), the arenas it reads and writes are bound, and the rows are B
+// samples of T or (offsets, host) B packed utterances with the contract of cgvc_generator_forward_packed.  *rows: the row count
+static int edge_entry(cgvc_engine* e, const char* what, int direction, int B, int T, const long long* offsets, bool grad, long long* rows) {
+  if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
+  if (!e->arena[CGVC_ARENA_PARAM] || (grad && !e->arena[CGVC_ARENA_GRAD]))
+    return fail(e, CGVC_ERR_UNBOUND, "%s: the PARAM%s arena must be bound", what, grad ? " and GRAD" : "");
+  if (!edge_on(e, e->gen[direction]))
+    return fail(e, CGVC_ERR_UNSUPPORTED, "%s: the edge layers are not tap-lowered here (option edge_lower, a tensor-core precision and "
+                "cgvc_params_updated are needed)", what);
+  if (B < 1 || B > 65535) return fail(e, CGVC_ERR_ARG, "%s: %d samples outside [1, 65535]", what, B);
+  if (offsets) {
+    if (offsets[0] != 0) return fail(e, CGVC_ERR_ARG, "%s: offsets[0] is %lld, must be 0", what, offsets[0]);
+    for (int u = 0; u < B; ++u) {
+      const long long len = offsets[u + 1] - offsets[u];
+      if (len <= 0 || len % 4 != 0)
+        return fail(e, CGVC_ERR_ARG, "%s: utterance %d: length %lld must be a positive multiple of 4", what, u, len);
+    }
+    *rows = offsets[B];
+  } else {
+    if (T < 1) return fail(e, CGVC_ERR_ARG, "%s: T %d", what, T);
+    *rows = (long long)B * T;
+  }
+  if (*rows > INT_MAX / 512) return fail(e, CGVC_ERR_ARG, "%s: %lld rows exceed %d", what, *rows, INT_MAX / 512);
+  return 0;
+}
+
+// the entry points' scratch, carved from the per-engine buffer: carve(ws) runs once on a null base to size it, then on the buffer
+template <class F> static cudaError_t edge_scratch(cgvc_engine* e, F&& carve) {
+  Bump ws; ws.reset(nullptr, 0);
+  carve(ws);
+  float* buf;
+  cudaError_t ce = grow_post_buf(e, ws.off / sizeof(float) + 1, &buf);
+  if (ce != cudaSuccess) return ce;
+  ws.reset(buf, e->post_elems * sizeof(float));
+  carve(ws);
+  return cudaSuccess;
+}
+
+// operand planes of `rows` rows of c channels in the engine's precision: bf16 hi / lo [rows, ru64(c)], F16F8 fp16 + two e4m3 [rows, ru128(c)]
+static void edge_planes(Bump& ws, long long rows, int c, __nv_bfloat16** hi, __nv_bfloat16** lo) {
+  const size_t n = (size_t)rows * edge_cpad(c);
+  *hi = ws.take<__nv_bfloat16>(n); *lo = ws.take<__nv_bfloat16>(n);
+}
+
+extern "C" {
+
+int cgvc_edge_h1_forward(cgvc_handle e, int direction, const float* x, int B, int T, const long long* offsets, float* p, float* y,
+                         void* hi, void* lo, void* stream) {
+  if (!e || !x || !p || !y || (!hi != !lo)) return fail(e, CGVC_ERR_ARG, "null argument");
+  long long rows;
+  RET(edge_entry(e, "cgvc_edge_h1_forward", direction, B, T, offsets, false, &rows));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenNet& N = e->gen[direction];
+  __nv_bfloat16 *xchi, *xclo; long long* off = nullptr;
+  CK(edge_scratch(e, [&](Bump& ws) {
+    edge_planes(ws, rows, N.h1.a.kw * e->cfg.num_features, &xchi, &xclo);
+    if (offsets) off = ws.take<long long>((size_t)B + 1);
+  }));
+  if (offsets) CK(cudaMemcpyAsync(off, offsets, ((size_t)B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  const int n = offsets ? 1 : B, W = offsets ? (int)rows : T;
+  const GLAct A{p, nullptr, y, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo};
+  return h1_edge_forward(e, N, x, n, W, off, offsets ? B : 0, xchi, xclo, p, post_params(e, N.h1, rows_io(n), A, W, true, nullptr), st);
+}
+
+int cgvc_edge_o1_forward(cgvc_handle e, int direction, const float* u, int B, int T, const long long* offsets, float* z, float* out,
+                         void* stream) {
+  if (!e || !u || !out) return fail(e, CGVC_ERR_ARG, "null argument");
+  long long rows;
+  RET(edge_entry(e, "cgvc_edge_o1_forward", direction, B, T, offsets, false, &rows));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenNet& N = e->gen[direction];
+  __nv_bfloat16 *uhi, *ulo; long long* off = nullptr; float* zs = nullptr;
+  CK(edge_scratch(e, [&](Bump& ws) {
+    edge_planes(ws, rows, N.o1.a.cin, &uhi, &ulo);
+    if (offsets) off = ws.take<long long>((size_t)B + 1);
+    if (!z) zs = ws.take<float>((size_t)rows * N.o1.a.kw * N.o1.a.cout);
+  }));
+  if (offsets) CK(cudaMemcpyAsync(off, offsets, ((size_t)B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CK(tc_split_planes(e->cfg.precision, u, rows, N.o1.a.cin, uhi, ulo, st));
+  const int n = offsets ? 1 : B, W = offsets ? (int)rows : T;
+  return o1_edge_forward(e, N, uhi, ulo, n, W, off, offsets ? B : 0, z ? z : zs, out, st);
+}
+
+int cgvc_edge_o1_backward(cgvc_handle e, int direction, const float* u, const float* d_out, int B, int T, float* du, void* dz_hi,
+                          void* dz_lo, void* stream) {
+  if (!e || !u || !d_out || !du || (!dz_hi != !dz_lo)) return fail(e, CGVC_ERR_ARG, "null argument");
+  long long rows;
+  RET(edge_entry(e, "cgvc_edge_o1_backward", direction, B, T, nullptr, true, &rows));
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenNet& N = e->gen[direction];
+  const int nf = e->cfg.num_features;
+  __nv_bfloat16 *uhi, *ulo, *zhi = (__nv_bfloat16*)dz_hi, *zlo = (__nv_bfloat16*)dz_lo;
+  CK(edge_scratch(e, [&](Bump& ws) {
+    edge_planes(ws, rows, N.o1.a.cin, &uhi, &ulo);
+    if (!dz_hi) edge_planes(ws, rows, N.o1.a.kw * nf, &zhi, &zlo);
+  }));
+  CK(tc_split_planes(e->cfg.precision, u, rows, N.o1.a.cin, uhi, ulo, st));
+  BwdScratch S; memset(&S, 0, sizeof S);
+  if (det) S.det = *det;
+  CK(launch_colsum(d_out, rows, nf, 0, nf, e->G() + N.o1.a.b, st, det));
+  return o1_edge_backward(e, N, d_out, uhi, ulo, B, T, PlanePair{zhi, zlo}, du, S, st);
+}
+
+int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const float* p, const float* dy, int B, int T, float* dp, float* dz,
+                          float* dx, void* stream) {
+  if (!e || !x || !p || !dy) return fail(e, CGVC_ERR_ARG, "null argument");
+  long long rows;
+  RET(edge_entry(e, "cgvc_edge_h1_backward", direction, B, T, nullptr, true, &rows));
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenNet& N = e->gen[direction];
+  const int nf = e->cfg.num_features, kc = N.h1.a.kw * nf;
+  __nv_bfloat16 *xchi, *xclo, *dphi, *dplo; float* zs = nullptr;
+  BwdScratch S; memset(&S, 0, sizeof S);
+  CK(edge_scratch(e, [&](Bump& ws) {
+    edge_planes(ws, rows, kc, &xchi, &xclo);
+    edge_planes(ws, rows, N.h1.width(), &dphi, &dplo);
+    S.post = ws.take<float>((size_t)B * 4 * 1024);
+    if (dx && !dz) zs = ws.take<float>((size_t)rows * kc);
+  }));
+  CK(launch_im2col_taps(x, rows, T, nf, N.h1.a.kw, +1, edge_cpad(kc), e->cfg.precision == CGVC_PREC_F16F8, xchi, xclo, st));
+  S.dP = dp; S.dPhi = dphi; S.dPlo = dplo;
+  if (det) S.det = *det;
+  const GLAct A{const_cast<float*>(p), nullptr, nullptr, nullptr, nullptr};
+  const PostBwdParams q = post_bwd_params(e, N.h1, dy, A, B, T, S, true, dp != nullptr, PlanePair{dphi, dplo});
+  CK(launch_post_bwd(q, e->opt.post, st));
+  return h1_edge_backward(e, N, xchi, xclo, PlanePair{q.dp_hi, q.dp_lo}, B, T, dz ? dz : zs, dx, S, st);
 }
 
 }  // extern "C"
