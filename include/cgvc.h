@@ -108,8 +108,21 @@ int cgvc_get_adam_step(cgvc_handle h, long long* t);
  * within 4e-4 of float64 while an activation / gradient operand's RMS lies in 2^-14 .. 2^12 (full precision for 2^-6 .. 2^6 with no
  * element above 256), a weight operand's from about 2^-13 up.  The batch-2 train step's gradients are within 1e-3 of float64 at every
  * scale from 2^4 up whose planes did not saturate (2^2: 1.2e-3, 2^0: 1.9e-3; the first saturation at 2^14), so the static scale
- * (2^10 at batch 2) lies 2^6 above the lower edge.  The scaler has no underflow signal: at batch 1 with lambda_cycle = 1e4 it settles
- * on 2, where the worst gradient is 1.2e-3 from float64 -- not parity-grade. */
+ * (2^10 at batch 2) lies 2^6 above the lower edge.  With one scale, at batch 1 with lambda_cycle = 1e4 it settles on 2, where the worst
+ * gradient is 1.2e-3 from float64 -- not parity-grade: the generators' L1 gradients force the scale down and the discriminators' LSGAN
+ * gradients, which do not grow with the lambdas, fall below the fp16 lower edge.  With "loss_scale_per_network" the same case settles
+ * on s_G = 2, s_D = 512 and the worst of the 280 gradients is 3.6e-4.  Below the edge the underflow count rises: at batch 2 the
+ * discriminators' ufl_grad / groups is 1.3e-2 at s_D = 2^10 and 1.6e-1 at 2^6, where their first update moves 1.2e-3.
+ * "loss_scale_per_network" = 1 (F16F8, modes 1 and 2; default 0, and 0 changes nothing): two scales.  s_D multiplies the discriminators'
+ *     D-loss heads and so everything that pass back-propagates, their weight gradients included; s_G the cycle and identity L1 gradients
+ *     and the adversarial head, and so the adversarial data gradient through the discriminator and both generator backward passes.  Adam
+ *     divides each GRAD range by its own network's scale.  The gradient-plane writers count per pass: sat_grad (saturated groups),
+ *     ufl_grad (groups with a finite non-zero value whose fp16 plane is subnormal or flushed, |fp16(x)| < 2^-14: the edge below which an
+ *     F16F8 product loses a bit per octave) and groups (all groups counted).  Dynamic mode skips a step when either network overflowed
+ *     (saturation in its block, or a non-finite value in its GRAD range), halves only the scale of a network that did, and doubles each
+ *     scale after "loss_scale_growth_interval" steps in which that network did not overflow.  ufl_grad is reported, not acted on.
+ *     Monitor mode uses the static scale for both.  cgvc_loss_scale_info keeps its meaning, with scale = s_G, sat_grad = both networks'
+ *     saturated groups and good_steps = consecutive steps not skipped. */
 typedef struct cgvc_loss_scale_info {
   float scale;                    /* the scale the next step's gradients are formed with (static: that of the last step's batch) */
   int good_steps;                 /* consecutive steps not skipped (dynamic) */
@@ -121,8 +134,23 @@ typedef struct cgvc_loss_scale_info {
 } cgvc_loss_scale_info;
 /* asynchronous: copies the state into out_dev (device memory) on the stream */
 int cgvc_loss_scale_state(cgvc_handle h, cgvc_loss_scale_info* out_dev, void* stream);
-/* resume a dynamic scale: scale in [1, 2^24]; last_skipped, nonfinite, sat_grad and sat_act are cleared.  Synchronises the stream. */
+/* resume a dynamic scale: scale in [1, 2^24]; last_skipped, nonfinite, sat_grad and sat_act are cleared.  Synchronises the stream.
+ * Sets both networks' scales and good-step counts too (a single-scale state resumed with "loss_scale_per_network"). */
 int cgvc_set_loss_scale_state(cgvc_handle h, float scale, int good_steps, long long skipped, void* stream);
+/* one network's share of the state with "loss_scale_per_network" (index 0 the generators, 1 the discriminators) */
+typedef struct cgvc_loss_scale_net_info {
+  float scale;                    /* s_G / s_D: the scale the next step's gradients of this network's passes are formed with */
+  int good_steps;                 /* consecutive steps in which this network did not overflow (dynamic) */
+  unsigned long long sat_grad;    /* the last step's saturated 4-value groups in this network's gradient planes (dynamic: summed over ranks) */
+  unsigned long long ufl_grad;    /* ... groups below the fp16 lower edge (see above; dynamic: summed over ranks) */
+  unsigned long long groups;      /* ... groups counted (dynamic: summed over ranks) */
+} cgvc_loss_scale_net_info;
+/* asynchronous: copies both networks' states into info_dev[2] (device memory) on the stream */
+int cgvc_loss_scale_net_state(cgvc_handle h, cgvc_loss_scale_net_info* info_dev, void* stream);
+/* resume one network's dynamic scale: net 0 or 1, scale in [1, 2^24] (net 0 also sets cgvc_loss_scale_info.scale).  Before any scale was
+ * set it calls cgvc_set_loss_scale_state(scale, good_steps, 0) first, so the other network starts from the same scale.  Synchronises the
+ * stream. */
+int cgvc_set_loss_scale_net_state(cgvc_handle h, int net, float scale, int good_steps, void* stream);
 
 /* -- the hot path: replaces CycleGAN.train (model.py:110-125) ------------------------------------------
  * One G step + one D step from the same pre-update weights, then both Adam updates.
@@ -233,7 +261,8 @@ int cgvc_kernel_launches(unsigned long long* count);
  * "post_stream" (default 1): gated layers without pixel shuffle whose samples have 32, 48 or 64 positions take the streaming
  * form of the one-pass GLU / instance-norm backward: persistent CTAs walk (sample, channel block) items through a cp.async double buffer
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
- * "loss_scale" (default 0; 0, 1 or 2) and "loss_scale_growth_interval" (default 2000; >= 1): see cgvc_loss_scale_state.
+ * "loss_scale" (default 0; 0, 1 or 2), "loss_scale_growth_interval" (default 2000; >= 1) and "loss_scale_per_network" (default 0): see
+ * cgvc_loss_scale_state.  Switching "loss_scale_per_network" on while a dynamic scale is in use starts both networks from it.
  * "deterministic" (default 0): 1 makes cgvc_train_step and cgvc_compute_gradients bitwise reproducible on one GPU.  The same inputs,
  * PARAM, ADAM_M / ADAM_V, Adam step, loss-scaler state, batch, frames, precision and options give the same bits of PARAM, GRAD, ADAM_M,
  * ADAM_V, the 8 losses, gen_A / gen_B and the scaler state, in every precision and loss_scale mode, on repeated calls and fresh
@@ -286,6 +315,10 @@ int cgvc_split_planes(cgvc_handle h, int precision, const float* x, long long ro
  *   when that row lies in the same sample, else 0.  dir = +1: the h1 input, -1: the o1 output gradient. */
 int cgvc_im2col_planes(cgvc_handle h, int precision, const float* x, long long rows, int T, int C, int kw, int dir, void* hi, void* lo,
                        unsigned long long* sat, void* stream);
+/* cgvc_set_plane_counters: ufl_groups_dev (device, 2 counters; NULL: none) receives, while it is set, what the F16F8 plane writers of
+ *   cgvc_split_planes, cgvc_im2col_planes, cgvc_in_glu_*_planes, cgvc_glu_*_planes and cgvc_disc_input_forward add to the
+ *   underflow counts of a train step with "loss_scale_per_network": [0] += groups below the fp16 lower edge, [1] += groups counted. */
+int cgvc_set_plane_counters(cgvc_handle h, unsigned long long* ufl_groups_dev);
 /* cgvc_in_glu_forward / _backward with the planes of y [B, R, C] / of dp (layout of p) written by the same kernels:
  *   precision CGVC_PREC_FP32_SIMT writes no planes (hi, lo, sat ignored: the two calls above);
  *   gate 1: the gated form above; gate 0: the residual block's h2 form, p [B, R/shuffle, C*shuffle], y = IN(a) (+ resid [B, R, C] if

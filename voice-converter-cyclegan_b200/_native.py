@@ -36,6 +36,12 @@ class LossScaleInfo(C.Structure):
                 ("nonfinite", C.c_uint), ("sat_grad", C.c_ulonglong), ("sat_act", C.c_ulonglong)]
 
 
+class LossScaleNetInfo(C.Structure):
+    """cgvc_loss_scale_net_info of include/cgvc.h: index 0 the generators, 1 the discriminators"""
+    _fields_ = [("scale", C.c_float), ("good_steps", C.c_int), ("sat_grad", C.c_ulonglong), ("ufl_grad", C.c_ulonglong),
+                ("groups", C.c_ulonglong)]
+
+
 class CgvcError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("libcgvc error %d: %s" % (code, msg))
@@ -59,6 +65,9 @@ def _declare(lib):
         "cgvc_get_adam_step": (ci, [vp, P(C.c_longlong)]),
         "cgvc_loss_scale_state": (ci, [vp, vp, vp]),
         "cgvc_set_loss_scale_state": (ci, [vp, cf, ci, C.c_longlong, vp]),
+        "cgvc_loss_scale_net_state": (ci, [vp, vp, vp]),
+        "cgvc_set_loss_scale_net_state": (ci, [vp, ci, cf, ci, vp]),
+        "cgvc_set_plane_counters": (ci, [vp, vp]),
         "cgvc_train_step": (ci, [vp, vp, vp, ci, ci, cf, cf, cf, cf, vp, vp, vp, vp]),
         "cgvc_compute_gradients": (ci, [vp, vp, vp, ci, ci, cf, cf, vp, vp, vp, vp]),
         "cgvc_adam_step": (ci, [vp, cf, cf, cf, vp]),

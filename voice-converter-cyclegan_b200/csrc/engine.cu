@@ -121,6 +121,7 @@ struct Options {
   int use_graphs = 1;           // "cuda_graph": replay the step as a CUDA graph (turned off when a capture fails)
   int ls_mode = 0;              // "loss_scale": 0 static, 1 monitor (static scale, counters collected), 2 dynamic
   int ls_growth = 2000;         // "loss_scale_growth_interval"
+  int ls_nets = 0;              // "loss_scale_per_network": one scale for the generators' passes, one for the discriminators' D-loss pass
   PostForms post = {1, 1};      // "post_onepass", "post_stream": the forms the instance-norm kernels may take (kernels.cuh)
 };
 
@@ -158,6 +159,9 @@ struct cgvc_engine {
   bool ls_ready = false;        // dynamic mode: ls->scale holds a scale (set on the first step from the static one, or by the caller)
   int ls_batch = 0;             // monitor mode: the batch whose static scale ls->scale reports
   bool counting = false;        // a train step is being enqueued: the plane writers count saturation (ls_mode != 0, F16F8)
+  int ls_net = 0;               // per-network loss scale: the network whose pass is being enqueued (0 generators, 1 discriminators);
+                                // it picks the scale of the loss gradients and the counter block of the gradient-plane writers
+  unsigned long long* plane_ufl = nullptr;   // cgvc_set_plane_counters: [ufl, groups] the per-kernel plane entry points add into
   cudaEvent_t ev_ls = nullptr;  // data parallel: the saturation all-reduce and the GRAD check are done (comm stream)
   // debug taps of the last forward
   std::map<std::string, std::pair<const float*, size_t>> taps;
@@ -349,16 +353,23 @@ static float loss_scale(const cgvc_engine* e, int batch) {
   int l = 0; while ((2 << l) <= batch && l < 9) ++l;       // floor(log2(batch)), capped
   return ldexpf(1.f, 9 + l);
 }
+// option "loss_scale_per_network" in effect: it applies in loss_scale modes 1 and 2, and only F16F8 has a scale other than 1
+static bool ls_nets(const cgvc_engine* e) { return e->opt.ls_nets && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8; }
 // the device copy of loss_scale(e, batch) (d_scalars[16 + floor(log2 batch)], written at creation), or in dynamic mode the scaler's
-// current scale: what the loss-gradient kernels multiply by
+// current scale (per network: that of the pass being enqueued, e->ls_net): what the loss-gradient kernels multiply by
 static const float* loss_scale_dev(const cgvc_engine* e, int batch) {
-  if (e->opt.ls_mode == 2) return &e->ls->scale;
+  if (e->opt.ls_mode == 2) return ls_nets(e) ? &e->ls->net[e->ls_net].scale : &e->ls->scale;
   int l = 0; while ((2 << l) <= batch && l < 9) ++l;
   return e->d_scalars + 16 + l;
 }
-// saturation counters of the plane writers (null: not counted): only F16F8 has reduced-range planes, only train steps are counted
+// saturation counters of the plane writers (null: not counted): only F16F8 has reduced-range planes, only train steps are counted.
+// Per network, the gradient planes count into the block of the pass being enqueued, which also takes their underflow counts
 static unsigned long long* sat_grad(const cgvc_engine* e) {
-  return e->counting && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_grad : nullptr;
+  if (!(e->counting && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8)) return nullptr;
+  return ls_nets(e) ? e->ls->cnt[e->ls_net] : &e->ls->sat_grad;
+}
+static unsigned long long* ufl_grad(const cgvc_engine* e) {
+  return e->counting && ls_nets(e) ? e->ls->cnt[e->ls_net] + 1 : nullptr;
 }
 static unsigned long long* sat_act(const cgvc_engine* e) {
   return e->counting && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8 ? &e->ls->sat_act : nullptr;
@@ -681,7 +692,7 @@ static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const
   q.dp = (!tc || need_fp32) ? S.dP : nullptr;
   if (tc) { q.dp_hi = out.hi; q.dp_lo = out.lo; }
   q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
-  q.sat = sat_grad(e);
+  q.sat = sat_grad(e); q.ufl = ufl_grad(e);
   if (wgrad) q.det = S.det;                 // passes without parameter gradients keep the faster (equally deterministic) forms
   return q;
 }
@@ -738,7 +749,7 @@ static int o1_edge_backward(cgvc_engine* e, const GenNet& N, const float* d_out,
   const int nf = e->cfg.num_features;
   float* Gm = e->G();
   CK(launch_im2col_taps(d_out, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
-                        dz.hi, dz.lo, st, nullptr, 0, sat_grad(e)));
+                        dz.hi, dz.lo, st, nullptr, 0, sat_grad(e), ufl_grad(e)));
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
     return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws, det_of(S)),
                      &N.o1.a, "weight gradient (tap-lowered)"); }));
@@ -786,7 +797,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
     PlanePair dp{nullptr, nullptr};
     if (use_tc(e, N.o1.tc_slot) && u2.xhi && S.dPhi) {
       dp = dp_planes(w, st);
-      CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st, sat_grad(e)));
+      CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st, sat_grad(e), ufl_grad(e)));
     }
     RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, u2, d_out_cl, dp, ws, det_of(S)); }));
     RET(conv_dgrad(e, N.o1, u2, d_out_cl, dp, S.bufA, 0, st));
@@ -851,7 +862,7 @@ static int disc_input_forward(cgvc_engine* e, const C1Layer& c, const float* x, 
                               cudaStream_t st) {
   const GatherGeom g = fwd_geom(n, H, W, c.kh, c.kw, c.sh, c.sw);
   if (fuse) {
-    CK(launch_conv_c1_glu_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat));
+    CK(launch_conv_c1_glu_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat, q.ufl));
     return 0;
   }
   CK(launch_conv_c1_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, st));
@@ -1237,9 +1248,46 @@ int cgvc_set_loss_scale_state(cgvc_handle e, float scale, int good_steps, long l
     return fail(e, CGVC_ERR_ARG, "cgvc_set_loss_scale_state: scale %g outside [1, 2^24] or negative counts", (double)scale);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   const cgvc_loss_scale_info v{scale, good_steps, skipped, 0, 0, 0, 0};     // the last step's flag and counters cleared
+  const LossScaler::Net n{scale, good_steps};                                  // both networks' scales (per-network option)
   CK(cudaMemcpyAsync(e->ls, &v, sizeof v, cudaMemcpyHostToDevice, (cudaStream_t)stream));
-  CK(cudaStreamSynchronize((cudaStream_t)stream));           // v lives on this stack frame
+  for (int k = 0; k < 2; ++k) CK(cudaMemcpyAsync(&e->ls->net[k], &n, sizeof n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  CK(cudaMemsetAsync(e->ls->cnt, 0, sizeof e->ls->cnt, (cudaStream_t)stream));
+  CK(cudaStreamSynchronize((cudaStream_t)stream));           // v and n live on this stack frame
   e->ls_ready = true;
+  return 0;
+}
+
+static_assert(sizeof(cgvc_loss_scale_net_info) == sizeof(LossScaler::Net) + sizeof(unsigned long long[3]) &&
+              offsetof(cgvc_loss_scale_net_info, good_steps) == offsetof(LossScaler::Net, good_steps) &&
+              offsetof(cgvc_loss_scale_net_info, sat_grad) == sizeof(LossScaler::Net) &&
+              offsetof(cgvc_loss_scale_info, good_steps) == offsetof(LossScaler::Net, good_steps),
+              "cgvc_loss_scale_net_info is a LossScaler::Net followed by that network's counters");
+int cgvc_loss_scale_net_state(cgvc_handle e, cgvc_loss_scale_net_info* out_dev, void* stream) {
+  if (!e || !out_dev) return fail(e, CGVC_ERR_ARG, "null argument");
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  for (int k = 0; k < 2; ++k) {
+    CK(cudaMemcpyAsync(&out_dev[k], &e->ls->net[k], sizeof(LossScaler::Net), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    CK(cudaMemcpyAsync(&out_dev[k].sat_grad, e->ls->cnt[k], sizeof e->ls->cnt[k], cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  }
+  return 0;
+}
+int cgvc_set_loss_scale_net_state(cgvc_handle e, int net, float scale, int good_steps, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if ((net != 0 && net != 1) || !(scale >= 1.f && scale <= 16777216.f) || good_steps < 0)
+    return fail(e, CGVC_ERR_ARG, "cgvc_set_loss_scale_net_state: net %d not 0 or 1, scale %g outside [1, 2^24] or negative count", net,
+                (double)scale);
+  // no scale set yet: the other network starts from the same one
+  if (!e->ls_ready) RET(cgvc_set_loss_scale_state(e, scale, good_steps, 0, stream));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  const LossScaler::Net n{scale, good_steps};
+  CK(cudaMemcpyAsync(&e->ls->net[net], &n, sizeof n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  if (net == 0) CK(cudaMemcpyAsync(&e->ls->scale, &scale, sizeof scale, cudaMemcpyHostToDevice, (cudaStream_t)stream));   // scale is s_G
+  CK(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+int cgvc_set_plane_counters(cgvc_handle e, unsigned long long* ufl_groups_dev) {
+  if (!e) return CGVC_ERR_ARG;
+  e->plane_ufl = ufl_groups_dev;
   return 0;
 }
 
@@ -1358,7 +1406,12 @@ static int run_lane(cgvc_engine* e, LanePlan& L, int lane, const float* Yreal_de
   if (gen_out_dev) CK(cudaMemcpyAsync(gen_out_dev, L.din + img, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
   RET(discriminator_forward(e, DN, L.d, L.din, st, false));
   // ---- losses and their gradients (model.py:57-90) ----
-  const float* ls = loss_scale_dev(e, B);                       // scales every gradient of the step (not the loss values); Adam divides it out
+  // the loss scale multiplies every gradient of the step (not the loss values); Adam divides it out.  Per network, the D-loss pass
+  // (its heads and everything they back-propagate) takes s_D, the generators' losses s_G
+  e->ls_net = 0;
+  const float* ls = loss_scale_dev(e, B);
+  e->ls_net = 1;
+  const float* lsD = loss_scale_dev(e, B);
   const DetSlab* det = det_of(L.S);
   CK(launch_l1_loss_grad(L.gcyc.out_cl, X_cl, (long long)img, Ls + 0, sc + 0, L.d_cyc, 0, st, ls, det));     // cycle term
   CK(launch_l1_loss_grad(idY_cl, Y_cl, (long long)img, Ls + 1, sc + 1, L.d_out + img, 0, st, ls, det));      // identity term
@@ -1367,10 +1420,11 @@ static int run_lane(cgvc_engine* e, LanePlan& L, int lane, const float* Yreal_de
   float* Dslot = Ls + (lane == 0 ? 6 : 5);                      // discriminator_loss_B / _A
   float* Gslot = Ls + (lane == 0 ? 2 : 3);                      // generator_loss_A2B / _B2A
   // discriminator loss: real half -> target 1, fake half -> target 0, each weighted 1/2 (model.py:81-88)
-  CK(launch_head_loss_bwd(L.d.prob, Y3, hrows, 1024, Pm + DN.dense_k, 1.f, 0.5f, Dslot, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, ls, det));
+  CK(launch_head_loss_bwd(L.d.prob, Y3, hrows, 1024, Pm + DN.dense_k, 1.f, 0.5f, Dslot, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, lsD, det));
   CK(launch_head_loss_bwd(L.d.prob + hrows, Y3 + hrows * 1024, hrows, 1024, Pm + DN.dense_k, 0.f, 0.5f, Dslot,
-                          L.dY3 + hrows * 1024, Gm + DN.dense_k, Gm + DN.dense_b, st, ls, det));
+                          L.dY3 + hrows * 1024, Gm + DN.dense_k, Gm + DN.dense_b, st, lsD, det));
   RET(discriminator_backward(e, DN, L.d, L.dY3, true, nullptr, L.S, st));
+  e->ls_net = 0;                                                // the rest of the lane is the generators' pass
   // generator adversarial loss on the fake half: target 1 (model.py:68-69); the gradient flows to the fake only
   DiscActs V = disc_view(e, L.d, B, B);
   CK(launch_head_loss_bwd(V.prob, V.d[2].Y, hrows, 1024, Pm + DN.dense_k, 1.f, 1.f, Gslot, L.dY3, nullptr, nullptr, st, ls, det));
@@ -1408,6 +1462,7 @@ static int forward_backward(cgvc_engine* e, const float* A_dev, const float* B_d
   (void)lc;                                                  // lambdas are already in d_scalars[0..1] (set_step_scalars)
   CK(cudaMemsetAsync(L, 0, 8 * sizeof(float), st));
   if (e->opt.ls_mode) CK(cudaMemsetAsync(&e->ls->nonfinite, 0, (char*)(&e->ls->sat_act + 1) - (char*)&e->ls->nonfinite, st));   // this step's counters
+  if (ls_nets(e)) CK(cudaMemsetAsync(e->ls->cnt, 0, sizeof e->ls->cnt, st));
   struct Counting { cgvc_engine* e; ~Counting() { e->counting = false; } } counting{e};
   e->counting = true;
   CK(cudaMemsetAsync(e->G(), 0, e->n_params * sizeof(float), st));
@@ -1477,8 +1532,18 @@ static int ls_check_grads(cgvc_engine* e, cudaStream_t st) {
   CK(launch_check_finite(e->G(), (long long)e->n_params, (long long)e->gen[1].end, &e->ls->nonfinite, st));
   return 0;
 }
+// dynamic mode; per network also monitor mode, where it only sums the networks' counts into sat_grad
 static int ls_update(cgvc_engine* e, cudaStream_t st) {
-  CK(launch_loss_scale_update(e->ls, e->d_scalars + 2, e->cfg.precision == CGVC_PREC_F16F8, e->opt.ls_growth, ADAM_B1, ADAM_B2, st));
+  const int nets = ls_nets(e) ? (e->opt.ls_mode == 2 ? 1 : 2) : 0;
+  CK(launch_loss_scale_update(e->ls, e->d_scalars + 2, e->cfg.precision == CGVC_PREC_F16F8, e->opt.ls_growth, ADAM_B1, ADAM_B2, st, nets));
+  return 0;
+}
+// the saturation counts summed over ranks, so that every rank takes the same decision (dynamic mode): per network both blocks at once
+static int ls_allreduce_counts(cgvc_engine* e, cudaStream_t st) {
+  unsigned long long* c = ls_nets(e) ? e->ls->cnt[0] : &e->ls->sat_grad;
+  const size_t n = ls_nets(e) ? sizeof e->ls->cnt / sizeof(unsigned long long) : 1;
+  int r = e->nccl.AllReduce(c, c, n, 5, 0, e->comm, st);                                                    // ncclUint64, ncclSum
+  if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
   return 0;
 }
 static const int* ls_skip(const cgvc_engine* e) { return e->opt.ls_mode == 2 ? &e->ls->last_skipped : nullptr; }
@@ -1490,6 +1555,7 @@ static int ls_prepare(cgvc_engine* e, int batch, cudaStream_t st) {
   if (!dyn && !mon) return 0;
   const float v[6] = {loss_scale(e, batch), 0, 0, 0, 0, 0};
   CK(launch_set_scalars(&e->ls->scale, 0, 1, v, st));
+  if (ls_nets(e)) for (int k = 0; k < 2; ++k) CK(launch_set_scalars(&e->ls->net[k].scale, 0, 1, v, st));
   e->ls_ready = e->opt.ls_mode == 2; e->ls_batch = e->opt.ls_mode == 1 ? batch : 0;
   return 0;
 }
@@ -1558,7 +1624,11 @@ int cgvc_compute_gradients(cgvc_handle e, const float* A_dev, const float* B_dev
   RET(ls_prepare(e, batch, (cudaStream_t)stream));
   RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, (cudaStream_t)stream));
   // the gradients are handed out, not fed to Adam: remove the loss scale here (in dynamic mode the device scale they were formed with)
-  if (e->opt.ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
+  if (e->opt.ls_mode == 2 && ls_nets(e)) {                 // each GRAD range its own network's scale
+    const long long gend = (long long)e->gen[1].end;
+    CK(launch_scale(e->G(), gend, 1.f, (cudaStream_t)stream, &e->ls->net[0].scale));
+    CK(launch_scale(e->G() + gend, (long long)e->n_params - gend, 1.f, (cudaStream_t)stream, &e->ls->net[1].scale));
+  } else if (e->opt.ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
   else if (loss_scale(e, batch) != 1.f) CK(launch_scale(e->G(), (long long)e->n_params, 1.f / loss_scale(e, batch), (cudaStream_t)stream));
   return 0;
 }
@@ -1637,11 +1707,9 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
     if (e->opt.ls_mode) {
       // every rank takes the same decision: the saturation counts are summed like the gradients (the GRAD check after the sum is
       // consistent by construction), and in dynamic mode each network's Adam waits for the scaler
-      if (e->opt.ls_mode == 2) {
-        int r = e->nccl.AllReduce(&e->ls->sat_grad, &e->ls->sat_grad, 1, 5, 0, e->comm, e->comm_stream);     // ncclUint64, ncclSum
-        if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
-      }
+      if (e->opt.ls_mode == 2) RET(ls_allreduce_counts(e, e->comm_stream));
       RET(ls_check_grads(e, e->comm_stream));
+      if (e->opt.ls_mode == 1 && ls_nets(e)) RET(ls_update(e, e->comm_stream));
       CK(cudaEventRecord(e->ev_ls, e->comm_stream));
       if (e->opt.ls_mode == 2) { CK(cudaStreamWaitEvent(st, e->ev_ls, 0)); RET(ls_update(e, st)); }
     }
@@ -1665,15 +1733,12 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
   }
   if (e->comm) {
     RET(cgvc_allreduce_grads(e, stream));
-    if (e->opt.ls_mode == 2) {
-      int r = e->nccl.AllReduce(&e->ls->sat_grad, &e->ls->sat_grad, 1, 5, 0, e->comm, st);                      // ncclUint64, ncclSum
-      if (r != 0) return fail(e, CGVC_ERR_NCCL, "ncclAllReduce: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(r) : "?");
-    }
+    if (e->opt.ls_mode == 2) RET(ls_allreduce_counts(e, st));
   }
   GraphKey k2; memset(&k2, 0, sizeof k2); k2.kind = 1;
   RET(run_captured(e, k2, st, [&](cudaStream_t s) {
     if (e->opt.ls_mode) RET(ls_check_grads(e, s));
-    if (e->opt.ls_mode == 2) RET(ls_update(e, s));
+    if (e->opt.ls_mode == 2 || ls_nets(e)) RET(ls_update(e, s));
     return adam_body(e, s, ls_skip(e));
   }));
   rollback.armed = false;
@@ -1744,6 +1809,7 @@ static const OptionDef kOptions[] = {
   OPT("debug_taps", 0, 1, opt.debug_taps),          OPT("cuda_graph", 0, 1, opt.use_graphs),
   OPT("post_onepass", 0, 1, opt.post.onepass),      OPT("post_stream", 0, 1, opt.post.stream),
   OPT("loss_scale", 0, 2, opt.ls_mode),             OPT("loss_scale_growth_interval", 1, INT_MAX, opt.ls_growth),
+  OPT("loss_scale_per_network", 0, 1, opt.ls_nets),
   OPT("wgrad_f16", 0, 1, tcw.wgrad16),              OPT("prep_batched", 0, 1, tcw.prep_batched),
   OPT("tc_debug", 0, 7, tcw.debug),
 };
@@ -1766,6 +1832,12 @@ int cgvc_set_option(cgvc_handle e, const char* name, int value) {
     RET(cgvc_set_adam_step(e, t));
     e->ls_ready = false; e->ls_batch = 0;
   }
+  if (field == &e->opt.ls_nets && value && e->ls_ready) {
+    // a dynamic scale in use: both networks continue from it ({scale, good_steps} is the head's layout)
+    DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+    for (int k = 0; k < 2; ++k) CK(cudaMemcpy(&e->ls->net[k], e->ls, sizeof(LossScaler::Net), cudaMemcpyDeviceToDevice));
+  }
+  if (field == &e->opt.ls_nets) e->ls_batch = 0;            // monitor mode writes the networks' static scales on the next step
   *field = value;
   drop_graphs(e);
   return 0;
@@ -1857,7 +1929,7 @@ int cgvc_split_planes(cgvc_handle e, int precision, const float* x, long long ro
   RET(plane_precision(e, precision, hi, lo));
   if (rows < 0 || C < 1) return fail(e, CGVC_ERR_ARG, "cgvc_split_planes: bad shape [%lld, %d]", rows, C);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  CK(tc_split_planes(precision, x, rows, C, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, (cudaStream_t)stream, sat));
+  CK(tc_split_planes(precision, x, rows, C, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, (cudaStream_t)stream, sat, e->plane_ufl));
   return 0;
 }
 
@@ -1869,7 +1941,7 @@ int cgvc_im2col_planes(cgvc_handle e, int precision, const float* x, long long r
     return fail(e, CGVC_ERR_ARG, "cgvc_im2col_planes: bad shape (rows %lld, T %d, C %d, kw %d, dir %d)", rows, T, C, kw, dir);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   CK(launch_im2col_taps(x, rows, T, C, kw, dir, edge_cpad(kw * C), precision == CGVC_PREC_F16F8, hi, lo, (cudaStream_t)stream,
-                        nullptr, 0, sat));
+                        nullptr, 0, sat, e->plane_ufl));
   return 0;
 }
 
@@ -1886,6 +1958,7 @@ int cgvc_in_glu_forward_planes(cgvc_handle e, const float* p, const float* beta_
   q.y = y; q.stats = stats;
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.y_hi = (__nv_bfloat16*)hi; q.y_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
+    q.ufl = q.qmode ? e->plane_ufl : nullptr;
   }
   CK(grow_post_buf(e, (size_t)B * 4 * C, &q.scratch));
   CK(launch_post_fwd(q, e->opt.post, (cudaStream_t)stream));
@@ -1910,6 +1983,7 @@ int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, 
   q.dp = dp; q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = dbeta_g; q.dgamma_g = dgamma_g;
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
+    q.ufl = q.qmode ? e->plane_ufl : nullptr;
   }
   CK(grow_post_buf(e, (size_t)B * 4 * C, &q.scratch));
   CK(launch_post_bwd(q, e->opt.post, (cudaStream_t)stream));
@@ -1993,6 +2067,7 @@ static PostParams glu_fwd_params(cgvc_engine* e, const float* p, float* y, int B
   PostParams q = post_params(e, glu_layer(C), rows_io(B), A, R, true, nullptr);
   q.qmode = precision == CGVC_PREC_F16F8;
   q.sat = q.qmode && hi ? sat : nullptr;
+  q.ufl = q.qmode && hi ? e->plane_ufl : nullptr;
   return q;
 }
 static PostBwdParams glu_bwd_params(cgvc_engine* e, const float* dy, const float* p, float* dp, float* dbias_a, float* dbias_g, int B, int R,
@@ -2003,6 +2078,7 @@ static PostBwdParams glu_bwd_params(cgvc_engine* e, const float* dy, const float
   q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo;
   q.qmode = precision == CGVC_PREC_F16F8;
   q.sat = q.qmode && hi ? sat : nullptr;
+  q.ufl = q.qmode && hi ? e->plane_ufl : nullptr;
   q.dbias_a = dbias_a; q.dbias_g = dbias_g;
   if (dbias_a && det) q.det = *det;
   return q;

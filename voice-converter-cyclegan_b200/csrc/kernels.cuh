@@ -58,6 +58,21 @@ __device__ __forceinline__ void cgvc_count_hits(unsigned long long* ctr, unsigne
   const unsigned n = cg::reduce(g, hits, cg::plus<unsigned>());
   if (n && g.thread_rank() == 0) atomicAdd(ctr, (unsigned long long)n);
 }
+// Whether cgvc_quant4's fp16 plane of 4 values lies below its lower edge: one of them is finite and non-zero while |fp16(x)| < 2^-14, i.e.
+// fp16(x) is subnormal or flushed to zero.  Below that edge an F16F8 product loses a bit per octave (DESIGN.md section 10)
+__device__ __forceinline__ bool cgvc_ufl4(const float (&v)[4]) {
+  bool low = false;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    low |= isfinite(v[k]) && v[k] != 0.f && fabsf(__half2float(__float2half_rn(v[k]))) < 0x1p-14f;
+  return low;
+}
+// The counters of a plane writer for one 4-value group (each null: not counted): sat += cgvc_sat4, ufl[0] += cgvc_ufl4, ufl[1] += 1
+// (the groups counted, so that ufl[0] reads as a fraction).  Activation-role scales
+__device__ __forceinline__ void cgvc_count_planes(unsigned long long* sat, unsigned long long* ufl, const float (&v)[4]) {
+  if (sat) cgvc_count_hits(sat, cgvc_sat4(v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
+  if (ufl) { cgvc_count_hits(ufl, cgvc_ufl4(v)); cgvc_count_hits(ufl + 1, 1u); }
+}
 #endif
 
 // ---- dynamic loss scaling (engine option "loss_scale"; DESIGN.md section 10).  One per engine, in device memory.  The first fields
@@ -74,10 +89,22 @@ struct LossScaler {
   // engine-internal
   long long t;                    // Adam step count (dynamic mode)
   float scale_used;               // the scale the last step's gradients were formed with
+  // option "loss_scale_per_network": [0] the generators, [1] the discriminators.  Net has the layout of the head's first two fields;
+  // cnt[k] = {sat, ufl, groups} of network k's gradient planes in the last step (the writers' targets: sat = cnt[k], ufl = cnt[k] + 1,
+  // see cgvc_count_planes), one contiguous block so that one all-reduce sums both networks' counts over ranks
+  struct Net {
+    float scale;                  // the scale this network's passes form their gradients with
+    int good_steps;               // consecutive steps in which this network's planes and GRAD range did not overflow (dynamic)
+  } net[2];
+  unsigned long long cnt[2][3];
 };
 // the Adam hyper-parameters of both optimizers after a step: hyper = d_scalars + 2 = [lr_G, 1/nranks, lr_D, 1/nranks] as the host wrote
 // them on entry, overwritten with [lr_t G, grad_scale, lr_t D, grad_scale] unless the step is skipped (see simt_kernels.cu)
-cudaError_t launch_loss_scale_update(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, cudaStream_t st);
+// nets = 1: a scale per network (F16F8): the step is skipped when either network overflowed, only an overflowing network's scale halves,
+// each grows after growth_interval of its own good steps, and grad_scale divides by that network's scale.  nets = 2 (monitor mode) only
+// sums the counters: sat_grad = cnt[0][0] + cnt[1][0]
+cudaError_t launch_loss_scale_update(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, cudaStream_t st,
+                                     int nets = 0);
 // nonfinite |= (bit 0 if a non-finite value lies in g[0, cut), bit 1 if in g[cut, n))
 cudaError_t launch_check_finite(const float* g, long long n, long long cut, unsigned* nonfinite, cudaStream_t st);
 
@@ -182,6 +209,7 @@ struct PostParams {
   // rows in all (the planes' extent is seg_rows * C); R = the longest sample (grid size).  launch_post_fwd only
   PackGeom seg; long long seg_rows;
   unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
+  unsigned long long* ufl;              // qmode: [ufl, groups] of the planes (cgvc_count_planes), or null
 };
 // Which forms of the kernels a launch may take (the engine's options "post_onepass" and "post_stream", include/cgvc.h).
 // onepass: samples of <= 64 positions take the one-pass backward kernel, else always sums + apply.  stream: the layer shapes that
@@ -203,6 +231,7 @@ struct PostBwdParams {
   int qmode;                            // 1: dp_hi / dp_lo are F16F8 planes (q16; q8hi followed by q8lo) with the activation-role scales
   float* scratch;                       // [B,4,C] fp32 workspace (required when has_in)
   unsigned long long* sat;              // qmode: count of saturated 4-value groups of the planes (cgvc_quant4_sat), or null
+  unsigned long long* ufl;              // qmode: [ufl, groups] of the planes (cgvc_count_planes), or null
   DetSlab det;                          // deterministic mode (det.p != null): the sums + apply form, parameter and bias gradients reduced in order
 };
 cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st);
@@ -252,17 +281,18 @@ cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float*
 // fp32 [M, C] (row stride ld) -> zero-padded bf16 hi/lo planes [M, Cpad]
 cudaError_t launch_pad_split(const float* x, long long M, int C, int ld, int Cpad, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st);
 // same into F16F8 planes: q16 [M, Cpad] halves, q8 = [M*Cpad bytes of q8hi | M*Cpad bytes of q8lo] (activation scales)
-// sat (may be null): count of saturated 4-value groups (cgvc_quant4_sat)
+// sat (may be null): count of saturated 4-value groups (cgvc_quant4_sat); ufl (may be null): [ufl, groups] (cgvc_count_planes)
 cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st,
-                               unsigned long long* sat = nullptr);
+                               unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr);
 // tap lowering of the generator's 15-tap edge layers (simt_kernels.cu): im2col of a narrow channels-last tensor over the taps of a
 // stride-1 1-D TF-SAME convolution into operand planes [M, Cpad] (qmode 1: F16F8 planes q16 / q8hi|q8lo, else bf16 hi / lo), dir = +1:
 // out[m, t*C + c] = x[m + t - pl, c], dir = -1: x[m - t + pl, c] (zero outside the sample, pl = (kw - 1) / 2), and the matching sum
 // y[m, c] = bias[c] + sum_t z[m + dir*(t - pl), t*C + c]
 // With off (n + 1 device frame prefix sums, packed utterances) the samples are [off[u], off[u+1]) instead of T-row blocks (T ignored).
-// sat (qmode, may be null): count of saturated 4-value groups (cgvc_quant4_sat)
+// sat (qmode, may be null): count of saturated 4-value groups (cgvc_quant4_sat); ufl (qmode, may be null): [ufl, groups]
 cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st,
-                               const long long* off = nullptr, int n_off = 0, unsigned long long* sat = nullptr);
+                               const long long* off = nullptr, int n_off = 0, unsigned long long* sat = nullptr,
+                               unsigned long long* ufl = nullptr);
 cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st,
                                const long long* off = nullptr, int n_off = 0);
 // P[m, 0:2*cout] = [bias_a | bias_g] + sum_t x[src(m,t)] * [wa | wg][t]   (single input channel, TF kernels [taps][1][cout])
@@ -273,7 +303,7 @@ cudaError_t launch_conv_c1_fwd(const GatherGeom& g, const float* x, const float*
 // operand planes (bf16 hi / lo, or with qmode the F16F8 planes q16; q8hi followed by q8lo); <= 9 taps
 cudaError_t launch_conv_c1_glu_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                                    int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st,
-                                   unsigned long long* sat = nullptr);
+                                   unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr);
 
 // s[off .. off+n) = v6_host[0..n)  (n <= 6), passed by value in the kernel arguments (no host-memory copy node)
 cudaError_t launch_set_scalars(float* s, int off, int n, const float* v6_host, cudaStream_t st);

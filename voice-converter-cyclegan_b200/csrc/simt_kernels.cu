@@ -433,16 +433,16 @@ __device__ __forceinline__ void st4_split(__nv_bfloat16* hi, __nv_bfloat16* lo, 
   *reinterpret_cast<uint2*>(hi) = hv;
   *reinterpret_cast<uint2*>(lo) = lv;
 }
-// F16F8 planes of 4 consecutive activation values (o = element offset, n = elements per plane); sat: see cgvc_count_hits (null: no count)
+// F16F8 planes of 4 consecutive activation values (o = element offset, n = elements per plane); sat, ufl: see cgvc_count_planes
 __device__ __forceinline__ void st4_quant(__nv_bfloat16* q16, __nv_bfloat16* q8, long long o, long long n, const F4& a,
-                                          unsigned long long* sat = nullptr) {
+                                          unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr) {
   uint2 h; uint32_t b_hi, b_lo;
   cgvc_quant4(a.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO, h, b_hi, b_lo);
   *reinterpret_cast<uint2*>(q16 + o) = h;
   uint8_t* base = reinterpret_cast<uint8_t*>(q8);
   *reinterpret_cast<uint32_t*>(base + o) = b_hi;
   *reinterpret_cast<uint32_t*>(base + n + o) = b_lo;
-  if (sat) cgvc_count_hits(sat, cgvc_sat4(a.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
+  cgvc_count_planes(sat, ufl, a.v);
 }
 __device__ __forceinline__ F4 zero4() { return F4{{0.f, 0.f, 0.f, 0.f}}; }
 __device__ __forceinline__ F4 one4() { return F4{{1.f, 1.f, 1.f, 1.f}}; }
@@ -454,6 +454,10 @@ __device__ __forceinline__ void atomic_add4(float* p, const F4& a) {
 // kernel's uncounted path alone
 __device__ __noinline__ unsigned sat_groups(const F4 da, const F4 dg, bool gate) {
   return cgvc_sat4(da.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO) + (gate && cgvc_sat4(dg.v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
+}
+// ... and their groups below the fp16 lower edge (cgvc_ufl4)
+__device__ __noinline__ unsigned ufl_groups(const F4 da, const F4 dg, bool gate) {
+  return cgvc_ufl4(da.v) + (gate && cgvc_ufl4(dg.v));
 }
 
 constexpr int kPostRows = 32;      // positions per CTA
@@ -596,7 +600,7 @@ post_apply_fwd_kernel(const __grid_constant__ PostParams q, const float* __restr
         for (int k = 0; k < 4; ++k) y.v[k] += rr.v[k]; }
       if (q.y) st4(q.y + o, y);
       if (q.y_hi) {
-        if (q.qmode) st4_quant(q.y_hi, q.y_lo, o, PK ? q.seg_rows * q.C : (long long)q.B * q.R * q.C, y, q.sat);
+        if (q.qmode) st4_quant(q.y_hi, q.y_lo, o, PK ? q.seg_rows * q.C : (long long)q.B * q.R * q.C, y, q.sat, q.ufl);
         else st4_split(q.y_hi + o, q.y_lo + o, y);
       }
     }
@@ -717,7 +721,7 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
   const float* pb = q.p + (long long)ix.b * Rw * q.ldp;
   const long long dpoff = (long long)ix.b * Rw * q.ldp;
   F4 bsum[2] = {zero4(), zero4()};                      // this thread's share of the conv-bias gradients (a, g)
-  unsigned nsat = 0;                                     // saturated plane groups (q.sat), added to the counter after the loop
+  unsigned nsat = 0, nufl = 0, ngrp = 0;                 // plane groups counted for q.sat / q.ufl, added to the counters after the loop
   if (ix.cvalid) {
     // per channel (Appendix A.7):  xhat = x*r + h ; norm = x*sc + of ; dx = c1*dn - c2 - xhat*c3
     F4 ra = one4(), ha = zero4(), sca = one4(), ofa = zero4(), c1a = one4(), c2a = zero4(), c3a = zero4();
@@ -782,6 +786,7 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
             st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da);
             if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg);
             if (q.sat) nsat += sat_groups(da, dg, HAS_GATE);
+            if (q.ufl) { nufl += ufl_groups(da, dg, HAS_GATE); ngrp += HAS_GATE ? 2 : 1; }
           } else {
             st4_split(q.dp_hi + dpoff + a, q.dp_lo + dpoff + a, da);
             if (HAS_GATE) st4_split(q.dp_hi + dpoff + a + q.Cc, q.dp_lo + dpoff + a + q.Cc, dg);
@@ -791,6 +796,7 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
     }
   }
   if (q.sat) cgvc_count_hits(q.sat, nsat);
+  if (q.ufl) { cgvc_count_hits(q.ufl, nufl); cgvc_count_hits(q.ufl + 1, ngrp); }
   if (q.dbias_a) {
     // positions of lane rl have shuffle phase rl % sh (chunk size and lane stride are even): reduce per phase
     red[0][ix.rl][lane] = make_float4(bsum[0].v[0], bsum[0].v[1], bsum[0].v[2], bsum[0].v[3]);
@@ -919,8 +925,8 @@ post_bwd_onepass_kernel(const __grid_constant__ PostBwdParams q) {
         if (q.dp_hi) {
           if (q.qmode) {                                     // F16F8 gradient planes (activation-role scales): q16, then q8hi | q8lo
             const long long nq = (long long)q.B * Rw * q.ldp;
-            st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da, q.sat);
-            if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg, q.sat);
+            st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da, q.sat, q.ufl);
+            if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg, q.sat, q.ufl);
           } else {
             st4_split(q.dp_hi + dpoff + a, q.dp_lo + dpoff + a, da);
             if (HAS_GATE) st4_split(q.dp_hi + dpoff + a + q.Cc, q.dp_lo + dpoff + a + q.Cc, dg);
@@ -1104,7 +1110,7 @@ post_bwd_stream_kernel(const __grid_constant__ PostBwdParams q, int items, int c
       const long long a = dpoff + (long long)(r >> shs) * q.ldp + (r & shs) * q.C;
       if (q.dp) { st4(q.dp + a, da); if (GATE) st4(q.dp + a + q.Cc, dg); }
       if (q.dp_hi) {
-        if (q.qmode) { st4_quant(q.dp_hi, q.dp_lo, a, nplane, da, q.sat); if (GATE) st4_quant(q.dp_hi, q.dp_lo, a + q.Cc, nplane, dg, q.sat); }
+        if (q.qmode) { st4_quant(q.dp_hi, q.dp_lo, a, nplane, da, q.sat, q.ufl); if (GATE) st4_quant(q.dp_hi, q.dp_lo, a + q.Cc, nplane, dg, q.sat, q.ufl); }
         else { st4_split(q.dp_hi + a, q.dp_lo + a, da); if (GATE) st4_split(q.dp_hi + a + q.Cc, q.dp_lo + a + q.Cc, dg); }
       }
     }
@@ -1243,7 +1249,7 @@ post_fwd_stream_kernel(const __grid_constant__ PostParams q, int items, int cblo
       const long long e = ((long long)b * R + r) * q.C + c;
       if (q.y) st4(q.y + e, y);
       if (q.y_hi) {
-        if (q.qmode) st4_quant(q.y_hi, q.y_lo, e, nplane, y, q.sat);
+        if (q.qmode) st4_quant(q.y_hi, q.y_lo, e, nplane, y, q.sat, q.ufl);
         else st4_split(q.y_hi + e, q.y_lo + e, y);
       }
     }
@@ -1632,7 +1638,42 @@ cudaError_t launch_check_finite(const float* g, long long n, long long cut, unsi
 // (the precisions without reduced-range gradient planes): the scale stays where it is and only the skip applies.  lr_t uses the same
 // double-precision formula as the host's set_adam_scalars (engine.cu); CUDA's pow is within 2 ulp, not correctly rounded, so the fp32
 // result can differ from the host's in the last bit when the double lies at an fp32 rounding boundary.
-__global__ void loss_scale_update_kernel(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2) {
+// nets = 1: one scale per network (option "loss_scale_per_network"; net 0 the generators, 1 the discriminators).  Network k overflowed
+// when its planes saturated or its GRAD range (nonfinite bit k) holds a non-finite value: its scale halves (floor 1) and its good-step
+// count resets; otherwise that count advances and after growth_interval such steps its scale doubles (cap 2^24).  The step is skipped,
+// both optimizers alike, when either network overflowed, and each optimizer's grad_scale divides by its own network's scale.  The head
+// of the state keeps its meaning: scale = s_G, sat_grad = both networks' saturated groups, good_steps = consecutive steps not skipped.
+// nets = 2 (per network, monitor mode): the sum into sat_grad only.
+__device__ void loss_scale_update_nets(LossScaler* s, float* hyper, int nets, int growth_interval, float beta1, float beta2) {
+  s->sat_grad = s->cnt[0][0] + s->cnt[1][0];
+  if (nets == 2) return;
+  const float used[2] = {s->net[0].scale, s->net[1].scale};
+  bool skip = false;
+  for (int k = 0; k < 2; ++k) {
+    LossScaler::Net& n = s->net[k];
+    if (s->cnt[k][0] > 0 || ((s->nonfinite >> k) & 1u)) {
+      skip = true; n.good_steps = 0; n.scale = fmaxf(1.f, used[k] * 0.5f);
+    } else if (++n.good_steps >= growth_interval) {
+      n.good_steps = 0; n.scale = fminf(16777216.f, used[k] * 2.f);
+    }
+  }
+  s->scale = s->net[0].scale;
+  s->scale_used = used[0];
+  if (skip) {
+    s->last_skipped = 1; s->good_steps = 0; s->skipped += 1;
+    return;
+  }
+  s->last_skipped = 0;
+  s->t += 1;
+  s->good_steps += 1;
+  const double t = (double)s->t;
+  const double corr = sqrt(1.0 - pow((double)beta2, t)) / (1.0 - pow((double)beta1, t));
+  hyper[0] = (float)(hyper[0] * corr); hyper[1] = hyper[1] / used[0];   // generator optimizer: lr -> lr_t, 1/nranks -> 1/(nranks s_G)
+  hyper[2] = (float)(hyper[2] * corr); hyper[3] = hyper[3] / used[1];   // discriminator optimizer: 1/(nranks s_D)
+}
+
+__global__ void loss_scale_update_kernel(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, int nets) {
+  if (nets) { loss_scale_update_nets(s, hyper, nets, growth_interval, beta1, beta2); return; }
   const float used = s->scale;
   s->scale_used = used;
   if (s->sat_grad > 0 || s->nonfinite) {
@@ -1652,8 +1693,9 @@ __global__ void loss_scale_update_kernel(LossScaler* s, float* hyper, int adapt,
   hyper[2] = (float)(hyper[2] * corr); hyper[3] = hyper[3] / used;      // discriminator optimizer
 }
 
-cudaError_t launch_loss_scale_update(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, cudaStream_t st) {
-  ++g_cgvc_launches; loss_scale_update_kernel<<<1, 1, 0, st>>>(s, hyper, adapt, growth_interval, beta1, beta2);
+cudaError_t launch_loss_scale_update(LossScaler* s, float* hyper, int adapt, int growth_interval, float beta1, float beta2, cudaStream_t st,
+                                     int nets) {
+  ++g_cgvc_launches; loss_scale_update_kernel<<<1, 1, 0, st>>>(s, hyper, adapt, growth_interval, beta1, beta2, nets);
   return cudaGetLastError();
 }
 
@@ -2044,7 +2086,7 @@ pad_split_kernel(const float* __restrict__ x, long long M, int C, int ld, int Cp
 // fp32 rows [M, C] -> F16F8 planes [M, Cpad] (Cpad a multiple of 4), zero channels [C, Cpad)
 __global__ void __launch_bounds__(256)
 pad_split_q_kernel(const float* __restrict__ x, long long M, int C, int ld, int Cpad, __half* __restrict__ q16, uint8_t* __restrict__ q8,
-                   unsigned long long* __restrict__ sat) {
+                   unsigned long long* __restrict__ sat, unsigned long long* __restrict__ ufl) {
   const long long n = M * Cpad, nq = n / 4;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nq; i += (long long)gridDim.x * 256) {
     const long long e = i * 4; const int c = (int)(e % Cpad); const long long m = e / Cpad;
@@ -2056,16 +2098,17 @@ pad_split_q_kernel(const float* __restrict__ x, long long M, int C, int ld, int 
     *reinterpret_cast<uint2*>(q16 + e) = h;
     *reinterpret_cast<uint32_t*>(q8 + e) = b_hi;
     *reinterpret_cast<uint32_t*>(q8 + n + e) = b_lo;
-    if (sat) cgvc_count_hits(sat, cgvc_sat4(v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
+    cgvc_count_planes(sat, ufl, v);
   }
 }
 
-cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st, unsigned long long* sat) {
+cudaError_t launch_pad_split_q(const float* x, long long M, int C, int ld, int Cpad, void* q16, void* q8, cudaStream_t st, unsigned long long* sat,
+                               unsigned long long* ufl) {
   if (M == 0) return cudaSuccess;
   if (Cpad % 4) return cudaErrorInvalidValue;
   long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
-  pad_split_q_kernel<<<(unsigned)nb, 256, 0, st>>>(x, M, C, ld, Cpad, (__half*)q16, (uint8_t*)q8, sat);
+  pad_split_q_kernel<<<(unsigned)nb, 256, 0, st>>>(x, M, C, ld, Cpad, (__half*)q16, (uint8_t*)q8, sat, ufl);
   return cudaGetLastError();
 }
 
@@ -2101,7 +2144,8 @@ __device__ __forceinline__ int tap_sample(long long m, int T, const long long* _
 template <int Q>
 __global__ void __launch_bounds__(256)
 im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int kw, int pl, int dir, int Cpad, void* __restrict__ hi, void* __restrict__ lo,
-                   const long long* __restrict__ off, int n_off, unsigned long long* __restrict__ sat) {
+                   const long long* __restrict__ off, int n_off, unsigned long long* __restrict__ sat,
+                   unsigned long long* __restrict__ ufl) {
   const long long n = M * Cpad, nq = n / 4;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nq; i += (long long)gridDim.x * 256) {
     const long long e = i * 4; const int col = (int)(e % Cpad); const long long m = e / Cpad;
@@ -2118,7 +2162,7 @@ im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int k
       *reinterpret_cast<uint2*>((__half*)hi + e) = h;
       *reinterpret_cast<uint32_t*>((uint8_t*)lo + e) = b_hi;
       *reinterpret_cast<uint32_t*>((uint8_t*)lo + n + e) = b_lo;
-      if (sat) cgvc_count_hits(sat, cgvc_sat4(v, CGVC_Q_ACT_SHI, CGVC_Q_ACT_SLO));
+      cgvc_count_planes(sat, ufl, v);
     } else {
       __align__(8) __nv_bfloat16 h[4]; __align__(8) __nv_bfloat16 l[4];
 #pragma unroll
@@ -2130,14 +2174,14 @@ im2col_taps_kernel(const float* __restrict__ x, long long M, int T, int C, int k
 }
 
 cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw, int dir, int Cpad, int qmode, void* hi, void* lo, cudaStream_t st,
-                               const long long* off, int n_off, unsigned long long* sat) {
+                               const long long* off, int n_off, unsigned long long* sat, unsigned long long* ufl) {
   if (M == 0) return cudaSuccess;
   if (C % 4 || Cpad % 4 || Cpad < kw * C || (!off && (T <= 0 || M % T)) || (off && n_off < 1)) return cudaErrorInvalidValue;
   const int pl = (kw - 1) / 2;                      // TF SAME at stride 1: total pad kw - 1, the smaller half on the left
   long long n = M * Cpad / 4; long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 16) nb = CGVC_NUM_SMS * 16;
   ++g_cgvc_launches;
-  if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off, sat);
-  else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off, nullptr);
+  if (qmode) im2col_taps_kernel<1><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off, sat, ufl);
+  else im2col_taps_kernel<0><<<(unsigned)nb, 256, 0, st>>>(x, M, T, C, kw, pl, dir, Cpad, hi, lo, off, n_off, nullptr, nullptr);
   return cudaGetLastError();
 }
 
@@ -2231,7 +2275,7 @@ __global__ void __launch_bounds__(256)
 conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ x, const float* __restrict__ wa, const float* __restrict__ wg,
                        const float* __restrict__ ba, const float* __restrict__ bg, int cout, float* __restrict__ P,
                        float* __restrict__ y, __nv_bfloat16* __restrict__ y_hi, __nv_bfloat16* __restrict__ y_lo, int qmode, long long plane_elems,
-                       int rows_per_block, unsigned long long* __restrict__ sat) {
+                       int rows_per_block, unsigned long long* __restrict__ sat, unsigned long long* __restrict__ ufl) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   const int nq = cout / 4;                             // channel quads (host guarantees nq divides 256)
   const int cq = threadIdx.x % nq, rl = threadIdx.x / nq, rstep = 256 / nq;
@@ -2269,7 +2313,7 @@ conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __rest
       const long long e = m * cout + n;
       if (y) st4(y + e, o);
       if (y_hi) {
-        if (qmode) st4_quant(y_hi, y_lo, e, plane_elems, o, sat);
+        if (qmode) st4_quant(y_hi, y_lo, e, plane_elems, o, sat, ufl);
         else st4_split(y_hi + e, y_lo + e, o);
       }
     }
@@ -2278,14 +2322,14 @@ conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __rest
 
 cudaError_t launch_conv_c1_glu_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                                    int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st,
-                                   unsigned long long* sat) {
+                                   unsigned long long* sat, unsigned long long* ufl) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = cout / 4;
   if (cout % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9) return cudaErrorInvalidValue;
   int rpb = 4 * kC1Rows;
   ++g_cgvc_launches;
-  conv_c1_glu_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode, M * cout, rpb, sat);
+  conv_c1_glu_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode, M * cout, rpb, sat, ufl);
   return cudaGetLastError();
 }
 

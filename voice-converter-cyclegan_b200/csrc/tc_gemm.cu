@@ -1899,8 +1899,8 @@ int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, si
 }
 
 cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st,
-                            unsigned long long* sat) {
-  return precision == 3 ? launch_pad_split_q(x, rows, C, C, ru(C, 128), hi, lo, st, sat) : launch_pad_split(x, rows, C, C, ru(C, 64), hi, lo, st);
+                            unsigned long long* sat, unsigned long long* ufl) {
+  return precision == 3 ? launch_pad_split_q(x, rows, C, C, ru(C, 128), hi, lo, st, sat, ufl) : launch_pad_split(x, rows, C, C, ru(C, 64), hi, lo, st);
 }
 
 int tc_conv_fwd(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,

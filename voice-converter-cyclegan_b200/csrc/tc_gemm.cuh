@@ -82,9 +82,9 @@ int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, si
 
 // x [rows, C] fp32 -> the operand planes of `precision` with C zero-padded to the contraction width: bf16 hi / lo [rows, ru64(C)],
 // F16F8: q16 (hi) and q8hi followed by q8lo (lo) [rows, ru128(C)].  cudaError_t
-// sat (F16F8, may be null): count of saturated 4-value groups of the planes (kernels.cuh cgvc_quant4_sat)
+// sat (F16F8, may be null): count of saturated 4-value groups of the planes (kernels.cuh cgvc_quant4_sat); ufl: [ufl, groups] likewise
 cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st,
-                            unsigned long long* sat = nullptr);
+                            unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr);
 
 // The slot-based calls below read and write the planes of w.precision (tc_split_planes), with their channel count rounded up
 // (zero-filled): x [n,H,W,cin], dP [rows, Ntot].  They return 0, TC_UNSUPPORTED (no launch: the shape has no tensor-core form)

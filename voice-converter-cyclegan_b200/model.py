@@ -12,7 +12,9 @@ Differences a user of the reference should know:
   * with `torch.distributed` initialised and `data_parallel=True`, one process per GPU trains data-parallel:
     a single NCCL all-reduce of the flat gradient arena per step
   * `loss_scale='monitor'` counts saturated F16F8 gradient / activation planes and non-finite gradients every step;
-    `loss_scale='dynamic'` also skips such steps and adapts the loss scale (include/cgvc.h, DESIGN.md section 10)
+    `loss_scale='dynamic'` also skips such steps and adapts the loss scale (include/cgvc.h, DESIGN.md section 10);
+    `loss_scale_per_network=True` gives the generators and the discriminators a scale each and counts their planes apart, with the
+    groups below the fp16 lower edge beside the saturated ones (F16F8 only)
   * `deterministic=True` makes every train step bit-reproducible on one GPU: the same weights, Adam and loss-scale state and inputs give
     the same bits whatever the stream schedule or CUDA-graph replay, so a rerun of a seed or a resumed checkpoint follows the
     same trajectory (include/cgvc.h option "deterministic", DESIGN.md section 11; the NCCL sum of a data-parallel step is not covered)
@@ -40,7 +42,7 @@ class CycleGAN(object):
 
     def __init__(self, num_features, discriminator=_discriminator, generator=_generator_gatedcnn, mode='train',
                  log_dir='./log', *, max_batch=1, max_frames=None, precision='bf16x3', device=None, seed=0,
-                 data_parallel=False, summary_interval=0, loss_scale='static', deterministic=False):
+                 data_parallel=False, summary_interval=0, loss_scale='static', deterministic=False, loss_scale_per_network=False):
         for net in (discriminator, generator):
             if not hasattr(net, "check_engine_table"):
                 raise TypeError("CycleGAN(discriminator=..., generator=...) takes network descriptors (cgvc.module.generator_gatedcnn / "
@@ -66,6 +68,8 @@ class CycleGAN(object):
             raise ValueError("loss_scale must be one of %s, got %r" % (sorted(N.LOSS_SCALE_MODES), loss_scale))
         if loss_scale != 'static':
             self._options["loss_scale"] = N.LOSS_SCALE_MODES[loss_scale]     # applied by _create_engine, like any remembered option
+        if loss_scale_per_network:
+            self._options["loss_scale_per_network"] = 1
         if deterministic:
             self._options["deterministic"] = 1
         self.last_step_skipped = False
@@ -132,6 +136,8 @@ class CycleGAN(object):
         self._losses_host = torch.zeros(8, dtype=torch.float32).pin_memory()
         self._ls_dev = torch.zeros(C.sizeof(N.LossScaleInfo), dtype=torch.uint8, device=self.device)
         self._ls_host = torch.zeros(C.sizeof(N.LossScaleInfo), dtype=torch.uint8).pin_memory()
+        self._lsn_dev = torch.zeros(2 * C.sizeof(N.LossScaleNetInfo), dtype=torch.uint8, device=self.device)
+        self._lsn_host = torch.zeros(2 * C.sizeof(N.LossScaleNetInfo), dtype=torch.uint8).pin_memory()
         self._staging = {}
         for name, value in self._options.items():            # the engine is re-created when batch / frames outgrow it
             self._chk(self._lib.cgvc_set_option(self._handle, name.encode(), int(value)))
@@ -160,22 +166,38 @@ class CycleGAN(object):
         mode = self._options.get("loss_scale", 0)
         return next(k for k, v in N.LOSS_SCALE_MODES.items() if v == mode)
 
+    @property
+    def loss_scale_per_network(self):
+        """engine option "loss_scale_per_network": a loss scale each for the generators and the discriminators"""
+        return bool(self._options.get("loss_scale_per_network", 0))
+
     def _enqueue_loss_scale_state(self):
         self._chk(self._lib.cgvc_loss_scale_state(self._handle, _ptr(self._ls_dev), self._stream()))
         self._ls_host.copy_(self._ls_dev, non_blocking=True)
+        if self.loss_scale_per_network:
+            self._chk(self._lib.cgvc_loss_scale_net_state(self._handle, _ptr(self._lsn_dev), self._stream()))
+            self._lsn_host.copy_(self._lsn_dev, non_blocking=True)
 
     def _read_loss_scale_state(self):
         """after the stream synchronisation that follows _enqueue_loss_scale_state"""
         info = N.LossScaleInfo.from_buffer_copy(self._ls_host.numpy().tobytes())
         self.last_loss_scale = {f: getattr(info, f) for f, _ in N.LossScaleInfo._fields_}
         self.last_loss_scale["last_skipped"] = bool(info.last_skipped)
+        if self.loss_scale_per_network:
+            nets = (N.LossScaleNetInfo * 2).from_buffer_copy(self._lsn_host.numpy().tobytes())
+            for net, tag in zip(nets, ("G", "D")):
+                self.last_loss_scale.update({"scale_" + tag: net.scale, "good_steps_" + tag: net.good_steps,
+                                             "sat_grad_" + tag: net.sat_grad, "ufl_grad_" + tag: net.ufl_grad,
+                                             "groups_" + tag: net.groups})
         self.last_step_skipped = self.last_loss_scale["last_skipped"]
         return dict(self.last_loss_scale)
 
     def loss_scale_state(self):
         """The loss scaler's state after the most recent step (synchronises): scale, good_steps, skipped, last_skipped and the last
         step's sat_grad / sat_act (saturated 4-value groups of the F16F8 gradient / activation planes) and nonfinite (bit 0: a
-        generator gradient, bit 1: a discriminator gradient).  The counters are collected in 'monitor' and 'dynamic' mode only."""
+        generator gradient, bit 1: a discriminator gradient).  The counters are collected in 'monitor' and 'dynamic' mode only.
+        With loss_scale_per_network also, per network (suffix _G the generators, _D the discriminators): scale, good_steps and the
+        last step's sat_grad, ufl_grad (groups whose fp16 plane is subnormal or flushed) and groups (all counted)."""
         self._enqueue_loss_scale_state()
         torch.cuda.current_stream(self.device).synchronize()
         return self._read_loss_scale_state()
@@ -195,12 +217,20 @@ class CycleGAN(object):
         self._lib.cgvc_set_adam_step(self._handle, step)
         if ls is not None and ls["scale"] >= 1:
             self._chk(self._lib.cgvc_set_loss_scale_state(self._handle, ls["scale"], ls["good_steps"], ls["skipped"], self._stream()))
+            if self.loss_scale_per_network:
+                self._set_net_scales(ls)
         if self._data_parallel:
             # cgvc_destroy freed the NCCL communicator with the old engine: a data-parallel model must get a new one, or it would
             # silently train without the all-reduce.  Collective: every rank has to grow in the same call (same batch / frames).
             self._attach_communicator()
         else:
             self._params_updated()
+
+    def _set_net_scales(self, ls):
+        for k, tag in enumerate(("G", "D")):
+            if ls.get("scale_" + tag, 0) >= 1:
+                self._chk(self._lib.cgvc_set_loss_scale_net_state(self._handle, k, float(ls["scale_" + tag]),
+                                                                  int(ls["good_steps_" + tag]), self._stream()))
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
@@ -470,6 +500,9 @@ class CycleGAN(object):
             blob["loss_scale"] = np.float32(ls["scale"])
             blob["loss_scale_good_steps"] = np.int64(ls["good_steps"])
             blob["loss_scale_skipped"] = np.int64(ls["skipped"])
+            for tag in ("G", "D") if self.loss_scale_per_network else ():
+                blob["loss_scale_" + tag] = np.float32(ls["scale_" + tag])
+                blob["loss_scale_good_steps_" + tag] = np.int64(ls["good_steps_" + tag])
         blob["train_step"] = np.int64(self.train_step)
         with open(path + ".npz" if not path.endswith(".npz") else path, "wb") as f:
             np.savez(f, **blob)
@@ -494,8 +527,16 @@ class CycleGAN(object):
         if "train_step" in z:
             self.train_step = int(z["train_step"])
         if self.loss_scale == 'dynamic' and "loss_scale" in z and float(z["loss_scale"]) >= 1:
+            # a single-scale checkpoint sets both networks' scales; a per-network one then sets each
             self._chk(self._lib.cgvc_set_loss_scale_state(self._handle, float(z["loss_scale"]), int(z["loss_scale_good_steps"]),
                                                           int(z["loss_scale_skipped"]), self._stream()))
+            if self.loss_scale_per_network:
+                ls = {}
+                for tag in ("G", "D"):
+                    if "loss_scale_" + tag in z:
+                        ls["scale_" + tag] = float(z["loss_scale_" + tag])
+                        ls["good_steps_" + tag] = int(z["loss_scale_good_steps_" + tag])
+                self._set_net_scales(ls)
         self._params_updated()
 
     def _load_tf_bundle(self, prefix):

@@ -151,18 +151,25 @@ def loss_scale_log(model, loss_scale):
     ls = model.last_loss_scale if loss_scale != 'static' else None
     if not ls:
         return ''
+    if 'scale_G' in ls:                                           # loss_scale_per_network: both scales, the underflow fractions
+        frac = lambda tag: ls['ufl_grad_' + tag] / ls['groups_' + tag] if ls['groups_' + tag] else 0.0
+        return (', Loss Scale (G / D): {:g} / {:g}, Skipped Steps: {:d}, Saturated Groups (gradient G / D, activation): {:d} / {:d}, '
+                '{:d}, Underflow Fraction (G / D): {:.2e} / {:.2e}{}').format(
+            ls['scale_G'], ls['scale_D'], ls['skipped'], ls['sat_grad_G'], ls['sat_grad_D'], ls['sat_act'], frac('G'), frac('D'),
+            ', Non-finite Gradients' if ls['nonfinite'] else '')
     return ', Loss Scale: {:g}, Skipped Steps: {:d}, Saturated Groups (gradient / activation): {:d} / {:d}{}'.format(
         ls['scale'], ls['skipped'], ls['sat_grad'], ls['sat_act'], ', Non-finite Gradients' if ls['nonfinite'] else '')
 
 
 def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epochs, mini_batch_size, synthetic=0,
           precision="bf16x3", log_every=50, device_data=True, validation_A_dir=None, validation_B_dir=None, output_dir='./validation_output',
-          tensorboard_log_dir='./log', loss_scale='static', deterministic=False):
+          tensorboard_log_dir='./log', loss_scale='static', deterministic=False, loss_scale_per_network=False):
     """The reference's training loop (train.py:78-118).  device_data=True (default): the normalised corpus is uploaded once and the
     epoch sampler runs on the device (DeviceDataset), so no step copies anything host -> device and the losses are read back only
     when they are printed; device_data=False feeds host minibatches from the numpy sampler through CycleGAN.train(), like the
     reference's feed_dict.  loss_scale: 'static', 'monitor' or 'dynamic' (CycleGAN); when not static the log line also reports the
-    loss scale, the skipped steps and the last step's saturated F16F8 plane groups.  deterministic: bit-reproducible steps
+    loss scale, the skipped steps and the last step's saturated F16F8 plane groups; loss_scale_per_network: a scale each for the
+    generators and the discriminators (CycleGAN), logged with each network's fraction of gradient groups below the fp16 lower edge.  deterministic: bit-reproducible steps
     (CycleGAN), so that a rerun of the same seed writes the same checkpoints."""
     from .model import CycleGAN
     np.random.seed(random_seed)                                   # train.py:13
@@ -184,7 +191,8 @@ def train(train_A_dir, train_B_dir, model_dir, model_name, random_seed, num_epoc
         logf0_stats = {'mean_A': mA, 'std_A': sA, 'mean_B': mB, 'std_B': sB}
     mcep_stats = {'mean_A': A_mean, 'std_A': A_std, 'mean_B': B_mean, 'std_B': B_std}
     model = CycleGAN(num_features=NUM_MCEP, max_batch=mini_batch_size, max_frames=N_FRAMES, precision=precision, seed=random_seed,
-                     log_dir=tensorboard_log_dir, loss_scale=loss_scale, deterministic=deterministic)
+                     log_dir=tensorboard_log_dir, loss_scale=loss_scale, deterministic=deterministic,
+                     loss_scale_per_network=loss_scale_per_network)
     test_model = None
     data = DeviceDataset(model, A_norm, B_norm, mini_batch_size, N_FRAMES, seed=random_seed) if device_data else None
     g_loss = d_loss = float("nan")
@@ -245,11 +253,14 @@ def main():
     p.add_argument('--host_data', action='store_true', help='feed host minibatches from the numpy sampler every step (the reference\'s feed) '
                                                              'instead of the device-resident corpus + device sampler')
     p.add_argument('--deterministic', action='store_true', help='bit-reproducible train steps (fixed-order gradient and loss reductions)')
+    p.add_argument('--loss_scale_per_network', action='store_true',
+                   help='with --loss_scale monitor or dynamic (F16F8): a loss scale each for the generators and the discriminators')
     a = p.parse_args()
     none = lambda v: None if v in ('None', 'none') else v                                # train.py:191-192
     train(a.train_A_dir, a.train_B_dir, a.model_dir, a.model_name, a.random_seed, a.epochs, a.batch_size, a.synthetic, a.precision,
           device_data=not a.host_data, validation_A_dir=none(a.validation_A_dir), validation_B_dir=none(a.validation_B_dir),
-          output_dir=a.output_dir, tensorboard_log_dir=a.tensorboard_log_dir, loss_scale=a.loss_scale, deterministic=a.deterministic)
+          output_dir=a.output_dir, tensorboard_log_dir=a.tensorboard_log_dir, loss_scale=a.loss_scale, deterministic=a.deterministic,
+          loss_scale_per_network=a.loss_scale_per_network)
 
 
 if __name__ == '__main__':
