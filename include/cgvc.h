@@ -171,7 +171,11 @@ int cgvc_compute_gradients(cgvc_handle h, const float* A_dev, const float* B_dev
 
 /* TF-style Adam on the bound arenas (model.py:107-108; tf.train.AdamOptimizer beta1=0.5): advances t by one.
  * grad_scale multiplies every gradient first (1/nranks after a sum-all-reduce).  The same in every "loss_scale" mode (no skip: the
- * GRAD arena is the caller's); with "loss_scale" = 2, where t lives on the device, the call synchronises the device twice. */
+ * GRAD arena is the caller's); with "loss_scale" = 2, where t lives on the device, the call synchronises the device twice.
+ * Loss scale of the tape backward calls (cgvc_*_backward_tape): in CGVC_PREC_F16F8 they leave their GRAD contributions multiplied by
+ * the static loss scale of their tape's batch, s = 2^(9 + floor(log2 batch)) (1 in the other precisions; see cgvc_loss_scale_state);
+ * Adam over such gradients takes grad_scale = 1 / s (times 1/nranks after an all-reduce).  Gradients of tapes of batches with different
+ * scales do not share one GRAD: zero it in between. */
 int cgvc_adam_step(cgvc_handle h, float lr_generator, float lr_discriminator, float grad_scale, void* stream);
 
 /* -- replaces CycleGAN.test (model.py:128-137): one generator forward.  direction 0 = 'A2B', 1 = 'B2A';
@@ -191,6 +195,39 @@ int cgvc_generator_forward_packed(cgvc_handle h, int direction, const float* in_
 /* discriminator forward, which 0 = discriminator_A, 1 = discriminator_B: out [batch, 6, frames/16] (module.py:188-213) */
 int cgvc_discriminator_forward(cgvc_handle h, int which, const float* in_dev, float* out_dev,
                                int batch, int frames, void* stream);
+
+/* -- activation tapes: the two networks as differentiable operators (the reference composes module.py:148-213 into its loss graph,
+ * model.py:44-108; here a caller composes them into any objective and runs each application's backward itself).
+ * A tape is caller-owned device memory (256-byte aligned, at least cgvc_tape_bytes) that a forward fills with what the backward of that
+ * one network application reads: its input and its layers' pre-norm outputs, statistics, outputs and operand planes, as a train step
+ * keeps them.  kind 0 = generator, 1 = discriminator; batch <= max_batch, frames <= max_frames (a multiple of 4 / 16).
+ *   - Forward: the same outputs, bit for bit, as cgvc_generator_forward / cgvc_discriminator_forward.  A tape starts with a header
+ *     written by the forward (kind, direction or which, batch, frames, the writing engine and its parameter generation); the engine
+ *     keeps a copy, so that a backward checks its tape without reading the device.  cgvc_params_updated, cgvc_bind_arena and every Adam
+ *     update (cgvc_adam_step, cgvc_train_step) advance the parameter generation.
+ *   - Backward: from d out [batch, 24, frames] (generator) or d prob [batch, 6, frames/16] (discriminator), the network's kernel / bias /
+ *     beta / gamma gradients are ADDED into its GRAD range and d in [batch, 24, frames] is written to din_dev (NULL = none).  It does not
+ *     modify the tape: a tape can be back-propagated any number of times (each adds its gradients again).
+ *   - Errors, all before anything is enqueued: a tape this engine did not write, one written before the parameters last changed or one
+ *     of the other kind: CGVC_ERR_ARG.  A tape buffer smaller than cgvc_tape_bytes: CGVC_ERR_UNBOUND.  A backward on an engine without
+ *     GRAD or without a training WORK arena (train = 0): CGVC_ERR_UNBOUND.
+ *   - Scratch: the backward borrows the backward scratch of a train step at max_batch in WORK; WORK is not enlarged for it.
+ *   - Loss scaling (F16F8): the upstream gradient is multiplied by the static loss scale of the tape's batch before its gradient planes
+ *     are formed and d in is returned with it removed (exact: a power of two); the GRAD contributions keep it (see cgvc_adam_step).
+ *     With "loss_scale" = 1 the backward counts its saturated gradient-plane groups into the counters of cgvc_loss_scale_state (and the
+ *     per-network ones: the generator's into index 0, the discriminator's into index 1), adding to them until the next train step clears
+ *     them.  The dynamic policy ("loss_scale" = 2) does not act on tape calls: no skip, no scale change; they use the static scale.
+ *   - Options: "deterministic" makes repeated forward / backward sequences give the same GRAD bits; the kernel-choice options act as in a
+ *     train step.  Tape calls run eagerly on `stream`, never as captured graphs.
+ * Not covered: packed (variable-length) tapes, per-call or per-network loss scales, data-parallel reduction (cgvc_allreduce_grads
+ * sums GRAD over ranks). */
+int cgvc_tape_bytes(cgvc_handle h, int kind, int batch, int frames, size_t* bytes);
+int cgvc_generator_forward_tape(cgvc_handle h, int direction, const float* in_dev, float* out_dev, int batch, int frames,
+                                void* tape_dev, size_t tape_bytes, void* stream);
+int cgvc_discriminator_forward_tape(cgvc_handle h, int which, const float* in_dev, float* prob_dev, int batch, int frames,
+                                    void* tape_dev, size_t tape_bytes, void* stream);
+int cgvc_generator_backward_tape(cgvc_handle h, const void* tape_dev, const float* dout_dev, float* din_dev, void* stream);
+int cgvc_discriminator_backward_tape(cgvc_handle h, const void* tape_dev, const float* dprob_dev, float* din_dev, void* stream);
 
 /* Debug/parity taps: copy a named layer-boundary activation of the most recent cgvc_generator_forward /
  * cgvc_discriminator_forward (channels-last, fp32) into out_dev.  The generator forward only keeps them when the option
@@ -395,6 +432,10 @@ int cgvc_disc_input_backward(cgvc_handle h, const float* dy, const float* p, con
 int cgvc_head_forward(cgvc_handle h, const float* y, long long rows, const float* w, const float* b, float* prob, void* stream);
 int cgvc_head_loss_backward(cgvc_handle h, const float* prob, const float* y, long long rows, const float* w, float target, float coef,
                             const float* grad_mult, float* loss, float* dy, float* dw, float* db, void* stream);
+/* cgvc_head_backward: the same head from an upstream gradient dprob [rows] instead of the loss (cgvc_discriminator_backward_tape):
+ *   dz = g dprob[r] prob[r] (1 - prob[r]), g = *grad_mult (NULL: 1); dy, dw, db as above. */
+int cgvc_head_backward(cgvc_handle h, const float* prob, const float* y, long long rows, const float* w, const float* dprob,
+                       const float* grad_mult, float* dy, float* dw, float* db, void* stream);
 int cgvc_l1_loss_grad(cgvc_handle h, const float* yhat, const float* y, long long n, const float* gscale, const float* grad_mult, float* loss,
                       float* d, int accumulate, void* stream);
 /* The generator's two 15-tap edge layers as the step runs them with option "edge_lower" (module.py:85-86 h1, module.py:148 o1): dense

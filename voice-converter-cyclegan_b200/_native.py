@@ -15,6 +15,8 @@ _LIB = None
 ARENA_PARAM, ARENA_GRAD, ARENA_ADAM_M, ARENA_ADAM_V, ARENA_WORK = range(5)
 PREC_FP32_SIMT, PREC_BF16X3, PREC_BF16, PREC_F16F8 = 0, 1, 2, 3
 PRECISIONS = {"fp32": PREC_FP32_SIMT, "fp32_simt": PREC_FP32_SIMT, "bf16x3": PREC_BF16X3, "bf16": PREC_BF16, "f16f8": PREC_F16F8}
+ERR_ARG = -1
+ERR_UNBOUND = -3
 ERR_DIRECTION = -4
 ERR_UNSUPPORTED = -5
 
@@ -102,11 +104,17 @@ def _declare(lib):
         "cgvc_disc_input_backward": (ci, [vp] * 11 + [ci] * 9 + [P(ci), vp]),
         "cgvc_head_forward": (ci, [vp, vp, C.c_longlong, vp, vp, vp, vp]),
         "cgvc_head_loss_backward": (ci, [vp, vp, vp, C.c_longlong, vp, cf, cf] + [vp] * 6),
+        "cgvc_head_backward": (ci, [vp, vp, vp, C.c_longlong] + [vp] * 7),
         "cgvc_l1_loss_grad": (ci, [vp, vp, vp, C.c_longlong] + [vp] * 4 + [ci, vp]),
         "cgvc_edge_h1_forward": (ci, [vp, ci, vp, ci, ci] + [vp] * 6),
         "cgvc_edge_o1_forward": (ci, [vp, ci, vp, ci, ci] + [vp] * 4),
         "cgvc_edge_o1_backward": (ci, [vp, ci, vp, vp, ci, ci] + [vp] * 4),
         "cgvc_edge_h1_backward": (ci, [vp, ci, vp, vp, vp, ci, ci] + [vp] * 4),
+        "cgvc_tape_bytes": (ci, [vp, ci, ci, ci, P(sz)]),
+        "cgvc_generator_forward_tape": (ci, [vp, ci, vp, vp, ci, ci, vp, sz, vp]),
+        "cgvc_discriminator_forward_tape": (ci, [vp, ci, vp, vp, ci, ci, vp, sz, vp]),
+        "cgvc_generator_backward_tape": (ci, [vp, vp, vp, vp, vp]),
+        "cgvc_discriminator_backward_tape": (ci, [vp, vp, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the library does not export a declared symbol

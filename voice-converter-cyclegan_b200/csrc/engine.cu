@@ -7,6 +7,7 @@
 #include "tc_gemm.cuh"
 #include "geom.h"
 
+#include <atomic>
 #include <dlfcn.h>
 #include <limits.h>
 #include <stddef.h>
@@ -68,6 +69,18 @@ struct GraphKey {
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 struct GraphEntry { cudaGraphExec_t exec; unsigned long long launches; };
+
+// The header at the start of an activation tape (cgvc_*_forward_tape), also kept by the engine that wrote it, keyed by the tape's
+// address: a backward call checks its tape against that copy, so that it needs no device-to-host read before it enqueues anything
+struct TapeHeader {
+  unsigned long long magic;     // kTapeMagic
+  unsigned long long engine;    // cgvc_engine::id of the writer
+  unsigned long long gen;       // cgvc_engine::param_gen when it was written
+  int kind, which, batch, frames;
+};
+static const unsigned long long kTapeMagic = 0x45504154435647ull;   // "GVCTAPE"
+static const size_t kTapeHead = 256;                                // the activations start 256 bytes in
+static std::atomic<unsigned long long> g_engine_ids{0};
 
 struct Bump {
   char* base = nullptr; size_t cap = 0, off = 0; bool overflow = false;
@@ -167,6 +180,10 @@ struct cgvc_engine {
   std::map<std::string, std::pair<const float*, size_t>> taps;
   // the instance-norm sums scratch of the calls outside a train step (which has its WORK slices): conversions, cgvc_in_glu_*
   float* post_buf = nullptr; size_t post_elems = 0;
+  // activation tapes: this engine's id, the parameter generation (advanced whenever PARAM may have changed: cgvc_params_updated,
+  // cgvc_bind_arena, every Adam update) and the headers of the tapes written since the parameters last changed
+  unsigned long long id = 0, param_gen = 0;
+  std::map<const void*, TapeHeader> tapes;
 
   float* P() const { return (float*)arena[CGVC_ARENA_PARAM]; }
   float* G() const { return (float*)arena[CGVC_ARENA_GRAD]; }
@@ -355,12 +372,16 @@ static float loss_scale(const cgvc_engine* e, int batch) {
 }
 // option "loss_scale_per_network" in effect: it applies in loss_scale modes 1 and 2, and only F16F8 has a scale other than 1
 static bool ls_nets(const cgvc_engine* e) { return e->opt.ls_nets && e->opt.ls_mode && e->cfg.precision == CGVC_PREC_F16F8; }
-// the device copy of loss_scale(e, batch) (d_scalars[16 + floor(log2 batch)], written at creation), or in dynamic mode the scaler's
-// current scale (per network: that of the pass being enqueued, e->ls_net): what the loss-gradient kernels multiply by
-static const float* loss_scale_dev(const cgvc_engine* e, int batch) {
-  if (e->opt.ls_mode == 2) return ls_nets(e) ? &e->ls->net[e->ls_net].scale : &e->ls->scale;
+// the device copy of loss_scale(e, batch): d_scalars[16 + floor(log2 batch)], written at creation
+static const float* static_scale_dev(const cgvc_engine* e, int batch) {
   int l = 0; while ((2 << l) <= batch && l < 9) ++l;
   return e->d_scalars + 16 + l;
+}
+// ... or in dynamic mode the scaler's current scale (per network: that of the pass being enqueued, e->ls_net): what the loss-gradient
+// kernels multiply by
+static const float* loss_scale_dev(const cgvc_engine* e, int batch) {
+  if (e->opt.ls_mode == 2) return ls_nets(e) ? &e->ls->net[e->ls_net].scale : &e->ls->scale;
+  return static_scale_dev(e, batch);
 }
 // saturation counters of the plane writers (null: not counted): only F16F8 has reduced-range planes, only train steps are counted.
 // Per network, the gradient planes count into the block of the pass being enqueued, which also takes their underflow counts
@@ -1075,6 +1096,7 @@ int cgvc_create(const cgvc_config* cfg, cgvc_handle* out) {
   if (prop.major != 9 || prop.minor != 0) return fail(nullptr, CGVC_ERR_CUDA, "libcgvc is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
   cgvc_engine* e = new cgvc_engine();
   e->cfg = *cfg;
+  e->id = ++g_engine_ids;
   TableBuilder tb{e->tensors};
   const char* gn[2] = {"generator_A2B", "generator_B2A"}; const char* dn[2] = {"discriminator_A", "discriminator_B"};
   for (int i = 0; i < 2; ++i) { tb.scope = gn[i]; build_generator(tb, e->gen[i], cfg->num_features); }
@@ -1174,6 +1196,7 @@ int cgvc_bind_arena(cgvc_handle e, int arena, void* p, size_t bytes) {
   if ((uintptr_t)p & 255) return fail(e, CGVC_ERR_ARG, "arena %d must be 256-byte aligned", arena);
   e->arena[arena] = p; e->arena_bytes[arena] = bytes;
   drop_graphs(e);
+  ++e->param_gen;
   return 0;
 }
 
@@ -1203,6 +1226,7 @@ static int need_arenas(cgvc_engine* e, bool train) {
 int cgvc_params_updated(cgvc_handle e, void* stream) {
   if (!e) return CGVC_ERR_ARG;
   if (!e->arena[CGVC_ARENA_PARAM]) return fail(e, CGVC_ERR_UNBOUND, "PARAM arena must be bound");
+  ++e->param_gen;
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   if (e->cfg.precision != CGVC_PREC_FP32_SIMT) {
     int r = tc_refresh_weights(e->tcw, e->P(), (cudaStream_t)stream);
@@ -1654,6 +1678,7 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
   if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
   for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
   RET(check_work_train(e, batch, frames));
+  ++e->param_gen;                                            // a replayed graph does not run adam_body's host code
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const float gscale = (e->comm ? 1.f / (float)e->nranks : 1.f) / loss_scale(e, batch);
@@ -2180,6 +2205,17 @@ int cgvc_head_loss_backward(cgvc_handle e, const float* prob, const float* y, lo
   return 0;
 }
 
+int cgvc_head_backward(cgvc_handle e, const float* prob, const float* y, long long rows, const float* w, const float* dprob,
+                       const float* grad_mult, float* dy, float* dw, float* db, void* stream) {
+  if (!e || !prob || !w || !dprob || ((dw || db) && !y) || (!dw != !db)) return fail(e, CGVC_ERR_ARG, "null argument");
+  if (rows < 0) return fail(e, CGVC_ERR_ARG, "cgvc_head_backward: rows %lld", rows);
+  DetSlab slab; const DetSlab* det;
+  RET(plan_entry_det(e, &slab, &det));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  CK(launch_head_loss_bwd(prob, y, rows, 1024, w, 0.f, 0.f, nullptr, dy, dw, db, (cudaStream_t)stream, grad_mult, det, dprob));
+  return 0;
+}
+
 int cgvc_l1_loss_grad(cgvc_handle e, const float* yhat, const float* y, long long n, const float* gscale, const float* grad_mult, float* loss,
                       float* d, int accumulate, void* stream) {
   if (!e || !yhat || !y) return fail(e, CGVC_ERR_ARG, "null argument");
@@ -2329,6 +2365,168 @@ int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const fl
   const PostBwdParams q = post_bwd_params(e, N.h1, dy, A, B, T, S, true, dp != nullptr, PlanePair{dphi, dplo});
   CK(launch_post_bwd(q, e->opt.post, st));
   return h1_edge_backward(e, N, xchi, xclo, PlanePair{q.dp_hi, q.dp_lo}, B, T, dz ? dz : zs, dx, S, st);
+}
+
+}  // extern "C"
+
+// ---- activation tapes: the forward of one network application that records what its backward reads, and that backward ------------
+// Layout: the TapeHeader in the first kTapeHead bytes, then the network's input (generator: channels-last [B, T, 24]; discriminator:
+// [B, 24, T]) and the activations of plan_generator / plan_discriminator for (batch, frames), as a train step keeps them.  kind 0 the
+// generator, 1 the discriminator.  Returns the bytes the plan needs; g / d / x receive it at base (base may be null for sizing)
+static size_t tape_plan(cgvc_engine* e, int kind, void* base, int batch, int frames, GenActs* g, DiscActs* d, float** x) {
+  Bump ws; ws.reset((char*)base + kTapeHead, (size_t)1 << 62);
+  *x = ws.take<float>((size_t)batch * e->cfg.num_features * frames);
+  if (kind == 0) plan_generator(e, ws, *g, batch, frames);
+  else plan_discriminator(e, ws, *d, batch, frames);
+  return kTapeHead + ws.off;
+}
+
+// What a tape forward checks before it launches anything; *hd receives the header it is going to write
+static int tape_forward_entry(cgvc_engine* e, int kind, int which, const void* in, const void* out, int batch, int frames, void* tape,
+                              size_t tape_bytes, TapeHeader* hd) {
+  if (!in || !out || !tape) return fail(e, CGVC_ERR_ARG, "null buffer");
+  if ((uintptr_t)tape & 255) return fail(e, CGVC_ERR_ARG, "a tape must be 256-byte aligned");
+  RET(check_bt(e, batch, frames, kind == 0 ? 4 : 16));
+  RET(need_arenas(e, false));
+  GenActs g; DiscActs d; float* x;
+  const size_t need = tape_plan(e, kind, nullptr, batch, frames, &g, &d, &x);
+  if (tape_bytes < need) return fail(e, CGVC_ERR_UNBOUND, "tape of %zu bytes, batch %d x %d frames needs %zu", tape_bytes, batch, frames, need);
+  *hd = TapeHeader{kTapeMagic, e->id, e->param_gen, kind, which, batch, frames};
+  return 0;
+}
+
+// The header is written behind the forward on its stream; the engine's copy replaces any earlier tape at that address, and the tapes of
+// older parameters are forgotten (their backward is refused either way)
+static int tape_record(cgvc_engine* e, void* tape, const TapeHeader& hd, cudaStream_t st) {
+  CK(cudaMemcpyAsync(tape, &hd, sizeof hd, cudaMemcpyHostToDevice, st));
+  for (auto it = e->tapes.begin(); it != e->tapes.end();) it = it->second.gen != e->param_gen ? e->tapes.erase(it) : std::next(it);
+  e->tapes[tape] = hd;
+  return 0;
+}
+
+// What a tape backward checks before it launches anything: the tape is one this engine wrote for `kind` under its current parameters,
+// GRAD is bound and WORK holds a train step's plan at max_batch, whose lane-0 BwdScratch (sized for 2 max_batch samples) and upstream
+// buffers the backward borrows: *S, and the lane plan *L for its d_out / in / dY3 buffers
+static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const void* dout, TapeHeader* hd, LanePlan* L) {
+  if (!tape || !dout) return fail(e, CGVC_ERR_ARG, "null buffer");
+  auto it = e->tapes.find(tape);
+  if (it == e->tapes.end())
+    return fail(e, CGVC_ERR_ARG, "%p is not a tape written by this engine's cgvc_*_forward_tape since its parameters last changed", tape);
+  *hd = it->second;
+  if (hd->gen != e->param_gen) return fail(e, CGVC_ERR_ARG, "stale tape: the parameters changed after its forward");
+  if (hd->kind != kind)
+    return fail(e, CGVC_ERR_ARG, "a %s tape given to the %s backward", hd->kind ? "discriminator" : "generator", kind ? "discriminator" : "generator");
+  if (!e->cfg.train || !e->arena[CGVC_ARENA_GRAD])
+    return fail(e, CGVC_ERR_UNBOUND, "a tape backward needs the GRAD arena and a WORK arena sized for training (train = 1)");
+  RET(need_arenas(e, true));
+  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
+  TrainPlan P; plan_train(e, ws, P, e->cfg.max_batch, e->cfg.max_frames);
+  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small for the backward scratch");
+  *L = P.lane[0];
+  L->S.sq = nullptr;                                        // the weight gradients stay on the caller's stream
+  return 0;
+}
+
+// the upstream gradient is counted like a train step's in monitor mode (loss_scale = 1), into network `net`'s block
+struct TapeCounting {
+  cgvc_engine* e;
+  TapeCounting(cgvc_engine* en, int net) : e(en) { e->counting = e->opt.ls_mode == 1; e->ls_net = net; }
+  ~TapeCounting() { e->counting = false; e->ls_net = 0; }
+};
+
+extern "C" {
+
+int cgvc_tape_bytes(cgvc_handle e, int kind, int batch, int frames, size_t* bytes) {
+  if (!e || !bytes || (kind != 0 && kind != 1)) return fail(e, CGVC_ERR_ARG, "cgvc_tape_bytes: bad argument");
+  RET(check_bt(e, batch, frames, kind == 0 ? 4 : 16));
+  GenActs g; DiscActs d; float* x;
+  *bytes = tape_plan(e, kind, nullptr, batch, frames, &g, &d, &x);
+  return 0;
+}
+
+int cgvc_generator_forward_tape(cgvc_handle e, int direction, const float* in_dev, float* out_dev, int batch, int frames, void* tape_dev,
+                                size_t tape_bytes, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
+  TapeHeader hd;
+  RET(tape_forward_entry(e, 0, direction, in_dev, out_dev, batch, frames, tape_dev, tape_bytes, &hd));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  GenActs A; DiscActs D; float* x_cl;
+  tape_plan(e, 0, tape_dev, batch, frames, &A, &D, &x_cl);
+  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &A.post));
+  CK(launch_transpose_ft(in_dev, x_cl, batch, e->cfg.num_features, frames, st));
+  RET(generator_forward(e, e->gen[direction], A, x_cl, st, false, true));
+  CK(launch_transpose_ft(A.out_cl, out_dev, batch, frames, e->cfg.num_features, st));
+  return tape_record(e, tape_dev, hd, st);
+}
+
+int cgvc_discriminator_forward_tape(cgvc_handle e, int which, const float* in_dev, float* prob_dev, int batch, int frames, void* tape_dev,
+                                    size_t tape_bytes, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if (which != 0 && which != 1) return fail(e, CGVC_ERR_ARG, "which must be 0 (discriminator_A) or 1 (discriminator_B)");
+  TapeHeader hd;
+  RET(tape_forward_entry(e, 1, which, in_dev, prob_dev, batch, frames, tape_dev, tape_bytes, &hd));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t img = (size_t)batch * e->cfg.num_features * frames;
+  GenActs G; DiscActs A; float* x;
+  tape_plan(e, 1, tape_dev, batch, frames, &G, &A, &x);
+  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &A.post));
+  CK(cudaMemcpyAsync(x, in_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));        // the input layer's backward reads it
+  RET(discriminator_forward(e, e->disc[which], A, x, st, false));
+  CK(cudaMemcpyAsync(prob_dev, A.prob, (size_t)batch * (e->cfg.num_features / 4) * (frames / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return tape_record(e, tape_dev, hd, st);
+}
+
+int cgvc_generator_backward_tape(cgvc_handle e, const void* tape_dev, const float* dout_dev, float* din_dev, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  TapeHeader hd; LanePlan L;
+  RET(tape_backward_entry(e, 0, tape_dev, dout_dev, &hd, &L));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = hd.batch, T = hd.frames, nf = e->cfg.num_features;
+  const long long img = (long long)B * nf * T;
+  GenActs A; DiscActs D; float* x_cl;
+  tape_plan(e, 0, const_cast<void*>(tape_dev), B, T, &A, &D, &x_cl);
+  A.x_cl = x_cl; A.post = L.S.post;
+  // the upstream gradient channels-last, times the loss scale of the F16F8 gradient planes (a power of two: exact)
+  const float s = loss_scale(e, B);
+  CK(launch_transpose_ft(dout_dev, L.d_out, B, nf, T, st));
+  if (s != 1.f) CK(launch_scale(L.d_out, img, s, st));
+  {
+    TapeCounting counting(e, 0);
+    RET(generator_backward(e, e->gen[hd.which], A, L.d_out, din_dev ? L.in : nullptr, L.S, st));
+  }
+  if (!din_dev) return 0;
+  CK(launch_transpose_ft(L.in, din_dev, B, T, nf, st));
+  if (s != 1.f) CK(launch_scale(din_dev, img, 1.f / s, st));
+  return 0;
+}
+
+int cgvc_discriminator_backward_tape(cgvc_handle e, const void* tape_dev, const float* dprob_dev, float* din_dev, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  TapeHeader hd; LanePlan L;
+  RET(tape_backward_entry(e, 1, tape_dev, dprob_dev, &hd, &L));
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = hd.batch, T = hd.frames, nf = e->cfg.num_features;
+  GenActs G; DiscActs A; float* x;
+  tape_plan(e, 1, const_cast<void*>(tape_dev), B, T, &G, &A, &x);
+  A.x = x; A.post = L.S.post;
+  const DiscNet& DN = e->disc[hd.which];
+  const float* Pm = e->P(); float* Gm = e->G();
+  const long long rows = (long long)B * (nf / 4) * (T / 16);
+  {
+    TapeCounting counting(e, 1);
+    // dz = s dprob p (1 - p) through the head: dY3 and the dense kernel / bias gradients
+    CK(launch_head_loss_bwd(A.prob, A.d[2].Y, rows, 1024, Pm + DN.dense_k, 0.f, 0.f, nullptr, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st,
+                            static_scale_dev(e, B), det_of(L.S), dprob_dev));
+    RET(discriminator_backward(e, DN, A, L.dY3, true, din_dev, L.S, st));
+  }
+  const float s = loss_scale(e, B);
+  if (din_dev && s != 1.f) CK(launch_scale(din_dev, (long long)B * nf * T, 1.f / s, st));
+  return 0;
 }
 
 }  // extern "C"

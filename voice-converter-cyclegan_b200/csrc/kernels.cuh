@@ -241,10 +241,12 @@ cudaError_t post_init_kernels();   // shared-memory opt-in of the streaming kern
 cudaError_t launch_head_fwd(const float* y, long long rows, int C, const float* w, const float* b, float* prob, cudaStream_t st);
 // loss_slot += coef * mean((p - target)^2) over `rows`; dz = coef * 2 (p-target)/rows * p (1-p);
 // dy[row,:] = dz * w (if dy);  dw += sum dz*y[row,:], db += sum dz (if dw)
+// dprob (may be null): an upstream gradient d prob [rows] instead of the loss: dz = grad_mult * dprob[row] * p (1-p), target and coef
+// unused, loss_slot must be null
 cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long rows, int C, const float* w,
                                  float target, float coef, float* loss_slot,
                                  float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev = nullptr,
-                                 const DetSlab* det = nullptr);
+                                 const DetSlab* det = nullptr, const float* dprob = nullptr);
 
 // ---- L1 loss + gradient (utils.py:6-8): loss_slot += mean|yhat - y|; d[i] = gscale * sign(yhat - y)/n  (accumulate optional)
 cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, float* loss_slot,

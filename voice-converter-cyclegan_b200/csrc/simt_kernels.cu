@@ -1394,7 +1394,7 @@ __global__ void __launch_bounds__(256)
 head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y, long long rows, int C,
                      const float* __restrict__ w, float target, float coef, float* __restrict__ loss_slot,
                      float* __restrict__ dy, float* __restrict__ dw, float* __restrict__ db, const float* __restrict__ grad_mult_dev,
-                     float* __restrict__ part) {
+                     float* __restrict__ part, const float* __restrict__ dprob) {
   __shared__ float red[8][32];
   float* prow = part ? part + (long long)blockIdx.x * (C + 2) : nullptr;     // det: [dw (C) | db | loss] of this CTA
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1406,9 +1406,14 @@ head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y
   const float inv = 1.f / (float)rows;
   for (long long row = (long long)blockIdx.x * 8 + warp; row < rows; row += (long long)gridDim.x * 8) {
     float p = prob[row];
-    float d = p - target;
-    lsum += d * d;
-    float dz = grad_mult * coef * 2.f * d * inv * p * (1.f - p);       // grad_mult: loss scale of the reduced-precision gradient planes (1 otherwise)
+    float dz;
+    if (dprob) {                                                        // upstream d prob instead of the LSGAN loss (no loss term)
+      dz = grad_mult * dprob[row] * p * (1.f - p);
+    } else {
+      float d = p - target;
+      lsum += d * d;
+      dz = grad_mult * coef * 2.f * d * inv * p * (1.f - p);           // grad_mult: loss scale of the reduced-precision gradient planes (1 otherwise)
+    }
     dbsum += dz;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -1451,14 +1456,16 @@ head_loss_bwd_kernel(const float* __restrict__ prob, const float* __restrict__ y
 
 cudaError_t launch_head_loss_bwd(const float* prob, const float* y, long long rows, int C, const float* w,
                                  float target, float coef, float* loss_slot,
-                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev, const DetSlab* det) {
+                                 float* dy, float* dw, float* db, cudaStream_t st, const float* grad_mult_dev, const DetSlab* det,
+                                 const float* dprob) {
   if (rows == 0) return cudaSuccess;
-  if (C != 1024) return cudaErrorInvalidValue;
+  if (C != 1024 || (dprob && loss_slot)) return cudaErrorInvalidValue;
   long long nb = (rows + 7) / 8;
   if (nb > 296) nb = 296;
   float* part = det ? det->p : nullptr;
   if (part && nb * (C + 2) > det->cap) return cudaErrorInvalidValue;
-  ++g_cgvc_launches; head_loss_bwd_kernel<<<(unsigned)nb, 256, 0, st>>>(prob, y, rows, C, w, target, coef, loss_slot, dy, dw, db, grad_mult_dev, part);
+  ++g_cgvc_launches; head_loss_bwd_kernel<<<(unsigned)nb, 256, 0, st>>>(prob, y, rows, C, w, target, coef, loss_slot, dy, dw, db, grad_mult_dev, part,
+                                                                      dprob);
   if (!part) return cudaGetLastError();
   return launch_reduce_parts(part, nb, C + 2, DetSegs{{dw, db, loss_slot}, {0, C, C + 1}, {dw ? C : 0, db ? 1 : 0, loss_slot ? 1 : 0}}, st);
 }

@@ -18,6 +18,10 @@ Differences a user of the reference should know:
   * `deterministic=True` makes every train step bit-reproducible on one GPU: the same weights, Adam and loss-scale state and inputs give
     the same bits whatever the stream schedule or CUDA-graph replay, so a rerun of a seed or a resumed checkpoint follows the
     same trajectory (include/cgvc.h option "deterministic", DESIGN.md section 11; the NCCL sum of a data-parallel step is not covered)
+  * `generator(x, direction)` / `discriminator(x, which)` are the four networks as differentiable torch operators on CUDA tensors, for
+    objectives other than the fused step's: `loss.backward()` adds their weight gradients into the gradient arena, `zero_grad()`,
+    `grads()` and `adam_step()` complete a step (include/cgvc.h "activation tapes", DESIGN.md section 12).  The network descriptors
+    given to the constructor are `generator_descriptor` / `discriminator_descriptor`
 """
 from __future__ import annotations
 
@@ -51,8 +55,8 @@ class CycleGAN(object):
             raise RuntimeError("CycleGAN needs a CUDA device (sm_90a); there is no CPU fallback")
         self.num_features = num_features
         self.input_shape = [None, num_features, None]
-        self.discriminator = discriminator
-        self.generator = generator
+        self.discriminator_descriptor = discriminator
+        self.generator_descriptor = generator
         self.mode = mode
         self.precision = precision
         self._lib = N.load()
@@ -74,6 +78,8 @@ class CycleGAN(object):
             self._options["deterministic"] = 1
         self.last_step_skipped = False
         self.last_loss_scale = None
+        self._tape_scales = set()        # loss scales of the tape backward calls since zero_grad (adam_step divides by it)
+        self._grad_token = None
         self._create_engine()
         # the descriptors state the architecture the caller expects (model.py:14-15); the engine must implement exactly that
         for scope in ("generator_A2B", "generator_B2A"):
@@ -289,6 +295,107 @@ class CycleGAN(object):
     def get_grads(self):
         torch.cuda.synchronize(self.device)
         return OrderedDict((n, self._view(N.ARENA_GRAD, n).cpu().numpy()) for n in self._table)
+
+    # ------------------------------------------------------------------ differentiable networks (activation tapes)
+    def generator(self, x, direction):
+        """Differentiable generator forward: x a CUDA tensor [batch, 24, frames] (frames a multiple of 4) -> [batch, 24, frames], bit
+        for bit what test() gives.  Its backward adds d loss / d (the generator's variables) into the gradient arena (grads()) and
+        returns d loss / d x.  direction 'A2B' or 'B2A'."""
+        d = {'A2B': 0, 'B2A': 1}.get(direction)
+        if d is None:
+            raise Exception('Conversion direction must be specified.')
+        return _NetFn.apply(x, self._token(), self, 0, d)
+
+    def discriminator(self, x, which):
+        """Differentiable discriminator forward: x a CUDA tensor [batch, 24, frames] (frames a multiple of 16) -> probabilities
+        [batch, 6, frames / 16, 1] as discriminate() gives them.  Backward as generator().  which 'A' or 'B'."""
+        w = {'A': 0, 'B': 1}.get(which)
+        if w is None:
+            raise ValueError("which must be 'A' or 'B', got %r" % (which,))
+        return _NetFn.apply(x, self._token(), self, 1, w)
+
+    def _token(self):
+        # a leaf that requires grad, so that autograd runs a network's backward -- and with it the weight gradients -- even when its
+        # input does not require grad (a real sample)
+        if self._grad_token is None:
+            self._grad_token = torch.zeros(0, device=self.device, requires_grad=True)
+        return self._grad_token
+
+    def tape_loss_scale(self, batch):
+        """The factor the tape backward calls of a `batch`-sample application leave in the gradient arena: the static loss scale of the
+        F16F8 gradient planes, 2^(9 + min(floor(log2 batch), 9)), and 1 in the other precisions (include/cgvc.h cgvc_adam_step)."""
+        if N.PRECISIONS[self.precision] != N.PREC_F16F8:
+            return 1.0
+        return float(2 ** (9 + min(int(batch).bit_length() - 1, 9)))
+
+    def _tape_forward(self, kind, which, x):
+        if not (isinstance(x, torch.Tensor) and x.device.type == self.device.type):
+            raise TypeError("the differentiable networks take a tensor on the engine's device (%s)" % self.device)
+        x = x.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        if x.dim() != 3 or x.shape[1] != self.num_features:
+            raise ValueError("expected [batch, %d, frames], got %r" % (self.num_features, tuple(x.shape)))
+        batch, _, frames = x.shape
+        self._ensure_capacity(batch, frames)
+        nbytes = C.c_size_t(0)
+        self._chk(self._lib.cgvc_tape_bytes(self._handle, kind, batch, frames, C.byref(nbytes)))
+        tape = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)     # the caching allocator aligns to 512 bytes
+        if kind == 0:
+            y = torch.empty_like(x)
+            fn = self._lib.cgvc_generator_forward_tape
+        else:
+            y = torch.empty((batch, self.num_features // 4, frames // 16, 1), dtype=torch.float32, device=self.device)
+            fn = self._lib.cgvc_discriminator_forward_tape
+        self._chk(fn(self._handle, which, _ptr(x), _ptr(y), batch, frames, _ptr(tape), nbytes.value, self._stream()))
+        return y, tape
+
+    def _tape_backward(self, kind, tape, x_shape, dy, want_dx):
+        dy = dy.to(device=self.device, dtype=torch.float32).contiguous()
+        dx = torch.empty(x_shape, dtype=torch.float32, device=self.device) if want_dx else None
+        fn = self._lib.cgvc_generator_backward_tape if kind == 0 else self._lib.cgvc_discriminator_backward_tape
+        self._chk(fn(self._handle, _ptr(tape), _ptr(dy), _ptr(dx), self._stream()))
+        self._tape_scales.add(self.tape_loss_scale(x_shape[0]))
+        return dx
+
+    def zero_grad(self, network=None):
+        """Zero the gradient arena before the backward passes of a new step; with network ('generator_A2B', ..., 'discriminator_B')
+        only that network's variables -- e.g. a discriminator's after the generator loss was back-propagated through it, since its
+        optimizer follows the discriminator loss alone (model.py:107-108)."""
+        if network is None:
+            self._arenas[N.ARENA_GRAD].zero_()
+            self._tape_scales.clear()
+            return
+        names = [n for n in self._table if n.startswith(network + "/")]
+        if not names:
+            raise KeyError("no network %r" % (network,))
+        for n in names:
+            self._view(N.ARENA_GRAD, n).zero_()
+
+    def grads(self, network=None):
+        """name -> d loss / d variable (TF layout) as the tape backward calls since zero_grad() accumulated it, on the device, with
+        their loss scale removed: views of the gradient arena when that scale is 1, else scaled copies -- read them, do not write
+        them.  network: 'generator_A2B', 'generator_B2A', 'discriminator_A' or 'discriminator_B' (None: all four)."""
+        s = self._grad_scale()
+        out = OrderedDict()
+        for n in self._table:
+            if network is None or n.startswith(network + "/"):
+                v = self._view(N.ARENA_GRAD, n).detach()
+                out[n] = v if s == 1.0 else v * s
+        if not out:
+            raise KeyError("no network %r" % (network,))
+        return out
+
+    def _grad_scale(self):
+        if len(self._tape_scales) > 1:
+            raise RuntimeError("the gradient arena mixes tape backward calls of different loss scales (batches %s): zero_grad() between "
+                               "batches whose scales differ" % sorted(self._tape_scales))
+        return 1.0 / next(iter(self._tape_scales)) if self._tape_scales else 1.0
+
+    def adam_step(self, generator_learning_rate, discriminator_learning_rate):
+        """One Adam update of all four networks (model.py:107-108) from the gradient arena that the tape backward calls filled, with
+        their loss scale removed; advances the Adam step count like train()."""
+        self._chk(self._lib.cgvc_adam_step(self._handle, float(generator_learning_rate), float(discriminator_learning_rate),
+                                           self._grad_scale(), self._stream()))
+        self.train_step += 1
 
     # ------------------------------------------------------------------ data parallel
     def _attach_communicator(self):
@@ -581,3 +688,22 @@ class CycleGAN(object):
         for n, v in self.last_losses.items():
             scope = 'generator_summaries/' if not n.startswith('discriminator') else 'discriminator_summaries/'
             self.writer.add_scalar(scope + n, v, self.train_step)
+
+
+class _NetFn(torch.autograd.Function):
+    """One network application (kind 0 generator, 1 discriminator) with its activation tape: forward writes it, backward consumes it
+    (the tape is not modified, so retain_graph backward passes each add their gradients again)."""
+
+    @staticmethod
+    def forward(ctx, x, token, model, kind, which):
+        y, tape = model._tape_forward(kind, which, x)
+        ctx.model, ctx.kind, ctx.x_shape = model, kind, tuple(x.shape)
+        ctx.save_for_backward(tape)
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        tape, = ctx.saved_tensors
+        dx = ctx.model._tape_backward(ctx.kind, tape, ctx.x_shape, dy, ctx.needs_input_grad[0])
+        return dx, None, None, None, None

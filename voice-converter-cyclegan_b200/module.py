@@ -13,6 +13,9 @@ scope on the first call and reuse them on later calls (`reuse=True`).  Here each
     network on `inputs` ([batch, 24, frames], numpy or CUDA tensor) with the variables of `scope_name`, created
     (glorot-uniform, like tf.get_variable's default) on the first call and reused with `reuse=True`, with TF's error
     behaviour for the two misuse cases.  `scope_variables` / `assign_scope_variables` read and inject those variables.
+    Given a numpy array it returns one; given a CUDA tensor it returns a CUDA tensor that autograd differentiates through the native
+    network (CycleGAN.generator / CycleGAN.discriminator): its backward returns d inputs and adds the scope's variable gradients up,
+    which `scope_gradients` reads and `zero_scope_gradients` clears.
 """
 from __future__ import annotations
 
@@ -144,9 +147,26 @@ def _scope(desc, scope_name, reuse):
     return ei, 0
 
 
+def _train_model(ei):
+    """the engine of slot group ei as a training engine (gradient arena and backward workspace), made on the first differentiable call"""
+    m = _ENGINES[ei]["model"]
+    if m.mode != 'train':
+        from .model import CycleGAN
+        t = CycleGAN(num_features=24, mode='train', max_batch=m._max_batch, max_frames=m._max_frames, log_dir='/tmp/cgvc_log')
+        t.set_params(m.get_params())
+        t.zero_grad()
+        _ENGINES[ei]["model"] = m = t
+    return m
+
+
 def _apply(desc, inputs, reuse, scope_name):
     ei, slot = _scope(desc, scope_name, reuse)
     m = _ENGINES[ei]["model"]
+    if hasattr(inputs, "is_cuda") and inputs.is_cuda:
+        m = _train_model(ei)
+        if desc.kind == "generator":
+            return m.generator(inputs, 'A2B' if slot == 0 else 'B2A')
+        return m.discriminator(inputs, 'A' if slot == 0 else 'B')
     if desc.kind == "generator":
         return m.test(inputs, 'A2B' if slot == 0 else 'B2A')
     return m.discriminate(inputs, 'A' if slot == 0 else 'B')
@@ -169,6 +189,22 @@ def assign_scope_variables(scope_name, values):
         rel = n[len(scope_name) + 1:] if n.startswith(scope_name + "/") else n
         upd[pre + rel] = v
     _ENGINES[ei]["model"].set_params(upd)
+
+
+def scope_gradients(scope_name):
+    """OrderedDict TF variable name -> d loss / d variable (CUDA tensors) that the backward passes of the scope's differentiable calls
+    added up since zero_scope_gradients (loss scale removed)."""
+    kind, ei, slot = _SCOPES[scope_name]
+    pre = _SLOT_SCOPE[kind][slot]
+    G = _train_model(ei).grads(pre)
+    return OrderedDict((scope_name + n[len(pre):], v) for n, v in G.items())
+
+
+def zero_scope_gradients():
+    """Clear the variable gradients of every scope."""
+    for e in _ENGINES:
+        if e["model"].mode == 'train':
+            e["model"].zero_grad()
 
 
 def reset_default_graph():
