@@ -369,6 +369,22 @@ int cgvc_in_glu_backward_planes(cgvc_handle h, const float* dy, const float* p, 
                                 float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
                                 int B, int R, int C, int shuffle, int precision, int gate,
                                 void* hi, void* lo, unsigned long long* sat, void* stream);
+/* cgvc_in_glu_forward_planes over packed utterances, as cgvc_generator_forward_packed normalises them: p holds R / shuffle conv rows
+ *   in all, of which utterance u owns [offsets[u] / div, offsets[u + 1] / div).  offsets (device): n_utt + 1 frame prefix sums, each
+ *   length a multiple of 4; div = 1, 2 or 4 (P's level), a multiple of shuffle; max_len: the longest utterance in frames.  Each
+ *   utterance is normalised over its own positions; stats is [n_utt, 4, C]. */
+int cgvc_in_glu_forward_packed(cgvc_handle h, const float* p, const float* beta_a, const float* gamma_a,
+                               const float* beta_g, const float* gamma_g, float* y, float* stats,
+                               int R, int C, int shuffle, int precision, int gate, const float* resid,
+                               const long long* offsets, int n_utt, int div, int max_len,
+                               void* hi, void* lo, unsigned long long* sat, void* stream);
+/* cgvc_in_glu_backward_planes that also accumulates the conv-bias gradients dbias_a, dbias_g [C * shuffle] (the column sums of dp, as
+ *   the train step does; dbias_g needs dbias_a and is unused when gate is 0). */
+int cgvc_in_glu_backward_bias(cgvc_handle h, const float* dy, const float* p, const float* stats,
+                              const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                              float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
+                              float* dbias_a, float* dbias_g, int B, int R, int C, int shuffle, int precision, int gate,
+                              void* hi, void* lo, unsigned long long* sat, void* stream);
 /* One generator layer with its instance norm, as a train step or a conversion runs it, so that the fused gather-GEMM epilogues can be
  * checked against float64 and against the separate kernels.  precision CGVC_PREC_BF16X3, _BF16 or _F16F8 (planes as above).
  * fuse = 1: the instance norm runs in the GEMM epilogue where the shape allows (1-D layer, R = 32, 64 or 128 positions per sample);

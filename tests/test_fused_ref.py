@@ -109,3 +109,81 @@ def test_certificate_of_every_lattice_case():
         if dx0 is not None:
             bound = bound + torch.from_numpy(np.abs(dx0)).double()
         assert float(bound.max()) < 2 ** 24, (pair, B, R)
+
+
+@pytest.mark.parametrize("gated,shuffle", [(True, 1), (True, 2), (False, 1), (False, 2)])
+def test_shuffle_backward_and_conv_bias_match_autograd(gated, shuffle):
+    """the closed form in the shuffled view and the conv-bias gradients (per conv column, so per phase) against autograd of the oracle"""
+    rng = np.random.default_rng(5)
+    B, Rw, C = 3, 8, 4
+    nt = C * shuffle * (2 if gated else 1)
+    bp = (rng.standard_normal((B, Rw, nt)) * 1.5 + 0.2).astype(np.float32)
+    par = tuple((rng.standard_normal(C) * 0.3 + k).astype(np.float32) for k in (0.0, 1.0, 0.0, 1.0))
+    if not gated:
+        par = par[:2] + (None, None)
+    dy = rng.standard_normal((B, Rw * shuffle, C)).astype(np.float32)
+    dp, grads, bias = F.backward(bp, par, dy, gated, shuffle=shuffle, bias=True)
+    dp_ag, grads_ag, bias_ag = F.backward_autograd(bp, par, dy, gated, shuffle=shuffle, bias=True)
+    torch.testing.assert_close(dp, dp_ag, rtol=1e-10, atol=1e-10)
+    for g, ga in zip(grads, grads_ag):
+        if ga is not None:
+            torch.testing.assert_close(g, ga, rtol=1e-10, atol=1e-10)
+    torch.testing.assert_close(torch.cat([b for b in bias if b is not None]), bias_ag, rtol=1e-10, atol=1e-10)
+    if shuffle == 2:                      # not analytically zero: the norm removes the mean over both phases, not per phase
+        assert bias[0].abs().max() > 1e-3
+    else:
+        assert bias[0].abs().max() < 1e-9
+
+
+def test_norm_bounds_hold_for_a_float32_replay():
+    """the statistics and dP bounds of fused_ref hold for float32 evaluations of the kernels' formulas (a CPU replay, sequential sums)"""
+    rng = np.random.default_rng(9)
+    B, R, C = 4, 96, 8
+    v = (rng.standard_normal((B, R, C)) * np.array([1e-4, 1.0, 30.0, 1e-2])[:, None, None] + rng.standard_normal((B, 1, C)) * 50)
+    v[3, 0] += 2000 * 1e-2                                      # a far outlier at position 0
+    v = v.astype(np.float32)
+    v64 = torch.from_numpy(v).double()
+    for form in ("stream", "shifted"):
+        x = v
+        if form == "stream":
+            m = (x.sum(axis=1, dtype=np.float32) * np.float32(1 / R)).astype(np.float32)
+            d = (x - m[:, None]).astype(np.float32)
+            var = ((d * d).sum(axis=1, dtype=np.float32) * np.float32(1 / R)).astype(np.float32)
+        else:
+            k = x[:, 0]
+            d = (x - k[:, None]).astype(np.float32)
+            m1 = d.sum(axis=1, dtype=np.float32) * np.float32(1 / R)
+            var = np.maximum((d * d).sum(axis=1, dtype=np.float32) * np.float32(1 / R) - m1 * m1, 0).astype(np.float32)
+            m = (k + m1).astype(np.float32)
+        rs = np.float32(1) / np.sqrt(var + np.float32(F.EPS))
+        m64, r64 = F.stats_of(v64)
+        em, er = F.stats_bound(v64, form, R + 13)
+        assert (torch.from_numpy(m).double() - m64).abs().le(em).all(), form
+        assert (torch.from_numpy(rs).double() / r64 - 1).abs().le(er).all(), form
+
+
+def test_dispatch_mirror_matches_the_launch_code():
+    """fused_ref's dispatch mirror against the configuration macros and rules parsed from simt_kernels.cu"""
+    import os
+    import re
+    src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "voice-converter-cyclegan_b200", "csrc",
+                            "simt_kernels.cu")).read()
+    fwd = [tuple(int(n) for n in t) for t in re.findall(r"X\((\d+), (\d+)\)", re.search(r"#define STREAM_FWD_CONFIGS\(X\)(.*)", src).group(1))]
+    bwd = [(int(a), int(b), c == "true") for a, b, c in
+           re.findall(r"X\((\d+), (\d+), (true|false)\)", re.search(r"#define STREAM_CONFIGS\(X\)(.*)", src).group(1))]
+    assert sorted(fwd) == sorted(F.STREAM_FWD) and sorted(bwd) == sorted(F.STREAM_BWD)
+    # each dispatch line: R == 256 / NQL * NRT, C % (4 NQL)
+    for R, cm, nql, nrt in re.findall(r"if \(R == (\d+) && C % (\d+) == 0\) \{ \*err = launch_post_fwd_stream<(\d+), (\d+)>", src):
+        assert int(R) == 256 // int(nql) * int(nrt) and int(cm) == 4 * int(nql)
+        assert F.post_fwd_kernels(2, int(R), int(cm), 1, True) == ["post_fwd_stream_kernel<%s, %s>" % (nql, nrt)]
+    for R, cm, nql, nrt, g in re.findall(r"if \(R == (\d+) && C % (\d+) == 0(?: && pp.sh == 1)?\) \{ \*err = launch_post_bwd_stream<(\d+), (\d+), (\w+)>", src):
+        assert int(R) == 256 // int(nql) * int(nrt) and int(cm) == 4 * int(nql)
+        assert F.post_bwd_kernels(2, int(R), int(cm), 1, g == "true") == ["post_bwd_stream_kernel<%s, %s, %s>" % (nql, nrt, g)]
+    assert "if (pp.R <= 32) ONEPASS(4); else if (pp.R <= 48) ONEPASS(6); else ONEPASS(8);" in src
+    assert "pp.has_in && pp.R <= 64 && forms.onepass" in src
+    assert F.post_bwd_kernels(2, 40, 128, 1, True) == ["post_bwd_onepass_kernel<true, 6>"]
+    assert F.post_bwd_kernels(2, 64, 128, 2, False) == ["post_bwd_onepass_kernel<false, 8>"]
+    assert F.post_bwd_kernels(2, 384, 16, 1, True, det=True, bias=True) == ["post_bwd_sums_kernel<true>", "reduce_parts_kernel",
+                                                                 "post_apply_bwd_kernel<true, true>", "reduce_parts_kernel"]
+    assert F.post_fwd_kernels(2, 384, 16, 1, True, resid=True) == ["post_stats_kernel<true, false>", "post_apply_fwd_kernel<true, true, false>"]
+    assert len(F.post_instantiations(src)) == 6 + 7 + 6 + 12

@@ -113,9 +113,12 @@ def test_chain_lengths_follow_the_launch_grids():
 REACHED = {
     "gg_simt_kernel": "test_gpu_kernels.py", "wgrad_simt_kernel": "test_gpu_kernels.py",
     "colsum_kernel": "test_gpu_kernels.py", "reduce_parts_kernel": "test_gpu_deterministic.py",
-    "post_stats_kernel": "test_gpu_planes.py", "post_apply_fwd_kernel": "test_gpu_planes.py / test_gpu_glu_layers.py (GLU-only form)",
-    "post_bwd_sums_kernel": "test_gpu_planes.py", "post_apply_bwd_kernel": "test_gpu_planes.py / test_gpu_glu_layers.py (GLU-only form)",
-    "post_bwd_onepass_kernel": "test_gpu_planes.py", "post_fwd_stream_kernel": "test_gpu_planes.py", "post_bwd_stream_kernel": "test_gpu_planes.py",
+    "post_stats_kernel": "test_gpu_norm_layers.py",
+    "post_apply_fwd_kernel": "test_gpu_norm_layers.py / test_gpu_glu_layers.py (GLU-only form)",
+    "post_bwd_sums_kernel": "test_gpu_norm_layers.py",
+    "post_apply_bwd_kernel": "test_gpu_norm_layers.py / test_gpu_glu_layers.py (GLU-only form)",
+    "post_bwd_onepass_kernel": "test_gpu_norm_layers.py", "post_fwd_stream_kernel": "test_gpu_norm_layers.py",
+    "post_bwd_stream_kernel": "test_gpu_norm_layers.py",
     "head_fwd_kernel": "test_gpu_glu_layers.py", "head_loss_bwd_kernel": "test_gpu_glu_layers.py", "l1_loss_grad_kernel": "test_gpu_glu_layers.py",
     "wgrad_c1_kernel": "test_gpu_glu_layers.py", "gather_taps_kernel": "test_gpu_glu_layers.py", "glu_bwd_wgrad_c1_kernel": "test_gpu_glu_layers.py",
     "glu_bwd_proj_c1_kernel": "test_gpu_glu_layers.py", "proj_taps_kernel": "test_gpu_glu_layers.py", "conv_c1_fwd_kernel": "test_gpu_glu_layers.py",

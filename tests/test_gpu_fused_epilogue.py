@@ -50,7 +50,6 @@ FALLBACK_Y_L2 = 1e-4     # per-sample relative L2 between the fused and the fall
 DP_L2 = 2e-5             # per-sample relative L2 of the dP planes' value
 DP_MAX = 1e-4            # per (sample, channel): max |dP - float64| / max of the column's |terms|
 AFFINE_L2 = 2e-5         # dbeta / dgamma relative L2
-NORM_ULPS = 8            # y_bound: the normalised value's rounding
 
 # (B, R): 128-row tiles of whole samples at R = 32, 64, 128, and tails (M % 128 != 0) at R = 32 and 64
 SHAPES = [(8, 32), (4, 64), (3, 128), (5, 32), (3, 64)]
@@ -200,29 +199,6 @@ def _fwd(eng, prec, layer, B, R, ops, form="train", fuse=1):
     return {"p": p, "stats": stats, "y": y, "hi": hi, "lo": lo, "fused": fused.value}
 
 
-def y_bound(P, st, par, gated, shuffle, resid):
-    """per-element bound of |y - float64(y from the kernel's P and statistics)|, u = 2^-24:
-    normalised value n = fma(v, sc, of), sc = fl(rstd gamma), of = fl(beta - fl(mean sc)): four roundings, |dn| <= NORM_ULPS u (|v sc| +
-    |mean sc| + |beta|) with a factor 2 over them;
-    EPI 2: y = n + resid, one more rounding of |y|;  EPI 1 / 5: y = n_a * s(n_g), s = __fdividef(1, 1 + __expf(-n_g)) with __expf
-    within 2 + 1.173 |n_g| ulp and __fdividef within 2 ulp: |ds| <= s (1 - s) |dn_g| + s (6 + 1.2 |n_g|) u, then one rounding of |y|"""
-    a, g = F.branches(P, gated, shuffle)
-    beta_a, gamma_a, beta_g, gamma_g = (None if t is None else torch.from_numpy(t).double().to(a.device) for t in par)
-    ma, ra, mg, rg = st[:, 0, None], st[:, 1, None], st[:, 2, None], st[:, 3, None]
-
-    def norm_err(v, m, r, gam, bet):
-        sc = (r * gam).abs()
-        return (v * (r * gam) + bet - m * (r * gam)), NORM_ULPS * U * ((v * sc).abs() + (m * sc).abs() + bet.abs())
-    na, ea = norm_err(a, ma, ra, gamma_a, beta_a)
-    if not gated:
-        y = na + torch.from_numpy(resid).double().to(a.device)
-        return ea + U * y.abs() + 1e-45
-    ng, eg = norm_err(g, mg, rg, gamma_g, beta_g)
-    s = torch.sigmoid(ng)
-    y = na * s
-    return s * ea + na.abs() * (s * (1 - s) * eg + s * (6 + 1.2 * ng.abs()) * U) + U * y.abs() + 1e-45
-
-
 def _check_stats(layer, R, prec, got, P, exact_mean, what, rstd_ulps=RSTD_ULPS):
     """the kernel's statistics against float64 of its own P; returns (worst mean error in u * mean|P|, worst rstd error in u)"""
     _, _, Cout, _, gated, sh, epi = F.LAYERS[layer]
@@ -256,7 +232,7 @@ def _check_y(layer, R, prec, out, P, par, resid, what):
     _, _, Cout, _, gated, sh, _ = F.LAYERS[layer]
     st = out["stats"].double()
     ref, _ = F.forward(P, par, gated, sh, resid=resid, stats=st)
-    bound = y_bound(P, st, par, gated, sh, resid)
+    bound = F.y_bound(P, st, par, gated, sh, resid)
     y = out["y"].double()
     err = (y - ref).abs()
     where = lambda i: _where_fwd(layer, R, "y", i)

@@ -96,6 +96,8 @@ def _declare(lib):
         "cgvc_im2col_planes": (ci, [vp, ci, vp, C.c_longlong, ci, ci, ci, ci, vp, vp, vp, vp]),
         "cgvc_in_glu_forward_planes": (ci, [vp] * 8 + [ci] * 6 + [vp] * 5),
         "cgvc_in_glu_backward_planes": (ci, [vp] * 13 + [ci] * 6 + [vp] * 4),
+        "cgvc_in_glu_forward_packed": (ci, [vp] * 8 + [ci] * 5 + [vp] * 2 + [ci] * 3 + [vp] * 4),
+        "cgvc_in_glu_backward_bias": (ci, [vp] * 15 + [ci] * 6 + [vp] * 4),
         "cgvc_conv_in_forward": (ci, [vp, ci] + [vp] * 15 + [ci] * 8 + [P(ci), vp]),
         "cgvc_conv_in_backward": (ci, [vp, ci] + [vp] * 16 + [ci] * 8 + [P(ci), vp]),
         "cgvc_glu_forward_planes": (ci, [vp] * 3 + [ci] * 4 + [vp] * 4),

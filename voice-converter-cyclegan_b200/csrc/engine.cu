@@ -1970,42 +1970,63 @@ int cgvc_im2col_planes(cgvc_handle e, int precision, const float* x, long long r
   return 0;
 }
 
-int cgvc_in_glu_forward_planes(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g,
-                               const float* gamma_g, float* y, float* stats, int B, int R, int C, int shuffle, int precision, int gate,
-                               const float* resid, void* hi, void* lo, unsigned long long* sat, void* stream) {
+// An instance-normed layer in the engine's own description, for the entry points below: gated or residual (the h2 form), shuffle 1
+// or 2, C channels after the pixel-shuffle view.  post_params / post_bwd_params build its launch parameters as a train step does; the
+// entry points then point the affine, plane and counter fields at the caller's buffers.
+static Layer in_layer(int C, int gate, int shuffle) {
+  Layer L{}; L.a.cout = C * shuffle; L.g.cout = gate ? C * shuffle : 0; L.a.cin = L.g.cin = 1; L.has_in = 1; L.sh = L.sw = 1;
+  L.shuffle = shuffle;
+  return L;
+}
+
+// the forward of such a layer over B samples of R positions, or (offsets != null) over packed utterances
+static int in_glu_forward(cgvc_engine* e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g,
+                          const float* gamma_g, float* y, float* stats, int B, int R, int C, int shuffle, int precision, int gate,
+                          const float* resid, const long long* offsets, int n_utt, int div, int max_len, void* hi, void* lo,
+                          unsigned long long* sat, void* stream) {
   if (!e || !p || !y || !stats) return fail(e, CGVC_ERR_ARG, "null argument");
   if (C % 32 != 0 || shuffle < 1 || R % shuffle != 0) return fail(e, CGVC_ERR_UNSUPPORTED, "C must be a multiple of 32 and R of shuffle");
+  if (offsets && (B != 1 || n_utt < 1 || n_utt > 65535 || (div != 1 && div != 2 && div != 4) || div % shuffle || max_len < 4 || max_len % 4))
+    return fail(e, CGVC_ERR_ARG, "cgvc_in_glu_forward_packed: bad packed geometry (B %d, n_utt %d, div %d, max_len %d)", B, n_utt, div, max_len);
   if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  PostParams q; memset(&q, 0, sizeof q);
-  q.p = p; q.ldp = (gate ? 2 : 1) * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
-  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = gate != 0; q.resid = resid;
-  q.y = y; q.stats = stats;
+  ConvIO io{}; io.n = B;
+  if (offsets) { io.n = io.H = 1; io.W = R / shuffle; io.pk = PackGeom{offsets, n_utt, div, max_len}; }
+  const GLAct A{const_cast<float*>(p), stats, y, nullptr, nullptr};
+  PostParams q = post_params(e, in_layer(C, gate, shuffle), io, A, R / shuffle, true, nullptr, resid);
+  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = gate ? beta_g : nullptr; q.gamma_g = gate ? gamma_g : nullptr;
+  q.qmode = 0; q.sat = q.ufl = nullptr;
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.y_hi = (__nv_bfloat16*)hi; q.y_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
     q.ufl = q.qmode ? e->plane_ufl : nullptr;
   }
-  CK(grow_post_buf(e, (size_t)B * 4 * C, &q.scratch));
+  CK(grow_post_buf(e, (size_t)q.B * 4 * C, &q.scratch));
   CK(launch_post_fwd(q, e->opt.post, (cudaStream_t)stream));
   return 0;
 }
 
-int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, const float* stats,
-                                const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
-                                float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
-                                int B, int R, int C, int shuffle, int precision, int gate, void* hi, void* lo, unsigned long long* sat,
-                                void* stream) {
+// its backward, with the conv-bias gradients when dbias_a is given
+static int in_glu_backward(cgvc_engine* e, const float* dy, const float* p, const float* stats,
+                           const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                           float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g, float* dbias_a, float* dbias_g,
+                           int B, int R, int C, int shuffle, int precision, int gate, void* hi, void* lo, unsigned long long* sat,
+                           void* stream) {
   if (!e || !dy || !p || !stats || !dp) return fail(e, CGVC_ERR_ARG, "null argument");
   if (C % 32 != 0 || shuffle < 1 || R % shuffle != 0) return fail(e, CGVC_ERR_UNSUPPORTED, "C must be a multiple of 32 and R of shuffle");
+  if (!dbias_a && dbias_g) return fail(e, CGVC_ERR_ARG, "cgvc_in_glu_backward_bias: dbias_g needs dbias_a");
   if (precision != CGVC_PREC_FP32_SIMT) RET(plane_precision(e, precision, hi, lo));
   DetSlab slab; const DetSlab* det;
   RET(plan_entry_det(e, &slab, &det));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  PostBwdParams q; memset(&q, 0, sizeof q);
+  const GLAct A{const_cast<float*>(p), const_cast<float*>(stats), nullptr, nullptr, nullptr};
+  BwdScratch S; memset(&S, 0, sizeof S); S.dP = dp;
+  if (det) S.det = *det;
+  PostBwdParams q = post_bwd_params(e, in_layer(C, gate, shuffle), dy, A, B, R / shuffle, S, false, true, PlanePair{nullptr, nullptr});
+  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = gate ? beta_g : nullptr; q.gamma_g = gate ? gamma_g : nullptr;
+  q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = gate ? dbeta_g : nullptr; q.dgamma_g = gate ? dgamma_g : nullptr;
+  q.dbias_a = dbias_a; q.dbias_g = gate ? dbias_g : nullptr;
   if (det) q.det = *det;
-  q.dy1 = dy; q.p = p; q.ldp = (gate ? 2 : 1) * C * shuffle; q.Cc = C * shuffle; q.B = B; q.R = R; q.C = C; q.sh = shuffle;
-  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = beta_g; q.gamma_g = gamma_g; q.has_in = 1; q.has_gate = gate != 0; q.stats = stats;
-  q.dp = dp; q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = dbeta_g; q.dgamma_g = dgamma_g;
+  q.qmode = 0; q.sat = q.ufl = nullptr;
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
     q.ufl = q.qmode ? e->plane_ufl : nullptr;
@@ -2060,6 +2081,40 @@ int cgvc_conv_in_backward(cgvc_handle e, int precision, const float* dp, const f
   f.dbeta_a = dbeta_a; f.dgamma_a = dgamma_a; f.dbeta_g = dbeta_g; f.dgamma_g = dgamma_g;
   return tc_result(e, tc_conv_in_bwd_adhoc(precision, e->tcw.debug, e->opt.post, dp, w_a, w_g, f, dx, accumulate, B, R, Cin, kw, Cout, fuse, fused, det, (cudaStream_t)stream),
                    nullptr, "conv data gradient + instance norm backward");
+}
+
+int cgvc_in_glu_forward_planes(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g,
+                               const float* gamma_g, float* y, float* stats, int B, int R, int C, int shuffle, int precision, int gate,
+                               const float* resid, void* hi, void* lo, unsigned long long* sat, void* stream) {
+  return in_glu_forward(e, p, beta_a, gamma_a, beta_g, gamma_g, y, stats, B, R, C, shuffle, precision, gate, resid, nullptr, 0, 0, 0,
+                        hi, lo, sat, stream);
+}
+
+int cgvc_in_glu_forward_packed(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g,
+                               const float* gamma_g, float* y, float* stats, int R, int C, int shuffle, int precision, int gate,
+                               const float* resid, const long long* offsets, int n_utt, int div, int max_len, void* hi, void* lo,
+                               unsigned long long* sat, void* stream) {
+  if (!offsets) return fail(e, CGVC_ERR_ARG, "null argument");
+  return in_glu_forward(e, p, beta_a, gamma_a, beta_g, gamma_g, y, stats, 1, R, C, shuffle, precision, gate, resid, offsets, n_utt, div,
+                        max_len, hi, lo, sat, stream);
+}
+
+int cgvc_in_glu_backward_planes(cgvc_handle e, const float* dy, const float* p, const float* stats,
+                                const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                                float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g,
+                                int B, int R, int C, int shuffle, int precision, int gate, void* hi, void* lo, unsigned long long* sat,
+                                void* stream) {
+  return in_glu_backward(e, dy, p, stats, beta_a, gamma_a, beta_g, gamma_g, dp, dbeta_a, dgamma_a, dbeta_g, dgamma_g, nullptr, nullptr,
+                         B, R, C, shuffle, precision, gate, hi, lo, sat, stream);
+}
+
+int cgvc_in_glu_backward_bias(cgvc_handle e, const float* dy, const float* p, const float* stats,
+                              const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
+                              float* dp, float* dbeta_a, float* dgamma_a, float* dbeta_g, float* dgamma_g, float* dbias_a, float* dbias_g,
+                              int B, int R, int C, int shuffle, int precision, int gate, void* hi, void* lo, unsigned long long* sat,
+                              void* stream) {
+  return in_glu_backward(e, dy, p, stats, beta_a, gamma_a, beta_g, gamma_g, dp, dbeta_a, dgamma_a, dbeta_g, dgamma_g, dbias_a, dbias_g,
+                         B, R, C, shuffle, precision, gate, hi, lo, sat, stream);
 }
 
 int cgvc_in_glu_forward(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g, const float* gamma_g,
