@@ -235,6 +235,32 @@ int cgvc_discriminator_backward_tape(cgvc_handle h, const void* tape_dev, const 
  * h1_glu d1 d2 d3 (discriminator).  n_out receives the element count. */
 int cgvc_debug_activation(cgvc_handle h, const char* name, float* out_dev, size_t capacity, size_t* n_out, void* stream);
 
+/* Read-only view of the tensor-core weight store: the reduced-precision copies of PARAM in GEMM layout ("weight planes") that every
+ * tensor-core GEMM reads instead of PARAM, rebuilt whenever PARAM changes (tests/test_gpu_weight_planes.py checks them against
+ * tests/weight_planes_ref.py).  Layers are numbered in registration order, 0 .. n_layers - 1 (no layers: CGVC_PREC_FP32_SIMT).
+ * Extents: *_k rounded up to 64, *_n and *_q to 128; Ntot = cout * (gated ? 2 : 1). */
+typedef struct cgvc_weight_layer_info {
+  int n_layers;                     /* layers in the store */
+  int kh, kw, cin, cout, gated;     /* the registered shape: TF kernel [kh, kw, cin, cout] per branch */
+  int shuffle;                      /* 2: the output goes through the pixel shuffler (forward rows then in the shuffle order) */
+  int fold;                         /* > 0: a 1 x 1 layer whose cout columns are the (tap, channel) pairs of a [1, fold, cin, cout / fold] kernel */
+  long long ka, kg, ba, bg;         /* PARAM offsets (elements) of kernel_a / kernel_g / bias_a / bias_g */
+  int nt_n, cin_k, cin_n, nt_k, cin_q, nt_q;   /* padded extents of the planes below */
+  int q_ok;                         /* the layer's shape has F16F8 planes (cin a multiple of 4) */
+} cgvc_weight_layer_info;
+/* cgvc_weight_planes: *info (may be NULL) receives layer `layer`'s registration; with `plane` non-NULL, *bytes_out the size of that
+ * plane (padding included) and, when out_dev is non-NULL, a copy of it enqueued on `stream` (capacity: bytes at out_dev).  Planes:
+ *   "wf_hi", "wf_lo"    bf16 [taps][nt_n][cin_k]   forward layout (row order: see tc_gemm.cu perm_row)
+ *   "wd_hi", "wd_lo"    bf16 [taps][cin_n][nt_k]   data-gradient layout (gate branch at column offset cout)
+ *   "wq16", "wq8hi", "wq8lo"      fp16 / e4m3 / e4m3 [taps][nt_n][cin_q]   F16F8, forward layout, weight-role scales
+ *   "wdq16", "wdq8hi", "wdq8lo"   fp16 / e4m3 / e4m3 [taps][cin_n][nt_q]   F16F8, data-gradient layout (training engines)
+ *   "bias"              fp32 [nt_n] in forward row order (zero for tap-folded layers)
+ * A plane the engine does not keep is refused with CGVC_ERR_ARG: the F16F8 planes outside CGVC_PREC_F16F8, the F16F8 data-gradient
+ * planes of a forward-only engine, and in CGVC_PREC_F16F8 the bf16 planes of a layer with F16F8 planes.  Launches no kernel; refused
+ * while `stream` is capturing a graph. */
+int cgvc_weight_planes(cgvc_handle h, int layer, cgvc_weight_layer_info* info, const char* plane, void* out_dev, size_t capacity,
+                       size_t* bytes_out, void* stream);
+
 /* -- device-resident training data (replaces the per-step host feed of train.py:90-107 / preprocess.py:207-238) ---------------
  * The caller uploads each speaker's normalised MCEP corpus once: utterance u as a row-major [num_features][len_u] block at element
  * num_features * offsets[u] of corpus_X_dev, offsets_X_dev = n_X + 1 frame prefix sums (int64).

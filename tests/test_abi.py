@@ -26,6 +26,20 @@ def test_library_exports_every_declared_symbol():
     assert lib.cgvc_abi_version() == 1
 
 
+def test_weight_layer_info_matches_the_header():
+    """cgvc_weight_layer_info (include/cgvc.h) and its ctypes mirror: the same fields in the same order, of the same C types"""
+    from cgvc import native
+    src = open(os.path.join(ROOT, "include", "cgvc.h")).read()
+    body = re.search(r"typedef struct cgvc_weight_layer_info \{(.*?)\} cgvc_weight_layer_info;", src, flags=re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    decl = []
+    for ctype, names in re.findall(r"(long long|int)\s+([\w\s,]+);", body):
+        decl += [(n.strip(), ctype) for n in names.split(",")]
+    mirror = [(n, {C.c_int: "int", C.c_longlong: "long long"}[t]) for n, t in native.WeightLayerInfo._fields_]
+    assert mirror == decl
+    assert native.load().cgvc_weight_planes.argtypes[2] == C.POINTER(native.WeightLayerInfo)
+
+
 def test_library_is_sm90a_with_wgmma():
     import subprocess
     from cgvc import native

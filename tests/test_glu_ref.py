@@ -1,5 +1,5 @@
 """CPU checks of tests/glu_ref.py (the float64 references of the layers without an instance norm and of the loss heads), and the map from
-every kernel of csrc/simt_kernels.cu to the unit test that reaches it."""
+every kernel of csrc/simt_kernels.cu and csrc/tc_gemm.cu to the unit test that reaches it."""
 import os
 import re
 
@@ -141,14 +141,37 @@ EXEMPT = {
 }
 
 
-def test_every_kernel_has_a_unit_test_or_an_exemption():
-    src = open(os.path.join(ROOT, "voice-converter-cyclegan_b200", "csrc", "simt_kernels.cu")).read()
-    names = set(re.findall(r"__global__\s+(?:void\s+)?(?:__launch_bounds__\([^)]*\)\s*)?(?:void\s+)?(\w+)\s*\(", src))
-    assert len(names) > 20, sorted(names)
-    missing = sorted(n for n in names if n not in REACHED and n not in EXEMPT)
+# the same for csrc/tc_gemm.cu
+REACHED_TC = {
+    "tc_gg_nt_kernel": "test_gpu_gemm_exact.py", "tc_gg_tn_kernel": "test_gpu_gemm_exact.py",
+    "prep_weights_kernel": "test_gpu_weight_planes.py", "copy_bias_kernel": "test_gpu_weight_planes.py",
+    "prep_weights_q_kernel": "test_gpu_weight_planes.py (prep_batched 0)", "prep_weights_qd_kernel": "test_gpu_weight_planes.py (prep_batched 0)",
+    "prep_weights_q_all_kernel": "test_gpu_weight_planes.py",
+}
+
+
+def _kernels(source):
+    src = open(os.path.join(ROOT, "voice-converter-cyclegan_b200", "csrc", source)).read()
+    return set(re.findall(r"__global__\s+(?:void\s+)?(?:__launch_bounds__\([^)]*\)\s*)?(?:void\s+)?(\w+)\s*\(", src))
+
+
+def _audit(names, reached, exempt):
+    missing = sorted(n for n in names if n not in reached and n not in exempt)
     assert not missing, "kernels with neither a unit test nor an exemption: %s" % missing
-    stale = sorted(n for n in list(REACHED) + list(EXEMPT) if n not in names)
+    stale = sorted(n for n in list(reached) + list(exempt) if n not in names)
     assert not stale, "entries for kernels that no longer exist: %s" % stale
-    for n, where in REACHED.items():
+    for n, where in reached.items():
         f = where.split(" ")[0]
         assert os.path.exists(os.path.join(ROOT, "tests", f)), (n, f)
+
+
+def test_every_kernel_has_a_unit_test_or_an_exemption():
+    names = _kernels("simt_kernels.cu")
+    assert len(names) > 20, sorted(names)
+    _audit(names, REACHED, EXEMPT)
+
+
+def test_every_tensor_core_kernel_has_a_unit_test():
+    names = _kernels("tc_gemm.cu")
+    assert len(names) >= 7, sorted(names)
+    _audit(names, REACHED_TC, {})

@@ -44,6 +44,13 @@ class LossScaleNetInfo(C.Structure):
                 ("groups", C.c_ulonglong)]
 
 
+class WeightLayerInfo(C.Structure):
+    """cgvc_weight_layer_info of include/cgvc.h"""
+    _fields_ = [(n, C.c_int) for n in ("n_layers", "kh", "kw", "cin", "cout", "gated", "shuffle", "fold")] + \
+               [(n, C.c_longlong) for n in ("ka", "kg", "ba", "bg")] + \
+               [(n, C.c_int) for n in ("nt_n", "cin_k", "cin_n", "nt_k", "cin_q", "nt_q", "q_ok")]
+
+
 class CgvcError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("libcgvc error %d: %s" % (code, msg))
@@ -77,6 +84,7 @@ def _declare(lib):
         "cgvc_generator_forward_packed": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp]),
         "cgvc_discriminator_forward": (ci, [vp, ci, vp, vp, ci, ci, vp]),
         "cgvc_debug_activation": (ci, [vp, C.c_char_p, vp, sz, P(sz), vp]),
+        "cgvc_weight_planes": (ci, [vp, ci, P(WeightLayerInfo), C.c_char_p, vp, sz, P(sz), vp]),
         "cgvc_comm_unique_id": (ci, [vp, vp]),
         "cgvc_comm_init": (ci, [vp, vp, ci, ci]),
         "cgvc_comm_destroy": (ci, [vp]),

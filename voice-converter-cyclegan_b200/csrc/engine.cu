@@ -1409,6 +1409,32 @@ int cgvc_debug_activation(cgvc_handle e, const char* name, float* out_dev, size_
   return 0;
 }
 
+int cgvc_weight_planes(cgvc_handle e, int layer, cgvc_weight_layer_info* info, const char* plane, void* out_dev, size_t capacity,
+                       size_t* bytes_out, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  const int n = (int)e->tcw.layers.size();
+  if (layer < 0 || layer >= n) return fail(e, CGVC_ERR_ARG, "cgvc_weight_planes: layer %d outside [0, %d)", layer, n);
+  const TcLayer& L = e->tcw.layers[layer];
+  if (info) {
+    int d[7]; tc_layer_dims(e->tcw, layer, d);
+    *info = cgvc_weight_layer_info{n, L.kh, L.kw, L.cin, L.cout, L.gated, L.shuffle, L.fold,
+                                   (long long)L.ka, (long long)L.kg, (long long)L.ba, (long long)L.bg, d[0], d[1], d[2], d[3], d[4], d[5], d[6]};
+  }
+  if (!plane) return 0;
+  const void* src = nullptr; size_t bytes = 0;
+  if (tc_layer_plane(e->tcw, layer, plane, &src, &bytes) != 0) return fail(e, CGVC_ERR_ARG, "cgvc_weight_planes: unknown plane '%s'", plane);
+  if (!src) return fail(e, CGVC_ERR_ARG, "cgvc_weight_planes: layer %d keeps no plane '%s' in this engine", layer, plane);
+  if (bytes_out) *bytes_out = bytes;
+  if (!out_dev) return 0;
+  if (capacity < bytes) return fail(e, CGVC_ERR_ARG, "cgvc_weight_planes: plane '%s' of layer %d needs %zu bytes", plane, layer, bytes);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CK(cudaStreamIsCapturing((cudaStream_t)stream, &cs));
+  if (cs != cudaStreamCaptureStatusNone) return fail(e, CGVC_ERR_ARG, "cgvc_weight_planes: stream is capturing a graph");
+  CK(cudaMemcpyAsync(out_dev, src, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+
 // forward + losses + backward of one training step; leaves gradients in GRAD (model.py:44-90,107-108)
 // one lane of the step (see LanePlan), enqueued on stream st
 static int run_lane(cgvc_engine* e, LanePlan& L, int lane, const float* Yreal_dev, int B, int T, float lambda_identity,

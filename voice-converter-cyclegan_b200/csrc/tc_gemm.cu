@@ -25,6 +25,7 @@
 #include <cuda.h>      // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint, no libcuda link)
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 
 namespace {
 
@@ -1896,6 +1897,28 @@ int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, si
     }
   }
   return 0;
+}
+
+void tc_layer_dims(const TcWeights& w, int slot, int dims[7]) {
+  const TcLayer& L = w.layers[slot];
+  const int d[7] = {nt_n(L), cin_k(L), cin_n(L), nt_k(L), cin_q(L), nt_q(L), layer_ok_q(L) ? 1 : 0};
+  for (int i = 0; i < 7; ++i) dims[i] = d[i];
+}
+
+int tc_layer_plane(const TcWeights& w, int slot, const char* name, const void** p, size_t* bytes) {
+  const TcLayer& L = w.layers[slot];
+  const bool bf = w.pool && !L.wq16;                 // refresh_layer writes the bf16 planes only for layers without F16F8 planes
+  struct Plane { const char* name; const void* p; size_t bytes; };
+  const Plane planes[] = {
+    {"wf_hi", bf ? L.wf_hi : nullptr, wf_elems(L) * 2}, {"wf_lo", bf ? L.wf_lo : nullptr, wf_elems(L) * 2},
+    {"wd_hi", bf ? L.wd_hi : nullptr, wd_elems(L) * 2}, {"wd_lo", bf ? L.wd_lo : nullptr, wd_elems(L) * 2},
+    {"wq16", L.wq16, wq_elems(L) * 2}, {"wq8hi", L.wq8hi, wq_elems(L)}, {"wq8lo", L.wq8lo, wq_elems(L)},
+    {"wdq16", L.wdq16, wdq_elems(L) * 2}, {"wdq8hi", L.wdq8hi, wdq_elems(L)}, {"wdq8lo", L.wdq8lo, wdq_elems(L)},
+    {"bias", w.pool ? L.bias : nullptr, (size_t)nt_n(L) * sizeof(float)},
+  };
+  for (const Plane& q : planes)
+    if (!strcmp(q.name, name)) { *p = q.p; *bytes = q.p ? q.bytes : 0; return 0; }
+  return -1;
 }
 
 cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st,

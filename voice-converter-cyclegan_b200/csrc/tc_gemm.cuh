@@ -79,6 +79,11 @@ int tc_alloc(TcWeights& w, int precision, bool train);
 void tc_free(TcWeights& w);
 int tc_refresh_weights(TcWeights& w, const float* params, cudaStream_t st);
 int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, size_t end, cudaStream_t st);
+// Read-only view of registered layer `slot` (include/cgvc.h cgvc_weight_planes).  dims = {nt_n, cin_k, cin_n, nt_k, cin_q, nt_q, layer_ok_q}.
+// tc_layer_plane: the device address and size in bytes (padding included) of a named plane; *p = null when the store keeps no such plane
+// current (not allocated, or the bf16 planes of a layer that an F16F8 store serves from its F16F8 planes).  Returns -1 for an unknown name.
+void tc_layer_dims(const TcWeights& w, int slot, int dims[7]);
+int tc_layer_plane(const TcWeights& w, int slot, const char* name, const void** p, size_t* bytes);
 
 // x [rows, C] fp32 -> the operand planes of `precision` with C zero-padded to the contraction width: bf16 hi / lo [rows, ru64(C)],
 // F16F8: q16 (hi) and q8hi followed by q8lo (lo) [rows, ru128(C)].  cudaError_t
