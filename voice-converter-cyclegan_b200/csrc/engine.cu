@@ -325,28 +325,28 @@ static int conv_out_dims(const ConvW& c, int sh, int sw, int H, int W, int& Ho, 
 }
 
 // y[., coff:coff+cout] = conv(x, w) + b  into a row-major [rows, ld] buffer
-static int conv_fwd_simt(cgvc_engine* e, const float* Pm, const ConvW& c, int sh, int sw, const ConvIO& io,
+static int conv_fwd_simt(cgvc_engine* e, const float* w, const float* bias, const ConvW& c, int sh, int sw, const ConvIO& io,
                          float* dst, int ld, int coff, cudaStream_t st) {
   if (!io.x) return fail(e, CGVC_ERR_UNSUPPORTED, "fp32 activations were not kept for a layer that fell back to the SIMT path");
   GatherGeom g = fwd_geom(io.n, io.H, io.W, c.kh, c.kw, sh, sw);
   GemmOperands op; memset(&op, 0, sizeof op);
   op.src = io.x; op.s_ld = c.cin; op.s_coff = 0; op.C = c.cin;
-  op.w = Pm + c.k; op.w_ts = (long long)c.cin * c.cout; op.w_cs = c.cout; op.w_ns = 1; op.N = c.cout;
-  op.dst = dst; op.d_ld = ld; op.d_coff = coff; op.bias = Pm + c.b; op.accumulate = 0;
+  op.w = w; op.w_ts = (long long)c.cin * c.cout; op.w_cs = c.cout; op.w_ns = 1; op.N = c.cout;
+  op.dst = dst; op.d_ld = ld; op.d_coff = coff; op.bias = bias; op.accumulate = 0;
   if (io.pk.off) CK(launch_gg_simt_packed(g, op, io.pk, st));
   else CK(launch_gg_simt(g, op, st));
   return 0;
 }
 
 // dx (+)= dgrad(dy[., coff:coff+cout], w)
-static int conv_dgrad_simt(cgvc_engine* e, const float* Pm, const ConvW& c, int sh, int sw, int n, int H, int W,
+static int conv_dgrad_simt(cgvc_engine* e, const float* w, const ConvW& c, int sh, int sw, int n, int H, int W,
                            const float* dy, int ld, int coff, float* dx, int accumulate, cudaStream_t st) {
   if (!dy) return fail(e, CGVC_ERR_UNSUPPORTED, "fp32 gradients were not kept for a layer that fell back to the SIMT path");
   std::vector<GatherGeom> gs = dgrad_geoms(n, H, W, c.kh, c.kw, sh, sw);
   for (const GatherGeom& g : gs) {
     GemmOperands op; memset(&op, 0, sizeof op);
     op.src = dy; op.s_ld = ld; op.s_coff = coff; op.C = c.cout;
-    op.w = Pm + c.k; op.w_ts = (long long)c.cin * c.cout; op.w_cs = 1; op.w_ns = c.cout; op.N = c.cin;
+    op.w = w; op.w_ts = (long long)c.cin * c.cout; op.w_cs = 1; op.w_ns = c.cout; op.N = c.cin;
     op.dst = dx; op.d_ld = c.cin; op.d_coff = 0; op.bias = nullptr; op.accumulate = accumulate;
     CK(launch_gg_simt(g, op, st));
   }
@@ -354,11 +354,11 @@ static int conv_dgrad_simt(cgvc_engine* e, const float* Pm, const ConvW& c, int 
 }
 
 // dW += x^T * dy (forward geometry); the bias gradient comes from the IN/GLU backward kernel (or launch_colsum for o1)
-static int conv_wgrad_simt(cgvc_engine* e, float* Gm, const ConvW& c, int sh, int sw, const ConvIO& io,
+static int conv_wgrad_simt(cgvc_engine* e, float* dw, const ConvW& c, int sh, int sw, const ConvIO& io,
                            const float* dy, int ld, int coff, cudaStream_t st, const DetSlab* det) {
   if (!io.x || !dy) return fail(e, CGVC_ERR_UNSUPPORTED, "fp32 tensors were not kept for a layer that fell back to the SIMT path");
   GatherGeom g = fwd_geom(io.n, io.H, io.W, c.kh, c.kw, sh, sw);
-  CK(launch_wgrad_simt(g, io.x, c.cin, 0, c.cin, dy, ld, coff, c.cout, Gm + c.k, (long long)c.cin * c.cout, c.cout, 1, st, det != nullptr));
+  CK(launch_wgrad_simt(g, io.x, c.cin, 0, c.cin, dy, ld, coff, c.cout, dw, (long long)c.cin * c.cout, c.cout, 1, st, det != nullptr));
   return 0;
 }
 
@@ -399,76 +399,104 @@ static unsigned long long* sat_act(const cgvc_engine* e) {
 static bool tc_enabled(const cgvc_engine* e) { return e->cfg.precision != CGVC_PREC_FP32_SIMT && e->tcw.ready; }
 static bool use_tc(const cgvc_engine* e, int slot) { return slot >= 0 && tc_enabled(e); }
 
-// How a tensor-core call on layer c (null: an ad-hoc convolution) ended: done (*done = true); unsupported (TC_UNSUPPORTED, nothing
+// One layer's tensors by pointer, so that the train step, the conversions, the tapes and the test entry points run the same launches:
+// kernels, biases and instance-norm affine parameters of branches a and g (null where the layer has none), their gradients (null: no
+// gradient), and the tensor-core layer whose planes the convolutions read (null: the fp32 SIMT path) with the precision and the store
+// options (TcWeights::debug, TcWeights::wgrad16) it runs with
+struct LayerTensors {
+  const float *ka, *kg, *ba, *bg, *beta_a, *gamma_a, *beta_g, *gamma_g;
+  float *dka, *dkg, *dba, *dbg, *dbeta_a, *dgamma_a, *dbeta_g, *dgamma_g;
+  const TcLayer* tc;
+  int precision, debug, wgrad16;
+};
+
+// ... of registered layer L: PARAM, with grads GRAD, and the engine's tensor-core store
+static LayerTensors layer_tensors(const cgvc_engine* e, const Layer& L, bool grads) {
+  LayerTensors t; memset(&t, 0, sizeof t);
+  const float* Pm = e->P();
+  t.ka = Pm + L.a.k; t.ba = Pm + L.a.b;
+  if (L.gated()) { t.kg = Pm + L.g.k; t.bg = Pm + L.g.b; }
+  if (L.has_in) { t.beta_a = Pm + L.ina.beta; t.gamma_a = Pm + L.ina.gamma; }
+  if (L.has_in && L.gated()) { t.beta_g = Pm + L.ing.beta; t.gamma_g = Pm + L.ing.gamma; }
+  if (grads) {
+    float* Gm = e->G();
+    t.dka = Gm + L.a.k; t.dba = Gm + L.a.b;
+    if (L.gated()) { t.dkg = Gm + L.g.k; t.dbg = Gm + L.g.b; }
+    if (L.has_in) { t.dbeta_a = Gm + L.ina.beta; t.dgamma_a = Gm + L.ina.gamma; }
+    if (L.has_in && L.gated()) { t.dbeta_g = Gm + L.ing.beta; t.dgamma_g = Gm + L.ing.gamma; }
+  }
+  t.tc = use_tc(e, L.tc_slot) ? &e->tcw.layers[L.tc_slot] : nullptr;
+  t.precision = e->cfg.precision; t.debug = e->tcw.debug; t.wgrad16 = e->tcw.wgrad16;
+  return t;
+}
+
+// How a tensor-core call on layer c ended: done (*done = true); unsupported (TC_UNSUPPORTED, nothing
 // launched): the caller falls back to SIMT where it passes `done`, else CGVC_ERR_UNSUPPORTED; or failed: CGVC_ERR_CUDA
 static int tc_result(cgvc_engine* e, int r, const ConvW* c, const char* what, bool* done = nullptr) {
   if (r == 0) { if (done) *done = true; return 0; }
   if (r == TC_UNSUPPORTED && done) return 0;
   std::string where = what;
-  if (c) for (const TensorInfo& t : e->tensors) if (t.off == c->k) where = t.name + " " + what;
+  for (const TensorInfo& t : e->tensors) if (t.off == c->k) where = t.name + " " + what;
   if (r == TC_UNSUPPORTED) return fail(e, CGVC_ERR_UNSUPPORTED, "%s: shape not supported by the tensor-core path", where.c_str());
   return fail(e, CGVC_ERR_CUDA, "%s on the tensor cores: %s", where.c_str(), cudaGetErrorString((cudaError_t)r));
 }
 
 // P = conv(x) + bias, plain epilogue (gated: conv_a || conv_g -> P [rows, 2*cout])
-static int conv_fwd(cgvc_engine* e, const Layer& L, const ConvIO& io, float* P, cudaStream_t st) {
+static int conv_fwd(cgvc_engine* e, const Layer& L, const LayerTensors& t, const ConvIO& io, float* P, cudaStream_t st) {
   bool done = false;
-  if (use_tc(e, L.tc_slot) && io.xhi)
-    RET(tc_result(e, tc_conv_fwd(e->tcw, L.tc_slot, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, P, st, nullptr, nullptr, packed(io)),
+  if (t.tc && io.xhi)
+    RET(tc_result(e, tc_conv_fwd(*t.tc, t.precision, t.debug, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, P, st, nullptr, nullptr, packed(io)),
                   &L.a, "forward", &done));
   if (done) return 0;
-  const float* Pm = e->P();
   if (L.gated() && L.a.cin == 1 && io.x && !io.pk.off && L.a.cout % 4 == 0 && 256 % (L.a.cout / 2) == 0) {   // discriminator h1: HBM-bound special
     GatherGeom g = fwd_geom(io.n, io.H, io.W, L.a.kh, L.a.kw, L.sh, L.sw);
-    CK(launch_conv_c1_fwd(g, io.x, Pm + L.a.k, Pm + L.g.k, Pm + L.a.b, Pm + L.g.b, L.a.cout, P, st));
+    CK(launch_conv_c1_fwd(g, io.x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, st));
     return 0;
   }
-  RET(conv_fwd_simt(e, Pm, L.a, L.sh, L.sw, io, P, L.width(), 0, st));
-  if (L.gated()) RET(conv_fwd_simt(e, Pm, L.g, L.sh, L.sw, io, P, L.width(), L.a.cout, st));
+  RET(conv_fwd_simt(e, t.ka, t.ba, L.a, L.sh, L.sw, io, P, L.width(), 0, st));
+  if (L.gated()) RET(conv_fwd_simt(e, t.kg, t.bg, L.g, L.sh, L.sw, io, P, L.width(), L.a.cout, st));
   return 0;
 }
 
 // dx[io's n,H,W] (+)= dgrad(dP); fuse: see tc_conv_dgrad
-static int conv_dgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const float* dP, PlanePair dp, float* dx, int accumulate,
-                      cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr) {
+static int conv_dgrad(cgvc_engine* e, const Layer& L, const LayerTensors& t, const ConvIO& io, const float* dP, PlanePair dp, float* dx,
+                      int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr) {
   bool done = false;
-  if (use_tc(e, L.tc_slot) && dp.hi)
-    RET(tc_result(e, tc_conv_dgrad(e->tcw, L.tc_slot, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, dx, accumulate, st, fuse, fused),
+  if (t.tc && dp.hi)
+    RET(tc_result(e, tc_conv_dgrad(*t.tc, t.precision, t.debug, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, dx, accumulate, st, fuse, fused),
                   &L.a, "data gradient", &done));
   if (done) return 0;
-  RET(conv_dgrad_simt(e, e->P(), L.a, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), 0, dx, accumulate, st));
-  if (L.gated()) RET(conv_dgrad_simt(e, e->P(), L.g, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), L.a.cout, dx, 1, st));
+  RET(conv_dgrad_simt(e, t.ka, L.a, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), 0, dx, accumulate, st));
+  if (L.gated()) RET(conv_dgrad_simt(e, t.kg, L.g, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), L.a.cout, dx, 1, st));
   return 0;
 }
 
 // det: deterministic mode (the lane's partials slab), else null
-static int conv_wgrad(cgvc_engine* e, const Layer& L, const ConvIO& io, const float* dP, PlanePair dp, cudaStream_t st, const DetSlab* det) {
-  float* Gm = e->G();
+static int conv_wgrad(cgvc_engine* e, const Layer& L, const LayerTensors& t, const ConvIO& io, const float* dP, PlanePair dp, cudaStream_t st,
+                      const DetSlab* det) {
   bool done = false;
-  if (use_tc(e, L.tc_slot) && dp.hi && io.xhi)
-    RET(tc_result(e, tc_conv_wgrad(e->tcw, L.tc_slot, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw,
-                                   Gm + L.a.k, L.gated() ? Gm + L.g.k : nullptr, st, det), &L.a, "weight gradient", &done));
+  if (t.tc && dp.hi && io.xhi)
+    RET(tc_result(e, tc_conv_wgrad(*t.tc, t.precision, t.wgrad16, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, t.dka, t.dkg,
+                                   st, det), &L.a, "weight gradient", &done));
   if (done) return 0;
-  RET(conv_wgrad_simt(e, Gm, L.a, L.sh, L.sw, io, dP, L.width(), 0, st, det));
-  if (L.gated()) RET(conv_wgrad_simt(e, Gm, L.g, L.sh, L.sw, io, dP, L.width(), L.a.cout, st, det));
+  RET(conv_wgrad_simt(e, t.dka, L.a, L.sh, L.sw, io, dP, L.width(), 0, st, det));
+  if (L.gated()) RET(conv_wgrad_simt(e, t.dkg, L.g, L.sh, L.sw, io, dP, L.width(), L.a.cout, st, det));
   return 0;
 }
 
 // instance norm (+ GLU | + resid) and pixel shuffle of A.P, the output of L's convolution over io (rows_per_sample_out rows per sample)
-static PostParams post_params(const cgvc_engine* e, const Layer& L, const ConvIO& io, const GLAct& A, int rows_per_sample_out, bool keep_y,
-                              float* scratch, const float* resid = nullptr) {
+static PostParams post_params(const cgvc_engine* e, const Layer& L, const LayerTensors& t, const ConvIO& io, const GLAct& A,
+                              int rows_per_sample_out, bool keep_y, float* scratch, const float* resid = nullptr) {
   PostParams q; memset(&q, 0, sizeof q);
   q.scratch = scratch;
-  const float* Pm = e->P();
   q.p = A.P; q.ldp = L.width(); q.Cc = L.a.cout; q.B = io.n; q.sh = L.shuffle;
   q.R = rows_per_sample_out * L.shuffle; q.C = L.a.cout / L.shuffle;
   q.has_in = L.has_in; q.has_gate = L.gated();
-  if (L.has_in) { q.beta_a = Pm + L.ina.beta; q.gamma_a = Pm + L.ina.gamma; }
-  if (L.has_in && L.gated()) { q.beta_g = Pm + L.ing.beta; q.gamma_g = Pm + L.ing.gamma; }
+  q.beta_a = t.beta_a; q.gamma_a = t.gamma_a; q.beta_g = t.beta_g; q.gamma_g = t.gamma_g;
   q.resid = resid;
   q.y = (keep_y || !A.Yhi) ? A.Y : nullptr;      // without planes the fp32 activation is the only copy
   q.stats = L.has_in ? A.stats : nullptr; q.y_hi = A.Yhi; q.y_lo = A.Ylo;
-  q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+  q.qmode = t.precision == CGVC_PREC_F16F8;
   q.sat = sat_act(e);
   if (io.pk.off && L.has_in) {
     // packed utterances: q describes one sample holding all q.R view rows; instance norm runs per utterance over its own view rows
@@ -484,26 +512,26 @@ static PostParams post_params(const cgvc_engine* e, const Layer& L, const ConvIO
 // One layer's forward: convolution, then instance norm (+ GLU | + resid) and pixel shuffle into A.  The paths, in order: tensor
 // cores with the norm fused into the GEMM epilogue (1-D layer, not packed, whole samples per 128-row tile); else tensor cores with
 // the plain epilogue, or SIMT, then the instance-norm kernels.  keep_y: also write the fp32 output.  save_pre = false (inference):
-// the fused epilogue need not write the pre-norm output and statistics, as nothing runs backward
-static int layer_forward(cgvc_engine* e, const Layer& L, const ConvIO& io, const GLAct& A, int rows_per_sample_out, bool keep_y,
-                         bool save_pre, float* post_scratch, cudaStream_t st, const float* resid = nullptr) {
+// the fused epilogue need not write the pre-norm output and statistics, as nothing runs backward.  fuse: the fused epilogue may run
+// (option fuse_in); *fused (may be null) is set when it did
+static int layer_forward(cgvc_engine* e, const Layer& L, const LayerTensors& t, const ConvIO& io, const GLAct& A, int rows_per_sample_out,
+                         bool keep_y, bool save_pre, bool fuse, float* post_scratch, cudaStream_t st, const float* resid = nullptr,
+                         bool* fused = nullptr) {
   bool done = false;
-  if (use_tc(e, L.tc_slot) && io.xhi && !io.pk.off && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && e->opt.fuse_in) {
-    const float* Pm = e->P();
+  if (t.tc && io.xhi && !io.pk.off && L.has_in && (L.shuffle == 1 || L.shuffle == 2) && io.H == 1 && A.Yhi && fuse) {
     TcFuse f; memset(&f, 0, sizeof f);
     f.R = rows_per_sample_out;
-    f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta;
-    if (L.gated()) { f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta; }
+    f.gamma_a = t.gamma_a; f.beta_a = t.beta_a; f.gamma_g = t.gamma_g; f.beta_g = t.beta_g;
     f.stats = save_pre ? A.stats : nullptr; f.resid = resid; f.y = keep_y ? A.Y : nullptr; f.y_hi = A.Yhi; f.y_lo = A.Ylo;
-    bool fused = false;
-    int r = tc_conv_fwd(e->tcw, L.tc_slot, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, save_pre ? A.P : nullptr, st, &f, &fused);
+    bool in_epi = false;
+    int r = tc_conv_fwd(*t.tc, t.precision, t.debug, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, save_pre ? A.P : nullptr, st, &f, &in_epi);
     if (r != 0 && !save_pre)                                  // shape not fusable: the two-kernel path needs P as its intermediate
-      r = tc_conv_fwd(e->tcw, L.tc_slot, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, A.P, st, &f, &fused);
+      r = tc_conv_fwd(*t.tc, t.precision, t.debug, io.xhi, io.xlo, io.n, io.H, io.W, L.sh, L.sw, A.P, st, &f, &in_epi);
     RET(tc_result(e, r, &L.a, "forward", &done));
-    if (fused) return 0;
+    if (in_epi) { if (fused) *fused = true; return 0; }
   }
-  if (!done) RET(conv_fwd(e, L, io, A.P, st));
-  PostParams q = post_params(e, L, io, A, rows_per_sample_out, keep_y, post_scratch, resid);
+  if (!done) RET(conv_fwd(e, L, t, io, A.P, st));
+  PostParams q = post_params(e, L, t, io, A, rows_per_sample_out, keep_y, post_scratch, resid);
   CK(launch_post_fwd(q, e->opt.post, st));
   return 0;
 }
@@ -561,7 +589,8 @@ static int h1_edge_forward(cgvc_engine* e, const GenNet& N, const float* x, int 
   const int nf = e->cfg.num_features;
   CK(launch_im2col_taps(x, (long long)n * T, T, nf, N.h1.a.kw, +1, edge_cpad(N.h1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
                         xchi, xclo, st, off, n_off, sat_act(e)));
-  RET(tc_result(e, tc_conv_fwd(e->tcw, N.h1c_slot, xchi, xclo, n, 1, T, 1, 1, P, st), &N.h1.a, "forward (tap-lowered)"));
+  RET(tc_result(e, tc_conv_fwd(e->tcw.layers[N.h1c_slot], e->cfg.precision, e->tcw.debug, xchi, xclo, n, 1, T, 1, 1, P, st), &N.h1.a,
+                "forward (tap-lowered)"));
   CK(launch_post_fwd(q, e->opt.post, st));
   return 0;
 }
@@ -570,7 +599,8 @@ static int h1_edge_forward(cgvc_engine* e, const GenNet& N, const float* x, int 
 static int o1_edge_forward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16* uhi, const __nv_bfloat16* ulo, int n, int W,
                            const long long* off, int n_off, float* z, float* out, cudaStream_t st) {
   const int nf = e->cfg.num_features;
-  RET(tc_result(e, tc_conv_fwd(e->tcw, N.o1f_slot, uhi, ulo, n, 1, W, 1, 1, z, st), &N.o1.a, "forward (tap-lowered)"));
+  RET(tc_result(e, tc_conv_fwd(e->tcw.layers[N.o1f_slot], e->cfg.precision, e->tcw.debug, uhi, ulo, n, 1, W, 1, 1, z, st), &N.o1.a,
+                "forward (tap-lowered)"));
   CK(launch_col2im_taps(z, N.o1.a.kw * nf, (long long)n * W, W, nf, N.o1.a.kw, +1, e->P() + N.o1.a.b, out, st, off, n_off));
   return 0;
 }
@@ -589,32 +619,36 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
     return io;
   };
   auto of = [&](const GLAct& a, int W) { return at((keep_y || !a.Yhi) ? a.Y : nullptr, a.Yhi, a.Ylo, W); };   // a layer output as input
+  auto fwd = [&](const Layer& L, const ConvIO& in, const GLAct& a, int W, bool y, const float* resid = nullptr) {
+    return layer_forward(e, L, layer_tensors(e, L, false), in, a, W, y, save_pre, e->opt.fuse_in, A.post, st, resid);
+  };
   A.x_cl = x_cl;
   const bool edge = edge_on(e, N) && A.xchi && A.z;
   ConvIO io = at(x_cl, A.xhi, A.xlo, T);
   if (edge) {
     // h1 = dense [n*T, kw*F] x [kw*F, 2*128] GEMM on the im2col of the input
-    RET(h1_edge_forward(e, N, x_cl, n, T, A.off, A.n, A.xchi, A.xclo, A.h1.P, post_params(e, N.h1, io, A.h1, T, keep_y, A.post), st));
+    const PostParams q = post_params(e, N.h1, layer_tensors(e, N.h1, false), io, A.h1, T, keep_y, A.post);
+    RET(h1_edge_forward(e, N, x_cl, n, T, A.off, A.n, A.xchi, A.xclo, A.h1.P, q, st));
   } else {
     if (A.xhi && tc_enabled(e)) CK(tc_split_planes(e->cfg.precision, x_cl, (long long)n * T, nf, A.xhi, A.xlo, st, sat_act(e)));
-    RET(layer_forward(e, N.h1, io, A.h1, T, keep_y, save_pre, A.post, st));
+    RET(fwd(N.h1, io, A.h1, T, keep_y));
   }
   const GLAct* cur = &A.h1;
   int W = T;
   for (int i = 0; i < 2; ++i) {
     io = of(*cur, W);
     W /= 2;
-    RET(layer_forward(e, N.d[i], io, A.d[i], W, keep_y || i == 1, save_pre, A.post, st));   // d2's fp32 output is the first residual input
+    RET(fwd(N.d[i], io, A.d[i], W, keep_y || i == 1));   // d2's fp32 output is the first residual input
     cur = &A.d[i];
   }
   for (int i = 0; i < 6; ++i) {       // cur: the block input, whose fp32 copy is always written
-    RET(layer_forward(e, N.r[i].h1, at(cur->Y, cur->Yhi, cur->Ylo, W), A.r[i].h1, W, keep_y, save_pre, A.post, st));
-    RET(layer_forward(e, N.r[i].h2, of(A.r[i].h1, W), A.r[i].h2, W, true, save_pre, A.post, st, cur->Y));
+    RET(fwd(N.r[i].h1, at(cur->Y, cur->Yhi, cur->Ylo, W), A.r[i].h1, W, keep_y));
+    RET(fwd(N.r[i].h2, of(A.r[i].h1, W), A.r[i].h2, W, true, cur->Y));
     cur = &A.r[i].h2;
   }
   io = at(cur->Y, cur->Yhi, cur->Ylo, W);
   for (int i = 0; i < 2; ++i) {
-    RET(layer_forward(e, N.u[i], io, A.u[i], W, keep_y, save_pre, A.post, st));      // W = conv rows per sample; the shuffle doubles them
+    RET(fwd(N.u[i], io, A.u[i], W, keep_y));      // W = conv rows per sample; the shuffle doubles them
     W *= 2;
     io = of(A.u[i], W);
   }
@@ -622,7 +656,7 @@ static int generator_forward(cgvc_engine* e, const GenNet& N, GenActs& A, const 
     // o1: Z[m, (t, c)] = U[m, :] . W[t][:, c] as one dense GEMM, then out[m, c] = b[c] + sum_t Z[m + t - 7, (t, c)]
     RET(o1_edge_forward(e, N, io.xhi, io.xlo, n, W, A.off, A.n, A.z, A.out_cl, st));
   } else {
-    RET(conv_fwd(e, N.o1, io, A.out_cl, st));
+    RET(conv_fwd(e, N.o1, layer_tensors(e, N.o1, false), io, A.out_cl, st));
   }
   if (keep_y) {
     e->taps.clear();
@@ -691,75 +725,77 @@ static void side_join(const BwdScratch& S, cudaStream_t st) {
   for (int b = 0; b < 2; ++b) if (q->used[b]) { cudaStreamWaitEvent(st, q->done[b], 0); q->used[b] = false; }
 }
 
-// GLU / instance-norm backward of a layer into dP planes `out`; fp32 dP is only materialised when a SIMT kernel will read it
-static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const float* dy, const GLAct& A, int n, int rows_per_sample_out,
-                                     const BwdScratch& S, bool wgrad, bool need_fp32, PlanePair out) {
+// GLU / instance-norm backward of a layer into dP planes `out`, with the parameter gradients t holds; fp32 dP is only materialised when
+// a SIMT kernel will read it
+static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const LayerTensors& t, const float* dy, const GLAct& A, int n,
+                                     int rows_per_sample_out, const BwdScratch& S, bool need_fp32, PlanePair out) {
   PostBwdParams q; memset(&q, 0, sizeof q);
-  const float* Pm = e->P(); float* Gm = e->G();
   q.dy1 = dy; q.p = A.P; q.ldp = L.width(); q.Cc = L.a.cout; q.B = n; q.sh = L.shuffle;
   q.R = rows_per_sample_out * L.shuffle; q.C = L.a.cout / L.shuffle;
   q.has_in = L.has_in; q.has_gate = L.gated(); q.stats = A.stats;
-  if (L.has_in) {
-    q.beta_a = Pm + L.ina.beta; q.gamma_a = Pm + L.ina.gamma;
-    if (wgrad) { q.dbeta_a = Gm + L.ina.beta; q.dgamma_a = Gm + L.ina.gamma; }
-  }
-  if (L.has_in && L.gated()) {
-    q.beta_g = Pm + L.ing.beta; q.gamma_g = Pm + L.ing.gamma;
-    if (wgrad) { q.dbeta_g = Gm + L.ing.beta; q.dgamma_g = Gm + L.ing.gamma; }
-  }
-  if (wgrad) { q.dbias_a = Gm + L.a.b; if (L.gated()) q.dbias_g = Gm + L.g.b; }
+  q.beta_a = t.beta_a; q.gamma_a = t.gamma_a; q.beta_g = t.beta_g; q.gamma_g = t.gamma_g;
+  q.dbeta_a = t.dbeta_a; q.dgamma_a = t.dgamma_a; q.dbeta_g = t.dbeta_g; q.dgamma_g = t.dgamma_g;
+  q.dbias_a = t.dba; q.dbias_g = t.dbg;
   q.scratch = S.post;
-  const bool tc = use_tc(e, L.tc_slot) && S.dPhi;
+  const bool tc = t.tc && S.dPhi;
   q.dp = (!tc || need_fp32) ? S.dP : nullptr;
   if (tc) { q.dp_hi = out.hi; q.dp_lo = out.lo; }
-  q.qmode = e->cfg.precision == CGVC_PREC_F16F8;
+  q.qmode = t.precision == CGVC_PREC_F16F8;
   q.sat = sat_grad(e); q.ufl = ufl_grad(e);
-  if (wgrad) q.det = S.det;                 // passes without parameter gradients keep the faster (equally deterministic) forms
+  if (t.dba || t.dbeta_a) q.det = S.det;    // passes without parameter gradients keep the faster (equally deterministic) forms
   return q;
 }
 
 // the fused backward epilogue (tc_conv_dgrad) of L's instance norm (+ GLU; no pixel shuffle), writing its dP planes into `out`
-static TcBwdFuse bwd_fuse(const cgvc_engine* e, const Layer& L, const GLAct& A, int rows_per_sample, PlanePair out) {
+static TcBwdFuse bwd_fuse(const Layer& L, const LayerTensors& t, const GLAct& A, int rows_per_sample, PlanePair out) {
   TcBwdFuse f; memset(&f, 0, sizeof f);
-  const float* Pm = e->P(); float* Gm = e->G();
   f.R = (L.has_in && L.shuffle == 1) ? rows_per_sample : 0;      // R = 0: not fusable
   f.gated = L.gated(); f.bp = A.P; f.bp_ld = L.width(); f.stats = A.stats;
-  f.gamma_a = Pm + L.ina.gamma; f.beta_a = Pm + L.ina.beta;
+  f.gamma_a = t.gamma_a; f.beta_a = t.beta_a; f.gamma_g = t.gamma_g; f.beta_g = t.beta_g;
   f.dp_hi = out.hi; f.dp_lo = out.lo; f.dp_ld = L.width();
-  f.dgamma_a = Gm + L.ina.gamma; f.dbeta_a = Gm + L.ina.beta;
-  if (L.gated()) { f.gamma_g = Pm + L.ing.gamma; f.beta_g = Pm + L.ing.beta; f.dgamma_g = Gm + L.ing.gamma; f.dbeta_g = Gm + L.ing.beta; }
+  f.dgamma_a = t.dgamma_a; f.dbeta_a = t.dbeta_a; f.dgamma_g = t.dgamma_g; f.dbeta_g = t.dbeta_g;
   return f;
 }
 
 // dP of a layer: the GLU / instance-norm backward kernel, unless the previous data-gradient launch's fused epilogue wrote it
-static int layer_dp(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAct& A, const float* dy, int n, int rows_per_sample_out,
-                    bool wgrad, cudaStream_t st, PostBwdParams& q) {
+static int layer_dp(cgvc_engine* e, BwdWalk& w, const Layer& L, const LayerTensors& t, const GLAct& A, const float* dy, int n,
+                    int rows_per_sample_out, cudaStream_t st, PostBwdParams& q) {
   bool written = false;
   const PlanePair out = dp_planes(w, st, &written);
-  q = post_bwd_params(e, L, dy, A, n, rows_per_sample_out, w.S, wgrad, false, out);
+  q = post_bwd_params(e, L, t, dy, A, n, rows_per_sample_out, w.S, false, out);
   if (!written) CK(launch_post_bwd(q, e->opt.post, st));
   return 0;
 }
 
-// Backward through one layer, whose input was `in` and upstream gradient is dy: (1) dP (layer_dp); (2) with wgrad, the weight
-// gradient (run_wgrad); (3) dx (+)= the data gradient (dx null: none), with the instance-norm backward of `up` -- the layer whose
-// output is `in`, activations upA -- fused into its epilogue under fuse_bwd where the shape allows
-static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAct& A, const ConvIO& in, const float* dy,
-                          int rows_per_sample_out, bool wgrad, float* dx, int accumulate, cudaStream_t st,
-                          const Layer* up = nullptr, const GLAct* upA = nullptr) {
-  PostBwdParams q;
-  RET(layer_dp(e, w, L, A, dy, in.n, rows_per_sample_out, wgrad, st, q));
-  const PlanePair dp{q.dp_hi, q.dp_lo};
-  if (wgrad) RET(run_wgrad(w.S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, L, in, q.dp, dp, ws, det_of(w.S)); }));
-  if (!dx) return 0;
+// dx (+)= the data gradient of L from its dP (fp32 dP, planes dp), with the instance-norm backward of `up` (tensors ut, activations upA)
+// -- the layer whose output was L's input -- fused into its epilogue under w.fuse where the shape allows; the fused epilogue writes up's
+// dP planes into the walk's other plane pair, which up's layer_dp then takes without a launch
+static int layer_dx(cgvc_engine* e, BwdWalk& w, const Layer& L, const LayerTensors& t, const ConvIO& in, const float* dP, PlanePair dp,
+                    float* dx, int accumulate, cudaStream_t st, const Layer* up, const LayerTensors* ut, const GLAct* upA) {
   const int other = 1 - w.cur;
   TcBwdFuse f;
   const bool fuse = up && w.fuse && dp.hi;
-  if (fuse) f = bwd_fuse(e, *up, *upA, in.W, w.pb[other]);
+  if (fuse) f = bwd_fuse(*up, *ut, *upA, in.W, w.pb[other]);
   bool fused = false;
-  RET(conv_dgrad(e, L, in, q.dp, dp, dx, accumulate, st, fuse ? &f : nullptr, &fused));
+  RET(conv_dgrad(e, L, t, in, dP, dp, dx, accumulate, st, fuse ? &f : nullptr, &fused));
   if (fused) w.have = other;
   return 0;
+}
+
+// Backward through one layer, whose input was `in` and upstream gradient is dy: (1) dP (layer_dp); (2) with wgrad, the weight
+// gradient (run_wgrad); (3) with dx, layer_dx (up, upA: the layer whose output is `in` and its activations)
+static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAct& A, const ConvIO& in, const float* dy,
+                          int rows_per_sample_out, bool wgrad, float* dx, int accumulate, cudaStream_t st,
+                          const Layer* up = nullptr, const GLAct* upA = nullptr) {
+  const LayerTensors t = layer_tensors(e, L, wgrad);
+  PostBwdParams q;
+  RET(layer_dp(e, w, L, t, A, dy, in.n, rows_per_sample_out, st, q));
+  const PlanePair dp{q.dp_hi, q.dp_lo};
+  if (wgrad) RET(run_wgrad(w.S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, L, t, in, q.dp, dp, ws, det_of(w.S)); }));
+  if (!dx) return 0;
+  LayerTensors ut{};
+  if (up) ut = layer_tensors(e, *up, wgrad);
+  return layer_dx(e, w, L, t, in, q.dp, dp, dx, accumulate, st, up, &ut, upA);
 }
 
 // The tap-lowered edge layers' backward (see h1_edge_forward), n samples of T rows.
@@ -769,12 +805,15 @@ static int o1_edge_backward(cgvc_engine* e, const GenNet& N, const float* d_out,
                             int T, PlanePair dz, float* du, const BwdScratch& S, cudaStream_t st) {
   const int nf = e->cfg.num_features;
   float* Gm = e->G();
+  const TcLayer& O = e->tcw.layers[N.o1f_slot];
   CK(launch_im2col_taps(d_out, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
                         dz.hi, dz.lo, st, nullptr, 0, sat_grad(e), ufl_grad(e)));
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-    return tc_result(e, tc_conv_wgrad(e->tcw, N.o1f_slot, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws, det_of(S)),
+    return tc_result(e, tc_conv_wgrad(O, e->cfg.precision, e->tcw.wgrad16, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws,
+                                      det_of(S)),
                      &N.o1.a, "weight gradient (tap-lowered)"); }));
-  RET(tc_result(e, tc_conv_dgrad(e->tcw, N.o1f_slot, dz.hi, dz.lo, n, 1, T, 1, 1, du, 0, st), &N.o1.a, "data gradient (tap-lowered)"));
+  RET(tc_result(e, tc_conv_dgrad(O, e->cfg.precision, e->tcw.debug, dz.hi, dz.lo, n, 1, T, 1, 1, du, 0, st), &N.o1.a,
+                "data gradient (tap-lowered)"));
   return 0;
 }
 
@@ -785,11 +824,13 @@ static int h1_edge_backward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16
                             int T, float* dz, float* dx, const BwdScratch& S, cudaStream_t st) {
   const int nf = e->cfg.num_features;
   float* Gm = e->G();
+  const TcLayer& H = e->tcw.layers[N.h1c_slot];
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-    return tc_result(e, tc_conv_wgrad(e->tcw, N.h1c_slot, xchi, xclo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.h1.a.k, Gm + N.h1.g.k, ws,
-                                      det_of(S)),
+    return tc_result(e, tc_conv_wgrad(H, e->cfg.precision, e->tcw.wgrad16, xchi, xclo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.h1.a.k,
+                                      Gm + N.h1.g.k, ws, det_of(S)),
                      &N.h1.a, "weight gradient (tap-lowered)"); }));
-  if (dz) RET(tc_result(e, tc_conv_dgrad(e->tcw, N.h1c_slot, dp.hi, dp.lo, n, 1, T, 1, 1, dz, 0, st), &N.h1.a, "data gradient (tap-lowered)"));
+  if (dz) RET(tc_result(e, tc_conv_dgrad(H, e->cfg.precision, e->tcw.debug, dp.hi, dp.lo, n, 1, T, 1, 1, dz, 0, st), &N.h1.a,
+                        "data gradient (tap-lowered)"));
   if (dz && dx) CK(launch_col2im_taps(dz, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, dx, st));
   return 0;
 }
@@ -815,13 +856,14 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
     // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
     RET(o1_edge_backward(e, N, d_out_cl, u2.xhi, u2.xlo, n, T, dp_planes(w, st), S.bufA, S, st));
   } else {
+    const LayerTensors t = layer_tensors(e, N.o1, true);
     PlanePair dp{nullptr, nullptr};
-    if (use_tc(e, N.o1.tc_slot) && u2.xhi && S.dPhi) {
+    if (t.tc && u2.xhi && S.dPhi) {
       dp = dp_planes(w, st);
       CK(tc_split_planes(e->cfg.precision, d_out_cl, (long long)n * T, nf, dp.hi, dp.lo, st, sat_grad(e), ufl_grad(e)));
     }
-    RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, u2, d_out_cl, dp, ws, det_of(S)); }));
-    RET(conv_dgrad(e, N.o1, u2, d_out_cl, dp, S.bufA, 0, st));
+    RET(run_wgrad(S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, N.o1, t, u2, d_out_cl, dp, ws, det_of(S)); }));
+    RET(conv_dgrad(e, N.o1, t, u2, d_out_cl, dp, S.bufA, 0, st));
   }
   float* cur = S.bufA; float* oth = S.bufB;
   // up-sampling blocks, convolutions at T/2 and T/4 (the shuffle doubles the rows).  u1's data gradient is d loss / d (residual block
@@ -850,7 +892,7 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   // tap-lowered h1: the weight gradient is im2col(x)^T dP straight into the [15,24,128] kernels' GRAD ranges; the data gradient
   // (cycle passes only) is the dense dP . W^T [n*T, kw*F] followed by the tap-shifted sum
   PostBwdParams q;
-  RET(layer_dp(e, w, N.h1, A.h1, cur, n, T, true, st, q));
+  RET(layer_dp(e, w, N.h1, layer_tensors(e, N.h1, true), A.h1, cur, n, T, st, q));
   return h1_edge_backward(e, N, A.xchi, A.xclo, PlanePair{q.dp_hi, q.dp_lo}, n, T, d_in_cl ? oth : nullptr, d_in_cl, S, st);
 }
 
@@ -867,45 +909,39 @@ static void plan_discriminator(cgvc_engine* e, Bump& ws, DiscActs& A, int n, int
   A.prob = ws.take<float>((size_t)r3);
 }
 
-// The discriminator's input layer (one input channel, <= 9 taps, gate without instance norm: module.py:196-203), its weights and
-// gradients by pointer, so that the walk and the test entry points (cgvc_disc_input_forward / _backward) run the same launches.
-struct C1Layer { const float *wa, *wg, *ba, *bg; int kh, kw, cout, sh, sw; };
-struct C1Grads { float *dwa, *dwg, *dba, *dbg; };      // all null: no weight gradient
-static C1Layer c1_layer(const cgvc_engine* e, const Layer& L) {
-  const float* Pm = e->P();
-  return C1Layer{Pm + L.a.k, Pm + L.g.k, Pm + L.a.b, Pm + L.g.b, L.a.kh, L.a.kw, L.a.cout, L.sh, L.sw};
-}
-
+// The discriminator's input layer L (one input channel, <= 9 taps, gate without instance norm: module.py:196-203), its tensors t by
+// pointer, so that the walk and the test entry points (cgvc_disc_input_forward / _backward) run the same launches.
 // P [n * Ho * Wo, 2 cout] = [a | g] = conv(x [n, H, W]) + bias, and the GLU that q describes (q.p = P: y, its planes and their count).
 // fuse: convolution + GLU in one HBM-bound pass (P is written for the backward pass but not read back); else the convolution, then the
 // GLU-only post kernels
-static int disc_input_forward(cgvc_engine* e, const C1Layer& c, const float* x, int n, int H, int W, float* P, const PostParams& q, bool fuse,
-                              cudaStream_t st) {
-  const GatherGeom g = fwd_geom(n, H, W, c.kh, c.kw, c.sh, c.sw);
+static int disc_input_forward(cgvc_engine* e, const Layer& L, const LayerTensors& t, const float* x, int n, int H, int W, float* P,
+                              const PostParams& q, bool fuse, cudaStream_t st) {
+  const GatherGeom g = fwd_geom(n, H, W, L.a.kh, L.a.kw, L.sh, L.sw);
   if (fuse) {
-    CK(launch_conv_c1_glu_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat, q.ufl));
+    CK(launch_conv_c1_glu_fwd(g, x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat, q.ufl));
     return 0;
   }
-  CK(launch_conv_c1_fwd(g, x, c.wa, c.wg, c.ba, c.bg, c.cout, P, st));
+  CK(launch_conv_c1_fwd(g, x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, st));
   CK(launch_post_fwd(q, e->opt.post, st));
   return 0;
 }
 
-// Backward of the same layer from dy [n * Ho * Wo, cout] and the saved P: d's weight and bias gradients += (d.dwa null: none), dx [n, H, W]
+// Backward of the same layer from dy [n * Ho * Wo, cout] and the saved P: t's weight and bias gradients += (t.dka null: none), dx [n, H, W]
 // = the data gradient (null: none), Z scratch [n * Ho * Wo, taps].  fuse: dP = (dy s(g), dy a s(g) (1 - s(g))) formed in registers inside
 // the weight-gradient and data-gradient kernels; else the GLU-only backward q (bias gradients included) writes the fp32 dP q.dp, which
 // wgrad_c1 and dgrad_c1 read.  det: deterministic mode's partials slab, else null
-static int disc_input_backward(cgvc_engine* e, const C1Layer& c, const C1Grads& d, const float* x, const float* dy, const float* P, int n, int H,
-                               int W, float* dx, float* Z, bool fuse, const PostBwdParams& q, const DetSlab* det, cudaStream_t st) {
-  const GatherGeom g = fwd_geom(n, H, W, c.kh, c.kw, c.sh, c.sw);
+static int disc_input_backward(cgvc_engine* e, const Layer& L, const LayerTensors& t, const float* x, const float* dy, const float* P, int n,
+                               int H, int W, float* dx, float* Z, bool fuse, const PostBwdParams& q, const DetSlab* det, cudaStream_t st) {
+  const int kh = L.a.kh, kw = L.a.kw, cout = L.a.cout;
+  const GatherGeom g = fwd_geom(n, H, W, kh, kw, L.sh, L.sw);
   if (fuse) {
-    if (d.dwa) CK(launch_glu_bwd_wgrad_c1(g, x, dy, P, c.cout, d.dwa, d.dwg, d.dba, d.dbg, st, det));
-    if (dx) CK(launch_glu_bwd_dgrad_c1(dy, P, c.cout, c.wa, c.wg, Z, dx, n, H, W, c.kh, c.kw, c.sh, c.sw, st));
+    if (t.dka) CK(launch_glu_bwd_wgrad_c1(g, x, dy, P, cout, t.dka, t.dkg, t.dba, t.dbg, st, det));
+    if (dx) CK(launch_glu_bwd_dgrad_c1(dy, P, cout, t.ka, t.kg, Z, dx, n, H, W, kh, kw, L.sh, L.sw, st));
     return 0;
   }
   CK(launch_post_bwd(q, e->opt.post, st));
-  if (d.dwa) CK(launch_wgrad_c1(g, x, q.dp, 2 * c.cout, 2 * c.cout, d.dwa, d.dwg, c.cout, nullptr, nullptr, st, det));
-  if (dx) CK(launch_dgrad_c1(q.dp, 2 * c.cout, c.wa, c.wg, c.cout, Z, dx, n, H, W, c.kh, c.kw, c.sh, c.sw, st));
+  if (t.dka) CK(launch_wgrad_c1(g, x, q.dp, 2 * cout, 2 * cout, t.dka, t.dkg, cout, nullptr, nullptr, st, det));
+  if (dx) CK(launch_dgrad_c1(q.dp, 2 * cout, t.ka, t.kg, cout, Z, dx, n, H, W, kh, kw, L.sh, L.sw, st));
   return 0;
 }
 
@@ -921,12 +957,14 @@ static int discriminator_forward(cgvc_engine* e, const DiscNet& N, DiscActs& A, 
   ConvIO io; io.x = x; io.xhi = nullptr; io.xlo = nullptr; io.n = n; io.H = H0; io.W = T;
   int H = H0, W = T / 2;
   // input layer: one input channel, K = 9, gate without norm; P is kept for the backward pass
-  RET(disc_input_forward(e, c1_layer(e, N.h1), x, n, H0, T, A.h1.P, post_params(e, N.h1, io, A.h1, H * W, keep_y, A.post), c1_fused(e, N.h1), st));
+  const LayerTensors t1 = layer_tensors(e, N.h1, false);
+  RET(disc_input_forward(e, N.h1, t1, x, n, H0, T, A.h1.P, post_params(e, N.h1, t1, io, A.h1, H * W, keep_y, A.post), c1_fused(e, N.h1), st));
   const GLAct* cur = &A.h1;
   for (int i = 0; i < 3; ++i) {
     io.x = (keep_y || !cur->Yhi) ? cur->Y : nullptr; io.xhi = cur->Yhi; io.xlo = cur->Ylo; io.H = H; io.W = W;
     int Ho, Wo; conv_out_dims(N.d[i].a, N.d[i].sh, N.d[i].sw, H, W, Ho, Wo); H = Ho; W = Wo;
-    RET(layer_forward(e, N.d[i], io, A.d[i], H * W, keep_y, true, A.post, st));     // d3 has no planes: its fp32 output feeds the head
+    // d3 has no planes: its fp32 output feeds the head
+    RET(layer_forward(e, N.d[i], layer_tensors(e, N.d[i], false), io, A.d[i], H * W, keep_y, true, e->opt.fuse_in, A.post, st));
     cur = &A.d[i];
   }
   CK(launch_head_fwd(cur->Y, (long long)n * H * W, 1024, Pm + N.dense_k, Pm + N.dense_b, A.prob, st));
@@ -977,10 +1015,9 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   }
   // h1: one input channel (K = 9), gate without instance norm.  Fused form: the GLU backward is recomputed inside the weight-gradient /
   // data-gradient kernels, dP never goes to HBM.  D.h1 has no tensor-core slot, so the unfused form's dP is fp32 (no planes)
-  float* Gm = e->G();
-  const C1Grads d = wgrad ? C1Grads{Gm + N.h1.a.k, Gm + N.h1.g.k, Gm + N.h1.a.b, Gm + N.h1.g.b} : C1Grads{nullptr, nullptr, nullptr, nullptr};
-  const PostBwdParams q = post_bwd_params(e, N.h1, dy, A.h1, n, Hs[0] * Ws[0], S, wgrad, true, PlanePair{S.dPhi, S.dPlo});
-  return disc_input_backward(e, c1_layer(e, N.h1), d, A.x, dy, A.h1.P, n, H0, T, d_in, bufs[flip], c1_fused(e, N.h1), q, det_of(S), st);
+  const LayerTensors t = layer_tensors(e, N.h1, wgrad);
+  const PostBwdParams q = post_bwd_params(e, N.h1, t, dy, A.h1, n, Hs[0] * Ws[0], S, true, PlanePair{S.dPhi, S.dPlo});
+  return disc_input_backward(e, N.h1, t, A.x, dy, A.h1.P, n, H0, T, d_in, bufs[flip], c1_fused(e, N.h1), q, det_of(S), st);
 }
 
 // ---- workspace sizing ---------------------------------------------------------------------------------------
@@ -1928,20 +1965,77 @@ int cgvc_gather_minibatch(cgvc_handle e, const float* corpus_A_dev, const long l
   return 0;
 }
 
+}  // extern "C"
+
 // ---- per-kernel entry points ---------------------------------------------------------------------------------
+// the entry points' scratch, carved from the per-engine buffer: carve(ws) runs once on a null base to size it, then on the buffer
+template <class F> static cudaError_t entry_scratch(cgvc_engine* e, F&& carve) {
+  Bump ws; ws.reset(nullptr, 0);
+  carve(ws);
+  float* buf;
+  cudaError_t ce = grow_post_buf(e, ws.off / sizeof(float) + 1, &buf);
+  if (ce != cudaSuccess) return ce;
+  ws.reset(buf, e->post_elems * sizeof(float));
+  carve(ws);
+  return cudaSuccess;
+}
+
+// room for the operand planes of `rows` rows of c channels in any precision: bf16 hi / lo [rows, ru64(c)], F16F8 fp16 + two e4m3 [rows, ru128(c)]
+static void take_planes(Bump& ws, long long rows, int c, __nv_bfloat16** hi, __nv_bfloat16** lo) {
+  const size_t n = (size_t)rows * edge_cpad(c);
+  *hi = ws.take<__nv_bfloat16>(n); *lo = ws.take<__nv_bfloat16>(n);
+}
+
+// One convolution layer in the engine's own description for the convolution entry points, whose tensors they take by pointer
+// (a.k = b = -1: no PARAM tensor, which tc_result would name)
+static Layer conv_layer(int kh, int kw, int cin, int cout, bool gated, int sh, int sw, int shuffle = 1) {
+  Layer L{}; L.a = ConvW{(size_t)-1, (size_t)-1, kh, kw, cin, cout}; if (gated) L.g = L.a;
+  L.sh = sh; L.sw = sw; L.shuffle = shuffle;
+  return L;
+}
+
+// The tensor-core planes of such a layer in t.precision: a one-layer store, refreshed from t's weights (null biases read as the zeros
+// `zero` [cout] is set to) on st, which the call synchronises before the store is freed.  Sets t.tc and the store options
+struct EntryStore {
+  TcWeights w;
+  ~EntryStore() { tc_free(w); }
+};
+static int entry_store(cgvc_engine* e, EntryStore& S, const Layer& L, LayerTensors& t, float* zero, cudaStream_t st) {
+  tc_register(S.w, 0, 0, 0, 0, L.a.kh, L.a.kw, L.a.cin, L.a.cout, L.gated(), L.shuffle);
+  int r = tc_alloc(S.w, t.precision, true);
+  if (r != 0) return fail(e, CGVC_ERR_CUDA, "tc_alloc: %s", cudaGetErrorString((cudaError_t)r));
+  CK(cudaStreamSynchronize(nullptr));                   // tc_alloc zeroes the planes' padding on the legacy stream
+  if (!t.ba || (L.gated() && !t.bg)) CK(cudaMemsetAsync(zero, 0, L.a.cout * sizeof(float), st));
+  TcLayer& T = S.w.layers[0];
+  r = tc_refresh_layer(T, t.ka, t.kg, t.ba ? t.ba : zero, t.bg ? t.bg : zero, st);
+  if (r != 0) return fail(e, CGVC_ERR_CUDA, "tc_refresh_layer: %s", cudaGetErrorString((cudaError_t)r));
+  t.tc = &T; t.debug = e->tcw.debug; t.wgrad16 = e->tcw.wgrad16;
+  return 0;
+}
+
+extern "C" {
+
 int cgvc_conv_forward(cgvc_handle e, int precision, const float* x, const float* w, const float* bias, float* y,
                       int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, void* stream) {
   if (!e || !x || !w || !y) return fail(e, CGVC_ERR_ARG, "null argument");
   if (kh * kw > CGVC_MAX_TAPS) return fail(e, CGVC_ERR_UNSUPPORTED, "at most %d filter taps", CGVC_MAX_TAPS);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision != CGVC_PREC_FP32_SIMT)
-    return tc_result(e, tc_conv_fwd_adhoc(precision, e->tcw.debug, x, w, bias, y, B, H, W, Cin, kh, kw, Cout, sh, sw, st), nullptr, "conv forward");
-  GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
-  GemmOperands op; memset(&op, 0, sizeof op);
-  op.src = x; op.s_ld = Cin; op.C = Cin; op.w = w; op.w_ts = (long long)Cin * Cout; op.w_cs = Cout; op.w_ns = 1; op.N = Cout;
-  op.dst = y; op.d_ld = Cout; op.bias = bias;
-  CK(launch_gg_simt(g, op, st));
+  const Layer L = conv_layer(kh, kw, Cin, Cout, false, sh, sw);
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.ka = w; t.ba = bias; t.precision = precision;
+  ConvIO io{}; io.x = x; io.n = B; io.H = H; io.W = W;
+  if (precision == CGVC_PREC_FP32_SIMT) return conv_fwd(e, L, t, io, y, st);
+  // the tensor-core path reads x through its planes only (as a train step does), so that a shape it refuses is CGVC_ERR_UNSUPPORTED
+  float* zero;
+  __nv_bfloat16 *xhi, *xlo;
+  CK(entry_scratch(e, [&](Bump& ws) { take_planes(ws, (long long)B * H * W, Cin, &xhi, &xlo); zero = ws.take<float>(Cout); }));
+  EntryStore S;
+  RET(entry_store(e, S, L, t, zero, st));
+  CK(tc_split_planes(precision, x, (long long)B * H * W, Cin, xhi, xlo, st));
+  io.x = nullptr; io.xhi = xhi; io.xlo = xlo;
+  RET(conv_fwd(e, L, t, io, y, st));
+  CK(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -1953,16 +2047,32 @@ int cgvc_conv_backward(cgvc_handle e, int precision, const float* x, const float
   RET(plan_entry_det(e, &slab, &det));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision != CGVC_PREC_FP32_SIMT)
-    return tc_result(e, tc_conv_bwd_adhoc(precision, e->tcw.debug, x, w, dy, dx, dw, dbias, B, H, W, Cin, kh, kw, Cout, sh, sw, st, e->tcw.wgrad16, det),
-                     nullptr, "conv backward");
-  ConvW c; c.k = 0; c.b = 0; c.kh = kh; c.kw = kw; c.cin = Cin; c.cout = Cout;
-  if (dx) RET(conv_dgrad_simt(e, w, c, sh, sw, B, H, W, dy, Cout, 0, dx, 0, st));
-  if (dw) {
-    GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
-    CK(launch_wgrad_simt(g, x, Cin, 0, Cin, dy, Cout, 0, Cout, dw, (long long)Cin * Cout, Cout, 1, st, det != nullptr));
-    if (dbias) CK(launch_colsum(dy, (long long)g.B * g.Hy * g.Wx, Cout, 0, Cout, dbias, st, det));
+  const Layer L = conv_layer(kh, kw, Cin, Cout, false, sh, sw);
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.ka = w; t.dka = dw; t.precision = precision;
+  ConvIO io{}; io.x = x; io.n = B; io.H = H; io.W = W;
+  const GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
+  const long long rows = (long long)B * H * W, orows = (long long)g.B * g.Hy * g.Wx;
+  const float* dP = dy;
+  PlanePair dp{nullptr, nullptr};
+  EntryStore S;
+  if (precision != CGVC_PREC_FP32_SIMT) {                // planes only, as in cgvc_conv_forward
+    __nv_bfloat16 *xhi, *xlo;
+    float* zero;
+    CK(entry_scratch(e, [&](Bump& ws) {
+      take_planes(ws, rows, Cin, &xhi, &xlo); take_planes(ws, orows, Cout, &dp.hi, &dp.lo); zero = ws.take<float>(Cout);
+    }));
+    RET(entry_store(e, S, L, t, zero, st));
+    CK(tc_split_planes(precision, x, rows, Cin, xhi, xlo, st));
+    CK(tc_split_planes(precision, dy, orows, Cout, dp.hi, dp.lo, st));
+    io.x = nullptr; io.xhi = xhi; io.xlo = xlo; dP = nullptr;
   }
+  if (dx) RET(conv_dgrad(e, L, t, io, dP, dp, dx, 0, st));
+  if (dw) {
+    RET(conv_wgrad(e, L, t, io, dP, dp, st, det));
+    if (dbias) CK(launch_colsum(dy, orows, Cout, 0, Cout, dbias, st, det));
+  }
+  if (precision != CGVC_PREC_FP32_SIMT) CK(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -2019,9 +2129,10 @@ static int in_glu_forward(cgvc_engine* e, const float* p, const float* beta_a, c
   ConvIO io{}; io.n = B;
   if (offsets) { io.n = io.H = 1; io.W = R / shuffle; io.pk = PackGeom{offsets, n_utt, div, max_len}; }
   const GLAct A{const_cast<float*>(p), stats, y, nullptr, nullptr};
-  PostParams q = post_params(e, in_layer(C, gate, shuffle), io, A, R / shuffle, true, nullptr, resid);
-  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = gate ? beta_g : nullptr; q.gamma_g = gate ? gamma_g : nullptr;
-  q.qmode = 0; q.sat = q.ufl = nullptr;
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.beta_a = beta_a; t.gamma_a = gamma_a; t.beta_g = gate ? beta_g : nullptr; t.gamma_g = gate ? gamma_g : nullptr;
+  PostParams q = post_params(e, in_layer(C, gate, shuffle), t, io, A, R / shuffle, true, nullptr, resid);
+  q.sat = q.ufl = nullptr;
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.y_hi = (__nv_bfloat16*)hi; q.y_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
     q.ufl = q.qmode ? e->plane_ufl : nullptr;
@@ -2047,12 +2158,13 @@ static int in_glu_backward(cgvc_engine* e, const float* dy, const float* p, cons
   const GLAct A{const_cast<float*>(p), const_cast<float*>(stats), nullptr, nullptr, nullptr};
   BwdScratch S; memset(&S, 0, sizeof S); S.dP = dp;
   if (det) S.det = *det;
-  PostBwdParams q = post_bwd_params(e, in_layer(C, gate, shuffle), dy, A, B, R / shuffle, S, false, true, PlanePair{nullptr, nullptr});
-  q.beta_a = beta_a; q.gamma_a = gamma_a; q.beta_g = gate ? beta_g : nullptr; q.gamma_g = gate ? gamma_g : nullptr;
-  q.dbeta_a = dbeta_a; q.dgamma_a = dgamma_a; q.dbeta_g = gate ? dbeta_g : nullptr; q.dgamma_g = gate ? dgamma_g : nullptr;
-  q.dbias_a = dbias_a; q.dbias_g = gate ? dbias_g : nullptr;
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.beta_a = beta_a; t.gamma_a = gamma_a; t.beta_g = gate ? beta_g : nullptr; t.gamma_g = gate ? gamma_g : nullptr;
+  t.dbeta_a = dbeta_a; t.dgamma_a = dgamma_a; t.dbeta_g = gate ? dbeta_g : nullptr; t.dgamma_g = gate ? dgamma_g : nullptr;
+  t.dba = dbias_a; t.dbg = gate ? dbias_g : nullptr;
+  PostBwdParams q = post_bwd_params(e, in_layer(C, gate, shuffle), t, dy, A, B, R / shuffle, S, true, PlanePair{nullptr, nullptr});
   if (det) q.det = *det;
-  q.qmode = 0; q.sat = q.ufl = nullptr;
+  q.sat = q.ufl = nullptr;
   if (precision != CGVC_PREC_FP32_SIMT) {
     q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo; q.qmode = precision == CGVC_PREC_F16F8; q.sat = q.qmode ? sat : nullptr;
     q.ufl = q.qmode ? e->plane_ufl : nullptr;
@@ -2076,11 +2188,30 @@ int cgvc_conv_in_forward(cgvc_handle e, int precision, const float* x, const flo
   if (B < 1 || W < 1 || Cin < 1 || kw < 1 || kw > CGVC_MAX_TAPS || sw < 1 || (shuffle != 1 && shuffle != 2) || Cout % (32 * shuffle))
     return fail(e, CGVC_ERR_ARG, "cgvc_conv_in_forward: bad shape (B %d, W %d, Cin %d, kw %d, Cout %d, sw %d, shuffle %d)", B, W, Cin, kw, Cout, sw, shuffle);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  TcFuse f; memset(&f, 0, sizeof f);
-  f.gamma_a = gamma_a; f.beta_a = beta_a; f.gamma_g = gamma_g; f.beta_g = beta_g;
-  f.stats = stats; f.resid = resid; f.y = y; f.y_hi = (__nv_bfloat16*)hi; f.y_lo = (__nv_bfloat16*)lo;
-  return tc_result(e, tc_conv_in_fwd_adhoc(precision, e->tcw.debug, e->opt.post, x, w_a, w_g, b_a, b_g, f, p, B, W, Cin, kw, Cout, sw, shuffle, fuse, fused, (cudaStream_t)stream),
-                   nullptr, "conv + instance norm forward");
+  cudaStream_t st = (cudaStream_t)stream;
+  Layer L = conv_layer(1, kw, Cin, Cout, gated, 1, sw, shuffle);
+  L.has_in = 1;
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.ka = w_a; t.kg = w_g; t.ba = b_a; t.bg = b_g; t.beta_a = beta_a; t.gamma_a = gamma_a; t.precision = precision;
+  if (gated) { t.beta_g = beta_g; t.gamma_g = gamma_g; }
+  // p and stats may be null: the inference form (neither) runs as a conversion does, with scratch for the fallback's intermediates
+  const int Wo = (W + sw - 1) / sw, C = Cout / shuffle;
+  __nv_bfloat16 *xhi, *xlo;
+  float *ps, *ss, *post;
+  CK(entry_scratch(e, [&](Bump& ws) {
+    take_planes(ws, (long long)B * W, Cin, &xhi, &xlo);
+    ps = ws.take<float>((size_t)B * Wo * L.width()); ss = ws.take<float>((size_t)B * 4 * C); post = ws.take<float>((size_t)B * 4 * C);
+  }));
+  EntryStore S;
+  RET(entry_store(e, S, L, t, nullptr, st));
+  CK(tc_split_planes(precision, x, (long long)B * W, Cin, xhi, xlo, st));
+  ConvIO io{}; io.xhi = xhi; io.xlo = xlo; io.n = B; io.H = 1; io.W = W;
+  const GLAct A{p ? p : ps, stats ? stats : ss, y, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo};
+  bool f = false;
+  RET(layer_forward(e, L, t, io, A, Wo, true, p || stats, fuse != 0, post, st, resid, &f));
+  CK(cudaStreamSynchronize(st));
+  if (fused) *fused = f;
+  return 0;
 }
 
 int cgvc_conv_in_backward(cgvc_handle e, int precision, const float* dp, const float* w_a, const float* w_g, const float* bp, const float* stats,
@@ -2100,13 +2231,42 @@ int cgvc_conv_in_backward(cgvc_handle e, int precision, const float* dp, const f
   DetSlab slab; const DetSlab* det;
   RET(plan_entry_det(e, &slab, &det));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  TcBwdFuse f; memset(&f, 0, sizeof f);
-  f.gated = gate != 0; f.bp = bp; f.stats = stats;
-  f.gamma_a = gamma_a; f.beta_a = beta_a; f.gamma_g = gamma_g; f.beta_g = beta_g;
-  f.dp_hi = (__nv_bfloat16*)hi; f.dp_lo = (__nv_bfloat16*)lo;
-  f.dbeta_a = dbeta_a; f.dgamma_a = dgamma_a; f.dbeta_g = dbeta_g; f.dgamma_g = dgamma_g;
-  return tc_result(e, tc_conv_in_bwd_adhoc(precision, e->tcw.debug, e->opt.post, dp, w_a, w_g, f, dx, accumulate, B, R, Cin, kw, Cout, fuse, fused, det, (cudaStream_t)stream),
-                   nullptr, "conv data gradient + instance norm backward");
+  cudaStream_t st = (cudaStream_t)stream;
+  // L: the stride-1 layer whose data gradient this is; U: the upstream layer whose output L read, whose dP planes are hi / lo
+  const Layer L = conv_layer(1, kw, Cin, Cout, w_g != nullptr, 1, 1);
+  const Layer U = in_layer(Cin, gate, 1);
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.ka = w_a; t.kg = w_g; t.precision = precision;
+  const long long rows = (long long)B * R;
+  __nv_bfloat16 *dphi, *dplo;
+  float *zero, *dY = dx;
+  BwdScratch S; memset(&S, 0, sizeof S);
+  CK(entry_scratch(e, [&](Bump& ws) {
+    take_planes(ws, rows, L.width(), &dphi, &dplo);
+    zero = ws.take<float>(Cout); S.post = ws.take<float>((size_t)B * 4 * Cin);
+    if (gate) dY = ws.take<float>((size_t)rows * Cin);
+  }));
+  EntryStore store;
+  RET(entry_store(e, store, L, t, zero, st));
+  LayerTensors u; memset(&u, 0, sizeof u);
+  u.beta_a = beta_a; u.gamma_a = gamma_a; u.dbeta_a = dbeta_a; u.dgamma_a = dgamma_a;
+  if (gate) { u.beta_g = beta_g; u.gamma_g = gamma_g; u.dbeta_g = dbeta_g; u.dgamma_g = dgamma_g; }
+  u.tc = t.tc; u.precision = precision;                   // (tc: U's dP goes to operand planes)
+  CK(tc_split_planes(precision, dp, rows, L.width(), dphi, dplo, st));
+  // dY = dgrad(dp) (+ dx): the residual form keeps it in dx; the gated form works on a copy, so that dx is only read
+  if (gate && accumulate) CK(cudaMemcpyAsync(dY, dx, (size_t)rows * Cin * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  S.dPhi = S.dP2hi = (__nv_bfloat16*)hi; S.dPlo = S.dP2lo = (__nv_bfloat16*)lo;
+  if (det) S.det = *det;
+  BwdWalk w(S, fuse && !det);
+  ConvIO in{}; in.n = B; in.H = 1; in.W = R;
+  const GLAct UA{const_cast<float*>(bp), const_cast<float*>(stats), nullptr, nullptr, nullptr};
+  RET(layer_dx(e, w, L, t, in, nullptr, PlanePair{dphi, dplo}, dY, accumulate, st, &U, &u, &UA));
+  const bool f = w.have >= 0;
+  PostBwdParams q;
+  RET(layer_dp(e, w, U, u, UA, dY, B, R, st, q));
+  CK(cudaStreamSynchronize(st));
+  if (fused) *fused = f;
+  return 0;
 }
 
 int cgvc_in_glu_forward_planes(cgvc_handle e, const float* p, const float* beta_a, const float* gamma_a, const float* beta_g,
@@ -2170,8 +2330,9 @@ static ConvIO rows_io(int B) { ConvIO io{}; io.n = B; return io; }
 static PostParams glu_fwd_params(cgvc_engine* e, const float* p, float* y, int B, int R, int C, int precision, void* hi, void* lo,
                                  unsigned long long* sat) {
   const GLAct A{const_cast<float*>(p), nullptr, y, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo};
-  PostParams q = post_params(e, glu_layer(C), rows_io(B), A, R, true, nullptr);
-  q.qmode = precision == CGVC_PREC_F16F8;
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.precision = precision;
+  PostParams q = post_params(e, glu_layer(C), t, rows_io(B), A, R, true, nullptr);
   q.sat = q.qmode && hi ? sat : nullptr;
   q.ufl = q.qmode && hi ? e->plane_ufl : nullptr;
   return q;
@@ -2180,12 +2341,12 @@ static PostBwdParams glu_bwd_params(cgvc_engine* e, const float* dy, const float
                                     int C, int precision, void* hi, void* lo, unsigned long long* sat, const DetSlab* det) {
   const GLAct A{const_cast<float*>(p), nullptr, nullptr, nullptr, nullptr};
   BwdScratch S; memset(&S, 0, sizeof S); S.dP = dp;
-  PostBwdParams q = post_bwd_params(e, glu_layer(C), dy, A, B, R, S, false, true, PlanePair{nullptr, nullptr});
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.dba = dbias_a; t.dbg = dbias_g; t.precision = precision;
+  PostBwdParams q = post_bwd_params(e, glu_layer(C), t, dy, A, B, R, S, true, PlanePair{nullptr, nullptr});
   q.dp_hi = (__nv_bfloat16*)hi; q.dp_lo = (__nv_bfloat16*)lo;
-  q.qmode = precision == CGVC_PREC_F16F8;
   q.sat = q.qmode && hi ? sat : nullptr;
   q.ufl = q.qmode && hi ? e->plane_ufl : nullptr;
-  q.dbias_a = dbias_a; q.dbias_g = dbias_g;
   if (dbias_a && det) q.det = *det;
   return q;
 }
@@ -2236,8 +2397,10 @@ int cgvc_disc_input_forward(cgvc_handle e, int precision, const float* x, const 
   else hi = lo = nullptr;
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   const int R = ((H + sh - 1) / sh) * ((W + sw - 1) / sw);
-  const C1Layer c{w_a, w_g, b_a, b_g, kh, kw, Cout, sh, sw};
-  RET(disc_input_forward(e, c, x, B, H, W, p, glu_fwd_params(e, p, y, B, R, Cout, precision, hi, lo, sat), fuse != 0, (cudaStream_t)stream));
+  const Layer L = conv_layer(kh, kw, 1, Cout, true, sh, sw);
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.ka = w_a; t.kg = w_g; t.ba = b_a; t.bg = b_g;
+  RET(disc_input_forward(e, L, t, x, B, H, W, p, glu_fwd_params(e, p, y, B, R, Cout, precision, hi, lo, sat), fuse != 0, (cudaStream_t)stream));
   if (fused) *fused = fuse != 0;
   return 0;
 }
@@ -2259,10 +2422,12 @@ int cgvc_disc_input_backward(cgvc_handle e, const float* dy, const float* p, con
   const long long ndp = fuse ? 0 : rows * 2 * Cout;
   float* buf;
   CK(grow_post_buf(e, (size_t)(ndp + rows * kh * kw), &buf));
-  const C1Layer c{w_a, w_g, nullptr, nullptr, kh, kw, Cout, sh, sw};
+  const Layer L = conv_layer(kh, kw, 1, Cout, true, sh, sw);
+  LayerTensors t; memset(&t, 0, sizeof t);
+  t.ka = w_a; t.kg = w_g; t.dka = dw_a; t.dkg = dw_g; t.dba = db_a; t.dbg = db_g;
   const PostBwdParams q = glu_bwd_params(e, dy, p, fuse ? nullptr : buf, db_a, db_g, B, (int)(rows / B), Cout, CGVC_PREC_FP32_SIMT, nullptr,
                                          nullptr, nullptr, det);
-  RET(disc_input_backward(e, c, C1Grads{dw_a, dw_g, db_a, db_g}, x, dy, p, B, H, W, dx, buf + ndp, fuse != 0, q, det, (cudaStream_t)stream));
+  RET(disc_input_backward(e, L, t, x, dy, p, B, H, W, dx, buf + ndp, fuse != 0, q, det, (cudaStream_t)stream));
   if (fused) *fused = fuse != 0;
   return 0;
 }
@@ -2338,24 +2503,6 @@ static int edge_entry(cgvc_engine* e, const char* what, int direction, int B, in
   return 0;
 }
 
-// the entry points' scratch, carved from the per-engine buffer: carve(ws) runs once on a null base to size it, then on the buffer
-template <class F> static cudaError_t edge_scratch(cgvc_engine* e, F&& carve) {
-  Bump ws; ws.reset(nullptr, 0);
-  carve(ws);
-  float* buf;
-  cudaError_t ce = grow_post_buf(e, ws.off / sizeof(float) + 1, &buf);
-  if (ce != cudaSuccess) return ce;
-  ws.reset(buf, e->post_elems * sizeof(float));
-  carve(ws);
-  return cudaSuccess;
-}
-
-// operand planes of `rows` rows of c channels in the engine's precision: bf16 hi / lo [rows, ru64(c)], F16F8 fp16 + two e4m3 [rows, ru128(c)]
-static void edge_planes(Bump& ws, long long rows, int c, __nv_bfloat16** hi, __nv_bfloat16** lo) {
-  const size_t n = (size_t)rows * edge_cpad(c);
-  *hi = ws.take<__nv_bfloat16>(n); *lo = ws.take<__nv_bfloat16>(n);
-}
-
 extern "C" {
 
 int cgvc_edge_h1_forward(cgvc_handle e, int direction, const float* x, int B, int T, const long long* offsets, float* p, float* y,
@@ -2367,14 +2514,15 @@ int cgvc_edge_h1_forward(cgvc_handle e, int direction, const float* x, int B, in
   cudaStream_t st = (cudaStream_t)stream;
   const GenNet& N = e->gen[direction];
   __nv_bfloat16 *xchi, *xclo; long long* off = nullptr;
-  CK(edge_scratch(e, [&](Bump& ws) {
-    edge_planes(ws, rows, N.h1.a.kw * e->cfg.num_features, &xchi, &xclo);
+  CK(entry_scratch(e, [&](Bump& ws) {
+    take_planes(ws, rows, N.h1.a.kw * e->cfg.num_features, &xchi, &xclo);
     if (offsets) off = ws.take<long long>((size_t)B + 1);
   }));
   if (offsets) CK(cudaMemcpyAsync(off, offsets, ((size_t)B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
   const int n = offsets ? 1 : B, W = offsets ? (int)rows : T;
   const GLAct A{p, nullptr, y, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo};
-  return h1_edge_forward(e, N, x, n, W, off, offsets ? B : 0, xchi, xclo, p, post_params(e, N.h1, rows_io(n), A, W, true, nullptr), st);
+  const PostParams q = post_params(e, N.h1, layer_tensors(e, N.h1, false), rows_io(n), A, W, true, nullptr);
+  return h1_edge_forward(e, N, x, n, W, off, offsets ? B : 0, xchi, xclo, p, q, st);
 }
 
 int cgvc_edge_o1_forward(cgvc_handle e, int direction, const float* u, int B, int T, const long long* offsets, float* z, float* out,
@@ -2386,8 +2534,8 @@ int cgvc_edge_o1_forward(cgvc_handle e, int direction, const float* u, int B, in
   cudaStream_t st = (cudaStream_t)stream;
   const GenNet& N = e->gen[direction];
   __nv_bfloat16 *uhi, *ulo; long long* off = nullptr; float* zs = nullptr;
-  CK(edge_scratch(e, [&](Bump& ws) {
-    edge_planes(ws, rows, N.o1.a.cin, &uhi, &ulo);
+  CK(entry_scratch(e, [&](Bump& ws) {
+    take_planes(ws, rows, N.o1.a.cin, &uhi, &ulo);
     if (offsets) off = ws.take<long long>((size_t)B + 1);
     if (!z) zs = ws.take<float>((size_t)rows * N.o1.a.kw * N.o1.a.cout);
   }));
@@ -2409,9 +2557,9 @@ int cgvc_edge_o1_backward(cgvc_handle e, int direction, const float* u, const fl
   const GenNet& N = e->gen[direction];
   const int nf = e->cfg.num_features;
   __nv_bfloat16 *uhi, *ulo, *zhi = (__nv_bfloat16*)dz_hi, *zlo = (__nv_bfloat16*)dz_lo;
-  CK(edge_scratch(e, [&](Bump& ws) {
-    edge_planes(ws, rows, N.o1.a.cin, &uhi, &ulo);
-    if (!dz_hi) edge_planes(ws, rows, N.o1.a.kw * nf, &zhi, &zlo);
+  CK(entry_scratch(e, [&](Bump& ws) {
+    take_planes(ws, rows, N.o1.a.cin, &uhi, &ulo);
+    if (!dz_hi) take_planes(ws, rows, N.o1.a.kw * nf, &zhi, &zlo);
   }));
   CK(tc_split_planes(e->cfg.precision, u, rows, N.o1.a.cin, uhi, ulo, st));
   BwdScratch S; memset(&S, 0, sizeof S);
@@ -2433,9 +2581,9 @@ int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const fl
   const int nf = e->cfg.num_features, kc = N.h1.a.kw * nf;
   __nv_bfloat16 *xchi, *xclo, *dphi, *dplo; float* zs = nullptr;
   BwdScratch S; memset(&S, 0, sizeof S);
-  CK(edge_scratch(e, [&](Bump& ws) {
-    edge_planes(ws, rows, kc, &xchi, &xclo);
-    edge_planes(ws, rows, N.h1.width(), &dphi, &dplo);
+  CK(entry_scratch(e, [&](Bump& ws) {
+    take_planes(ws, rows, kc, &xchi, &xclo);
+    take_planes(ws, rows, N.h1.width(), &dphi, &dplo);
     S.post = ws.take<float>((size_t)B * 4 * 1024);
     if (dx && !dz) zs = ws.take<float>((size_t)rows * kc);
   }));
@@ -2443,7 +2591,7 @@ int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const fl
   S.dP = dp; S.dPhi = dphi; S.dPlo = dplo;
   if (det) S.det = *det;
   const GLAct A{const_cast<float*>(p), nullptr, nullptr, nullptr, nullptr};
-  const PostBwdParams q = post_bwd_params(e, N.h1, dy, A, B, T, S, true, dp != nullptr, PlanePair{dphi, dplo});
+  const PostBwdParams q = post_bwd_params(e, N.h1, layer_tensors(e, N.h1, true), dy, A, B, T, S, dp != nullptr, PlanePair{dphi, dplo});
   CK(launch_post_bwd(q, e->opt.post, st));
   return h1_edge_backward(e, N, xchi, xclo, PlanePair{q.dp_hi, q.dp_lo}, B, T, dz ? dz : zs, dx, S, st);
 }

@@ -1617,8 +1617,10 @@ bool make_layer_maps_q(TcLayer& L) {
   return ok;
 }
 
+}  // namespace
 
-int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba, const float* bg, cudaStream_t st) {
+// ------------------------------------------------------------------------------------------------ public API
+int tc_refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba, const float* bg, cudaStream_t st) {
   const int taps = L.kh * L.kw;
   dim3 grid((L.cout + 31) / 32, (L.cin + 31) / 32, taps);
   g_cgvc_launches += L.gated ? 4 : 2;
@@ -1646,8 +1648,8 @@ int refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba,
 }
 
 // x planes: [n,H,W,cin_k] (channels beyond cin are zero)
-int layer_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
-              float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused_out = nullptr, const PackGeom* pk = nullptr) {
+int tc_conv_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
+                float* P, cudaStream_t st, const TcFuse* fuse, bool* fused_out, const PackGeom* pk) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   if (pk && (n != 1 || H != 1 || L.kh != 1 || fuse)) return (int)cudaErrorInvalidValue;
   TcNTParams p; memset(&p, 0, sizeof p);
@@ -1684,8 +1686,8 @@ int layer_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16* x
 }
 
 // dP planes: [rows_out, nt_k]
-int layer_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused_out = nullptr) {
+int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
+                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused_out) {
   if (fused_out) *fused_out = false;
   if (!layer_ok(L) || (precision == 3 && (!layer_ok_q(L) || !L.wdq16))) return TC_UNSUPPORTED;     // F16F8 needs the data-gradient planes (training engines)
   std::vector<GatherGeom> gs = dgrad_geoms(n, H, W, L.kh, L.kw, sh, sw);
@@ -1722,9 +1724,9 @@ int layer_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16*
   return 0;
 }
 
-int layer_wgrad(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                float* dwa, float* dwg, cudaStream_t st, int w16 = 0, const DetSlab* det = nullptr) {
+int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+                  const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
+                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   TcTNParams p; memset(&p, 0, sizeof p);
   p.w16 = (precision == 3 && w16) ? 1 : 0;
@@ -1748,9 +1750,6 @@ int layer_wgrad(const TcLayer& L, int precision, const __nv_bfloat16* xhi, const
   return (int)launch_tn(p, precision, st, det);
 }
 
-}  // namespace
-
-// ------------------------------------------------------------------------------------------------ public API
 int tc_register(TcWeights& w, size_t ka, size_t kg, size_t ba, size_t bg, int kh, int kw, int cin, int cout, int gated, int shuffle, int fold) {
   TcLayer L{}; L.ka = ka; L.kg = kg; L.ba = ba; L.bg = bg; L.kh = kh; L.kw = kw; L.cin = cin; L.cout = cout; L.gated = gated; L.shuffle = shuffle; L.fold = fold;
   w.layers.push_back(L);
@@ -1761,7 +1760,6 @@ static cudaError_t tc_init_kernels();
 
 int tc_alloc(TcWeights& w, int precision, bool train) {
   { cudaError_t ie = tc_init_kernels(); if (ie != cudaSuccess) return (int)ie; }
-  w.precision = precision;
   w.quant = precision == 3;
   w.quant_bwd = w.quant && train;
   w.wgrad16 = w.quant;                              // option "wgrad_f16"
@@ -1868,7 +1866,7 @@ int tc_refresh_weights(TcWeights& w, const float* params, cudaStream_t st) {
   const bool batched = w.prep_batched && w.prep_jobs;
   for (TcLayer& L : w.layers) {
     if (batched && L.wq16) continue;
-    int r = refresh_layer(L, params + L.ka, params + L.kg, params + L.ba, params + L.bg, st);
+    int r = tc_refresh_layer(L, params + L.ka, params + L.kg, params + L.ba, params + L.bg, st);
     if (r != 0) return r;
   }
   if (batched) { int r = refresh_jobs(w, params, 0, (int)w.job_ka.size(), st); if (r != 0) return r; }
@@ -1883,7 +1881,7 @@ int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, si
   for (TcLayer& L : w.layers) {
     if (L.ka < begin || L.ka >= end) continue;
     if (batched && L.wq16) continue;
-    int r = refresh_layer(L, params + L.ka, params + L.kg, params + L.ba, params + L.bg, st);
+    int r = tc_refresh_layer(L, params + L.ka, params + L.kg, params + L.ba, params + L.bg, st);
     if (r != 0) return r;
   }
   if (batched) {
@@ -1907,7 +1905,7 @@ void tc_layer_dims(const TcWeights& w, int slot, int dims[7]) {
 
 int tc_layer_plane(const TcWeights& w, int slot, const char* name, const void** p, size_t* bytes) {
   const TcLayer& L = w.layers[slot];
-  const bool bf = w.pool && !L.wq16;                 // refresh_layer writes the bf16 planes only for layers without F16F8 planes
+  const bool bf = w.pool && !L.wq16;                 // tc_refresh_layer writes the bf16 planes only for layers without F16F8 planes
   struct Plane { const char* name; const void* p; size_t bytes; };
   const Plane planes[] = {
     {"wf_hi", bf ? L.wf_hi : nullptr, wf_elems(L) * 2}, {"wf_lo", bf ? L.wf_lo : nullptr, wf_elems(L) * 2},
@@ -1924,22 +1922,6 @@ int tc_layer_plane(const TcWeights& w, int slot, const char* name, const void** 
 cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st,
                             unsigned long long* sat, unsigned long long* ufl) {
   return precision == 3 ? launch_pad_split_q(x, rows, C, C, ru(C, 128), hi, lo, st, sat, ufl) : launch_pad_split(x, rows, C, C, ru(C, 64), hi, lo, st);
-}
-
-int tc_conv_fwd(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
-                float* P, cudaStream_t st, const TcFuse* fuse, bool* fused, const PackGeom* pk) {
-  return layer_fwd(w.layers[slot], w.precision, w.debug, xhi, xlo, n, H, W, sh, sw, P, st, fuse, fused, pk);
-}
-
-int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused) {
-  return layer_dgrad(w.layers[slot], w.precision, w.debug, dPhi, dPlo, n, H, W, sh, sw, dx, accumulate, st, fuse, fused);
-}
-
-int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
-                  const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det) {
-  return layer_wgrad(w.layers[slot], w.precision, xhi, xlo, dPhi, dPlo, n, H, W, sh, sw, dwa, dwg, st, w.wgrad16, det);
 }
 
 bool tc_profile_is_on() { return g_prof_on; }
@@ -1976,172 +1958,4 @@ int tc_profile_launches(double* ms, double* flops, long long* meta4, int capacit
   }
   if (n_out) *n_out = n;
   return 0;
-}
-
-// ---- self-contained versions for the unit tests: fp32 in/out, temporary planes ----
-namespace {
-struct Temp {
-  std::vector<void*> ptrs;
-  ~Temp() { for (void* p : ptrs) cudaFree(p); }
-  template <class T> T* get(size_t n) { void* p = nullptr; if (cudaMalloc(&p, n * sizeof(T) + 256) != cudaSuccess) return nullptr; ptrs.push_back(p); return (T*)p; }
-};
-}  // namespace
-
-static int adhoc_layer_q(Temp& T, TcLayer& L, cudaStream_t st) {
-  L.wq16 = T.get<uint16_t>(wq_elems(L)); L.wq8hi = T.get<uint8_t>(wq_elems(L)); L.wq8lo = T.get<uint8_t>(wq_elems(L));
-  if (!L.wq16 || !L.wq8hi || !L.wq8lo) return (int)cudaErrorMemoryAllocation;
-  cudaMemsetAsync(L.wq16, 0, wq_elems(L) * 2, st); cudaMemsetAsync(L.wq8hi, 0, wq_elems(L), st); cudaMemsetAsync(L.wq8lo, 0, wq_elems(L), st);
-  L.wdq16 = T.get<uint16_t>(wdq_elems(L)); L.wdq8hi = T.get<uint8_t>(wdq_elems(L)); L.wdq8lo = T.get<uint8_t>(wdq_elems(L));
-  if (!L.wdq16 || !L.wdq8hi || !L.wdq8lo) return (int)cudaErrorMemoryAllocation;
-  cudaMemsetAsync(L.wdq16, 0, wdq_elems(L) * 2, st); cudaMemsetAsync(L.wdq8hi, 0, wdq_elems(L), st); cudaMemsetAsync(L.wdq8lo, 0, wdq_elems(L), st);
-  return make_layer_maps_q(L) ? 0 : (int)cudaErrorInvalidValue;
-}
-
-static int adhoc_layer(Temp& T, TcLayer& L, cudaStream_t st) {
-  L.wf_hi = T.get<__nv_bfloat16>(wf_elems(L)); L.wf_lo = T.get<__nv_bfloat16>(wf_elems(L));
-  L.wd_hi = T.get<__nv_bfloat16>(wd_elems(L)); L.wd_lo = T.get<__nv_bfloat16>(wd_elems(L));
-  L.bias = T.get<float>(nt_n(L));
-  if (!L.wf_hi || !L.wf_lo || !L.wd_hi || !L.wd_lo || !L.bias) return (int)cudaErrorMemoryAllocation;
-  cudaMemsetAsync(L.wf_hi, 0, wf_elems(L) * 2, st); cudaMemsetAsync(L.wf_lo, 0, wf_elems(L) * 2, st);
-  cudaMemsetAsync(L.wd_hi, 0, wd_elems(L) * 2, st); cudaMemsetAsync(L.wd_lo, 0, wd_elems(L) * 2, st);
-  cudaMemsetAsync(L.bias, 0, nt_n(L) * sizeof(float), st);
-  if (!make_layer_maps(L)) return (int)cudaErrorInvalidValue;
-  return 0;
-}
-
-int tc_conv_fwd_adhoc(int precision, int debug, const float* x, const float* w, const float* bias, float* y,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st) {
-  TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
-  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
-  Temp T;
-  int r = adhoc_layer(T, L, st); if (r) return r;
-  size_t rows = (size_t)B * H * W;
-  const int cpad = precision == 3 ? cin_q(L) : cin_k(L);
-  if (precision == 3) { r = adhoc_layer_q(T, L, st); if (r) return r; }
-  __nv_bfloat16* xhi = T.get<__nv_bfloat16>(rows * cpad); __nv_bfloat16* xlo = T.get<__nv_bfloat16>(rows * cpad);
-  float* zero = T.get<float>(Cout);
-  if (!xhi || !xlo || !zero) return (int)cudaErrorMemoryAllocation;
-  cudaMemsetAsync(zero, 0, Cout * sizeof(float), st);
-  r = refresh_layer(L, w, nullptr, bias ? bias : zero, nullptr, st); if (r) return r;
-  cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
-  if (e != cudaSuccess) return (int)e;
-  r = layer_fwd(L, precision, debug, xhi, xlo, B, H, W, sh, sw, y, st); if (r) return r;
-  return (int)cudaStreamSynchronize(st);
-}
-
-int tc_conv_bwd_adhoc(int precision, int debug, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16, const DetSlab* det) {
-  TcLayer L{}; L.kh = kh; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = 0;
-  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
-  Temp T;
-  int r = adhoc_layer(T, L, st); if (r) return r;
-  if (precision == 3) { r = adhoc_layer_q(T, L, st); if (r) return r; }
-  GatherGeom g = fwd_geom(B, H, W, kh, kw, sh, sw);
-  size_t rows = (size_t)B * H * W, orows = (size_t)g.B * g.Hy * g.Wx;
-  const int xpad = precision == 3 ? cin_q(L) : cin_k(L), gpad = precision == 3 ? nt_q(L) : nt_k(L);
-  __nv_bfloat16* xhi = T.get<__nv_bfloat16>(rows * xpad); __nv_bfloat16* xlo = T.get<__nv_bfloat16>(rows * xpad);
-  __nv_bfloat16* ghi = T.get<__nv_bfloat16>(orows * gpad); __nv_bfloat16* glo = T.get<__nv_bfloat16>(orows * gpad);
-  float* zero = T.get<float>(Cout);
-  if (!xhi || !xlo || !ghi || !glo || !zero) return (int)cudaErrorMemoryAllocation;
-  cudaMemsetAsync(zero, 0, Cout * sizeof(float), st);
-  r = refresh_layer(L, w, nullptr, zero, nullptr, st); if (r) return r;
-  cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
-  if (e != cudaSuccess) return (int)e;
-  e = tc_split_planes(precision, dy, (long long)orows, Cout, ghi, glo, st);
-  if (e != cudaSuccess) return (int)e;
-  if (dx) { r = layer_dgrad(L, precision, debug, ghi, glo, B, H, W, sh, sw, dx, 0, st); if (r) return r; }
-  if (dw) {
-    r = layer_wgrad(L, precision, xhi, xlo, ghi, glo, B, H, W, sh, sw, dw, nullptr, st, w16, det); if (r) return r;
-    if (dbias) { e = launch_colsum(dy, (long long)orows, Cout, 0, Cout, dbias, st, det); if (e != cudaSuccess) return (int)e; }
-  }
-  return (int)cudaStreamSynchronize(st);
-}
-
-// an ad-hoc 1-D layer (kh = 1) with its weight planes and bias, gated when wg is given
-static int adhoc_layer_1d(Temp& T, TcLayer& L, int precision, const float* wa, const float* wg, const float* ba, const float* bg,
-                          int Cin, int kw, int Cout, int shuffle, cudaStream_t st) {
-  L.kh = 1; L.kw = kw; L.cin = Cin; L.cout = Cout; L.gated = wg != nullptr; L.shuffle = shuffle;
-  if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
-  int r = adhoc_layer(T, L, st); if (r) return r;
-  if (precision == 3) { r = adhoc_layer_q(T, L, st); if (r) return r; }
-  float* zero = T.get<float>(Cout);
-  if (!zero) return (int)cudaErrorMemoryAllocation;
-  cudaMemsetAsync(zero, 0, Cout * sizeof(float), st);
-  return refresh_layer(L, wa, wg, ba ? ba : zero, bg ? bg : zero, st);
-}
-
-int tc_conv_in_fwd_adhoc(int precision, int debug, PostForms forms, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
-                         const TcFuse& fz, float* P, int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused,
-                         cudaStream_t st) {
-  if (fused) *fused = 0;
-  TcLayer L{};
-  Temp T;
-  int r = adhoc_layer_1d(T, L, precision, wa, wg, ba, bg, Cin, kw, Cout, shuffle, st); if (r) return r;
-  const size_t rows = (size_t)B * W;
-  const int Wo = (W + sw - 1) / sw, cpad = precision == 3 ? cin_q(L) : cin_k(L);
-  __nv_bfloat16* xhi = T.get<__nv_bfloat16>(rows * cpad); __nv_bfloat16* xlo = T.get<__nv_bfloat16>(rows * cpad);
-  if (!xhi || !xlo) return (int)cudaErrorMemoryAllocation;
-  cudaError_t e = tc_split_planes(precision, x, (long long)rows, Cin, xhi, xlo, st);
-  if (e != cudaSuccess) return (int)e;
-  TcFuse f = fz; f.R = Wo;
-  bool have_p = false;
-  if (fuse) {
-    bool done = false;
-    r = layer_fwd(L, precision, debug, xhi, xlo, B, 1, W, 1, sw, P, st, &f, &done);
-    if (r != 0 && (done || P)) return r;                 // a failed launch (not the missing P of a shape the epilogue refuses)
-    if (done) { if (fused) *fused = 1; return (int)cudaStreamSynchronize(st); }
-    have_p = P != nullptr;                                 // refused: P already holds the plain-epilogue output
-  }
-  // the engine's fallback: the plain epilogue, then the instance-norm kernels
-  float* Pw = P ? P : T.get<float>((size_t)B * Wo * Ntot(L));
-  float* stats = fz.stats ? fz.stats : T.get<float>((size_t)B * 4 * (Cout / shuffle));
-  float* scratch = T.get<float>((size_t)B * 4 * (Cout / shuffle));
-  if (!Pw || !stats || !scratch) return (int)cudaErrorMemoryAllocation;
-  if (!have_p) { r = layer_fwd(L, precision, debug, xhi, xlo, B, 1, W, 1, sw, Pw, st); if (r) return r; }
-  PostParams q; memset(&q, 0, sizeof q);
-  q.p = Pw; q.ldp = Ntot(L); q.Cc = Cout; q.B = B; q.sh = shuffle; q.R = Wo * shuffle; q.C = Cout / shuffle;
-  q.has_in = 1; q.has_gate = L.gated;
-  q.beta_a = fz.beta_a; q.gamma_a = fz.gamma_a; q.beta_g = fz.beta_g; q.gamma_g = fz.gamma_g; q.resid = fz.resid;
-  q.y = fz.y; q.stats = stats; q.y_hi = fz.y_hi; q.y_lo = fz.y_lo; q.qmode = precision == 3; q.scratch = scratch;
-  e = launch_post_fwd(q, forms, st);
-  if (e != cudaSuccess) return (int)e;
-  return (int)cudaStreamSynchronize(st);
-}
-
-int tc_conv_in_bwd_adhoc(int precision, int debug, PostForms forms, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
-                         int B, int R, int Cin, int kw, int Cout, int fuse, int* fused, const DetSlab* det, cudaStream_t st) {
-  if (fused) *fused = 0;
-  TcLayer L{};
-  Temp T;
-  int r = adhoc_layer_1d(T, L, precision, wa, wg, nullptr, nullptr, Cin, kw, Cout, 1, st); if (r) return r;
-  const size_t rows = (size_t)B * R;
-  const int gpad = precision == 3 ? nt_q(L) : nt_k(L);
-  __nv_bfloat16* ghi = T.get<__nv_bfloat16>(rows * gpad); __nv_bfloat16* glo = T.get<__nv_bfloat16>(rows * gpad);
-  if (!ghi || !glo) return (int)cudaErrorMemoryAllocation;
-  cudaError_t e = tc_split_planes(precision, dP, (long long)rows, Ntot(L), ghi, glo, st);
-  if (e != cudaSuccess) return (int)e;
-  // dY = dgrad(dP) (+ dx): the residual form keeps it in dx; the gated form works on a copy, so that dx is only read
-  float* dY = dx;
-  if (uf.gated) {
-    dY = T.get<float>(rows * Cin);
-    if (!dY) return (int)cudaErrorMemoryAllocation;
-    if (accumulate) { e = cudaMemcpyAsync(dY, dx, rows * Cin * sizeof(float), cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) return (int)e; }
-  }
-  TcBwdFuse f = uf; f.R = R; f.bp_ld = f.dp_ld = (uf.gated ? 2 : 1) * Cin;
-  bool done = false;
-  r = layer_dgrad(L, precision, debug, ghi, glo, B, 1, R, 1, 1, dY, accumulate, st, fuse && !det ? &f : nullptr, &done);
-  if (r) return r;
-  if (done) { if (fused) *fused = 1; return (int)cudaStreamSynchronize(st); }
-  // the engine's fallback: the plain data gradient above, then the instance-norm (+ GLU) backward kernels
-  float* scratch = T.get<float>((size_t)B * 4 * Cin);
-  if (!scratch) return (int)cudaErrorMemoryAllocation;
-  PostBwdParams q; memset(&q, 0, sizeof q);
-  if (det) q.det = *det;
-  q.dy1 = dY; q.p = uf.bp; q.ldp = f.bp_ld; q.Cc = Cin; q.B = B; q.R = R; q.C = Cin; q.sh = 1;
-  q.beta_a = uf.beta_a; q.gamma_a = uf.gamma_a; q.beta_g = uf.beta_g; q.gamma_g = uf.gamma_g; q.has_in = 1; q.has_gate = uf.gated;
-  q.stats = uf.stats; q.dp_hi = uf.dp_hi; q.dp_lo = uf.dp_lo; q.qmode = precision == 3;
-  q.dbeta_a = uf.dbeta_a; q.dgamma_a = uf.dgamma_a; q.dbeta_g = uf.dbeta_g; q.dgamma_g = uf.dgamma_g; q.scratch = scratch;
-  e = launch_post_bwd(q, forms, st);
-  if (e != cudaSuccess) return (int)e;
-  return (int)cudaStreamSynchronize(st);
 }

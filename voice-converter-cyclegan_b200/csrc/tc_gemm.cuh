@@ -39,7 +39,6 @@ struct TcWeights {
   void* pool = nullptr;
   size_t pool_bytes = 0;
   bool ready = false;
-  int precision = 0;              // the engine's CGVC_PREC_* (set by tc_alloc): the operand planes every slot-based call reads and writes
   bool quant = false;             // also keep the F16F8 forward planes (precision F16F8)
   bool quant_bwd = false;         // ... and the F16F8 data-gradient planes (training in that precision)
   void* prep_jobs = nullptr;      // device job table of the batched F16F8 plane kernel (tc_gemm.cu PrepJob), one job per layer branch
@@ -78,6 +77,8 @@ int tc_register(TcWeights& w, size_t ka, size_t kg, size_t ba, size_t bg, int kh
 int tc_alloc(TcWeights& w, int precision, bool train);
 void tc_free(TcWeights& w);
 int tc_refresh_weights(TcWeights& w, const float* params, cudaStream_t st);
+// the planes and bias of one layer from its TF kernels ka / kg and biases ba / bg (the per-layer step of tc_refresh_weights)
+int tc_refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* ba, const float* bg, cudaStream_t st);
 int tc_refresh_weights_range(TcWeights& w, const float* params, size_t begin, size_t end, cudaStream_t st);
 // Read-only view of registered layer `slot` (include/cgvc.h cgvc_weight_planes).  dims = {nt_n, cin_k, cin_n, nt_k, cin_q, nt_q, layer_ok_q}.
 // tc_layer_plane: the device address and size in bytes (padding included) of a named plane; *p = null when the store keeps no such plane
@@ -91,45 +92,27 @@ int tc_layer_plane(const TcWeights& w, int slot, const char* name, const void** 
 cudaError_t tc_split_planes(int precision, const float* x, long long rows, int C, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st,
                             unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr);
 
-// The slot-based calls below read and write the planes of w.precision (tc_split_planes), with their channel count rounded up
-// (zero-filled): x [n,H,W,cin], dP [rows, Ntot].  They return 0, TC_UNSUPPORTED (no launch: the shape has no tensor-core form)
-// or a cudaError_t.
+// The convolutions of layer L below read and write the planes of `precision` (tc_split_planes), with their channel count rounded up
+// (zero-filled): x [n,H,W,cin], dP [rows, Ntot].  debug and w16: the store's TcWeights::debug and TcWeights::wgrad16.  They return
+// 0, TC_UNSUPPORTED (no launch: the shape has no tensor-core form) or a cudaError_t.
 // P[rows, Ntot] = conv(x) + bias.
 //   fuse: instance norm (+ GLU | + residual) fused into the epilogue when the shape allows (1-D layer, whole samples per 128-row
 //         tile: R in {32,64,128}); *fused tells the caller whether it happened (if not, P is written and the caller runs the
 //         separate instance-norm kernels).
 //   pk:   a 1-D layer over packed variable-length utterances (kernels.cuh PackGeom): n = H = 1, x planes [W, .] at the source level
 //         of divisor pk->div; every tap reads only its own utterance's rows.  Plain epilogue only.
-int tc_conv_fwd(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
-                float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused = nullptr, const PackGeom* pk = nullptr);
+int tc_conv_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W,
+                int sh, int sw, float* P, cudaStream_t st, const TcFuse* fuse = nullptr, bool* fused = nullptr, const PackGeom* pk = nullptr);
 // dx[n,H,W,cin] (+)= dgrad(dP)            (dP planes [rows_out, Ntot]; H, W are the INPUT dims)
 //   fuse: the upstream layer's instance-norm (+ GLU) backward fused into the epilogue when the shape allows (stride-1 1-D layer,
 //         whole samples per 128-row tile): the launch then writes that layer's dP planes (and, for gated = 0, dx = dY) instead
 //         of / besides dx; *fused tells whether it happened (if not, dx holds the plain data gradient).
-int tc_conv_dgrad(TcWeights& w, int slot, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr);
+int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W,
+                  int sh, int sw, float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr);
 // dW_a/dW_g (TF layout) += x^T dP  (the bias gradients are column sums of dP: the instance-norm backward kernels or launch_colsum)
-int tc_conv_wgrad(TcWeights& w, int slot, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dwa, float* dwg, cudaStream_t st, const DetSlab* det = nullptr);   // det: deterministic mode (kernels.cuh DetSlab)
-// self-contained versions for unit tests (fp32 in/out, temporary planes allocated internally); debug, w16 and forms: the calling
-// engine's TcWeights::debug, TcWeights::wgrad16 and instance-norm kernel forms
-int tc_conv_fwd_adhoc(int precision, int debug, const float* x, const float* w, const float* bias, float* y,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st);
-int tc_conv_bwd_adhoc(int precision, int debug, const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias,
-                      int B, int H, int W, int Cin, int kh, int kw, int Cout, int sh, int sw, cudaStream_t st, int w16,
-                      const DetSlab* det);
-// one generator layer as the engine runs it (include/cgvc.h cgvc_conv_in_forward): the 1-D convolution of x [B, W, Cin] (gated when wg
-// is given) and the instance norm of fz (fz.R is set here).  fuse: the fused epilogue where the shape allows (*fused = 1), else the
-// plain epilogue and launch_post_fwd; P may be null (inference: a temporary when the shape needs the fallback)
-int tc_conv_in_fwd_adhoc(int precision, int debug, PostForms forms, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
-                         const TcFuse& fz, float* P, int B, int W, int Cin, int kw, int Cout, int sw, int shuffle, int fuse, int* fused,
-                         cudaStream_t st);
-// the data gradient of a stride-1 1-D layer from fp32 dP [B*R, Ntot] with the upstream layer's instance-norm (+ GLU) backward uf
-// (uf.R, bp_ld and dp_ld are set here; include/cgvc.h cgvc_conv_in_backward): fused where the shape allows, else the plain data
-// gradient and launch_post_bwd.  det: deterministic mode (never fused)
-int tc_conv_in_bwd_adhoc(int precision, int debug, PostForms forms, const float* dP, const float* wa, const float* wg, const TcBwdFuse& uf, float* dx, int accumulate,
-                         int B, int R, int Cin, int kw, int Cout, int fuse, int* fused, const DetSlab* det, cudaStream_t st);
 
 // per-launch CUDA-event timing of the tensor-core kernels (class 0 = forward/dgrad kernel with the plain epilogue,
 // 1 = wgrad kernel, 2 = forward kernel with the fused instance-norm epilogue)
