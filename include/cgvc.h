@@ -200,30 +200,40 @@ int cgvc_discriminator_forward(cgvc_handle h, int which, const float* in_dev, fl
  * model.py:44-108; here a caller composes them into any objective and runs each application's backward itself).
  * A tape is caller-owned device memory (256-byte aligned, at least cgvc_tape_bytes) that a forward fills with what the backward of that
  * one network application reads: its input and its layers' pre-norm outputs, statistics, outputs and operand planes, as a train step
- * keeps them.  kind 0 = generator, 1 = discriminator; batch <= max_batch, frames <= max_frames (a multiple of 4 / 16).
+ * keeps them.  kind 0 = generator, 1 = discriminator; batch <= max_batch, frames <= max_frames (a multiple of 4 / 16).  kind 2 = packed
+ * generator (cgvc_generator_forward_packed_tape): cgvc_tape_bytes(h, 2, n, rows, &bytes) with n utterances of rows = offsets[n] frames in
+ * all, n <= max_batch and rows <= max_batch x max_frames as cgvc_generator_forward_packed takes them.
  *   - Forward: the same outputs, bit for bit, as cgvc_generator_forward / cgvc_discriminator_forward.  A tape starts with a header
  *     written by the forward (kind, direction or which, batch, frames, the writing engine and its parameter generation); the engine
  *     keeps a copy, so that a backward checks its tape without reading the device.  cgvc_params_updated, cgvc_bind_arena and every Adam
  *     update (cgvc_adam_step, cgvc_train_step) advance the parameter generation.
  *   - Backward: from d out [batch, 24, frames] (generator) or d prob [batch, 6, frames/16] (discriminator), the network's kernel / bias /
  *     beta / gamma gradients are ADDED into its GRAD range and d in [batch, 24, frames] is written to din_dev (NULL = none).  It does not
- *     modify the tape: a tape can be back-propagated any number of times (each adds its gradients again).
+ *     modify the tape: a tape can be back-propagated any number of times (each adds its gradients again).  cgvc_generator_backward_tape
+ *     takes kinds 0 and 2; of a packed tape, d out and d in have the packed layout of cgvc_generator_forward_packed (utterance u is the
+ *     [24][len_u] block at element 24 * offsets[u]), and every tap, instance norm and edge-layer sum stays inside its utterance, as in
+ *     the forward.  The tape holds its own copy of the offsets: a later call that reuses WORK does not change what its backward reads.
  *   - Errors, all before anything is enqueued: a tape this engine did not write, one written before the parameters last changed or one
  *     of the other kind: CGVC_ERR_ARG.  A tape buffer smaller than cgvc_tape_bytes: CGVC_ERR_UNBOUND.  A backward on an engine without
  *     GRAD or without a training WORK arena (train = 0): CGVC_ERR_UNBOUND.
  *   - Scratch: the backward borrows the backward scratch of a train step at max_batch in WORK; WORK is not enlarged for it.
- *   - Loss scaling (F16F8): the upstream gradient is multiplied by the static loss scale of the tape's batch before its gradient planes
+ *   - Loss scaling (F16F8): the upstream gradient is multiplied by the static loss scale of the tape's batch (of a packed tape: of a
+ *     batch of n, its utterance count) before its gradient planes
  *     are formed and d in is returned with it removed (exact: a power of two); the GRAD contributions keep it (see cgvc_adam_step).
  *     With "loss_scale" = 1 the backward counts its saturated gradient-plane groups into the counters of cgvc_loss_scale_state (and the
  *     per-network ones: the generator's into index 0, the discriminator's into index 1), adding to them until the next train step clears
  *     them.  The dynamic policy ("loss_scale" = 2) does not act on tape calls: no skip, no scale change; they use the static scale.
  *   - Options: "deterministic" makes repeated forward / backward sequences give the same GRAD bits; the kernel-choice options act as in a
  *     train step.  Tape calls run eagerly on `stream`, never as captured graphs.
- * Not covered: packed (variable-length) tapes, per-call or per-network loss scales, data-parallel reduction (cgvc_allreduce_grads
- * sums GRAD over ranks). */
+ * Not covered: packed discriminator tapes, per-call or per-network loss scales, data-parallel reduction (cgvc_allreduce_grads sums
+ * GRAD over ranks). */
 int cgvc_tape_bytes(cgvc_handle h, int kind, int batch, int frames, size_t* bytes);
 int cgvc_generator_forward_tape(cgvc_handle h, int direction, const float* in_dev, float* out_dev, int batch, int frames,
                                 void* tape_dev, size_t tape_bytes, void* stream);
+/* cgvc_generator_forward_packed with a kind 2 tape: the same argument checks and errors (all before anything is enqueued), then the
+ * tape checks above; out_dev bit for bit what cgvc_generator_forward_packed writes.  The offsets are copied into the tape. */
+int cgvc_generator_forward_packed_tape(cgvc_handle h, int direction, const float* in_dev, float* out_dev, const long long* offsets_host,
+                                       int n, void* tape_dev, size_t tape_bytes, void* stream);
 int cgvc_discriminator_forward_tape(cgvc_handle h, int which, const float* in_dev, float* prob_dev, int batch, int frames,
                                     void* tape_dev, size_t tape_bytes, void* stream);
 int cgvc_generator_backward_tape(cgvc_handle h, const void* tape_dev, const float* dout_dev, float* din_dev, void* stream);

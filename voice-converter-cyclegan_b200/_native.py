@@ -122,6 +122,7 @@ def _declare(lib):
         "cgvc_edge_h1_backward": (ci, [vp, ci, vp, vp, vp, ci, ci] + [vp] * 4),
         "cgvc_tape_bytes": (ci, [vp, ci, ci, ci, P(sz)]),
         "cgvc_generator_forward_tape": (ci, [vp, ci, vp, vp, ci, ci, vp, sz, vp]),
+        "cgvc_generator_forward_packed_tape": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp, sz, vp]),
         "cgvc_discriminator_forward_tape": (ci, [vp, ci, vp, vp, ci, ci, vp, sz, vp]),
         "cgvc_generator_backward_tape": (ci, [vp, vp, vp, vp, vp]),
         "cgvc_discriminator_backward_tape": (ci, [vp, vp, vp, vp, vp]),

@@ -76,7 +76,9 @@ struct TapeHeader {
   unsigned long long magic;     // kTapeMagic
   unsigned long long engine;    // cgvc_engine::id of the writer
   unsigned long long gen;       // cgvc_engine::param_gen when it was written
-  int kind, which, batch, frames;
+  int kind, which, batch, frames;  // kind 2 (packed generator tape): batch = the utterance count n, frames = 0
+  long long rows;               // kind 2: offsets[n], the frames of all utterances
+  int max_len;                  // kind 2: the longest utterance
 };
 static const unsigned long long kTapeMagic = 0x45504154435647ull;   // "GVCTAPE"
 static const size_t kTapeHead = 256;                                // the activations start 256 bytes in
@@ -339,8 +341,10 @@ static int conv_fwd_simt(cgvc_engine* e, const float* w, const float* bias, cons
 }
 
 // dx (+)= dgrad(dy[., coff:coff+cout], w)
+// pk: packed utterances (n = H = 1, pk->div the input level's divisor): every parity class reads dy at the output level, of divisor
+// pk->div * sw (DESIGN.md section 12)
 static int conv_dgrad_simt(cgvc_engine* e, const float* w, const ConvW& c, int sh, int sw, int n, int H, int W,
-                           const float* dy, int ld, int coff, float* dx, int accumulate, cudaStream_t st) {
+                           const float* dy, int ld, int coff, float* dx, int accumulate, cudaStream_t st, const PackGeom* pk = nullptr) {
   if (!dy) return fail(e, CGVC_ERR_UNSUPPORTED, "fp32 gradients were not kept for a layer that fell back to the SIMT path");
   std::vector<GatherGeom> gs = dgrad_geoms(n, H, W, c.kh, c.kw, sh, sw);
   for (const GatherGeom& g : gs) {
@@ -348,7 +352,8 @@ static int conv_dgrad_simt(cgvc_engine* e, const float* w, const ConvW& c, int s
     op.src = dy; op.s_ld = ld; op.s_coff = coff; op.C = c.cout;
     op.w = w; op.w_ts = (long long)c.cin * c.cout; op.w_cs = 1; op.w_ns = c.cout; op.N = c.cin;
     op.dst = dx; op.d_ld = c.cin; op.d_coff = 0; op.bias = nullptr; op.accumulate = accumulate;
-    CK(launch_gg_simt(g, op, st));
+    if (pk) { PackGeom q = *pk; q.div = pk->div * sw; CK(launch_gg_simt_packed(g, op, q, st)); }
+    else CK(launch_gg_simt(g, op, st));
   }
   return 0;
 }
@@ -358,7 +363,7 @@ static int conv_wgrad_simt(cgvc_engine* e, float* dw, const ConvW& c, int sh, in
                            const float* dy, int ld, int coff, cudaStream_t st, const DetSlab* det) {
   if (!io.x || !dy) return fail(e, CGVC_ERR_UNSUPPORTED, "fp32 tensors were not kept for a layer that fell back to the SIMT path");
   GatherGeom g = fwd_geom(io.n, io.H, io.W, c.kh, c.kw, sh, sw);
-  CK(launch_wgrad_simt(g, io.x, c.cin, 0, c.cin, dy, ld, coff, c.cout, dw, (long long)c.cin * c.cout, c.cout, 1, st, det != nullptr));
+  CK(launch_wgrad_simt(g, io.x, c.cin, 0, c.cin, dy, ld, coff, c.cout, dw, (long long)c.cin * c.cout, c.cout, 1, st, det != nullptr, packed(io)));
   return 0;
 }
 
@@ -463,11 +468,11 @@ static int conv_dgrad(cgvc_engine* e, const Layer& L, const LayerTensors& t, con
                       int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr) {
   bool done = false;
   if (t.tc && dp.hi)
-    RET(tc_result(e, tc_conv_dgrad(*t.tc, t.precision, t.debug, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, dx, accumulate, st, fuse, fused),
-                  &L.a, "data gradient", &done));
+    RET(tc_result(e, tc_conv_dgrad(*t.tc, t.precision, t.debug, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, dx, accumulate, st, fuse, fused,
+                                   packed(io)), &L.a, "data gradient", &done));
   if (done) return 0;
-  RET(conv_dgrad_simt(e, t.ka, L.a, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), 0, dx, accumulate, st));
-  if (L.gated()) RET(conv_dgrad_simt(e, t.kg, L.g, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), L.a.cout, dx, 1, st));
+  RET(conv_dgrad_simt(e, t.ka, L.a, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), 0, dx, accumulate, st, packed(io)));
+  if (L.gated()) RET(conv_dgrad_simt(e, t.kg, L.g, L.sh, L.sw, io.n, io.H, io.W, dP, L.width(), L.a.cout, dx, 1, st, packed(io)));
   return 0;
 }
 
@@ -477,7 +482,7 @@ static int conv_wgrad(cgvc_engine* e, const Layer& L, const LayerTensors& t, con
   bool done = false;
   if (t.tc && dp.hi && io.xhi)
     RET(tc_result(e, tc_conv_wgrad(*t.tc, t.precision, t.wgrad16, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, t.dka, t.dkg,
-                                   st, det), &L.a, "weight gradient", &done));
+                                   st, det, packed(io)), &L.a, "weight gradient", &done));
   if (done) return 0;
   RET(conv_wgrad_simt(e, t.dka, L.a, L.sh, L.sw, io, dP, L.width(), 0, st, det));
   if (L.gated()) RET(conv_wgrad_simt(e, t.dkg, L.g, L.sh, L.sw, io, dP, L.width(), L.a.cout, st, det));
@@ -726,9 +731,11 @@ static void side_join(const BwdScratch& S, cudaStream_t st) {
 }
 
 // GLU / instance-norm backward of a layer into dP planes `out`, with the parameter gradients t holds; fp32 dP is only materialised when
-// a SIMT kernel will read it
+// a SIMT kernel will read it.  in (may be null): the layer's input; when it is packed and L has an instance norm, *seg receives the
+// utterance segments the norm follows (launch_post_bwd's PostBwdSeg), else seg->seg.off stays null
 static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const LayerTensors& t, const float* dy, const GLAct& A, int n,
-                                     int rows_per_sample_out, const BwdScratch& S, bool need_fp32, PlanePair out) {
+                                     int rows_per_sample_out, const BwdScratch& S, bool need_fp32, PlanePair out,
+                                     const ConvIO* in = nullptr, PostBwdSeg* seg = nullptr) {
   PostBwdParams q; memset(&q, 0, sizeof q);
   q.dy1 = dy; q.p = A.P; q.ldp = L.width(); q.Cc = L.a.cout; q.B = n; q.sh = L.shuffle;
   q.R = rows_per_sample_out * L.shuffle; q.C = L.a.cout / L.shuffle;
@@ -743,6 +750,14 @@ static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const
   q.qmode = t.precision == CGVC_PREC_F16F8;
   q.sat = sat_grad(e); q.ufl = ufl_grad(e);
   if (t.dba || t.dbeta_a) q.det = S.det;    // passes without parameter gradients keep the faster (equally deterministic) forms
+  if (seg) seg->seg.off = nullptr;
+  if (seg && in && in->pk.off && L.has_in) {
+    // packed utterances, as post_params: per utterance over its own view rows (the GLU-only layer is row-local and keeps one sample)
+    const long long view_rows = q.R;
+    const int div = (int)((long long)in->pk.div * in->W / view_rows);
+    *seg = PostBwdSeg{PackGeom{in->pk.off, in->pk.n, div, in->pk.max_len}, view_rows};
+    q.B = in->pk.n; q.R = in->pk.max_len / div;
+  }
   return q;
 }
 
@@ -759,11 +774,12 @@ static TcBwdFuse bwd_fuse(const Layer& L, const LayerTensors& t, const GLAct& A,
 
 // dP of a layer: the GLU / instance-norm backward kernel, unless the previous data-gradient launch's fused epilogue wrote it
 static int layer_dp(cgvc_engine* e, BwdWalk& w, const Layer& L, const LayerTensors& t, const GLAct& A, const float* dy, int n,
-                    int rows_per_sample_out, cudaStream_t st, PostBwdParams& q) {
+                    int rows_per_sample_out, cudaStream_t st, PostBwdParams& q, const ConvIO* in = nullptr) {
   bool written = false;
   const PlanePair out = dp_planes(w, st, &written);
-  q = post_bwd_params(e, L, t, dy, A, n, rows_per_sample_out, w.S, false, out);
-  if (!written) CK(launch_post_bwd(q, e->opt.post, st));
+  PostBwdSeg seg;
+  q = post_bwd_params(e, L, t, dy, A, n, rows_per_sample_out, w.S, false, out, in, &seg);
+  if (!written) CK(launch_post_bwd(q, e->opt.post, st, seg.seg.off ? &seg : nullptr));
   return 0;
 }
 
@@ -789,7 +805,7 @@ static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAc
                           const Layer* up = nullptr, const GLAct* upA = nullptr) {
   const LayerTensors t = layer_tensors(e, L, wgrad);
   PostBwdParams q;
-  RET(layer_dp(e, w, L, t, A, dy, in.n, rows_per_sample_out, st, q));
+  RET(layer_dp(e, w, L, t, A, dy, in.n, rows_per_sample_out, st, q, &in));
   const PlanePair dp{q.dp_hi, q.dp_lo};
   if (wgrad) RET(run_wgrad(w.S, dp.hi != nullptr, st, [&](cudaStream_t ws) { return conv_wgrad(e, L, t, in, q.dp, dp, ws, det_of(w.S)); }));
   if (!dx) return 0;
@@ -801,13 +817,14 @@ static int layer_backward(cgvc_engine* e, BwdWalk& w, const Layer& L, const GLAc
 // The tap-lowered edge layers' backward (see h1_edge_forward), n samples of T rows.
 // o1 from d_out [n*T, F]: its dZ planes (the im2col of d_out, dir -1), the kernel gradient U^T dZ into GRAD (run_wgrad, folded columns
 // scattered by tn_dst) and du [n*T, 256] = dZ . W'^T.  The bias gradient, the column sums of d_out, is the caller's
+// (off, n_off: packed utterances, as o1_edge_forward)
 static int o1_edge_backward(cgvc_engine* e, const GenNet& N, const float* d_out, const __nv_bfloat16* uhi, const __nv_bfloat16* ulo, int n,
-                            int T, PlanePair dz, float* du, const BwdScratch& S, cudaStream_t st) {
+                            int T, PlanePair dz, float* du, const BwdScratch& S, cudaStream_t st, const long long* off = nullptr, int n_off = 0) {
   const int nf = e->cfg.num_features;
   float* Gm = e->G();
   const TcLayer& O = e->tcw.layers[N.o1f_slot];
   CK(launch_im2col_taps(d_out, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
-                        dz.hi, dz.lo, st, nullptr, 0, sat_grad(e), ufl_grad(e)));
+                        dz.hi, dz.lo, st, off, n_off, sat_grad(e), ufl_grad(e)));
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
     return tc_result(e, tc_conv_wgrad(O, e->cfg.precision, e->tcw.wgrad16, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws,
                                       det_of(S)),
@@ -821,7 +838,7 @@ static int o1_edge_backward(cgvc_engine* e, const GenNet& N, const float* d_out,
 // the [15,24,128] a and g ranges of GRAD (run_wgrad); with dz, dz [n*T, kw*F] = dP . W^T, and with dx too, dx [n*T, F] = the
 // tap-shifted sum of dz (dir -1)
 static int h1_edge_backward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16* xchi, const __nv_bfloat16* xclo, PlanePair dp, int n,
-                            int T, float* dz, float* dx, const BwdScratch& S, cudaStream_t st) {
+                            int T, float* dz, float* dx, const BwdScratch& S, cudaStream_t st, const long long* off = nullptr, int n_off = 0) {
   const int nf = e->cfg.num_features;
   float* Gm = e->G();
   const TcLayer& H = e->tcw.layers[N.h1c_slot];
@@ -831,7 +848,7 @@ static int h1_edge_backward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16
                      &N.h1.a, "weight gradient (tap-lowered)"); }));
   if (dz) RET(tc_result(e, tc_conv_dgrad(H, e->cfg.precision, e->tcw.debug, dp.hi, dp.lo, n, 1, T, 1, 1, dz, 0, st), &N.h1.a,
                         "data gradient (tap-lowered)"));
-  if (dz && dx) CK(launch_col2im_taps(dz, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, dx, st));
+  if (dz && dx) CK(launch_col2im_taps(dz, N.h1.a.kw * nf, (long long)n * T, T, nf, N.h1.a.kw, -1, nullptr, dx, st, off, n_off));
   return 0;
 }
 
@@ -839,22 +856,28 @@ static int h1_edge_backward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16
 // Weight gradients are accumulated into the GRAD arena; d_in_cl (optional) receives d loss / d input (channels-last).
 static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A, const float* d_out_cl, float* d_in_cl,
                               const BwdScratch& S, cudaStream_t st) {
-  const int n = A.n, T = A.T, nf = e->cfg.num_features;
+  // packed utterances (A.off), as generator_forward: one sequence of all rows whose taps, instance norms and edge-layer tap lowering
+  // follow the utterance boundaries
+  const bool packed = A.off != nullptr;
+  const int n = packed ? 1 : A.n, T = packed ? (int)A.rows : A.T, nf = e->cfg.num_features;
   float* Gm = e->G();
   auto at = [&](const float* x, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int W) {
-    ConvIO io; io.x = x; io.xhi = hi; io.xlo = lo; io.n = n; io.H = 1; io.W = W; return io;
+    ConvIO io; io.x = x; io.xhi = hi; io.xlo = lo; io.n = n; io.H = 1; io.W = W;
+    if (packed) io.pk = PackGeom{A.off, A.n, (int)(A.rows / W), A.max_len};
+    return io;
   };
   auto of = [&](const GLAct& a, int W) { return at(a.Y, a.Yhi, a.Ylo, W); };
-  // the fused backward epilogues do not count saturation: a step whose planes are counted takes the separate kernels
-  BwdWalk w(S, e->opt.fuse_bwd && !e->opt.deterministic && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi && A.r[0].h1.Yhi &&
-               A.r[0].h2.Yhi);
+  // the fused backward epilogues do not count saturation: a step whose planes are counted takes the separate kernels.  Nor do they
+  // take packed rows: they need whole equal-length samples per 128-row tile
+  BwdWalk w(S, e->opt.fuse_bwd && !packed && !e->opt.deterministic && !sat_grad(e) && !side_on(S) && tc_enabled(e) && S.dPhi && S.dP2hi &&
+               A.r[0].h1.Yhi && A.r[0].h2.Yhi);
   const bool edge = edge_on(e, N) && A.xchi && A.z;
   // o1 (no norm, no gate): bias gradient = column sums of d_out
   CK(launch_colsum(d_out_cl, (long long)n * T, nf, 0, nf, Gm + N.o1.a.b, st, det_of(S)));
   const ConvIO u2 = of(A.u[1], T);
   if (edge && u2.xhi && S.dPhi) {
     // tap-lowered o1: dZ[m, (t, c)] = d_out[m - t + 7, c] (im2col of the 24-channel gradient), then dense weight and data gradients
-    RET(o1_edge_backward(e, N, d_out_cl, u2.xhi, u2.xlo, n, T, dp_planes(w, st), S.bufA, S, st));
+    RET(o1_edge_backward(e, N, d_out_cl, u2.xhi, u2.xlo, n, T, dp_planes(w, st), S.bufA, S, st, A.off, A.n));
   } else {
     const LayerTensors t = layer_tensors(e, N.o1, true);
     PlanePair dp{nullptr, nullptr};
@@ -892,8 +915,8 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
   // tap-lowered h1: the weight gradient is im2col(x)^T dP straight into the [15,24,128] kernels' GRAD ranges; the data gradient
   // (cycle passes only) is the dense dP . W^T [n*T, kw*F] followed by the tap-shifted sum
   PostBwdParams q;
-  RET(layer_dp(e, w, N.h1, layer_tensors(e, N.h1, true), A.h1, cur, n, T, st, q));
-  return h1_edge_backward(e, N, A.xchi, A.xclo, PlanePair{q.dp_hi, q.dp_lo}, n, T, d_in_cl ? oth : nullptr, d_in_cl, S, st);
+  RET(layer_dp(e, w, N.h1, layer_tensors(e, N.h1, true), A.h1, cur, n, T, st, q, &x));
+  return h1_edge_backward(e, N, A.xchi, A.xclo, PlanePair{q.dp_hi, q.dp_lo}, n, T, d_in_cl ? oth : nullptr, d_in_cl, S, st, A.off, A.n);
 }
 
 // ---- discriminator ---------------------------------------------------------------------------------------
@@ -1379,23 +1402,33 @@ int cgvc_generator_forward(cgvc_handle e, int direction, const float* in_dev, fl
   return 0;
 }
 
-int cgvc_generator_forward_packed(cgvc_handle e, int direction, const float* in_dev, float* out_dev,
-                                  const long long* offsets_host, int n, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
+// The argument checks of the packed generator calls (cgvc_generator_forward_packed, cgvc_generator_forward_packed_tape): *rows and
+// *max_len receive offsets[n] and the longest utterance
+static int packed_args(cgvc_engine* e, int direction, const void* in_dev, const void* out_dev, const long long* offsets_host, int n,
+                       long long* rows, long long* max_len) {
   if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
   if (!in_dev || !out_dev || !offsets_host) return fail(e, CGVC_ERR_ARG, "null buffer");
   if (n < 1 || n > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", n, e->cfg.max_batch);
   if (offsets_host[0] != 0) return fail(e, CGVC_ERR_ARG, "offsets[0] is %lld, must be 0", offsets_host[0]);
-  long long max_len = 0;
+  *max_len = 0;
   for (int u = 0; u < n; ++u) {
     const long long len = offsets_host[u + 1] - offsets_host[u];
     if (len <= 0 || len % 4 != 0)
       return fail(e, CGVC_ERR_ARG, "utterance %d: length %lld (offsets %lld .. %lld) must be a positive multiple of 4", u, len,
                   offsets_host[u], offsets_host[u + 1]);
-    if (len > max_len) max_len = len;
+    if (len > *max_len) *max_len = len;
   }
-  const long long rows = offsets_host[n], cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
-  if (rows > cap) return fail(e, CGVC_ERR_ARG, "%lld frames in all exceed the engine's capacity of max_batch x max_frames = %lld", rows, cap);
+  *rows = offsets_host[n];
+  const long long cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
+  if (*rows > cap) return fail(e, CGVC_ERR_ARG, "%lld frames in all exceed the engine's capacity of max_batch x max_frames = %lld", *rows, cap);
+  return 0;
+}
+
+int cgvc_generator_forward_packed(cgvc_handle e, int direction, const float* in_dev, float* out_dev,
+                                  const long long* offsets_host, int n, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  long long rows, max_len;
+  RET(packed_args(e, direction, in_dev, out_dev, offsets_host, n, &rows, &max_len));
   RET(need_arenas(e, false));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -2601,11 +2634,20 @@ int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const fl
 // ---- activation tapes: the forward of one network application that records what its backward reads, and that backward ------------
 // Layout: the TapeHeader in the first kTapeHead bytes, then the network's input (generator: channels-last [B, T, 24]; discriminator:
 // [B, 24, T]) and the activations of plan_generator / plan_discriminator for (batch, frames), as a train step keeps them.  kind 0 the
-// generator, 1 the discriminator.  Returns the bytes the plan needs; g / d / x receive it at base (base may be null for sizing)
-static size_t tape_plan(cgvc_engine* e, int kind, void* base, int batch, int frames, GenActs* g, DiscActs* d, float** x) {
+// generator, 1 the discriminator.  Kind 2, the packed generator (batch = n utterances, frames = rows = offsets[n]): the n + 1 frame
+// offsets (*off; the forward copies them there, so that a later call that reuses WORK cannot change what the backward reads), the
+// channels-last input [rows, 24] and plan_generator_rows(n, rows).  Returns the bytes the plan needs; g / d / x receive it at base
+// (base may be null for sizing)
+static size_t tape_plan(cgvc_engine* e, int kind, void* base, int batch, int frames, GenActs* g, DiscActs* d, float** x,
+                        long long** off = nullptr) {
   Bump ws; ws.reset((char*)base + kTapeHead, (size_t)1 << 62);
-  *x = ws.take<float>((size_t)batch * e->cfg.num_features * frames);
+  if (kind == 2) {
+    long long* o = ws.take<long long>((size_t)batch + 1);
+    if (off) *off = o;
+  }
+  *x = ws.take<float>((size_t)(kind == 2 ? 1 : batch) * e->cfg.num_features * frames);
   if (kind == 0) plan_generator(e, ws, *g, batch, frames);
+  else if (kind == 2) plan_generator_rows(e, ws, *g, batch, frames);
   else plan_discriminator(e, ws, *d, batch, frames);
   return kTapeHead + ws.off;
 }
@@ -2643,8 +2685,9 @@ static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const
     return fail(e, CGVC_ERR_ARG, "%p is not a tape written by this engine's cgvc_*_forward_tape since its parameters last changed", tape);
   *hd = it->second;
   if (hd->gen != e->param_gen) return fail(e, CGVC_ERR_ARG, "stale tape: the parameters changed after its forward");
-  if (hd->kind != kind)
-    return fail(e, CGVC_ERR_ARG, "a %s tape given to the %s backward", hd->kind ? "discriminator" : "generator", kind ? "discriminator" : "generator");
+  static const char* const names[3] = {"generator", "discriminator", "packed generator"};
+  if ((hd->kind == 1) != (kind == 1))        // the generator backward takes kinds 0 and 2
+    return fail(e, CGVC_ERR_ARG, "a %s tape given to the %s backward", names[hd->kind], names[kind]);
   if (!e->cfg.train || !e->arena[CGVC_ARENA_GRAD])
     return fail(e, CGVC_ERR_UNBOUND, "a tape backward needs the GRAD arena and a WORK arena sized for training (train = 1)");
   RET(need_arenas(e, true));
@@ -2666,8 +2709,16 @@ struct TapeCounting {
 extern "C" {
 
 int cgvc_tape_bytes(cgvc_handle e, int kind, int batch, int frames, size_t* bytes) {
-  if (!e || !bytes || (kind != 0 && kind != 1)) return fail(e, CGVC_ERR_ARG, "cgvc_tape_bytes: bad argument");
-  RET(check_bt(e, batch, frames, kind == 0 ? 4 : 16));
+  if (!e || !bytes || kind < 0 || kind > 2) return fail(e, CGVC_ERR_ARG, "cgvc_tape_bytes: bad argument");
+  if (kind == 2) {
+    // batch = n utterances, frames = rows = offsets[n]: the limits of cgvc_generator_forward_packed
+    const long long cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
+    if (batch < 1 || batch > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", batch, e->cfg.max_batch);
+    if (frames < 4 * (long long)batch || frames % 4 || frames > cap)
+      return fail(e, CGVC_ERR_ARG, "%d frames of %d utterances: must be a multiple of 4 in [%d, %lld]", frames, batch, 4 * batch, cap);
+  } else {
+    RET(check_bt(e, batch, frames, kind == 0 ? 4 : 16));
+  }
   GenActs g; DiscActs d; float* x;
   *bytes = tape_plan(e, kind, nullptr, batch, frames, &g, &d, &x);
   return 0;
@@ -2687,6 +2738,32 @@ int cgvc_generator_forward_tape(cgvc_handle e, int direction, const float* in_de
   CK(launch_transpose_ft(in_dev, x_cl, batch, e->cfg.num_features, frames, st));
   RET(generator_forward(e, e->gen[direction], A, x_cl, st, false, true));
   CK(launch_transpose_ft(A.out_cl, out_dev, batch, frames, e->cfg.num_features, st));
+  return tape_record(e, tape_dev, hd, st);
+}
+
+int cgvc_generator_forward_packed_tape(cgvc_handle e, int direction, const float* in_dev, float* out_dev, const long long* offsets_host, int n,
+                                       void* tape_dev, size_t tape_bytes, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  long long rows, max_len;
+  RET(packed_args(e, direction, in_dev, out_dev, offsets_host, n, &rows, &max_len));
+  if (!tape_dev) return fail(e, CGVC_ERR_ARG, "null buffer");
+  if ((uintptr_t)tape_dev & 255) return fail(e, CGVC_ERR_ARG, "a tape must be 256-byte aligned");
+  RET(need_arenas(e, false));
+  GenActs A; DiscActs D; float* x_cl; long long* off_dev;
+  const size_t need = tape_plan(e, 2, nullptr, n, (int)rows, &A, &D, &x_cl, &off_dev);
+  if (tape_bytes < need)
+    return fail(e, CGVC_ERR_UNBOUND, "tape of %zu bytes, %d utterances of %lld frames in all need %zu", tape_bytes, n, rows, need);
+  TapeHeader hd{kTapeMagic, e->id, e->param_gen, 2, direction, n, 0, rows, (int)max_len};
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nf = e->cfg.num_features;
+  tape_plan(e, 2, tape_dev, n, (int)rows, &A, &D, &x_cl, &off_dev);
+  A.off = off_dev; A.max_len = (int)max_len;
+  CK(grow_post_buf(e, (size_t)n * 4 * 1024, &A.post));
+  CK(cudaMemcpyAsync(off_dev, offsets_host, ((size_t)n + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CK(launch_transpose_packed(in_dev, x_cl, off_dev, n, rows, nf, 1, st));
+  RET(generator_forward(e, e->gen[direction], A, x_cl, st, false, true));
+  CK(launch_transpose_packed(A.out_cl, out_dev, off_dev, n, rows, nf, 0, st));
   return tape_record(e, tape_dev, hd, st);
 }
 
@@ -2714,21 +2791,27 @@ int cgvc_generator_backward_tape(cgvc_handle e, const void* tape_dev, const floa
   RET(tape_backward_entry(e, 0, tape_dev, dout_dev, &hd, &L));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  const int B = hd.batch, T = hd.frames, nf = e->cfg.num_features;
-  const long long img = (long long)B * nf * T;
-  GenActs A; DiscActs D; float* x_cl;
-  tape_plan(e, 0, const_cast<void*>(tape_dev), B, T, &A, &D, &x_cl);
+  // kind 2 (packed): B utterances of rows frames in all, in the packed [24][len_u] blocks of cgvc_generator_forward_packed
+  const bool pk = hd.kind == 2;
+  const int B = hd.batch, T = pk ? (int)hd.rows : hd.frames, nf = e->cfg.num_features;
+  const long long img = (long long)nf * (pk ? hd.rows : (long long)B * T);
+  GenActs A; DiscActs D; float* x_cl; long long* off = nullptr;
+  tape_plan(e, hd.kind, const_cast<void*>(tape_dev), B, T, &A, &D, &x_cl, &off);
   A.x_cl = x_cl; A.post = L.S.post;
-  // the upstream gradient channels-last, times the loss scale of the F16F8 gradient planes (a power of two: exact)
+  if (pk) { A.off = off; A.max_len = hd.max_len; }
+  // the upstream gradient channels-last, times the loss scale of the F16F8 gradient planes (a power of two: exact); a packed tape of B
+  // utterances takes the scale of a batch of B
   const float s = loss_scale(e, B);
-  CK(launch_transpose_ft(dout_dev, L.d_out, B, nf, T, st));
+  if (pk) CK(launch_transpose_packed(dout_dev, L.d_out, off, B, hd.rows, nf, 1, st));
+  else CK(launch_transpose_ft(dout_dev, L.d_out, B, nf, T, st));
   if (s != 1.f) CK(launch_scale(L.d_out, img, s, st));
   {
     TapeCounting counting(e, 0);
     RET(generator_backward(e, e->gen[hd.which], A, L.d_out, din_dev ? L.in : nullptr, L.S, st));
   }
   if (!din_dev) return 0;
-  CK(launch_transpose_ft(L.in, din_dev, B, T, nf, st));
+  if (pk) CK(launch_transpose_packed(L.in, din_dev, off, B, hd.rows, nf, 0, st));
+  else CK(launch_transpose_ft(L.in, din_dev, B, T, nf, st));
   if (s != 1.f) CK(launch_scale(din_dev, img, 1.f / s, st));
   return 0;
 }

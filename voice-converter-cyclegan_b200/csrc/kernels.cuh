@@ -186,9 +186,10 @@ cudaError_t launch_gg_simt(const GatherGeom& g, const GemmOperands& op, cudaStre
 // level's divisor; taps read only their own utterance's rows (TF-SAME zero padding at every utterance edge)
 cudaError_t launch_gg_simt_packed(const GatherGeom& g, const GemmOperands& op, const PackGeom& pk, cudaStream_t st);
 // weight gradient in forward geometry: dW[widx[t]][c][n] += sum_m S[src(m,t), c] * G[m, n]   (atomic accumulate)
+// pk: packed utterances, g and pk as launch_gg_simt_packed takes them; a tap outside its row's utterance contributes a zero row
 cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, int s_coff, int C,
                               const float* grad, int g_ld, int g_coff, int N,
-                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det = 0);
+                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det = 0, const PackGeom* pk = nullptr);
 // db[n] += sum_m G[m, g_coff + n]
 cudaError_t launch_colsum(const float* grad, long long rows, int g_ld, int g_coff, int N, float* db, cudaStream_t st,
                           const DetSlab* det = nullptr);
@@ -234,7 +235,12 @@ struct PostBwdParams {
   unsigned long long* ufl;              // qmode: [ufl, groups] of the planes (cgvc_count_planes), or null
   DetSlab det;                          // deterministic mode (det.p != null): the sums + apply form, parameter and bias gradients reduced in order
 };
-cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st);
+// Packed variable-length samples of launch_post_bwd (instance-normed layers; the sums + apply form only): sample b = view rows
+// [seg.off[b] / seg.div, seg.off[b+1] / seg.div) of `rows` view rows in all, with its own statistics; PostBwdParams::B = seg.n and R =
+// the longest sample (grid size).  A kernel argument of the packed instantiations only: PostBwdParams, the parameter block of the
+// equal-length kernels, stays as it is
+struct PostBwdSeg { PackGeom seg; long long rows; };
+cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st, const PostBwdSeg* seg = nullptr);
 cudaError_t post_init_kernels();   // shared-memory opt-in of the streaming kernels (call once, outside any stream capture)
 
 // ---- discriminator head: dense(1024->1) + sigmoid (module.py:211) and LSGAN loss (model.py:68-69,81-86)

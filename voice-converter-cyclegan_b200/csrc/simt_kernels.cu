@@ -232,11 +232,15 @@ cudaError_t launch_gg_simt(const GatherGeom& g, const GemmOperands& op, cudaStre
 // ------------------------------------------------------------------------------------------------
 // weight gradient (forward geometry), split over rows with atomic accumulation into the GRAD arena
 // ------------------------------------------------------------------------------------------------
-template <bool VEC>
+// Packed variable-length utterances (launch_wgrad_simt with pk; VEC only): the instantiation with one trailing PackGeom argument.  Row m
+// (an output row of all packed rows) reads its source row from its own utterance; a tap outside it contributes a zero row.
+template <bool VEC, class... PKs>
 __global__ void __launch_bounds__(256)
 wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ src, int s_ld, int s_coff, int C,
                   const float* __restrict__ grad, int g_ld, int g_coff, int N,
-                  float* __restrict__ dw, long long w_ts, int w_cs, int w_ns, int ksplit) {
+                  float* __restrict__ dw, long long w_ts, int w_cs, int w_ns, int ksplit, const PKs... pks) {
+  constexpr bool PK = sizeof...(PKs) > 0;
+  static_assert(VEC || !PK, "the packed form reads 4-channel quads");
   __shared__ __align__(16) float As[16][64 + 4];
   __shared__ __align__(16) float Gs[16][64 + 4];
   const int tid = threadIdx.x;
@@ -261,6 +265,15 @@ wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict_
     long long m = mb + lrow;
     float4 av = make_float4(0.f, 0.f, 0.f, 0.f), gv = make_float4(0.f, 0.f, 0.f, 0.f);
     if (m < mend) {
+      if constexpr (PK) {
+        const PackGeom& pk = pack_arg(pks...);
+        const int dout = pk.div * g.sx;
+        const int u = pack_find(pk.off, pk.n, m * dout);
+        const long long o0 = __ldg(pk.off + u), o1 = __ldg(pk.off + u + 1);
+        const int xx = (int)(m - o0 / dout) * g.sx + g.ox[t];
+        if (xx >= 0 && xx < (int)((o1 - o0) / pk.div) && c0 + lq < C)
+          av = *reinterpret_cast<const float4*>(src + (o0 / pk.div + xx) * s_ld + s_coff + c0 + lq);
+      } else {
       int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
       int y = rem / g.Wx; int x = rem - y * g.Wx;
       int yy = y * g.sy + g.oy[t], xx = x * g.sx + g.ox[t];
@@ -273,6 +286,7 @@ wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict_
           if (c0 + lq + 2 < C) av.z = sp[c0 + lq + 2];
           if (c0 + lq + 3 < C) av.w = sp[c0 + lq + 3];
         }
+      }
       }
       const float* gp = grad + m * g_ld + g_coff;
       if (VEC) { if (n0 + lq < N) gv = *reinterpret_cast<const float4*>(gp + n0 + lq); }
@@ -313,9 +327,10 @@ wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict_
 
 cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, int s_coff, int C,
                               const float* grad, int g_ld, int g_coff, int N,
-                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det) {
+                              float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det, const PackGeom* pk) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
+  if (pk && (!pk->off || g.B != 1 || g.Hy != 1 || g.Hs != 1)) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
   int tiles = ((N + 63) / 64) * ((C + 63) / 64) * g.ntaps;
   int ksplit = det ? 1 : (592 + tiles - 1) / tiles;       // det: one CTA, one thread and one add per element
@@ -326,7 +341,11 @@ cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, i
   dim3 grid((N + 63) / 64, (C + 63) / 64, g.ntaps * ksplit);
   bool vec = (C % 4 == 0) && (N % 4 == 0) && (s_ld % 4 == 0) && (s_coff % 4 == 0) && (g_ld % 4 == 0) && (g_coff % 4 == 0) &&
              ((reinterpret_cast<uintptr_t>(src) & 15) == 0) && ((reinterpret_cast<uintptr_t>(grad) & 15) == 0);
-  if (vec) wgrad_simt_kernel<true><<<grid, 256, 0, st>>>(g, src, s_ld, s_coff, C, grad, g_ld, g_coff, N, dw, w_ts, w_cs, w_ns, ksplit);
+  if (pk) {
+    if (!vec) return cudaErrorInvalidValue;
+    wgrad_simt_kernel<true, PackGeom><<<grid, 256, 0, st>>>(g, src, s_ld, s_coff, C, grad, g_ld, g_coff, N, dw, w_ts, w_cs, w_ns, ksplit, *pk);
+  }
+  else if (vec) wgrad_simt_kernel<true><<<grid, 256, 0, st>>>(g, src, s_ld, s_coff, C, grad, g_ld, g_coff, N, dw, w_ts, w_cs, w_ns, ksplit);
   else     wgrad_simt_kernel<false><<<grid, 256, 0, st>>>(g, src, s_ld, s_coff, C, grad, g_ld, g_coff, N, dw, w_ts, w_cs, w_ns, ksplit);
   return cudaGetLastError();
 }
@@ -650,14 +669,34 @@ cudaError_t launch_post_fwd(const PostParams& pp, PostForms forms, cudaStream_t 
 
 // ---- backward (SURVEY.md Appendix A.7) ----
 // scratch[b][q][c], q = 0..3: S1a = sum dna, S2a = sum dna*ahat, S1g, S2g; also accumulates dgamma / dbeta
-template <bool HAS_GATE>
+// Packed variable-length samples (launch_post_bwd with a PostBwdSeg): the instantiations with one trailing PostBwdSeg argument, whose
+// sample b is view rows [s0, s0 + R) of post_bwd_seg and has its own statistics.  The equal-length instantiations take no such argument.
+// Sample b's first view row, its view rows, its first conv row (Rw: conv rows per equal-length sample) and the rows of the planes.
+template <class... Seg> __device__ __forceinline__ long long bwd_first(const PostBwdParams& q, int b, const Seg&... sg) {
+  if constexpr (sizeof...(Seg) > 0) { const PostBwdSeg& s = (sg, ...); return s.seg.off[b] / s.seg.div; }
+  else return (long long)b * q.R;
+}
+template <class... Seg> __device__ __forceinline__ int bwd_len(const PostBwdParams& q, int b, const Seg&... sg) {
+  if constexpr (sizeof...(Seg) > 0) { const PostBwdSeg& s = (sg, ...); return (int)((s.seg.off[b + 1] - s.seg.off[b]) / s.seg.div); }
+  else return q.R;
+}
+template <class... Seg> __device__ __forceinline__ long long bwd_conv0(const PostBwdParams& q, int b, int Rw, const Seg&... sg) {
+  if constexpr (sizeof...(Seg) > 0) return bwd_first(q, b, sg...) / q.sh;         // a multiple of sh: whole conv rows
+  else return (long long)b * Rw;
+}
+template <class... Seg> __device__ __forceinline__ long long bwd_conv_rows(const PostBwdParams& q, int Rw, const Seg&... sg) {
+  if constexpr (sizeof...(Seg) > 0) { const PostBwdSeg& s = (sg, ...); return s.rows / q.sh; }
+  else return (long long)q.B * Rw;
+}
+
+template <bool HAS_GATE, class... Seg>
 __global__ void __launch_bounds__(256)
-post_bwd_sums_kernel(const __grid_constant__ PostBwdParams q, float* __restrict__ scratch) {
+post_bwd_sums_kernel(const __grid_constant__ PostBwdParams q, float* __restrict__ scratch, const Seg... sg) {
   __shared__ float4 red[8][32];
   const PostIdx ix(q.C);
   const int lane = threadIdx.x & 31;
   const int Rw = q.R / q.sh;
-  const float* pb = q.p + (long long)ix.b * Rw * q.ldp;
+  const float* pb = q.p + bwd_conv0(q, ix.b, Rw, sg...) * q.ldp;
   F4 acc[4] = {zero4(), zero4(), zero4(), zero4()};
   if (ix.cvalid) {
     // per channel: xhat = x*r + h ; norm = x*sc + of
@@ -675,10 +714,10 @@ post_bwd_sums_kernel(const __grid_constant__ PostBwdParams q, float* __restrict_
     }
     const int shs = q.sh - 1;
 #pragma unroll 2
-    for (int r = ix.rl; r < q.R; r += 8) {               // whole position range in one CTA (grid.y == 1): deterministic
+    for (int r = ix.rl; r < bwd_len(q, ix.b, sg...); r += 8) {   // whole position range in one CTA (grid.y == 1): deterministic
       const int w = r >> shs, s = r & shs;
       const long long a = (long long)w * q.ldp + s * q.C + ix.c;
-      const long long o = ((long long)ix.b * q.R + r) * q.C + ix.c;
+      const long long o = (bwd_first(q, ix.b, sg...) + r) * q.C + ix.c;
       F4 xa = ld4(pb + a), xg = HAS_GATE ? ld4(pb + a + q.Cc) : zero4(), dy = ld4(q.dy1 + o);
       if (q.dy2) { F4 d2 = ld4(q.dy2 + o);
 #pragma unroll
@@ -783,6 +822,117 @@ post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __re
         if (q.dp_hi) {
           if (q.qmode) {                                     // F16F8 gradient planes (activation-role scales): q16, then q8hi | q8lo
             const long long nq = (long long)q.B * Rw * q.ldp;
+            st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da);
+            if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg);
+            if (q.sat) nsat += sat_groups(da, dg, HAS_GATE);
+            if (q.ufl) { nufl += ufl_groups(da, dg, HAS_GATE); ngrp += HAS_GATE ? 2 : 1; }
+          } else {
+            st4_split(q.dp_hi + dpoff + a, q.dp_lo + dpoff + a, da);
+            if (HAS_GATE) st4_split(q.dp_hi + dpoff + a + q.Cc, q.dp_lo + dpoff + a + q.Cc, dg);
+          }
+        }
+      }
+    }
+  }
+  if (q.sat) cgvc_count_hits(q.sat, nsat);
+  if (q.ufl) { cgvc_count_hits(q.ufl, nufl); cgvc_count_hits(q.ufl + 1, ngrp); }
+  if (q.dbias_a) {
+    // positions of lane rl have shuffle phase rl % sh (chunk size and lane stride are even): reduce per phase
+    red[0][ix.rl][lane] = make_float4(bsum[0].v[0], bsum[0].v[1], bsum[0].v[2], bsum[0].v[3]);
+    red[1][ix.rl][lane] = make_float4(bsum[1].v[0], bsum[1].v[1], bsum[1].v[2], bsum[1].v[3]);
+    __syncthreads();
+    if (ix.rl < q.sh && ix.cvalid) {
+#pragma unroll
+      for (int br = 0; br < 2; ++br) {
+        float* db = br == 0 ? q.dbias_a : q.dbias_g;
+        if (!db || (br == 1 && !HAS_GATE)) continue;
+        F4 t = zero4();
+        for (int w = ix.rl; w < 8; w += q.sh) { float4 v = red[br][w][lane]; t.v[0] += v.x; t.v[1] += v.y; t.v[2] += v.z; t.v[3] += v.w; }
+        if (q.det.p) st4(q.det.p + ((long long)blockIdx.z * gridDim.y + blockIdx.y) * 2 * q.Cc + br * q.Cc + ix.rl * q.C + ix.c, t);
+        else atomic_add4(db + ix.rl * q.C + ix.c, t);
+      }
+    }
+  }
+}
+
+// The packed form of post_apply_bwd_kernel (instance-normed layers only): sample b = view rows [bwd_first, + bwd_len) of seg, with its
+// own statistics and sums.  An overload of its own, so that the equal-length instantiations keep their code
+template <bool HAS_GATE>
+__global__ void __launch_bounds__(256)
+post_apply_bwd_kernel(const __grid_constant__ PostBwdParams q, const float* __restrict__ scratch, const PostBwdSeg sg) {
+  constexpr bool HAS_IN = true;
+  __shared__ float4 red[2][8][32];
+  const PostIdx ix(q.C);
+  const int lane = threadIdx.x & 31;
+  const int Rw = q.R / q.sh;
+  // past the end of a shorter sample: nothing to do, except in deterministic mode, where every (sample, block) row of bias partials
+  // is written (zeros here)
+  if ((int)blockIdx.y * kPostRows >= bwd_len(q, ix.b, sg) && !q.det.p) return;
+  const float* pb = q.p + bwd_conv0(q, ix.b, Rw, sg) * q.ldp;
+  const long long dpoff = bwd_conv0(q, ix.b, Rw, sg) * q.ldp;
+  F4 bsum[2] = {zero4(), zero4()};                      // this thread's share of the conv-bias gradients (a, g)
+  unsigned nsat = 0, nufl = 0, ngrp = 0;                 // plane groups counted for q.sat / q.ufl, added to the counters after the loop
+  if (ix.cvalid) {
+    // per channel (Appendix A.7):  xhat = x*r + h ; norm = x*sc + of ; dx = c1*dn - c2 - xhat*c3
+    F4 ra = one4(), ha = zero4(), sca = one4(), ofa = zero4(), c1a = one4(), c2a = zero4(), c3a = zero4();
+    F4 rg = one4(), hg = zero4(), scg = one4(), ofg = zero4(), c1g = one4(), c2g = zero4(), c3g = zero4();
+    if (HAS_IN) {
+      const float* st = q.stats + (long long)ix.b * 4 * q.C + ix.c;
+      const float* sc = scratch + (long long)ix.b * 4 * q.C + ix.c;
+      const float invR = 1.f / (float)bwd_len(q, ix.b, sg);
+      {
+        F4 mean = ld4(st), rstd = ld4(st + q.C), gam = ld4(q.gamma_a + ix.c), bet = ld4(q.beta_a + ix.c), S1 = ld4(sc), S2 = ld4(sc + q.C);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          ra.v[k] = rstd.v[k]; ha.v[k] = -mean.v[k] * rstd.v[k];
+          sca.v[k] = rstd.v[k] * gam.v[k]; ofa.v[k] = bet.v[k] - mean.v[k] * sca.v[k];
+          c1a.v[k] = sca.v[k]; c2a.v[k] = sca.v[k] * S1.v[k] * invR; c3a.v[k] = sca.v[k] * S2.v[k] * invR;
+        }
+      }
+      if (HAS_GATE) {
+        F4 mean = ld4(st + 2 * q.C), rstd = ld4(st + 3 * q.C), gam = ld4(q.gamma_g + ix.c), bet = ld4(q.beta_g + ix.c), S1 = ld4(sc + 2 * q.C), S2 = ld4(sc + 3 * q.C);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          rg.v[k] = rstd.v[k]; hg.v[k] = -mean.v[k] * rstd.v[k];
+          scg.v[k] = rstd.v[k] * gam.v[k]; ofg.v[k] = bet.v[k] - mean.v[k] * scg.v[k];
+          c1g.v[k] = scg.v[k]; c2g.v[k] = scg.v[k] * S1.v[k] * invR; c3g.v[k] = scg.v[k] * S2.v[k] * invR;
+        }
+      }
+    }
+    const int shs = q.sh - 1;
+#pragma unroll
+    for (int i = 0; i < kPostRows / 8; ++i) {
+      const int r = ix.r0 + 8 * i;
+      if (r < bwd_len(q, ix.b, sg)) {
+        const int w = r >> shs, s = r & shs;
+        const long long a = (long long)w * q.ldp + s * q.C + ix.c;
+        const long long o = (bwd_first(q, ix.b, sg) + r) * q.C + ix.c;
+        F4 xa = ld4(pb + a), xg = HAS_GATE ? ld4(pb + a + q.Cc) : zero4(), dy = ld4(q.dy1 + o), da, dg = zero4();
+        if (q.dy2) { F4 d2 = ld4(q.dy2 + o);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) dy.v[k] += d2.v[k]; }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float dna = dy.v[k], dng = 0.f;
+          if (HAS_GATE) {
+            float na = HAS_IN ? fmaf(xa.v[k], sca.v[k], ofa.v[k]) : xa.v[k];
+            float ng = HAS_IN ? fmaf(xg.v[k], scg.v[k], ofg.v[k]) : xg.v[k];
+            float sg = sigmoidf_(ng);
+            dna = dy.v[k] * sg;
+            dng = dna * na * (1.f - sg);                          // dy * na * s * (1 - s)
+          }
+          float a_ = dna, g_ = dng;
+          if (HAS_IN) {
+            float ah = fmaf(xa.v[k], ra.v[k], ha.v[k]);
+            a_ = fmaf(c1a.v[k], dna, -fmaf(ah, c3a.v[k], c2a.v[k]));
+            if (HAS_GATE) { float gh = fmaf(xg.v[k], rg.v[k], hg.v[k]); g_ = fmaf(c1g.v[k], dng, -fmaf(gh, c3g.v[k], c2g.v[k])); }
+          }
+          da.v[k] = a_; dg.v[k] = g_; bsum[0].v[k] += a_; bsum[1].v[k] += g_;
+        }
+        if (q.dp) { st4(q.dp + dpoff + a, da); if (HAS_GATE) st4(q.dp + dpoff + a + q.Cc, dg); }
+        if (q.dp_hi) {
+          if (q.qmode) {                                     // F16F8 gradient planes (activation-role scales): q16, then q8hi | q8lo
+            const long long nq = bwd_conv_rows(q, Rw, sg) * q.ldp;
             st4_quant(q.dp_hi, q.dp_lo, dpoff + a, nq, da);
             if (HAS_GATE) st4_quant(q.dp_hi, q.dp_lo, dpoff + a + q.Cc, nq, dg);
             if (q.sat) nsat += sat_groups(da, dg, HAS_GATE);
@@ -1323,7 +1473,7 @@ static bool post_bwd_stream_dispatch(const PostBwdParams& pp, PostForms forms, c
 }
 
 
-cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st) {
+cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream_t st, const PostBwdSeg* seg) {
   if (pp.B == 0) return cudaSuccess;
   if (!post_aligned(pp.p, pp.dy1, pp.dy2, pp.ldp, pp.C, pp.Cc) || (pp.sh != 1 && pp.sh != 2) || pp.B > 65535 || (pp.has_in && !pp.scratch))
     return cudaErrorInvalidValue;
@@ -1333,8 +1483,12 @@ cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream
   const bool det = pp.det.p != nullptr;
   const bool det_bias = det && pp.dbias_a;
   if (det_bias && (long long)pp.B * grid.y * 2 * pp.Cc > pp.det.cap) return cudaErrorInvalidValue;
-  if (!det) { cudaError_t se = cudaSuccess; if (post_bwd_stream_dispatch(pp, forms, st, &se)) return se; }
-  if (!det && pp.has_in && pp.R <= 64 && forms.onepass) {
+  // packed variable-length samples (seg): the sums + apply form only, one CTA column per sample, grid.y sized by the longest; samples
+  // start on whole conv rows (off[u] / div % sh == 0)
+  const bool pk = seg && seg->seg.off;
+  if (pk && (!pp.has_in || seg->seg.div < 1 || 4 % (seg->seg.div * pp.sh) || seg->seg.n != pp.B)) return cudaErrorInvalidValue;
+  if (!det && !pk) { cudaError_t se = cudaSuccess; if (post_bwd_stream_dispatch(pp, forms, st, &se)) return se; }
+  if (!det && !pk && pp.has_in && pp.R <= 64 && forms.onepass) {
     ++g_cgvc_launches;
     const dim3 g1(grid.x, 1, grid.z);
 #define ONEPASS(NR_) do { if (pp.has_gate) post_bwd_onepass_kernel<true, NR_><<<g1, 256, 0, st>>>(pp); else post_bwd_onepass_kernel<false, NR_><<<g1, 256, 0, st>>>(pp); } while (0)
@@ -1345,7 +1499,9 @@ cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream
   float* scratch = pp.scratch;
   if (pp.has_in) {
     ++g_cgvc_launches;
-    if (pp.has_gate) post_bwd_sums_kernel<true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
+    if (pk) { if (pp.has_gate) post_bwd_sums_kernel<true, PostBwdSeg><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch, *seg);
+              else post_bwd_sums_kernel<false, PostBwdSeg><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch, *seg); }
+    else if (pp.has_gate) post_bwd_sums_kernel<true><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
     else post_bwd_sums_kernel<false><<<dim3(grid.x, 1, grid.z), 256, 0, st>>>(pp, scratch);
     if (det && pp.dgamma_a) {                            // scratch[b] = [S1a | S2a | S1g | S2g] = sample b's dbeta_a, dgamma_a, dbeta_g, dgamma_g
       const long long C = pp.C, g = pp.has_gate ? C : 0;
@@ -1354,7 +1510,9 @@ cudaError_t launch_post_bwd(const PostBwdParams& pp, PostForms forms, cudaStream
     }
   }
   ++g_cgvc_launches;
-  if (pp.has_in) { if (pp.has_gate) post_apply_bwd_kernel<true, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_bwd_kernel<true, false><<<grid, 256, 0, st>>>(pp, scratch); }
+  if (pk) { if (pp.has_gate) post_apply_bwd_kernel<true><<<grid, 256, 0, st>>>(pp, scratch, *seg);
+            else post_apply_bwd_kernel<false><<<grid, 256, 0, st>>>(pp, scratch, *seg); }
+  else if (pp.has_in) { if (pp.has_gate) post_apply_bwd_kernel<true, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_bwd_kernel<true, false><<<grid, 256, 0, st>>>(pp, scratch); }
   else           { if (pp.has_gate) post_apply_bwd_kernel<false, true><<<grid, 256, 0, st>>>(pp, scratch); else post_apply_bwd_kernel<false, false><<<grid, 256, 0, st>>>(pp, scratch); }
   if (!det_bias) return cudaGetLastError();
   const long long Cc = pp.Cc;

@@ -222,6 +222,8 @@ struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[
   int fold_n;                                            // != 0: tap-folded layer (TcLayer::fold): column = t * fold_n + n of a [taps][C][fold_n] TF kernel
   // deterministic form (DET): split k stores its partial tile to part + k * part_k, laid out like [dw_a | dw_g] (dw_g at numel_a)
   float* part; long long part_k, numel_a;
+  // packed variable-length utterances (the PK kernels): g is the 1-D forward geometry of all rows, pk.div the source level's divisor
+  PackGeom pk;
 };
 
 // address of weight-gradient element (tap slab, channel c, column col) in the TF-layout kernel [taps][C][ncols]; with fold_n the layer's
@@ -1079,7 +1081,9 @@ struct TNCfg {
 // concurrently running CTAs share the same rows of X and dP in L2).  Each consumer warpgroup owns 64 of the 128 channels.
 // DET (deterministic mode, ksplit > 1): the fragments are stored to the K-split's partial slab instead of added into dW; launch_tn then
 // adds the partials in K-split order (launch_reduce_parts)
-template <int NPL, int W16, int DET>
+// PK: the packed form (packed generator tapes).  K-row m (an output row of all packed rows) gathers its source row from its own
+// utterance u = pack_find(m * dout): local position (m - off[u] / dout) * stride + tap offset, a zero row outside [0, len_u / div)
+template <int NPL, int W16, int DET, bool PK = false>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   static_assert(W16 == 0 || NPL == 3, "the fp16-only weight gradient is a form of CGVC_PREC_F16F8");
@@ -1139,12 +1143,20 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
           const long long m = w.mbeg + (long long)kb * 64 + rsub + 16 * i;
           xoff[i] = -1;
           if (m < w.mend) {
-            const uint32_t mu = (uint32_t)m;
-            int b = (int)fdiv(mu, p.div_hw); int rem = (int)(mu - (uint32_t)b * (uint32_t)HW);
-            int y = (int)fdiv((uint32_t)rem, p.div_w); int x = rem - y * g.Wx;
-            int yy = y * g.sy + g.oy[w.tap], xx = x * g.sx + g.ox[w.tap];
-            if (yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws)
-              xoff[i] = ((long long)(b * g.Hs + yy) * g.Ws + xx) * p.x_ld + w.c0 + chunk * 8;
+            if constexpr (PK) {
+              const int dout = p.pk.div * g.sx;
+              const int u = pack_find(p.pk.off, p.pk.n, m * dout);
+              const long long o0 = __ldg(p.pk.off + u), o1 = __ldg(p.pk.off + u + 1);
+              const int xx = (int)(m - o0 / dout) * g.sx + g.ox[w.tap];
+              if (xx >= 0 && xx < (int)((o1 - o0) / p.pk.div)) xoff[i] = (o0 / p.pk.div + xx) * p.x_ld + w.c0 + chunk * 8;
+            } else {
+              const uint32_t mu = (uint32_t)m;
+              int b = (int)fdiv(mu, p.div_hw); int rem = (int)(mu - (uint32_t)b * (uint32_t)HW);
+              int y = (int)fdiv((uint32_t)rem, p.div_w); int x = rem - y * g.Wx;
+              int yy = y * g.sy + g.oy[w.tap], xx = x * g.sx + g.ox[w.tap];
+              if (yy >= 0 && yy < g.Hs && xx >= 0 && xx < g.Ws)
+                xoff[i] = ((long long)(b * g.Hs + yy) * g.Ws + xx) * p.x_ld + w.c0 + chunk * 8;
+            }
           }
         }
         if (NPL == 3 && pass == 0) {
@@ -1544,13 +1556,24 @@ cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st, const DetSla
   cudaError_t e;
   ++g_cgvc_launches;
   prof_begin(st, 2.0 * (double)M * p.N * p.g.ntaps * p.C, 1, M, p.N, p.g.ntaps * p.C);
-#define LAUNCH_TN(NPL_, W16_, DET_)                                                               \
-  do {                                                                                            \
-    e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_>, TNCfg<NPL_, W16_>::SMEM);                     \
-    if (e != cudaSuccess) return e;                                                               \
-    tc_gg_tn_kernel<NPL_, W16_, DET_><<<grid, kNTThreads, TNCfg<NPL_, W16_>::SMEM, st>>>(p);      \
+#define LAUNCH_TN(NPL_, W16_, DET_, ...)                                                                      \
+  do {                                                                                                        \
+    e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_, ##__VA_ARGS__>, TNCfg<NPL_, W16_>::SMEM);                  \
+    if (e != cudaSuccess) return e;                                                                           \
+    tc_gg_tn_kernel<NPL_, W16_, DET_, ##__VA_ARGS__><<<grid, kNTThreads, TNCfg<NPL_, W16_>::SMEM, st>>>(p);   \
   } while (0)
-  if (det_split) {
+  if (p.pk.off) {                                           // packed utterances
+    if (p.g.B != 1 || p.g.Hy != 1) return cudaErrorInvalidValue;
+    if (det_split) {
+      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1, true); else LAUNCH_TN(3, 0, 1, true); }
+      else if (precision == 1) LAUNCH_TN(2, 0, 1, true);
+      else                     LAUNCH_TN(1, 0, 1, true);
+    } else {
+      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 0, true); else LAUNCH_TN(3, 0, 0, true); }
+      else if (precision == 1) LAUNCH_TN(2, 0, 0, true);
+      else                     LAUNCH_TN(1, 0, 0, true);
+    }
+  } else if (det_split) {
     if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1); else LAUNCH_TN(3, 0, 1); }
     else if (precision == 1) LAUNCH_TN(2, 0, 1);
     else                     LAUNCH_TN(1, 0, 1);
@@ -1687,9 +1710,11 @@ int tc_conv_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16*
 
 // dP planes: [rows_out, nt_k]
 int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused_out) {
+                  float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused_out, const PackGeom* pk) {
   if (fused_out) *fused_out = false;
   if (!layer_ok(L) || (precision == 3 && (!layer_ok_q(L) || !L.wdq16))) return TC_UNSUPPORTED;     // F16F8 needs the data-gradient planes (training engines)
+  if (pk && (n != 1 || H != 1 || L.kh != 1)) return (int)cudaErrorInvalidValue;
+  if (pk) fuse = nullptr;
   std::vector<GatherGeom> gs = dgrad_geoms(n, H, W, L.kh, L.kw, sh, sw);
   for (const GatherGeom& g : gs) if (g.ntaps == 0) return TC_UNSUPPORTED;     // (never the case for this model's layers)
   // fused backward epilogue: stride-1 1-D layer (one geometry, dense rows), whole samples per 128-row tile, 256-wide tiles
@@ -1701,6 +1726,10 @@ int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat1
   for (const GatherGeom& g : gs) {
     TcNTParams p; memset(&p, 0, sizeof p);
     p.g = g;
+    if (pk) {
+      // packed: every class reads dP at the output level, of divisor pk->div * sw (see DESIGN.md section 12 for the parity classes)
+      p.pk = *pk; p.pk.div = pk->div * sw;
+    }
     p.a_hi = dPhi; p.a_lo = dPlo; p.a_ld = nt_k(L); p.C = nt_k(L);
     p.b_hi = L.wd_hi; p.b_lo = L.wd_lo; p.Nw = cin_n(L); p.N = L.cin;
     p.dst = dx; p.d_ld = L.cin; p.bias = nullptr; p.accumulate = accumulate;
@@ -1726,9 +1755,11 @@ int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat1
 
 int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det) {
+                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det, const PackGeom* pk) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
+  if (pk && (n != 1 || H != 1 || L.kh != 1)) return (int)cudaErrorInvalidValue;
   TcTNParams p; memset(&p, 0, sizeof p);
+  if (pk) p.pk = *pk;
   p.w16 = (precision == 3 && w16) ? 1 : 0;
   p.fold_n = L.fold ? L.cout / L.fold : 0;
   p.g = fwd_geom(n, H, W, L.kh, L.kw, sh, sw);
@@ -1842,6 +1873,10 @@ static cudaError_t tc_init_kernels() {
 #define INIT_TN(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
   INIT_TN(3, 1, 0) INIT_TN(3, 0, 0) INIT_TN(2, 0, 0) INIT_TN(1, 0, 0)
   INIT_TN(3, 1, 1) INIT_TN(3, 0, 1) INIT_TN(2, 0, 1) INIT_TN(1, 0, 1)
+#define INIT_TN_PK(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_, true>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
+  INIT_TN_PK(3, 1, 0) INIT_TN_PK(3, 0, 0) INIT_TN_PK(2, 0, 0) INIT_TN_PK(1, 0, 0)
+  INIT_TN_PK(3, 1, 1) INIT_TN_PK(3, 0, 1) INIT_TN_PK(2, 0, 1) INIT_TN_PK(1, 0, 1)
+#undef INIT_TN_PK
 #undef INIT_TN
   return cudaSuccess;
 }

@@ -107,12 +107,17 @@ int tc_conv_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16*
 //   fuse: the upstream layer's instance-norm (+ GLU) backward fused into the epilogue when the shape allows (stride-1 1-D layer,
 //         whole samples per 128-row tile): the launch then writes that layer's dP planes (and, for gated = 0, dx = dY) instead
 //         of / besides dx; *fused tells whether it happened (if not, dx holds the plain data gradient).
+//   pk:   packed utterances as in tc_conv_fwd, pk->div the divisor of the INPUT level; plain epilogue only (fuse is ignored)
 int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W,
-                  int sh, int sw, float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr);
+                  int sh, int sw, float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse = nullptr, bool* fused = nullptr,
+                  const PackGeom* pk = nullptr);
 // dW_a/dW_g (TF layout) += x^T dP  (the bias gradients are column sums of dP: the instance-norm backward kernels or launch_colsum)
+//   pk:   packed utterances as in tc_conv_fwd (x planes at the source level of divisor pk->div): a tap outside its row's utterance
+//         contributes a zero row
 int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
-                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det = nullptr);   // det: deterministic mode (kernels.cuh DetSlab)
+                  float* dwa, float* dwg, cudaStream_t st, const DetSlab* det = nullptr,   // det: deterministic mode (kernels.cuh DetSlab)
+                  const PackGeom* pk = nullptr);
 
 // per-launch CUDA-event timing of the tensor-core kernels (class 0 = forward/dgrad kernel with the plain epilogue,
 // 1 = wgrad kernel, 2 = forward kernel with the fused instance-norm epilogue)

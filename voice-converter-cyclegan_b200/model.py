@@ -21,7 +21,8 @@ Differences a user of the reference should know:
   * `generator(x, direction)` / `discriminator(x, which)` are the four networks as differentiable torch operators on CUDA tensors, for
     objectives other than the fused step's: `loss.backward()` adds their weight gradients into the gradient arena, `zero_grad()`,
     `grads()` and `adam_step()` complete a step (include/cgvc.h "activation tapes", DESIGN.md section 12).  The network descriptors
-    given to the constructor are `generator_descriptor` / `discriminator_descriptor`
+    given to the constructor are `generator_descriptor` / `discriminator_descriptor`; `generator_packed(inputs, direction)` is the
+    generator over a list of utterances of different lengths in one call, for utterance-level objectives
 """
 from __future__ import annotations
 
@@ -314,6 +315,20 @@ class CycleGAN(object):
             raise ValueError("which must be 'A' or 'B', got %r" % (which,))
         return _NetFn.apply(x, self._token(), self, 1, w)
 
+    def generator_packed(self, inputs, direction):
+        """Differentiable packed generator: inputs a list of CUDA tensors [24, T_i] (every T_i a positive multiple of 4) -> the list of
+        converted [24, T_i] tensors, bit for bit what test_packed() gives on them.  One engine call runs the forward of all utterances and
+        one their backward, which adds d loss / d (the generator's variables) into the gradient arena -- with the loss scale of a batch
+        of len(inputs), tape_loss_scale(len(inputs)) -- and returns d loss / d x_i for the inputs that require it.  Every convolution
+        tap, instance norm and edge-layer sum stays inside its own utterance, forward and backward.  direction 'A2B' or 'B2A'."""
+        d = {'A2B': 0, 'B2A': 1}.get(direction)
+        if d is None:
+            raise Exception('Conversion direction must be specified.')
+        inputs = list(inputs)
+        if not inputs:
+            return []
+        return list(_PackedGenFn.apply(self._token(), self, d, *inputs))
+
     def _token(self):
         # a leaf that requires grad, so that autograd runs a network's backward -- and with it the weight gradients -- even when its
         # input does not require grad (a real sample)
@@ -347,6 +362,32 @@ class CycleGAN(object):
             fn = self._lib.cgvc_discriminator_forward_tape
         self._chk(fn(self._handle, which, _ptr(x), _ptr(y), batch, frames, _ptr(tape), nbytes.value, self._stream()))
         return y, tape
+
+    def _packed_tape_forward(self, direction, xs):
+        for x in xs:
+            if not (isinstance(x, torch.Tensor) and x.device.type == self.device.type):
+                raise TypeError("the differentiable networks take a tensor on the engine's device (%s)" % self.device)
+        lengths, offsets = self._packed_offsets(xs)
+        n, total, F = len(lengths), int(offsets[-1]), self.num_features
+        x = torch.cat([t.detach().to(device=self.device, dtype=torch.float32).reshape(-1) for t in xs])
+        nbytes = C.c_size_t(0)
+        self._chk(self._lib.cgvc_tape_bytes(self._handle, 2, n, total, C.byref(nbytes)))
+        tape = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
+        y = torch.empty_like(x)
+        off = offsets.ctypes.data_as(C.POINTER(C.c_longlong))
+        self._chk(self._lib.cgvc_generator_forward_packed_tape(self._handle, direction, _ptr(x), _ptr(y), off, n, _ptr(tape), nbytes.value,
+                                                               self._stream()))
+        return [y[F * offsets[u]:F * offsets[u + 1]].view(F, lengths[u]) for u in range(n)], tape, offsets
+
+    def _packed_tape_backward(self, tape, offsets, dys, want_dx):
+        F, n = self.num_features, len(offsets) - 1
+        dy = torch.cat([g.to(device=self.device, dtype=torch.float32).reshape(-1) for g in dys])
+        dx = torch.empty_like(dy) if want_dx else None
+        self._chk(self._lib.cgvc_generator_backward_tape(self._handle, _ptr(tape), _ptr(dy), _ptr(dx), self._stream()))
+        self._tape_scales.add(self.tape_loss_scale(n))
+        if dx is None:
+            return [None] * n
+        return [dx[F * offsets[u]:F * offsets[u + 1]].view(F, int(offsets[u + 1] - offsets[u])) for u in range(n)]
 
     def _tape_backward(self, kind, tape, x_shape, dy, want_dx):
         dy = dy.to(device=self.device, dtype=torch.float32).contiguous()
@@ -532,17 +573,8 @@ class CycleGAN(object):
         if len(inputs) == 0:
             return []
         on_device = all(isinstance(x, torch.Tensor) and x.is_cuda for x in inputs)
-        lengths = []
-        for x in inputs:
-            if len(x.shape) != 2 or x.shape[0] != self.num_features:
-                raise ValueError("expected [%d, frames] utterances, got %r" % (self.num_features, tuple(x.shape)))
-            lengths.append(int(x.shape[1]))
-        offsets = np.zeros(len(lengths) + 1, dtype=np.int64)
-        np.cumsum(lengths, out=offsets[1:])
+        lengths, offsets = self._packed_offsets(inputs)
         n, total = len(lengths), int(offsets[-1])
-        if n > self._max_batch or total > self._max_batch * self._max_frames:
-            batch = max(n, self._max_batch)
-            self._ensure_capacity(batch, max(self._max_frames, -(-total // (4 * batch)) * 4))
         F = self.num_features
         if on_device:
             x = torch.cat([t.to(dtype=torch.float32).reshape(-1) for t in inputs])
@@ -563,6 +595,21 @@ class CycleGAN(object):
         torch.cuda.current_stream(self.device).synchronize()
         ov = out.numpy()
         return [ov[F * offsets[u]:F * offsets[u + 1]].reshape(F, lengths[u]).copy() for u in range(n)]
+
+    def _packed_offsets(self, inputs):
+        """lengths and the n + 1 frame offsets of packed [24, T_i] utterances; grows the engine to hold them"""
+        lengths = []
+        for x in inputs:
+            if len(x.shape) != 2 or x.shape[0] != self.num_features:
+                raise ValueError("expected [%d, frames] utterances, got %r" % (self.num_features, tuple(x.shape)))
+            lengths.append(int(x.shape[1]))
+        offsets = np.zeros(len(lengths) + 1, dtype=np.int64)
+        np.cumsum(lengths, out=offsets[1:])
+        n, total = len(lengths), int(offsets[-1])
+        if n > self._max_batch or total > self._max_batch * self._max_frames:
+            batch = max(n, self._max_batch)
+            self._ensure_capacity(batch, max(self._max_frames, -(-total // (4 * batch)) * 4))
+        return lengths, offsets
 
     def discriminate(self, inputs, which):
         """Discriminator forward (module.py:188-213): which in {'A','B'}; returns [B, 6, T/16, 1]."""
@@ -707,3 +754,23 @@ class _NetFn(torch.autograd.Function):
         tape, = ctx.saved_tensors
         dx = ctx.model._tape_backward(ctx.kind, tape, ctx.x_shape, dy, ctx.needs_input_grad[0])
         return dx, None, None, None, None
+
+
+class _PackedGenFn(torch.autograd.Function):
+    """One packed generator application over utterances of different lengths (CycleGAN.generator_packed) with its kind 2 activation
+    tape: forward writes it, backward consumes it (unmodified, as _NetFn's)"""
+
+    @staticmethod
+    def forward(ctx, token, model, direction, *xs):
+        ys, tape, offsets = model._packed_tape_forward(direction, xs)
+        ctx.model, ctx.offsets = model, offsets
+        ctx.save_for_backward(tape)
+        return tuple(ys)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, *dys):
+        tape, = ctx.saved_tensors
+        want = ctx.needs_input_grad[3:]
+        dxs = ctx.model._packed_tape_backward(tape, ctx.offsets, dys, any(want))
+        return (None, None, None) + tuple(dx if w else None for dx, w in zip(dxs, want))
