@@ -70,15 +70,23 @@ struct GraphKey {
 };
 struct GraphEntry { cudaGraphExec_t exec; unsigned long long launches; };
 
+// What one network application (a forward of the C ABI, or an activation tape) runs over.  kind 0: the generator over n samples of
+// T frames; 1: the discriminator likewise; 2: the generator over n packed utterances (T = 0).  which: the generator's direction, or
+// the discriminator
+struct NetGeom {
+  int kind, which, n, T;
+  long long rows;               // rows at full resolution: n * T, or (kind 2) offsets[n]
+  int max_len;                  // kind 2: the longest utterance
+};
+static NetGeom net_geom(int kind, int which, int n, int T) { return NetGeom{kind, which, n, T, (long long)n * T, 0}; }
+
 // The header at the start of an activation tape (cgvc_*_forward_tape), also kept by the engine that wrote it, keyed by the tape's
 // address: a backward call checks its tape against that copy, so that it needs no device-to-host read before it enqueues anything
 struct TapeHeader {
   unsigned long long magic;     // kTapeMagic
   unsigned long long engine;    // cgvc_engine::id of the writer
   unsigned long long gen;       // cgvc_engine::param_gen when it was written
-  int kind, which, batch, frames;  // kind 2 (packed generator tape): batch = the utterance count n, frames = 0
-  long long rows;               // kind 2: offsets[n], the frames of all utterances
-  int max_len;                  // kind 2: the longest utterance
+  NetGeom geom;                 // what the forward applied the network to
 };
 static const unsigned long long kTapeMagic = 0x45504154435647ull;   // "GVCTAPE"
 static const size_t kTapeHead = 256;                                // the activations start 256 bytes in
@@ -1098,17 +1106,36 @@ static void plan_train(cgvc_engine* e, Bump& ws, TrainPlan& P, int B, int T) {
   }
 }
 
-struct FwdPlan { GenActs g; DiscActs d; float* in_cl; };
+// The buffers of one network application: its input, kind 2's device offsets and the activations of its network (g or d)
+struct AppPlan { GenActs g; DiscActs d; float* x; long long* off; };
+
+// Lays out the buffers of application a from base: for a tape first the TapeHeader's kTapeHead bytes, then for kind 2 the n + 1
+// device frame offsets (off), the input x (generator: channels-last rows [rows, 24]; discriminator: [n, 24, T]) and the activations,
+// as a train step keeps them.  Returns the bytes it takes from base; a null base sizes it
+static size_t plan_app(cgvc_engine* e, const NetGeom& a, void* base, bool tape, AppPlan& P) {
+  const size_t head = tape ? kTapeHead : 0;
+  Bump ws; ws.reset((char*)base + head, (size_t)1 << 62);
+  P.off = a.kind == 2 ? ws.take<long long>((size_t)a.n + 1) : nullptr;
+  P.x = ws.take<float>((size_t)a.rows * e->cfg.num_features);
+  if (a.kind == 1) {
+    plan_discriminator(e, ws, P.d, a.n, a.T);
+    P.d.x = P.x;
+  } else {
+    plan_generator_rows(e, ws, P.g, a.n, a.rows);
+    P.g.T = a.T; P.g.off = P.off; P.g.max_len = a.max_len; P.g.x_cl = P.x;
+  }
+  return head + ws.off;
+}
 
 static size_t work_bytes_needed(cgvc_engine* e) {
   Bump ws; ws.reset(nullptr, 0);
   size_t need = 0;
   if (e->cfg.train) { TrainPlan P; plan_train(e, ws, P, e->cfg.max_batch, e->cfg.max_frames); need = ws.off; }
-  ws.reset(nullptr, 0);
-  FwdPlan F; F.in_cl = ws.take<float>((size_t)e->cfg.max_batch * e->cfg.num_features * e->cfg.max_frames);
-  plan_generator(e, ws, F.g, e->cfg.max_batch, e->cfg.max_frames);
-  plan_discriminator(e, ws, F.d, e->cfg.max_batch, e->cfg.max_frames);
-  if (ws.off > need) need = ws.off;
+  for (int kind = 0; kind < 3; ++kind) {      // the forwards at their largest (kind 2: max_batch utterances of max_batch x max_frames rows)
+    AppPlan F;
+    const size_t fwd = plan_app(e, net_geom(kind, 0, e->cfg.max_batch, e->cfg.max_frames), nullptr, false, F);
+    if (fwd > need) need = fwd;
+  }
   if (e->opt.deterministic) {                 // the per-kernel entry points' slab (plan_entry_det)
     ws.reset(nullptr, 0); ws.take<float>((size_t)CGVC_DET_SLAB_FLOATS);
     if (ws.off > need) need = ws.off;
@@ -1379,91 +1406,6 @@ static int check_bt(cgvc_engine* e, int batch, int frames, int mult) {
   if (batch < 1 || batch > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "batch %d outside [1, %d]", batch, e->cfg.max_batch);
   if (frames < mult || frames % mult != 0 || frames > e->cfg.max_frames)
     return fail(e, CGVC_ERR_ARG, "frames %d must be a multiple of %d in [%d, %d]", frames, mult, mult, e->cfg.max_frames);
-  return 0;
-}
-
-int cgvc_generator_forward(cgvc_handle e, int direction, const float* in_dev, float* out_dev, int batch, int frames, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
-  if (!in_dev || !out_dev) return fail(e, CGVC_ERR_ARG, "null buffer");
-  RET(check_bt(e, batch, frames, 4));
-  RET(need_arenas(e, false));
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
-  FwdPlan F; F.in_cl = ws.take<float>((size_t)batch * e->cfg.num_features * frames);
-  plan_generator(e, ws, F.g, batch, frames);
-  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
-  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &F.g.post));
-  CK(launch_transpose_ft(in_dev, F.in_cl, batch, e->cfg.num_features, frames, st));
-  if (!e->opt.debug_taps) e->taps.clear();
-  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->opt.debug_taps != 0, false));
-  CK(launch_transpose_ft(F.g.out_cl, out_dev, batch, frames, e->cfg.num_features, st));
-  return 0;
-}
-
-// The argument checks of the packed generator calls (cgvc_generator_forward_packed, cgvc_generator_forward_packed_tape): *rows and
-// *max_len receive offsets[n] and the longest utterance
-static int packed_args(cgvc_engine* e, int direction, const void* in_dev, const void* out_dev, const long long* offsets_host, int n,
-                       long long* rows, long long* max_len) {
-  if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
-  if (!in_dev || !out_dev || !offsets_host) return fail(e, CGVC_ERR_ARG, "null buffer");
-  if (n < 1 || n > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", n, e->cfg.max_batch);
-  if (offsets_host[0] != 0) return fail(e, CGVC_ERR_ARG, "offsets[0] is %lld, must be 0", offsets_host[0]);
-  *max_len = 0;
-  for (int u = 0; u < n; ++u) {
-    const long long len = offsets_host[u + 1] - offsets_host[u];
-    if (len <= 0 || len % 4 != 0)
-      return fail(e, CGVC_ERR_ARG, "utterance %d: length %lld (offsets %lld .. %lld) must be a positive multiple of 4", u, len,
-                  offsets_host[u], offsets_host[u + 1]);
-    if (len > *max_len) *max_len = len;
-  }
-  *rows = offsets_host[n];
-  const long long cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
-  if (*rows > cap) return fail(e, CGVC_ERR_ARG, "%lld frames in all exceed the engine's capacity of max_batch x max_frames = %lld", *rows, cap);
-  return 0;
-}
-
-int cgvc_generator_forward_packed(cgvc_handle e, int direction, const float* in_dev, float* out_dev,
-                                  const long long* offsets_host, int n, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  long long rows, max_len;
-  RET(packed_args(e, direction, in_dev, out_dev, offsets_host, n, &rows, &max_len));
-  RET(need_arenas(e, false));
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nf = e->cfg.num_features;
-  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
-  FwdPlan F; F.in_cl = ws.take<float>((size_t)rows * nf);
-  plan_generator_rows(e, ws, F.g, n, rows);                  // within work_bytes_needed: n <= max_batch, rows <= max_batch x max_frames
-  long long* off_dev = ws.take<long long>((size_t)n + 1);    // (inside the discriminator's share of the plan)
-  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
-  F.g.off = off_dev; F.g.max_len = (int)max_len;
-  CK(grow_post_buf(e, (size_t)n * 4 * 1024, &F.g.post));
-  CK(cudaMemcpyAsync(off_dev, offsets_host, ((size_t)n + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CK(launch_transpose_packed(in_dev, F.in_cl, off_dev, n, rows, nf, 1, st));
-  if (!e->opt.debug_taps) e->taps.clear();
-  RET(generator_forward(e, e->gen[direction], F.g, F.in_cl, st, e->opt.debug_taps != 0, false));
-  CK(launch_transpose_packed(F.g.out_cl, out_dev, off_dev, n, rows, nf, 0, st));
-  return 0;
-}
-
-int cgvc_discriminator_forward(cgvc_handle e, int which, const float* in_dev, float* out_dev, int batch, int frames, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  if (which != 0 && which != 1) return fail(e, CGVC_ERR_ARG, "which must be 0 (discriminator_A) or 1 (discriminator_B)");
-  if (!in_dev || !out_dev) return fail(e, CGVC_ERR_ARG, "null buffer");
-  RET(check_bt(e, batch, frames, 16));
-  RET(need_arenas(e, false));
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
-  FwdPlan F; F.in_cl = ws.take<float>((size_t)batch * e->cfg.num_features * frames);
-  plan_generator(e, ws, F.g, batch, frames);   // keep layout identical to work_bytes_needed
-  plan_discriminator(e, ws, F.d, batch, frames);
-  if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small");
-  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &F.d.post));
-  RET(discriminator_forward(e, e->disc[which], F.d, in_dev, st, true));
-  CK(cudaMemcpyAsync(out_dev, F.d.prob, (size_t)batch * (e->cfg.num_features / 4) * (frames / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -2631,38 +2573,67 @@ int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const fl
 
 }  // extern "C"
 
-// ---- activation tapes: the forward of one network application that records what its backward reads, and that backward ------------
-// Layout: the TapeHeader in the first kTapeHead bytes, then the network's input (generator: channels-last [B, T, 24]; discriminator:
-// [B, 24, T]) and the activations of plan_generator / plan_discriminator for (batch, frames), as a train step keeps them.  kind 0 the
-// generator, 1 the discriminator.  Kind 2, the packed generator (batch = n utterances, frames = rows = offsets[n]): the n + 1 frame
-// offsets (*off; the forward copies them there, so that a later call that reuses WORK cannot change what the backward reads), the
-// channels-last input [rows, 24] and plan_generator_rows(n, rows).  Returns the bytes the plan needs; g / d / x receive it at base
-// (base may be null for sizing)
-static size_t tape_plan(cgvc_engine* e, int kind, void* base, int batch, int frames, GenActs* g, DiscActs* d, float** x,
-                        long long** off = nullptr) {
-  Bump ws; ws.reset((char*)base + kTapeHead, (size_t)1 << 62);
-  if (kind == 2) {
-    long long* o = ws.take<long long>((size_t)batch + 1);
-    if (off) *off = o;
+// ---- network applications: the forwards of the C ABI, and the activation tapes that record what a backward reads ----------------
+// A forward checks its geometry, plans its buffers (plan_app) in WORK or in the caller's tape, runs its network and, into a tape,
+// records the header.  A tape backward re-plans the tape from that header and borrows a train step's backward scratch from WORK.
+
+// The geometry checks of every call that takes one: the forwards, their tapes and cgvc_tape_bytes.  Kind 2 with the host offsets off
+// checks them and sets a.rows and a.max_len; without them (cgvc_tape_bytes) it checks the a.rows given
+static int check_geom(cgvc_engine* e, NetGeom& a, const long long* off) {
+  if (a.which != 0 && a.which != 1)
+    return a.kind == 1 ? fail(e, CGVC_ERR_ARG, "which must be 0 (discriminator_A) or 1 (discriminator_B)")
+                       : fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
+  if (a.kind != 2) return check_bt(e, a.n, a.T, a.kind == 0 ? 4 : 16);
+  if (a.n < 1 || a.n > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", a.n, e->cfg.max_batch);
+  if (off) {
+    if (off[0] != 0) return fail(e, CGVC_ERR_ARG, "offsets[0] is %lld, must be 0", off[0]);
+    for (int u = 0; u < a.n; ++u) {
+      const long long len = off[u + 1] - off[u];
+      if (len <= 0 || len % 4 != 0)
+        return fail(e, CGVC_ERR_ARG, "utterance %d: length %lld (offsets %lld .. %lld) must be a positive multiple of 4", u, len, off[u],
+                    off[u + 1]);
+      if (len > a.max_len) a.max_len = (int)len;
+    }
+    a.rows = off[a.n];
   }
-  *x = ws.take<float>((size_t)(kind == 2 ? 1 : batch) * e->cfg.num_features * frames);
-  if (kind == 0) plan_generator(e, ws, *g, batch, frames);
-  else if (kind == 2) plan_generator_rows(e, ws, *g, batch, frames);
-  else plan_discriminator(e, ws, *d, batch, frames);
-  return kTapeHead + ws.off;
+  const long long cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
+  if (a.rows < 4ll * a.n || a.rows % 4 != 0 || a.rows > cap)
+    return fail(e, CGVC_ERR_ARG, "%lld frames of %d utterances: must be a multiple of 4 in [%d, %lld] (max_batch x max_frames)", a.rows,
+                a.n, 4 * a.n, cap);
+  return 0;
 }
 
-// What a tape forward checks before it launches anything; *hd receives the header it is going to write
-static int tape_forward_entry(cgvc_engine* e, int kind, int which, const void* in, const void* out, int batch, int frames, void* tape,
-                              size_t tape_bytes, TapeHeader* hd) {
-  if (!in || !out || !tape) return fail(e, CGVC_ERR_ARG, "null buffer");
-  if ((uintptr_t)tape & 255) return fail(e, CGVC_ERR_ARG, "a tape must be 256-byte aligned");
-  RET(check_bt(e, batch, frames, kind == 0 ? 4 : 16));
-  RET(need_arenas(e, false));
-  GenActs g; DiscActs d; float* x;
-  const size_t need = tape_plan(e, kind, nullptr, batch, frames, &g, &d, &x);
-  if (tape_bytes < need) return fail(e, CGVC_ERR_UNBOUND, "tape of %zu bytes, batch %d x %d frames needs %zu", tape_bytes, batch, frames, need);
-  *hd = TapeHeader{kTapeMagic, e->id, e->param_gen, kind, which, batch, frames};
+// A generator's input or output between the caller's layout ([n, 24, T], or kind 2 the [24][len_u] block of utterance u at element
+// 24 offsets[u]) and channels-last rows: into the rows (to_rows) or out of them
+static cudaError_t transpose_app(const cgvc_engine* e, const NetGeom& a, const GenActs& g, const float* in, float* out, bool to_rows,
+                                 cudaStream_t st) {
+  const int nf = e->cfg.num_features;
+  if (a.kind == 2) return launch_transpose_packed(in, out, g.off, a.n, a.rows, nf, to_rows, st);
+  return to_rows ? launch_transpose_ft(in, out, a.n, nf, a.T, st) : launch_transpose_ft(in, out, a.n, a.T, nf, st);
+}
+
+// The generator from in to out.  A conversion keeps the fp32 layer outputs only for the debug taps and no pre-norm outputs; a tape
+// forward keeps what the backward reads
+static int generator_app(cgvc_engine* e, const NetGeom& a, AppPlan& P, const long long* off, const float* in, float* out, bool tape,
+                         cudaStream_t st) {
+  CK(grow_post_buf(e, (size_t)a.n * 4 * 1024, &P.g.post));
+  if (P.off) CK(cudaMemcpyAsync(P.off, off, ((size_t)a.n + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CK(transpose_app(e, a, P.g, in, P.x, true, st));
+  const bool keep_y = !tape && e->opt.debug_taps;
+  if (!tape && !keep_y) e->taps.clear();
+  RET(generator_forward(e, e->gen[a.which], P.g, P.x, st, keep_y, tape));
+  CK(transpose_app(e, a, P.g, P.g.out_cl, out, false, st));
+  return 0;
+}
+
+// The discriminator from in to the probabilities out.  cgvc_discriminator_forward reads in where it is and keeps every fp32 layer
+// output (its taps); a tape forward copies in into the tape, where the input layer's backward reads it
+static int discriminator_app(cgvc_engine* e, const NetGeom& a, AppPlan& P, const float* in, float* out, bool tape, cudaStream_t st) {
+  const int nf = e->cfg.num_features;
+  CK(grow_post_buf(e, (size_t)a.n * 4 * 1024, &P.d.post));
+  if (tape) CK(cudaMemcpyAsync(P.x, in, (size_t)a.rows * nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  RET(discriminator_forward(e, e->disc[a.which], P.d, tape ? P.x : in, st, !tape));
+  CK(cudaMemcpyAsync(out, P.d.prob, (size_t)a.n * (nf / 4) * (a.T / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -2675,27 +2646,61 @@ static int tape_record(cgvc_engine* e, void* tape, const TapeHeader& hd, cudaStr
   return 0;
 }
 
+struct TapeBuf { void* p; size_t bytes; };   // the caller's tape of a tape forward
+
+// Every forward of the C ABI: application a from in to out, in WORK, or with tape in that tape.  off: kind 2's host offsets.  Every
+// refusal comes before anything is enqueued
+static int forward_app(cgvc_engine* e, NetGeom a, const long long* off, const float* in, float* out, const TapeBuf* tape, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if (!in || !out || (a.kind == 2 && !off) || (tape && !tape->p)) return fail(e, CGVC_ERR_ARG, "null buffer");
+  RET(check_geom(e, a, off));
+  if (tape && ((uintptr_t)tape->p & 255)) return fail(e, CGVC_ERR_ARG, "a tape must be 256-byte aligned");
+  RET(need_arenas(e, false));
+  AppPlan P;
+  const size_t need = plan_app(e, a, tape ? tape->p : e->arena[CGVC_ARENA_WORK], tape != nullptr, P);
+  const size_t have = tape ? tape->bytes : e->arena_bytes[CGVC_ARENA_WORK];
+  if (need > have)
+    return fail(e, CGVC_ERR_UNBOUND, "%s of %zu bytes: %d %s of %lld frames in all need %zu", tape ? "tape" : "WORK arena", have, a.n,
+                a.kind == 2 ? "utterances" : "samples", a.rows, need);
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  RET(a.kind == 1 ? discriminator_app(e, a, P, in, out, tape != nullptr, st) : generator_app(e, a, P, off, in, out, tape != nullptr, st));
+  return tape ? tape_record(e, tape->p, TapeHeader{kTapeMagic, e->id, e->param_gen, a}, st) : 0;
+}
+
 // What a tape backward checks before it launches anything: the tape is one this engine wrote for `kind` under its current parameters,
 // GRAD is bound and WORK holds a train step's plan at max_batch, whose lane-0 BwdScratch (sized for 2 max_batch samples) and upstream
-// buffers the backward borrows: *S, and the lane plan *L for its d_out / in / dY3 buffers
-static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const void* dout, TapeHeader* hd, LanePlan* L) {
+// buffers the backward borrows.  *a and *P receive the tape's geometry and plan, *L the lane plan for its d_out / in / dY3 buffers
+static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const void* dout, NetGeom* a, AppPlan* P, LanePlan* L) {
   if (!tape || !dout) return fail(e, CGVC_ERR_ARG, "null buffer");
   auto it = e->tapes.find(tape);
   if (it == e->tapes.end())
     return fail(e, CGVC_ERR_ARG, "%p is not a tape written by this engine's cgvc_*_forward_tape since its parameters last changed", tape);
-  *hd = it->second;
-  if (hd->gen != e->param_gen) return fail(e, CGVC_ERR_ARG, "stale tape: the parameters changed after its forward");
+  const TapeHeader& hd = it->second;
+  if (hd.gen != e->param_gen) return fail(e, CGVC_ERR_ARG, "stale tape: the parameters changed after its forward");
   static const char* const names[3] = {"generator", "discriminator", "packed generator"};
-  if ((hd->kind == 1) != (kind == 1))        // the generator backward takes kinds 0 and 2
-    return fail(e, CGVC_ERR_ARG, "a %s tape given to the %s backward", names[hd->kind], names[kind]);
+  if ((hd.geom.kind == 1) != (kind == 1))    // the generator backward takes kinds 0 and 2
+    return fail(e, CGVC_ERR_ARG, "a %s tape given to the %s backward", names[hd.geom.kind], names[kind]);
   if (!e->cfg.train || !e->arena[CGVC_ARENA_GRAD])
     return fail(e, CGVC_ERR_UNBOUND, "a tape backward needs the GRAD arena and a WORK arena sized for training (train = 1)");
   RET(need_arenas(e, true));
   Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
-  TrainPlan P; plan_train(e, ws, P, e->cfg.max_batch, e->cfg.max_frames);
+  TrainPlan TP; plan_train(e, ws, TP, e->cfg.max_batch, e->cfg.max_frames);
   if (ws.overflow) return fail(e, CGVC_ERR_UNBOUND, "WORK arena too small for the backward scratch");
-  *L = P.lane[0];
+  *L = TP.lane[0];
   L->S.sq = nullptr;                                        // the weight gradients stay on the caller's stream
+  *a = hd.geom;
+  plan_app(e, *a, const_cast<void*>(tape), true, *P);
+  P->g.post = P->d.post = L->S.post;
+  return 0;
+}
+
+// d in of a tape backward to the caller (din null: none): a generator's out of the channels-last rows, with the loss scale s of the
+// gradient planes taken out (exact: a power of two)
+static int tape_din(cgvc_engine* e, const NetGeom& a, const AppPlan& P, const float* rows, float* din, float s, cudaStream_t st) {
+  if (!din) return 0;
+  if (a.kind != 1) CK(transpose_app(e, a, P.g, rows, din, false, st));
+  if (s != 1.f) CK(launch_scale(din, a.rows * e->cfg.num_features, 1.f / s, st));
   return 0;
 }
 
@@ -2708,137 +2713,81 @@ struct TapeCounting {
 
 extern "C" {
 
+int cgvc_generator_forward(cgvc_handle e, int direction, const float* in_dev, float* out_dev, int batch, int frames, void* stream) {
+  return forward_app(e, net_geom(0, direction, batch, frames), nullptr, in_dev, out_dev, nullptr, stream);
+}
+
+int cgvc_generator_forward_packed(cgvc_handle e, int direction, const float* in_dev, float* out_dev,
+                                  const long long* offsets_host, int n, void* stream) {
+  return forward_app(e, net_geom(2, direction, n, 0), offsets_host, in_dev, out_dev, nullptr, stream);
+}
+
+int cgvc_discriminator_forward(cgvc_handle e, int which, const float* in_dev, float* out_dev, int batch, int frames, void* stream) {
+  return forward_app(e, net_geom(1, which, batch, frames), nullptr, in_dev, out_dev, nullptr, stream);
+}
+
 int cgvc_tape_bytes(cgvc_handle e, int kind, int batch, int frames, size_t* bytes) {
   if (!e || !bytes || kind < 0 || kind > 2) return fail(e, CGVC_ERR_ARG, "cgvc_tape_bytes: bad argument");
-  if (kind == 2) {
-    // batch = n utterances, frames = rows = offsets[n]: the limits of cgvc_generator_forward_packed
-    const long long cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
-    if (batch < 1 || batch > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", batch, e->cfg.max_batch);
-    if (frames < 4 * (long long)batch || frames % 4 || frames > cap)
-      return fail(e, CGVC_ERR_ARG, "%d frames of %d utterances: must be a multiple of 4 in [%d, %lld]", frames, batch, 4 * batch, cap);
-  } else {
-    RET(check_bt(e, batch, frames, kind == 0 ? 4 : 16));
-  }
-  GenActs g; DiscActs d; float* x;
-  *bytes = tape_plan(e, kind, nullptr, batch, frames, &g, &d, &x);
+  // kind 2: batch = n utterances, frames = rows = offsets[n]
+  NetGeom a = kind == 2 ? NetGeom{2, 0, batch, 0, frames, 0} : net_geom(kind, 0, batch, frames);
+  RET(check_geom(e, a, nullptr));
+  AppPlan P;
+  *bytes = plan_app(e, a, nullptr, true, P);
   return 0;
 }
 
 int cgvc_generator_forward_tape(cgvc_handle e, int direction, const float* in_dev, float* out_dev, int batch, int frames, void* tape_dev,
                                 size_t tape_bytes, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  if (direction != 0 && direction != 1) return fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
-  TapeHeader hd;
-  RET(tape_forward_entry(e, 0, direction, in_dev, out_dev, batch, frames, tape_dev, tape_bytes, &hd));
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  GenActs A; DiscActs D; float* x_cl;
-  tape_plan(e, 0, tape_dev, batch, frames, &A, &D, &x_cl);
-  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &A.post));
-  CK(launch_transpose_ft(in_dev, x_cl, batch, e->cfg.num_features, frames, st));
-  RET(generator_forward(e, e->gen[direction], A, x_cl, st, false, true));
-  CK(launch_transpose_ft(A.out_cl, out_dev, batch, frames, e->cfg.num_features, st));
-  return tape_record(e, tape_dev, hd, st);
+  const TapeBuf tape{tape_dev, tape_bytes};
+  return forward_app(e, net_geom(0, direction, batch, frames), nullptr, in_dev, out_dev, &tape, stream);
 }
 
 int cgvc_generator_forward_packed_tape(cgvc_handle e, int direction, const float* in_dev, float* out_dev, const long long* offsets_host, int n,
                                        void* tape_dev, size_t tape_bytes, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  long long rows, max_len;
-  RET(packed_args(e, direction, in_dev, out_dev, offsets_host, n, &rows, &max_len));
-  if (!tape_dev) return fail(e, CGVC_ERR_ARG, "null buffer");
-  if ((uintptr_t)tape_dev & 255) return fail(e, CGVC_ERR_ARG, "a tape must be 256-byte aligned");
-  RET(need_arenas(e, false));
-  GenActs A; DiscActs D; float* x_cl; long long* off_dev;
-  const size_t need = tape_plan(e, 2, nullptr, n, (int)rows, &A, &D, &x_cl, &off_dev);
-  if (tape_bytes < need)
-    return fail(e, CGVC_ERR_UNBOUND, "tape of %zu bytes, %d utterances of %lld frames in all need %zu", tape_bytes, n, rows, need);
-  TapeHeader hd{kTapeMagic, e->id, e->param_gen, 2, direction, n, 0, rows, (int)max_len};
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nf = e->cfg.num_features;
-  tape_plan(e, 2, tape_dev, n, (int)rows, &A, &D, &x_cl, &off_dev);
-  A.off = off_dev; A.max_len = (int)max_len;
-  CK(grow_post_buf(e, (size_t)n * 4 * 1024, &A.post));
-  CK(cudaMemcpyAsync(off_dev, offsets_host, ((size_t)n + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CK(launch_transpose_packed(in_dev, x_cl, off_dev, n, rows, nf, 1, st));
-  RET(generator_forward(e, e->gen[direction], A, x_cl, st, false, true));
-  CK(launch_transpose_packed(A.out_cl, out_dev, off_dev, n, rows, nf, 0, st));
-  return tape_record(e, tape_dev, hd, st);
+  const TapeBuf tape{tape_dev, tape_bytes};
+  return forward_app(e, net_geom(2, direction, n, 0), offsets_host, in_dev, out_dev, &tape, stream);
 }
 
 int cgvc_discriminator_forward_tape(cgvc_handle e, int which, const float* in_dev, float* prob_dev, int batch, int frames, void* tape_dev,
                                     size_t tape_bytes, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  if (which != 0 && which != 1) return fail(e, CGVC_ERR_ARG, "which must be 0 (discriminator_A) or 1 (discriminator_B)");
-  TapeHeader hd;
-  RET(tape_forward_entry(e, 1, which, in_dev, prob_dev, batch, frames, tape_dev, tape_bytes, &hd));
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t img = (size_t)batch * e->cfg.num_features * frames;
-  GenActs G; DiscActs A; float* x;
-  tape_plan(e, 1, tape_dev, batch, frames, &G, &A, &x);
-  CK(grow_post_buf(e, (size_t)batch * 4 * 1024, &A.post));
-  CK(cudaMemcpyAsync(x, in_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));        // the input layer's backward reads it
-  RET(discriminator_forward(e, e->disc[which], A, x, st, false));
-  CK(cudaMemcpyAsync(prob_dev, A.prob, (size_t)batch * (e->cfg.num_features / 4) * (frames / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return tape_record(e, tape_dev, hd, st);
+  const TapeBuf tape{tape_dev, tape_bytes};
+  return forward_app(e, net_geom(1, which, batch, frames), nullptr, in_dev, prob_dev, &tape, stream);
 }
 
 int cgvc_generator_backward_tape(cgvc_handle e, const void* tape_dev, const float* dout_dev, float* din_dev, void* stream) {
   if (!e) return CGVC_ERR_ARG;
-  TapeHeader hd; LanePlan L;
-  RET(tape_backward_entry(e, 0, tape_dev, dout_dev, &hd, &L));
+  NetGeom a; AppPlan P; LanePlan L;
+  RET(tape_backward_entry(e, 0, tape_dev, dout_dev, &a, &P, &L));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  // kind 2 (packed): B utterances of rows frames in all, in the packed [24][len_u] blocks of cgvc_generator_forward_packed
-  const bool pk = hd.kind == 2;
-  const int B = hd.batch, T = pk ? (int)hd.rows : hd.frames, nf = e->cfg.num_features;
-  const long long img = (long long)nf * (pk ? hd.rows : (long long)B * T);
-  GenActs A; DiscActs D; float* x_cl; long long* off = nullptr;
-  tape_plan(e, hd.kind, const_cast<void*>(tape_dev), B, T, &A, &D, &x_cl, &off);
-  A.x_cl = x_cl; A.post = L.S.post;
-  if (pk) { A.off = off; A.max_len = hd.max_len; }
-  // the upstream gradient channels-last, times the loss scale of the F16F8 gradient planes (a power of two: exact); a packed tape of B
-  // utterances takes the scale of a batch of B
-  const float s = loss_scale(e, B);
-  if (pk) CK(launch_transpose_packed(dout_dev, L.d_out, off, B, hd.rows, nf, 1, st));
-  else CK(launch_transpose_ft(dout_dev, L.d_out, B, nf, T, st));
-  if (s != 1.f) CK(launch_scale(L.d_out, img, s, st));
+  // the upstream gradient channels-last, times the loss scale of the F16F8 gradient planes; a packed tape of n utterances takes the
+  // scale of a batch of n
+  const float s = loss_scale(e, a.n);
+  CK(transpose_app(e, a, P.g, dout_dev, L.d_out, true, st));
+  if (s != 1.f) CK(launch_scale(L.d_out, a.rows * e->cfg.num_features, s, st));
   {
     TapeCounting counting(e, 0);
-    RET(generator_backward(e, e->gen[hd.which], A, L.d_out, din_dev ? L.in : nullptr, L.S, st));
+    RET(generator_backward(e, e->gen[a.which], P.g, L.d_out, din_dev ? L.in : nullptr, L.S, st));
   }
-  if (!din_dev) return 0;
-  if (pk) CK(launch_transpose_packed(L.in, din_dev, off, B, hd.rows, nf, 0, st));
-  else CK(launch_transpose_ft(L.in, din_dev, B, T, nf, st));
-  if (s != 1.f) CK(launch_scale(din_dev, img, 1.f / s, st));
-  return 0;
+  return tape_din(e, a, P, L.in, din_dev, s, st);
 }
 
 int cgvc_discriminator_backward_tape(cgvc_handle e, const void* tape_dev, const float* dprob_dev, float* din_dev, void* stream) {
   if (!e) return CGVC_ERR_ARG;
-  TapeHeader hd; LanePlan L;
-  RET(tape_backward_entry(e, 1, tape_dev, dprob_dev, &hd, &L));
+  NetGeom a; AppPlan P; LanePlan L;
+  RET(tape_backward_entry(e, 1, tape_dev, dprob_dev, &a, &P, &L));
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  const int B = hd.batch, T = hd.frames, nf = e->cfg.num_features;
-  GenActs G; DiscActs A; float* x;
-  tape_plan(e, 1, const_cast<void*>(tape_dev), B, T, &G, &A, &x);
-  A.x = x; A.post = L.S.post;
-  const DiscNet& DN = e->disc[hd.which];
+  const DiscNet& DN = e->disc[a.which];
   const float* Pm = e->P(); float* Gm = e->G();
-  const long long rows = (long long)B * (nf / 4) * (T / 16);
   {
     TapeCounting counting(e, 1);
     // dz = s dprob p (1 - p) through the head: dY3 and the dense kernel / bias gradients
-    CK(launch_head_loss_bwd(A.prob, A.d[2].Y, rows, 1024, Pm + DN.dense_k, 0.f, 0.f, nullptr, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st,
-                            static_scale_dev(e, B), det_of(L.S), dprob_dev));
-    RET(discriminator_backward(e, DN, A, L.dY3, true, din_dev, L.S, st));
+    CK(launch_head_loss_bwd(P.d.prob, P.d.d[2].Y, (long long)a.n * (e->cfg.num_features / 4) * (a.T / 16), 1024, Pm + DN.dense_k, 0.f,
+                            0.f, nullptr, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, static_scale_dev(e, a.n), det_of(L.S), dprob_dev));
+    RET(discriminator_backward(e, DN, P.d, L.dY3, true, din_dev, L.S, st));
   }
-  const float s = loss_scale(e, B);
-  if (din_dev && s != 1.f) CK(launch_scale(din_dev, (long long)B * nf * T, 1.f / s, st));
-  return 0;
+  return tape_din(e, a, P, nullptr, din_dev, loss_scale(e, a.n), st);
 }
 
 }  // extern "C"

@@ -43,6 +43,14 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def _direction(direction):
+    """'A2B' -> 0, 'B2A' -> 1 (model.py:128-137)"""
+    d = {'A2B': 0, 'B2A': 1}.get(direction)
+    if d is None:
+        raise Exception('Conversion direction must be specified.')
+    return d
+
+
 class CycleGAN(object):
 
     def __init__(self, num_features, discriminator=_discriminator, generator=_generator_gatedcnn, mode='train',
@@ -302,10 +310,7 @@ class CycleGAN(object):
         """Differentiable generator forward: x a CUDA tensor [batch, 24, frames] (frames a multiple of 4) -> [batch, 24, frames], bit
         for bit what test() gives.  Its backward adds d loss / d (the generator's variables) into the gradient arena (grads()) and
         returns d loss / d x.  direction 'A2B' or 'B2A'."""
-        d = {'A2B': 0, 'B2A': 1}.get(direction)
-        if d is None:
-            raise Exception('Conversion direction must be specified.')
-        return _NetFn.apply(x, self._token(), self, 0, d)
+        return _NetFn.apply(x, self._token(), self, 0, _direction(direction))
 
     def discriminator(self, x, which):
         """Differentiable discriminator forward: x a CUDA tensor [batch, 24, frames] (frames a multiple of 16) -> probabilities
@@ -321,9 +326,7 @@ class CycleGAN(object):
         one their backward, which adds d loss / d (the generator's variables) into the gradient arena -- with the loss scale of a batch
         of len(inputs), tape_loss_scale(len(inputs)) -- and returns d loss / d x_i for the inputs that require it.  Every convolution
         tap, instance norm and edge-layer sum stays inside its own utterance, forward and backward.  direction 'A2B' or 'B2A'."""
-        d = {'A2B': 0, 'B2A': 1}.get(direction)
-        if d is None:
-            raise Exception('Conversion direction must be specified.')
+        d = _direction(direction)
         inputs = list(inputs)
         if not inputs:
             return []
@@ -344,6 +347,7 @@ class CycleGAN(object):
         return float(2 ** (9 + min(int(batch).bit_length() - 1, 9)))
 
     def _tape_forward(self, kind, which, x):
+        """x [batch, 24, frames] through the generator (kind 0) or the discriminator (kind 1), with its activation tape: (y, tape)."""
         if not (isinstance(x, torch.Tensor) and x.device.type == self.device.type):
             raise TypeError("the differentiable networks take a tensor on the engine's device (%s)" % self.device)
         x = x.detach().to(device=self.device, dtype=torch.float32).contiguous()
@@ -351,51 +355,51 @@ class CycleGAN(object):
             raise ValueError("expected [batch, %d, frames], got %r" % (self.num_features, tuple(x.shape)))
         batch, _, frames = x.shape
         self._ensure_capacity(batch, frames)
-        nbytes = C.c_size_t(0)
-        self._chk(self._lib.cgvc_tape_bytes(self._handle, kind, batch, frames, C.byref(nbytes)))
-        tape = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)     # the caching allocator aligns to 512 bytes
-        if kind == 0:
-            y = torch.empty_like(x)
-            fn = self._lib.cgvc_generator_forward_tape
-        else:
+        if kind == 1:
             y = torch.empty((batch, self.num_features // 4, frames // 16, 1), dtype=torch.float32, device=self.device)
-            fn = self._lib.cgvc_discriminator_forward_tape
-        self._chk(fn(self._handle, which, _ptr(x), _ptr(y), batch, frames, _ptr(tape), nbytes.value, self._stream()))
-        return y, tape
+        else:
+            y = torch.empty_like(x)
+        return y, self._tape_call(kind, which, x, y, batch, frames, (batch, frames))
 
     def _packed_tape_forward(self, direction, xs):
+        """The [24, T_i] utterances xs through the generator in one call, with its kind 2 activation tape: (ys, tape, offsets)."""
         for x in xs:
             if not (isinstance(x, torch.Tensor) and x.device.type == self.device.type):
                 raise TypeError("the differentiable networks take a tensor on the engine's device (%s)" % self.device)
-        lengths, offsets = self._packed_offsets(xs)
-        n, total, F = len(lengths), int(offsets[-1]), self.num_features
-        x = torch.cat([t.detach().to(device=self.device, dtype=torch.float32).reshape(-1) for t in xs])
-        nbytes = C.c_size_t(0)
-        self._chk(self._lib.cgvc_tape_bytes(self._handle, 2, n, total, C.byref(nbytes)))
-        tape = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
+        offsets = self._packed_offsets(xs)
+        x = self._pack(xs)
         y = torch.empty_like(x)
-        off = offsets.ctypes.data_as(C.POINTER(C.c_longlong))
-        self._chk(self._lib.cgvc_generator_forward_packed_tape(self._handle, direction, _ptr(x), _ptr(y), off, n, _ptr(tape), nbytes.value,
-                                                               self._stream()))
-        return [y[F * offsets[u]:F * offsets[u + 1]].view(F, lengths[u]) for u in range(n)], tape, offsets
+        n = len(offsets) - 1
+        tape = self._tape_call(2, direction, x, y, n, int(offsets[-1]), (offsets.ctypes.data_as(C.POINTER(C.c_longlong)), n))
+        return self._unpack(y, offsets), tape, offsets
 
-    def _packed_tape_backward(self, tape, offsets, dys, want_dx):
-        F, n = self.num_features, len(offsets) - 1
-        dy = torch.cat([g.to(device=self.device, dtype=torch.float32).reshape(-1) for g in dys])
-        dx = torch.empty_like(dy) if want_dx else None
-        self._chk(self._lib.cgvc_generator_backward_tape(self._handle, _ptr(tape), _ptr(dy), _ptr(dx), self._stream()))
-        self._tape_scales.add(self.tape_loss_scale(n))
-        if dx is None:
-            return [None] * n
-        return [dx[F * offsets[u]:F * offsets[u + 1]].view(F, int(offsets[u + 1] - offsets[u])) for u in range(n)]
+    def _tape_call(self, kind, which, x, y, batch, frames, geom):
+        """A tape of `kind` sized by cgvc_tape_bytes(batch, frames) (kind 2: n utterances of offsets[n] frames in all), written by that
+        kind's forward from x to y; geom: the forward's geometry arguments.  The caching allocator aligns the tape to 512 bytes."""
+        nbytes = C.c_size_t(0)
+        self._chk(self._lib.cgvc_tape_bytes(self._handle, kind, batch, frames, C.byref(nbytes)))
+        tape = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
+        fn = getattr(self._lib, ("cgvc_generator_forward_tape", "cgvc_discriminator_forward_tape",
+                                 "cgvc_generator_forward_packed_tape")[kind])
+        self._chk(fn(self._handle, which, _ptr(x), _ptr(y), *geom, _ptr(tape), nbytes.value, self._stream()))
+        return tape
 
-    def _tape_backward(self, kind, tape, x_shape, dy, want_dx):
-        dy = dy.to(device=self.device, dtype=torch.float32).contiguous()
+    def _tape_backward(self, kind, tape, geom, dy, want_dx):
+        """d loss / d x of a tape's application from d loss / d y, or None without want_dx; adds the network's variable gradients into
+        the gradient arena.  geom: x's shape, or for a kind 2 tape the utterances' offsets, with dy and d x lists of their blocks."""
+        if kind == 2:
+            dy = self._pack(dy)
+            x_shape, batch = dy.shape, len(geom) - 1
+        else:
+            dy = dy.to(device=self.device, dtype=torch.float32).contiguous()
+            x_shape, batch = geom, geom[0]
         dx = torch.empty(x_shape, dtype=torch.float32, device=self.device) if want_dx else None
-        fn = self._lib.cgvc_generator_backward_tape if kind == 0 else self._lib.cgvc_discriminator_backward_tape
+        fn = self._lib.cgvc_discriminator_backward_tape if kind == 1 else self._lib.cgvc_generator_backward_tape
         self._chk(fn(self._handle, _ptr(tape), _ptr(dy), _ptr(dx), self._stream()))
-        self._tape_scales.add(self.tape_loss_scale(x_shape[0]))
-        return dx
+        self._tape_scales.add(self.tape_loss_scale(batch))
+        if kind != 2:
+            return dx
+        return self._unpack(dx, geom) if want_dx else [None] * batch
 
     def zero_grad(self, network=None):
         """Zero the gradient arena before the backward passes of a new step; with network ('generator_A2B', ..., 'discriminator_B')
@@ -464,14 +468,39 @@ class CycleGAN(object):
         a = np.asarray(x)
         if a.ndim != 3 or a.shape[1] != self.num_features:
             raise ValueError("expected [batch, %d, frames], got %r" % (self.num_features, a.shape))
+        return self._stage([a], key).view(a.shape)
+
+    def _stage(self, arrays, key):
+        """Host arrays (any float dtype) -> one fp32 CUDA tensor holding them back to back, through the pinned buffer kept for `key`."""
+        n = sum(a.size for a in arrays)
         st = self._staging.get(key)
-        if st is None or st[0].shape != a.shape:
-            st = (torch.empty(a.shape, dtype=torch.float32).pin_memory(),
-                  torch.empty(a.shape, dtype=torch.float32, device=self.device))
+        if st is None or st[0].numel() != n:
+            st = (torch.empty(n, dtype=torch.float32).pin_memory(), torch.empty(n, dtype=torch.float32, device=self.device))
             self._staging[key] = st
-        st[0].numpy()[...] = a            # cast to fp32 at the boundary, like the placeholder feed (model.py:35-42)
+        hv, o = st[0].numpy(), 0
+        for a in arrays:                  # cast to fp32 at the boundary, like the placeholder feed (model.py:35-42)
+            hv[o:o + a.size] = a.reshape(-1)
+            o += a.size
         st[1].copy_(st[0], non_blocking=True)
         return st[1]
+
+    def _pack(self, tensors):
+        """Tensors on the engine's device -> one fp32 tensor holding them back to back (the packed utterance layout)."""
+        return torch.cat([t.detach().to(device=self.device, dtype=torch.float32).reshape(-1) for t in tensors])
+
+    def _unpack(self, y, offsets):
+        """The [24, T_i] utterances of a packed tensor or array y, as views."""
+        F = self.num_features
+        return [y[F * offsets[u]:F * offsets[u + 1]].reshape(F, -1) for u in range(len(offsets) - 1)]
+
+    def _result(self, y, on_device):
+        """A result on the device as it is, or for host inputs as a float32 numpy array (synchronises)."""
+        if on_device:
+            return y
+        out = torch.empty(y.shape, dtype=torch.float32).pin_memory()
+        out.copy_(y, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        return out.numpy().copy()
 
     # ------------------------------------------------------------------ the reference API
     def train(self, input_A, input_B, lambda_cycle, lambda_identity, generator_learning_rate, discriminator_learning_rate):
@@ -541,75 +570,41 @@ class CycleGAN(object):
 
     def test(self, inputs, direction):
         """Generator forward (model.py:128-137).  inputs [B, 24, T] with T a multiple of 4."""
-        if direction == 'A2B':
-            d = 0
-        elif direction == 'B2A':
-            d = 1
-        else:
-            raise Exception('Conversion direction must be specified.')
+        d = _direction(direction)
         x = self._to_device(inputs, "test")
         batch, _, frames = x.shape
         self._ensure_capacity(batch, frames)
         y = torch.empty_like(x)
         self._chk(self._lib.cgvc_generator_forward(self._handle, d, _ptr(x), _ptr(y), batch, frames, self._stream()))
-        if isinstance(inputs, torch.Tensor) and inputs.is_cuda:
-            return y
-        out = torch.empty(y.shape, dtype=torch.float32).pin_memory()
-        out.copy_(y, non_blocking=True)
-        torch.cuda.current_stream(self.device).synchronize()
-        return out.numpy().copy()
+        return self._result(y, isinstance(inputs, torch.Tensor) and inputs.is_cuda)
 
     def test_packed(self, inputs, direction):
         """Generator forward of utterances of different lengths in one engine call.  inputs: a list of [24, T_i] arrays, every
         T_i a positive multiple of 4: host arrays of any float dtype (returns a list of float32 numpy arrays) or CUDA tensors
         (returns a list of CUDA tensors).  Each result is what test() gives for that utterance alone, up to the summation order
         of its instance-norm statistics."""
-        if direction == 'A2B':
-            d = 0
-        elif direction == 'B2A':
-            d = 1
-        else:
-            raise Exception('Conversion direction must be specified.')
+        d = _direction(direction)
         if len(inputs) == 0:
             return []
         on_device = all(isinstance(x, torch.Tensor) and x.is_cuda for x in inputs)
-        lengths, offsets = self._packed_offsets(inputs)
-        n, total = len(lengths), int(offsets[-1])
-        F = self.num_features
-        if on_device:
-            x = torch.cat([t.to(dtype=torch.float32).reshape(-1) for t in inputs])
-        else:
-            host = torch.empty(total * F, dtype=torch.float32).pin_memory()
-            hv = host.numpy()
-            for u, a in enumerate(inputs):       # cast to fp32 at the boundary, like test()
-                hv[F * offsets[u]:F * offsets[u + 1]].reshape(F, lengths[u])[...] = np.asarray(a)
-            x = torch.empty(total * F, dtype=torch.float32, device=self.device)
-            x.copy_(host, non_blocking=True)
+        offsets = self._packed_offsets(inputs)
+        x = self._pack(inputs) if on_device else self._stage([np.asarray(a) for a in inputs], "test_packed")
         y = torch.empty_like(x)
         off = offsets.ctypes.data_as(C.POINTER(C.c_longlong))
-        self._chk(self._lib.cgvc_generator_forward_packed(self._handle, d, _ptr(x), _ptr(y), off, n, self._stream()))
-        if on_device:
-            return [y[F * offsets[u]:F * offsets[u + 1]].view(F, lengths[u]) for u in range(n)]
-        out = torch.empty(y.shape, dtype=torch.float32).pin_memory()
-        out.copy_(y, non_blocking=True)
-        torch.cuda.current_stream(self.device).synchronize()
-        ov = out.numpy()
-        return [ov[F * offsets[u]:F * offsets[u + 1]].reshape(F, lengths[u]).copy() for u in range(n)]
+        self._chk(self._lib.cgvc_generator_forward_packed(self._handle, d, _ptr(x), _ptr(y), off, len(offsets) - 1, self._stream()))
+        return self._unpack(self._result(y, on_device), offsets)
 
     def _packed_offsets(self, inputs):
-        """lengths and the n + 1 frame offsets of packed [24, T_i] utterances; grows the engine to hold them"""
-        lengths = []
+        """the n + 1 frame offsets of packed [24, T_i] utterances; grows the engine to hold them"""
         for x in inputs:
             if len(x.shape) != 2 or x.shape[0] != self.num_features:
                 raise ValueError("expected [%d, frames] utterances, got %r" % (self.num_features, tuple(x.shape)))
-            lengths.append(int(x.shape[1]))
-        offsets = np.zeros(len(lengths) + 1, dtype=np.int64)
-        np.cumsum(lengths, out=offsets[1:])
-        n, total = len(lengths), int(offsets[-1])
+        offsets = np.cumsum([0] + [int(x.shape[1]) for x in inputs], dtype=np.int64)
+        n, total = len(inputs), int(offsets[-1])
         if n > self._max_batch or total > self._max_batch * self._max_frames:
             batch = max(n, self._max_batch)
             self._ensure_capacity(batch, max(self._max_frames, -(-total // (4 * batch)) * 4))
-        return lengths, offsets
+        return offsets
 
     def discriminate(self, inputs, which):
         """Discriminator forward (module.py:188-213): which in {'A','B'}; returns [B, 6, T/16, 1]."""
@@ -772,5 +767,5 @@ class _PackedGenFn(torch.autograd.Function):
     def backward(ctx, *dys):
         tape, = ctx.saved_tensors
         want = ctx.needs_input_grad[3:]
-        dxs = ctx.model._packed_tape_backward(tape, ctx.offsets, dys, any(want))
+        dxs = ctx.model._tape_backward(2, tape, ctx.offsets, dys, any(want))
         return (None, None, None) + tuple(dx if w else None for dx, w in zip(dxs, want))
