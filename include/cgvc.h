@@ -195,6 +195,17 @@ int cgvc_generator_forward_packed(cgvc_handle h, int direction, const float* in_
 /* discriminator forward, which 0 = discriminator_A, 1 = discriminator_B: out [batch, 6, frames/16] (module.py:188-213) */
 int cgvc_discriminator_forward(cgvc_handle h, int which, const float* in_dev, float* out_dev,
                                int batch, int frames, void* stream);
+/* discriminator forward of n utterances of different lengths in one call: utterance u is the row-major [num_features][len_u] block at
+ * element num_features * offsets_host[u] of in_dev (the layout cgvc_generator_forward_packed writes), and its probabilities are the
+ * row-major [num_features / 4][len_u / 16] block at element (num_features / 4) * offsets_host[u] / 16 of prob_dev.  Every len_u must
+ * be a positive multiple of 16 (the four stride-2 stages along time).  Every layer keeps to its utterance: each convolution pads with
+ * zeros at the utterance's own edges and each instance norm takes its statistics over the utterance alone, so every utterance's result
+ * is what cgvc_discriminator_forward gives for it alone, up to the summation order.  Argument checks and errors are those of
+ * cgvc_generator_forward_packed (n <= max_batch, offsets_host[n] <= max_batch * max_frames, CGVC_ERR_ARG naming a bad utterance), all
+ * before anything is enqueued.  Inside, every level of the network is stored utterance after utterance: utterance u owns rows
+ * H_l * offsets[u] / d_l ... H_l * offsets[u+1] / d_l of a level with H_l rows at time divisor d_l, as [y][x][channel]. */
+int cgvc_discriminator_forward_packed(cgvc_handle h, int which, const float* in_dev, float* prob_dev,
+                                      const long long* offsets_host, int n, void* stream);
 
 /* -- activation tapes: the two networks as differentiable operators (the reference composes module.py:148-213 into its loss graph,
  * model.py:44-108; here a caller composes them into any objective and runs each application's backward itself).
@@ -225,9 +236,17 @@ int cgvc_discriminator_forward(cgvc_handle h, int which, const float* in_dev, fl
  *     them.  The dynamic policy ("loss_scale" = 2) does not act on tape calls: no skip, no scale change; they use the static scale.
  *   - Options: "deterministic" makes repeated forward / backward sequences give the same GRAD bits; the kernel-choice options act as in a
  *     train step.  Tape calls run eagerly on `stream`, never as captured graphs.
- * Not covered: packed discriminator tapes, per-call or per-network loss scales, data-parallel reduction (cgvc_allreduce_grads sums
+ * Kind 3 = packed discriminator (cgvc_discriminator_forward_packed_tape): cgvc_tape_bytes(h, 3, n, rows, &bytes) as for kind 2, every length a
+ * multiple of 16; cgvc_discriminator_backward_tape takes kinds 1 and 3, with d prob and d in in the packed layouts of
+ * cgvc_discriminator_forward_packed, every tap and instance norm inside its utterance; the generator backward refuses kind 3.
+ * Not covered: per-call or per-network loss scales, data-parallel reduction (cgvc_allreduce_grads sums
  * GRAD over ranks). */
 int cgvc_tape_bytes(cgvc_handle h, int kind, int batch, int frames, size_t* bytes);
+/* cgvc_discriminator_forward_packed with a kind 3 tape: the same argument checks and errors, all before anything is enqueued, then the
+ * tape checks above; prob_dev bit for bit what cgvc_discriminator_forward_packed writes.  The offsets and the row prefix sums of the
+ * network's levels are copied into the tape. */
+int cgvc_discriminator_forward_packed_tape(cgvc_handle h, int which, const float* in_dev, float* prob_dev, const long long* offsets_host,
+                                           int n, void* tape_dev, size_t tape_bytes, void* stream);
 int cgvc_generator_forward_tape(cgvc_handle h, int direction, const float* in_dev, float* out_dev, int batch, int frames,
                                 void* tape_dev, size_t tape_bytes, void* stream);
 /* cgvc_generator_forward_packed with a kind 2 tape: the same argument checks and errors (all before anything is enqueued), then the

@@ -82,6 +82,7 @@ def _declare(lib):
         "cgvc_adam_step": (ci, [vp, cf, cf, cf, vp]),
         "cgvc_generator_forward": (ci, [vp, ci, vp, vp, ci, ci, vp]),
         "cgvc_generator_forward_packed": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp]),
+        "cgvc_discriminator_forward_packed": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp]),
         "cgvc_discriminator_forward": (ci, [vp, ci, vp, vp, ci, ci, vp]),
         "cgvc_debug_activation": (ci, [vp, C.c_char_p, vp, sz, P(sz), vp]),
         "cgvc_weight_planes": (ci, [vp, ci, P(WeightLayerInfo), C.c_char_p, vp, sz, P(sz), vp]),
@@ -123,6 +124,7 @@ def _declare(lib):
         "cgvc_tape_bytes": (ci, [vp, ci, ci, ci, P(sz)]),
         "cgvc_generator_forward_tape": (ci, [vp, ci, vp, vp, ci, ci, vp, sz, vp]),
         "cgvc_generator_forward_packed_tape": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp, sz, vp]),
+        "cgvc_discriminator_forward_packed_tape": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp, sz, vp]),
         "cgvc_discriminator_forward_tape": (ci, [vp, ci, vp, vp, ci, ci, vp, sz, vp]),
         "cgvc_generator_backward_tape": (ci, [vp, vp, vp, vp, vp]),
         "cgvc_discriminator_backward_tape": (ci, [vp, vp, vp, vp, vp]),

@@ -62,7 +62,14 @@ struct GenActs {
   float* out_cl;
   float* post;                  // scratch for the instance-norm sums [n,4,1024]
 };
-struct DiscActs { int n, T; const float* x; GLAct h1, d[3]; float* prob; float* post; };
+struct DiscActs {
+  int n, T; const float* x; GLAct h1, d[3]; float* prob; float* post;
+  // packed utterances (cgvc_discriminator_forward_packed): n + 1 device frame prefix sums, else null; then every level is a packed 2-D
+  // grid (kernels.cuh PackGeom2) and seg[i] holds the n + 1 row prefix sums of d[i]'s output grid (its instance-norm segments)
+  const long long* off; const long long* seg[3];
+  long long rows;               // frames in all: n * T, or off[n]
+  int max_len;                  // packed: the longest utterance
+};
 
 struct GraphKey {
   int batch, frames, id_off, kind;
@@ -71,13 +78,15 @@ struct GraphKey {
 struct GraphEntry { cudaGraphExec_t exec; unsigned long long launches; };
 
 // What one network application (a forward of the C ABI, or an activation tape) runs over.  kind 0: the generator over n samples of
-// T frames; 1: the discriminator likewise; 2: the generator over n packed utterances (T = 0).  which: the generator's direction, or
-// the discriminator
+// T frames; 1: the discriminator likewise; 2: the generator over n packed utterances (T = 0); 3: the discriminator over n packed
+// utterances (T = 0).  which: the generator's direction, or the discriminator
 struct NetGeom {
   int kind, which, n, T;
-  long long rows;               // rows at full resolution: n * T, or (kind 2) offsets[n]
-  int max_len;                  // kind 2: the longest utterance
+  long long rows;               // rows at full resolution: n * T, or (kinds 2, 3) offsets[n]
+  int max_len;                  // kinds 2, 3: the longest utterance
 };
+static bool packed_kind(int kind) { return kind == 2 || kind == 3; }
+static bool disc_kind(int kind) { return kind == 1 || kind == 3; }
 static NetGeom net_geom(int kind, int which, int n, int T) { return NetGeom{kind, which, n, T, (long long)n * T, 0}; }
 
 // The header at the start of an activation tape (cgvc_*_forward_tape), also kept by the engine that wrote it, keyed by the tape's
@@ -324,7 +333,9 @@ static void build_discriminator(TableBuilder& tb, DiscNet& d) {
 struct ConvIO {               // one convolution application
   const float* x; const __nv_bfloat16 *xhi, *xlo;   // input [n,H,W,Cin] fp32 (may be null on the tensor-core path) + bf16 planes
   int n, H, W;
-  PackGeom pk{};              // packed utterances (pk.off != null): n = H = 1, W = rows at the level of divisor pk.div
+  PackGeom pk{};              // packed utterances (pk.off != null): n = H = 1, W = rows at the level of divisor pk.div; or with H > 1
+                              // packed 2-D grids (kernels.cuh PackGeom2): n = 1, W = all frames / pk.div
+  const long long* seg_out{}; // packed 2-D grids: the n + 1 row prefix sums of the layer's output grid (instance-norm segments)
 };
 static const PackGeom* packed(const ConvIO& io) { return io.pk.off ? &io.pk : nullptr; }
 
@@ -511,7 +522,12 @@ static PostParams post_params(const cgvc_engine* e, const Layer& L, const LayerT
   q.stats = L.has_in ? A.stats : nullptr; q.y_hi = A.Yhi; q.y_lo = A.Ylo;
   q.qmode = t.precision == CGVC_PREC_F16F8;
   q.sat = sat_act(e);
-  if (io.pk.off && L.has_in) {
+  if (io.pk.off && L.has_in && io.seg_out) {
+    // packed 2-D grids: instance norm per utterance over its rows of the output grid, H_out x len_u / d_out of them
+    const long long frames = (long long)io.pk.div * io.W, view_rows = q.R;
+    q.B = io.pk.n; q.R = (int)(view_rows * io.pk.max_len / frames);
+    q.seg = PackGeom{io.seg_out, io.pk.n, 1, q.R}; q.seg_rows = view_rows;
+  } else if (io.pk.off && L.has_in) {
     // packed utterances: q describes one sample holding all q.R view rows; instance norm runs per utterance over its own view rows
     // (the GLU-only layer is row-local and keeps that view)
     const long long view_rows = q.R;
@@ -759,7 +775,12 @@ static PostBwdParams post_bwd_params(const cgvc_engine* e, const Layer& L, const
   q.sat = sat_grad(e); q.ufl = ufl_grad(e);
   if (t.dba || t.dbeta_a) q.det = S.det;    // passes without parameter gradients keep the faster (equally deterministic) forms
   if (seg) seg->seg.off = nullptr;
-  if (seg && in && in->pk.off && L.has_in) {
+  if (seg && in && in->pk.off && L.has_in && in->seg_out) {
+    // packed 2-D grids, as post_params: per utterance over its rows of the output grid (n + 1 row prefix sums in->seg_out, div 1)
+    const long long frames = (long long)in->pk.div * in->W, view_rows = q.R;
+    q.B = in->pk.n; q.R = (int)(view_rows * in->pk.max_len / frames);
+    *seg = PostBwdSeg{PackGeom{in->seg_out, in->pk.n, 1, q.R}, view_rows};
+  } else if (seg && in && in->pk.off && L.has_in) {
     // packed utterances, as post_params: per utterance over its own view rows (the GLU-only layer is row-local and keeps one sample)
     const long long view_rows = q.R;
     const int div = (int)((long long)in->pk.div * in->W / view_rows);
@@ -928,11 +949,12 @@ static int generator_backward(cgvc_engine* e, const GenNet& N, const GenActs& A,
 }
 
 // ---- discriminator ---------------------------------------------------------------------------------------
-static void plan_discriminator(cgvc_engine* e, Bump& ws, DiscActs& A, int n, int T) {
+// activations of n samples of `frames` frames in all (n x T, or n packed utterances: every length a multiple of 16)
+static void plan_discriminator_rows(cgvc_engine* e, Bump& ws, DiscActs& A, int n, long long frames) {
   const bool pl = e->cfg.precision != CGVC_PREC_FP32_SIMT;
-  A.n = n; A.T = T; A.post = nullptr;
+  A.n = n; A.T = 0; A.post = nullptr; A.off = nullptr; A.seg[0] = A.seg[1] = A.seg[2] = nullptr; A.rows = frames; A.max_len = 0;
   const int H = e->cfg.num_features;
-  long long r0 = (long long)n * H * (T / 2), r1 = (long long)n * (H / 2) * (T / 4), r2 = (long long)n * (H / 4) * (T / 8), r3 = (long long)n * (H / 4) * (T / 16);
+  long long r0 = H * (frames / 2), r1 = (H / 2) * (frames / 4), r2 = (H / 4) * (frames / 8), r3 = (H / 4) * (frames / 16);
   plan_gated(ws, A.h1, r0, 256, n, 128, pl, r0 * 128);
   plan_gated(ws, A.d[0], r1, 512, n, 256, pl, r1 * 256);
   plan_gated(ws, A.d[1], r2, 1024, n, 512, pl, r2 * 512);
@@ -940,19 +962,25 @@ static void plan_discriminator(cgvc_engine* e, Bump& ws, DiscActs& A, int n, int
   A.prob = ws.take<float>((size_t)r3);
 }
 
+static void plan_discriminator(cgvc_engine* e, Bump& ws, DiscActs& A, int n, int T) {
+  plan_discriminator_rows(e, ws, A, n, (long long)n * T);
+  A.T = T;
+}
+
 // The discriminator's input layer L (one input channel, <= 9 taps, gate without instance norm: module.py:196-203), its tensors t by
 // pointer, so that the walk and the test entry points (cgvc_disc_input_forward / _backward) run the same launches.
 // P [n * Ho * Wo, 2 cout] = [a | g] = conv(x [n, H, W]) + bias, and the GLU that q describes (q.p = P: y, its planes and their count).
 // fuse: convolution + GLU in one HBM-bound pass (P is written for the backward pass but not read back); else the convolution, then the
 // GLU-only post kernels
+// pk (may be null): x and P are packed 2-D grids (n = 1, W = all frames)
 static int disc_input_forward(cgvc_engine* e, const Layer& L, const LayerTensors& t, const float* x, int n, int H, int W, float* P,
-                              const PostParams& q, bool fuse, cudaStream_t st) {
+                              const PostParams& q, bool fuse, cudaStream_t st, const PackGeom* pk = nullptr) {
   const GatherGeom g = fwd_geom(n, H, W, L.a.kh, L.a.kw, L.sh, L.sw);
   if (fuse) {
-    CK(launch_conv_c1_glu_fwd(g, x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat, q.ufl));
+    CK(launch_conv_c1_glu_fwd(g, x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, q.y, q.y_hi, q.y_lo, q.qmode, st, q.sat, q.ufl, pk));
     return 0;
   }
-  CK(launch_conv_c1_fwd(g, x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, st));
+  CK(launch_conv_c1_fwd(g, x, t.ka, t.kg, t.ba, t.bg, L.a.cout, P, st, pk));
   CK(launch_post_fwd(q, e->opt.post, st));
   return 0;
 }
@@ -961,18 +989,20 @@ static int disc_input_forward(cgvc_engine* e, const Layer& L, const LayerTensors
 // = the data gradient (null: none), Z scratch [n * Ho * Wo, taps].  fuse: dP = (dy s(g), dy a s(g) (1 - s(g))) formed in registers inside
 // the weight-gradient and data-gradient kernels; else the GLU-only backward q (bias gradients included) writes the fp32 dP q.dp, which
 // wgrad_c1 and dgrad_c1 read.  det: deterministic mode's partials slab, else null
+// pk (may be null): packed 2-D grids, as disc_input_forward
 static int disc_input_backward(cgvc_engine* e, const Layer& L, const LayerTensors& t, const float* x, const float* dy, const float* P, int n,
-                               int H, int W, float* dx, float* Z, bool fuse, const PostBwdParams& q, const DetSlab* det, cudaStream_t st) {
+                               int H, int W, float* dx, float* Z, bool fuse, const PostBwdParams& q, const DetSlab* det, cudaStream_t st,
+                               const PackGeom* pk = nullptr) {
   const int kh = L.a.kh, kw = L.a.kw, cout = L.a.cout;
   const GatherGeom g = fwd_geom(n, H, W, kh, kw, L.sh, L.sw);
   if (fuse) {
-    if (t.dka) CK(launch_glu_bwd_wgrad_c1(g, x, dy, P, cout, t.dka, t.dkg, t.dba, t.dbg, st, det));
-    if (dx) CK(launch_glu_bwd_dgrad_c1(dy, P, cout, t.ka, t.kg, Z, dx, n, H, W, kh, kw, L.sh, L.sw, st));
+    if (t.dka) CK(launch_glu_bwd_wgrad_c1(g, x, dy, P, cout, t.dka, t.dkg, t.dba, t.dbg, st, det, pk));
+    if (dx) CK(launch_glu_bwd_dgrad_c1(dy, P, cout, t.ka, t.kg, Z, dx, n, H, W, kh, kw, L.sh, L.sw, st, pk));
     return 0;
   }
   CK(launch_post_bwd(q, e->opt.post, st));
-  if (t.dka) CK(launch_wgrad_c1(g, x, q.dp, 2 * cout, 2 * cout, t.dka, t.dkg, cout, nullptr, nullptr, st, det));
-  if (dx) CK(launch_dgrad_c1(q.dp, 2 * cout, t.ka, t.kg, cout, Z, dx, n, H, W, kh, kw, L.sh, L.sw, st));
+  if (t.dka) CK(launch_wgrad_c1(g, x, q.dp, 2 * cout, 2 * cout, t.dka, t.dkg, cout, nullptr, nullptr, st, det, pk));
+  if (dx) CK(launch_dgrad_c1(q.dp, 2 * cout, t.ka, t.kg, cout, Z, dx, n, H, W, kh, kw, L.sh, L.sw, st, pk));
   return 0;
 }
 
@@ -981,18 +1011,23 @@ static bool c1_fused(const cgvc_engine* e, const Layer& L) {
   return e->opt.fuse_c1 && !use_tc(e, L.tc_slot) && L.a.cin == 1 && !L.has_in && L.a.kh * L.a.kw <= 9 && L.a.cout == 128;
 }
 
+// Packed utterances (A.off): the walk runs over one sample of all A.rows frames whose levels are packed 2-D grids, so n = 1 and T =
+// A.rows below; each convolution keeps to its utterance and each instance norm takes its statistics over its utterance (A.seg)
 static int discriminator_forward(cgvc_engine* e, const DiscNet& N, DiscActs& A, const float* x, cudaStream_t st, bool keep_y) {
-  const int n = A.n, T = A.T, H0 = e->cfg.num_features;
+  const int n = A.off ? 1 : A.n, T = A.off ? (int)A.rows : A.T, H0 = e->cfg.num_features;
   const float* Pm = e->P();
   A.x = x;
   ConvIO io; io.x = x; io.xhi = nullptr; io.xlo = nullptr; io.n = n; io.H = H0; io.W = T;
+  if (A.off) io.pk = PackGeom{A.off, A.n, 1, A.max_len};
   int H = H0, W = T / 2;
   // input layer: one input channel, K = 9, gate without norm; P is kept for the backward pass
   const LayerTensors t1 = layer_tensors(e, N.h1, false);
-  RET(disc_input_forward(e, N.h1, t1, x, n, H0, T, A.h1.P, post_params(e, N.h1, t1, io, A.h1, H * W, keep_y, A.post), c1_fused(e, N.h1), st));
+  RET(disc_input_forward(e, N.h1, t1, x, n, H0, T, A.h1.P, post_params(e, N.h1, t1, io, A.h1, H * W, keep_y, A.post), c1_fused(e, N.h1), st,
+                         packed(io)));
   const GLAct* cur = &A.h1;
   for (int i = 0; i < 3; ++i) {
     io.x = (keep_y || !cur->Yhi) ? cur->Y : nullptr; io.xhi = cur->Yhi; io.xlo = cur->Ylo; io.H = H; io.W = W;
+    if (A.off) { io.pk.div = T / W; io.seg_out = A.seg[i]; }
     int Ho, Wo; conv_out_dims(N.d[i].a, N.d[i].sh, N.d[i].sw, H, W, Ho, Wo); H = Ho; W = Wo;
     // d3 has no planes: its fp32 output feeds the head
     RET(layer_forward(e, N.d[i], layer_tensors(e, N.d[i], false), io, A.d[i], H * W, keep_y, true, e->opt.fuse_in, A.post, st));
@@ -1030,9 +1065,10 @@ static DiscActs disc_view(const cgvc_engine* e, const DiscActs& A, int s0, int n
 }
 
 // dY3: gradient w.r.t. the d3 GLU output [n*48, 1024].  wgrad: accumulate weight gradients.  d_in: optional [n,24,T].
+// Packed utterances (A.off): over one sample of all A.rows frames, as discriminator_forward
 static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscActs& A, const float* dY3, bool wgrad, float* d_in,
                                   const BwdScratch& S, cudaStream_t st) {
-  const int n = A.n, T = A.T, H0 = e->cfg.num_features;
+  const int n = A.off ? 1 : A.n, T = A.off ? (int)A.rows : A.T, H0 = e->cfg.num_features;
   int Hs[4] = {H0, H0 / 2, H0 / 4, H0 / 4}, Ws[4] = {T / 2, T / 4, T / 8, T / 16};   // output dims of h1, d1, d2, d3
   const float* dy = dY3;
   float* bufs[2] = {S.bufA, S.bufB};
@@ -1041,6 +1077,7 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   for (int i = 2; i >= 0; --i) {
     const GLAct& in = (i == 0) ? A.h1 : A.d[i - 1];
     ConvIO io; io.x = in.Y; io.xhi = in.Yhi; io.xlo = in.Ylo; io.n = n; io.H = Hs[i]; io.W = Ws[i];
+    if (A.off) { io.pk = PackGeom{A.off, A.n, T / Ws[i], A.max_len}; io.seg_out = A.seg[i]; }
     RET(layer_backward(e, w, N.d[i], A.d[i], io, dy, Hs[i + 1] * Ws[i + 1], wgrad, bufs[flip], 0, st));
     dy = bufs[flip]; flip ^= 1;
   }
@@ -1048,7 +1085,9 @@ static int discriminator_backward(cgvc_engine* e, const DiscNet& N, const DiscAc
   // data-gradient kernels, dP never goes to HBM.  D.h1 has no tensor-core slot, so the unfused form's dP is fp32 (no planes)
   const LayerTensors t = layer_tensors(e, N.h1, wgrad);
   const PostBwdParams q = post_bwd_params(e, N.h1, t, dy, A.h1, n, Hs[0] * Ws[0], S, true, PlanePair{S.dPhi, S.dPlo});
-  return disc_input_backward(e, N.h1, t, A.x, dy, A.h1.P, n, H0, T, d_in, bufs[flip], c1_fused(e, N.h1), q, det_of(S), st);
+  const PackGeom pk{A.off, A.n, 1, A.max_len};
+  return disc_input_backward(e, N.h1, t, A.x, dy, A.h1.P, n, H0, T, d_in, bufs[flip], c1_fused(e, N.h1), q, det_of(S), st,
+                             A.off ? &pk : nullptr);
 }
 
 // ---- workspace sizing ---------------------------------------------------------------------------------------
@@ -1115,11 +1154,16 @@ struct AppPlan { GenActs g; DiscActs d; float* x; long long* off; };
 static size_t plan_app(cgvc_engine* e, const NetGeom& a, void* base, bool tape, AppPlan& P) {
   const size_t head = tape ? kTapeHead : 0;
   Bump ws; ws.reset((char*)base + head, (size_t)1 << 62);
-  P.off = a.kind == 2 ? ws.take<long long>((size_t)a.n + 1) : nullptr;
+  // kind 3: the frame offsets, then the row prefix sums of the outputs of d1, d2 and d3 (DiscActs::seg), (n + 1) each
+  P.off = packed_kind(a.kind) ? ws.take<long long>((size_t)(a.kind == 3 ? 4 : 1) * (a.n + 1)) : nullptr;
   P.x = ws.take<float>((size_t)a.rows * e->cfg.num_features);
-  if (a.kind == 1) {
-    plan_discriminator(e, ws, P.d, a.n, a.T);
-    P.d.x = P.x;
+  if (disc_kind(a.kind)) {
+    plan_discriminator_rows(e, ws, P.d, a.n, a.rows);
+    P.d.T = a.T; P.d.x = P.x;
+    if (a.kind == 3) {
+      P.d.off = P.off; P.d.max_len = a.max_len;
+      for (int i = 0; i < 3; ++i) P.d.seg[i] = P.off + (size_t)(i + 1) * (a.n + 1);
+    }
   } else {
     plan_generator_rows(e, ws, P.g, a.n, a.rows);
     P.g.T = a.T; P.g.off = P.off; P.g.max_len = a.max_len; P.g.x_cl = P.x;
@@ -1131,7 +1175,7 @@ static size_t work_bytes_needed(cgvc_engine* e) {
   Bump ws; ws.reset(nullptr, 0);
   size_t need = 0;
   if (e->cfg.train) { TrainPlan P; plan_train(e, ws, P, e->cfg.max_batch, e->cfg.max_frames); need = ws.off; }
-  for (int kind = 0; kind < 3; ++kind) {      // the forwards at their largest (kind 2: max_batch utterances of max_batch x max_frames rows)
+  for (int kind = 0; kind < 4; ++kind) {      // the forwards at their largest (kinds 2, 3: max_batch utterances of max_batch x max_frames rows)
     AppPlan F;
     const size_t fwd = plan_app(e, net_geom(kind, 0, e->cfg.max_batch, e->cfg.max_frames), nullptr, false, F);
     if (fwd > need) need = fwd;
@@ -2581,25 +2625,26 @@ int cgvc_edge_h1_backward(cgvc_handle e, int direction, const float* x, const fl
 // checks them and sets a.rows and a.max_len; without them (cgvc_tape_bytes) it checks the a.rows given
 static int check_geom(cgvc_engine* e, NetGeom& a, const long long* off) {
   if (a.which != 0 && a.which != 1)
-    return a.kind == 1 ? fail(e, CGVC_ERR_ARG, "which must be 0 (discriminator_A) or 1 (discriminator_B)")
+    return disc_kind(a.kind) ? fail(e, CGVC_ERR_ARG, "which must be 0 (discriminator_A) or 1 (discriminator_B)")
                        : fail(e, CGVC_ERR_DIRECTION, "Conversion direction must be specified.");
-  if (a.kind != 2) return check_bt(e, a.n, a.T, a.kind == 0 ? 4 : 16);
+  if (!packed_kind(a.kind)) return check_bt(e, a.n, a.T, a.kind == 0 ? 4 : 16);
+  const int mult = a.kind == 3 ? 16 : 4;     // the discriminator halves time four times, the generator twice
   if (a.n < 1 || a.n > e->cfg.max_batch) return fail(e, CGVC_ERR_ARG, "%d utterances outside [1, %d]", a.n, e->cfg.max_batch);
   if (off) {
     if (off[0] != 0) return fail(e, CGVC_ERR_ARG, "offsets[0] is %lld, must be 0", off[0]);
     for (int u = 0; u < a.n; ++u) {
       const long long len = off[u + 1] - off[u];
-      if (len <= 0 || len % 4 != 0)
-        return fail(e, CGVC_ERR_ARG, "utterance %d: length %lld (offsets %lld .. %lld) must be a positive multiple of 4", u, len, off[u],
-                    off[u + 1]);
+      if (len <= 0 || len % mult != 0)
+        return fail(e, CGVC_ERR_ARG, "utterance %d: length %lld (offsets %lld .. %lld) must be a positive multiple of %d", u, len, off[u],
+                    off[u + 1], mult);
       if (len > a.max_len) a.max_len = (int)len;
     }
     a.rows = off[a.n];
   }
   const long long cap = (long long)e->cfg.max_batch * e->cfg.max_frames;
-  if (a.rows < 4ll * a.n || a.rows % 4 != 0 || a.rows > cap)
-    return fail(e, CGVC_ERR_ARG, "%lld frames of %d utterances: must be a multiple of 4 in [%d, %lld] (max_batch x max_frames)", a.rows,
-                a.n, 4 * a.n, cap);
+  if (a.rows < (long long)mult * a.n || a.rows % mult != 0 || a.rows > cap)
+    return fail(e, CGVC_ERR_ARG, "%lld frames of %d utterances: must be a multiple of %d in [%d, %lld] (max_batch x max_frames)", a.rows,
+                a.n, mult, mult * a.n, cap);
   return 0;
 }
 
@@ -2627,13 +2672,24 @@ static int generator_app(cgvc_engine* e, const NetGeom& a, AppPlan& P, const lon
 }
 
 // The discriminator from in to the probabilities out.  cgvc_discriminator_forward reads in where it is and keeps every fp32 layer
-// output (its taps); a tape forward copies in into the tape, where the input layer's backward reads it
-static int discriminator_app(cgvc_engine* e, const NetGeom& a, AppPlan& P, const float* in, float* out, bool tape, cudaStream_t st) {
+// output (its taps); a tape forward copies in into the tape, where the input layer's backward reads it.  Kind 3 (off: the host
+// offsets) also copies the offsets and the instance-norm segments of its levels, computed here, in front of its plan
+static int discriminator_app(cgvc_engine* e, const NetGeom& a, AppPlan& P, const long long* off, const float* in, float* out, bool tape,
+                             cudaStream_t st) {
   const int nf = e->cfg.num_features;
   CK(grow_post_buf(e, (size_t)a.n * 4 * 1024, &P.d.post));
+  if (P.off) {
+    const int Hl[3] = {nf / 2, nf / 4, nf / 4}, dl[3] = {4, 8, 16};      // (H, divisor) of the outputs of d1, d2, d3
+    std::vector<long long> h((size_t)4 * (a.n + 1));
+    for (int u = 0; u <= a.n; ++u) {
+      h[u] = off[u];
+      for (int i = 0; i < 3; ++i) h[(size_t)(i + 1) * (a.n + 1) + u] = Hl[i] * off[u] / dl[i];
+    }
+    CK(cudaMemcpyAsync(P.off, h.data(), h.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  }
   if (tape) CK(cudaMemcpyAsync(P.x, in, (size_t)a.rows * nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
   RET(discriminator_forward(e, e->disc[a.which], P.d, tape ? P.x : in, st, !tape));
-  CK(cudaMemcpyAsync(out, P.d.prob, (size_t)a.n * (nf / 4) * (a.T / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(out, P.d.prob, (size_t)(nf / 4) * (a.rows / 16) * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -2652,7 +2708,7 @@ struct TapeBuf { void* p; size_t bytes; };   // the caller's tape of a tape forw
 // refusal comes before anything is enqueued
 static int forward_app(cgvc_engine* e, NetGeom a, const long long* off, const float* in, float* out, const TapeBuf* tape, void* stream) {
   if (!e) return CGVC_ERR_ARG;
-  if (!in || !out || (a.kind == 2 && !off) || (tape && !tape->p)) return fail(e, CGVC_ERR_ARG, "null buffer");
+  if (!in || !out || (packed_kind(a.kind) && !off) || (tape && !tape->p)) return fail(e, CGVC_ERR_ARG, "null buffer");
   RET(check_geom(e, a, off));
   if (tape && ((uintptr_t)tape->p & 255)) return fail(e, CGVC_ERR_ARG, "a tape must be 256-byte aligned");
   RET(need_arenas(e, false));
@@ -2661,10 +2717,10 @@ static int forward_app(cgvc_engine* e, NetGeom a, const long long* off, const fl
   const size_t have = tape ? tape->bytes : e->arena_bytes[CGVC_ARENA_WORK];
   if (need > have)
     return fail(e, CGVC_ERR_UNBOUND, "%s of %zu bytes: %d %s of %lld frames in all need %zu", tape ? "tape" : "WORK arena", have, a.n,
-                a.kind == 2 ? "utterances" : "samples", a.rows, need);
+                packed_kind(a.kind) ? "utterances" : "samples", a.rows, need);
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  RET(a.kind == 1 ? discriminator_app(e, a, P, in, out, tape != nullptr, st) : generator_app(e, a, P, off, in, out, tape != nullptr, st));
+  RET(disc_kind(a.kind) ? discriminator_app(e, a, P, off, in, out, tape != nullptr, st) : generator_app(e, a, P, off, in, out, tape != nullptr, st));
   return tape ? tape_record(e, tape->p, TapeHeader{kTapeMagic, e->id, e->param_gen, a}, st) : 0;
 }
 
@@ -2678,8 +2734,8 @@ static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const
     return fail(e, CGVC_ERR_ARG, "%p is not a tape written by this engine's cgvc_*_forward_tape since its parameters last changed", tape);
   const TapeHeader& hd = it->second;
   if (hd.gen != e->param_gen) return fail(e, CGVC_ERR_ARG, "stale tape: the parameters changed after its forward");
-  static const char* const names[3] = {"generator", "discriminator", "packed generator"};
-  if ((hd.geom.kind == 1) != (kind == 1))    // the generator backward takes kinds 0 and 2
+  static const char* const names[4] = {"generator", "discriminator", "packed generator", "packed discriminator"};
+  if (disc_kind(hd.geom.kind) != (kind == 1))    // the generator backward takes kinds 0 and 2, the discriminator's 1 and 3
     return fail(e, CGVC_ERR_ARG, "a %s tape given to the %s backward", names[hd.geom.kind], names[kind]);
   if (!e->cfg.train || !e->arena[CGVC_ARENA_GRAD])
     return fail(e, CGVC_ERR_UNBOUND, "a tape backward needs the GRAD arena and a WORK arena sized for training (train = 1)");
@@ -2699,7 +2755,7 @@ static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const
 // gradient planes taken out (exact: a power of two)
 static int tape_din(cgvc_engine* e, const NetGeom& a, const AppPlan& P, const float* rows, float* din, float s, cudaStream_t st) {
   if (!din) return 0;
-  if (a.kind != 1) CK(transpose_app(e, a, P.g, rows, din, false, st));
+  if (!disc_kind(a.kind)) CK(transpose_app(e, a, P.g, rows, din, false, st));
   if (s != 1.f) CK(launch_scale(din, a.rows * e->cfg.num_features, 1.f / s, st));
   return 0;
 }
@@ -2726,10 +2782,15 @@ int cgvc_discriminator_forward(cgvc_handle e, int which, const float* in_dev, fl
   return forward_app(e, net_geom(1, which, batch, frames), nullptr, in_dev, out_dev, nullptr, stream);
 }
 
+int cgvc_discriminator_forward_packed(cgvc_handle e, int which, const float* in_dev, float* prob_dev, const long long* offsets_host, int n,
+                                      void* stream) {
+  return forward_app(e, net_geom(3, which, n, 0), offsets_host, in_dev, prob_dev, nullptr, stream);
+}
+
 int cgvc_tape_bytes(cgvc_handle e, int kind, int batch, int frames, size_t* bytes) {
-  if (!e || !bytes || kind < 0 || kind > 2) return fail(e, CGVC_ERR_ARG, "cgvc_tape_bytes: bad argument");
-  // kind 2: batch = n utterances, frames = rows = offsets[n]
-  NetGeom a = kind == 2 ? NetGeom{2, 0, batch, 0, frames, 0} : net_geom(kind, 0, batch, frames);
+  if (!e || !bytes || kind < 0 || kind > 3) return fail(e, CGVC_ERR_ARG, "cgvc_tape_bytes: bad argument");
+  // kinds 2, 3: batch = n utterances, frames = rows = offsets[n]
+  NetGeom a = packed_kind(kind) ? NetGeom{kind, 0, batch, 0, frames, 0} : net_geom(kind, 0, batch, frames);
   RET(check_geom(e, a, nullptr));
   AppPlan P;
   *bytes = plan_app(e, a, nullptr, true, P);
@@ -2746,6 +2807,12 @@ int cgvc_generator_forward_packed_tape(cgvc_handle e, int direction, const float
                                        void* tape_dev, size_t tape_bytes, void* stream) {
   const TapeBuf tape{tape_dev, tape_bytes};
   return forward_app(e, net_geom(2, direction, n, 0), offsets_host, in_dev, out_dev, &tape, stream);
+}
+
+int cgvc_discriminator_forward_packed_tape(cgvc_handle e, int which, const float* in_dev, float* prob_dev, const long long* offsets_host,
+                                           int n, void* tape_dev, size_t tape_bytes, void* stream) {
+  const TapeBuf tape{tape_dev, tape_bytes};
+  return forward_app(e, net_geom(3, which, n, 0), offsets_host, in_dev, prob_dev, &tape, stream);
 }
 
 int cgvc_discriminator_forward_tape(cgvc_handle e, int which, const float* in_dev, float* prob_dev, int batch, int frames, void* tape_dev,
@@ -2783,7 +2850,7 @@ int cgvc_discriminator_backward_tape(cgvc_handle e, const void* tape_dev, const 
   {
     TapeCounting counting(e, 1);
     // dz = s dprob p (1 - p) through the head: dY3 and the dense kernel / bias gradients
-    CK(launch_head_loss_bwd(P.d.prob, P.d.d[2].Y, (long long)a.n * (e->cfg.num_features / 4) * (a.T / 16), 1024, Pm + DN.dense_k, 0.f,
+    CK(launch_head_loss_bwd(P.d.prob, P.d.d[2].Y, (long long)(e->cfg.num_features / 4) * (a.rows / 16), 1024, Pm + DN.dense_k, 0.f,
                             0.f, nullptr, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, static_scale_dev(e, a.n), det_of(L.S), dprob_dev));
     RET(discriminator_backward(e, DN, P.d, L.dY3, true, din_dev, L.S, st));
   }

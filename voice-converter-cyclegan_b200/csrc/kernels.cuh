@@ -171,6 +171,31 @@ __device__ __forceinline__ int pack_find(const long long* __restrict__ off, int 
 }
 #endif
 
+// Packed variable-length 2-D grids (cgvc_discriminator_forward_packed): every length a multiple of 16, and a grid of H rows at divisor
+// div (<= 16) holds utterance u as [H][len_u / div] at rows H * off[u] / div ... H * off[u+1] / div, so that the levels of the
+// discriminator lie utterance after utterance.  A gather over such grids takes its GatherGeom from fwd_geom / dgrad_geoms(1, H, total
+// frames / div, ...) and its PackGeom as for the 1-D form: pk.div the source grid's divisor, pk.div * g.sx the output grid's and
+// pk.div * g.sx / g.dsx the destination grid's.  PackGeom2 is that PackGeom as the trailing argument of the 2-D kernel instantiations.
+struct PackGeom2 { PackGeom pk; };
+#ifdef __CUDACC__
+// row m of a grid of H rows at divisor div: its utterance u (frames o0 .. o1) and its (y, x) there
+struct Pack2Pos { int u; long long o0, o1; int y, x; };
+__device__ __forceinline__ Pack2Pos pack2_pos(const PackGeom& pk, int H, int div, long long m) {
+  Pack2Pos r;
+  r.u = pack_find(pk.off, pk.n, m * div / H);               // H off[u] / div <= m  <=>  off[u] <= floor(m div / H)
+  r.o0 = __ldg(pk.off + r.u); r.o1 = __ldg(pk.off + r.u + 1);
+  const int w = (int)((r.o1 - r.o0) / div);
+  const long long l = m - H * r.o0 / div;
+  r.y = (int)(l / w); r.x = (int)(l - (long long)r.y * w);
+  return r;
+}
+// the row of (y, x) of utterance o0 .. o1 in a grid of H rows at divisor div, or -1 outside its [0, H) x [0, len / div)
+__device__ __forceinline__ long long pack2_row(long long o0, long long o1, int H, int div, int y, int x) {
+  const int w = (int)((o1 - o0) / div);
+  return y >= 0 && y < H && x >= 0 && x < w ? H * o0 / div + (long long)y * w + x : -1;
+}
+#endif
+
 struct GemmOperands {
   const float* src; int s_ld; int s_coff; int C;      // gathered operand: row stride, column offset, #channels contracted
   const float* w; long long w_ts; int w_cs; int w_ns; // weight element (tap slab, c, n) = w[widx*w_ts + c*w_cs + n*w_ns]
@@ -183,7 +208,8 @@ struct GemmOperands {
 // ---- fp32 SIMT path (reference arithmetic on the GPU; also the permanent path for the tiny-K layers)
 cudaError_t launch_gg_simt(const GatherGeom& g, const GemmOperands& op, cudaStream_t st);
 // the same over a packed geometry: g = fwd_geom(1, 1, rows at the source level, 1, kw, 1, sw) of a 1-D layer, pk.div = the source
-// level's divisor; taps read only their own utterance's rows (TF-SAME zero padding at every utterance edge)
+// level's divisor; taps read only their own utterance's rows (TF-SAME zero padding at every utterance edge).  A geometry with more
+// than one row along y is a 2-D packed one (PackGeom2)
 cudaError_t launch_gg_simt_packed(const GatherGeom& g, const GemmOperands& op, const PackGeom& pk, cudaStream_t st);
 // weight gradient in forward geometry: dW[widx[t]][c][n] += sum_m S[src(m,t), c] * G[m, n]   (atomic accumulate)
 // pk: packed utterances, g and pk as launch_gg_simt_packed takes them; a tap outside its row's utterance contributes a zero row
@@ -282,10 +308,11 @@ cudaError_t launch_split_bf16(const float* x, __nv_bfloat16* hi, __nv_bfloat16* 
 // ---- single-input-channel specials (discriminator h1, K = 9, HBM-bound)
 // dW[t][0][n] += sum_m x[src(m,t)] * G[m,n]; columns [0,n_split) -> dw_a, the rest -> dw_g; db = column sums (optional)
 cudaError_t launch_wgrad_c1(const GatherGeom& g, const float* src, const float* grad, int g_ld, int N,
-                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det = nullptr);
+                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det = nullptr,
+                            const PackGeom* pk = nullptr);
 // dx[B,H,W] = conv-transpose of G [rows, C] with w = [wa | wg] ([taps][c_split], [taps][C - c_split]); Z is scratch [rows, taps]
 cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float* wg, int c_split, float* Z, float* dx,
-                            int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st);
+                            int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st, const PackGeom* pk = nullptr);
 // fp32 [M, C] (row stride ld) -> zero-padded bf16 hi/lo planes [M, Cpad]
 cudaError_t launch_pad_split(const float* x, long long M, int C, int ld, int Cpad, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t st);
 // same into F16F8 planes: q16 [M, Cpad] halves, q8 = [M*Cpad bytes of q8hi | M*Cpad bytes of q8lo] (activation scales)
@@ -304,14 +331,15 @@ cudaError_t launch_im2col_taps(const float* x, long long M, int T, int C, int kw
 cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int C, int kw, int dir, const float* bias, float* y, cudaStream_t st,
                                const long long* off = nullptr, int n_off = 0);
 // P[m, 0:2*cout] = [bias_a | bias_g] + sum_t x[src(m,t)] * [wa | wg][t]   (single input channel, TF kernels [taps][1][cout])
+// pk (both c1 forwards, may be null): x and P are packed 2-D grids (PackGeom2), g = fwd_geom(1, H, total frames, ...)
 cudaError_t launch_conv_c1_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
-                               int cout, float* P, cudaStream_t st);
+                               int cout, float* P, cudaStream_t st, const PackGeom* pk = nullptr);
 
 // ... and with the layer's GLU in the same pass (gate without instance norm): also y = a * sigmoid(g) as fp32 [M, cout] (optional) and as
 // operand planes (bf16 hi / lo, or with qmode the F16F8 planes q16; q8hi followed by q8lo); <= 9 taps
 cudaError_t launch_conv_c1_glu_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                                    int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st,
-                                   unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr);
+                                   unsigned long long* sat = nullptr, unsigned long long* ufl = nullptr, const PackGeom* pk = nullptr);
 
 // s[off .. off+n) = v6_host[0..n)  (n <= 6), passed by value in the kernel arguments (no host-memory copy node)
 cudaError_t launch_set_scalars(float* s, int off, int n, const float* v6_host, cudaStream_t st);
@@ -328,6 +356,8 @@ cudaError_t launch_gather_minibatch(const float* cA, const long long* off_A, con
 // formed in registers and consumed in place -- weight + bias gradients, or the data gradient (Z scratch [rows, taps]) -- instead of
 // being written to HBM and read back.  C = channels per branch (128).
 cudaError_t launch_glu_bwd_wgrad_c1(const GatherGeom& g, const float* src, const float* dy, const float* P, int C,
-                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det = nullptr);
+                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det = nullptr,
+                                    const PackGeom* pk = nullptr);
 cudaError_t launch_glu_bwd_dgrad_c1(const float* dy, const float* P, int C, const float* wa, const float* wg, float* Z, float* dx,
-                                    int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st);
+                                    int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st, const PackGeom* pk = nullptr);
+// pk (the six c1 kernels, may be null): x / dx, P and dy are packed 2-D grids (PackGeom2: B = 1, W = all frames, pk.div = 1)

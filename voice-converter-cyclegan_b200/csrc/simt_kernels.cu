@@ -19,12 +19,18 @@ unsigned long long g_cgvc_launches = 0;   // kernels launched by this library (b
 // ------------------------------------------------------------------------------------------------
 // Packed variable-length utterances (launch_gg_simt_packed; VEC only): the instantiations with one trailing PackGeom argument.  Their
 // A-row slots keep (first source row of the utterance, its length at the source level, local position * stride) where the dense form
-// keeps (b, y, x).  The dense instantiations take no such argument.
+// keeps (b, y, x).  The dense instantiations take no such argument.  With a trailing PackGeom2 (packed 2-D grids) the slots keep
+// (first source row of the utterance, y * sy, x * sx) and the utterance's source width, and the epilogue stores into the row's own
+// utterance of the destination grid.
 __device__ __forceinline__ const PackGeom& pack_arg(const PackGeom& p) { return p; }
+__device__ __forceinline__ const PackGeom& pack_arg(const PackGeom2& p) { return p.pk; }
+template <class... PKs> struct pack_is_2d { static constexpr bool value = false; };
+template <> struct pack_is_2d<PackGeom2> { static constexpr bool value = true; };
 template <int BM, int BK, bool VEC, class... PKs>
 __global__ void __launch_bounds__(256)
 gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ GemmOperands op, const PKs... pks) {
   constexpr bool PK = sizeof...(PKs) > 0;
+  constexpr bool PK2 = pack_is_2d<PKs...>::value;
   static_assert(VEC || !PK, "the packed form gathers 4-channel quads");
   constexpr int BN = 64;
   constexpr int TM = BM / 16;
@@ -49,6 +55,8 @@ gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ Gem
     constexpr int QPR = BK / 4;                       // quads per row
     constexpr int SLOTS = (BM * QPR + 255) / 256;
     int rb[SLOTS], ry[SLOTS], rx[SLOTS], rrow[SLOTS], rkq[SLOTS];
+    int rw[PK2 ? SLOTS : 1];                          // PK2: the source width of the row's utterance
+    long long rb2[PK2 ? SLOTS : 1];                   // PK2: the first source row of the row's utterance
     bool rvalid[SLOTS];
 #pragma unroll
     for (int s = 0; s < SLOTS; ++s) {
@@ -58,7 +66,11 @@ gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ Gem
       long long m = m0 + row;
       rvalid[s] = (idx < BM * QPR) && (m < M);
       long long mm = rvalid[s] ? m : 0;
-      if constexpr (PK) {
+      if constexpr (PK2) {
+        const PackGeom& pk = pack_arg(pks...);
+        const Pack2Pos o = pack2_pos(pk, g.Hy, pk.div * g.sx, mm);
+        rb2[s] = g.Hs * o.o0 / pk.div; rw[s] = (int)((o.o1 - o.o0) / pk.div); ry[s] = o.y * g.sy; rx[s] = o.x * g.sx;
+      } else if constexpr (PK) {
         const PackGeom& pk = pack_arg(pks...);
         const int dout = pk.div * g.sx;
         const int u = pack_find(pk.off, pk.n, mm * dout);
@@ -74,7 +86,11 @@ gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ Gem
       const float* aptr[SLOTS];
 #pragma unroll
       for (int s = 0; s < SLOTS; ++s) {
-        if constexpr (PK) {
+        if constexpr (PK2) {
+          const int yy = ry[s] + g.oy[t], xx = rx[s] + g.ox[t];
+          const bool ok = rvalid[s] && yy >= 0 && yy < g.Hs && xx >= 0 && xx < rw[s];
+          aptr[s] = ok ? op.src + (rb2[s] + (long long)yy * rw[s] + xx) * op.s_ld + op.s_coff + rkq[s] : nullptr;
+        } else if constexpr (PK) {
           const int xx = rx[s] + g.ox[t];
           aptr[s] = rvalid[s] && xx >= 0 && xx < ry[s] ? op.src + (long long)(rb[s] + xx) * op.s_ld + op.s_coff + rkq[s] : nullptr;
         } else {
@@ -176,9 +192,18 @@ gg_simt_kernel(const __grid_constant__ GatherGeom g, const __grid_constant__ Gem
   for (int i = 0; i < TM; ++i) {
     long long m = m0 + ty * TM + i;
     if (m >= M) continue;
-    int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
-    int y = rem / g.Wx; int x = rem - y * g.Wx;
-    long long drow = ((long long)(b * g.Hd + y * g.dsy + g.doy) * g.Wd + x * g.dsx + g.dox);
+    long long drow;
+    if constexpr (PK2) {
+      const PackGeom& pk = pack_arg(pks...);
+      const int dout = pk.div * g.sx;
+      const Pack2Pos o = pack2_pos(pk, g.Hy, dout, m);
+      drow = pack2_row(o.o0, o.o1, g.Hd, dout / g.dsx, o.y * g.dsy + g.doy, o.x * g.dsx + g.dox);
+      if (drow < 0) continue;                         // (a data-gradient class row always lies inside its utterance)
+    } else {
+      int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
+      int y = rem / g.Wx; int x = rem - y * g.Wx;
+      drow = ((long long)(b * g.Hd + y * g.dsy + g.doy) * g.Wd + x * g.dsx + g.dox);
+    }
     float* d = op.dst + drow * op.d_ld + op.d_coff;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -197,10 +222,19 @@ cudaError_t launch_gg_simt_packed(const GatherGeom& g, const GemmOperands& op, c
   const long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0 || op.N == 0) return cudaSuccess;
   const bool aligned = (op.s_ld % 4 == 0) && (op.s_coff % 4 == 0) && ((reinterpret_cast<uintptr_t>(op.src) & 15) == 0);
-  if (!pk.off || g.B != 1 || g.Hy != 1 || g.Hs != 1 || g.Hd != 1 || !aligned || op.C % 8) return cudaErrorInvalidValue;
+  if (!pk.off || g.B != 1 || !aligned || op.C % 8) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
   const dim3 block(256);
-  if (op.C % 16 == 0) {
+  if (g.Hy > 1 || g.Hs > 1 || g.Hd > 1) {                   // packed 2-D grids
+    const PackGeom2 p2{pk};
+    if (op.C % 16 == 0) {
+      if (M >= 4096) gg_simt_kernel<128, 16, true, PackGeom2><<<dim3((unsigned)((M + 127) / 128), (op.N + 63) / 64), block, 0, st>>>(g, op, p2);
+      else           gg_simt_kernel<64, 16, true, PackGeom2><<<dim3((unsigned)((M + 63) / 64), (op.N + 63) / 64), block, 0, st>>>(g, op, p2);
+    } else {
+      if (M >= 4096) gg_simt_kernel<128, 8, true, PackGeom2><<<dim3((unsigned)((M + 127) / 128), (op.N + 63) / 64), block, 0, st>>>(g, op, p2);
+      else           gg_simt_kernel<64, 8, true, PackGeom2><<<dim3((unsigned)((M + 63) / 64), (op.N + 63) / 64), block, 0, st>>>(g, op, p2);
+    }
+  } else if (op.C % 16 == 0) {
     if (M >= 4096) gg_simt_kernel<128, 16, true, PackGeom><<<dim3((unsigned)((M + 127) / 128), (op.N + 63) / 64), block, 0, st>>>(g, op, pk);
     else           gg_simt_kernel<64, 16, true, PackGeom><<<dim3((unsigned)((M + 63) / 64), (op.N + 63) / 64), block, 0, st>>>(g, op, pk);
   } else {
@@ -240,6 +274,7 @@ wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict_
                   const float* __restrict__ grad, int g_ld, int g_coff, int N,
                   float* __restrict__ dw, long long w_ts, int w_cs, int w_ns, int ksplit, const PKs... pks) {
   constexpr bool PK = sizeof...(PKs) > 0;
+  constexpr bool PK2 = pack_is_2d<PKs...>::value;
   static_assert(VEC || !PK, "the packed form reads 4-channel quads");
   __shared__ __align__(16) float As[16][64 + 4];
   __shared__ __align__(16) float Gs[16][64 + 4];
@@ -265,7 +300,12 @@ wgrad_simt_kernel(const __grid_constant__ GatherGeom g, const float* __restrict_
     long long m = mb + lrow;
     float4 av = make_float4(0.f, 0.f, 0.f, 0.f), gv = make_float4(0.f, 0.f, 0.f, 0.f);
     if (m < mend) {
-      if constexpr (PK) {
+      if constexpr (PK2) {                           // packed 2-D grids: a tap outside the row's utterance gives a zero row
+        const PackGeom& pk = pack_arg(pks...);
+        const Pack2Pos o = pack2_pos(pk, g.Hy, pk.div * g.sx, m);
+        const long long r = pack2_row(o.o0, o.o1, g.Hs, pk.div, o.y * g.sy + g.oy[t], o.x * g.sx + g.ox[t]);
+        if (r >= 0 && c0 + lq < C) av = *reinterpret_cast<const float4*>(src + r * s_ld + s_coff + c0 + lq);
+      } else if constexpr (PK) {
         const PackGeom& pk = pack_arg(pks...);
         const int dout = pk.div * g.sx;
         const int u = pack_find(pk.off, pk.n, m * dout);
@@ -330,7 +370,7 @@ cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, i
                               float* dw, long long w_ts, int w_cs, int w_ns, cudaStream_t st, int det, const PackGeom* pk) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
-  if (pk && (!pk->off || g.B != 1 || g.Hy != 1 || g.Hs != 1)) return cudaErrorInvalidValue;
+  if (pk && (!pk->off || g.B != 1)) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
   int tiles = ((N + 63) / 64) * ((C + 63) / 64) * g.ntaps;
   int ksplit = det ? 1 : (592 + tiles - 1) / tiles;       // det: one CTA, one thread and one add per element
@@ -341,7 +381,11 @@ cudaError_t launch_wgrad_simt(const GatherGeom& g, const float* src, int s_ld, i
   dim3 grid((N + 63) / 64, (C + 63) / 64, g.ntaps * ksplit);
   bool vec = (C % 4 == 0) && (N % 4 == 0) && (s_ld % 4 == 0) && (s_coff % 4 == 0) && (g_ld % 4 == 0) && (g_coff % 4 == 0) &&
              ((reinterpret_cast<uintptr_t>(src) & 15) == 0) && ((reinterpret_cast<uintptr_t>(grad) & 15) == 0);
-  if (pk) {
+  if (pk && (g.Hy > 1 || g.Hs > 1)) {                       // packed 2-D grids
+    if (!vec) return cudaErrorInvalidValue;
+    wgrad_simt_kernel<true, PackGeom2><<<grid, 256, 0, st>>>(g, src, s_ld, s_coff, C, grad, g_ld, g_coff, N, dw, w_ts, w_cs, w_ns, ksplit,
+                                                             PackGeom2{*pk});
+  } else if (pk) {
     if (!vec) return cudaErrorInvalidValue;
     wgrad_simt_kernel<true, PackGeom><<<grid, 256, 0, st>>>(g, src, s_ld, s_coff, C, grad, g_ld, g_coff, N, dw, w_ts, w_cs, w_ns, ksplit, *pk);
   }
@@ -1898,13 +1942,23 @@ cudaError_t launch_split_bf16(const float* x, __nv_bfloat16* hi, __nv_bfloat16* 
 // xs[row][tap] (zero outside the image / beyond m1).  All 256 threads participate.
 constexpr int kC1Rows = 64;
 constexpr int kC1Pad = 20;     // >= CGVC_MAX_TAPS, keeps rows 16-byte aligned
-__device__ __forceinline__ void c1_stage_taps(const GatherGeom& g, const float* __restrict__ src, long long m0, long long m1, float (*xs)[kC1Pad]) {
+// PKs: an optional trailing PackGeom2 (packed 2-D grids: every tap reads only its own utterance)
+template <class... PKs>
+__device__ __forceinline__ void c1_stage_taps(const GatherGeom& g, const float* __restrict__ src, long long m0, long long m1, float (*xs)[kC1Pad],
+                                              const PKs&... pks) {
   const int HW = g.Hy * g.Wx;
   for (int i = threadIdx.x; i < kC1Rows * g.ntaps; i += 256) {
     int rr = i / g.ntaps, t = i - rr * g.ntaps;
     long long m = m0 + rr;
     float v = 0.f;
-    if (m < m1) {
+    if constexpr (sizeof...(PKs) > 0) {
+      if (m < m1) {
+        const PackGeom& pk = pack_arg(pks...);
+        const Pack2Pos o = pack2_pos(pk, g.Hy, pk.div * g.sx, m);
+        const long long r = pack2_row(o.o0, o.o1, g.Hs, pk.div, o.y * g.sy + g.oy[t], o.x * g.sx + g.ox[t]);
+        if (r >= 0) v = src[r];
+      }
+    } else if (m < m1) {
       int b = (int)(m / HW); int rem = (int)(m - (long long)b * HW);
       int y = rem / g.Wx; int x = rem - y * g.Wx;
       int yy = y * g.sy + g.oy[t], xx = x * g.sx + g.ox[t];
@@ -1917,11 +1971,11 @@ __device__ __forceinline__ void c1_stage_taps(const GatherGeom& g, const float* 
 // weight gradient: dW[t][0][n] += sum_m x[src(m,t)] * G[m, n]   for n in [0, N), N <= 1024 (both branches at once).
 // thread = (column quad, position lane): G is streamed exactly once with 16-byte loads; the gathered inputs of 64 positions
 // are staged in shared memory per tile.
-template <int NT>
+template <int NT, class... PKs>
 __global__ void __launch_bounds__(256)
 wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ src, const float* __restrict__ grad, int g_ld, int N,
                 float* __restrict__ dw_a, float* __restrict__ dw_g, int n_split, float* __restrict__ db_a, float* __restrict__ db_g,
-                int rows_per_block, float* __restrict__ part) {
+                int rows_per_block, float* __restrict__ part, const PKs... pks) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   __shared__ float4 red[256];
   const int nq = N / 4;                                 // host guarantees nq divides 256
@@ -1935,7 +1989,7 @@ wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ 
   for (int t = 0; t <= NT; ++t) acc[t] = make_float4(0.f, 0.f, 0.f, 0.f);
   for (long long mb = r0; mb < r1; mb += kC1Rows) {
     __syncthreads();
-    c1_stage_taps(g, src, mb, r1, xs);
+    c1_stage_taps(g, src, mb, r1, xs, pks...);
     __syncthreads();
     const int cnt = (int)((r1 - mb) < kC1Rows ? (r1 - mb) : kC1Rows);
     for (int rr = rl; rr < cnt; rr += rstep) {
@@ -1975,17 +2029,21 @@ wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ 
 }
 
 cudaError_t launch_wgrad_c1(const GatherGeom& g, const float* src, const float* grad, int g_ld, int N,
-                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det) {
+                            float* dw_a, float* dw_g, int n_split, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det,
+                            const PackGeom* pk) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = N / 4;
-  if (N % 4 != 0 || nq > 256 || 256 % nq != 0 || n_split % 4 != 0 || g_ld % 4 != 0) return cudaErrorInvalidValue;
+  if (N % 4 != 0 || nq > 256 || 256 % nq != 0 || n_split % 4 != 0 || g_ld % 4 != 0 || (pk && (g.B != 1 || g.ntaps > 9)))
+    return cudaErrorInvalidValue;
   int rpb = (int)((M + CGVC_NUM_SMS * 8 - 1) / (CGVC_NUM_SMS * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
   const long long nb = (M + rpb - 1) / rpb, row = (long long)(g.ntaps + 1) * N, nt = g.ntaps;
   float* part = det ? det->p : nullptr;
   if (part && nb * row > det->cap) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
-  if (g.ntaps <= 9) wgrad_c1_kernel<9><<<(unsigned)nb, 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb, part);
+  if (pk) wgrad_c1_kernel<9, PackGeom2><<<(unsigned)nb, 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb, part,
+                                                                     PackGeom2{*pk});
+  else if (g.ntaps <= 9) wgrad_c1_kernel<9><<<(unsigned)nb, 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb, part);
   else wgrad_c1_kernel<CGVC_MAX_TAPS><<<(unsigned)nb, 256, 0, st>>>(g, src, grad, g_ld, N, dw_a, dw_g, n_split, db_a, db_g, rpb, part);
   if (!part) return cudaGetLastError();
   const long long na = n_split, ng = N - n_split;
@@ -1993,8 +2051,9 @@ cudaError_t launch_wgrad_c1(const GatherGeom& g, const float* src, const float* 
                                                     {nt * na, nt * ng, db_a ? na : 0, db_g ? ng : 0}}, st);
 }
 
+template <class... PKs>
 __global__ void gather_taps_kernel(const float* __restrict__ Z, float* __restrict__ dx, int B, int H, int W, int Ho, int Wo, int kh, int kw,
-                                   int sh, int sw, int ph, int pw);
+                                   int sh, int sw, int ph, int pw, const PKs... pks);
 // ---- discriminator input layer (one input channel, K = 9, no instance norm: module.py:196-199), backward fused --------------------
 // Its gated output is the largest activation of the step (805 MB of pre-activations per lane at batch 256), and its backward
 // used to be: GLU backward -> dP fp32 written, then read again by the weight gradient and by the data-gradient projection.  The two
@@ -2003,11 +2062,12 @@ __global__ void gather_taps_kernel(const float* __restrict__ Z, float* __restric
 //   glu_bwd_proj_c1_kernel:   Z[m,t] = sum_n dP[m,n] w[t][n]  (then gather_taps)                 (adversarial pass, the B fakes)
 // so dP never touches HBM (-1.6 GB and -0.8 GB per lane).  C = channels per branch (128): thread = (column quad j of BOTH branches,
 // position lane).
-template <int NT>
+template <int NT, class... PKs>
 __global__ void __launch_bounds__(256)
 glu_bwd_wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ src, const float* __restrict__ dy,
                         const float* __restrict__ P, int C, float* __restrict__ dw_a, float* __restrict__ dw_g,
-                        float* __restrict__ db_a, float* __restrict__ db_g, int rows_per_block, float* __restrict__ part) {
+                        float* __restrict__ db_a, float* __restrict__ db_g, int rows_per_block, float* __restrict__ part,
+                        const PKs... pks) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   __shared__ float4 red[256];
   const int nq = C / 4;                                 // column quads per branch; host guarantees nq divides 256
@@ -2021,7 +2081,7 @@ glu_bwd_wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __res
   for (int t = 0; t <= NT; ++t) { acc_a[t] = make_float4(0.f, 0.f, 0.f, 0.f); acc_g[t] = make_float4(0.f, 0.f, 0.f, 0.f); }
   for (long long mb = r0; mb < r1; mb += kC1Rows) {
     __syncthreads();
-    c1_stage_taps(g, src, mb, r1, xs);
+    c1_stage_taps(g, src, mb, r1, xs, pks...);
     __syncthreads();
     const int cnt = (int)((r1 - mb) < kC1Rows ? (r1 - mb) : kC1Rows);
 #pragma unroll 2
@@ -2071,17 +2131,20 @@ glu_bwd_wgrad_c1_kernel(const __grid_constant__ GatherGeom g, const float* __res
 }
 
 cudaError_t launch_glu_bwd_wgrad_c1(const GatherGeom& g, const float* src, const float* dy, const float* P, int C,
-                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det) {
+                                    float* dw_a, float* dw_g, float* db_a, float* db_g, cudaStream_t st, const DetSlab* det,
+                                    const PackGeom* pk) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = C / 4;
-  if (C % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9) return cudaErrorInvalidValue;
+  if (C % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9 || (pk && g.B != 1)) return cudaErrorInvalidValue;
   int rpb = (int)((M + CGVC_NUM_SMS * 8 - 1) / (CGVC_NUM_SMS * 8)); rpb = (rpb + kC1Rows - 1) / kC1Rows * kC1Rows;
   const long long nb = (M + rpb - 1) / rpb, nt = g.ntaps, Cl = C, row = 2 * (nt + 1) * Cl;
   float* part = det ? det->p : nullptr;
   if (part && nb * row > det->cap) return cudaErrorInvalidValue;
   ++g_cgvc_launches;
-  glu_bwd_wgrad_c1_kernel<9><<<(unsigned)nb, 256, 0, st>>>(g, src, dy, P, C, dw_a, dw_g, db_a, db_g, rpb, part);
+  if (pk) glu_bwd_wgrad_c1_kernel<9, PackGeom2><<<(unsigned)nb, 256, 0, st>>>(g, src, dy, P, C, dw_a, dw_g, db_a, db_g, rpb, part,
+                                                                             PackGeom2{*pk});
+  else glu_bwd_wgrad_c1_kernel<9><<<(unsigned)nb, 256, 0, st>>>(g, src, dy, P, C, dw_a, dw_g, db_a, db_g, rpb, part);
   if (!part) return cudaGetLastError();
   return launch_reduce_parts(part, nb, row, DetSegs{{dw_a, dw_g, db_a, db_g}, {0, nt * Cl, 2 * nt * Cl, (2 * nt + 1) * Cl},
                                                     {nt * Cl, nt * Cl, db_a ? Cl : 0, db_g ? Cl : 0}}, st);
@@ -2146,7 +2209,7 @@ glu_bwd_proj_c1_kernel(const float* __restrict__ dy, const float* __restrict__ P
 }
 
 cudaError_t launch_glu_bwd_dgrad_c1(const float* dy, const float* P, int C, const float* wa, const float* wg, float* Z, float* dx,
-                                    int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st) {
+                                    int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st, const PackGeom* pk) {
   int Ho = (H + sh - 1) / sh, Wo = (W + sw - 1) / sw;
   int th = (Ho - 1) * sh + kh - H; if (th < 0) th = 0; int tw = (Wo - 1) * sw + kw - W; if (tw < 0) tw = 0;
   int ph = th / 2, pw = tw / 2;
@@ -2157,7 +2220,8 @@ cudaError_t launch_glu_bwd_dgrad_c1(const float* dy, const float* P, int C, cons
   g_cgvc_launches += 2;
   glu_bwd_proj_c1_kernel<<<(unsigned)nb, 256, 0, st>>>(dy, P, rows, wa, wg, kh * kw, Z);
   long long n = (long long)B * H * W; long long nb2 = (n + 255) / 256; if (nb2 > CGVC_NUM_SMS * 16) nb2 = CGVC_NUM_SMS * 16;
-  gather_taps_kernel<<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw);
+  if (pk) gather_taps_kernel<PackGeom2><<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, PackGeom2{*pk});
+  else gather_taps_kernel<<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw);
   return cudaGetLastError();
 }
 
@@ -2201,12 +2265,30 @@ proj_taps_kernel(const float* __restrict__ G, long long rows, int C, const float
   }
 }
 
+// PKs: an optional trailing PackGeom2 (packed 2-D grids, B = 1, W = all frames): position idx of the input grid (divisor pk.div)
+// sums only the Z rows of its own utterance in the output grid (divisor pk.div * sw)
+template <class... PKs>
 __global__ void __launch_bounds__(256)
 gather_taps_kernel(const float* __restrict__ Z, float* __restrict__ dx, int B, int H, int W, int Ho, int Wo, int kh, int kw,
-                   int sh, int sw, int ph, int pw) {
+                   int sh, int sw, int ph, int pw, const PKs... pks) {
   long long n = (long long)B * H * W;
   const int ntaps = kh * kw;
   for (long long idx = (long long)blockIdx.x * 256 + threadIdx.x; idx < n; idx += (long long)gridDim.x * 256) {
+    if constexpr (sizeof...(PKs) > 0) {
+      const PackGeom& pk = pack_arg(pks...);
+      const Pack2Pos o = pack2_pos(pk, H, pk.div, idx);
+      float a = 0.f;
+      for (int i = 0; i < kh; ++i) {
+        int ny = o.y + ph - i; if (ny < 0 || ny % sh) continue;
+        for (int j = 0; j < kw; ++j) {
+          int nx = o.x + pw - j; if (nx < 0 || nx % sw) continue;
+          const long long r = pack2_row(o.o0, o.o1, Ho, pk.div * sw, ny / sh, nx / sw);
+          if (r >= 0) a += Z[r * ntaps + i * kw + j];
+        }
+      }
+      dx[idx] = a;
+      continue;
+    }
     int w = (int)(idx % W); long long r = idx / W; int h = (int)(r % H); int b = (int)(r / H);
     float a = 0.f;
     for (int i = 0; i < kh; ++i) {
@@ -2221,7 +2303,7 @@ gather_taps_kernel(const float* __restrict__ Z, float* __restrict__ dx, int B, i
 }
 
 cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float* wg, int c_split, float* Z, float* dx,
-                            int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st) {
+                            int B, int H, int W, int kh, int kw, int sh, int sw, cudaStream_t st, const PackGeom* pk) {
   int Ho = (H + sh - 1) / sh, Wo = (W + sw - 1) / sw;
   int th = (Ho - 1) * sh + kh - H; if (th < 0) th = 0; int tw = (Wo - 1) * sw + kw - W; if (tw < 0) tw = 0;
   int ph = th / 2, pw = tw / 2;
@@ -2233,7 +2315,8 @@ cudaError_t launch_dgrad_c1(const float* G, int C, const float* wa, const float*
   g_cgvc_launches += 2;
   proj_taps_kernel<<<(unsigned)nb, 256, smem, st>>>(G, rows, C, wa, wg, c_split, kh * kw, Z);
   long long n = (long long)B * H * W; long long nb2 = (n + 255) / 256; if (nb2 > CGVC_NUM_SMS * 16) nb2 = CGVC_NUM_SMS * 16;
-  gather_taps_kernel<<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw);
+  if (pk) gather_taps_kernel<PackGeom2><<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, PackGeom2{*pk});
+  else gather_taps_kernel<<<(unsigned)nb2, 256, 0, st>>>(Z, dx, B, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw);
   return cudaGetLastError();
 }
 
@@ -2384,10 +2467,11 @@ cudaError_t launch_col2im_taps(const float* z, int ldz, long long M, int T, int 
 
 // forward of the single-input-channel gated layer: P[m, n] = bias[n] + sum_t x[src(m,t)] * w[t][n], n over [a | g] columns.
 // HBM-bound on the output write (N*4 bytes per position); one thread = one column quad, 4 positions per CTA sweep.
-template <int NT>
+template <int NT, class... PKs>
 __global__ void __launch_bounds__(256)
 conv_c1_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ x, const float* __restrict__ wa, const float* __restrict__ wg,
-                   const float* __restrict__ ba, const float* __restrict__ bg, int cout, float* __restrict__ P, int rows_per_block) {
+                   const float* __restrict__ ba, const float* __restrict__ bg, int cout, float* __restrict__ P, int rows_per_block,
+                   const PKs... pks) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   const int nq = (2 * cout) / 4;                       // column quads (host guarantees nq divides 256)
   const int cq = threadIdx.x % nq, rl = threadIdx.x / nq, rstep = 256 / nq;
@@ -2402,7 +2486,7 @@ conv_c1_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __restrict
   long long m1 = m0 + rows_per_block < M ? m0 + rows_per_block : M;
   for (long long mb = m0; mb < m1; mb += kC1Rows) {
     __syncthreads();
-    c1_stage_taps(g, x, mb, m1, xs);
+    c1_stage_taps(g, x, mb, m1, xs, pks...);
     __syncthreads();
     const int cnt = (int)((m1 - mb) < kC1Rows ? (m1 - mb) : kC1Rows);
     for (int rr = rl; rr < cnt; rr += rstep) {
@@ -2420,14 +2504,15 @@ conv_c1_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __restrict
 }
 
 cudaError_t launch_conv_c1_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
-                               int cout, float* P, cudaStream_t st) {
+                               int cout, float* P, cudaStream_t st, const PackGeom* pk) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = (2 * cout) / 4;
-  if (cout % 4 != 0 || nq > 256 || 256 % nq != 0) return cudaErrorInvalidValue;
+  if (cout % 4 != 0 || nq > 256 || 256 % nq != 0 || (pk && (g.B != 1 || g.ntaps > 9))) return cudaErrorInvalidValue;
   int rpb = 4 * kC1Rows;
   ++g_cgvc_launches;
-  if (g.ntaps <= 9) conv_c1_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, rpb);
+  if (pk) conv_c1_fwd_kernel<9, PackGeom2><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, rpb, PackGeom2{*pk});
+  else if (g.ntaps <= 9) conv_c1_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, rpb);
   else conv_c1_fwd_kernel<CGVC_MAX_TAPS><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, rpb);
   return cudaGetLastError();
 }
@@ -2435,12 +2520,12 @@ cudaError_t launch_conv_c1_fwd(const GatherGeom& g, const float* x, const float*
 // The same layer with its GLU (gate without instance norm, module.py:193-195) in the same pass: one thread computes the a-quad AND the
 // g-quad of 4 channels, writes both to P (kept for the backward pass) and y = a * sigmoid(g) to the operand planes of the next layer
 // (+ the fp32 copy when asked) -- P is not read back by a second kernel (B*24*64*256*4 bytes per application of the discriminator).
-template <int NT>
+template <int NT, class... PKs>
 __global__ void __launch_bounds__(256)
 conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __restrict__ x, const float* __restrict__ wa, const float* __restrict__ wg,
                        const float* __restrict__ ba, const float* __restrict__ bg, int cout, float* __restrict__ P,
                        float* __restrict__ y, __nv_bfloat16* __restrict__ y_hi, __nv_bfloat16* __restrict__ y_lo, int qmode, long long plane_elems,
-                       int rows_per_block, unsigned long long* __restrict__ sat, unsigned long long* __restrict__ ufl) {
+                       int rows_per_block, unsigned long long* __restrict__ sat, unsigned long long* __restrict__ ufl, const PKs... pks) {
   __shared__ __align__(16) float xs[kC1Rows][kC1Pad];
   const int nq = cout / 4;                             // channel quads (host guarantees nq divides 256)
   const int cq = threadIdx.x % nq, rl = threadIdx.x / nq, rstep = 256 / nq;
@@ -2457,7 +2542,7 @@ conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __rest
   long long m1 = m0 + rows_per_block < M ? m0 + rows_per_block : M;
   for (long long mb = m0; mb < m1; mb += kC1Rows) {
     __syncthreads();
-    c1_stage_taps(g, x, mb, m1, xs);
+    c1_stage_taps(g, x, mb, m1, xs, pks...);
     __syncthreads();
     const int cnt = (int)((m1 - mb) < kC1Rows ? (m1 - mb) : kC1Rows);
     for (int rr = rl; rr < cnt; rr += rstep) {
@@ -2487,14 +2572,16 @@ conv_c1_glu_fwd_kernel(const __grid_constant__ GatherGeom g, const float* __rest
 
 cudaError_t launch_conv_c1_glu_fwd(const GatherGeom& g, const float* x, const float* wa, const float* wg, const float* ba, const float* bg,
                                    int cout, float* P, float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, int qmode, cudaStream_t st,
-                                   unsigned long long* sat, unsigned long long* ufl) {
+                                   unsigned long long* sat, unsigned long long* ufl, const PackGeom* pk) {
   long long M = (long long)g.B * g.Hy * g.Wx;
   if (M == 0) return cudaSuccess;
   int nq = cout / 4;
-  if (cout % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9) return cudaErrorInvalidValue;
+  if (cout % 4 != 0 || nq > 256 || 256 % nq != 0 || g.ntaps > 9 || (pk && g.B != 1)) return cudaErrorInvalidValue;
   int rpb = 4 * kC1Rows;
   ++g_cgvc_launches;
-  conv_c1_glu_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode, M * cout, rpb, sat, ufl);
+  if (pk) conv_c1_glu_fwd_kernel<9, PackGeom2><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode,
+                                                                                                M * cout, rpb, sat, ufl, PackGeom2{*pk});
+  else conv_c1_glu_fwd_kernel<9><<<(unsigned)((M + rpb - 1) / rpb), 256, 0, st>>>(g, x, wa, wg, ba, bg, cout, P, y, y_hi, y_lo, qmode, M * cout, rpb, sat, ufl);
   return cudaGetLastError();
 }
 

@@ -201,9 +201,16 @@ __device__ __forceinline__ RowPos nt_row(const TcNTParams& p, long long m) {
   r.x = (int)(rem - (uint32_t)r.b * p.div_w.d);
   return r;
 }
-// the taps the tile of rows m0 .. m0 + 127 contracts over: the same list for its producers and its consumers
+// the taps the tile of rows m0 .. m0 + 127 contracts over: the same list for its producers and its consumers.  PK 2 (packed 2-D
+// grids): a tile inside one utterance drops the taps as the dense form does, a tile that spans utterances walks every tap
+template <int PK = 0>
 __device__ __forceinline__ uint32_t nt_tile_taps(const TcNTParams& p, long long m0, long long M) {
   const long long m1 = m0 + 127 < M ? m0 + 127 : M - 1;
+  if constexpr (PK == 2) {
+    const int dout = p.pk.div * p.g.sx;
+    const Pack2Pos a = pack2_pos(p.pk, p.g.Hy, dout, m0), b = pack2_pos(p.pk, p.g.Hy, dout, m1);
+    return a.u == b.u ? gather_tap_mask(p.g, a.y, b.y) : (1u << p.g.ntaps) - 1u;
+  }
   return gather_tap_mask(p.g, nt_row(p, m0).y, nt_row(p, m1).y);
 }
 
@@ -826,7 +833,8 @@ __device__ __forceinline__ void rescale_acc(float (&d)[N], float scale) {
 // This thread's fragments are tile rows r and r + 8, columns 8 j + c + {0, 1} of every 8-column block j (c = 2 (t % 4)).  y = D (+ bias),
 // stored or (accumulate) added.  One float2 store of a warp covers 8 rows x 32 contiguous bytes: whole sectors.  Nothing passes through
 // the pipeline stages, so the producers fill them with the next tile's operands meanwhile.
-template <int BN>
+// PK 2: row m of the packed output grid goes to its own utterance's rows of the packed destination grid
+template <int BN, int PK = 0>
 __device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const float (&d)[BN / 2], const long long M,
                                                    const long long m0, const int n0, const int r, const int c) {
   const GatherGeom& g = p.g;
@@ -836,8 +844,15 @@ __device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const fl
     const long long m = m0 + r + 8 * h;
     rowp[h] = nullptr;
     if (m < M && p.dst) {
-      const RowPos o = nt_row(p, m);
-      rowp[h] = p.dst + ((long long)(o.b * g.Hd + o.y * g.dsy + g.doy) * g.Wd + o.x * g.dsx + g.dox) * p.d_ld;
+      if constexpr (PK == 2) {
+        const int dout = p.pk.div * g.sx;
+        const Pack2Pos o = pack2_pos(p.pk, g.Hy, dout, m);
+        const long long r = pack2_row(o.o0, o.o1, g.Hd, dout / g.dsx, o.y * g.dsy + g.doy, o.x * g.dsx + g.dox);
+        if (r >= 0) rowp[h] = p.dst + r * p.d_ld;            // (a data-gradient class row always lies inside its utterance)
+      } else {
+        const RowPos o = nt_row(p, m);
+        rowp[h] = p.dst + ((long long)(o.b * g.Hd + o.y * g.dsy + g.doy) * g.Wd + o.x * g.dsx + g.dox) * p.d_ld;
+      }
     }
   }
   const bool vec = (p.d_ld & 1) == 0;
@@ -881,9 +896,11 @@ __device__ __forceinline__ void nt_store_fragments(const TcNTParams& p, const fl
 //               the epilogue in two groups of 4.  (The accumulator of a 256-wide tile does not fit next to the stages: 128 KB.)
 constexpr int kNTThreads = 384;
 
-// PK: the packed form (cgvc_generator_forward_packed).  Row m's source rows are those of its own utterance: the producers keep
+// PK 1: the packed form (cgvc_generator_forward_packed).  Row m's source rows are those of its own utterance: the producers keep
 // (first source row of the utterance, its length at the source level, local position * stride) where the dense form keeps (b, y, x).
-template <int BN, int NPL, int EPI, bool PK = false>
+// PK 2: the packed 2-D form (cgvc_discriminator_forward_packed, kernels.cuh PackGeom2): the producers keep (first source row of the
+// utterance, y * sy, x * sx) and the utterance's source width
+template <int BN, int NPL, int EPI, int PK = 0>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   static_assert(!PK || EPI == 0, "packed rows never take the fused epilogues (they need whole equal-length samples per tile)");
@@ -934,13 +951,17 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
       const long long m0 = (long long)(n_fast ? tile / n_tiles : tile % m_tiles) * 128;
       const int n0 = (n_fast ? tile % n_tiles : tile / m_tiles) * BN;
       if (EPI != 0 && it > 0) mbar_wait(&acc_free_bar, (uint32_t)(it - 1) & 1u);   // the previous tile's epilogue has left the stages
-      const uint32_t taps = nt_tile_taps(p, m0, M);
+      const uint32_t taps = nt_tile_taps<PK>(p, m0, M);
       int rb[8], ry[8], rx[8];                              // decoded output coordinates of this thread's 8 A rows
+      int rw[PK == 2 ? 8 : 1];                              // PK 2: the source width of the row's utterance
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         long long m = m0 + rsub + 16 * i;
         if (m < M) {
-          if constexpr (PK) {                                // rb = first source row, ry = source length, rx = local position * stride
+          if constexpr (PK == 2) {
+            const Pack2Pos o = pack2_pos(p.pk, g.Hy, p.pk.div * g.sx, m);
+            rb[i] = (int)(g.Hs * o.o0 / p.pk.div); rw[i] = (int)((o.o1 - o.o0) / p.pk.div); ry[i] = o.y * g.sy; rx[i] = o.x * g.sx;
+          } else if constexpr (PK) {                         // rb = first source row, ry = source length, rx = local position * stride
             const int dout = p.pk.div * g.sx;
             const int u = pack_find(p.pk.off, p.pk.n, m * dout);
             const long long o0 = __ldg(p.pk.off + u), o1 = __ldg(p.pk.off + u + 1);
@@ -958,7 +979,10 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int cofs = NPL == 3 && pass == 0 ? (chunk & 3) * 16 : chunk * 8;
-          if constexpr (PK) {
+          if constexpr (PK == 2) {
+            const int yy = ry[i] + g.oy[tap], xx = rx[i] + g.ox[tap];
+            aoff[i] = rb[i] >= 0 && yy >= 0 && yy < g.Hs && xx >= 0 && xx < rw[i] ? ((long long)rb[i] + yy * rw[i] + xx) * p.a_ld + cofs : -1;
+          } else if constexpr (PK) {
             const int xx = rx[i] + g.ox[tap];
             aoff[i] = rb[i] >= 0 && xx >= 0 && xx < ry[i] ? (long long)(rb[i] + xx) * p.a_ld + cofs : -1;
           } else {
@@ -1023,7 +1047,7 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       int prev = -1;                                         // stage whose MMAs may still be in flight
-      const int kb_pass = __popc(nt_tile_taps(p, m0, M)) * cchunks;   // (> 0 for TF-SAME geometries; 0 is safe)
+      const int kb_pass = __popc(nt_tile_taps<PK>(p, m0, M)) * cchunks;   // (> 0 for TF-SAME geometries; 0 is safe)
       if constexpr (NPL == 3) {                             // e4m3 cross products, then the fp16 hi x hi products after the rescale of D
         consume_stages<BN, MMA_E4M3_CROSS, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
         rescale_acc(d, 1.f / (float)(1 << CGVC_Q_ACC_SHIFT));
@@ -1036,7 +1060,7 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       const int r0 = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2), c0 = 2 * (tw & 3);   // this thread's fragment rows r0, r0 + 8
       if constexpr (EPI == 0) {
-        if (!(p.debug & 3)) nt_store_fragments<BN>(p, d, M, m0, n0, r0, c0);
+        if (!(p.debug & 3)) nt_store_fragments<BN, PK>(p, d, M, m0, n0, r0, c0);
       } else {
         // the tile into shared memory once both warpgroups are done reading the stages
         consumer_bar();
@@ -1083,7 +1107,9 @@ struct TNCfg {
 // adds the partials in K-split order (launch_reduce_parts)
 // PK: the packed form (packed generator tapes).  K-row m (an output row of all packed rows) gathers its source row from its own
 // utterance u = pack_find(m * dout): local position (m - off[u] / dout) * stride + tap offset, a zero row outside [0, len_u / div)
-template <int NPL, int W16, int DET, bool PK = false>
+// PK 2: packed 2-D grids (kernels.cuh PackGeom2): K-row m finds (u, y, x) in the output grid and reads its own utterance's source row,
+// a zero row outside it
+template <int NPL, int W16, int DET, int PK = 0>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   static_assert(W16 == 0 || NPL == 3, "the fp16-only weight gradient is a form of CGVC_PREC_F16F8");
@@ -1143,7 +1169,11 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
           const long long m = w.mbeg + (long long)kb * 64 + rsub + 16 * i;
           xoff[i] = -1;
           if (m < w.mend) {
-            if constexpr (PK) {
+            if constexpr (PK == 2) {
+              const Pack2Pos o = pack2_pos(p.pk, g.Hy, p.pk.div * g.sx, m);
+              const long long r = pack2_row(o.o0, o.o1, g.Hs, p.pk.div, o.y * g.sy + g.oy[w.tap], o.x * g.sx + g.ox[w.tap]);
+              if (r >= 0) xoff[i] = r * p.x_ld + w.c0 + chunk * 8;
+            } else if constexpr (PK) {
               const int dout = p.pk.div * g.sx;
               const int u = pack_find(p.pk.off, p.pk.n, m * dout);
               const long long o0 = __ldg(p.pk.off + u), o1 = __ldg(p.pk.off + u + 1);
@@ -1496,12 +1526,19 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
     tc_gg_nt_kernel<BN_, NPL_, EPI_, ##__VA_ARGS__><<<grid, kNTThreads, NTCfg<BN_, NPL_>::SMEM, st>>>(p);      \
   } while (0)
   if (epi != 0 && bn != 256) return cudaErrorInvalidValue;
-  if (p.pk.off) {                                           // packed utterances: plain epilogue only
+  if (p.pk.off && (p.g.Hy > 1 || p.g.Hs > 1 || p.g.Hd > 1)) {   // packed 2-D grids (the discriminator's layers)
+    if (epi != 0 || p.g.B != 1 || p.g.ntaps > 31) return cudaErrorInvalidValue;
+    const int npl = precision == 3 ? 3 : x3 ? 2 : 1;
+    if (bn == 256)      { if (npl == 3) LAUNCH_NT(256, 3, 0, 2); else if (npl == 2) LAUNCH_NT(256, 2, 0, 2); else LAUNCH_NT(256, 1, 0, 2); }
+    else if (bn == 128) { if (npl == 3) LAUNCH_NT(128, 3, 0, 2); else if (npl == 2) LAUNCH_NT(128, 2, 0, 2); else LAUNCH_NT(128, 1, 0, 2); }
+    else                { if (npl == 3) LAUNCH_NT(32, 3, 0, 2);  else if (npl == 2) LAUNCH_NT(32, 2, 0, 2);  else LAUNCH_NT(32, 1, 0, 2); }
+  }
+  else if (p.pk.off) {                                      // packed utterances: plain epilogue only
     if (epi != 0 || p.g.B != 1 || p.g.Hy != 1) return cudaErrorInvalidValue;
     const int npl = precision == 3 ? 3 : x3 ? 2 : 1;
-    if (bn == 256)      { if (npl == 3) LAUNCH_NT(256, 3, 0, true); else if (npl == 2) LAUNCH_NT(256, 2, 0, true); else LAUNCH_NT(256, 1, 0, true); }
-    else if (bn == 128) { if (npl == 3) LAUNCH_NT(128, 3, 0, true); else if (npl == 2) LAUNCH_NT(128, 2, 0, true); else LAUNCH_NT(128, 1, 0, true); }
-    else                { if (npl == 3) LAUNCH_NT(32, 3, 0, true);  else if (npl == 2) LAUNCH_NT(32, 2, 0, true);  else LAUNCH_NT(32, 1, 0, true); }
+    if (bn == 256)      { if (npl == 3) LAUNCH_NT(256, 3, 0, 1); else if (npl == 2) LAUNCH_NT(256, 2, 0, 1); else LAUNCH_NT(256, 1, 0, 1); }
+    else if (bn == 128) { if (npl == 3) LAUNCH_NT(128, 3, 0, 1); else if (npl == 2) LAUNCH_NT(128, 2, 0, 1); else LAUNCH_NT(128, 1, 0, 1); }
+    else                { if (npl == 3) LAUNCH_NT(32, 3, 0, 1);  else if (npl == 2) LAUNCH_NT(32, 2, 0, 1);  else LAUNCH_NT(32, 1, 0, 1); }
   }
   else if (precision == 3) {                                // F16F8 (no fused backward epilogues in this precision)
     if (epi == 1)       LAUNCH_NT(256, 3, 1);
@@ -1562,16 +1599,27 @@ cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st, const DetSla
     if (e != cudaSuccess) return e;                                                                           \
     tc_gg_tn_kernel<NPL_, W16_, DET_, ##__VA_ARGS__><<<grid, kNTThreads, TNCfg<NPL_, W16_>::SMEM, st>>>(p);   \
   } while (0)
-  if (p.pk.off) {                                           // packed utterances
+  if (p.pk.off && (p.g.Hy > 1 || p.g.Hs > 1)) {             // packed 2-D grids
+    if (p.g.B != 1) return cudaErrorInvalidValue;
+    if (det_split) {
+      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1, 2); else LAUNCH_TN(3, 0, 1, 2); }
+      else if (precision == 1) LAUNCH_TN(2, 0, 1, 2);
+      else                     LAUNCH_TN(1, 0, 1, 2);
+    } else {
+      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 0, 2); else LAUNCH_TN(3, 0, 0, 2); }
+      else if (precision == 1) LAUNCH_TN(2, 0, 0, 2);
+      else                     LAUNCH_TN(1, 0, 0, 2);
+    }
+  } else if (p.pk.off) {                                    // packed utterances
     if (p.g.B != 1 || p.g.Hy != 1) return cudaErrorInvalidValue;
     if (det_split) {
-      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1, true); else LAUNCH_TN(3, 0, 1, true); }
-      else if (precision == 1) LAUNCH_TN(2, 0, 1, true);
-      else                     LAUNCH_TN(1, 0, 1, true);
+      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1, 1); else LAUNCH_TN(3, 0, 1, 1); }
+      else if (precision == 1) LAUNCH_TN(2, 0, 1, 1);
+      else                     LAUNCH_TN(1, 0, 1, 1);
     } else {
-      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 0, true); else LAUNCH_TN(3, 0, 0, true); }
-      else if (precision == 1) LAUNCH_TN(2, 0, 0, true);
-      else                     LAUNCH_TN(1, 0, 0, true);
+      if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 0, 1); else LAUNCH_TN(3, 0, 0, 1); }
+      else if (precision == 1) LAUNCH_TN(2, 0, 0, 1);
+      else                     LAUNCH_TN(1, 0, 0, 1);
     }
   } else if (det_split) {
     if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1); else LAUNCH_TN(3, 0, 1); }
@@ -1674,7 +1722,7 @@ int tc_refresh_layer(TcLayer& L, const float* ka, const float* kg, const float* 
 int tc_conv_fwd(const TcLayer& L, int precision, int debug, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo, int n, int H, int W, int sh, int sw,
                 float* P, cudaStream_t st, const TcFuse* fuse, bool* fused_out, const PackGeom* pk) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
-  if (pk && (n != 1 || H != 1 || L.kh != 1 || fuse)) return (int)cudaErrorInvalidValue;
+  if (pk && (n != 1 || (H == 1 && L.kh != 1) || fuse)) return (int)cudaErrorInvalidValue;     // H > 1: packed 2-D grids
   TcNTParams p; memset(&p, 0, sizeof p);
   p.g = fwd_geom(n, H, W, L.kh, L.kw, sh, sw);
   if (pk) p.pk = *pk;
@@ -1713,7 +1761,7 @@ int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat1
                   float* dx, int accumulate, cudaStream_t st, const TcBwdFuse* fuse, bool* fused_out, const PackGeom* pk) {
   if (fused_out) *fused_out = false;
   if (!layer_ok(L) || (precision == 3 && (!layer_ok_q(L) || !L.wdq16))) return TC_UNSUPPORTED;     // F16F8 needs the data-gradient planes (training engines)
-  if (pk && (n != 1 || H != 1 || L.kh != 1)) return (int)cudaErrorInvalidValue;
+  if (pk && (n != 1 || (H == 1 && L.kh != 1))) return (int)cudaErrorInvalidValue;     // H > 1: packed 2-D grids
   if (pk) fuse = nullptr;
   std::vector<GatherGeom> gs = dgrad_geoms(n, H, W, L.kh, L.kw, sh, sw);
   for (const GatherGeom& g : gs) if (g.ntaps == 0) return TC_UNSUPPORTED;     // (never the case for this model's layers)
@@ -1757,7 +1805,7 @@ int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16*
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dwa, float* dwg, cudaStream_t st, const DetSlab* det, const PackGeom* pk) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
-  if (pk && (n != 1 || H != 1 || L.kh != 1)) return (int)cudaErrorInvalidValue;
+  if (pk && (n != 1 || (H == 1 && L.kh != 1))) return (int)cudaErrorInvalidValue;     // H > 1: packed 2-D grids
   TcTNParams p; memset(&p, 0, sizeof p);
   if (pk) p.pk = *pk;
   p.w16 = (precision == 3 && w16) ? 1 : 0;
@@ -1866,16 +1914,20 @@ static cudaError_t tc_init_kernels() {
   INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4) INIT_NT(256, 2, 5) INIT_NT(256, 1, 5)
   INIT_NT(256, 3, 0) INIT_NT(128, 3, 0) INIT_NT(32, 3, 0) INIT_NT(256, 3, 1) INIT_NT(256, 3, 2) INIT_NT(256, 3, 5)
 #undef INIT_NT
-#define INIT_NT_PK(BN_, NPL_) if ((e = set_smem(tc_gg_nt_kernel<BN_, NPL_, 0, true>, NTCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
-  INIT_NT_PK(256, 1) INIT_NT_PK(256, 2) INIT_NT_PK(256, 3) INIT_NT_PK(128, 1) INIT_NT_PK(128, 2) INIT_NT_PK(128, 3)
-  INIT_NT_PK(32, 1) INIT_NT_PK(32, 2) INIT_NT_PK(32, 3)
+#define INIT_NT_PK(BN_, NPL_, PK_) if ((e = set_smem(tc_gg_nt_kernel<BN_, NPL_, 0, PK_>, NTCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
+  INIT_NT_PK(256, 1, 1) INIT_NT_PK(256, 2, 1) INIT_NT_PK(256, 3, 1) INIT_NT_PK(128, 1, 1) INIT_NT_PK(128, 2, 1) INIT_NT_PK(128, 3, 1)
+  INIT_NT_PK(32, 1, 1) INIT_NT_PK(32, 2, 1) INIT_NT_PK(32, 3, 1)
+  INIT_NT_PK(256, 1, 2) INIT_NT_PK(256, 2, 2) INIT_NT_PK(256, 3, 2) INIT_NT_PK(128, 1, 2) INIT_NT_PK(128, 2, 2) INIT_NT_PK(128, 3, 2)
+  INIT_NT_PK(32, 1, 2) INIT_NT_PK(32, 2, 2) INIT_NT_PK(32, 3, 2)
 #undef INIT_NT_PK
 #define INIT_TN(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
   INIT_TN(3, 1, 0) INIT_TN(3, 0, 0) INIT_TN(2, 0, 0) INIT_TN(1, 0, 0)
   INIT_TN(3, 1, 1) INIT_TN(3, 0, 1) INIT_TN(2, 0, 1) INIT_TN(1, 0, 1)
-#define INIT_TN_PK(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_, true>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
-  INIT_TN_PK(3, 1, 0) INIT_TN_PK(3, 0, 0) INIT_TN_PK(2, 0, 0) INIT_TN_PK(1, 0, 0)
-  INIT_TN_PK(3, 1, 1) INIT_TN_PK(3, 0, 1) INIT_TN_PK(2, 0, 1) INIT_TN_PK(1, 0, 1)
+#define INIT_TN_PK(NPL_, W16_, DET_, PK_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_, PK_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
+  INIT_TN_PK(3, 1, 0, 1) INIT_TN_PK(3, 0, 0, 1) INIT_TN_PK(2, 0, 0, 1) INIT_TN_PK(1, 0, 0, 1)
+  INIT_TN_PK(3, 1, 1, 1) INIT_TN_PK(3, 0, 1, 1) INIT_TN_PK(2, 0, 1, 1) INIT_TN_PK(1, 0, 1, 1)
+  INIT_TN_PK(3, 1, 0, 2) INIT_TN_PK(3, 0, 0, 2) INIT_TN_PK(2, 0, 0, 2) INIT_TN_PK(1, 0, 0, 2)
+  INIT_TN_PK(3, 1, 1, 2) INIT_TN_PK(3, 0, 1, 2) INIT_TN_PK(2, 0, 1, 2) INIT_TN_PK(1, 0, 1, 2)
 #undef INIT_TN_PK
 #undef INIT_TN
   return cudaSuccess;

@@ -21,8 +21,9 @@ Differences a user of the reference should know:
   * `generator(x, direction)` / `discriminator(x, which)` are the four networks as differentiable torch operators on CUDA tensors, for
     objectives other than the fused step's: `loss.backward()` adds their weight gradients into the gradient arena, `zero_grad()`,
     `grads()` and `adam_step()` complete a step (include/cgvc.h "activation tapes", DESIGN.md section 12).  The network descriptors
-    given to the constructor are `generator_descriptor` / `discriminator_descriptor`; `generator_packed(inputs, direction)` is the
-    generator over a list of utterances of different lengths in one call, for utterance-level objectives
+    given to the constructor are `generator_descriptor` / `discriminator_descriptor`; `generator_packed(inputs, direction)` and
+    `discriminator_packed(inputs, which)` are the networks over a list of utterances of different lengths in one call, for
+    utterance-level objectives
 """
 from __future__ import annotations
 
@@ -330,7 +331,22 @@ class CycleGAN(object):
         inputs = list(inputs)
         if not inputs:
             return []
-        return list(_PackedGenFn.apply(self._token(), self, d, *inputs))
+        return list(_PackedFn.apply(self._token(), self, 2, d, *inputs))
+
+    def discriminator_packed(self, inputs, which):
+        """Differentiable packed discriminator: inputs a list of CUDA tensors [24, T_i] (every T_i a positive multiple of 16) -> the
+        list of [6, T_i / 16, 1] probabilities, bit for bit what discriminate_packed() gives on them.  One engine call runs the forward
+        of all utterances and one their backward, which adds d loss / d (the discriminator's variables) into the gradient arena -- with
+        the loss scale of a batch of len(inputs) -- and returns d loss / d x_i for the inputs that require it.  Every convolution tap and
+        instance norm stays inside its own utterance, forward and backward, so the output of generator_packed() chains straight in.
+        which 'A' or 'B'."""
+        w = {'A': 0, 'B': 1}.get(which)
+        if w is None:
+            raise ValueError("which must be 'A' or 'B', got %r" % (which,))
+        inputs = list(inputs)
+        if not inputs:
+            return []
+        return list(_PackedFn.apply(self._token(), self, 3, w, *inputs))
 
     def _token(self):
         # a leaf that requires grad, so that autograd runs a network's backward -- and with it the weight gradients -- even when its
@@ -361,17 +377,23 @@ class CycleGAN(object):
             y = torch.empty_like(x)
         return y, self._tape_call(kind, which, x, y, batch, frames, (batch, frames))
 
-    def _packed_tape_forward(self, direction, xs):
-        """The [24, T_i] utterances xs through the generator in one call, with its kind 2 activation tape: (ys, tape, offsets)."""
+    def _packed_tape_forward(self, which, xs, kind=2):
+        """The [24, T_i] utterances xs through the generator (kind 2) or the discriminator (kind 3) in one call, with its activation
+        tape: (ys, tape, offsets)."""
         for x in xs:
             if not (isinstance(x, torch.Tensor) and x.device.type == self.device.type):
                 raise TypeError("the differentiable networks take a tensor on the engine's device (%s)" % self.device)
         offsets = self._packed_offsets(xs)
         x = self._pack(xs)
-        y = torch.empty_like(x)
+        y = torch.empty_like(x) if kind == 2 else torch.empty(self.num_features // 4 * int(offsets[-1]) // 16, device=self.device)
         n = len(offsets) - 1
-        tape = self._tape_call(2, direction, x, y, n, int(offsets[-1]), (offsets.ctypes.data_as(C.POINTER(C.c_longlong)), n))
-        return self._unpack(y, offsets), tape, offsets
+        tape = self._tape_call(kind, which, x, y, n, int(offsets[-1]), (offsets.ctypes.data_as(C.POINTER(C.c_longlong)), n))
+        return (self._unpack(y, offsets) if kind == 2 else self._unpack_prob(y, offsets)), tape, offsets
+
+    def _unpack_prob(self, p, offsets):
+        """The [6, T_i / 16, 1] probabilities of packed utterances in p, as views"""
+        H = self.num_features // 4
+        return [p[H * offsets[u] // 16:H * offsets[u + 1] // 16].reshape(H, -1, 1) for u in range(len(offsets) - 1)]
 
     def _tape_call(self, kind, which, x, y, batch, frames, geom):
         """A tape of `kind` sized by cgvc_tape_bytes(batch, frames) (kind 2: n utterances of offsets[n] frames in all), written by that
@@ -380,24 +402,25 @@ class CycleGAN(object):
         self._chk(self._lib.cgvc_tape_bytes(self._handle, kind, batch, frames, C.byref(nbytes)))
         tape = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
         fn = getattr(self._lib, ("cgvc_generator_forward_tape", "cgvc_discriminator_forward_tape",
-                                 "cgvc_generator_forward_packed_tape")[kind])
+                                 "cgvc_generator_forward_packed_tape", "cgvc_discriminator_forward_packed_tape")[kind])
         self._chk(fn(self._handle, which, _ptr(x), _ptr(y), *geom, _ptr(tape), nbytes.value, self._stream()))
         return tape
 
     def _tape_backward(self, kind, tape, geom, dy, want_dx):
         """d loss / d x of a tape's application from d loss / d y, or None without want_dx; adds the network's variable gradients into
-        the gradient arena.  geom: x's shape, or for a kind 2 tape the utterances' offsets, with dy and d x lists of their blocks."""
-        if kind == 2:
+        the gradient arena.  geom: x's shape, or for a packed tape (kinds 2, 3) the utterances' offsets, with dy and d x lists of their
+        blocks."""
+        if kind in (2, 3):
             dy = self._pack(dy)
-            x_shape, batch = dy.shape, len(geom) - 1
+            x_shape, batch = (self.num_features * int(geom[-1]),), len(geom) - 1
         else:
             dy = dy.to(device=self.device, dtype=torch.float32).contiguous()
             x_shape, batch = geom, geom[0]
         dx = torch.empty(x_shape, dtype=torch.float32, device=self.device) if want_dx else None
-        fn = self._lib.cgvc_discriminator_backward_tape if kind == 1 else self._lib.cgvc_generator_backward_tape
+        fn = self._lib.cgvc_discriminator_backward_tape if kind in (1, 3) else self._lib.cgvc_generator_backward_tape
         self._chk(fn(self._handle, _ptr(tape), _ptr(dy), _ptr(dx), self._stream()))
         self._tape_scales.add(self.tape_loss_scale(batch))
-        if kind != 2:
+        if kind not in (2, 3):
             return dx
         return self._unpack(dx, geom) if want_dx else [None] * batch
 
@@ -616,6 +639,23 @@ class CycleGAN(object):
         torch.cuda.synchronize(self.device)
         return y.cpu().numpy()
 
+    def discriminate_packed(self, inputs, which):
+        """Discriminator forward of utterances of different lengths in one engine call.  inputs: a list of [24, T_i] arrays, every
+        T_i a positive multiple of 16: host arrays of any float dtype (returns a list of float32 numpy arrays) or CUDA tensors
+        (returns a list of CUDA tensors).  Result i is [6, T_i / 16, 1], what discriminate() gives for that utterance alone, up to
+        the summation order of its instance-norm statistics."""
+        w = {'A': 0, 'B': 1}[which]
+        if len(inputs) == 0:
+            return []
+        on_device = all(isinstance(x, torch.Tensor) and x.is_cuda for x in inputs)
+        offsets = self._packed_offsets(inputs)
+        x = self._pack(inputs) if on_device else self._stage([np.asarray(a) for a in inputs], "disc_packed")
+        H = self.num_features // 4
+        p = torch.empty(H * int(offsets[-1]) // 16, dtype=torch.float32, device=self.device)
+        off = offsets.ctypes.data_as(C.POINTER(C.c_longlong))
+        self._chk(self._lib.cgvc_discriminator_forward_packed(self._handle, w, _ptr(x), _ptr(p), off, len(offsets) - 1, self._stream()))
+        return self._unpack_prob(self._result(p, on_device), offsets)
+
     def set_debug_taps(self, on=True):
         """Keep the fp32 copy of every generator layer output of the next test() calls for debug_activation() (parity tests).
         Off by default: the conversion path then writes only what the next layer reads."""
@@ -751,14 +791,15 @@ class _NetFn(torch.autograd.Function):
         return dx, None, None, None, None
 
 
-class _PackedGenFn(torch.autograd.Function):
-    """One packed generator application over utterances of different lengths (CycleGAN.generator_packed) with its kind 2 activation
-    tape: forward writes it, backward consumes it (unmodified, as _NetFn's)"""
+class _PackedFn(torch.autograd.Function):
+    """One packed application over utterances of different lengths -- the generator (kind 2, CycleGAN.generator_packed) or the
+    discriminator (kind 3, CycleGAN.discriminator_packed) -- with its activation tape: forward writes it, backward consumes it
+    (unmodified, as _NetFn's)"""
 
     @staticmethod
-    def forward(ctx, token, model, direction, *xs):
-        ys, tape, offsets = model._packed_tape_forward(direction, xs)
-        ctx.model, ctx.offsets = model, offsets
+    def forward(ctx, token, model, kind, which, *xs):
+        ys, tape, offsets = model._packed_tape_forward(which, xs, kind)
+        ctx.model, ctx.kind, ctx.offsets = model, kind, offsets
         ctx.save_for_backward(tape)
         return tuple(ys)
 
@@ -766,6 +807,6 @@ class _PackedGenFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, *dys):
         tape, = ctx.saved_tensors
-        want = ctx.needs_input_grad[3:]
-        dxs = ctx.model._tape_backward(2, tape, ctx.offsets, dys, any(want))
-        return (None, None, None) + tuple(dx if w else None for dx, w in zip(dxs, want))
+        want = ctx.needs_input_grad[4:]
+        dxs = ctx.model._tape_backward(ctx.kind, tape, ctx.offsets, dys, any(want))
+        return (None, None, None, None) + tuple(dx if w else None for dx, w in zip(dxs, want))
