@@ -10,7 +10,8 @@
 // Kernel anatomy (both kernels are persistent, one CTA per SM, 384 threads, tiles / work items walked with stride gridDim.x):
 //   warps 0-3   producers: gather the activation rows (im2col rows, zero-filled at the TF-SAME borders) with 16-byte cp.async
 //               into SWIZZLE_128B shared memory; one thread TMA-loads the weight (NT) / gradient (TN) tile; both complete on
-//               the stage's "full" mbarrier.
+//               the stage's "full" mbarrier.  Forward / data-gradient tiles that are boxes of the source planes (nt_tma_maps) take
+//               the TMA form instead: one thread loads both operand tiles by TMA, the padding zero-filled by the hardware.
 //   warps 4-11  two consumer warpgroups, 64 accumulator rows each: wgmma from the shared-memory stages into registers, stages
 //               released through the "empty" mbarriers.  NT: the plain epilogue (bias / accumulate) stores the accumulator
 //               fragments from registers; for the fused instance-norm (+GLU / +residual) forward epilogues and the opt-in fused
@@ -68,6 +69,22 @@ bool make_tmap3_t(CUtensorMap* m, const void* base, CUtensorMapDataType dt, int 
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// An activation plane [B][Hs][Ws][ld] (esize-byte elements) as the 4-D tensor (channel, x, y, sample), box [nb][1][bx][64 channels]
+// with traversal stride sx along x: a box at (c0, x * sx + ox, y * sy + oy, b) is the gathered operand of bx / sx output positions
+// x, x + 1, ... of nb samples b, b + 1, ..., one 64 * esize-byte row each (SWIZZLE_128B for 128-byte rows, else SWIZZLE_64B).
+// TF-SAME padding, negative coordinates included, and samples past the batch read as zeros (OOB fill NONE fills zeros).
+bool make_tmap_act(CUtensorMap* m, const void* base, int esize, uint64_t ld, const GatherGeom& g, uint32_t bx, uint32_t nb) {
+  EncodeTiledFn enc = get_encoder();
+  if (!enc) return false;
+  cuuint64_t dims[4] = {ld, (cuuint64_t)g.Ws, (cuuint64_t)g.Hs, (cuuint64_t)g.B};
+  cuuint64_t strides[3] = {ld * esize, ld * esize * g.Ws, ld * esize * g.Ws * g.Hs};
+  cuuint32_t box[4] = {64, bx, 1, nb};
+  cuuint32_t es[4] = {1, (cuuint32_t)g.sx, 1, 1};
+  return enc(m, esize == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), dims, strides, box, es,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, esize == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 // ------------------------------------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -100,6 +117,11 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void tma_load3(uint32_t dst_smem, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
                ::"r"(dst_smem), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
+}
+// rank 4 (the activation maps of make_tmap_act); out-of-bounds coordinates, negative ones included, land as zeros
+__device__ __forceinline__ void tma_load4(uint32_t dst_smem, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
+  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+               ::"r"(dst_smem), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
@@ -188,7 +210,11 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   // level's divisor; the output level's is pk.div * g.sx
   PackGeom pk;
   FastDiv div_bw, div_w;                                 // B * Wx and Wx: row m -> (y, b, x), see nt_row
+  // the TMA form of the dense kernel (TA, see nt_tma_maps): the activation planes as make_tmap_act maps, one box per plane and stage.
+  // NPL 1 / 2: the bf16 planes; NPL 3: tm_a_hi = the fp16 plane, tm_a8_hi / tm_a8_lo = the e4m3 planes (SWIZZLE_64B tiles)
+  CUtensorMap tm_a_hi, tm_a_lo, tm_a8_hi, tm_a8_lo;
 };
+static_assert(sizeof(TcNTParams) <= 4096, "kernel parameters are limited to 4 KB");
 
 // Rows of the NT kernel are walked output row y outermost: m = (y * B + b) * Wx + x, so that a 128-row tile spans few output rows and
 // skips the taps that read only the padding for all of them (gather_tap_mask).  With Hy == 1 this is the sample order m = b * Wx + x.
@@ -244,8 +270,8 @@ constexpr int kProducerThreads = 128;
 
 
 // Stages of 64 contraction channels.  F16F8 (NPL = 3) stages hold one 128-byte-row tile per operand, like NPL 1: an fp16 stage the
-// fp16 tiles; a cross-term stage the A rows as [64 a8_hi bytes | 64 a8_lo bytes] (SWIZZLE_128B) and the weight tile as two
-// SWIZZLE_64B tiles of 64-byte rows, b8_hi then b8_lo (TMA boxes of 64 bytes).
+// fp16 tiles; a cross-term stage the A rows as [64 a8_hi bytes | 64 a8_lo bytes] (SWIZZLE_128B; the TMA form: two SWIZZLE_64B tiles
+// of 64-byte rows, a8_hi then a8_lo) and the weight tile as two SWIZZLE_64B tiles, b8_hi then b8_lo (TMA boxes of 64 bytes).
 template <int BN, int NPL>
 struct NTCfg {
   static constexpr int A_PLANE = 128 * 128;            // bytes: 128 rows x 128 B
@@ -755,18 +781,19 @@ __device__ __forceinline__ void nt_tile_epilogue(const TcNTParams& p, const long
 // ------------------------------------------------------------------------------------------------ consumer K loop
 // MMAs of one pipeline stage.  The kind is a template argument, so that no wgmma sits under a runtime branch (which makes ptxas
 // serialise the asynchronous MMAs): F16F8 walks its two passes as two calls.
-enum { MMA_BF16 = 0, MMA_BF16X3 = 1, MMA_E4M3_CROSS = 2, MMA_F16 = 3, MMA_F16_CROSS = 4 };
+// MMA_E4M3_CROSS64: the same products from A rows held as two SWIZZLE_64B tiles (a8_hi, then a8_lo), as the TMA form loads them
+enum { MMA_BF16 = 0, MMA_BF16X3 = 1, MMA_E4M3_CROSS = 2, MMA_F16 = 3, MMA_F16_CROSS = 4, MMA_E4M3_CROSS64 = 5 };
 
 // One consumer warpgroup walks nkb pipeline stages: wait for the stage, issue its MMAs, release the previous stage once those have
 // completed.  TN = 0: both operands K-major, 128-byte rows (forward / data gradient); TN = 1: both MN-major, 64-element atoms at
-// 8192 B (weight gradient).  The warpgroup's A rows (NT) / channels (TN) start at wg * 8192.
+// 8192 B (weight gradient).  The warpgroup's A rows (NT) / channels (TN) start at wg * 8192 (MMA_E4M3_CROSS64: 64-byte rows, wg * 4096).
 template <int BN, int KIND, int TN, class Cfg>
 __device__ __forceinline__ void consume_stages(float (&d)[BN / 2], int nkb, int& stage, uint32_t& phase, int& prev,
                                                uint64_t* full_bar, uint64_t* empty_bar, uint32_t smem_base, int wg, int lane) {
   for (int kb = 0; kb < nkb; ++kb) {
     mbar_wait(&full_bar[stage], phase);
     fence_proxy_async();                                     // producers' generic-proxy writes (cp.async, st.shared) -> wgmma reads
-    const uint32_t sA = smem_base + stage * Cfg::STAGE + wg * 8192;
+    const uint32_t sA = smem_base + stage * Cfg::STAGE + wg * (KIND == MMA_E4M3_CROSS64 ? 4096 : 8192);
     const uint32_t sB = smem_base + stage * Cfg::STAGE + Cfg::PLANES * Cfg::A_PLANE;
     fence_acc(d);
     wgmma_fence();
@@ -776,6 +803,12 @@ __device__ __forceinline__ void consume_stages(float (&d)[BN / 2], int nkb, int&
         for (int k = 0; k < 2; ++k) {
           wgmma_e4m3<BN>(d, make_desc(sA + k * 32, 16, 1024), make_desc64(sB + Cfg::B_PLANE / 2 + k * 32), 1);
           wgmma_e4m3<BN>(d, make_desc(sA + 64 + k * 32, 16, 1024), make_desc64(sB + k * 32), 1);
+        }
+      } else if constexpr (KIND == MMA_E4M3_CROSS64) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          wgmma_e4m3<BN>(d, make_desc64(sA + k * 32), make_desc64(sB + Cfg::B_PLANE / 2 + k * 32), 1);
+          wgmma_e4m3<BN>(d, make_desc64(sA + Cfg::A_PLANE / 2 + k * 32), make_desc64(sB + k * 32), 1);
         }
       } else if constexpr (KIND == MMA_F16) {                // fp16 hi x hi, one 64-channel tile of K = 16 steps
 #pragma unroll
@@ -900,10 +933,14 @@ constexpr int kNTThreads = 384;
 // (first source row of the utterance, its length at the source level, local position * stride) where the dense form keeps (b, y, x).
 // PK 2: the packed 2-D form (cgvc_discriminator_forward_packed, kernels.cuh PackGeom2): the producers keep (first source row of the
 // utterance, y * sy, x * sx) and the utterance's source width
-template <int BN, int NPL, int EPI, int PK = 0>
+// TA: the dense form whose tiles are boxes of the activation planes (nt_tma_maps): one producer thread issues, per stage, one TMA of
+// each A plane beside the weight tile, and the full barriers expect that one arrival plus the bytes.  The stages' contents are those
+// of the gather, so every MMA sees the same operands in the same order.
+template <int BN, int NPL, int EPI, int PK = 0, int TA = 0>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   static_assert(!PK || EPI == 0, "packed rows never take the fused epilogues (they need whole equal-length samples per tile)");
+  static_assert(!PK || !TA, "the TMA form is dense");
   using Cfg = NTCfg<BN, NPL>;
   __shared__ float epi_xch[2][4][32];                        // cross-warp exchange of the fused epilogue, per group
   __shared__ __align__(16) float epi_bc[8][(EPI == 3 || EPI == 4) ? 384 : 128];   // per-warp broadcast of per-column coefficients (32 floats per quantity)
@@ -930,18 +967,65 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
   const bool n_fast = g.Hy > 1;
 
   if (threadIdx.x == 0) {
-    // full: 128 cp.async arrivals (A rows) + 1 arrive.expect_tx whose bytes the weight-tile TMA completes; empty / acc_free: one
-    // arrival per consumer warp
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], kProducerThreads + 1); mbar_init(&empty_bar[s], 8); }
+    // full: 128 cp.async arrivals (A rows) + 1 arrive.expect_tx whose bytes the weight-tile TMA completes (TA: that one arrival,
+    // whose bytes both operand TMAs complete); empty / acc_free: one arrival per consumer warp
+    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], TA ? 1 : kProducerThreads + 1); mbar_init(&empty_bar[s], 8); }
     mbar_init(&acc_free_bar, 8);
     fence_barrier_init();
     tma_prefetch_desc(&p.tm_b_hi);
     if (NPL == 2) tma_prefetch_desc(&p.tm_b_lo);
     if (NPL == 3) { tma_prefetch_desc(&p.tm_b8_hi); tma_prefetch_desc(&p.tm_b8_lo); }
+    if (TA) {
+      tma_prefetch_desc(&p.tm_a_hi);
+      if (NPL == 2) tma_prefetch_desc(&p.tm_a_lo);
+      if (NPL == 3) { tma_prefetch_desc(&p.tm_a8_hi); tma_prefetch_desc(&p.tm_a8_lo); }
+    }
   }
   __syncthreads();
 
-  if (warp < 4) {
+  if (TA && warp < 4) {
+    // ===================== producer (TMA form): thread 0 issues both operand tiles of every stage =====================
+    if (threadIdx.x == 0) {
+      int stage = 0; uint32_t phase = 0;
+      int it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        const long long m0 = (long long)(n_fast ? tile / n_tiles : tile % m_tiles) * 128;
+        const int n0 = (n_fast ? tile % n_tiles : tile / m_tiles) * BN;
+        if (EPI != 0 && it > 0) mbar_wait(&acc_free_bar, (uint32_t)(it - 1) & 1u);
+        const uint32_t taps = nt_tile_taps<PK>(p, m0, M);
+        const RowPos o = nt_row(p, m0);                        // the tile: positions o.x .. of samples o.b .. at output row o.y
+        const uint32_t a_bytes = (p.debug & 4) ? 0u : (uint32_t)Cfg::PLANES * Cfg::A_PLANE;
+        for (int pass = 0; pass < (NPL == 3 ? 2 : 1); ++pass)
+        for (int tap = 0; tap < g.ntaps; ++tap) {
+          if (!((taps >> tap) & 1u)) continue;
+          const int xs = o.x * g.sx + g.ox[tap], ys = o.y * g.sy + g.oy[tap];
+          for (int cc = 0; cc < cchunks; ++cc) {
+            const int c0 = cc << 6;
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            const uint32_t sA = smem_base + stage * Cfg::STAGE;
+            const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
+            mbar_expect_tx(&full_bar[stage], a_bytes + Cfg::PLANES * Cfg::B_PLANE);
+            if (NPL == 3 && pass == 0) {
+              tma_load3(sB, &p.tm_b8_hi, c0, n0, g.widx[tap], &full_bar[stage]);
+              tma_load3(sB + Cfg::B_PLANE / 2, &p.tm_b8_lo, c0, n0, g.widx[tap], &full_bar[stage]);
+              if (a_bytes) {
+                tma_load4(sA, &p.tm_a8_hi, c0, xs, ys, o.b, &full_bar[stage]);
+                tma_load4(sA + Cfg::A_PLANE / 2, &p.tm_a8_lo, c0, xs, ys, o.b, &full_bar[stage]);
+              }
+            } else {
+              tma_load3(sB, &p.tm_b_hi, c0, n0, g.widx[tap], &full_bar[stage]);
+              if (NPL == 2) tma_load3(sB + Cfg::B_PLANE, &p.tm_b_lo, c0, n0, g.widx[tap], &full_bar[stage]);
+              if (a_bytes) {
+                tma_load4(sA, &p.tm_a_hi, c0, xs, ys, o.b, &full_bar[stage]);
+                if (NPL == 2) tma_load4(sA + Cfg::A_PLANE, &p.tm_a_lo, c0, xs, ys, o.b, &full_bar[stage]);
+              }
+            }
+            if (++stage == S) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    }
+  } else if (warp < 4) {
     // ===================== producers =====================
     const int t = threadIdx.x;
     const int chunk = t & 7, rsub = t >> 3;                 // 8 threads cover one 128-byte row; 16 rows per pass
@@ -1049,7 +1133,7 @@ tc_gg_nt_kernel(const __grid_constant__ TcNTParams p) {
       int prev = -1;                                         // stage whose MMAs may still be in flight
       const int kb_pass = __popc(nt_tile_taps<PK>(p, m0, M)) * cchunks;   // (> 0 for TF-SAME geometries; 0 is safe)
       if constexpr (NPL == 3) {                             // e4m3 cross products, then the fp16 hi x hi products after the rescale of D
-        consume_stages<BN, MMA_E4M3_CROSS, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
+        consume_stages<BN, TA ? MMA_E4M3_CROSS64 : MMA_E4M3_CROSS, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
         rescale_acc(d, 1.f / (float)(1 << CGVC_Q_ACC_SHIFT));
         consume_stages<BN, MMA_F16, 0, Cfg>(d, kb_pass, stage, phase, prev, full_bar, empty_bar, smem_base, wg, lane);
       } else {
@@ -1505,6 +1589,21 @@ int num_sms() {
   return n;
 }
 
+// The TMA form of the dense kernel takes the geometries whose 128-row tiles are boxes of the source planes: a tile is 128 / Wx whole
+// samples (Wx divides 128) or 128 positions of one sample (128 divides Wx), all at one output row (rows are y-major, see nt_row: true
+// when Hy == 1 or 128 divides B * Wx).  Rows past M in the last tile are samples past the batch, which the box reads as zeros, as the
+// gather does.  Encodes p's activation maps and returns true; false leaves the geometry (or a plane the encoder refuses) to the gather.
+static bool nt_tma_maps(TcNTParams& p, int npl) {
+  const GatherGeom& g = p.g;
+  const int wx = g.Wx < 128 ? g.Wx : 128;
+  if (128 % wx || g.Wx % wx || (g.Hy > 1 && ((long long)g.B * g.Wx) % 128) || wx * g.sx > 256 || g.sx > 8) return false;
+  const uint32_t bx = (uint32_t)(wx * g.sx), nb = (uint32_t)(128 / wx);
+  if (npl == 3)
+    return make_tmap_act(&p.tm_a_hi, p.a_hi, 2, p.a_ld, g, bx, nb) && make_tmap_act(&p.tm_a8_hi, p.a8_hi, 1, p.a_ld, g, bx, nb) &&
+           make_tmap_act(&p.tm_a8_lo, p.a8_lo, 1, p.a_ld, g, bx, nb);
+  return make_tmap_act(&p.tm_a_hi, p.a_hi, 2, p.a_ld, g, bx, nb) && (npl != 2 || make_tmap_act(&p.tm_a_lo, p.a_lo, 2, p.a_ld, g, bx, nb));
+}
+
 cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
   if (M == 0) return cudaSuccess;
@@ -1540,23 +1639,29 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
     else if (bn == 128) { if (npl == 3) LAUNCH_NT(128, 3, 0, 1); else if (npl == 2) LAUNCH_NT(128, 2, 0, 1); else LAUNCH_NT(128, 1, 0, 1); }
     else                { if (npl == 3) LAUNCH_NT(32, 3, 0, 1);  else if (npl == 2) LAUNCH_NT(32, 2, 0, 1);  else LAUNCH_NT(32, 1, 0, 1); }
   }
-  else if (precision == 3) {                                // F16F8 (no fused backward epilogues in this precision)
-    if (epi == 1)       LAUNCH_NT(256, 3, 1);
-    else if (epi == 2)  LAUNCH_NT(256, 3, 2);
-    else if (epi == 5)  LAUNCH_NT(256, 3, 5);
-    else if (epi != 0)  return cudaErrorInvalidValue;
-    else if (bn == 256) LAUNCH_NT(256, 3, 0);
-    else if (bn == 128) LAUNCH_NT(128, 3, 0);
-    else                LAUNCH_NT(32, 3, 0);
+  else {
+    // dense rows: the TMA form where the tiles are boxes of the activation planes, else the gather
+    const bool ta = nt_tma_maps(p, precision == 3 ? 3 : x3 ? 2 : 1);
+#define LAUNCH_NT_D(BN_, NPL_, EPI_) do { if (ta) LAUNCH_NT(BN_, NPL_, EPI_, 0, 1); else LAUNCH_NT(BN_, NPL_, EPI_); } while (0)
+    if (precision == 3) {                                // F16F8 (no fused backward epilogues in this precision)
+      if (epi == 1)       LAUNCH_NT_D(256, 3, 1);
+      else if (epi == 2)  LAUNCH_NT_D(256, 3, 2);
+      else if (epi == 5)  LAUNCH_NT_D(256, 3, 5);
+      else if (epi != 0)  return cudaErrorInvalidValue;
+      else if (bn == 256) LAUNCH_NT_D(256, 3, 0);
+      else if (bn == 128) LAUNCH_NT_D(128, 3, 0);
+      else                LAUNCH_NT_D(32, 3, 0);
+    }
+    else if (epi == 1)  { if (x3) LAUNCH_NT_D(256, 2, 1); else LAUNCH_NT_D(256, 1, 1); }
+    else if (epi == 2)  { if (x3) LAUNCH_NT_D(256, 2, 2); else LAUNCH_NT_D(256, 1, 2); }
+    else if (epi == 3)  { if (x3) LAUNCH_NT_D(256, 2, 3); else LAUNCH_NT_D(256, 1, 3); }
+    else if (epi == 4)  { if (x3) LAUNCH_NT_D(256, 2, 4); else LAUNCH_NT_D(256, 1, 4); }
+    else if (epi == 5)  { if (x3) LAUNCH_NT_D(256, 2, 5); else LAUNCH_NT_D(256, 1, 5); }
+    else if (bn == 256) { if (x3) LAUNCH_NT_D(256, 2, 0); else LAUNCH_NT_D(256, 1, 0); }
+    else if (bn == 128) { if (x3) LAUNCH_NT_D(128, 2, 0); else LAUNCH_NT_D(128, 1, 0); }
+    else                { if (x3) LAUNCH_NT_D(32, 2, 0);  else LAUNCH_NT_D(32, 1, 0); }
+#undef LAUNCH_NT_D
   }
-  else if (epi == 1)  { if (x3) LAUNCH_NT(256, 2, 1); else LAUNCH_NT(256, 1, 1); }
-  else if (epi == 2)  { if (x3) LAUNCH_NT(256, 2, 2); else LAUNCH_NT(256, 1, 2); }
-  else if (epi == 3)  { if (x3) LAUNCH_NT(256, 2, 3); else LAUNCH_NT(256, 1, 3); }
-  else if (epi == 4)  { if (x3) LAUNCH_NT(256, 2, 4); else LAUNCH_NT(256, 1, 4); }
-  else if (epi == 5)  { if (x3) LAUNCH_NT(256, 2, 5); else LAUNCH_NT(256, 1, 5); }
-  else if (bn == 256) { if (x3) LAUNCH_NT(256, 2, 0); else LAUNCH_NT(256, 1, 0); }
-  else if (bn == 128) { if (x3) LAUNCH_NT(128, 2, 0); else LAUNCH_NT(128, 1, 0); }
-  else                { if (x3) LAUNCH_NT(32, 2, 0);  else LAUNCH_NT(32, 1, 0); }
 #undef LAUNCH_NT
   prof_end(st);
   return cudaGetLastError();
@@ -1909,6 +2014,12 @@ int tc_alloc(TcWeights& w, int precision, bool train) {
 static cudaError_t tc_init_kernels() {
   cudaError_t e;
 #define INIT_NT(BN_, NPL_, EPI_) if ((e = set_smem(tc_gg_nt_kernel<BN_, NPL_, EPI_>, NTCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
+  INIT_NT(256, 2, 0) INIT_NT(256, 1, 0) INIT_NT(128, 2, 0) INIT_NT(128, 1, 0) INIT_NT(32, 2, 0) INIT_NT(32, 1, 0)
+  INIT_NT(256, 2, 1) INIT_NT(256, 1, 1) INIT_NT(256, 2, 2) INIT_NT(256, 1, 2)
+  INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4) INIT_NT(256, 2, 5) INIT_NT(256, 1, 5)
+  INIT_NT(256, 3, 0) INIT_NT(128, 3, 0) INIT_NT(32, 3, 0) INIT_NT(256, 3, 1) INIT_NT(256, 3, 2) INIT_NT(256, 3, 5)
+#undef INIT_NT
+#define INIT_NT(BN_, NPL_, EPI_) if ((e = set_smem(tc_gg_nt_kernel<BN_, NPL_, EPI_, 0, 1>, NTCfg<BN_, NPL_>::SMEM)) != cudaSuccess) return e;
   INIT_NT(256, 2, 0) INIT_NT(256, 1, 0) INIT_NT(128, 2, 0) INIT_NT(128, 1, 0) INIT_NT(32, 2, 0) INIT_NT(32, 1, 0)
   INIT_NT(256, 2, 1) INIT_NT(256, 1, 1) INIT_NT(256, 2, 2) INIT_NT(256, 1, 2)
   INIT_NT(256, 2, 3) INIT_NT(256, 1, 3) INIT_NT(256, 2, 4) INIT_NT(256, 1, 4) INIT_NT(256, 2, 5) INIT_NT(256, 1, 5)
