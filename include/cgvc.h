@@ -364,9 +364,10 @@ int cgvc_kernel_launches(unsigned long long* count);
  * it, or the calls return CGVC_ERR_UNBOUND; cgvc_conv_backward and cgvc_in_glu_backward(_planes) honour it too and then need WORK
  * bound.  With a communicator attached each rank's gradients are deterministic; the NCCL all-reduce that sums them is not covered.
  * "debug_taps" (default 0): see cgvc_debug_activation.
- * "tc_debug" (default 0; 0 to 7): timing-experiment knobs of the forward/data-gradient kernel (results become garbage):
- * 1 = epilogue skips global stores, 2 = also skips the accumulator reads, 4 = producers skip the activation gather.  The plain
- * epilogue stores straight from the accumulator registers, so for it 2 acts as 1. */
+ * "tc_debug" (default 0; 0 to 7): timing-experiment knobs of the tensor-core kernels (results become garbage): 1 = the
+ * forward/data-gradient epilogue skips global stores, 2 = also skips the accumulator reads, 4 = the producers of every gather-GEMM,
+ * the weight gradient's included, skip the activation loads.  The plain epilogue stores straight from the accumulator registers, so
+ * for it 2 acts as 1. */
 int cgvc_set_option(cgvc_handle h, const char* name, int value);
 int cgvc_profile_enable(int on);
 int cgvc_profile_collect(double* ms3, double* flops3, long long* launches3);

@@ -500,7 +500,7 @@ static int conv_wgrad(cgvc_engine* e, const Layer& L, const LayerTensors& t, con
                       const DetSlab* det) {
   bool done = false;
   if (t.tc && dp.hi && io.xhi)
-    RET(tc_result(e, tc_conv_wgrad(*t.tc, t.precision, t.wgrad16, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, t.dka, t.dkg,
+    RET(tc_result(e, tc_conv_wgrad(*t.tc, t.precision, t.debug, t.wgrad16, io.xhi, io.xlo, dp.hi, dp.lo, io.n, io.H, io.W, L.sh, L.sw, t.dka, t.dkg,
                                    st, det, packed(io)), &L.a, "weight gradient", &done));
   if (done) return 0;
   RET(conv_wgrad_simt(e, t.dka, L.a, L.sh, L.sw, io, dP, L.width(), 0, st, det));
@@ -855,7 +855,7 @@ static int o1_edge_backward(cgvc_engine* e, const GenNet& N, const float* d_out,
   CK(launch_im2col_taps(d_out, (long long)n * T, T, nf, N.o1.a.kw, -1, edge_cpad(N.o1.a.kw * nf), e->cfg.precision == CGVC_PREC_F16F8,
                         dz.hi, dz.lo, st, off, n_off, sat_grad(e), ufl_grad(e)));
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-    return tc_result(e, tc_conv_wgrad(O, e->cfg.precision, e->tcw.wgrad16, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws,
+    return tc_result(e, tc_conv_wgrad(O, e->cfg.precision, e->tcw.debug, e->tcw.wgrad16, uhi, ulo, dz.hi, dz.lo, n, 1, T, 1, 1, Gm + N.o1.a.k, nullptr, ws,
                                       det_of(S)),
                      &N.o1.a, "weight gradient (tap-lowered)"); }));
   RET(tc_result(e, tc_conv_dgrad(O, e->cfg.precision, e->tcw.debug, dz.hi, dz.lo, n, 1, T, 1, 1, du, 0, st), &N.o1.a,
@@ -872,7 +872,7 @@ static int h1_edge_backward(cgvc_engine* e, const GenNet& N, const __nv_bfloat16
   float* Gm = e->G();
   const TcLayer& H = e->tcw.layers[N.h1c_slot];
   RET(run_wgrad(S, true, st, [&](cudaStream_t ws) {
-    return tc_result(e, tc_conv_wgrad(H, e->cfg.precision, e->tcw.wgrad16, xchi, xclo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.h1.a.k,
+    return tc_result(e, tc_conv_wgrad(H, e->cfg.precision, e->tcw.debug, e->tcw.wgrad16, xchi, xclo, dp.hi, dp.lo, n, 1, T, 1, 1, Gm + N.h1.a.k,
                                       Gm + N.h1.g.k, ws, det_of(S)),
                      &N.h1.a, "weight gradient (tap-lowered)"); }));
   if (dz) RET(tc_result(e, tc_conv_dgrad(H, e->cfg.precision, e->tcw.debug, dp.hi, dp.lo, n, 1, T, 1, 1, dz, 0, st), &N.h1.a,

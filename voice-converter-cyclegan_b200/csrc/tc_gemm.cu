@@ -11,7 +11,9 @@
 //   warps 0-3   producers: gather the activation rows (im2col rows, zero-filled at the TF-SAME borders) with 16-byte cp.async
 //               into SWIZZLE_128B shared memory; one thread TMA-loads the weight (NT) / gradient (TN) tile; both complete on
 //               the stage's "full" mbarrier.  Forward / data-gradient tiles that are boxes of the source planes (nt_tma_maps) take
-//               the TMA form instead: one thread loads both operand tiles by TMA, the padding zero-filled by the hardware.
+//               the TMA form instead: one thread loads both operand tiles by TMA, the padding zero-filled by the hardware.  So do
+//               weight-gradient stages of whole output rows (tn_tma_maps): the lanes of warp 0 issue the gradient atoms and one
+//               activation box per output row (or per stage) and channel atom.
 //   warps 4-11  two consumer warpgroups, 64 accumulator rows each: wgmma from the shared-memory stages into registers, stages
 //               released through the "empty" mbarriers.  NT: the plain epilogue (bias / accumulate) stores the accumulator
 //               fragments from registers; for the fused instance-norm (+GLU / +residual) forward epilogues and the opt-in fused
@@ -185,7 +187,8 @@ struct TcNTParams {                 // forward / data-gradient form: D[m,n] = su
   int n_tiles;                                           // column tiles to compute (host: covers the real columns only)
   int debug;                                             // diagnostic knobs (option "tc_debug", TcWeights::debug): 1 = epilogue skips its global stores, 2 = also skips
                                                          // the accumulator reads (the plain epilogue reads registers only: 2 acts as 1 there),
-                                                         // 4 = producers skip the A gather.  Results are garbage; timing only.
+                                                         // 4 = producers skip the A gather (the weight gradient's too: TcTNParams::debug).
+                                                         // Results are garbage; timing only.
   float* dst; int d_ld; const float* bias; int accumulate;
   int perm; int Cc;                                      // gated layers: weight rows / bias are stored tile-interleaved: tile j =
                                                          // [a-channels j*128..+127 | g-channels j*128..+127]; Cc = channels per branch
@@ -257,7 +260,12 @@ struct TcTNParams {                 // weight-gradient form: D_t[c,n] = sum_m X[
   float* part; long long part_k, numel_a;
   // packed variable-length utterances (the PK kernels): g is the 1-D forward geometry of all rows, pk.div the source level's divisor
   PackGeom pk;
+  int debug;                                             // TcNTParams::debug; the TN kernel reads bit 4 only (producers skip the X loads)
+  // the TMA form of the dense kernel (TA, see tn_tma_maps): the activation planes as make_tmap_act maps, one box per output row (or
+  // per stage when Hy == 1) and channel atom.  NPL 1 / 2: the bf16 planes; NPL 3 with W16: tm_x_hi = the fp16 plane
+  CUtensorMap tm_x_hi, tm_x_lo;
 };
+static_assert(sizeof(TcTNParams) <= 4096, "kernel parameters are limited to 4 KB");
 
 // address of weight-gradient element (tap slab, channel c, column col) in the TF-layout kernel [taps][C][ncols]; with fold_n the layer's
 // real taps live in the column dimension (col = t * fold_n + n) and the kernel in memory is [taps][C][fold_n]
@@ -1193,10 +1201,15 @@ struct TNCfg {
 // utterance u = pack_find(m * dout): local position (m - off[u] / dout) * stride + tap offset, a zero row outside [0, len_u / div)
 // PK 2: packed 2-D grids (kernels.cuh PackGeom2): K-row m finds (u, y, x) in the output grid and reads its own utterance's source row,
 // a zero row outside it
-template <int NPL, int W16, int DET, int PK = 0>
+// TA: the dense form whose stages are boxes of the activation planes (tn_tma_maps): the lanes of producer warp 0 issue, per stage, the
+// gradient atoms and one TMA per box of whole output rows and channel atom; lane 0 arms the full barrier with every box's bytes first.
+// The stages' contents are those of the gather (the boxes zero-fill padding, samples past the batch and channels past x_ld), so
+// every MMA sees the same operands in the same order.
+template <int NPL, int W16, int DET, int PK = 0, int TA = 0>
 __global__ void __launch_bounds__(kNTThreads, 1)
 tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   static_assert(W16 == 0 || NPL == 3, "the fp16-only weight gradient is a form of CGVC_PREC_F16F8");
+  static_assert(!TA || (!PK && (NPL != 3 || W16)), "the TMA form is dense and loads the planes as they are (no e4m3 widening)");
   using Cfg = TNCfg<NPL, W16>;
   constexpr int S = Cfg::STAGES;
   constexpr int BN = 256;
@@ -1228,14 +1241,59 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
   };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], kProducerThreads + 1); mbar_init(&empty_bar[s], 8); }
+    // full: 128 cp.async arrivals (X rows) + 1 arrive.expect_tx whose bytes the gradient-tile TMA completes (TA: that one arrival,
+    // whose bytes both operands' TMAs complete); empty: one arrival per consumer warp
+    for (int s = 0; s < S; ++s) { mbar_init(&full_bar[s], TA ? 1 : kProducerThreads + 1); mbar_init(&empty_bar[s], 8); }
     fence_barrier_init();
     tma_prefetch_desc(&p.tm_g_hi);
     if (NPL == 2) tma_prefetch_desc(&p.tm_g_lo);
+    if (TA) { tma_prefetch_desc(&p.tm_x_hi); if (NPL == 2) tma_prefetch_desc(&p.tm_x_lo); }
   }
   __syncthreads();
 
-  if (warp < 4) {
+  if (TA && warp < 4) {
+    // ---- producer (TMA form): lanes 0-3 load the gradient atoms, lanes 4 .. 4 + 2 * nbox - 1 one X box each (box j, atom a).  A box
+    // is box_rows K-rows: 64 / Wx whole samples at y = 0 (Hy == 1), one output row (b, y) of a 2-D grid, or 64 positions of one row;
+    // box j lands at row j * box_rows of both MN atoms, a 1024-byte boundary (Wx >= 8), so the 128B swizzle is the one sw128 writes
+    if (warp == 0) {
+      const int box_rows = (g.Hy == 1 || g.Wx >= 64) ? 64 : g.Wx;
+      const int nbox = 64 / box_rows;
+      const uint32_t x_bytes = (p.debug & 4) ? 0u : (uint32_t)Cfg::PLANES * Cfg::A_PLANE;   // both atoms, OOB-filled ones included
+      int stage = 0; uint32_t phase = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const Item w = decode(item);
+        for (int kb = 0; kb < w.num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          const uint32_t sA = smem_base + stage * Cfg::STAGE;
+          const uint32_t sB = sA + Cfg::PLANES * Cfg::A_PLANE;
+          const int row0 = (int)(w.mbeg + (long long)kb * 64);
+          if (lane == 0) {
+            int natoms = 0;
+#pragma unroll
+            for (int a = 0; a < 4; ++a) natoms += (w.n0 + a * 64) < p.g_ld ? 1 : 0;
+            mbar_expect_tx(&full_bar[stage], Cfg::PLANES * natoms * 8192 + x_bytes);
+          }
+          __syncwarp();                                        // the barrier expects the bytes before any of them can land
+          if (lane < 4) {
+            if ((w.n0 + lane * 64) < p.g_ld) {
+              tma_load3(sB + lane * 8192, &p.tm_g_hi, w.n0 + lane * 64, row0, 0, &full_bar[stage]);
+              if (NPL == 2) tma_load3(sB + Cfg::B_PLANE + lane * 8192, &p.tm_g_lo, w.n0 + lane * 64, row0, 0, &full_bar[stage]);
+            }
+          } else if (x_bytes && lane < 4 + 2 * nbox) {
+            const int j = (lane - 4) >> 1, a = (lane - 4) & 1;
+            const uint32_t mu = (uint32_t)(row0 + j * box_rows);     // rows past M are samples past the batch: zeros
+            const int b = (int)fdiv(mu, p.div_hw); const int rem = (int)(mu - (uint32_t)b * (uint32_t)HW);
+            const int y = (int)fdiv((uint32_t)rem, p.div_w); const int x = rem - y * g.Wx;
+            const int c0 = w.c0 + a * 64, xs = x * g.sx + g.ox[w.tap], ys = y * g.sy + g.oy[w.tap];
+            const uint32_t dst = sA + a * 8192 + j * box_rows * 128;
+            tma_load4(dst, &p.tm_x_hi, c0, xs, ys, b, &full_bar[stage]);
+            if (NPL == 2) tma_load4(dst + Cfg::A_PLANE, &p.tm_x_lo, c0, xs, ys, b, &full_bar[stage]);
+          }
+          if (++stage == S) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else if (warp < 4) {
     // ---- producers: every K-row (one output position m) is a contiguous run of channels / columns in global memory
     const int t = threadIdx.x;
     const int chunk = t & 7, rsub = t >> 3;                 // 8 threads x 16 B = one 128-byte atom row; 16 rows per pass
@@ -1281,6 +1339,7 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
             const uint32_t so = sw128(kr, chunk);
 #pragma unroll
             for (int a = 0; a < 2; ++a) {                     // 2 channel atoms of 64
+              if (p.debug & 4) break;                           // (tc_debug 4: the X rows are not loaded)
               const bool ok = xoff[i] >= 0 && (w.c0 + a * 64) < p.x_ld;
               uint2 vh = make_uint2(0u, 0u), vl = make_uint2(0u, 0u);
               if (ok) { vh = __ldg(reinterpret_cast<const uint2*>(p.x8_hi + xoff[i] + a * 64)); vl = __ldg(reinterpret_cast<const uint2*>(p.x8_lo + xoff[i] + a * 64)); }
@@ -1318,6 +1377,7 @@ tc_gg_tn_kernel(const __grid_constant__ TcTNParams p) {
               }
             }
           }
+          if (!(p.debug & 4))                                  // (tc_debug 4: the X rows are not loaded)
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const uint32_t so = sw128(rsub + 16 * i, chunk);   // (kr/8)*1024 + (kr%8)*128 + swizzled chunk
@@ -1667,6 +1727,19 @@ cudaError_t launch_nt(TcNTParams p, int precision, cudaStream_t st, int epi) {
   return cudaGetLastError();
 }
 
+// The TMA form of the weight-gradient kernel takes the dense geometries whose 64-row stages are boxes of the source planes: a stage is
+// 64 / Wx whole output rows (Wx divides 64) or 64 positions of one output row (64 divides Wx).  K-rows are sample-major, so a box of
+// whole rows may start in one sample and the next box in the next; with Hy == 1 the 64 / Wx samples of a stage share one box.  Wx >= 8
+// keeps every box on a 1024-byte boundary of the stage.  Rows past M in the last stage are samples past the batch, zeros in the box as
+// in the gather.  Encodes p's activation maps and returns true; false leaves the geometry (or a plane the encoder refuses) to the gather.
+static bool tn_tma_maps(TcTNParams& p, int npl) {
+  const GatherGeom& g = p.g;
+  const int wx = g.Wx < 64 ? g.Wx : 64;
+  if (g.Wx < 8 || 64 % wx || g.Wx % wx || wx * g.sx > 256 || g.sx > 8) return false;
+  const uint32_t bx = (uint32_t)(wx * g.sx), nb = g.Hy == 1 ? (uint32_t)(64 / wx) : 1u;
+  return make_tmap_act(&p.tm_x_hi, p.x_hi, 2, p.x_ld, g, bx, nb) && (npl != 2 || make_tmap_act(&p.tm_x_lo, p.x_lo, 2, p.x_ld, g, bx, nb));
+}
+
 cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st, const DetSlab* det) {
   const long long M = (long long)p.g.B * p.g.Hy * p.g.Wx;
   if (M == 0) return cudaSuccess;
@@ -1726,14 +1799,21 @@ cudaError_t launch_tn(TcTNParams p, int precision, cudaStream_t st, const DetSla
       else if (precision == 1) LAUNCH_TN(2, 0, 0, 1);
       else                     LAUNCH_TN(1, 0, 0, 1);
     }
-  } else if (det_split) {
-    if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 1); else LAUNCH_TN(3, 0, 1); }
-    else if (precision == 1) LAUNCH_TN(2, 0, 1);
-    else                     LAUNCH_TN(1, 0, 1);
   } else {
-    if (precision == 3) { if (p.w16) LAUNCH_TN(3, 1, 0); else LAUNCH_TN(3, 0, 0); }
-    else if (precision == 1) LAUNCH_TN(2, 0, 0);
-    else                     LAUNCH_TN(1, 0, 0);
+    // dense rows: the TMA form where the stages are boxes of the activation planes (not F16F8's cross pass, whose producers widen
+    // the e4m3 planes), else the gather
+    const bool ta = (precision != 3 || p.w16) && tn_tma_maps(p, precision == 1 ? 2 : 1);
+#define LAUNCH_TN_D(NPL_, W16_, DET_) do { if (ta) LAUNCH_TN(NPL_, W16_, DET_, 0, 1); else LAUNCH_TN(NPL_, W16_, DET_); } while (0)
+    if (det_split) {
+      if (precision == 3) { if (p.w16) LAUNCH_TN_D(3, 1, 1); else LAUNCH_TN(3, 0, 1); }
+      else if (precision == 1) LAUNCH_TN_D(2, 0, 1);
+      else                     LAUNCH_TN_D(1, 0, 1);
+    } else {
+      if (precision == 3) { if (p.w16) LAUNCH_TN_D(3, 1, 0); else LAUNCH_TN(3, 0, 0); }
+      else if (precision == 1) LAUNCH_TN_D(2, 0, 0);
+      else                     LAUNCH_TN_D(1, 0, 0);
+    }
+#undef LAUNCH_TN_D
   }
 #undef LAUNCH_TN
   prof_end(st);
@@ -1906,14 +1986,14 @@ int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat1
   return 0;
 }
 
-int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+int tc_conv_wgrad(const TcLayer& L, int precision, int debug, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dwa, float* dwg, cudaStream_t st, const DetSlab* det, const PackGeom* pk) {
   if (!layer_ok(L) || (precision == 3 && !layer_ok_q(L))) return TC_UNSUPPORTED;
   if (pk && (n != 1 || (H == 1 && L.kh != 1))) return (int)cudaErrorInvalidValue;     // H > 1: packed 2-D grids
   TcTNParams p; memset(&p, 0, sizeof p);
   if (pk) p.pk = *pk;
-  p.w16 = (precision == 3 && w16) ? 1 : 0;
+  p.w16 = (precision == 3 && w16) ? 1 : 0; p.debug = debug;
   p.fold_n = L.fold ? L.cout / L.fold : 0;
   p.g = fwd_geom(n, H, W, L.kh, L.kw, sh, sw);
   p.x_hi = xhi; p.x_lo = xlo; p.x_ld = cin_k(L); p.C = L.cin;
@@ -2034,6 +2114,10 @@ static cudaError_t tc_init_kernels() {
 #define INIT_TN(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
   INIT_TN(3, 1, 0) INIT_TN(3, 0, 0) INIT_TN(2, 0, 0) INIT_TN(1, 0, 0)
   INIT_TN(3, 1, 1) INIT_TN(3, 0, 1) INIT_TN(2, 0, 1) INIT_TN(1, 0, 1)
+#define INIT_TN_TA(NPL_, W16_, DET_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_, 0, 1>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
+  INIT_TN_TA(3, 1, 0) INIT_TN_TA(2, 0, 0) INIT_TN_TA(1, 0, 0)
+  INIT_TN_TA(3, 1, 1) INIT_TN_TA(2, 0, 1) INIT_TN_TA(1, 0, 1)
+#undef INIT_TN_TA
 #define INIT_TN_PK(NPL_, W16_, DET_, PK_) if ((e = set_smem(tc_gg_tn_kernel<NPL_, W16_, DET_, PK_>, TNCfg<NPL_, W16_>::SMEM)) != cudaSuccess) return e;
   INIT_TN_PK(3, 1, 0, 1) INIT_TN_PK(3, 0, 0, 1) INIT_TN_PK(2, 0, 0, 1) INIT_TN_PK(1, 0, 0, 1)
   INIT_TN_PK(3, 1, 1, 1) INIT_TN_PK(3, 0, 1, 1) INIT_TN_PK(2, 0, 1, 1) INIT_TN_PK(1, 0, 1, 1)

@@ -48,7 +48,7 @@ struct TcWeights {
   int wgrad16 = 0;                // "wgrad_f16" (F16F8 only; tc_alloc sets it there): weight gradients from the fp16 planes alone
                                   // (one MMA unit per product instead of two)
   int prep_batched = 1;           // "prep_batched": F16F8 weight planes of all layers in one launch; 0: per-layer kernels
-  int debug = 0;                  // "tc_debug": diagnostic knobs of the NT kernel (timing experiments only; see TcNTParams::debug)
+  int debug = 0;                  // "tc_debug": diagnostic knobs of the gather-GEMMs (timing experiments only; see TcNTParams::debug)
 };
 
 // what the fused forward epilogue needs besides the convolution itself (see tc_conv_fwd)
@@ -114,7 +114,7 @@ int tc_conv_dgrad(const TcLayer& L, int precision, int debug, const __nv_bfloat1
 // dW_a/dW_g (TF layout) += x^T dP  (the bias gradients are column sums of dP: the instance-norm backward kernels or launch_colsum)
 //   pk:   packed utterances as in tc_conv_fwd (x planes at the source level of divisor pk->div): a tap outside its row's utterance
 //         contributes a zero row
-int tc_conv_wgrad(const TcLayer& L, int precision, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
+int tc_conv_wgrad(const TcLayer& L, int precision, int debug, int w16, const __nv_bfloat16* xhi, const __nv_bfloat16* xlo,
                   const __nv_bfloat16* dPhi, const __nv_bfloat16* dPlo, int n, int H, int W, int sh, int sw,
                   float* dwa, float* dwg, cudaStream_t st, const DetSlab* det = nullptr,   // det: deterministic mode (kernels.cuh DetSlab)
                   const PackGeom* pk = nullptr);
