@@ -175,8 +175,20 @@ int cgvc_compute_gradients(cgvc_handle h, const float* A_dev, const float* B_dev
  * Loss scale of the tape backward calls (cgvc_*_backward_tape): in CGVC_PREC_F16F8 they leave their GRAD contributions multiplied by
  * the static loss scale of their tape's batch, s = 2^(9 + floor(log2 batch)) (1 in the other precisions; see cgvc_loss_scale_state);
  * Adam over such gradients takes grad_scale = 1 / s (times 1/nranks after an all-reduce).  Gradients of tapes of batches with different
- * scales do not share one GRAD: zero it in between. */
+ * scales do not share one GRAD: zero it in between.  No all-reduce: with a communicator, call cgvc_allreduce_grads first. */
 int cgvc_adam_step(cgvc_handle h, float lr_generator, float lr_discriminator, float grad_scale, void* stream);
+
+/* The optimizer tail of cgvc_train_step over the gradients that tape backward calls accumulated in GRAD (option "tape_loss_scale" = 1,
+ * which needs "loss_scale" = 2).  With a communicator: the per-network all-reduce of GRAD and of the counters (pipelined with each
+ * network's Adam when "pipelined_comm" is on).  Then the non-finite check of GRAD and the scaler update: on a saturated gradient plane
+ * or a non-finite gradient the step is skipped and the scale halves (per network with "loss_scale_per_network": that network's), else
+ * Adam runs with grad_scale = 1 / (scale x nranks) per optimizer and the scale doubles after "loss_scale_growth_interval" good steps.
+ * Then the weight-plane refresh; the parameter generation advances even when the step was skipped.  The Adam count t stays on the
+ * device, and nothing synchronises the host; cgvc_loss_scale_state reports the step as after a train step.  The counters and the
+ * non-finite flag of the next accumulation are cleared by its first tape backward (or by this call, when none ran).
+ * Errors, before anything is enqueued: the option off, or no scale yet (neither a tape backward nor cgvc_set_loss_scale_state since
+ * "loss_scale" became 2): CGVC_ERR_ARG; PARAM, GRAD, ADAM_M or ADAM_V unbound: CGVC_ERR_UNBOUND. */
+int cgvc_apply_gradients(cgvc_handle h, float lr_generator, float lr_discriminator, void* stream);
 
 /* -- replaces CycleGAN.test (model.py:128-137): one generator forward.  direction 0 = 'A2B', 1 = 'B2A';
  * anything else returns CGVC_ERR_DIRECTION ("Conversion direction must be specified.", model.py:135). */
@@ -233,14 +245,23 @@ int cgvc_discriminator_forward_packed(cgvc_handle h, int which, const float* in_
  *     are formed and d in is returned with it removed (exact: a power of two); the GRAD contributions keep it (see cgvc_adam_step).
  *     With "loss_scale" = 1 the backward counts its saturated gradient-plane groups into the counters of cgvc_loss_scale_state (and the
  *     per-network ones: the generator's into index 0, the discriminator's into index 1), adding to them until the next train step clears
- *     them.  The dynamic policy ("loss_scale" = 2) does not act on tape calls: no skip, no scale change; they use the static scale.
+ *     them.  With "loss_scale" = 2 and "tape_loss_scale" = 0 (the default) tape calls use the static scale and are not counted.
+ *   - "tape_loss_scale" = 1 (needs "loss_scale" = 2): the dynamic policy acts on tape calls.  The upstream gradient is multiplied by the
+ *     scaler's current scale, read on the device: s_G for a generator tape and s_D for a discriminator tape with
+ *     "loss_scale_per_network", else the one scale.  d in is returned with that scale removed, and the backward counts its gradient
+ *     planes (per network: into that network's block) for cgvc_apply_gradients, which checks, skips or applies the step and is the only
+ *     call that changes the scale, so that every tape backward between two of them uses one scale per network.  The first tape
+ *     backward before any scale was set starts the scaler from the static scale of its tape's batch, as a first train step does.  A
+ *     discriminator tape uses s_D also when back-propagated as part of a generator loss; its d in leaves unscaled, and the generator tape
+ *     then applies s_G.  A saturation in that pass therefore halves s_D and skips the step, even if its discriminator gradients are
+ *     discarded afterwards.  A train step in between discards the accumulation (it zeroes GRAD and the counters).
  *   - Options: "deterministic" makes repeated forward / backward sequences give the same GRAD bits; the kernel-choice options act as in a
  *     train step.  Tape calls run eagerly on `stream`, never as captured graphs.
  * Kind 3 = packed discriminator (cgvc_discriminator_forward_packed_tape): cgvc_tape_bytes(h, 3, n, rows, &bytes) as for kind 2, every length a
  * multiple of 16; cgvc_discriminator_backward_tape takes kinds 1 and 3, with d prob and d in in the packed layouts of
  * cgvc_discriminator_forward_packed, every tap and instance norm inside its utterance; the generator backward refuses kind 3.
- * Not covered: per-call or per-network loss scales, data-parallel reduction (cgvc_allreduce_grads sums
- * GRAD over ranks). */
+ * Not covered: loss scales the caller passes per call; without "tape_loss_scale", data-parallel reduction (cgvc_allreduce_grads sums
+ * GRAD over ranks; cgvc_apply_gradients all-reduces). */
 int cgvc_tape_bytes(cgvc_handle h, int kind, int batch, int frames, size_t* bytes);
 /* cgvc_discriminator_forward_packed with a kind 3 tape: the same argument checks and errors, all before anything is enqueued, then the
  * tape checks above; prob_dev bit for bit what cgvc_discriminator_forward_packed writes.  The offsets and the row prefix sums of the
@@ -355,6 +376,8 @@ int cgvc_kernel_launches(unsigned long long* count);
  * in shared memory instead of holding a sample's rows in registers (needs post_onepass = 1).
  * "loss_scale" (default 0; 0, 1 or 2), "loss_scale_growth_interval" (default 2000; >= 1) and "loss_scale_per_network" (default 0): see
  * cgvc_loss_scale_state.  Switching "loss_scale_per_network" on while a dynamic scale is in use starts both networks from it.
+ * "tape_loss_scale" (default 0): 1 puts the tape backward calls on the dynamic scaler (see the activation tapes and
+ * cgvc_apply_gradients).  Setting it to 1 outside "loss_scale" = 2, or moving "loss_scale" away from 2 while it is 1: CGVC_ERR_ARG.
  * "deterministic" (default 0): 1 makes cgvc_train_step and cgvc_compute_gradients bitwise reproducible on one GPU.  The same inputs,
  * PARAM, ADAM_M / ADAM_V, Adam step, loss-scaler state, batch, frames, precision and options give the same bits of PARAM, GRAD, ADAM_M,
  * ADAM_V, the 8 losses, gen_A / gen_B and the scaler state, in every precision and loss_scale mode, on repeated calls and fresh

@@ -80,6 +80,7 @@ def _declare(lib):
         "cgvc_train_step": (ci, [vp, vp, vp, ci, ci, cf, cf, cf, cf, vp, vp, vp, vp]),
         "cgvc_compute_gradients": (ci, [vp, vp, vp, ci, ci, cf, cf, vp, vp, vp, vp]),
         "cgvc_adam_step": (ci, [vp, cf, cf, cf, vp]),
+        "cgvc_apply_gradients": (ci, [vp, cf, cf, vp]),
         "cgvc_generator_forward": (ci, [vp, ci, vp, vp, ci, ci, vp]),
         "cgvc_generator_forward_packed": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp]),
         "cgvc_discriminator_forward_packed": (ci, [vp, ci, vp, vp, P(C.c_longlong), ci, vp]),

@@ -154,6 +154,7 @@ struct Options {
   int ls_mode = 0;              // "loss_scale": 0 static, 1 monitor (static scale, counters collected), 2 dynamic
   int ls_growth = 2000;         // "loss_scale_growth_interval"
   int ls_nets = 0;              // "loss_scale_per_network": one scale for the generators' passes, one for the discriminators' D-loss pass
+  int tape_ls = 0;              // "tape_loss_scale" (needs ls_mode 2): tape backwards scale by the scaler and count; cgvc_apply_gradients
   PostForms post = {1, 1};      // "post_onepass", "post_stream": the forms the instance-norm kernels may take (kernels.cuh)
 };
 
@@ -195,6 +196,7 @@ struct cgvc_engine {
                                 // it picks the scale of the loss gradients and the counter block of the gradient-plane writers
   unsigned long long* plane_ufl = nullptr;   // cgvc_set_plane_counters: [ufl, groups] the per-kernel plane entry points add into
   cudaEvent_t ev_ls = nullptr;  // data parallel: the saturation all-reduce and the GRAD check are done (comm stream)
+  bool tape_open = false;       // "tape_loss_scale": the counters of the gradients accumulating for cgvc_apply_gradients were cleared
   // debug taps of the last forward
   std::map<std::string, std::pair<const float*, size_t>> taps;
   // the instance-norm sums scratch of the calls outside a train step (which has its WORK slices): conversions, cgvc_in_glu_*
@@ -1719,82 +1721,22 @@ static int check_work_train(cgvc_engine* e, int batch, int frames) {
   return 0;
 }
 
-extern "C" {
-
-int cgvc_compute_gradients(cgvc_handle e, const float* A_dev, const float* B_dev, int batch, int frames,
-                           float lambda_cycle, float lambda_identity, float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream) {
-  if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
-  RET(check_work_train(e, batch, frames));
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  RET(set_lambdas(e, lambda_cycle, lambda_identity, (cudaStream_t)stream));
-  RET(ls_prepare(e, batch, (cudaStream_t)stream));
-  RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, (cudaStream_t)stream));
-  // the gradients are handed out, not fed to Adam: remove the loss scale here (in dynamic mode the device scale they were formed with)
-  if (e->opt.ls_mode == 2 && ls_nets(e)) {                 // each GRAD range its own network's scale
-    const long long gend = (long long)e->gen[1].end;
-    CK(launch_scale(e->G(), gend, 1.f, (cudaStream_t)stream, &e->ls->net[0].scale));
-    CK(launch_scale(e->G() + gend, (long long)e->n_params - gend, 1.f, (cudaStream_t)stream, &e->ls->net[1].scale));
-  } else if (e->opt.ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
-  else if (loss_scale(e, batch) != 1.f) CK(launch_scale(e->G(), (long long)e->n_params, 1.f / loss_scale(e, batch), (cudaStream_t)stream));
+// "tape_loss_scale": the gradients that tape backward calls accumulate for cgvc_apply_gradients are checked against counters of their own.
+// The first tape backward after a step (or cgvc_apply_gradients, when none ran) clears the counters and the non-finite flag, so that
+// those of the step before stay readable (cgvc_loss_scale_state) until the next accumulation starts
+static int tape_counts_open(cgvc_engine* e, cudaStream_t st) {
+  if (e->tape_open) return 0;
+  CK(cudaMemsetAsync(&e->ls->nonfinite, 0, (char*)(&e->ls->sat_act + 1) - (char*)&e->ls->nonfinite, st));
+  CK(cudaMemsetAsync(e->ls->cnt, 0, sizeof e->ls->cnt, st));
+  e->tape_open = true;
   return 0;
 }
 
-int cgvc_adam_step(cgvc_handle e, float lr_g, float lr_d, float grad_scale, void* stream) {
-  if (!e) return CGVC_ERR_ARG;
-  for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  // dynamic loss-scale mode keeps t on the device: bring it to the host (synchronises), step with the host's lr_t like the other
-  // modes, and write the advanced t back (synchronises again).  No skip: the caller decides on this step
-  if (e->opt.ls_mode == 2) { long long t; RET(cgvc_get_adam_step(e, &t)); }
-  const long long t_before = e->adam_t;
-  RET(set_adam_scalars(e, lr_g, lr_d, grad_scale, (cudaStream_t)stream));
-  int r = adam_body(e, (cudaStream_t)stream);
-  if (r != 0) { e->adam_t = t_before; return r; }
-  if (e->opt.ls_mode == 2) RET(cgvc_set_adam_step(e, e->adam_t));
-  return 0;
-}
-
-int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int batch, int frames,
-                    float lambda_cycle, float lambda_identity, float lr_g, float lr_d,
-                    float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream) {
-  if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
-  for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
-  RET(check_work_train(e, batch, frames));
-  ++e->param_gen;                                            // a replayed graph does not run adam_body's host code
-  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const float gscale = (e->comm ? 1.f / (float)e->nranks : 1.f) / loss_scale(e, batch);
-  RET(set_lambdas(e, lambda_cycle, lambda_identity, st));
-  // the Adam step counter advances only if the whole step was enqueued: a call that is refused further down (WORK arena too small,
-  // capture failure, NCCL error) must not change the bias correction of the next one
-  const long long adam_t_before = e->adam_t;
-  struct Rollback { cgvc_engine* e; long long t; bool armed; ~Rollback() { if (armed) e->adam_t = t; } } rollback{e, adam_t_before, true};
-  RET(set_adam_scalars(e, lr_g, lr_d, e->opt.ls_mode == 2 ? (e->comm ? 1.f / (float)e->nranks : 1.f) : gscale, st, e->opt.ls_mode == 2));
-  RET(ls_prepare(e, batch, st));
-  if (e->opt.use_graphs && !tc_profile_is_on()) {
-    // the graphs read the inputs from fixed staging buffers and leave the results in the WORK arena / d_scalars, so one
-    // captured graph serves any caller pointers; the copies either side are eager
-    const size_t img = (size_t)batch * e->cfg.num_features * frames;
-    const size_t cap = (size_t)e->cfg.max_batch * e->cfg.num_features * e->cfg.max_frames;
-    if (!e->stage) CK(cudaMalloc(&e->stage, 2 * cap * sizeof(float)));
-    float* sA = e->stage; float* sB = e->stage + cap;
-    CK(cudaMemcpyAsync(sA, A_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(sB, B_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    GraphKey key; memset(&key, 0, sizeof key);
-    key.batch = batch; key.frames = frames; key.id_off = lambda_identity == 0.f; key.kind = 0;
-    RET(run_captured(e, key, st, [&](cudaStream_t s) {
-      return forward_backward(e, sA, sB, batch, frames, lambda_cycle, lambda_identity, nullptr, nullptr, nullptr, s);
-    }));
-    if (gen_A_dev || gen_B_dev) {
-      Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
-      TrainPlan P; plan_train(e, ws, P, batch, frames);
-      if (gen_B_dev) CK(cudaMemcpyAsync(gen_B_dev, P.lane[0].din + img, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      if (gen_A_dev) CK(cudaMemcpyAsync(gen_A_dev, P.lane[1].din + img, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    }
-    if (losses_dev) CK(cudaMemcpyAsync(losses_dev, e->d_scalars + 8, 8 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  } else {
-    RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, st));
-  }
+// The optimizer tail of a step, behind the gradients in GRAD on stream st: with a communicator the gradient all-reduce (per network and
+// pipelined with each network's Adam and plane refresh when "pipelined_comm" is on), then with "loss_scale" != 0 the GRAD check and the
+// scaler update, then Adam (skipped by the scaler in dynamic mode) and the refresh of the tensor-core weight planes.  The Adam scalars
+// are already written (set_adam_scalars).  cgvc_train_step and cgvc_apply_gradients
+static int optimizer_tail(cgvc_engine* e, cudaStream_t st) {
   if (e->comm && e->opt.pipelined_comm && e->comm_stream) {
     // one all-reduce per network (arena order), all enqueued on the communication stream behind the step's gradients; the caller's
     // stream then takes the networks one by one: wait for its all-reduce, Adam over its range, refresh of its tensor-core planes
@@ -1835,11 +1777,10 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
       }));
     }
     if (e->opt.ls_mode == 1) CK(cudaStreamWaitEvent(st, e->ev_ls, 0));
-    rollback.armed = false;
     return 0;
   }
   if (e->comm) {
-    RET(cgvc_allreduce_grads(e, stream));
+    RET(cgvc_allreduce_grads(e, (void*)st));
     if (e->opt.ls_mode == 2) RET(ls_allreduce_counts(e, st));
   }
   GraphKey k2; memset(&k2, 0, sizeof k2); k2.kind = 1;
@@ -1848,7 +1789,105 @@ int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int b
     if (e->opt.ls_mode == 2 || ls_nets(e)) RET(ls_update(e, s));
     return adam_body(e, s, ls_skip(e));
   }));
+  return 0;
+}
+
+extern "C" {
+
+int cgvc_compute_gradients(cgvc_handle e, const float* A_dev, const float* B_dev, int batch, int frames,
+                           float lambda_cycle, float lambda_identity, float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream) {
+  if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
+  RET(check_work_train(e, batch, frames));
+  e->tape_open = false;
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  RET(set_lambdas(e, lambda_cycle, lambda_identity, (cudaStream_t)stream));
+  RET(ls_prepare(e, batch, (cudaStream_t)stream));
+  RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, (cudaStream_t)stream));
+  // the gradients are handed out, not fed to Adam: remove the loss scale here (in dynamic mode the device scale they were formed with)
+  if (e->opt.ls_mode == 2 && ls_nets(e)) {                 // each GRAD range its own network's scale
+    const long long gend = (long long)e->gen[1].end;
+    CK(launch_scale(e->G(), gend, 1.f, (cudaStream_t)stream, &e->ls->net[0].scale));
+    CK(launch_scale(e->G() + gend, (long long)e->n_params - gend, 1.f, (cudaStream_t)stream, &e->ls->net[1].scale));
+  } else if (e->opt.ls_mode == 2) CK(launch_scale(e->G(), (long long)e->n_params, 1.f, (cudaStream_t)stream, &e->ls->scale));
+  else if (loss_scale(e, batch) != 1.f) CK(launch_scale(e->G(), (long long)e->n_params, 1.f / loss_scale(e, batch), (cudaStream_t)stream));
+  return 0;
+}
+
+int cgvc_adam_step(cgvc_handle e, float lr_g, float lr_d, float grad_scale, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  // dynamic loss-scale mode keeps t on the device: bring it to the host (synchronises), step with the host's lr_t like the other
+  // modes, and write the advanced t back (synchronises again).  No skip: the caller decides on this step
+  if (e->opt.ls_mode == 2) { long long t; RET(cgvc_get_adam_step(e, &t)); }
+  const long long t_before = e->adam_t;
+  RET(set_adam_scalars(e, lr_g, lr_d, grad_scale, (cudaStream_t)stream));
+  int r = adam_body(e, (cudaStream_t)stream);
+  if (r != 0) { e->adam_t = t_before; return r; }
+  if (e->opt.ls_mode == 2) RET(cgvc_set_adam_step(e, e->adam_t));
+  return 0;
+}
+
+int cgvc_train_step(cgvc_handle e, const float* A_dev, const float* B_dev, int batch, int frames,
+                    float lambda_cycle, float lambda_identity, float lr_g, float lr_d,
+                    float* gen_A_dev, float* gen_B_dev, float* losses_dev, void* stream) {
+  if (!e || !A_dev || !B_dev) return fail(e, CGVC_ERR_ARG, "null argument");
+  for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
+  RET(check_work_train(e, batch, frames));
+  ++e->param_gen;                                            // a replayed graph does not run adam_body's host code
+  e->tape_open = false;                                      // the step zeroes GRAD and the counters: a tape accumulation starts anew
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const float gscale = (e->comm ? 1.f / (float)e->nranks : 1.f) / loss_scale(e, batch);
+  RET(set_lambdas(e, lambda_cycle, lambda_identity, st));
+  // the Adam step counter advances only if the whole step was enqueued: a call that is refused further down (WORK arena too small,
+  // capture failure, NCCL error) must not change the bias correction of the next one
+  const long long adam_t_before = e->adam_t;
+  struct Rollback { cgvc_engine* e; long long t; bool armed; ~Rollback() { if (armed) e->adam_t = t; } } rollback{e, adam_t_before, true};
+  RET(set_adam_scalars(e, lr_g, lr_d, e->opt.ls_mode == 2 ? (e->comm ? 1.f / (float)e->nranks : 1.f) : gscale, st, e->opt.ls_mode == 2));
+  RET(ls_prepare(e, batch, st));
+  if (e->opt.use_graphs && !tc_profile_is_on()) {
+    // the graphs read the inputs from fixed staging buffers and leave the results in the WORK arena / d_scalars, so one
+    // captured graph serves any caller pointers; the copies either side are eager
+    const size_t img = (size_t)batch * e->cfg.num_features * frames;
+    const size_t cap = (size_t)e->cfg.max_batch * e->cfg.num_features * e->cfg.max_frames;
+    if (!e->stage) CK(cudaMalloc(&e->stage, 2 * cap * sizeof(float)));
+    float* sA = e->stage; float* sB = e->stage + cap;
+    CK(cudaMemcpyAsync(sA, A_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(sB, B_dev, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    GraphKey key; memset(&key, 0, sizeof key);
+    key.batch = batch; key.frames = frames; key.id_off = lambda_identity == 0.f; key.kind = 0;
+    RET(run_captured(e, key, st, [&](cudaStream_t s) {
+      return forward_backward(e, sA, sB, batch, frames, lambda_cycle, lambda_identity, nullptr, nullptr, nullptr, s);
+    }));
+    if (gen_A_dev || gen_B_dev) {
+      Bump ws; ws.reset(e->arena[CGVC_ARENA_WORK], e->arena_bytes[CGVC_ARENA_WORK]);
+      TrainPlan P; plan_train(e, ws, P, batch, frames);
+      if (gen_B_dev) CK(cudaMemcpyAsync(gen_B_dev, P.lane[0].din + img, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      if (gen_A_dev) CK(cudaMemcpyAsync(gen_A_dev, P.lane[1].din + img, img * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    }
+    if (losses_dev) CK(cudaMemcpyAsync(losses_dev, e->d_scalars + 8, 8 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  } else {
+    RET(forward_backward(e, A_dev, B_dev, batch, frames, lambda_cycle, lambda_identity, gen_A_dev, gen_B_dev, losses_dev, st));
+  }
+  RET(optimizer_tail(e, st));
   rollback.armed = false;
+  return 0;
+}
+
+int cgvc_apply_gradients(cgvc_handle e, float lr_g, float lr_d, void* stream) {
+  if (!e) return CGVC_ERR_ARG;
+  if (!e->opt.tape_ls) return fail(e, CGVC_ERR_ARG, "cgvc_apply_gradients needs the option tape_loss_scale = 1 (else: cgvc_adam_step)");
+  for (int a = 0; a < 4; ++a) if (!e->arena[a]) return fail(e, CGVC_ERR_UNBOUND, "PARAM/GRAD/ADAM_M/ADAM_V arenas must be bound");
+  if (!e->ls_ready)
+    return fail(e, CGVC_ERR_ARG, "no loss scale yet: a tape backward or cgvc_set_loss_scale_state sets it before cgvc_apply_gradients");
+  ++e->param_gen;                                            // a replayed graph does not run adam_body's host code
+  DeviceGuard dguard; CK(dguard.set(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  RET(tape_counts_open(e, st));                              // no tape backward since the last step: nothing was counted
+  RET(set_adam_scalars(e, lr_g, lr_d, e->comm ? 1.f / (float)e->nranks : 1.f, st, true));
+  RET(optimizer_tail(e, st));
+  e->tape_open = false;
   return 0;
 }
 
@@ -1916,7 +1955,7 @@ static const OptionDef kOptions[] = {
   OPT("debug_taps", 0, 1, opt.debug_taps),          OPT("cuda_graph", 0, 1, opt.use_graphs),
   OPT("post_onepass", 0, 1, opt.post.onepass),      OPT("post_stream", 0, 1, opt.post.stream),
   OPT("loss_scale", 0, 2, opt.ls_mode),             OPT("loss_scale_growth_interval", 1, INT_MAX, opt.ls_growth),
-  OPT("loss_scale_per_network", 0, 1, opt.ls_nets),
+  OPT("loss_scale_per_network", 0, 1, opt.ls_nets),  OPT("tape_loss_scale", 0, 1, opt.tape_ls),
   OPT("wgrad_f16", 0, 1, tcw.wgrad16),              OPT("prep_batched", 0, 1, tcw.prep_batched),
   OPT("tc_debug", 0, 7, tcw.debug),
 };
@@ -1931,6 +1970,10 @@ int cgvc_set_option(cgvc_handle e, const char* name, int value) {
   if (value < d->lo || value > d->hi) return fail(e, CGVC_ERR_ARG, "option %s: bad value %d", name, value);
   int* field = d->field(e);
   if (*field == value) return 0;
+  if (field == &e->opt.tape_ls && value && e->opt.ls_mode != 2)
+    return fail(e, CGVC_ERR_ARG, "option tape_loss_scale = 1 needs loss_scale = 2 (dynamic)");
+  if (field == &e->opt.ls_mode && e->opt.tape_ls)
+    return fail(e, CGVC_ERR_ARG, "loss_scale must stay 2 while tape_loss_scale = 1");
   if (field == &e->opt.ls_mode) {
     DeviceGuard dguard; CK(dguard.set(e->cfg.device));
     long long t = 0;
@@ -2751,21 +2794,35 @@ static int tape_backward_entry(cgvc_engine* e, int kind, const void* tape, const
   return 0;
 }
 
-// d in of a tape backward to the caller (din null: none): a generator's out of the channels-last rows, with the loss scale s of the
-// gradient planes taken out (exact: a power of two)
-static int tape_din(cgvc_engine* e, const NetGeom& a, const AppPlan& P, const float* rows, float* din, float s, cudaStream_t st) {
-  if (!din) return 0;
-  if (!disc_kind(a.kind)) CK(transpose_app(e, a, P.g, rows, din, false, st));
-  if (s != 1.f) CK(launch_scale(din, a.rows * e->cfg.num_features, 1.f / s, st));
+// the upstream gradient is counted like a train step's in monitor mode (loss_scale = 1), and in dynamic mode with "tape_loss_scale",
+// into network `net`'s block
+struct TapeCounting {
+  cgvc_engine* e;
+  TapeCounting(cgvc_engine* en, int net) : e(en) { e->counting = e->opt.ls_mode == 1 || e->opt.tape_ls; e->ls_net = net; }
+  ~TapeCounting() { e->counting = false; e->ls_net = 0; }
+};
+
+// The loss scale of a tape backward's gradient planes: with "tape_loss_scale" the scaler's current scale of the network being enqueued
+// (e->ls_net), read on the device (dev), after the first such call set the scaler from the static scale of its tape's batch (as a first
+// train step does) and cleared the accumulation's counters; else the static scale s of the tape's batch (1 outside F16F8)
+struct TapeScale { float s; const float* dev; };
+static int tape_scale(cgvc_engine* e, const NetGeom& a, cudaStream_t st, TapeScale* ts) {
+  if (!e->opt.tape_ls) { *ts = TapeScale{loss_scale(e, a.n), nullptr}; return 0; }
+  RET(ls_prepare(e, a.n, st));
+  RET(tape_counts_open(e, st));
+  *ts = TapeScale{1.f, loss_scale_dev(e, a.n)};
   return 0;
 }
 
-// the upstream gradient is counted like a train step's in monitor mode (loss_scale = 1), into network `net`'s block
-struct TapeCounting {
-  cgvc_engine* e;
-  TapeCounting(cgvc_engine* en, int net) : e(en) { e->counting = e->opt.ls_mode == 1; e->ls_net = net; }
-  ~TapeCounting() { e->counting = false; e->ls_net = 0; }
-};
+// d in of a tape backward to the caller (din null: none): a generator's out of the channels-last rows, with the loss scale s of the
+// gradient planes taken out (exact: a power of two)
+static int tape_din(cgvc_engine* e, const NetGeom& a, const AppPlan& P, const float* rows, float* din, const TapeScale& s, cudaStream_t st) {
+  if (!din) return 0;
+  if (!disc_kind(a.kind)) CK(transpose_app(e, a, P.g, rows, din, false, st));
+  if (s.dev) CK(launch_scale(din, a.rows * e->cfg.num_features, 1.f, st, s.dev));
+  else if (s.s != 1.f) CK(launch_scale(din, a.rows * e->cfg.num_features, 1.f / s.s, st));
+  return 0;
+}
 
 extern "C" {
 
@@ -2828,14 +2885,14 @@ int cgvc_generator_backward_tape(cgvc_handle e, const void* tape_dev, const floa
   DeviceGuard dguard; CK(dguard.set(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   // the upstream gradient channels-last, times the loss scale of the F16F8 gradient planes; a packed tape of n utterances takes the
-  // scale of a batch of n
-  const float s = loss_scale(e, a.n);
+  // static scale of a batch of n
+  TapeCounting counting(e, 0);
+  TapeScale s;
+  RET(tape_scale(e, a, st, &s));
   CK(transpose_app(e, a, P.g, dout_dev, L.d_out, true, st));
-  if (s != 1.f) CK(launch_scale(L.d_out, a.rows * e->cfg.num_features, s, st));
-  {
-    TapeCounting counting(e, 0);
-    RET(generator_backward(e, e->gen[a.which], P.g, L.d_out, din_dev ? L.in : nullptr, L.S, st));
-  }
+  if (s.dev) CK(launch_scale_by(L.d_out, a.rows * e->cfg.num_features, 1.f, s.dev, st));
+  else if (s.s != 1.f) CK(launch_scale(L.d_out, a.rows * e->cfg.num_features, s.s, st));
+  RET(generator_backward(e, e->gen[a.which], P.g, L.d_out, din_dev ? L.in : nullptr, L.S, st));
   return tape_din(e, a, P, L.in, din_dev, s, st);
 }
 
@@ -2847,14 +2904,15 @@ int cgvc_discriminator_backward_tape(cgvc_handle e, const void* tape_dev, const 
   cudaStream_t st = (cudaStream_t)stream;
   const DiscNet& DN = e->disc[a.which];
   const float* Pm = e->P(); float* Gm = e->G();
-  {
-    TapeCounting counting(e, 1);
-    // dz = s dprob p (1 - p) through the head: dY3 and the dense kernel / bias gradients
-    CK(launch_head_loss_bwd(P.d.prob, P.d.d[2].Y, (long long)(e->cfg.num_features / 4) * (a.rows / 16), 1024, Pm + DN.dense_k, 0.f,
-                            0.f, nullptr, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, static_scale_dev(e, a.n), det_of(L.S), dprob_dev));
-    RET(discriminator_backward(e, DN, P.d, L.dY3, true, din_dev, L.S, st));
-  }
-  return tape_din(e, a, P, nullptr, din_dev, loss_scale(e, a.n), st);
+  TapeCounting counting(e, 1);
+  TapeScale s;
+  RET(tape_scale(e, a, st, &s));
+  // dz = s dprob p (1 - p) through the head: dY3 and the dense kernel / bias gradients
+  CK(launch_head_loss_bwd(P.d.prob, P.d.d[2].Y, (long long)(e->cfg.num_features / 4) * (a.rows / 16), 1024, Pm + DN.dense_k, 0.f,
+                          0.f, nullptr, L.dY3, Gm + DN.dense_k, Gm + DN.dense_b, st, s.dev ? s.dev : static_scale_dev(e, a.n), det_of(L.S),
+                          dprob_dev));
+  RET(discriminator_backward(e, DN, P.d, L.dY3, true, din_dev, L.S, st));
+  return tape_din(e, a, P, nullptr, din_dev, s, st);
 }
 
 }  // extern "C"

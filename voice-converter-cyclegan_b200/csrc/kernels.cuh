@@ -288,6 +288,8 @@ cudaError_t launch_l1_loss_grad(const float* yhat, const float* y, long long n, 
 // F16F8 gradient planes; a device pointer, so that a captured step follows the dynamic scale
 // x *= a, or with div_dev x *= a / *div_dev
 cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st, const float* div_dev = nullptr);
+// x *= a * *mul_dev (a tape backward's upstream gradient times the scaler's current loss scale)
+cudaError_t launch_scale_by(float* x, long long n, float a, const float* mul_dev, cudaStream_t st);
 // [B,F,T] <-> [B,T,F]
 cudaError_t launch_transpose_ft(const float* in, float* out, int B, int F, int T, cudaStream_t st);
 // packed [F][len_u] blocks (block u at element F * off[u]) <-> channels-last rows [off[n], F]; to_rows = 1: blocks -> rows

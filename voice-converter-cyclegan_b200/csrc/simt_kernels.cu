@@ -2676,14 +2676,23 @@ cudaError_t launch_gather_minibatch(const float* cA, const long long* off_A, con
 }
 
 
-// x *= a  (un-scaling the gradient arena after a loss-scaled backward pass whose result is handed out instead of going into Adam)
+// x *= a  (un-scaling the gradient arena after a loss-scaled backward pass whose result is handed out instead of going into Adam), or
+// with div x *= a / *div; MUL: x *= a * *div (a tape backward's upstream gradient times the scaler's current loss scale)
+template <bool MUL>
 __global__ void __launch_bounds__(256) scale_kernel(float* __restrict__ x, long long n, float a, const float* __restrict__ div) {
-  if (div) a = a / *div;
+  if (MUL) a = a * *div;
+  else if (div) a = a / *div;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) x[i] *= a;
 }
 cudaError_t launch_scale(float* x, long long n, float a, cudaStream_t st, const float* div_dev) {
   if (n == 0) return cudaSuccess;
   long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 8) nb = CGVC_NUM_SMS * 8;
-  ++g_cgvc_launches; scale_kernel<<<(unsigned)nb, 256, 0, st>>>(x, n, a, div_dev);
+  ++g_cgvc_launches; scale_kernel<false><<<(unsigned)nb, 256, 0, st>>>(x, n, a, div_dev);
+  return cudaGetLastError();
+}
+cudaError_t launch_scale_by(float* x, long long n, float a, const float* mul_dev, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  long long nb = (n + 255) / 256; if (nb > CGVC_NUM_SMS * 8) nb = CGVC_NUM_SMS * 8;
+  ++g_cgvc_launches; scale_kernel<true><<<(unsigned)nb, 256, 0, st>>>(x, n, a, mul_dev);
   return cudaGetLastError();
 }

@@ -24,6 +24,9 @@ Differences a user of the reference should know:
     given to the constructor are `generator_descriptor` / `discriminator_descriptor`; `generator_packed(inputs, direction)` and
     `discriminator_packed(inputs, which)` are the networks over a list of utterances of different lengths in one call, for
     utterance-level objectives
+  * `tape_loss_scale='dynamic'` (with `loss_scale='dynamic'`) puts those networks' backward passes on the engine's loss scaler:
+    `apply_gradients()` then all-reduces (data parallel), checks and updates the scale, and skips an overflowing step on the device,
+    as train() does (include/cgvc.h cgvc_apply_gradients, DESIGN.md section 12)
 """
 from __future__ import annotations
 
@@ -53,14 +56,21 @@ def _direction(direction):
 
 
 class CycleGAN(object):
+    _tape_dynamic = False            # tape_loss_scale='dynamic'
+    _grads_applied = False           # apply_gradients() ran since the last zero_grad()
 
     def __init__(self, num_features, discriminator=_discriminator, generator=_generator_gatedcnn, mode='train',
                  log_dir='./log', *, max_batch=1, max_frames=None, precision='bf16x3', device=None, seed=0,
-                 data_parallel=False, summary_interval=0, loss_scale='static', deterministic=False, loss_scale_per_network=False):
+                 data_parallel=False, summary_interval=0, loss_scale='static', deterministic=False, loss_scale_per_network=False,
+                 tape_loss_scale='static'):
         for net in (discriminator, generator):
             if not hasattr(net, "check_engine_table"):
                 raise TypeError("CycleGAN(discriminator=..., generator=...) takes network descriptors (cgvc.module.generator_gatedcnn / "
                                 "cgvc.module.discriminator or equivalents), not %r: the native engine runs its own kernel graph" % (net,))
+        if tape_loss_scale not in ('static', 'dynamic'):
+            raise ValueError("tape_loss_scale must be 'static' or 'dynamic', got %r" % (tape_loss_scale,))
+        if tape_loss_scale == 'dynamic' and loss_scale != 'dynamic':
+            raise ValueError("tape_loss_scale='dynamic' needs loss_scale='dynamic'")
         if not torch.cuda.is_available():
             raise RuntimeError("CycleGAN needs a CUDA device (sm_90a); there is no CPU fallback")
         self.num_features = num_features
@@ -84,6 +94,9 @@ class CycleGAN(object):
             self._options["loss_scale"] = N.LOSS_SCALE_MODES[loss_scale]     # applied by _create_engine, like any remembered option
         if loss_scale_per_network:
             self._options["loss_scale_per_network"] = 1
+        if tape_loss_scale == 'dynamic':
+            self._options["tape_loss_scale"] = 1                 # after "loss_scale": the engine accepts it in dynamic mode only
+        self._tape_dynamic = tape_loss_scale == 'dynamic'
         if deterministic:
             self._options["deterministic"] = 1
         self.last_step_skipped = False
@@ -163,6 +176,8 @@ class CycleGAN(object):
         remembered across engine re-creations."""
         self._chk(self._lib.cgvc_set_option(self._handle, name.encode(), int(value)))
         self._options[name] = int(value)
+        if name == "tape_loss_scale":
+            self._tape_dynamic = bool(value)
         if name == "deterministic":
             # the option changes the WORK plan: a larger arena is allocated and bound before the next call needs it
             nbytes = C.c_size_t(0)
@@ -357,7 +372,12 @@ class CycleGAN(object):
 
     def tape_loss_scale(self, batch):
         """The factor the tape backward calls of a `batch`-sample application leave in the gradient arena: the static loss scale of the
-        F16F8 gradient planes, 2^(9 + min(floor(log2 batch), 9)), and 1 in the other precisions (include/cgvc.h cgvc_adam_step)."""
+        F16F8 gradient planes, 2^(9 + min(floor(log2 batch), 9)), and 1 in the other precisions (include/cgvc.h cgvc_adam_step).
+        With tape_loss_scale='dynamic' the tapes use the scaler's current scale instead, which only the device knows: grads() and
+        apply_gradients() remove it there."""
+        if self._tape_dynamic:
+            raise RuntimeError("tape_loss_scale='dynamic': the tapes use the loss scaler's scale, not a static one; grads() and "
+                               "apply_gradients() remove it on the device")
         if N.PRECISIONS[self.precision] != N.PREC_F16F8:
             return 1.0
         return float(2 ** (9 + min(int(batch).bit_length() - 1, 9)))
@@ -419,7 +439,8 @@ class CycleGAN(object):
         dx = torch.empty(x_shape, dtype=torch.float32, device=self.device) if want_dx else None
         fn = self._lib.cgvc_discriminator_backward_tape if kind in (1, 3) else self._lib.cgvc_generator_backward_tape
         self._chk(fn(self._handle, _ptr(tape), _ptr(dy), _ptr(dx), self._stream()))
-        self._tape_scales.add(self.tape_loss_scale(batch))
+        if not self._tape_dynamic:
+            self._tape_scales.add(self.tape_loss_scale(batch))
         if kind not in (2, 3):
             return dx
         return self._unpack(dx, geom) if want_dx else [None] * batch
@@ -431,6 +452,7 @@ class CycleGAN(object):
         if network is None:
             self._arenas[N.ARENA_GRAD].zero_()
             self._tape_scales.clear()
+            self._grads_applied = False
             return
         names = [n for n in self._table if n.startswith(network + "/")]
         if not names:
@@ -441,16 +463,39 @@ class CycleGAN(object):
     def grads(self, network=None):
         """name -> d loss / d variable (TF layout) as the tape backward calls since zero_grad() accumulated it, on the device, with
         their loss scale removed: views of the gradient arena when that scale is 1, else scaled copies -- read them, do not write
-        them.  network: 'generator_A2B', 'generator_B2A', 'discriminator_A' or 'discriminator_B' (None: all four)."""
-        s = self._grad_scale()
+        them.  network: 'generator_A2B', 'generator_B2A', 'discriminator_A' or 'discriminator_B' (None: all four).
+        With tape_loss_scale='dynamic': copies divided by the scaler's current scale -- per network with loss_scale_per_network --
+        on the device, without a host synchronisation; refused after apply_gradients() until zero_grad(), since a skipped step has
+        already halved the scale the arena was formed with."""
+        if self._tape_dynamic:
+            if self._grads_applied:
+                raise RuntimeError("grads() after apply_gradients(): the loss scale may have changed since the gradient arena was formed; "
+                                   "read grads() before apply_gradients(), and zero_grad() starts the next step")
+            s_gen, s_disc = self._device_scales()
+        else:
+            s = self._grad_scale()
         out = OrderedDict()
         for n in self._table:
             if network is None or n.startswith(network + "/"):
                 v = self._view(N.ARENA_GRAD, n).detach()
-                out[n] = v if s == 1.0 else v * s
+                if self._tape_dynamic:
+                    out[n] = v / (s_gen if n.startswith("generator") else s_disc)
+                else:
+                    out[n] = v if s == 1.0 else v * s
         if not out:
             raise KeyError("no network %r" % (network,))
         return out
+
+    def _device_scales(self):
+        """The scaler's current scales of the generators' and the discriminators' gradients as device tensors, enqueued on the
+        current stream (no synchronisation).  Before the first tape backward sets the scaler they read 0, taken as 1."""
+        self._chk(self._lib.cgvc_loss_scale_state(self._handle, _ptr(self._ls_dev), self._stream()))
+        s = self._ls_dev[:4].view(torch.float32).clamp_min(1.0)
+        if not (self.loss_scale_per_network and N.PRECISIONS[self.precision] == N.PREC_F16F8):
+            return s, s
+        self._chk(self._lib.cgvc_loss_scale_net_state(self._handle, _ptr(self._lsn_dev), self._stream()))
+        k = C.sizeof(N.LossScaleNetInfo)
+        return self._lsn_dev[:4].view(torch.float32).clamp_min(1.0), self._lsn_dev[k:k + 4].view(torch.float32).clamp_min(1.0)
 
     def _grad_scale(self):
         if len(self._tape_scales) > 1:
@@ -460,9 +505,26 @@ class CycleGAN(object):
 
     def adam_step(self, generator_learning_rate, discriminator_learning_rate):
         """One Adam update of all four networks (model.py:107-108) from the gradient arena that the tape backward calls filled, with
-        their loss scale removed; advances the Adam step count like train()."""
+        their loss scale removed; advances the Adam step count like train().  It never skips a step, and with data_parallel=True it
+        does not all-reduce the gradient arena: replicas that call it drift apart.  tape_loss_scale='dynamic' takes
+        apply_gradients() instead, which does both."""
+        if self._tape_dynamic:
+            raise RuntimeError("tape_loss_scale='dynamic': use apply_gradients(), which removes the device loss scale and skips "
+                               "overflowing steps")
         self._chk(self._lib.cgvc_adam_step(self._handle, float(generator_learning_rate), float(discriminator_learning_rate),
                                            self._grad_scale(), self._stream()))
+        self.train_step += 1
+
+    def apply_gradients(self, generator_learning_rate, discriminator_learning_rate):
+        """The train step's optimizer tail over the gradient arena that the tape backward calls filled (tape_loss_scale='dynamic';
+        include/cgvc.h cgvc_apply_gradients): with data_parallel=True the all-reduce, then the non-finite check and the loss-scale
+        update, then Adam with the scale removed -- or, on overflow, a skipped step and a halved scale.  Enqueued without a host
+        synchronisation; loss_scale_state() reports skipped and the scales as after train().  Advances train_step like train()."""
+        if not self._tape_dynamic:
+            raise RuntimeError("apply_gradients() needs tape_loss_scale='dynamic'; static tapes take adam_step()")
+        self._chk(self._lib.cgvc_apply_gradients(self._handle, float(generator_learning_rate), float(discriminator_learning_rate),
+                                                 self._stream()))
+        self._grads_applied = True
         self.train_step += 1
 
     # ------------------------------------------------------------------ data parallel
